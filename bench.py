@@ -4,10 +4,10 @@
   metric  audio-sec/sec, E6D2 training step (encoder LSTM stack -> predictor -> joint -> rnnt_loss,
           forward + backward + Adam), B=32 per GPU, T=1000 frames (37.5 ms each), U=128, V=1024.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
   torchrun --nproc-per-node N bench.py --gpus N ...        (one rank per GPU, NCCL)
 
-"ours": the B200 engine in bf16 mode (tcgen05 GEMMs, fp32 accumulate / fp32 recurrent state),
+"ours": the H100 engine in bf16 mode (wgmma GEMMs, fp32 accumulate / fp32 recurrent state),
 weak scaling (B=32 per GPU), one all-reduce of the flat gradient bucket per step; the line also carries
 `strong_scaling` (BASELINE configs[2]: global B=256 as 8/N accumulation micro-steps of 32 per GPU, one all-reduce
 per optimizer step -- the reference's sub_batch mechanism, cli/baseline.py:214-237) and `parity_probe` (loss of the
@@ -19,6 +19,11 @@ the B=32 step is executed the way the reference itself runs a large batch on a s
 sub-batches of the same utterance shape (T=1000, U=128); each timed "step" is one sub-batch (a bounded sample:
 1/16 of the optimizer step), the optimizer update is applied every 16th sub-batch inside the timed region.
 Prints ONE JSON line on rank 0.
+
+--dump-outputs DIR (ours): after the timed steps of the headline leg, rank 0 writes what the last of them computed --
+loss.npy (the step's loss) and a fixed, seeded sample of the flat gradient and parameter buckets after the optimizer
+update (grads_sample.npy, params_sample.npy; sample_index.npy holds the bucket positions) -- so that two builds can be
+compared output for output on identical seeded inputs.
 """
 import argparse
 import json
@@ -45,7 +50,26 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sus=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sus=1400.0, src="fallback")
+    # NVIDIA's H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s -- bounds, not reached figures
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sus=989.0, src="H100 SXM data sheet")
+
+
+DUMP_SAMPLE = 1 << 21       # bucket elements sampled per dumped array: 32 MB in all with the float64 positions
+
+
+def dump_outputs(path, loss, opt):
+    """The headline leg's last step, as float arrays: loss, and a seeded sample of the gradient / parameter buckets."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    n = opt.flat_grads.numel()
+    g = torch.Generator().manual_seed(1234)
+    idx = torch.randperm(n, generator=g)[:min(n, DUMP_SAMPLE)].sort().values
+    di = idx.to(opt.flat_grads.device)
+    np.save(os.path.join(path, "loss.npy"), np.array([float(loss)], dtype=np.float64))
+    np.save(os.path.join(path, "grads_sample.npy"), opt.flat_grads[di].cpu().numpy().astype(np.float32))
+    np.save(os.path.join(path, "params_sample.npy"), opt.flat_params[di].cpu().numpy().astype(np.float32))
+    np.save(os.path.join(path, "sample_index.npy"), idx.numpy().astype(np.float64))
 
 
 class ClockSampler:
@@ -171,6 +195,8 @@ def run_ours(args):
     prof = ops.PROF.summary(base=e0)
     launches = ops.PROF.launches // args.steps
     ops.PROF.enabled = False
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss.detach(), opt)
 
     # ---- leg 2: end to end through the public API with host buffers --------------------------------
     # Every step's inputs are copied from pinned host memory and every step's loss is read back on the host,
@@ -268,14 +294,6 @@ def run_ours(args):
         roof["note"] = ("grid-synchronous recurrence: one exchange + barrier per timestep, %d sequential steps per "
                         "training step; the tensor-pipe fraction is what the dependency chain leaves, the figure "
                         "to track is us_per_timestep" % cell_steps)
-    roof["traffic"] = None
-    if top == "lstm_tc_bwd":
-        # one ncu capture of the BPTT kernel (profiles/r2/prof_r2_lstm_tc_bwd_noncluster.txt: 205.3 MB read + 46.6 MB
-        # written per 250-step launch, B = 32, H = 1024) scaled to this run's average launch length
-        per_step = (205.338368e6 + 46.582272e6) / 250.0
-        roof["traffic"] = round(per_step * roof["timesteps"] / max(1.0, kern[top]["calls_per_step"]))
-        roof["traffic_note"] = ("dram__bytes_read+write per launch from ncu (non-cluster variant, application replay), "
-                                "%.2f MB per timestep x the average launch length" % (per_step / 1e6))
     roof["peak_source"] = pk["src"] + (" (sustained)" if roof["bound"] == "tensor" else "")
     # the BASELINE.json side metric: joint+loss HBM fraction on the algorithmic bytes of SURVEY 8(d)
     n_logits = B * (T // 2) * (U + 1) * V
@@ -384,11 +402,16 @@ def run_reference(steps, warmup, sub_b=REF_SUB_B):
     dt = (time.perf_counter() - t0) / steps
     val = sub_b * T * FRAME_SEC / dt
     kind = "reference" if ol.have_ref() else "port"
+    if kind == "port":
+        print("bench.py: oracle/_ref/libwarprnnt_ref.so is not built: the CPU baseline's loss runs this project's C "
+              "oracle, NOT the reference's warp-transducer library", file=sys.stderr)
     sample = ("E6D2 B=32 T=1000 U=128 V=1024 fwd+loss+bwd+Adam fp32 as %d accumulation sub-batches of B=%d T=%d U=%d; "
               "%d sub-batch(es) timed (%.1f s each), optimizer step every %d" % (n_sub, sub_b, T, U, steps, dt, n_sub))
     return dict(value=round(val, 3), unit="audio-sec/sec", cores=cores,
                 kind=kind + " (warp-transducer CPU lib compiled from the reference; model = torch-CPU port "
-                            "calling the same ATen LSTM kernel as nn.LSTM)", sample=sample), dt
+                            "calling the same ATen LSTM kernel as nn.LSTM)" if kind == "reference" else
+                "port (oracle/_ref not built: loss from this project's C oracle, not the reference's library; model = "
+                "torch-CPU port calling the same ATen LSTM kernel as nn.LSTM)", sample=sample), dt
 
 
 def main():
@@ -400,6 +423,8 @@ def main():
     ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's loss and seeded gradient / parameter samples as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     if args.impl == "reference":

@@ -21,8 +21,8 @@ SIGNATURES = {
     "eb_rnnt_workspace_views": (I, [P, I, I, I, I, P, P, P, P, P]),
     "eb_gemm_f32": (I, [P, L, L, P, L, L, P, L, P, I, I, I, F, F, P]),
     "eb_gemm_bf16": (I, [P, I, P, I, P, I, P, I, L, I, L, P]),
-    "eb_gemm_bf16_ex": (I, [P, I, P, I, P, I, P, I, L, I, L, I, P]),
-    "eb_gemm_pair_mode": (I, [I]),
+    "eb_gemm_bf16_ex": (I, [P, I, P, I, P, I, P, I, L, I, L, I, P, L, P]),
+    "eb_gemm_bf16_partials": (L, [I, I, I, L, I, L, I]),
     "eb_gemm_bf16_dtanh": (I, [P, I, P, I, P, P, L, I, L, P]),
     "eb_joint_dpre_reduce": (I, [P, P, P, I, I, I, I, P]),
     "eb_lstm_scratch_bytes": (Z, [I, I]),
@@ -84,7 +84,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise LibraryMissing(
                 "edgedict_b200: %s not found -- build it with `python -m edgedict_b200.build` "
-                "(nvcc, sm_100a).  There is no CPU / PyTorch fallback for the hot path." % LIB_PATH)
+                "(nvcc, sm_90a).  There is no CPU / PyTorch fallback for the hot path." % LIB_PATH)
         h = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(h, name)              # AttributeError if a declared symbol is not exported

@@ -1,9 +1,9 @@
-"""In-tree build of libedgedict_b200.so with nvcc for sm_100a (no torch headers, no pybind).
+"""In-tree build of libedgedict_b200.so with nvcc for sm_90a (no torch headers, no pybind).
 
     python -m edgedict_b200.build            # incremental
     python -m edgedict_b200.build --force
 
-The .so lands next to this file (git-ignored, but it travels to the GPU box with the tree).
+The .so lands next to this file (git-ignored build product).
 """
 import hashlib
 import os
@@ -16,7 +16,8 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libedgedict_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]
 
 
@@ -56,7 +57,7 @@ def build(force=False, verbose=False):
         res = list(ex.map(lambda s: _compile(s, force), sources()))
     objs = [o for o, _ in res]
     if force or any(c for _, c in res) or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs
+        cmd = [NVCC, "-shared"] + ARCH + ["-o", LIB] + objs
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for the edgedict_b200 CUDA library (sm_100a only).
+// common.cuh -- shared device/host helpers for the edgedict_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -39,7 +39,7 @@ static inline int eb_num_sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
     }
     return n;
 }

@@ -1,4 +1,4 @@
-// decode.cu -- streaming greedy decode as ONE persistent kernel per audio chunk (sm_100a).
+// decode.cu -- streaming greedy decode as ONE persistent kernel per audio chunk (sm_90a).
 //
 // Replaces the Python loop of PytorchStreamDecoder.decode (rnnt/stream.py:93-120): per chunk the
 // reference runs the stateful encoder, then for every encoder frame joint -> argmax(.item(): a

@@ -1,4 +1,4 @@
-// elementwise.cu -- bandwidth-bound glue kernels of the RNN-T path (sm_100a).
+// elementwise.cu -- bandwidth-bound glue kernels of the RNN-T path (sm_90a).
 //
 //   layernorm fwd/bwd (+ fused residual add)      nn.LayerNorm in rnnt/models.py:47,124 and the
 //                                                 `xs = xs + xs_next` of rnnt/models.py:66-69
@@ -103,25 +103,18 @@ layernorm_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ x,
     }
 }
 
-// Fused backward for H % 128 == 0, H <= 1024: ONE pass over dy / x / res produces dz AND the parameter gradients
-// (the two-kernel version above re-reads the three inputs for dgamma/dbeta and issues 4-byte accesses: it ran
-// at 1.9 TB/s).  128-bit accesses, NV float4 per lane; dgamma/dbeta partials live in registers across the rows
-// of a warp, are combined per CTA in shared memory and leave with one global atomic per column and CTA.
+// dz for H % 128 == 0, H <= 1024: one warp per row, 128-bit accesses, NV float4 per lane.  The parameter gradients are
+// summed by layernorm_param_grad_kernel in a fixed order, so that they are the same bits on every run.
 constexpr int LNB_WARPS = 4;
 template <int NV>
 __global__ void __launch_bounds__(LNB_WARPS * 32)
 layernorm_bwd_fused_kernel(const float* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ res,
                            const float* __restrict__ gamma, const float* __restrict__ mean,
-                           const float* __restrict__ rstd, float* __restrict__ dz, float* __restrict__ dgamma,
-                           float* __restrict__ dbeta, long rows, int H) {
-    extern __shared__ float lnb_acc[];                       // [2][H]
+                           const float* __restrict__ rstd, float* __restrict__ dz, long rows, int H) {
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const int H4 = H >> 2;
     const long wstride = (long)gridDim.x * LNB_WARPS;
     const float inv_h = 1.f / (float)H;
-    float4 ag[NV], ab[NV];
-#pragma unroll
-    for (int i = 0; i < NV; ++i) { ag[i] = make_float4(0.f, 0.f, 0.f, 0.f); ab[i] = ag[i]; }
     const float4* g4 = reinterpret_cast<const float4*>(gamma);
     for (long r = (long)blockIdx.x * LNB_WARPS + w; r < rows; r += wstride) {
         const float mu = mean[r], rs = rstd[r];
@@ -143,8 +136,6 @@ layernorm_bwd_fused_kernel(const float* __restrict__ dy, const float* __restrict
                 const float4 g = make_float4(d[i].x * gm.x, d[i].y * gm.y, d[i].z * gm.z, d[i].w * gm.w);
                 s1 += (g.x + g.y) + (g.z + g.w);
                 s2 += (g.x * xh[i].x + g.y * xh[i].y) + (g.z * xh[i].z + g.w * xh[i].w);
-                ag[i].x += d[i].x * xh[i].x; ag[i].y += d[i].y * xh[i].y; ag[i].z += d[i].z * xh[i].z; ag[i].w += d[i].w * xh[i].w;
-                ab[i].x += d[i].x; ab[i].y += d[i].y; ab[i].z += d[i].z; ab[i].w += d[i].w;
             }
         }
         s1 = warp_sum(s1) * inv_h;
@@ -160,46 +151,41 @@ layernorm_bwd_fused_kernel(const float* __restrict__ dy, const float* __restrict
             }
         }
     }
-    for (int c = threadIdx.x; c < 2 * H; c += blockDim.x) lnb_acc[c] = 0.f;
-    __syncthreads();
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-        const int c = (lane + i * 32) * 4;
-        if (c < H) {
-            atomicAdd(lnb_acc + c, ag[i].x); atomicAdd(lnb_acc + c + 1, ag[i].y);
-            atomicAdd(lnb_acc + c + 2, ag[i].z); atomicAdd(lnb_acc + c + 3, ag[i].w);
-            atomicAdd(lnb_acc + H + c, ab[i].x); atomicAdd(lnb_acc + H + c + 1, ab[i].y);
-            atomicAdd(lnb_acc + H + c + 2, ab[i].z); atomicAdd(lnb_acc + H + c + 3, ab[i].w);
-        }
-    }
-    __syncthreads();
-    for (int c = threadIdx.x; c < H; c += blockDim.x) {
-        atomicAdd(dgamma + c, lnb_acc[c]);
-        atomicAdd(dbeta + c, lnb_acc[H + c]);
-    }
 }
 
-// dgamma[c] += sum_r dy*xhat ; dbeta[c] += sum_r dy   (thread per column, rows chunked over grid.y)
-__global__ void layernorm_param_grad_kernel(const float* __restrict__ dy, const float* __restrict__ x,
-                                            const float* __restrict__ res,
-                                            const float* __restrict__ mean,
-                                            const float* __restrict__ rstd, float* __restrict__ dgamma,
-                                            float* __restrict__ dbeta, long rows, int H,
-                                            long rows_per_block) {
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= H) return;
-    long r0 = (long)blockIdx.y * rows_per_block;
-    long r1 = r0 + rows_per_block < rows ? r0 + rows_per_block : rows;
+// dgamma[c] += sum_r dy*xhat ; dbeta[c] += sum_r dy.  One CTA per 8 columns (one 32-byte sector of a row); thread (c, k)
+// of the 8 x 128 block sums the rows k, k+128, ... of column c and a fixed-shape tree adds the 128 lanes of a column:
+// a fixed summation order, so the parameter gradients are the same bits on every run.
+__global__ void __launch_bounds__(1024) layernorm_param_grad_kernel(const float* __restrict__ dy, const float* __restrict__ x,
+                                                                     const float* __restrict__ res,
+                                                                     const float* __restrict__ mean,
+                                                                     const float* __restrict__ rstd, float* __restrict__ dgamma,
+                                                                     float* __restrict__ dbeta, long rows, int H) {
+    __shared__ float sg[128][9], sb[128][9];
+    const int cx = threadIdx.x & 7, k = threadIdx.x >> 3;
+    const int c = blockIdx.x * 8 + cx;
     float ag = 0.f, ab = 0.f;
-    for (long r = r0; r < r1; ++r) {
-        float z = x[r * H + c];
-        if (res) z += res[r * H + c];
-        float d = dy[r * H + c];
-        ag += d * (z - mean[r]) * rstd[r];
-        ab += d;
+    if (c < H) {
+        for (long r = k; r < rows; r += 128) {
+            float z = x[r * H + c];
+            if (res) z += res[r * H + c];
+            const float d = dy[r * H + c];
+            ag += d * (z - mean[r]) * rstd[r];
+            ab += d;
+        }
     }
-    atomicAdd(dgamma + c, ag);
-    atomicAdd(dbeta + c, ab);
+    sg[k][cx] = ag;
+    sb[k][cx] = ab;
+    __syncthreads();
+#pragma unroll 1
+    for (int st = 64; st > 0; st >>= 1) {
+        if (k < st) { sg[k][cx] += sg[k + st][cx]; sb[k][cx] += sb[k + st][cx]; }
+        __syncthreads();
+    }
+    if (k == 0 && c < H) {
+        dgamma[c] += sg[0][cx];
+        dbeta[c] += sb[0][cx];
+    }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -252,19 +238,33 @@ __global__ void embedding_fwd_kernel(const I* __restrict__ ids, const float* __r
         if (out16) out16[i] = __float2bfloat16(v);
     }
 }
+// dW[id] += sum of dout over the positions with that id.  The thread of the FIRST position of an id owns its row and
+// adds the positions in order (no atomics: the same bits on every run); E is walked by the threads of a warp.
+template <typename I>
+__device__ __forceinline__ long emb_id(const I* ids, long pos, int U, int U1, int prepend, int bos) {
+    const long b = pos / U1;
+    const int u = (int)(pos % U1);
+    return (prepend && u == 0) ? bos : (long)ids[b * U + u - prepend];
+}
 template <typename I>
 __global__ void embedding_bwd_kernel(const I* __restrict__ ids, const float* __restrict__ dout,
                                      float* __restrict__ dW, int B, int U, int E, int prepend,
                                      int bos, int pad) {
     const int U1 = U + prepend;
-    const long n = (long)B * U1 * E;
-    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
-        int e = (int)(i % E);
-        long bu = i / E;
-        int u = (int)(bu % U1);
-        int b = (int)(bu / U1);
-        long id = (prepend && u == 0) ? bos : (long)ids[(long)b * U + u - prepend];
-        if (id != pad) atomicAdd(dW + id * E + e, dout[i]);    // padding_idx row gets no gradient
+    const long n = (long)B * U1;
+    const int lane = threadIdx.x & 31;
+    for (long i = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += ((long)gridDim.x * blockDim.x) >> 5) {
+        const long id = emb_id(ids, i, U, U1, prepend, bos);
+        if (id == pad) continue;                              // padding_idx row gets no gradient
+        bool first = true;
+        for (long j = lane; j < i && first; j += 32) first = emb_id(ids, j, U, U1, prepend, bos) != id;
+        if (!__all_sync(0xffffffffu, first)) continue;
+        for (int e = lane; e < E; e += 32) {
+            float acc = 0.f;
+            for (long j = i; j < n; ++j)
+                if (emb_id(ids, j, U, U1, prepend, bos) == id) acc += dout[j * E + e];
+            dW[id * E + e] += acc;
+        }
     }
 }
 
@@ -402,11 +402,11 @@ __global__ void joint_hidden_bwd_u_f32_kernel(const float* __restrict__ dpre, fl
         ddp[((long)b * U + u) * J + j] = acc;
     }
 }
-// bf16: grid (B*U, TSPLIT): each CTA sums a T-range, one atomic per (j) at the end (ddp pre-zeroed)
+// bf16: one CTA per (b,u) sums all of T in order (no cross-CTA atomics: the same bits on every run)
 __global__ void joint_hidden_bwd_u_bf16_kernel(const __nv_bfloat16* __restrict__ dpre, float* __restrict__ ddp,
-                                               int T, int U, int J, int tchunk) {
+                                               int T, int U, int J) {
     const int b = blockIdx.x / U, u = blockIdx.x % U;
-    const int t0 = blockIdx.y * tchunk, t1 = min(T, t0 + tchunk);
+    const int t0 = 0, t1 = T;
     const int J8 = J / 8;
     for (int q = threadIdx.x; q < J8; q += blockDim.x) {
         const __nv_bfloat16* g = dpre + ((long)b * T * U + u) * J + q * 8;
@@ -423,44 +423,69 @@ __global__ void joint_hidden_bwd_u_bf16_kernel(const __nv_bfloat16* __restrict__
             }
         }
         float* o = ddp + ((long)b * U + u) * J + q * 8;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) atomicAdd(o + i, acc[i]);
+        *reinterpret_cast<float4*>(o) = make_float4(acc[0], acc[1], acc[2], acc[3]);
+        *reinterpret_cast<float4*>(o + 4) = make_float4(acc[4], acc[5], acc[6], acc[7]);
     }
 }
 
 // ------------------------------------------------------------------------------------------
-// column sums out[c] (+)= sum_r x[r,c]; grid (colblocks, rowblocks), atomics across rowblocks
+// column sums out[c] (+)= sum_r x[r,c].  One CTA owns a slab of columns over ALL rows: its row lanes sum strided rows,
+// then a fixed-shape tree in shared memory adds the lanes -- no cross-CTA atomics, the same bits on every run.
 // ------------------------------------------------------------------------------------------
+template <int RL, int CW>                      // RL row lanes x CW columns per CTA, RL * CW threads
+__device__ __forceinline__ float colsum_tree(float (*sh)[CW + 1], float v, int k, int cx) {
+    sh[k][cx] = v;
+    __syncthreads();
+#pragma unroll 1
+    for (int st = RL / 2; st > 0; st >>= 1) {
+        if (k < st) sh[k][cx] += sh[k + st][cx];
+        __syncthreads();
+    }
+    return sh[0][cx];
+}
 template <typename TI>
-__global__ void colsum_kernel(const TI* __restrict__ x, float* __restrict__ out, long rows, int N,
-                              long rows_per_block) {
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= N) return;
-    long r0 = (long)blockIdx.y * rows_per_block;
-    long r1 = r0 + rows_per_block < rows ? r0 + rows_per_block : rows;
+__global__ void __launch_bounds__(1024) colsum_kernel(const TI* __restrict__ x, float* __restrict__ out, long rows, int N) {
+    __shared__ float sh[32][33];
+    const int cx = threadIdx.x & 31, k = threadIdx.x >> 5;
+    const int c = blockIdx.x * 32 + cx;
     float acc = 0.f;
-    for (long r = r0; r < r1; ++r) acc += (float)x[r * N + c];
-    atomicAdd(out + c, acc);
+    if (c < N)
+        for (long r = k; r < rows; r += 32) acc += (float)x[r * N + c];
+    const float t = colsum_tree<32, 32>(sh, acc, k, cx);
+    if (k == 0 && c < N) out[c] += t;
 }
 
-// bf16 rows with N % 8 == 0: each thread owns 8 consecutive columns (one 16-byte load per row) and
-// keeps four independent row loads in flight; one atomic per column per CTA at the end
-__global__ void colsum_bf16_vec_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ out, long rows,
-                                       int N, long rows_per_block) {
-    const int c8 = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c8 * 8 >= N) return;
-    const long r0 = (long)blockIdx.y * rows_per_block;
-    const long r1 = r0 + rows_per_block < rows ? r0 + rows_per_block : rows;
+// bf16 rows with N % 8 == 0: a CTA owns 16 columns (two threads of 8 columns, one 16-byte load per row each) and 512
+// row lanes with four independent row loads in flight
+__global__ void __launch_bounds__(1024) colsum_bf16_vec_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ out,
+                                                               long rows, int N) {
+    __shared__ float sh[512][17];
+    const int half = threadIdx.x & 1, k = threadIdx.x >> 1;
+    const int c0 = blockIdx.x * 16 + half * 8;
     float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    const __nv_bfloat16* p = x + r0 * N + (long)c8 * 8;
-    long r = r0;
-    for (; r + 3 < r1; r += 4) {
-        uint4 v[4];
+    if (c0 < N) {
+        const __nv_bfloat16* p = x + (long)k * N + c0;
+        const long step = 512L * N;
+        long r = k;
+        for (; r + 3 * 512 < rows; r += 4 * 512) {
+            uint4 v[4];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) v[k] = *reinterpret_cast<const uint4*>(p + (long)k * N);
+            for (int q = 0; q < 4; ++q) v[q] = *reinterpret_cast<const uint4*>(p + q * step);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const uint32_t w[4] = {v[k].x, v[k].y, v[k].z, v[k].w};
+            for (int q = 0; q < 4; ++q) {
+                const uint32_t w[4] = {v[q].x, v[q].y, v[q].z, v[q].w};
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w[i]));
+                    acc[2 * i] += f.x;
+                    acc[2 * i + 1] += f.y;
+                }
+            }
+            p += 4 * step;
+        }
+        for (; r < rows; r += 512, p += step) {
+            const uint4 v = *reinterpret_cast<const uint4*>(p);
+            const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w[i]));
@@ -468,20 +493,13 @@ __global__ void colsum_bf16_vec_kernel(const __nv_bfloat16* __restrict__ x, floa
                 acc[2 * i + 1] += f.y;
             }
         }
-        p += 4L * N;
     }
-    for (; r < r1; ++r, p += N) {
-        const uint4 v = *reinterpret_cast<const uint4*>(p);
-        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w[i]));
-            acc[2 * i] += f.x;
-            acc[2 * i + 1] += f.y;
-        }
+#pragma unroll 1
+    for (int i = 0; i < 8; ++i) {
+        const float t = colsum_tree<512, 16>(sh, acc[i], k, half * 8 + i);
+        if (k == 0 && c0 < N) out[c0 + i] += t;
+        __syncthreads();
     }
-#pragma unroll
-    for (int i = 0; i < 8; ++i) atomicAdd(out + (long)c8 * 8 + i, acc[i]);
 }
 
 __global__ void cast_bf16_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, long n) {
@@ -611,26 +629,21 @@ EB_API int eb_layernorm_bwd(const float* dy, const float* x, const float* res, c
         long blocks_f = (rows + LNB_WARPS - 1) / LNB_WARPS;
         long cap_f = (long)eb_num_sms() * 3;
         const int grid_f = (int)(blocks_f < cap_f ? blocks_f : cap_f);
-        const size_t sm = sizeof(float) * 2 * (size_t)H;
-#define LN_BWDF(NV) layernorm_bwd_fused_kernel<NV><<<grid_f, LNB_WARPS * 32, sm, ST(stream)>>>( \
-        dy, x, res, gamma, mean, rstd, dz, dgamma, dbeta, rows, H)
+#define LN_BWDF(NV) layernorm_bwd_fused_kernel<NV><<<grid_f, LNB_WARPS * 32, 0, ST(stream)>>>( \
+        dy, x, res, gamma, mean, rstd, dz, rows, H)
         if (H <= 128) LN_BWDF(1); else if (H <= 256) LN_BWDF(2); else if (H <= 512) LN_BWDF(4); else LN_BWDF(8);
 #undef LN_BWDF
-        EB_CHECK_LAUNCH();
-        return EB_OK;
-    }
-    long blocks = (rows + LN_WARPS - 1) / LN_WARPS;
-    long cap = (long)eb_num_sms() * 8;
-    int grid = (int)(blocks < cap ? blocks : cap);
+    } else {
+        long blocks = (rows + LN_WARPS - 1) / LN_WARPS;
+        long cap = (long)eb_num_sms() * 8;
+        int grid = (int)(blocks < cap ? blocks : cap);
 #define LN_BWD(PL) layernorm_bwd_kernel<PL><<<grid, LN_WARPS * 32, 0, ST(stream)>>>( \
         dy, x, res, gamma, mean, rstd, dz, rows, H)
-    if (H <= 256) LN_BWD(8); else if (H <= 512) LN_BWD(16); else if (H <= 1024) LN_BWD(32); else LN_BWD(64);
+        if (H <= 256) LN_BWD(8); else if (H <= 512) LN_BWD(16); else if (H <= 1024) LN_BWD(32); else LN_BWD(64);
 #undef LN_BWD
+    }
     EB_CHECK_LAUNCH();
-    long rpb = (rows + 255) / 256;
-    if (rpb < 32) rpb = 32;
-    dim3 g2((H + 127) / 128, (unsigned)((rows + rpb - 1) / rpb));
-    layernorm_param_grad_kernel<<<g2, 128, 0, ST(stream)>>>(dy, x, res, mean, rstd, dgamma, dbeta, rows, H, rpb);
+    layernorm_param_grad_kernel<<<(H + 7) / 8, 1024, 0, ST(stream)>>>(dy, x, res, mean, rstd, dgamma, dbeta, rows, H);
     EB_CHECK_LAUNCH();
     return EB_OK;
 }
@@ -663,8 +676,9 @@ EB_API int eb_embedding_fwd(const void* ids, int ids_are_int64, const float* W, 
 }
 EB_API int eb_embedding_bwd(const void* ids, int ids_are_int64, const float* dout, float* dW, int B,
                             int U, int E, int prepend_bos, int bos, int pad, void* stream) {
-    long n = (long)B * (U + (prepend_bos ? 1 : 0)) * E;
-    if (n <= 0) return EB_OK;
+    const long npos = (long)B * (U + (prepend_bos ? 1 : 0));
+    if (npos <= 0 || E <= 0) return EB_OK;
+    const long n = npos * 32;                                // one warp per position
     if (ids_are_int64)
         embedding_bwd_kernel<long long><<<ew_grid(n, 256), 256, 0, ST(stream)>>>(
             (const long long*)ids, dout, dW, B, U, E, prepend_bos ? 1 : 0, bos, pad);
@@ -696,13 +710,7 @@ EB_API int eb_joint_hidden_bwd(void* dhidden_inout, const void* hidden, int is_b
         joint_hidden_bwd_t_bf16_kernel<<<B * T, 96, 0, ST(stream)>>>(
             (__nv_bfloat16*)dhidden_inout, (const __nv_bfloat16*)hidden, dep, T, U, J);
         EB_CHECK_LAUNCH();
-        EB_CUDA(cudaMemsetAsync(ddp, 0, sizeof(float) * (size_t)B * U * J, ST(stream)));
-        int tsplit = (4 * eb_num_sms() + B * U - 1) / (B * U);
-        if (tsplit < 1) tsplit = 1;
-        if (tsplit > T) tsplit = T;
-        const int tchunk = (T + tsplit - 1) / tsplit;
-        joint_hidden_bwd_u_bf16_kernel<<<dim3(B * U, (T + tchunk - 1) / tchunk), 96, 0, ST(stream)>>>(
-            (const __nv_bfloat16*)dhidden_inout, ddp, T, U, J, tchunk);
+        joint_hidden_bwd_u_bf16_kernel<<<B * U, 96, 0, ST(stream)>>>((const __nv_bfloat16*)dhidden_inout, ddp, T, U, J);
     } else {
         joint_hidden_bwd_t_f32_kernel<<<B * T, 256, 0, ST(stream)>>>(
             (float*)dhidden_inout, (const float*)hidden, dep, T, U, J);
@@ -721,32 +729,19 @@ EB_API int eb_joint_dpre_reduce(const void* dpre16, float* dep, float* ddp, int 
         return EB_ERR_INVALID;
     joint_dep_reduce_bf16_kernel<<<B * T, 96, 0, ST(stream)>>>((const __nv_bfloat16*)dpre16, dep, U, J);
     EB_CHECK_LAUNCH();
-    EB_CUDA(cudaMemsetAsync(ddp, 0, sizeof(float) * (size_t)B * U * J, ST(stream)));
-    int tsplit = (4 * eb_num_sms() + B * U - 1) / (B * U);
-    if (tsplit < 1) tsplit = 1;
-    if (tsplit > T) tsplit = T;
-    const int tchunk = (T + tsplit - 1) / tsplit;
-    joint_hidden_bwd_u_bf16_kernel<<<dim3(B * U, (T + tchunk - 1) / tchunk), 96, 0, ST(stream)>>>(
-        (const __nv_bfloat16*)dpre16, ddp, T, U, J, tchunk);
+    joint_hidden_bwd_u_bf16_kernel<<<B * U, 96, 0, ST(stream)>>>((const __nv_bfloat16*)dpre16, ddp, T, U, J);
     EB_CHECK_LAUNCH();
     return EB_OK;
 }
 
 EB_API int eb_colsum(const void* x, int x_bf16, float* out, long rows, int N, void* stream) {
     if (!x || !out || rows <= 0 || N <= 0) return EB_ERR_INVALID;
-    long rpb = (rows + 255) / 256;
-    if (rpb < 64) rpb = 64;
-    dim3 grid((N + 127) / 128, (unsigned)((rows + rpb - 1) / rpb));
-    if (x_bf16 && N % 8 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
-        long rpb2 = (rows + 1023) / 1024;
-        if (rpb2 < 128) rpb2 = 128;             // >= 128 rows per CTA: the per-CTA column atomics stay off the profile
-        const int nth = (N / 8 < 128) ? N / 8 : 128;
-        dim3 g2((N / 8 + nth - 1) / nth, (unsigned)((rows + rpb2 - 1) / rpb2));
-        colsum_bf16_vec_kernel<<<g2, nth, 0, ST(stream)>>>((const __nv_bfloat16*)x, out, rows, N, rpb2);
-    } else if (x_bf16)
-        colsum_kernel<__nv_bfloat16><<<grid, 128, 0, ST(stream)>>>((const __nv_bfloat16*)x, out, rows, N, rpb);
+    if (x_bf16 && N % 8 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0)
+        colsum_bf16_vec_kernel<<<(N + 15) / 16, 1024, 0, ST(stream)>>>((const __nv_bfloat16*)x, out, rows, N);
+    else if (x_bf16)
+        colsum_kernel<__nv_bfloat16><<<(N + 31) / 32, 1024, 0, ST(stream)>>>((const __nv_bfloat16*)x, out, rows, N);
     else
-        colsum_kernel<float><<<grid, 128, 0, ST(stream)>>>((const float*)x, out, rows, N, rpb);
+        colsum_kernel<float><<<(N + 31) / 32, 1024, 0, ST(stream)>>>((const float*)x, out, rows, N);
     EB_CHECK_LAUNCH();
     return EB_OK;
 }

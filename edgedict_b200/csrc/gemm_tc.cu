@@ -1,5 +1,5 @@
-// gemm_tc.cu -- bf16 tensor-core GEMM for sm_100a: TMA -> shared (128B swizzle) -> tcgen05.mma
-// (accumulators in TMEM) -> tcgen05.ld epilogue.  Hand-written PTX, no CUTLASS.
+// gemm_tc.cu -- bf16 tensor-core GEMM for sm_90a: TMA -> shared (128B swizzle) -> wgmma.mma_async (fp32
+// accumulators in registers) -> epilogue straight from the accumulator fragments.  Hand-written PTX, no CUTLASS.
 //
 // Used in bf16 mode for every dense contraction of the RNN-T path:
 //   LSTM input projections  xg = X * W_ih^T          (rnnt/models.py:45-46 -> nn.LSTM)
@@ -7,63 +7,45 @@
 //   joint logits            logits = tanh(.) * W2^T  (rnnt/models.py:165, 2.7 TFLOP at E6D2)
 //   and their dgrad / wgrad counterparts (operands read MN-major, no transposes materialised).
 //
-// Kernel anatomy (one CTA per SM, persistent over output tiles of 128 x 128 / 128 x 256 -- or one CTA PAIR per 256 x 256 tile
-// with tcgen05.mma.cta_group::2, see Cfg / PAIR_ --, BK = 64):
-//   warp 0      TMA producer: cp.async.bulk.tensor.2d into a 5-stage ring, mbarrier expect_tx
-//   warp 1      MMA issuer: one elected lane issues 4 x tcgen05.mma (M128 N128 K16) per stage,
-//               tcgen05.commit releases the stage / publishes the accumulator; owns TMEM alloc
-//   warps 2..5  epilogue: tcgen05.ld (32 lanes x 32 columns per warp), transpose through a padded
-//               shared tile so that global stores are 128-byte coalesced rows, + bias / + C
-//   TMEM: 2 accumulator buffers x 128 fp32 columns, so the epilogue of tile i overlaps the
-//   mainloop of tile i+1.
+// Kernel anatomy (one CTA per SM, persistent over output tiles of 128 x 128 / 128 x 256, BK = 64):
+//   warps 0-7   two consumer warpgroups: warpgroup g issues the wgmma (M64 N128|256 K16) of rows [64g, 64g+64) of the
+//               tile, four per stage; one stage of MMAs stays in flight and the stage before it is handed back to the
+//               producer.  At the end of the tile the warpgroup applies the epilogue (bias, + C, tanh', softmax
+//               statistics) to its own accumulators and stores them.
+//   warp 8      TMA producer: cp.async.bulk.tensor.2d into a STAGES-deep ring, mbarrier expect_tx.  It runs ahead into
+//               the next tile while the consumers are in the epilogue.
 #include <cuda.h>
 #include <stdlib.h>
 #include "common.cuh"
-#include "sm100.cuh"
+#include "sm90.cuh"
 #include "../../include/edgedict_b200.h"
 
 namespace {
 
 constexpr int BM = 128, BK = 64, UMMA_K = 16;
 constexpr int A_BYTES = BM * BK * 2;
-constexpr int EPI_WARP_BYTES = 32 * 36 * 4;
-// Tile width BN_ = 128 (5 stages, 2 x 128 TMEM columns) or 256 (4 stages, 2 x 256 = all 512 TMEM
-// columns).  A 128 x 128 x 16 MMA reads 8 KB of shared memory in 64 cycles = the 128 B/clk limit of
-// the SM; the 128 x 256 tile reads 12 KB in 128 cycles, which leaves headroom for the TMA writes.
-// EPW_ = epilogue warps: 4 (one per TMEM lane quadrant) or 8 (two per quadrant, alternating 32-column
-// chunks).  The epilogue of a short-K GEMM is latency-bound with a single warp per scheduler; with 8 warps
-// two of them interleave on every scheduler.  The wide tile then keeps 3 instead of 4 smem stages.
-// LOW_ = "co-resident" configuration: 3 stages of the narrow tile (115 KB of shared memory), so that a GEMM CTA
-// fits on an SM next to one CTA of a persistent recurrent kernel (lstm_tc.cu) -- used by the layer-wavefront
-// schedule of the encoder stack, where the input GEMM of one layer runs under the recurrence of another.
-// PAIR_ = cta_group::2: two CTAs of a cluster (one TPC) work on one 256 x 256 tile -- each owns 128 rows of it and
-// stages its own A rows plus HALF of the B tile (the tensor cores of both SMs read both halves), so a 128 x 256 x 64
-// block costs each SM 32 KB of L2 -> SM traffic instead of 48 KB; the pair's leader issues every MMA.
-template <int BN_, int EPW_ = 4, bool LOW_ = false, bool PAIR_ = false> struct Cfg {
-    static constexpr int NTHREADS = 64 + 32 * EPW_;
-    static constexpr int STAGES = PAIR_ ? (EPW_ == 8 ? 5 : 6) : LOW_ ? 3 : (BN_ == 256 ? (EPW_ == 8 ? 3 : 4) : 5);
-    static constexpr int B_BYTES = (PAIR_ ? BN_ / 2 : BN_) * BK * 2;
+constexpr int NTHREADS = 2 * 128 + 32;                       // two consumer warpgroups + the producer warp
+// Tile width BN_ = 128 (6 stages) or 256 (4 stages): ~193 KB of shared memory either way.
+// LOW_ = "co-resident" configuration: 3 stages of the narrow tile (97 KB of shared memory), so that a GEMM CTA fits on an
+// SM next to one CTA of a persistent recurrent kernel (lstm_c4.cu) -- used by the layer-wavefront schedule of the encoder
+// stack, where the input GEMM of one layer runs under the recurrence of another.
+template <int BN_, bool LOW_ = false> struct Cfg {
+    static constexpr int STAGES = LOW_ ? 3 : (BN_ == 256 ? 4 : 6);
+    static constexpr int B_BYTES = BN_ * BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    // two accumulator buffers in TMEM (the epilogue of tile i overlaps the mainloop of tile i+1).  The co-resident
-    // configuration's 256 columns fit next to ONE lstm_c4 forward CTA (256 columns); lstm_c4 pads its shared-memory
-    // request so that a GEMM CTA is never placed next to two of them (a single-buffer variant measured 20 % slower).
-    static constexpr int TMEM_COLS = 2 * BN_;
-    static constexpr int EPI_BYTES = EPW_ * EPI_WARP_BYTES;
-    static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + EPI_BYTES + 256;
+    static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 256;
 };
 
-// Persistent tile schedule (identical in the three warp roles).  Work item j of CTA b:
+// Persistent tile schedule (identical in the producer and the consumers).  Work item j of CTA b:
 //   split-K (weight gradients): K-split major -- the CTAs running concurrently stream the SAME rows
 //     of both operands, so the operand k-blocks are shared in L2 while hot;
 //   otherwise, when there are many more row blocks than CTAs: one CTA walks all column tiles of its
-//     row block back to back -- the A tile is re-read from the same SM's side of the L2 instead of
-//     being fetched from HBM once per die / after eviction by the output stream (ncu: 8.4 GB of DRAM
-//     reads for a 2.6 GB operand before this change);
+//     row block back to back -- the A tile is re-read from L2 instead of being fetched from HBM again
+//     after eviction by the output stream;
 //   else the plain round-robin over output tiles.
 struct Sched {
     long num_m; int num_n; int ksplit; long out_tiles; bool n_inner;
-    unsigned wid, nw;                                        // this worker (CTA, or CTA pair) and the number of workers
-    __device__ __forceinline__ long count() const { return out_tiles * ksplit; }
+    unsigned wid, nw;                                        // this worker (CTA) and the number of workers
     __device__ __forceinline__ bool get(long j, long& m_blk, int& n_blk, int& ks) const {
         if (n_inner) {
             const long grp = (long)wid + (j / num_n) * nw;
@@ -81,9 +63,10 @@ struct Sched {
 };
 
 // Optional fused epilogue of the joint's output GEMM (rows = lattice cells (b,t,u), columns = vocabulary):
-// while the logits tile leaves TMEM, each epilogue thread owns one row and keeps an online
-// (max, sum-exp) over the whole vocabulary across the consecutive column tiles of its row block, plus
-// the blank and label logits -- i.e. everything rnnt_denom_kernel would otherwise re-read 8 GB for.
+// while the logits tile leaves the accumulators, each thread keeps an online (max, sum-exp) of its two rows over
+// its columns of the whole vocabulary across the consecutive column tiles of its row block, plus the blank and label
+// logits; the four threads that share a row merge them at the end -- everything rnnt_denom_kernel would otherwise
+// re-read the logits for.
 struct LseArgs {
     const int* labels; const int* xlen; const int* ylen;     // [B,maxU-1], [B], [B]
     float* denom; float* lpb; float* lpl;                     // [B*maxT*maxU] each (loss workspace)
@@ -93,416 +76,270 @@ struct LseArgs {
     const __nv_bfloat16* aux;
 };
 
+__device__ __forceinline__ void st_bf16x2(__nv_bfloat16* p, float a, float b) {
+    *reinterpret_cast<__nv_bfloat162*>(p) = __floats2bfloat162_rn(a, b);
+}
+
 // A_MN / B_MN: operand stored with its M (resp. N) index contiguous ("MN-major"), else K contiguous.
-//   K-major tile in smem : [128 rows][64 k] bf16, 128 B per row, 128B swizzle; SBO = 1024 (8 rows)
-//   MN-major tile in smem: 2 x [64 k][64 mn] bf16, 128 B per k-row; SBO = 1024 (8 k-rows), LBO = 8192
-template <bool A_MN, bool B_MN, int BN_, bool LSE = false, int EPW_ = 4, bool LOW_ = false, bool PAIR_ = false>
-__global__ void __launch_bounds__(64 + 32 * EPW_, 1)
+//   K-major tile in smem : [rows][64 k] bf16, 128 B per row, 128B swizzle; SBO = 1024 (8 rows)
+//   MN-major tile in smem: [64 k][64 mn] bf16 boxes of 8 KB, 128 B per k-row; SBO = 1024 (8 k-rows), LBO = 8192
+// LOW_ is also capped to 112 registers per thread (two CTAs' worth per SM): the register file has to hold a recurrent
+// CTA beside it as well.
+template <bool A_MN, bool B_MN, int BN_, bool LSE = false, bool LOW_ = false>
+__global__ void __launch_bounds__(NTHREADS, LOW_ ? 2 : 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                void* __restrict__ Cout, int c_bf16, const float* __restrict__ bias, int accumulate,
-               long M, int N, long K, int ksplit, LseArgs lse = LseArgs()) {
-    using C_ = Cfg<BN_, EPW_, LOW_, PAIR_>;
-    static_assert(!PAIR_ || BN_ == 256, "the pair tile is 256 x 256");
-    constexpr int BN = BN_, STAGES = C_::STAGES, STAGE_BYTES = C_::STAGE_BYTES;
-    constexpr int TMEM_COLS = C_::TMEM_COLS, EPI_BYTES = C_::EPI_BYTES;
+               long M, int N, long K, int ksplit, LseArgs lse = LseArgs(), float* __restrict__ part = nullptr) {
+    using C_ = Cfg<BN_, LOW_>;
+    constexpr int BN = BN_, STAGES = C_::STAGES, STAGE_BYTES = C_::STAGE_BYTES, NACC = BN / 2;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* tiles = smem;
-    float* epi = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + EPI_BYTES);
-    // bars: full[S], empty[S], tmem_full[2], tmem_empty[2], then tmem base pointer
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+    // bars: full[S], empty[S]
     const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + STAGES);
-    const uint32_t tfull0 = smem_u32(bars + 2 * STAGES), tempty0 = smem_u32(bars + 2 * STAGES + 2);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    constexpr int TM = PAIR_ ? 2 * BM : BM;                  // rows of one work item (a pair's tile is 256 rows)
-    const uint32_t rank = PAIR_ ? cluster_ctarank() : 0u;    // 0 = the pair's leader (MMA issuer)
-    const long num_m = (M + TM - 1) / TM;
+    const long num_m = (M + BM - 1) / BM;
     const int num_n = (N + BN - 1) / BN;
     Sched sch;
     sch.num_m = num_m; sch.num_n = num_n; sch.ksplit = ksplit; sch.out_tiles = num_m * num_n;
-    sch.wid = PAIR_ ? blockIdx.x >> 1 : blockIdx.x; sch.nw = PAIR_ ? gridDim.x >> 1 : gridDim.x;
+    sch.wid = blockIdx.x; sch.nw = gridDim.x;
     sch.n_inner = LSE || ((ksplit == 1) && (num_m >= 2L * sch.nw));   // LSE needs a row block's tiles back to back
     const int nkb_total = (int)((K + BK - 1) / BK);
     const int kb_per = (nkb_total + ksplit - 1) / ksplit;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 1); }
-        // pair: the leader's tmem_empty collects the epilogue warps of both CTAs; full[] is used in the leader only
-        for (int a = 0; a < 2; ++a) { mbar_init(tfull0 + 8 * a, 1); mbar_init(tempty0 + 8 * a, PAIR_ ? 2 * EPW_ : EPW_); }
+        for (int s = 0; s < STAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 8); }   // 8 consumer warps
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" :: "l"(&tma_a) : "memory");
         asm volatile("prefetch.tensormap [%0];" :: "l"(&tma_b) : "memory");
     }
-    if (warp == 1) {
-        if (PAIR_) {
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;"
-                         :: "r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-        } else {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                         :: "r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-    }
-    tc_fence_before();
-    if (PAIR_) cluster_sync_all();                           // the peer's mbarriers exist before anything arrives on them
-    else __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    __syncthreads();
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             int stage = 0; uint32_t phase = 0;
             long mb; int nb, ksx;
+            // out-of-range rows / columns / k arrive as zeros and still count their bytes
+            constexpr uint32_t TX = A_BYTES + C_::B_BYTES;
             for (long jj = 0; sch.get(jj, mb, nb, ksx); ++jj) {
                 const int kb0 = ksx * kb_per, kb1 = min(nkb_total, kb0 + kb_per);
-                const int m0 = ((int)mb * (TM / BM) + (int)rank) * BM, n0 = nb * BN;
-                // a wide tile hanging over the last columns (N % 256 == 128) runs its MMAs 128 wide: MN-major B then
-                // needs half the boxes (K-major boxes are fixed by the tensor map; the unused rows arrive as zeros)
-                const int ninst = min(BN, ((N - n0 + 127) >> 7) << 7);
-                const int nbox = (PAIR_ ? ninst / 2 : ninst) / 64;
-                const uint32_t tx = A_BYTES + (B_MN ? (uint32_t)nbox * 8192u : (uint32_t)C_::B_BYTES);
+                const int m0 = (int)mb * BM, n0 = nb * BN;
                 for (int kb = kb0; kb < kb1; ++kb) {
                     mbar_wait(empty0 + 8 * stage, phase ^ 1);
                     const uint32_t sa = smem_u32(tiles + stage * STAGE_BYTES), sb = sa + A_BYTES;
-                    if (PAIR_) {
-                        // both CTAs' bytes complete on the LEADER's full barrier (its producer expects 2 stages' worth)
-                        const uint32_t fbl = map_to_rank(full0 + 8 * stage, 0);
-                        if (rank == 0) mbar_expect_tx(full0 + 8 * stage, 2 * tx);
-                        const int nh = n0 + (int)rank * (ninst / 2);    // this CTA's half of the B tile
-                        if (!A_MN) tma_load_2d_pair(sa, &tma_a, kb * BK, m0, fbl);
-                        else { tma_load_2d_pair(sa, &tma_a, m0, kb * BK, fbl); tma_load_2d_pair(sa + 8192, &tma_a, m0 + 64, kb * BK, fbl); }
-                        if (!B_MN) tma_load_2d_pair(sb, &tma_b, kb * BK, nh, fbl);
-                        else {
-#pragma unroll
-                            for (int bx = 0; bx < BN / 128; ++bx)
-                                if (bx < nbox) tma_load_2d_pair(sb + bx * 8192, &tma_b, nh + bx * 64, kb * BK, fbl);
-                        }
-                        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                        continue;
-                    }
                     const uint32_t fb = full0 + 8 * stage;
-                    mbar_expect_tx(fb, tx);
+                    mbar_expect_tx(fb, TX);
                     if (!A_MN) tma_load_2d(sa, &tma_a, kb * BK, m0, fb);
                     else { tma_load_2d(sa, &tma_a, m0, kb * BK, fb); tma_load_2d(sa + 8192, &tma_a, m0 + 64, kb * BK, fb); }
                     if (!B_MN) tma_load_2d(sb, &tma_b, kb * BK, n0, fb);
                     else {
 #pragma unroll
-                        for (int bx = 0; bx < BN / 64; ++bx)
-                            if (bx < nbox) tma_load_2d(sb + bx * 8192, &tma_b, n0 + bx * 64, kb * BK, fb);
+                        for (int bx = 0; bx < BN / 64; ++bx) tma_load_2d(sb + bx * 8192, &tma_b, n0 + bx * 64, kb * BK, fb);
                     }
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0 && rank == 0) {
-            // instruction descriptor: D=f32 (1<<4), A=B=bf16 (1<<7, 1<<10), majors @15/@16, N>>3 @17, M>>4 @24
-            const uint32_t idesc0 = (1u << 4) | (1u << 7) | (1u << 10) | ((A_MN ? 1u : 0u) << 15) |
-                                    ((B_MN ? 1u : 0u) << 16) | ((uint32_t)(TM >> 4) << 24);
-            int stage = 0; uint32_t phase = 0;
-            long it = 0;
-            long mb; int nb, ksx;
-            for (long jj = 0; sch.get(jj, mb, nb, ksx); ++jj, ++it) {
-                const int kb0 = ksx * kb_per, kb1 = min(nkb_total, kb0 + kb_per);
-                const uint32_t acc = (uint32_t)(it & 1), acc_phase = (uint32_t)((it >> 1) & 1);
-                if (PAIR_) mbar_wait_cluster(tempty0 + 8 * acc, acc_phase ^ 1);     // arrivals come from both CTAs
-                else mbar_wait(tempty0 + 8 * acc, acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * BN;
-                const int ninst = min(BN, ((N - nb * BN + 127) >> 7) << 7);       // see the producer
-                const uint32_t idesc = idesc0 | ((uint32_t)(ninst >> 3) << 17);
-                for (int kb = kb0; kb < kb1; ++kb) {
-                    mbar_wait(full0 + 8 * stage, phase);
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(tiles + stage * STAGE_BYTES), sb = sa + A_BYTES;
+        return;
+    }
+
+    // ---- consumers
+    const int wg = warp >> 2;                                // rows [64 wg, 64 wg + 64) of the tile
+    const int r_in = 64 * wg + 16 * (warp & 3) + (lane >> 2);   // tile row of fragment row h = 0 (h = 1: + 8)
+    const int cq = 2 * (lane & 3);                           // column of the thread's pair inside each 8-column group
+    float* Cf = reinterpret_cast<float*>(Cout);
+    __nv_bfloat16* const Ch = reinterpret_cast<__nv_bfloat16*>(Cout);
+    const bool vec2 = (N % 2) == 0;
+    float acc[NACC];
+    int stage = 0; uint32_t phase = 0;
+    long mb; int nb, ks;
+    float rm[2] = {-INFINITY, -INFINITY}, rs[2] = {0.f, 0.f}, xb[2] = {0.f, 0.f}, xl[2] = {0.f, 0.f};   // LSE row statistics
+    int lab[2] = {-1, -1};
+    bool cell_ok[2] = {false, false};
+    for (long jj = 0; sch.get(jj, mb, nb, ks); ++jj) {
+        const int kb0 = ks * kb_per, kb1 = min(nkb_total, kb0 + kb_per);
+        const long m0 = mb * BM;
+        const int n0 = nb * BN;
 #pragma unroll
-                    for (int k = 0; k < BK / UMMA_K; ++k) {
-                        const uint64_t ad = A_MN ? make_desc(sa + k * 2048, 8192, 1024) : make_desc(sa + k * 32, 0, 1024);
-                        const uint64_t bd = B_MN ? make_desc(sb + k * 2048, 8192, 1024) : make_desc(sb + k * 32, 0, 1024);
-                        if (PAIR_) tc_mma_bf16_pair(d_tmem, ad, bd, idesc, ((kb - kb0) | k) ? 1u : 0u);
-                        else tc_mma_bf16(d_tmem, ad, bd, idesc, ((kb - kb0) | k) ? 1u : 0u);
-                    }
-                    // frees the smem stage (pair: in both CTAs) when the MMAs retire
-                    if (PAIR_) tc_commit_pair(empty0 + 8 * stage); else tc_commit(empty0 + 8 * stage);
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                }
-                // accumulator complete -> epilogue (pair: of both CTAs)
-                if (PAIR_) tc_commit_pair(tfull0 + 8 * acc); else tc_commit(tfull0 + 8 * acc);
+        for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+        int prev = -1;
+        for (int kb = kb0; kb < kb1; ++kb) {
+            mbar_wait(full0 + 8 * stage, phase);
+            const uint32_t sa = smem_u32(tiles + stage * STAGE_BYTES) + (uint32_t)wg * 8192u, sb = smem_u32(tiles + stage * STAGE_BYTES) + A_BYTES;
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BK / UMMA_K; ++k) {
+                const uint64_t ad = A_MN ? make_desc(sa + k * 2048, 8192, 1024) : make_desc(sa + k * 32, 16, 1024);
+                const uint64_t bd = B_MN ? make_desc(sb + k * 2048, 8192, 1024) : make_desc(sb + k * 32, 16, 1024);
+                if constexpr (BN == 256) wgmma_m64n256k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, ad, bd, 1);
+                else wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, ad, bd, 1);
             }
+            wgmma_commit();
+            wgmma_wait<1>();                                 // the previous stage's MMAs have retired: hand it back
+            if (prev >= 0 && lane == 0) mbar_arrive(empty0 + 8 * prev);
+            prev = stage;
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-    } else {
-        const int q = warp & 3;                             // TMEM lane quadrant this warp may read
-        // per-warp staging tile [32 rows][36 floats] (16-byte aligned rows: conflict-free 128-bit
-        // writes by row and 128-bit reads by 8-lane row groups), addressed in the shared window
-        const uint32_t sbuf = smem_u32(epi) + (uint32_t)(warp - 2) * EPI_WARP_BYTES;
-        const int chalf = (warp - 2) >> 2;                    // EPW == 8: which chunks (even / odd) this warp drains
-        const int rsub = lane >> 3, c4 = lane & 7;          // read-back mapping: 4 rows x 8 float4 per pass
-        float* const Cf = reinterpret_cast<float*>(Cout);
-        __nv_bfloat16* const Ch = reinterpret_cast<__nv_bfloat16*>(Cout);
-        const bool vec_ok = (N % 4) == 0;
-        const bool bias_vec = (reinterpret_cast<uintptr_t>(bias) & 15) == 0;
-        long it = 0;
-        long mb; int nb, ks;
-        float rm = -INFINITY, rs = 0.f, xb = 0.f, xl = 0.f;     // LSE: running row statistics
-        int lab = -1; bool cell_ok = false;
-        for (long jj = 0; sch.get(jj, mb, nb, ks); ++jj, ++it) {
-            const bool empty_split = ks * kb_per >= nkb_total;      // (only when K is tiny) nothing accumulated
-            const uint32_t acc = (uint32_t)(it & 1), acc_phase = (uint32_t)((it >> 1) & 1);
-            const long m0 = (mb * (TM / BM) + rank) * BM;
-            const int n0 = nb * BN;
-            const bool full_m = vec_ok && (m0 + BM <= M);
-            if (LSE && nb == 0) {                                 // new row block: reset, decode (b,t,u) of my row
-                rm = -INFINITY; rs = 0.f; xb = 0.f; xl = 0.f; lab = -1; cell_ok = false;
-                const long cell = m0 + q * 32 + lane;
-                if (cell < M) {
-                    const int u = (int)(cell % lse.maxU);
-                    const long bt = cell / lse.maxU;
-                    const int t = (int)(bt % lse.maxT), b = (int)(bt / lse.maxT);
-                    const int Tn = lse.xlen[b], Un = lse.ylen[b] + 1;
-                    cell_ok = t < Tn && u < Un;
-                    if (cell_ok && u < Un - 1) lab = lse.labels[b * (lse.maxU - 1) + u];
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        if (prev >= 0 && lane == 0) mbar_arrive(empty0 + 8 * prev);
+
+        if constexpr (LSE) {
+            constexpr float LOG2E = 1.4426950408889634f;
+            if (nb == 0) {                                   // new row block: reset, decode (b,t,u) of my two rows
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    rm[h] = -INFINITY; rs[h] = 0.f; xb[h] = 0.f; xl[h] = 0.f; lab[h] = -1; cell_ok[h] = false;
+                    const long cell = m0 + r_in + 8 * h;
+                    if (cell < M) {
+                        const int u = (int)(cell % lse.maxU);
+                        const long bt = cell / lse.maxU;
+                        const int t = (int)(bt % lse.maxT), b = (int)(bt / lse.maxT);
+                        const int Tn = lse.xlen[b], Un = lse.ylen[b] + 1;
+                        cell_ok[h] = t < Tn && u < Un;
+                        if (cell_ok[h] && u < Un - 1) lab[h] = lse.labels[b * (lse.maxU - 1) + u];
+                    }
                 }
             }
-            mbar_wait(tfull0 + 8 * acc, acc_phase);
-            tc_fence_after();
-#pragma unroll 1
-            for (int c = (EPW_ == 8 ? chalf : 0); c < BN / 32; c += (EPW_ == 8 ? 2 : 1)) {
-                // a wide tile may hang over the last columns (N % 256 == 128): chunks past N are skipped, chunks
-                // inside keep the vector path
-                if (!LSE && n0 + c * 32 >= N) break;
-                const bool full = full_m && (n0 + c * 32 + 32 <= N);
-                uint32_t r[32];
-                tc_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + acc * BN + c * 32, r);
-                if (empty_split) {
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) r[i] = 0u;
+            for (int h = 0; h < 2; ++h) {
+                // add the bias here (the statistics are over logits = acc + b2), then the online softmax
+                float cm = -INFINITY;
+#pragma unroll
+                for (int i = 0; i < BN / 8; ++i) {
+                    const int col = n0 + 8 * i + cq;
+                    float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+                    v0 = col < N ? v0 + (bias ? __ldg(bias + col) : 0.f) : -INFINITY;
+                    v1 = col + 1 < N ? v1 + (bias ? __ldg(bias + col + 1) : 0.f) : -INFINITY;
+                    acc[4 * i + 2 * h] = v0; acc[4 * i + 2 * h + 1] = v1;
+                    cm = fmaxf(cm, fmaxf(v0, v1));
+                    if (col == lse.blank) xb[h] = v0;
+                    if (col + 1 == lse.blank) xb[h] = v1;
+                    if (col == lab[h]) xl[h] = v0;
+                    if (col + 1 == lab[h]) xl[h] = v1;
                 }
-                if (LSE) {      // add the bias here (the statistics are over logits = acc + b2), then online softmax
-                    const int col0 = n0 + c * 32;
-                    constexpr float LOG2E = 1.4426950408889634f;
-                    float cm = -INFINITY;
-                    if (col0 + 32 <= N && bias_vec) {             // whole chunk inside the vocabulary: no per-element guards
-#pragma unroll
-                        for (int i4 = 0; i4 < 8; ++i4) {
-                            const float4 b4 = bias ? __ldg(reinterpret_cast<const float4*>(bias + col0 + i4 * 4))
-                                                   : make_float4(0.f, 0.f, 0.f, 0.f);
-                            const float v0 = __uint_as_float(r[i4 * 4]) + b4.x, v1 = __uint_as_float(r[i4 * 4 + 1]) + b4.y;
-                            const float v2 = __uint_as_float(r[i4 * 4 + 2]) + b4.z, v3 = __uint_as_float(r[i4 * 4 + 3]) + b4.w;
-                            r[i4 * 4] = __float_as_uint(v0); r[i4 * 4 + 1] = __float_as_uint(v1);
-                            r[i4 * 4 + 2] = __float_as_uint(v2); r[i4 * 4 + 3] = __float_as_uint(v3);
-                            cm = fmaxf(fmaxf(cm, fmaxf(v0, v1)), fmaxf(v2, v3));
-                        }
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) {
-                            float v = __uint_as_float(r[i]) + ((bias && col0 + i < N) ? __ldg(bias + col0 + i) : 0.f);
-                            if (col0 + i >= N) v = -INFINITY;
-                            r[i] = __float_as_uint(v);
-                            cm = fmaxf(cm, v);
-                        }
-                    }
-                    const float nm = fmaxf(rm, cm);
+                const float nm = fmaxf(rm[h], cm);
+                if (nm != -INFINITY) {                       // (a thread may own no column of a narrow vocabulary)
                     const float nml = nm * LOG2E;
-                    float a0 = 0.f, a1 = 0.f;                     // exp(v - nm) = ex2(v*log2e - nm*log2e): FFMA + MUFU + FADD
+                    float a0 = 0.f, a1 = 0.f;                // exp(v - nm) = ex2(v*log2e - nm*log2e): FFMA + MUFU + FADD
 #pragma unroll
-                    for (int i = 0; i < 32; i += 2) {
-                        a0 += fast_ex2(fmaf(__uint_as_float(r[i]), LOG2E, -nml));
-                        a1 += fast_ex2(fmaf(__uint_as_float(r[i + 1]), LOG2E, -nml));
+                    for (int i = 0; i < BN / 8; ++i) {
+                        a0 += fast_ex2(fmaf(acc[4 * i + 2 * h], LOG2E, -nml));
+                        a1 += fast_ex2(fmaf(acc[4 * i + 2 * h + 1], LOG2E, -nml));
                     }
-                    rs = rs * fast_ex2((rm - nm) * LOG2E) + (a0 + a1);
-                    rm = nm;
+                    rs[h] = rs[h] * fast_ex2((rm[h] - nm) * LOG2E) + (a0 + a1);
+                    rm[h] = nm;
                 }
+                const long row = m0 + r_in + 8 * h;
+                if (row < M) {
 #pragma unroll
-                for (int i = 0; i < 8; ++i)
-                    asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" :: "r"(sbuf + (uint32_t)(lane * 36 + i * 4) * 4),
-                                 "r"(r[4 * i]), "r"(r[4 * i + 1]), "r"(r[4 * i + 2]), "r"(r[4 * i + 3]) : "memory");
-                __syncwarp();
-                if (LSE) {
-                    const int col0 = n0 + c * 32;
-                    if (lse.blank >= col0 && lse.blank < col0 + 32)
-                        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(xb) : "r"(sbuf + (uint32_t)(lane * 36 + lse.blank - col0) * 4) : "memory");
-                    if (lab >= col0 && lab < col0 + 32)
-                        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(xl) : "r"(sbuf + (uint32_t)(lane * 36 + lab - col0) * 4) : "memory");
-                }
-                const int col = n0 + c * 32 + c4 * 4;
-                float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (bias && ks == 0 && !LSE) {
-                    if (full && bias_vec) bv = *reinterpret_cast<const float4*>(bias + col);
-                    else {
-                        bv.x = col < N ? bias[col] : 0.f; bv.y = col + 1 < N ? bias[col + 1] : 0.f;
-                        bv.z = col + 2 < N ? bias[col + 2] : 0.f; bv.w = col + 3 < N ? bias[col + 3] : 0.f;
-                    }
-                }
-                const long row0 = m0 + q * 32 + rsub;
-                // all eight 128-bit reads of this lane are issued before anything consumes them (one warp per
-                // scheduler: back-to-back LDS -> FADD -> STG chains would expose the full LDS latency 8 times)
-                float4 vv[8];
-#pragma unroll
-                for (int rr = 0; rr < 8; ++rr)
-                    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];"
-                                 : "=f"(vv[rr].x), "=f"(vv[rr].y), "=f"(vv[rr].z), "=f"(vv[rr].w)
-                                 : "r"(sbuf + (uint32_t)((rr * 4 + rsub) * 36 + c4 * 4) * 4));
-                if (full && ksplit == 1 && !accumulate) {         // the common case, free of per-store mode tests
-                    if (c_bf16 && !LSE && lse.aux) {
-                        uint2 hq[8];
-#pragma unroll
-                        for (int rr = 0; rr < 8; ++rr)
-                            hq[rr] = __ldg(reinterpret_cast<const uint2*>(lse.aux + (row0 + rr * 4) * N + col));
-#pragma unroll
-                        for (int rr = 0; rr < 8; ++rr) {
-                            const float4 v = vv[rr];
-                            const float2 h0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&hq[rr].x));
-                            const float2 h1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&hq[rr].y));
-                            __nv_bfloat162 p0 = __floats2bfloat162_rn((v.x + bv.x) * (1.f - h0.x * h0.x), (v.y + bv.y) * (1.f - h0.y * h0.y));
-                            __nv_bfloat162 p1 = __floats2bfloat162_rn((v.z + bv.z) * (1.f - h1.x * h1.x), (v.w + bv.w) * (1.f - h1.y * h1.y));
-                            uint2 o;
-                            o.x = *reinterpret_cast<uint32_t*>(&p0);
-                            o.y = *reinterpret_cast<uint32_t*>(&p1);
-                            *reinterpret_cast<uint2*>(Ch + (row0 + rr * 4) * N + col) = o;
+                    for (int i = 0; i < BN / 8; ++i) {
+                        const int col = n0 + 8 * i + cq;
+                        __nv_bfloat16* cp = Ch + row * N + col;
+                        if (vec2 && col + 1 < N) st_bf16x2(cp, acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+                        else {
+                            if (col < N) cp[0] = __float2bfloat16(acc[4 * i + 2 * h]);
+                            if (col + 1 < N) cp[1] = __float2bfloat16(acc[4 * i + 2 * h + 1]);
                         }
-                    } else if (c_bf16) {
+                    }
+                }
+            }
+            if (nb == num_n - 1) {                           // whole vocabulary seen: merge the quad, publish
 #pragma unroll
-                        for (int rr = 0; rr < 8; ++rr) {
-                            const float4 v = vv[rr];
-                            __nv_bfloat162 p0 = __floats2bfloat162_rn(v.x + bv.x, v.y + bv.y);
-                            __nv_bfloat162 p1 = __floats2bfloat162_rn(v.z + bv.z, v.w + bv.w);
-                            uint2 o;
-                            o.x = *reinterpret_cast<uint32_t*>(&p0);
-                            o.y = *reinterpret_cast<uint32_t*>(&p1);
-                            *reinterpret_cast<uint2*>(Ch + (row0 + rr * 4) * N + col) = o;
+                for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                    for (int o = 1; o <= 2; o <<= 1) {
+                        const float m2 = __shfl_xor_sync(0xffffffffu, rm[h], o), s2 = __shfl_xor_sync(0xffffffffu, rs[h], o);
+                        xb[h] += __shfl_xor_sync(0xffffffffu, xb[h], o);
+                        xl[h] += __shfl_xor_sync(0xffffffffu, xl[h], o);
+                        const float m = fmaxf(rm[h], m2);
+                        rs[h] = (rm[h] == -INFINITY ? 0.f : rs[h] * fast_ex2((rm[h] - m) * LOG2E)) +
+                                (m2 == -INFINITY ? 0.f : s2 * fast_ex2((m2 - m) * LOG2E));
+                        rm[h] = m;
+                    }
+                    if ((lane & 3) == 0 && cell_ok[h]) {
+                        const long cell = m0 + r_in + 8 * h;
+                        const float d = -(rm[h] + logf(rs[h]));
+                        lse.denom[cell] = d;
+                        lse.lpb[cell] = d + xb[h];
+                        lse.lpl[cell] = d + xl[h];
+                    }
+                }
+            }
+        } else {
+            const bool add_bias = bias && ks == 0;
+            // split-K: each split stores its partial tile in its own slice of the workspace (splitk_reduce_kernel adds
+            // the slices in split order -- no atomics, the same bits on every run)
+            if (ksplit > 1) Cf = part + (long)ks * M * N;
+            const int acc_c = ksplit > 1 ? 0 : accumulate;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const long row = m0 + r_in + 8 * h;
+                if (row >= M) continue;
+#pragma unroll
+                for (int i = 0; i < BN / 8; ++i) {
+                    const int col = n0 + 8 * i + cq;
+                    if (col >= N) break;
+                    const bool two = col + 1 < N, pair = two && vec2;
+                    float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+                    if (add_bias) { v0 += __ldg(bias + col); if (two) v1 += __ldg(bias + col + 1); }
+                    const long off = row * N + col;
+                    if (c_bf16) {
+                        __nv_bfloat16* cp = Ch + off;
+                        if (lse.aux) {
+                            float h0, h1 = 0.f;
+                            if (pair) {
+                                const float2 hh = __bfloat1622float2(__ldg(reinterpret_cast<const __nv_bfloat162*>(lse.aux + off)));
+                                h0 = hh.x; h1 = hh.y;
+                            } else {
+                                h0 = __bfloat162float(lse.aux[off]);
+                                if (two) h1 = __bfloat162float(lse.aux[off + 1]);
+                            }
+                            v0 *= 1.f - h0 * h0; v1 *= 1.f - h1 * h1;
+                        }
+                        if (pair) {
+                            if (accumulate) {
+                                const float2 o = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(cp));
+                                v0 += o.x; v1 += o.y;
+                            }
+                            st_bf16x2(cp, v0, v1);
+                        } else {
+                            if (accumulate) { v0 += __bfloat162float(cp[0]); if (two) v1 += __bfloat162float(cp[1]); }
+                            cp[0] = __float2bfloat16(v0);
+                            if (two) cp[1] = __float2bfloat16(v1);
                         }
                     } else {
-#pragma unroll
-                        for (int rr = 0; rr < 8; ++rr) {
-                            const float4 v = vv[rr];
-                            *reinterpret_cast<float4*>(Cf + (row0 + rr * 4) * N + col) =
-                                make_float4(v.x + bv.x, v.y + bv.y, v.z + bv.z, v.w + bv.w);
-                        }
-                    }
-                } else if (full && ksplit == 1 && !c_bf16) {      // C += A B in fp32 (the LSTM d-x GEMM accumulates into dz):
-                    float4 ov[8];                                 // all eight reads of C in flight before the first store --
-#pragma unroll                                                    // read-add-store per row exposed one DRAM round trip each
-                    for (int rr = 0; rr < 8; ++rr)                // (217 us for a 134 GFLOP product in the step's timeline)
-                        ov[rr] = *reinterpret_cast<const float4*>(Cf + (row0 + rr * 4) * N + col);
-#pragma unroll
-                    for (int rr = 0; rr < 8; ++rr) {
-                        const float4 v = vv[rr];
-                        *reinterpret_cast<float4*>(Cf + (row0 + rr * 4) * N + col) =
-                            make_float4(v.x + bv.x + ov[rr].x, v.y + bv.y + ov[rr].y, v.z + bv.z + ov[rr].z, v.w + bv.w + ov[rr].w);
-                    }
-                } else
-#pragma unroll
-                for (int rr = 0; rr < 8; ++rr) {
-                    float4 v = vv[rr];
-                    v.x += bv.x; v.y += bv.y; v.z += bv.z; v.w += bv.w;
-                    const long row = row0 + rr * 4;
-                    if (full) {
-                        if (ksplit > 1) {
-                            float* cp = Cf + row * N + col;
-                            atomicAdd(cp, v.x); atomicAdd(cp + 1, v.y); atomicAdd(cp + 2, v.z); atomicAdd(cp + 3, v.w);
-                        } else if (c_bf16) {
-                            __nv_bfloat16* cp = Ch + row * N + col;
-                            if (!LSE && lse.aux) {
-                                const __nv_bfloat16* hp = lse.aux + row * N + col;
-                                const float h0 = __bfloat162float(hp[0]), h1 = __bfloat162float(hp[1]);
-                                const float h2 = __bfloat162float(hp[2]), h3 = __bfloat162float(hp[3]);
-                                v.x *= 1.f - h0 * h0; v.y *= 1.f - h1 * h1; v.z *= 1.f - h2 * h2; v.w *= 1.f - h3 * h3;
-                            }
-                            if (accumulate) {
-                                const uint2 o = *reinterpret_cast<const uint2*>(cp);
-                                const float2 o0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&o.x));
-                                const float2 o1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&o.y));
-                                v.x += o0.x; v.y += o0.y; v.z += o1.x; v.w += o1.y;
-                            }
-                            __nv_bfloat162 p0 = __floats2bfloat162_rn(v.x, v.y), p1 = __floats2bfloat162_rn(v.z, v.w);
-                            uint2 o;
-                            o.x = *reinterpret_cast<uint32_t*>(&p0);
-                            o.y = *reinterpret_cast<uint32_t*>(&p1);
-                            *reinterpret_cast<uint2*>(cp) = o;
+                        float* cp = Cf + off;
+                        if (pair) {
+                            if (acc_c) { const float2 o = *reinterpret_cast<const float2*>(cp); v0 += o.x; v1 += o.y; }
+                            *reinterpret_cast<float2*>(cp) = make_float2(v0, v1);
                         } else {
-                            float* cp = Cf + row * N + col;
-                            if (accumulate) {
-                                const float4 o = *reinterpret_cast<const float4*>(cp);
-                                v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w;
-                            }
-                            *reinterpret_cast<float4*>(cp) = v;
-                        }
-                    } else if (row < M) {                      // edge tile: element-wise, guarded
-                        const float vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            if (col + e >= N) continue;
-                            float x = vv[e];
-                            if (ksplit > 1) atomicAdd(Cf + row * N + col + e, x);
-                            else if (c_bf16) {
-                                __nv_bfloat16* cp = Ch + row * N + col + e;
-                                if (!LSE && lse.aux) { const float h = __bfloat162float(lse.aux[row * N + col + e]); x *= 1.f - h * h; }
-                                if (accumulate) x += __bfloat162float(*cp);
-                                *cp = __float2bfloat16(x);
-                            } else {
-                                float* cp = Cf + row * N + col + e;
-                                if (accumulate) x += *cp;
-                                *cp = x;
-                            }
+                            if (acc_c) { v0 += cp[0]; if (two) v1 += cp[1]; }
+                            cp[0] = v0;
+                            if (two) cp[1] = v1;
                         }
                     }
                 }
-                __syncwarp();
-            }
-            if (LSE && nb == num_n - 1) {                         // whole vocabulary seen: publish the row statistics
-                if (EPW_ == 8) {
-                    // the two warps of a TMEM quadrant saw alternate 32-column chunks: merge their running
-                    // (max, sum, x_blank, x_label) through the staging tile of the second one
-                    const uint32_t sb2 = smem_u32(epi) + (uint32_t)((warp - 2) | 4) * EPI_WARP_BYTES;
-                    if (chalf == 1)
-                        asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" :: "r"(sb2 + (uint32_t)lane * 16), "f"(rm), "f"(rs),
-                                     "f"(xb), "f"(xl) : "memory");
-                    asm volatile("bar.sync %0, 64;" :: "r"(1 + q) : "memory");
-                    if (chalf == 0) {
-                        float m2, s2, b2v, l2v;
-                        asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(m2), "=f"(s2), "=f"(b2v), "=f"(l2v)
-                                     : "r"(sb2 + (uint32_t)lane * 16) : "memory");
-                        const float m = fmaxf(rm, m2);
-                        rs = rs * fast_ex2((rm - m) * 1.4426950408889634f) + s2 * fast_ex2((m2 - m) * 1.4426950408889634f);
-                        rm = m; xb += b2v; xl += l2v;
-                    }
-                    asm volatile("bar.sync %0, 64;" :: "r"(1 + q) : "memory");
-                }
-                if (cell_ok && (EPW_ != 8 || chalf == 0)) {
-                    const long cell = m0 + q * 32 + lane;
-                    const float d = -(rm + logf(rs));
-                    lse.denom[cell] = d;
-                    lse.lpb[cell] = d + xb;
-                    lse.lpl[cell] = d + xl;
-                }
-            }
-            tc_fence_before();
-            if (lane == 0) {
-                if (PAIR_) mbar_arrive_remote(map_to_rank(tempty0 + 8 * acc, 0));
-                else mbar_arrive(tempty0 + 8 * acc);
             }
         }
     }
-    tc_fence_before();
-    if (PAIR_) cluster_sync_all();                           // neither CTA's shared / tensor memory goes away under the other
-    else __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        if (PAIR_) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "r"(TMEM_COLS) : "memory");
-        else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "r"(TMEM_COLS) : "memory");
+}
+
+// C[i] = (accumulate ? C[i] : 0) + part[0][i] + part[1][i] + ...: the split-K partial tiles added in split order
+__global__ void splitk_reduce_kernel(const float* __restrict__ part, int ksplit, long mn, float* __restrict__ C, int accumulate) {
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < mn; i += (long)gridDim.x * blockDim.x) {
+        float v = accumulate ? C[i] : 0.f;
+        for (int s = 0; s < ksplit; ++s) v += part[(long)s * mn + i];
+        C[i] = v;
     }
 }
 
 // split-K (weight gradients: few output tiles, contraction over up to millions of rows).  The persistent grid
-// processes tiles*ksplit work items in waves of one per worker (SM, or CTA pair); a ragged last wave idles most of
-// the machine (20 tiles x 15 splits = 300 items = 2.03 waves ran at 67 %), so ksplit is chosen to fill whole waves:
-// maximise  wave efficiency / (1 + r * ksplit / nkb):  items / (waves * workers) against the cost of one more
-// atomic tile epilogue per split, which was measured at r ~ 32 k-blocks of MMA time for the 128x256 tile
-// (lstm dW, 128 tiles, 500 k-blocks: ksplit 3 -> 228 us, 8 -> 254 us; joint dW2, 20 tiles, 32250 k-blocks:
-// ksplit 15 -> 3.7 ms, 22 -> 2.8 ms).  Partial tiles are reduced with fp32 atomics.
+// processes tiles*ksplit work items in waves of one per CTA; a ragged last wave idles most of the machine, so ksplit is
+// chosen to fill whole waves: maximise  wave efficiency / (1 + r * ksplit / nkb):  items / (waves * workers) against the
+// cost of one more partial tile per split, r k-blocks of MMA time.  Partial tiles go to a caller-provided workspace.
 int choose_ksplit(long out_tiles, long nkb, long workers, double r) {
     int ksplit = 1;
     long cap = nkb / 16;
@@ -517,117 +354,74 @@ int choose_ksplit(long out_tiles, long nkb, long workers, double r) {
     return ksplit;
 }
 
+// one persistent launch over `work` items, at most one CTA per SM
+template <bool A_MN, bool B_MN, int BN_, bool LSE, bool LOW_>
+int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_bf16, const float* bias, int accumulate,
+                  long M, int N, long K, int ksplit, long work, const LseArgs& ea, cudaStream_t st, float* part = nullptr) {
+    using C_ = Cfg<BN_, LOW_>;
+    auto kern = gemm_tc_kernel<A_MN, B_MN, BN_, LSE, LOW_>;
+    static bool attr_done = false;
+    if (!attr_done) {
+        EB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM_BYTES));
+        attr_done = true;
+    }
+    const int grid = (int)(work < eb_num_sms() ? work : eb_num_sms());
+    kern<<<grid, NTHREADS, C_::SMEM_BYTES, st>>>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, ksplit, ea, part);
+    EB_CHECK_LAUNCH();
+    if (ksplit > 1) {
+        const long mn = M * (long)N;
+        const long blocks = (mn + 255) / 256, cap = 4L * eb_num_sms();
+        splitk_reduce_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, st>>>(part, ksplit, mn, (float*)C, accumulate);
+        EB_CHECK_LAUNCH();
+    }
+    return EB_OK;
+}
+
 template <bool A_MN, bool B_MN, int BN_>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_bf16, const float* bias, int accumulate,
-           long M, int N, long K, cudaStream_t st, const void* aux = nullptr) {
+           long M, int N, long K, int ksplit, float* part, cudaStream_t st, const void* aux = nullptr) {
     LseArgs ea = LseArgs();
     ea.aux = reinterpret_cast<const __nv_bfloat16*>(aux);
-    constexpr int BN = BN_;
+    const long out_tiles = ((M + BM - 1) / BM) * ((N + BN_ - 1) / BN_);
+    return launch_kernel<A_MN, B_MN, BN_, false, false>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, ksplit,
+                                                        out_tiles * ksplit, ea, st, part);
+}
+
+// Tile width and split-K factor of a product (the one decision shared by eb_gemm_bf16_partials and the launch).
+void plan(int a_mn_major, int c_bf16, int accumulate, long M, int N, long K, int flags, bool& wide, int& ksplit) {
+    const bool low = (flags & EB_GEMM_CORESIDENT) != 0;
+    static int force_bn = -1;
+    if (force_bn < 0) { const char* e = getenv("EDGEDICT_GEMM_BN"); force_bn = e ? atoi(e) : 0; }
+    // 256-wide tiles when they tile N exactly and there is enough work to fill the machine with them
+    const long wide_tiles = ((M + BM - 1) / BM) * (N / 256);
+    // (split-K weight gradients take their parallelism from K: the wide tile only has to exist a few times -- it
+    //  moves 48 KB of operands per 128x256x64 block where two narrow tiles move 64 KB)
+    wide = (N % 256 == 0) && (wide_tiles >= eb_num_sms() || (!c_bf16 && (K + BK - 1) / BK >= 64 && wide_tiles >= 8));
+    // N = 256 k + 128 with many row blocks (the joint's d-hidden GEMM, N = 640): wide tiles with a half-empty last
+    // column tile move 20 % fewer operand bytes than 128-wide tiles for 20 % more (idle anyway) MMA issue
+    if (!wide && N % 256 == 128 && N >= 512 && (M + BM - 1) / BM >= 4L * eb_num_sms() && accumulate == 0) wide = true;
+    if (force_bn == 128) wide = false;
+    if (force_bn == 256 && N % 128 == 0) wide = true;
+    if (low) wide = false;
+    (void)a_mn_major;
+    const int BN = wide ? 256 : 128;
     const long out_tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
     const long nkb = (K + BK - 1) / BK;
-    int ksplit = 1;
-    if (!c_bf16 && nkb >= 64 && out_tiles < eb_num_sms()) ksplit = choose_ksplit(out_tiles, nkb, eb_num_sms(), BN == 256 ? 32.0 : 16.0);
-    if (ksplit > 1 && !accumulate) EB_CUDA(cudaMemsetAsync(C, 0, sizeof(float) * (size_t)M * N, st));
-    const long tiles = out_tiles * ksplit;
-    const int grid = (int)(tiles < eb_num_sms() ? tiles : eb_num_sms());
-    // short contraction per tile => the epilogue, not the MMA, paces the tile: use 8 epilogue warps
-    static int force_epw = -1;
-    if (force_epw < 0) { const char* e = getenv("EDGEDICT_GEMM_EPW"); force_epw = e ? atoi(e) : 0; }
-    const bool epi8 = force_epw ? (force_epw == 8) : ((K + ksplit - 1) / ksplit <= 2048);
-    if (epi8) {
-        auto kern = gemm_tc_kernel<A_MN, B_MN, BN_, false, 8>;
-        static bool attr_done = false;
-        if (!attr_done) {
-            EB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN_, 8>::SMEM_BYTES));
-            attr_done = true;
-        }
-        kern<<<grid, Cfg<BN_, 8>::NTHREADS, Cfg<BN_, 8>::SMEM_BYTES, st>>>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, ksplit, ea);
-    } else {
-        auto kern = gemm_tc_kernel<A_MN, B_MN, BN_, false, 4>;
-        static bool attr_done = false;
-        if (!attr_done) {
-            EB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN_, 4>::SMEM_BYTES));
-            attr_done = true;
-        }
-        kern<<<grid, Cfg<BN_, 4>::NTHREADS, Cfg<BN_, 4>::SMEM_BYTES, st>>>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, ksplit, ea);
-    }
-    EB_CHECK_LAUNCH();
-    return EB_OK;
+    ksplit = 1;
+    if (!low && !c_bf16 && nkb >= 64 && out_tiles < eb_num_sms())
+        ksplit = choose_ksplit(out_tiles, nkb, eb_num_sms(), BN == 256 ? 32.0 : 16.0);
 }
 
 // co-resident configuration (see Cfg): plain nt GEMM, narrow tile, no split-K
 int launch_low(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_bf16, const float* bias, int accumulate,
                long M, int N, long K, cudaStream_t st) {
-    using C_ = Cfg<128, 4, true>;
-    auto kern = gemm_tc_kernel<false, false, 128, false, 4, true>;
-    static bool attr_done = false;
-    if (!attr_done) {
-        EB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM_BYTES));
-        attr_done = true;
-    }
     const long tiles = ((M + BM - 1) / BM) * ((N + 127) / 128);
-    const int grid = (int)(tiles < eb_num_sms() ? tiles : eb_num_sms());
-    kern<<<grid, C_::NTHREADS, C_::SMEM_BYTES, st>>>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, 1, LseArgs());
-    EB_CHECK_LAUNCH();
-    return EB_OK;
+    return launch_kernel<false, false, 128, false, true>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, 1, tiles, LseArgs(), st);
 }
 
-// cta_group::2 configuration (see Cfg): clusters of two CTAs, one 256 x 256 tile per pair, 8 epilogue warps per CTA.
-// mode: EDGEDICT_GEMM_PAIR / eb_gemm_pair_mode -- -1 auto (bf16-output GEMMs with many row blocks), 0 never, 1 whenever legal
-int g_pair_mode = -2;
-int pair_mode() {
-    if (g_pair_mode == -2) { const char* e = getenv("EDGEDICT_GEMM_PAIR"); g_pair_mode = e ? atoi(e) : -1; }
-    return g_pair_mode;
-}
-
-template <bool A_MN, bool B_MN, bool LSE>
-int launch_pair(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_bf16, const float* bias, int accumulate,
-                long M, int N, long K, const LseArgs& ea, cudaStream_t st) {
-    using C_ = Cfg<256, 8, false, true>;
-    auto kern = gemm_tc_kernel<A_MN, B_MN, 256, LSE, 8, false, true>;
-    cudaLaunchConfig_t cfg = {};
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.blockDim = dim3(C_::NTHREADS); cfg.dynamicSmemBytes = C_::SMEM_BYTES; cfg.stream = st;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    static int max_pairs = 0;
-    if (!max_pairs) {
-        EB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM_BYTES));
-        cfg.gridDim = dim3(2 * (eb_num_sms() / 2));
-        int n = 0;
-        EB_CUDA(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
-        if (n <= 0) return EB_ERR_CUDA;
-        max_pairs = n < eb_num_sms() / 2 ? n : eb_num_sms() / 2;
-    }
-    const long out_tiles = ((M + 255) / 256) * ((N + 255) / 256), nkb = (K + BK - 1) / BK;
-    int ks1 = 1;                                             // split-K as in launch(), one work item per CTA pair
-    if (!LSE && !c_bf16 && nkb >= 64 && out_tiles < max_pairs) ks1 = choose_ksplit(out_tiles, nkb, max_pairs, 32.0);
-    if (ks1 > 1 && !accumulate) EB_CUDA(cudaMemsetAsync(C, 0, sizeof(float) * (size_t)M * N, st));
-    const long work = LSE ? (M + 255) / 256 : out_tiles * ks1;
-    const int pairs = (int)(work < max_pairs ? work : max_pairs);
-    cfg.gridDim = dim3(2 * pairs);
-    int c16 = c_bf16, acc = accumulate;
-    EB_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, C, c16, bias, acc, M, N, K, ks1, ea));
-    EB_CHECK_LAUNCH();
-    return EB_OK;
-}
-
-template <int BN_>
 int launch_lse(const CUtensorMap& ta, const CUtensorMap& tb, void* C, const float* bias, long M, int N, long K,
                const LseArgs& lse, cudaStream_t st) {
-    using C_ = Cfg<BN_, 8>;                                  // two epilogue warps per TMEM quadrant (see kernel)
-    auto kern = gemm_tc_kernel<false, false, BN_, true, 8>;
-    static bool attr_done = false;
-    if (!attr_done) {
-        EB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM_BYTES));
-        attr_done = true;
-    }
-    const long num_m = (M + BM - 1) / BM;
-    const int grid = (int)(num_m < eb_num_sms() ? num_m : eb_num_sms());
-    kern<<<grid, C_::NTHREADS, C_::SMEM_BYTES, st>>>(ta, tb, C, 1, bias, 0, M, N, K, 1, lse);
-    EB_CHECK_LAUNCH();
-    return EB_OK;
+    return launch_kernel<false, false, 128, true, false>(ta, tb, C, 1, bias, 0, M, N, K, 1, (M + BM - 1) / BM, lse, st);
 }
 
 }  // namespace
@@ -647,42 +441,42 @@ EB_API int eb_joint_logits_lse(const void* hidden16, const void* w2_16, const fl
         (b2 && (reinterpret_cast<uintptr_t>(b2) & 15)))
         return EB_ERR_INVALID;
     const long M = (long)B * maxT * maxU;
-    const bool wide = (V % 256 == 0);
-    // cta_group::2 tiles when there are enough 256-row blocks for every CTA pair: a third less L2 -> SM operand traffic
-    // (15.9 -> 10.6 GB per launch at E6D2, profiles/r2/prof_r2_gemm_pair.txt), 1.33 -> 1.25 ms alone, -0.3 ms per step
-    const bool pair = wide && (pair_mode() == 1 || (pair_mode() < 0 && (M + 255) / 256 >= 2L * (eb_num_sms() / 2)));
+    // 128-wide tiles: the softmax statistics of a 256-wide tile do not fit the registers beside its accumulators
     CUtensorMap ta, tb;
-    if (!make_map(&ta, hidden16, (uint64_t)J, (uint64_t)M, 128) ||
-        !make_map(&tb, w2_16, (uint64_t)J, (uint64_t)V, (wide && !pair) ? 256 : 128)) {
+    if (!make_map(&ta, hidden16, (uint64_t)J, (uint64_t)M, 128) || !make_map(&tb, w2_16, (uint64_t)J, (uint64_t)V, 128)) {
         fprintf(stderr, "[edgedict_b200] cuTensorMapEncodeTiled failed\n");
         return EB_ERR_CUDA;
     }
     LseArgs lse;
     lse.labels = labels; lse.xlen = xlen; lse.ylen = ylen; lse.denom = denom; lse.lpb = lpb; lse.lpl = lpl;
-    lse.maxT = maxT; lse.maxU = maxU; lse.blank = blank;
+    lse.maxT = maxT; lse.maxU = maxU; lse.blank = blank; lse.aux = nullptr;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    if (pair) return launch_pair<false, false, true>(ta, tb, logits16, 1, b2, 0, M, V, J, lse, st);
-    return wide ? launch_lse<256>(ta, tb, logits16, b2, M, V, J, lse, st) : launch_lse<128>(ta, tb, logits16, b2, M, V, J, lse, st);
-}
-
-EB_API int eb_gemm_pair_mode(int mode) {
-    const int prev = pair_mode();
-    g_pair_mode = mode < 0 ? -1 : (mode ? 1 : 0);
-    return prev;
+    return launch_lse(ta, tb, logits16, b2, M, V, J, lse, st);
 }
 
 EB_API int eb_gemm_bf16(const void* A, int a_mn_major, const void* B, int b_mn_major, void* C, int c_bf16,
                         const float* bias, int accumulate, long M, int N, long K, void* stream) {
-    return eb_gemm_bf16_ex(A, a_mn_major, B, b_mn_major, C, c_bf16, bias, accumulate, M, N, K, 0, stream);
+    return eb_gemm_bf16_ex(A, a_mn_major, B, b_mn_major, C, c_bf16, bias, accumulate, M, N, K, 0, nullptr, 0, stream);
 }
 
 static int gemm_dispatch(const void* A, int a_mn_major, const void* B, int b_mn_major, void* C, int c_bf16,
                          const float* bias, int accumulate, long M, int N, long K, int flags, const void* aux,
-                         void* stream);
+                         float* partials, long partial_floats, void* stream);
+
+// floats of split-K workspace eb_gemm_bf16_ex can use for this product (0: it runs without split-K)
+EB_API long eb_gemm_bf16_partials(int a_mn_major, int c_bf16, int accumulate, long M, int N, long K, int flags) {
+    if (M <= 0 || N <= 0 || K <= 0) return 0;
+    bool wide;
+    int ksplit;
+    plan(a_mn_major, c_bf16, accumulate, M, N, K, flags, wide, ksplit);
+    return ksplit > 1 ? (long)ksplit * M * N : 0;
+}
 
 EB_API int eb_gemm_bf16_ex(const void* A, int a_mn_major, const void* B, int b_mn_major, void* C, int c_bf16,
-                           const float* bias, int accumulate, long M, int N, long K, int flags, void* stream) {
-    return gemm_dispatch(A, a_mn_major, B, b_mn_major, C, c_bf16, bias, accumulate, M, N, K, flags, nullptr, stream);
+                           const float* bias, int accumulate, long M, int N, long K, int flags, float* partials,
+                           long partial_floats, void* stream) {
+    return gemm_dispatch(A, a_mn_major, B, b_mn_major, C, c_bf16, bias, accumulate, M, N, K, flags, nullptr, partials,
+                         partial_floats, stream);
 }
 
 // C16[M,N] = bf16( (A B) * (1 - hid16^2) ): the joint's d hidden GEMM with tanh' applied in the epilogue (Joint.forward's
@@ -690,64 +484,39 @@ EB_API int eb_gemm_bf16_ex(const void* A, int a_mn_major, const void* B, int b_m
 EB_API int eb_gemm_bf16_dtanh(const void* A, int a_mn_major, const void* B, int b_mn_major, void* C16,
                               const void* hid16, long M, int N, long K, void* stream) {
     if (!hid16 || (reinterpret_cast<uintptr_t>(hid16) & 7) || (reinterpret_cast<uintptr_t>(C16) & 7) || N % 4) return EB_ERR_INVALID;
-    return gemm_dispatch(A, a_mn_major, B, b_mn_major, C16, 1, nullptr, 0, M, N, K, 0, hid16, stream);
+    return gemm_dispatch(A, a_mn_major, B, b_mn_major, C16, 1, nullptr, 0, M, N, K, 0, hid16, nullptr, 0, stream);
 }
 
 static int gemm_dispatch(const void* A, int a_mn_major, const void* B, int b_mn_major, void* C, int c_bf16,
                          const float* bias, int accumulate, long M, int N, long K, int flags, const void* aux,
-                         void* stream) {
+                         float* partials, long partial_floats, void* stream) {
     if (!A || !B || !C || M <= 0 || N <= 0 || K <= 0) return EB_ERR_INVALID;
     const bool low = (flags & EB_GEMM_CORESIDENT) != 0;
     if (low && (a_mn_major || b_mn_major)) return EB_ERR_INVALID;
     if ((reinterpret_cast<uintptr_t>(A) & 15) || (reinterpret_cast<uintptr_t>(B) & 15)) return EB_ERR_INVALID;
     // contiguous dimension must keep row pitches 16-byte aligned
     if ((a_mn_major ? M : K) % 8 || (b_mn_major ? (long)N : K) % 8) return EB_ERR_INVALID;
-    // 256-wide tiles when they tile N exactly and there is enough work to fill the machine with them
-    static int force_bn = -1;
-    if (force_bn < 0) { const char* e = getenv("EDGEDICT_GEMM_BN"); force_bn = e ? atoi(e) : 0; }
-    const long wide_tiles = ((M + BM - 1) / BM) * (N / 256);
-    // (split-K weight gradients take their parallelism from K: the wide tile only has to exist a few times -- it
-    //  moves 48 KB of operands per 128x256x64 block where two narrow tiles move 64 KB, and these GEMMs sit at the
-    //  L2 -> SM limit, ~12-14 TB/s by l1tex__m_xbar2l1tex_read_bytes)
-    bool wide = (N % 256 == 0) && (wide_tiles >= eb_num_sms() || (!c_bf16 && (K + BK - 1) / BK >= 64 && wide_tiles >= 8));
-    // N = 256 k + 128 with many row blocks (the joint's d-hidden GEMM, N = 640): the 128-wide tiles are bound by
-    // L2 -> SM operand traffic (32 KB per 128x128x64 block); wide tiles with a half-empty last column tile move
-    // 20 % fewer bytes for 20 % more (idle anyway) MMA issue
-    if (!wide && N % 256 == 128 && N >= 512 && (M + BM - 1) / BM >= 4L * eb_num_sms() && accumulate == 0) wide = true;
-    if (force_bn == 128) wide = false;
-    if (force_bn == 256 && N % 128 == 0) wide = true;
-    if (low) wide = false;
-    // split-K weight gradients with both operands MN-major take pair tiles only on request (mode 1): the joint's dW2
-    // (1024 x 640 over 1 M lattice cells) runs 1.42 -> 1.11 ms alone, but inside the step -- on the side stream, next to
-    // the d-hidden GEMM -- the same-box A/B showed no gain (47.95 vs 48.0 ms), and the LSTM weight gradients lose 0.3 ms
-    const bool wgrad_pair = !c_bf16 && a_mn_major && b_mn_major && !low && N % 128 == 0 && N >= 256 && M >= 256 &&
-                            pair_mode() == 1;
-    if (wgrad_pair) wide = true;
-    if (pair_mode() == 1 && c_bf16 && !a_mn_major && !low && N % 128 == 0 && N >= 256) wide = true;   // (tests) any legal shape
-    // cta_group::2 pairs: bf16 outputs (no split-K), A K-major, wide tiles.  Automatic with enough 256-row blocks for
-    // every pair -- the joint's d-hidden GEMM, 1.53 -> 1.34 ms at E6D2 -- and on request (mode 1) for any legal shape.
-    const bool pair = wgrad_pair || (wide && c_bf16 && !a_mn_major &&
-                      (pair_mode() == 1 || (pair_mode() < 0 && (M + 255) / 256 >= 2L * (eb_num_sms() / 2))));
+    bool wide;
+    int ksplit;
+    plan(a_mn_major, c_bf16, accumulate, M, N, K, flags, wide, ksplit);
+    // split-K needs its workspace: with less (or none) the split count shrinks to what fits, down to no split
+    if (ksplit > 1) {
+        const long fit = (partials && (reinterpret_cast<uintptr_t>(partials) & 7) == 0) ? partial_floats / (M * (long)N) : 0;
+        if (fit < ksplit) ksplit = fit > 1 ? (int)fit : 1;
+    }
     CUtensorMap ta, tb;
     bool ok = a_mn_major ? make_map(&ta, A, (uint64_t)M, (uint64_t)K, 64) : make_map(&ta, A, (uint64_t)K, (uint64_t)M, 128);
     ok = ok && (b_mn_major ? make_map(&tb, B, (uint64_t)N, (uint64_t)K, 64)
-                           : make_map(&tb, B, (uint64_t)K, (uint64_t)N, (wide && !pair) ? 256 : 128));
+                           : make_map(&tb, B, (uint64_t)K, (uint64_t)N, wide ? 256 : 128));
     if (!ok) {
         fprintf(stderr, "[edgedict_b200] cuTensorMapEncodeTiled failed\n");
         return EB_ERR_CUDA;
     }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (low) return launch_low(ta, tb, C, c_bf16, bias, accumulate, M, N, K, st);
-    if (pair) {
-        LseArgs ea = LseArgs();
-        ea.aux = reinterpret_cast<const __nv_bfloat16*>(aux);
-        if (a_mn_major) return launch_pair<true, true, false>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, ea, st);
-        return b_mn_major ? launch_pair<false, true, false>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, ea, st)
-                          : launch_pair<false, false, false>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, ea, st);
-    }
-#define EB_GO(AM, BMN)                                                                              \
-    return wide ? launch<AM, BMN, 256>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, st, aux)      \
-                : launch<AM, BMN, 128>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, st, aux)
+#define EB_GO(AM, BMN)                                                                                          \
+    return wide ? launch<AM, BMN, 256>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, ksplit, partials, st, aux) \
+                : launch<AM, BMN, 128>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, ksplit, partials, st, aux)
     if (a_mn_major) {
         if (b_mn_major) { EB_GO(true, true); }
         EB_GO(true, false);

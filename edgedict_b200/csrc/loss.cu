@@ -1,4 +1,4 @@
-// loss.cu -- RNN-Transducer loss for sm_100a.
+// loss.cu -- RNN-Transducer loss for sm_90a.
 //
 // Replaces the reference's GPU path  warp-transducer/include/detail/gpu_rnnt.h:82-215
 // (memset + reduce_max + reduce_exp + alphas + betas + grad + D2H, three host syncs) with
@@ -490,7 +490,7 @@ rnntStatus_t compat_entry(const T* acts, T* grads, const int* labels, const int*
     if (o.loc != RNNT_GPU) {
         // The reference prints a diagnostic when the requested location is not compiled in
         // (rnnt_entrypoint.cpp:86-88).  This library is GPU-only by design: no CPU fallback.
-        fprintf(stderr, "CPU execution requested, but edgedict_b200 is a GPU-only (sm_100a) build\n");
+        fprintf(stderr, "CPU execution requested, but edgedict_b200 is a GPU-only (sm_90a) build\n");
         return RNNT_STATUS_EXECUTION_FAILED;
     }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(o.stream);

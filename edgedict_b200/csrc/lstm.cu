@@ -1,4 +1,4 @@
-// lstm.cu -- persistent-RNN LSTM layer, fp32 (parity mode), sm_100a.
+// lstm.cu -- persistent-RNN LSTM layer, fp32 (parity mode), sm_90a.
 //
 // Replaces the recurrent half of nn.LSTM (rnnt/models.py:45-46,64-65 encoder layers,
 // :145-147,154-155 predictor): the input projection W_ih*x + b_ih + b_hh for all timesteps is a

@@ -1,4 +1,4 @@
-// lstm_c4.cu -- persistent-RNN LSTM layer on tcgen05 tensor cores inside thread-block clusters (bf16 operands,
+// lstm_c4.cu -- persistent-RNN LSTM layer on wgmma tensor cores inside thread-block clusters (bf16 operands,
 // fp32 accumulate / state): the bf16-mode recurrent kernels for H % 256 == 0, H <= 1024 (the encoder and predictor
 // sizes of every BASELINE config except E4D1, which keeps lstm_tc.cu).
 //
@@ -9,27 +9,26 @@
 // [r*H/4, (r+1)*H/4) of h_{t-1} for ALL 128 gate rows of its cluster:
 //   * its W_hh slice [128 x H/4] bf16 (64 KB at H = 1024) is staged ONCE into shared memory in the canonical
 //     K-major 128B-swizzle layout and stays there for the whole sequence -- no weight lives in registers;
-//   * per step ONE thread waits on the grid barrier, pulls the CTA's K slice of h_{t-1} (32 x H/4 bf16 = 16 KB,
-//     a quarter of what a full-K design pulls: the L2 -> SM fabric was the limiter of lstm_tc.cu) with TMA into
-//     swizzled shared memory and issues H/64 tcgen05.mma (M128 N32 K16), accumulator [128 gate rows x 32 batch]
-//     fp32 in TENSOR MEMORY;
-//   * the four TMEM lane quadrants are the partial sums destined to the four CTAs of the cluster: warp q reads
-//     its quadrant with tcgen05.ld and pushes it into CTA q's shared memory through DISTRIBUTED SHARED MEMORY
-//     (st.shared::cluster) and arrives on CTA q's mbarrier (release.cluster) -- no cluster-wide barrier;
+//   * per step the CTA waits on the grid barrier of its K slice, pulls the slice of h_{t-1} (32 x H/4 bf16 = 16 KB,
+//     a quarter of what a full-K design pulls) into swizzled shared memory and its warpgroup issues wgmma
+//     (M64 N32 K16), accumulator [128 gate rows x 32 batch] fp32 in registers;
+//   * the four 32-row blocks of the accumulator are the partial sums destined to the four CTAs of the cluster: they
+//     are staged in shared memory and the three remote ones are pushed into the peers' shared memory by DSMEM bulk
+//     copies that complete on the destination's mbarrier -- no cluster-wide barrier;
 //   * every CTA adds the four partials of its own 8 units, applies the gates thread-locally (two (unit, batch)
 //     pairs per thread, cell state in registers), publishes h_t in bf16 (16 B per batch row) and arrives on the
 //     grid barrier; y, the h_{t-1}-shifted bf16 copy for the weight-gradient GEMM and the saved gates / cell
 //     states leave after the arrival, as full 16-byte / 8-byte coalesced stores in a CTA-private layout.
 // Backward (BPTT): the same structure with the roles of the operands swapped: a cluster of CS (8, else 4) CTAs
-// owns 8*CS units; rank r contracts over the K slice [r*4H/CS, ...) of dG_t (tcgen05.mma M64 N32 K16:
-// rows = units, the M = 64 accumulator occupies lanes 0-15 of each TMEM quadrant), the partial dh tiles are
-// pushed through DSMEM, and the gate-gradient math of step t-1 runs on the owning threads with dh/dc in
-// registers.  The exchange buffer orders the contraction index as k' = 32*cta + 8*pair + 2*gate + e so that a
-// thread publishes its eight gate gradients with one 16-byte store.
+// owns 8*CS units; rank r contracts over the K slice [r*4H/CS, ...) of dG_t (wgmma M64 N32 K16: rows = units; for
+// CS = 4 rows 32-63 are discarded), the partial dh tiles are pushed through DSMEM (st.shared::cluster), and the
+// gate-gradient math of step t-1 runs on the owning threads with dh/dc in registers.  The exchange buffer orders the
+// contraction index as k' = 32*cta + 8*pair + 2*gate + e so that a thread publishes its eight gate gradients with
+// one 16-byte store.
 #include <cuda.h>
 #include <stdlib.h>
 #include "common.cuh"
-#include "sm100.cuh"
+#include "sm90.cuh"
 #include "../../include/edgedict_b200.h"
 
 namespace {
@@ -39,10 +38,7 @@ constexpr int UPC = 8;            // hidden units finalised per CTA
 constexpr int RP = 36;            // floats per row of the DSMEM receive tiles (16-byte aligned, conflict-free)
 // forward receive / staging tiles: [src or dest][32 rows][32 floats], 16-byte chunk c of row r stored at chunk c ^ (r & 7)
 __device__ __forceinline__ int swz(int row, int b) { return row * 32 + ((((b >> 2) ^ (row & 7)) << 2) | (b & 3)); }
-__device__ __forceinline__ void st_shared_f4(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-    asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" :: "r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-constexpr int NGT = 128;          // gate threads (warps 0-3); warp 4 = barrier poller / TMA / MMA issuer
+constexpr int NGT = 128;          // gate threads (warps 0-3, one warpgroup); backward: warp 4 = barrier poller / TMA
 constexpr int NTHR = 160;
 constexpr size_t C4_HDR = 4096;   // scratch: grid barrier counters, one per K slice, 1 KB apart (different L2 slices)
 constexpr int CTR_STRIDE = 256;   // uints between two slice counters
@@ -82,36 +78,6 @@ __device__ __forceinline__ uint32_t cluster_id_x() {
     return r;
 }
 __device__ __forceinline__ void named_bar_gate() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc32(uint32_t slot_saddr) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 32;" :: "r"(slot_saddr) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc_n(uint32_t slot_saddr, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(slot_saddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_free_n(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(taddr), "r"(ncols) : "memory");
-}
-// 32 consecutive 32-bit columns of this thread's TMEM lane <- registers
-__device__ __forceinline__ void tc_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-        "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-        :: "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-           "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-           "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-           "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31]) : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]: the A operand read from TENSOR MEMORY (lane = row, two bf16 per 32-bit column along K)
-__device__ __forceinline__ void tc_mma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n"
-                 " tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n}\n"
-                 :: "r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_free32(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 32;" :: "r"(taddr) : "memory");
-}
 
 // ---------------------------------------------------------------------------------------------------------
 struct C4FwdP {
@@ -124,12 +90,12 @@ struct C4FwdP {
     uint4* gsave;                 // [T][H/8][128] post-activation gates, bf16 (i0 i1 f0 f1 g0 g1 o0 o1); may be null
     float2* csave;                // [T][H/8][128] cell states; may be null
     __nv_bfloat16* hx;            // [2][NB][H] exchange
-    unsigned* bar;                // grid barrier counter (one flag per CTA + a polling warp measured 1000 cycles SLOWER)
+    unsigned* bar;                // grid barrier counters (one per K slice)
     long long* trace;             // debug: [steps][16] clock64 stamps of CTA 0 (eb_lstm_c4_set_trace), else null
     int trace_steps;
     float* gates_std; float* cseq_std;   // optional saves in the layout of eb_lstm_tc_bwd: [B,T,4H] gates, [B,T,H] cells (fp32)
-    int wpoll;                    // every warp polls the barrier counter itself instead of one poller + block barrier (default;
-                                  // EDGEDICT_LSTM_WPOLL bit 0 = this kernel, bit 1 = the BPTT kernel: -0.15 / -1.05 ms per step)
+    int wpoll;                    // every warp polls the barrier counter itself instead of one poller + block barrier
+                                  // (EDGEDICT_LSTM_WPOLL bit 0 = this kernel, bit 1 = the BPTT kernel)
     int B, T, H;
 };
 
@@ -137,39 +103,30 @@ __device__ __forceinline__ void cp_async16(uint32_t saddr, const void* gmem) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"(saddr), "l"(gmem) : "memory");
 }
 
-// TA: the W_hh slice lives in TENSOR MEMORY (A operand of tcgen05.mma from TMEM: 128 lanes x H/8 columns) instead of shared
-// memory: the MMAs stop re-reading 64 KB of shared memory per step (4 KB per MMA at 128 B/clk was what paced them, and two
-// co-resident CTAs shared that bandwidth) and the CTA's shared-memory footprint drops from 111 KB to 46 KB.
-// NACC: independent accumulators (k step j goes to accumulator j % NACC, summed by the epilogue): back-to-back tcgen05.mma
-// into ONE accumulator with N = 32 run at ~75 cycles each whatever the operand source -- a dependent chain, not a bandwidth limit.
-// MINB: register budget as CTAs per SM (2 -> 255, 3 -> 168, 4 -> 128 registers per thread).  Two of these CTAs share an SM in the
-// layer wavefront; at 232 registers they left 6 K of the SM's 64 K registers, so that neither the LayerNorm nor anything else of
-// the wavefront could run beside them; 168 registers cost 8 bytes more stack (EDGEDICT_C4_MINB).
-template <bool TA, int NACC, int MINB = 3>
-__global__ void __launch_bounds__(NGT, MINB) lstm_c4_fwd_kernel(C4FwdP p) {
+// The CTA is one warpgroup.  Its W_hh slice [128 gate rows x H/4] stays in shared memory for the whole sequence; per step
+// the warpgroup issues H/64 x 2 wgmma (M64 N32 K16: gate rows [0,64) and [64,128) against the 32 batch rows of h_{t-1}).
+// Three CTAs per SM fit the register budget (168 per thread); two fit the shared memory at H = 1024.
+__global__ void __launch_bounds__(NGT, 3) lstm_c4_fwd_kernel(C4FwdP p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const int H = p.H, B = p.B, T = p.T;
-    const int KS = H >> 2, NA = TA ? 0 : (KS >> 6), NAT = KS >> 6;   // K slice per CTA, 64-wide swizzle atoms in it
+    const int KS = H >> 2, NA = KS >> 6;                     // K slice per CTA, 64-wide swizzle atoms in it
     const int NC = H / UPC;
     const int CPR = KS >> 3;                                 // 16-byte chunks per row of the h slice (8 .. 32)
     const int NLD = CPR >> 2;                                // chunks per thread and step: 32 rows * CPR / 128
-    uint8_t* sA = smem;                                      // [NA][128 rows][128 B]   W_hh slice, resident (not TA)
-    uint8_t* sB = sA + NA * 16384;                           // [NAT][32 rows][128 B]   h_{t-1} slice of the step
+    uint8_t* sA = smem;                                      // [NA][128 rows][128 B]   W_hh slice, resident
+    uint8_t* sB = sA + NA * 16384;                           // [NA][32 rows][128 B]    h_{t-1} slice of the step
     float* stage = reinterpret_cast<float*>(sB + 16384);     // [4 dest][32 rows][32]   outgoing partial tiles (swz)
     float* recv = stage + 4 * 1024;                          // [3 src][32 rows][32]    incoming partial tiles (swz)
     uint64_t* bars = reinterpret_cast<uint64_t*>(recv + 3 * 1024);
-    const uint32_t accb = smem_u32(bars), rbar = smem_u32(bars + 1);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3);
+    const uint32_t rbar = smem_u32(bars);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const uint32_t rank = cluster_ctarank();
     const int grp = (int)cluster_id_x();
     const int cta = grp * 4 + (int)rank;                     // owner of units [8 cta, 8 cta + 8)
     const unsigned ncta = gridDim.x;
-    const uint32_t acols = (KS / 2 <= 32) ? 32u : (KS / 2 <= 64) ? 64u : 128u;     // TMEM columns of the A slice (power of 2)
 
     // W_hh slice -> shared (row m = 32*dest_rank + 8*gate + unit; K-major, 128B swizzle)
-    if (!TA)
     for (int idx = tid; idx < 128 * CPR; idx += NGT) {
         const int m = idx / CPR, cc = idx - m * CPR;
         const int q = m >> 5, gate = (m >> 3) & 3, u = m & 7;
@@ -179,40 +136,12 @@ __global__ void __launch_bounds__(NGT, MINB) lstm_c4_fwd_kernel(C4FwdP p) {
         *reinterpret_cast<uint4*>(sA + a * 16384 + m * 128 + ((c ^ (m & 7)) << 4)) = v;
     }
     if (tid == 0) {
-        mbar_init(accb, NACC == 4 ? (uint32_t)NAT : 1u);     // one tcgen05.commit per issuing thread
         mbar_init(rbar, 1);                                  // one local arrive.expect_tx per step + 3 x 4 KB of copies
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 0) {
-        if (TA) tmem_alloc_n(smem_u32(tmem_slot + 1), acols);
-        tmem_alloc_n(smem_u32(tmem_slot), 32u * NACC);
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     fence_proxy_async();                                     // the A tile was written through the generic proxy
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
     cluster_sync_all();                                      // peers' mbarriers exist before any copy completes on them
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tmem_a = TA ? tmem_slot[1] : 0u;
-    if (TA) {
-        // row m = 32*warp + lane of the slice (gate = lane / 8, unit = lane % 8 of destination rank `warp`): its KS bf16 are
-        // KS/2 consecutive 32-bit TMEM columns of lane m (element k in the low half of column k/2 for even k)
-        const __nv_bfloat16* src = p.whh + ((size_t)(lane >> 3) * H + 32 * grp + 8 * warp + (lane & 7)) * H + (size_t)rank * KS;
-        for (int c0 = 0; c0 < KS / 2; c0 += 32) {
-            uint32_t r[32];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const uint4 v = *reinterpret_cast<const uint4*>(src + (size_t)(c0 + 4 * i) * 2);
-                r[4 * i] = v.x; r[4 * i + 1] = v.y; r[4 * i + 2] = v.z; r[4 * i + 3] = v.w;
-            }
-            tc_st32(tmem_a + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, r);
-        }
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-        tc_fence_before();
-        __syncthreads();
-        tc_fence_after();
-    }
 
     const int b = tid >> 2, up = tid & 3;
     const int j = cta * UPC + 2 * up;
@@ -229,7 +158,7 @@ __global__ void __launch_bounds__(NGT, MINB) lstm_c4_fwd_kernel(C4FwdP p) {
     }
     __syncthreads();
     // Grid barrier per K SLICE: the CTA of rank r only consumes the h units of slice r, produced by the NC/4 CTAs
-    // [r*NC/4, (r+1)*NC/4): it waits for those arrivals alone (counter r, 128 bytes apart).  Every cluster consumes
+    // [r*NC/4, (r+1)*NC/4): it waits for those arrivals alone (counter r, 1 KB apart).  Every cluster consumes
     // all four slices, so no CTA can run a step ahead of any producer and the double-buffered exchange stays safe.
     const unsigned nprod = ncta >> 2;
     unsigned* const my_ctr = p.bar + (cta / (int)nprod) * CTR_STRIDE;
@@ -240,48 +169,35 @@ __global__ void __launch_bounds__(NGT, MINB) lstm_c4_fwd_kernel(C4FwdP p) {
 #pragma unroll
     for (int g = 0; g < 4; ++g) xr[g] = own ? __ldg(reinterpret_cast<const float2*>(xgp + (size_t)g * H)) : make_float2(0.f, 0.f);
     size_t oy = (size_t)b * T * H + j;
-    const uint32_t stage_w = smem_u32(stage) + (uint32_t)warp * 4096u;            // tile destined to CTA `warp`
-    const uint32_t slot_at_dst = (rank < (uint32_t)warp) ? rank : rank - 1;       // my slot in CTA `warp`'s recv
-    const uint32_t push_dst = map_to_rank(smem_u32(recv) + slot_at_dst * 4096u, (uint32_t)warp);
-    const uint32_t rbar_dst = map_to_rank(rbar, (uint32_t)warp);
+    // thread d < 4 (d != rank) hands the partial tile destined to CTA d to the copy engine
+    const uint32_t dst = (uint32_t)(tid & 3);
+    const uint32_t slot_at_dst = (rank < dst) ? rank : rank - 1;                  // my slot in CTA dst's recv
+    const uint32_t push_dst = map_to_rank(smem_u32(recv) + slot_at_dst * 4096u, dst);
+    const uint32_t rbar_dst = map_to_rank(rbar, dst);
     const int ro0 = swz(2 * up, b), ro1 = swz(2 * up + 1, b);     // (row & 7) is the same for every gate / source
     const float* own_tile = stage + rank * 1024;
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(NB >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
     const uint32_t sa = smem_u32(sA), sb = smem_u32(sB);
     // pull map: chunk q = i*128 + tid of the [32 rows][CPR chunks] slice (CPR divides 128 or is 24)
     const bool regular = (NGT % CPR) == 0;
     const int cc0 = tid % CPR, rw0 = tid / CPR, rstep = NGT / CPR;
+    // accumulator fragment rows of this thread: m = 64*mi + 16*warp + lane/4 + 8*h -> destination m/32, row m%32
+    const int frow = 16 * (warp & 1) + (lane >> 2), fcol = 2 * (lane & 3);
 
     for (int t = 0; t < T; ++t) {
         const uint32_t ph = (uint32_t)(t & 1);
-        // ---- grid barrier: every CTA has published h_{t-1}; one poller, then the block
+        // ---- grid barrier: every producer of my K slice has published h_{t-1}
         if (p.wpoll) {
             if (lane == 0) spin_wait_ge(wait_ctr, (unsigned)(t + 1) * nprod);
             __syncwarp();
         } else {
-            if (tid == 0) spin_wait_ge(wait_ctr, (unsigned)(t + 1) * nprod);   // (a back-off between polls changes nothing: measured)
+            if (tid == 0) spin_wait_ge(wait_ctr, (unsigned)(t + 1) * nprod);
             __syncthreads();
         }
         if (tid == 0) C4_STAMP(t, 0);
         // ---- A. pull this CTA's K slice of h_{t-1} (L2 -> swizzled shared tile)
-        if (NACC == 4) {
-            // warp a pulls swizzle atom a (32 rows x 64 k = 4 KB) and issues its MMAs as soon as ITS data is there: no
-            // block barrier between the pull and the MMAs
-            if (warp < NAT) {
-                const __nv_bfloat16* src = p.hx + (size_t)((t + 1) & 1) * xstride + (size_t)rank * KS + warp * 64;
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const int row = i * 4 + (lane >> 3), c = lane & 7;
-                    cp_async16(sb + (uint32_t)(warp * 4096 + row * 128 + ((c ^ (row & 7)) << 4)), src + (size_t)row * H + c * 8);
-                }
-                asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
-                if (tid == 0) C4_STAMP(t, 9);
-                fence_proxy_async_smem();
-                __syncwarp();
-            }
-        } else {
+        {
             const __nv_bfloat16* src = p.hx + (size_t)((t + 1) & 1) * xstride + (size_t)rank * KS;
-            // cp.async straight into the swizzled tile (register staging + st.shared measured 450 cycles slower)
+            // cp.async straight into the swizzled tile
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
                 if (i < NLD) {
@@ -292,76 +208,48 @@ __global__ void __launch_bounds__(NGT, MINB) lstm_c4_fwd_kernel(C4FwdP p) {
                 }
             }
             asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
-            if (tid == 0) C4_STAMP(t, 9);
             fence_proxy_async_smem();
             __syncthreads();
         }
-        if (NACC == 4) {
-            // One thread issues a tcgen05.mma every ~75 cycles whatever its size or operand source (measured: shared-memory
-            // or tensor-memory A, 1 / 2 / 4 accumulators all give 1230 cycles for 16 MMAs), so the K slice is issued by FOUR
-            // threads in parallel: lane 0 of warp a issues the four k steps of swizzle atom a into accumulator a and commits
-            // them itself (tcgen05.commit tracks the MMAs of the executing thread; the barrier counts NAT arrivals).
-            if (lane == 0 && warp < NAT) {
-                if (tid == 0) C4_STAMP(t, 1);
-                tc_fence_after();
-                const int a = warp;
-                const uint32_t d = tmem_base + (uint32_t)a * 32u;
+        if (tid == 0) { C4_STAMP(t, 1); mbar_expect_tx(rbar, 3 * 4096); }
+        // ---- B. partial gate pre-activations of the cluster's 128 gate rows over my K slice
+        float acc0[16], acc1[16];
 #pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    if (TA) tc_mma_bf16_ts(d, tmem_a + (uint32_t)(a * 4 + k) * 8u, make_desc(sb + a * 4096 + k * 32, 0, 1024), idesc, k ? 1u : 0u);
-                    else tc_mma_bf16(d, make_desc(sa + a * 16384 + k * 32, 0, 1024), make_desc(sb + a * 4096 + k * 32, 0, 1024), idesc,
-                                     k ? 1u : 0u);
-                }
-                tc_commit(accb);
-                if (tid == 0) { C4_STAMP(t, 2); mbar_expect_tx(rbar, 3 * 4096); }
-            }
-        } else if (tid == 0) {
-            C4_STAMP(t, 1);
-            tc_fence_after();
-            for (int a = 0; a < NAT; ++a) {
+        for (int i = 0; i < 16; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+        wgmma_fence();
+        for (int a = 0; a < NA; ++a) {
 #pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const int j = a * 4 + k;
-                    const uint32_t d = tmem_base + (uint32_t)(j % NACC) * 32u, accum = j >= NACC ? 1u : 0u;
-                    if (TA) tc_mma_bf16_ts(d, tmem_a + (uint32_t)j * 8u, make_desc(sb + a * 4096 + k * 32, 0, 1024), idesc, accum);
-                    else tc_mma_bf16(d, make_desc(sa + a * 16384 + k * 32, 0, 1024),
-                                     make_desc(sb + a * 4096 + k * 32, 0, 1024), idesc, accum);
-                }
+            for (int k = 0; k < 4; ++k) {
+                const uint64_t bd = make_desc(sb + a * 4096 + k * 32, 16, 1024);
+                wgmma_m64n32k16<0, 0>(acc0, make_desc(sa + a * 16384 + k * 32, 16, 1024), bd, 1);
+                wgmma_m64n32k16<0, 0>(acc1, make_desc(sa + a * 16384 + 8192 + k * 32, 16, 1024), bd, 1);
             }
-            tc_commit(accb);
-            C4_STAMP(t, 2);
-            mbar_expect_tx(rbar, 3 * 4096);
         }
-        mbar_wait(accb, ph);
-        tc_fence_after();
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc0);
+        wgmma_fence_regs(acc1);
+        if (tid == 0) C4_STAMP(t, 2);
+        // ---- C. reduce the partial tiles across the cluster: stage the four 32-row blocks (block q = the partial sums
+        // of CTA q's 32 gate rows), hand the three remote ones to the copy engine (DSMEM bulk copies complete on the
+        // destination's mbarrier)
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi) {
+            const float* accv = mi ? acc1 : acc0;
+            float* tile = stage + (2 * mi + (warp >> 1)) * 1024;
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+                    *reinterpret_cast<float2*>(tile + swz(frow + 8 * h, 8 * i + fcol)) =
+                        make_float2(accv[4 * i + 2 * h], accv[4 * i + 2 * h + 1]);
+        }
+        fence_proxy_async_smem();
+        __syncthreads();                                     // every partial tile is staged
+        if (tid < 4 && dst != rank) bulk_s2c(push_dst, smem_u32(stage) + dst * 4096u, 4096u, rbar_dst);
         if (tid == 0) C4_STAMP(t, 3);
-        // ---- B. reduce the partial tiles across the cluster: stage the four TMEM quadrants (quadrant q = the partial
-        // sums of CTA q's 32 gate rows), hand the three remote ones to the copy engine (DSMEM bulk copies complete on
-        // the destination's mbarrier; per-thread st.shared::cluster pushes measured 2100 cycles against 1250)
-        uint32_t r[32];
-        tc_ld32(tmem_base + ((uint32_t)(warp * 32) << 16), r);
-#pragma unroll
-        for (int q = 1; q < NACC; ++q) {
-            if (NACC == 4 && q >= NAT) break;                // one accumulator per swizzle atom of the K slice
-            uint32_t r2[32];
-            tc_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)q * 32u, r2);
-#pragma unroll
-            for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) + __uint_as_float(r2[i]));
-        }
-        tc_fence_before();
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-            st_shared_f4(stage_w + (uint32_t)lane * 128u + (uint32_t)((i ^ (lane & 7)) << 4), r[4 * i], r[4 * i + 1],
-                         r[4 * i + 2], r[4 * i + 3]);
-        if ((uint32_t)warp != rank) {
-            fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) bulk_s2c(push_dst, stage_w, 4096u, rbar_dst);
-        }
-        if (tid == 0) C4_STAMP(t, 4);
-        __syncthreads();                                     // the tile for myself is staged
         mbar_wait_cluster(rbar, ph);
-        if (tid == 0) C4_STAMP(t, 5);
+        if (tid == 0) C4_STAMP(t, 4);
         float pre[4][2];
 #pragma unroll
         for (int g = 0; g < 4; ++g) {
@@ -384,13 +272,12 @@ __global__ void __launch_bounds__(NGT, MINB) lstm_c4_fwd_kernel(C4FwdP p) {
         if (!own) { hn0 = 0.f; hn1 = 0.f; }
         const uint32_t hp = pack2(hn0, hn1);
         *reinterpret_cast<uint32_t*>(p.hx + (size_t)(t & 1) * xstride + (size_t)b * H + j) = hp;
-        if (tid == 0) C4_STAMP(t, 6);
+        if (tid == 0) C4_STAMP(t, 5);
         __syncthreads();
         if (tid == 0) {
-            C4_STAMP(t, 7);
             __threadfence();
-            C4_STAMP(t, 8);
             atomicAdd(my_ctr, 1u);
+            C4_STAMP(t, 6);
         }
         // everything below overlaps the other CTAs' progress towards the barrier
         if (own) {
@@ -419,14 +306,8 @@ __global__ void __launch_bounds__(NGT, MINB) lstm_c4_fwd_kernel(C4FwdP p) {
             for (int g = 0; g < 4; ++g) xr[g] = __ldg(reinterpret_cast<const float2*>(xgp + (size_t)g * H));
         }
     }
-    tc_fence_before();
     __syncthreads();
     cluster_sync_all();                                      // no CTA exits while a peer may still address its smem
-    if (warp == 0) {
-        tc_fence_after();
-        tmem_free_n(tmem_base, 32u * NACC);
-        if (TA) tmem_free_n(tmem_a, acols);
-    }
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -440,11 +321,15 @@ struct C4BwdP {
     float* dh0; float* dc0;
     __nv_bfloat16* gx;            // [2][NB][4H] exchange, contraction index k' = 32*cta + 8*pair + 2*gate + e
     unsigned* bar;
-    long long* trace;
-    int trace_steps;
     int B, T, H;
 };
 
+__device__ __forceinline__ void st_cluster_f2(uint32_t caddr, float a, float b) {
+    asm volatile("st.shared::cluster.v2.f32 [%0], {%1,%2};" :: "r"(caddr), "f"(a), "f"(b) : "memory");
+}
+
+// Warps 0-3 (one warpgroup): gate-gradient math of the owned (unit, batch) pairs and the wgmma of the step; warp 4: grid
+// barrier poller and TMA producer of the dG_t slice.
 template <int CS>
 __global__ void __launch_bounds__(NTHR, CS == 8 ? 2 : 1) lstm_c4_bwd_kernel(const __grid_constant__ CUtensorMap gmap, C4BwdP p) {
     constexpr int MR = 8 * CS;                               // valid accumulator rows (units of the cluster)
@@ -457,8 +342,7 @@ __global__ void __launch_bounds__(NTHR, CS == 8 ? 2 : 1) lstm_c4_bwd_kernel(cons
     uint8_t* sB = sA + (size_t)NA * APITCH;                  //  an atom alias the next atom / the B tile: discarded rows)
     float* recv = reinterpret_cast<float*>(sB + NA * 4096);  // [CS src][8 units][RP]
     uint64_t* bars = reinterpret_cast<uint64_t*>(recv + CS * 8 * RP);
-    const uint32_t full0 = smem_u32(bars), accb = smem_u32(bars + 4), rbar = smem_u32(bars + 5);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 6);
+    const uint32_t full0 = smem_u32(bars), rbar = smem_u32(bars + 5);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const uint32_t rank = cluster_ctarank();
     const int grp = (int)cluster_id_x();
@@ -485,18 +369,13 @@ __global__ void __launch_bounds__(NTHR, CS == 8 ? 2 : 1) lstm_c4_bwd_kernel(cons
     }
     if (tid == 0) {
         for (int a = 0; a < 4; ++a) mbar_init(full0 + 8 * a, 1);
-        mbar_init(accb, 1);
         mbar_init(rbar, CS);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" :: "l"(&gmap) : "memory");
     }
-    if (warp == 4) tmem_alloc32(smem_u32(tmem_slot));
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
     cluster_sync_all();
-    const uint32_t tmem_base = *tmem_slot;
     const size_t xstride = (size_t)NB * H4;
     const int NQ = NA >> 2;                                  // atoms per TMA barrier (4 barriers)
 
@@ -507,13 +386,16 @@ __global__ void __launch_bounds__(NTHR, CS == 8 ? 2 : 1) lstm_c4_bwd_kernel(cons
         float dh0v = 0.f, dh1v = 0.f, dc0v = 0.f, dc1v = 0.f;
         if (own && p.dhT) { dh0v = p.dhT[(size_t)b * H + j]; dh1v = p.dhT[(size_t)b * H + j + 1]; }
         if (own && p.dcT) { dc0v = p.dcT[(size_t)b * H + j]; dc1v = p.dcT[(size_t)b * H + j + 1]; }
-        // M = 64 accumulator: row 16*warp + lane (lane < 16) -> destination rank row / 8
-        const int row = 16 * warp + lane;
-        const bool pusher = lane < 16 && row < MR;
-        const uint32_t dstrank = (uint32_t)(row >> 3) % CS;
-        const uint32_t push = map_to_rank(smem_u32(recv) + (uint32_t)((rank * 8 + (row & 7)) * RP) * 4u, dstrank);
-        const uint32_t rbar_dst = map_to_rank(rbar, dstrank);
+        // M = 64 accumulator fragment: rows 16*warp + lane/4 + 8*h (h = 0, 1) = units of destination rank 2*warp + h
+        const int frow = 16 * warp + (lane >> 2), fcol = 2 * (lane & 3);
+        const bool push0 = frow < MR, push1 = frow + 8 < MR;
+        const uint32_t rslot = smem_u32(recv) + (uint32_t)((rank * 8 + (frow & 7)) * RP + fcol) * 4u;
+        const uint32_t dst0 = push0 ? map_to_rank(rslot, (uint32_t)(frow >> 3)) : 0u;
+        const uint32_t dst1 = push1 ? map_to_rank(rslot, (uint32_t)((frow + 8) >> 3)) : 0u;
+        const uint32_t rbar0 = push0 ? map_to_rank(rbar, (uint32_t)(2 * warp)) : 0u;
+        const uint32_t rbar1 = push1 ? map_to_rank(rbar, (uint32_t)(2 * warp + 1)) : 0u;
         const float* rbase = recv + (2 * up) * RP + b;
+        const uint32_t sa = smem_u32(sA), sb = smem_u32(sB);
         // prefetched inputs of step t: saved gates, c_t (cur), c_{t-1} (prv), dy_t
         const size_t sstep = (size_t)NC * NGT;
         size_t si = ((size_t)(T - 1) * NC + cta) * NGT + tid;
@@ -565,21 +447,36 @@ __global__ void __launch_bounds__(NTHR, CS == 8 ? 2 : 1) lstm_c4_bwd_kernel(cons
                     dyv = *reinterpret_cast<const float2*>(p.dy + oy);
                 }
             }
-            // ---- dh_rec of step t-1: partial tiles of the cluster
-            const uint32_t ph = (uint32_t)((T - 1 - t) & 1);
-            mbar_wait(accb, ph);
-            tc_fence_after();
-            uint32_t r[32];
-            tc_ld32(tmem_base + ((uint32_t)(warp * 32) << 16), r);
-            if (pusher) {
+            // ---- dh_rec of step t-1: the cluster's units against my K slice of dG_t, as each quarter of it lands
+            const int e = T - 1 - t;
+            const uint32_t ph = (uint32_t)(e & 1);
+            float acc[16];
 #pragma unroll
-                for (int i = 0; i < 8; ++i)
-                    st_cluster_f4(push + i * 16, __uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1]),
-                                  __uint_as_float(r[4 * i + 2]), __uint_as_float(r[4 * i + 3]));
+            for (int i = 0; i < 16; ++i) acc[i] = 0.f;
+            for (int q = 0; q < 4; ++q) {
+                mbar_wait(full0 + 8 * q, ph);
+                wgmma_fence();
+                for (int a = q * NQ; a < (q + 1) * NQ; ++a) {
+#pragma unroll
+                    for (int k = 0; k < 4; ++k)
+                        wgmma_m64n32k16<0, 0>(acc, make_desc(sa + a * APITCH + k * 32, 16, 1024),
+                                              make_desc(sb + a * 4096 + k * 32, 16, 1024), 1);
+                }
+                wgmma_commit();
             }
-            tc_fence_before();
+            wgmma_wait<0>();
+            wgmma_fence_regs(acc);
+            // partial dh tiles -> the owning CTAs' shared memory (DSMEM), one release arrival per destination
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                if (push0) st_cluster_f2(dst0 + i * 32, acc[4 * i], acc[4 * i + 1]);
+                if (push1) st_cluster_f2(dst1 + i * 32, acc[4 * i + 2], acc[4 * i + 3]);
+            }
             __syncwarp();
-            if (pusher && (lane & 7) == 0) mbar_arrive_cluster(rbar_dst);
+            if (lane == 0) {
+                if (push0) mbar_arrive_cluster(rbar0);
+                if (push1) mbar_arrive_cluster(rbar1);
+            }
             mbar_wait_cluster(rbar, ph);
             float s0 = 0.f, s1 = 0.f;
 #pragma unroll
@@ -595,62 +492,30 @@ __global__ void __launch_bounds__(NTHR, CS == 8 ? 2 : 1) lstm_c4_bwd_kernel(cons
             *reinterpret_cast<float2*>(p.dc0 + (size_t)b * H + j) = make_float2(dc0v, dc1v);
         }
     } else if (lane == 0) {
-        const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(NB >> 3) << 17) | ((uint32_t)(64 >> 4) << 24);
-        const uint32_t sa = smem_u32(sA), sb = smem_u32(sB);
+        const uint32_t sb = smem_u32(sB);
         const int k0 = (int)rank * KSL;
         for (int t = T - 1; t >= 0; --t) {
             const int e = T - 1 - t;
             spin_wait_ge(p.bar, (unsigned)(e + 1) * ncta);   // every CTA has published dG_t
             fence_proxy_async();
-            tc_fence_after();
             const int row0 = (t & 1) * NB;
             for (int q = 0; q < 4; ++q) {
                 mbar_expect_tx(full0 + 8 * q, 4096u * NQ);
                 for (int a = q * NQ; a < (q + 1) * NQ; ++a)
                     tma_load_2d(sb + a * 4096, &gmap, k0 + a * 64, row0, full0 + 8 * q);
             }
-            for (int q = 0; q < 4; ++q) {
-                mbar_wait(full0 + 8 * q, (uint32_t)(e & 1));
-                tc_fence_after();
-                for (int a = q * NQ; a < (q + 1) * NQ; ++a) {
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        tc_mma_bf16(tmem_base, make_desc(sa + a * APITCH + k * 32, 0, 1024),
-                                    make_desc(sb + a * 4096 + k * 32, 0, 1024), idesc, (a | k) ? 1u : 0u);
-                }
-            }
-            tc_commit(accb);
         }
     }
-    tc_fence_before();
     __syncthreads();
     cluster_sync_all();
-    if (warp == 4) { tc_fence_after(); tmem_free32(tmem_base); }
 }
 
 // ---------------------------------------------------------------------------------------------------------
 inline bool c4_shape_ok(int B, int H) { return B >= 1 && H % 256 == 0 && H <= 1024; }
 
-inline int fwd_nacc() {             // independent accumulators of the forward MMAs: 1, 2 or 4 (EDGEDICT_C4_NACC)
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("EDGEDICT_C4_NACC"); v = e ? atoi(e) : 4; if (v != 1 && v != 2 && v != 4) v = 4; }
-    return v;
-}
-inline bool fwd_tmem_a() {          // W_hh slice in tensor memory (default) or in shared memory (EDGEDICT_C4_TMEMA=0)
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("EDGEDICT_C4_TMEMA"); v = (e && atoi(e) == 0) ? 0 : 1; }
-    return v == 1;
-}
 inline size_t fwd_smem(int H) {
-    const int NA = fwd_tmem_a() ? 0 : H / 256;
-    size_t b = 1024 + (size_t)NA * 16384 + 16384 + 7 * 4096 + 128;
-    // Tensor-memory budget: with the weights in TMEM a forward CTA holds up to 256 of the SM's 512 columns (128 A + 4 x 32
-    // accumulators).  Two of them fill the SM's tensor memory, and a co-resident GEMM CTA placed next to them would sit in
-    // tcgen05.alloc until a recurrence ends -- so the request is padded to 58 KB: two forward CTAs + the 115 KB
-    // co-resident GEMM configuration then exceed the SM's shared memory, and GEMM CTAs only land next to ONE forward CTA
-    // (256 + 128 columns).
-    if (fwd_tmem_a() && b < 58 * 1024) b = 58 * 1024;
-    return b;
+    const int NA = H / 256;
+    return 1024 + (size_t)NA * 16384 + 16384 + 7 * 4096 + 128;
 }
 template <int CS> size_t bwd_smem(int H) {
     const int NA = 4 * H / CS / 64;
@@ -717,34 +582,7 @@ int bwd_cs(int H) {
     return c;
 }
 
-inline int fwd_minb() {             // register budget of the default variant (TA, 4 accumulators): EDGEDICT_C4_MINB = 2 | 3 | 4
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("EDGEDICT_C4_MINB"); v = e ? atoi(e) : 3; if (v < 2 || v > 4) v = 3; }
-    return v;
-}
-
-// the forward kernel variant selected by the environment (TA x NACC)
-#define C4_FWD_DISPATCH(EXPR)                                                                        \
-    do {                                                                                             \
-        const int n_ = fwd_nacc();                                                                   \
-        if (fwd_tmem_a()) {                                                                          \
-            if (n_ == 1) { auto kern = lstm_c4_fwd_kernel<true, 1>; EXPR; }                          \
-            else if (n_ == 2) { auto kern = lstm_c4_fwd_kernel<true, 2>; EXPR; }                     \
-            else if (fwd_minb() == 2) { auto kern = lstm_c4_fwd_kernel<true, 4, 2>; EXPR; }          \
-            else if (fwd_minb() == 4) { auto kern = lstm_c4_fwd_kernel<true, 4, 4>; EXPR; }          \
-            else { auto kern = lstm_c4_fwd_kernel<true, 4>; EXPR; }                                  \
-        } else {                                                                                     \
-            if (n_ == 1) { auto kern = lstm_c4_fwd_kernel<false, 1>; EXPR; }                         \
-            else if (n_ == 2) { auto kern = lstm_c4_fwd_kernel<false, 2>; EXPR; }                    \
-            else { auto kern = lstm_c4_fwd_kernel<false, 4>; EXPR; }                                 \
-        }                                                                                            \
-    } while (0)
-
-int fwd_max_clusters(int H) {
-    int n = -1;
-    C4_FWD_DISPATCH(n = max_clusters_of(kern, H / 8, 4, fwd_smem(H), NGT));
-    return n;
-}
+int fwd_max_clusters(int H) { return max_clusters_of(lstm_c4_fwd_kernel, H / 8, 4, fwd_smem(H), NGT); }
 
 bool fwd_ok(int H) {
     static int cache[5] = {-1, -1, -1, -1, -1};
@@ -755,7 +593,7 @@ bool fwd_ok(int H) {
 
 }  // namespace
 
-// 1 when the cluster/tcgen05 recurrent kernels can run this layer (shape + co-residency of all clusters)
+// 1 when the cluster/wgmma recurrent kernels can run this layer (shape + co-residency of all clusters)
 EB_API int eb_lstm_c4_supported(int B, int H) {
     static int off = -1;
     if (off < 0) { const char* e = getenv("EDGEDICT_LSTM_C4"); off = (e && atoi(e) == 0) ? 1 : 0; }
@@ -801,11 +639,7 @@ EB_API int eb_lstm_c4_fwd(const float* xg, const void* whh16, const float* h0, c
         return EB_ERR_INVALID;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const size_t smem = fwd_smem(H);
-    {
-        cudaError_t e_ = cudaSuccess;
-        C4_FWD_DISPATCH(e_ = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        EB_CUDA(e_);
-    }
+    EB_CUDA(cudaFuncSetAttribute(lstm_c4_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     char* base = reinterpret_cast<char*>(scratch);
     const size_t tile_save = (size_t)T * (H / UPC) * NGT;
     for (int b0 = 0, tile = 0; b0 < B; b0 += NB, ++tile) {
@@ -828,9 +662,7 @@ EB_API int eb_lstm_c4_fwd(const float* xg, const void* whh16, const float* h0, c
         { static int wp = -1; if (wp < 0) { const char* e = getenv("EDGEDICT_LSTM_WPOLL"); wp = e ? atoi(e) : 3; } p.wpoll = wp & 1; }
         p.cseq_std = cseq_std ? cseq_std + (size_t)b0 * T * H : nullptr;
         EB_CUDA(cudaMemsetAsync(scratch, 0, C4_HDR, st));
-        bool ok = false;
-        C4_FWD_DISPATCH(ok = launch_clustered(kern, H / UPC, NGT, 4, smem, st, p));
-        if (!ok) return EB_ERR_CUDA;
+        if (!launch_clustered(lstm_c4_fwd_kernel, H / UPC, NGT, 4, smem, st, p)) return EB_ERR_CUDA;
     }
     return EB_OK;
 }
@@ -868,7 +700,6 @@ EB_API int eb_lstm_c4_bwd(const float* dy, const void* gsave, const void* csave,
         p.gx = reinterpret_cast<__nv_bfloat16*>(base + C4_HDR);
         p.bar = reinterpret_cast<unsigned*>(base);
         p.B = (B - b0 < NB) ? (B - b0) : NB; p.T = T; p.H = H;
-        p.trace = g_trace; p.trace_steps = g_trace_steps;
         EB_CUDA(cudaMemsetAsync(scratch, 0, C4_HDR, st));
         bool ok;
         if (cs == 8) {

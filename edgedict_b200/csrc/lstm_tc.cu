@@ -25,7 +25,7 @@
 #include <cooperative_groups.h>
 #include <stdlib.h>
 #include "common.cuh"
-#include "sm100.cuh"
+#include "sm90.cuh"
 #include "../../include/edgedict_b200.h"
 
 namespace cg = cooperative_groups;
@@ -106,10 +106,8 @@ __device__ __forceinline__ void warp_pull(__nv_bfloat16* dst, int dst_ld, const 
 }
 
 // Grid barrier = monotonic counter: every CTA adds 1 after publishing (one thread: fence + atomic),
-// ONE thread per CTA polls with ld.acquire.gpu, then a block barrier.  Alternatives that were
-// measured and rejected (profiles/r1/lstm_fwd_sync_experiments.txt): a poller per warp (+1.1 us per
-// step of contention on the counter line), one flag per producer with st.release and vector polls
-// (+2..6 us), fence.acq_rel / red.release instead of __threadfence (no change).
+// ONE thread per CTA polls with ld.acquire.gpu, then a block barrier.  (A poller per warp contends on the
+// counter line; one flag per producer with st.release and vector polls costs more polls per step.)
 // B fragments for one k-step and all four batch n-tiles out of a padded [NB][ld] bf16 tile
 template <int NT>
 __device__ __forceinline__ void load_b(uint32_t (&b01)[4], uint32_t (&b23)[4], const __nv_bfloat16* tile, int ld,
@@ -131,9 +129,8 @@ struct FwdP {
     int B, T, H;
 };
 
-// One batch tile of up to NBT = 32 rows per launch.  (Splitting the tile into two independent 16-row halves that
-// are co-resident on every SM was measured: no gain, each half is as latency-bound as the whole --
-// profiles/r1/lstm_pairing_experiments.txt.  Pairing DIFFERENT layers is what pays: functional.LSTMStack.)
+// One batch tile of up to NBT = 32 rows per launch.  (Two independent 16-row halves co-resident on every SM would each be
+// as latency-bound as the whole; pairing DIFFERENT layers is what pays: functional.LSTMStack.)
 constexpr int NBT = NB;
 __global__ void __launch_bounds__(NW * 32, EB_LSTM_MINB) lstm_tc_fwd_kernel(FwdP p) {
     constexpr int NT = NBT / 8;                              // batch n-tiles
@@ -299,7 +296,7 @@ struct BwdP {
     int b0, Btot, nseg;
     int seg_off[9];
     int wpoll;                    // every warp polls the barrier counter itself (default; EDGEDICT_LSTM_WPOLL bit 1): the pull of a warp
-                                  // starts when IT sees the counter, no block barrier behind a single poller: 21.8 -> 20.8 ms per step
+                                  // starts when IT sees the counter, no block barrier behind a single poller
 };
 #define TC_STAMP(step, s)                                                                          \
     do {                                                                                           \
@@ -311,9 +308,8 @@ int g_tc_trace_steps = 0;
 // REMAP selects the phase-A thread -> (unit, batch row) map:
 //   true  (default): unit = lane / 4, row = 4 * warp + lane % 4, the forward kernel's map: the 8 units of a row are one sector, a
 //          warp-wide load of a saved gate touches 4 sectors, and -- what counts on the critical path -- the exchange store of a warp
-//          is 4 rows x 64 contiguous bytes instead of 32 rows x 8 bytes: gate math + store 800 -> 350 cycles, the barrier behind it
-//          opens 800 cycles earlier (fewer write transactions to fence), 9807 -> 8544 cycles per step (profiles/r2);
-//   false (EDGEDICT_LSTM_BWD_REMAP=0, every measurement of round 1): unit = warp, row = lane: 32 sectors per load for 4 useful bytes each.
+//          is 4 rows x 64 contiguous bytes instead of 32 rows x 8 bytes: fewer write transactions to fence before the barrier;
+//   false (EDGEDICT_LSTM_BWD_REMAP=0): unit = warp, row = lane: 32 sectors per load for 4 useful bytes each.
 template <int CS, bool CLUSTER, bool REMAP = false>
 __global__ void __launch_bounds__(NW * 32, 1) lstm_tc_bwd_kernel(BwdP p) {
     constexpr int MT = CS / 2;                               // m16 tiles: 8*CS units

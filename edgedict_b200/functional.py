@@ -2,7 +2,7 @@
 (edgedict_b200/ops.py).  torch.autograd only stitches them together -- it never differentiates
 through a torch op on the hot path.
 
-Reference semantics per Function are cited next to each class (paths under /root/reference).
+Reference semantics per Function are cited next to each class (paths relative to the reference project).
 """
 import torch
 
@@ -11,10 +11,9 @@ from . import ops
 import os
 
 f32, bf16 = torch.float32, torch.bfloat16
-# bf16 mode: the joint's output GEMM also emits the softmax statistics of the loss from its fp32 TMEM accumulators
+# bf16 mode: the joint's output GEMM also emits the softmax statistics of the loss from its fp32 accumulators
 # and writes bf16 logits; the 8 GB denominator pass disappears and the gradient pass runs in place on 4 GB
-# (EDGEDICT_FUSE_LSE=0 selects the unfused fp32-logits path).  Measured at E6D2: joint GEMM + loss 4.8 ms against
-# 7.2 ms unfused, once the epilogue used ex2.approx.ftz, unguarded full chunks and eight epilogue warps.
+# (EDGEDICT_FUSE_LSE=0 selects the unfused fp32-logits path).
 FUSE_JOINT_LSE = os.environ.get("EDGEDICT_FUSE_LSE", "1") != "0"
 
 
@@ -122,7 +121,7 @@ class LSTMLayer(torch.autograd.Function):
         tc = precision == "bf16" and ops.lstm_tc_supported(B, H)
         c4 = precision == "bf16" and ops.lstm_c4_supported(B, H)
         if c4:
-            # cluster / tcgen05 kernels: saves in their CTA-private layout, y16 IS the h_{t-1}-shifted copy
+            # cluster / wgmma kernels: saves in their CTA-private layout, y16 IS the h_{t-1}-shifted copy
             y, y16, hT, cT, gates, cseq = ops.lstm_c4_fwd(xg, ops.cast_bf16(_c(w_hh)), h0c, c0c, need,
                                                           std_saves=None if ops.C4_BWD else True)
         elif tc:
@@ -179,12 +178,12 @@ class LSTMLayer(torch.autograd.Function):
 
 # ---- layer-wavefront schedule of the LSTM stack ------------------------------------------------------------
 # The recurrence of one layer is a chain of T grid-synchronous steps that is bound by exchange/barrier LATENCY
-# (DESIGN.md section 7): one layer's persistent kernel uses ~1 of 4 issue slots of 128 SMs.  Layer l+1 at frame t
+# (DESIGN.md section 4a): one layer's persistent kernel leaves its SMs idle most of the time.  Layer l+1 at frame t
 # only needs layer l up to frame t, so the time axis is cut into chunks and layer l+1 runs chunk c on a second
-# stream while layer l runs chunk c+1: two persistent kernels (compiled for <= 128 registers, ~100 KB of shared
-# memory each) are co-resident on every SM and hide each other's latency.  The per-chunk input GEMM uses the
+# stream while layer l runs chunk c+1: two persistent kernels (the lstm_c4 forward CTA: 128 threads, <= 168 registers,
+# 109 KB of shared memory at H = 1024) fit on every SM and hide each other's latency.  The per-chunk input GEMM uses the
 # co-resident tile configuration (EB_GEMM_CORESIDENT) so that it fits next to the other layer's recurrent CTA.
-WAVEFRONT_CHUNKS = int(os.environ.get("EDGEDICT_WAVEFRONT_CHUNKS", "6"))     # 0 disables; 4/6/8 measured: 54.43/54.09/54.40 ms
+WAVEFRONT_CHUNKS = int(os.environ.get("EDGEDICT_WAVEFRONT_CHUNKS", "6"))     # 0 disables
 _wave_streams = {}
 
 
@@ -499,7 +498,7 @@ def _joint_bwd(ctx_p, dlog2, hid, he2, hd2, w1, w2, dims, db2=None):
         if db2 is None:
             db2 = ops.colsum(dlog2)
         if p == "bf16" and V % 256 == 0:
-            # compute dW2^T = hidden^T dlogits ([J, V]: 256-wide tcgen05 tiles divide V, not J) and flip it
+            # compute dW2^T = hidden^T dlogits ([J, V]: 256-wide GEMM tiles divide V, not J) and flip it
             dw2 = ops.mm_tn(hid2, dl16, p, dy16=hid2, x16=dl16).t().contiguous()
         else:
             dw2 = ops.mm_tn(dlog2, hid2, p, dy16=dl16, x16=hid2 if p == "bf16" else None)
@@ -608,7 +607,7 @@ class JointLoss(torch.autograd.Function):
         fused = precision == "bf16" and FUSE_JOINT_LSE and J % 8 == 0 and U <= 1024
         if fused:
             # bf16 mode: the logits GEMM epilogue also produces the softmax statistics (fp32, from the
-            # TMEM accumulators) and writes bf16 logits; the denominator pass over 8 GB disappears
+            # register accumulators) and writes bf16 logits; the denominator pass over 8 GB disappears
             b2a = b2 if (b2.is_contiguous() and b2.data_ptr() % 16 == 0) else b2.clone()
             logits, ws = ops.joint_logits_lse(hid2, ops.cast_bf16(w2.contiguous()), b2a, labels, act_lens,
                                               label_lens, B, T, U, blank)

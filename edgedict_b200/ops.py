@@ -124,19 +124,17 @@ def gemm_f32(A, sam, sak, B, sbk, sbn, M, N, K, bias=None, out=None, beta=0.0, a
 GEMM_CORESIDENT = 1      # include/edgedict_b200.h EB_GEMM_CORESIDENT
 
 
-def gemm_pair_mode(mode):
-    """-1 automatic / 0 never / 1 whenever legal: cta_group::2 tiles in the bf16-output GEMMs (eb_gemm_pair_mode);
-    returns the previous mode."""
-    return int(lib().eb_gemm_pair_mode(int(mode)))
-
-
 def gemm_bf16(A, a_mn, B, b_mn, M, N, K, bias=None, out=None, out_bf16=False, accumulate=False, tag=None, flags=0):
     if out is None:
         out = torch.empty(M, N, dtype=bf16 if out_bf16 else f32, device=A.device)
     name = tag or ("gemm_bf16_%s%s" % ("t" if a_mn else "n", "n" if b_mn else "t"))
     with _timed(name, 1, 2.0 * (M * K + N * K) + out.element_size() * M * N, 2.0 * M * N * K):
-        check(lib().eb_gemm_bf16_ex(_p(A), int(a_mn), _p(B), int(b_mn), _p(out), int(out.dtype == bf16), _p(bias),
-                                    int(accumulate), M, N, K, int(flags), _s()), "eb_gemm_bf16")
+        c16 = int(out.dtype == bf16)
+        # split-K workspace (partial tiles summed in a fixed order: the same bits on every run)
+        nws = int(lib().eb_gemm_bf16_partials(int(a_mn), c16, int(accumulate), M, N, K, int(flags)))
+        ws = torch.empty(nws, dtype=f32, device=A.device) if nws else None
+        check(lib().eb_gemm_bf16_ex(_p(A), int(a_mn), _p(B), int(b_mn), _p(out), c16, _p(bias), int(accumulate), M, N, K,
+                                    int(flags), _p(ws), nws, _s()), "eb_gemm_bf16")
     return out
 
 
@@ -356,7 +354,7 @@ def lstm_tc_bwd_chunks(dy, gates, cseq, whhT16, lens, B, out):
     return out, dh0, dc0
 
 
-# ---- cluster / tcgen05 recurrent kernels (csrc/lstm_c4.cu) ------------------------------------------
+# ---- cluster / wgmma recurrent kernels (csrc/lstm_c4.cu) ------------------------------------------
 _c4_ok = {}
 
 

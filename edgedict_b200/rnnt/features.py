@@ -1,4 +1,4 @@
-"""B200-native mirror of the reference's log-mel front end (``rnnt/features.py`` + the feature part of
+"""H100-native mirror of the reference's log-mel front end (``rnnt/features.py`` + the feature part of
 ``rnnt/transforms.py``): same class names, constructor arguments and output layouts, arithmetic in
 csrc/frontend.cu (pre-emphasis / reflect padding, direct-DFT GEMM, power, mel GEMM, log + frame stacking).
 

@@ -1,7 +1,7 @@
-"""B200-native mirror of the reference's ``rnnt/models.py`` hot path.
+"""H100-native mirror of the reference's ``rnnt/models.py`` hot path.
 
 Same class names, constructor arguments, ``forward`` signatures, return values and
-``state_dict`` keys as /root/reference/rnnt/models.py:16-269, so ``cli/train.py``,
+``state_dict`` keys as the reference's rnnt/models.py:16-269, so ``cli/train.py``,
 ``cli/baseline.py``, ``cli/lightning.py`` and ``rnnt/stream.py`` can import this module
 unchanged.  The torch ``nn.LSTM`` / ``nn.LayerNorm`` / ``nn.Linear`` / ``nn.Embedding`` objects
 below are PARAMETER CONTAINERS ONLY (identical default initialisation and checkpoint keys); their
@@ -9,7 +9,7 @@ below are PARAMETER CONTAINERS ONLY (identical default initialisation and checkp
 (edgedict_b200/functional.py).  CUDA tensors are mandatory: there is no CPU fallback.
 
 precision: "fp32" (default; parity mode, CUDA-core GEMMs, matches torch-CPU fp32 to ~1e-5) or
-"bf16" (tcgen05 tensor-core GEMMs with fp32 accumulation; also selected automatically inside
+"bf16" (wgmma tensor-core GEMMs with fp32 accumulation; also selected automatically inside
 ``torch.autocast('cuda')``, the modern spelling of the reference's apex-O1 switch).
 """
 import os
@@ -277,7 +277,7 @@ class Transducer(nn.Module):
         ys = ys[:, :int(ylen.max())].contiguous()
         if xs.is_cuda and _PREDICTOR_STREAM:
             # The prediction network (2 x 129 recurrent steps) is independent of the encoder until the joint: it runs on
-            # a side stream under the encoder's recurrence (its kernels use 32 of the 148 SMs at H_d = 256); autograd
+            # a side stream under the encoder's recurrence (its kernels use 32 of the 132 SMs at H_d = 256); autograd
             # replays each node's backward on the stream of its forward, so the backward passes overlap the same way.
             main = torch.cuda.current_stream(xs.device)
             side = _predictor_stream(xs.device)

@@ -1,4 +1,4 @@
-"""B200-native mirror of the reference's streaming decoder interface (rnnt/stream.py:15-120).
+"""H100-native mirror of the reference's streaming decoder interface (rnnt/stream.py:15-120).
 
 ``PytorchStreamDecoder(FLAGS)`` keeps the reference's attributes and methods -- ``reset()``,
 ``decode(frame) -> str``, ``reset_profile()``, ``encoder_elapsed / decoder_elapsed /

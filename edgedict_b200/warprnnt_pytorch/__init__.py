@@ -56,7 +56,7 @@ def rnnt_loss(acts, labels, act_lens, label_lens, blank=0, reduction='mean'):
     """acts [B,T,U+1,V] raw logits on CUDA (fp32 or fp64); labels [B,U] int32; lengths int32."""
     certify_inputs(acts, labels, act_lens, label_lens)
     if not acts.is_cuda:
-        raise RuntimeError("edgedict_b200.warprnnt_pytorch is CUDA-only (sm_100a); got CPU activations")
+        raise RuntimeError("edgedict_b200.warprnnt_pytorch is CUDA-only (sm_90a); got CPU activations")
     if acts.dtype not in (torch.float32, torch.float64):
         raise TypeError("unsupported data type {} (float32/float64 only, as in binding.cpp:46-80)".format(acts.dtype))
     dev = acts.device

@@ -1,12 +1,12 @@
-/* include/edgedict_b200.h -- C ABI of libedgedict_b200.so (sm_100a).
+/* include/edgedict_b200.h -- C ABI of libedgedict_b200.so (sm_90a).
  *
  * Plain pointers and sizes only; every pointer is a DEVICE pointer unless its name ends in
  * _host; every call is asynchronous on `stream` (a cudaStream_t passed as void*) and returns
  * 0 on success, 2 for invalid arguments, 3 for a CUDA error.  No call allocates memory:
  * callers own all buffers (same ownership rule as warp-transducer, README.md:36-37).
  *
- * Each entry point names the piece of the reference it replaces (paths relative to
- * /root/reference).  The reference has no FFI for the model path (it calls torch.nn modules),
+ * Each entry point names the piece of the reference it replaces (paths relative to the
+ * root of the reference project).  The reference has no FFI for the model path (it calls torch.nn modules),
  * so those entry points mirror the module boundaries of rnnt/models.py.
  */
 #pragma once
@@ -49,25 +49,25 @@ int eb_gemm_f32(const float* A, long sam, long sak, const float* B, long sbk, lo
                 long ldc, const float* bias, int M, int N, int K, float alpha, float beta,
                 void* stream);
 
-/* ---- bf16 tensor-core GEMM (tcgen05 + TMA + TMEM), fp32 accumulate ------------------------
+/* ---- bf16 tensor-core GEMM (wgmma + TMA), fp32 accumulate ----------------------------------
  * same call sites in bf16 mode.  A: [M,K] (a_mn_major=0, K contiguous) or [K,M] (a_mn_major=1);
  * B: [N,K] (b_mn_major=0) or [K,N] (b_mn_major=1); C row-major [M,N] fp32 or bf16;
  * C = A*B (+ bias[n]) (+ C when accumulate).  Pointers 16-byte aligned, contiguous dim % 8 == 0. */
 int eb_gemm_bf16(const void* A, int a_mn_major, const void* B, int b_mn_major, void* C, int c_bf16,
                  const float* bias, int accumulate, long M, int N, long K, void* stream);
 
-/* eb_gemm_bf16 with launch flags.  EB_GEMM_CORESIDENT (A and B K-major only): a 115 KB / 192-thread
- * configuration that shares an SM with one CTA of a persistent recurrent kernel (eb_lstm_tc_fwd), used by the
- * layer-wavefront schedule of the encoder stack (functional.LSTMStack). */
+/* eb_gemm_bf16 with launch flags and a split-K workspace.  EB_GEMM_CORESIDENT (A and B K-major only): a 97 KB,
+ * 112-register configuration that shares an SM with one CTA of a persistent recurrent kernel (eb_lstm_c4_fwd), used by
+ * the layer-wavefront schedule of the encoder stack (functional.LSTMStack).  fp32-output products with few output tiles
+ * split K across CTAs: every split writes its partial tile into `partials` (8-byte aligned, `partial_floats` floats;
+ * eb_gemm_bf16_partials says how many it can use) and the splits are added in a fixed order, so the result is the same
+ * bits on every run.  With a smaller workspace the split count shrinks to what fits (NULL / 0: no split; eb_gemm_bf16
+ * passes none). */
 #define EB_GEMM_CORESIDENT 1
+long eb_gemm_bf16_partials(int a_mn_major, int c_bf16, int accumulate, long M, int N, long K, int flags);
 int eb_gemm_bf16_ex(const void* A, int a_mn_major, const void* B, int b_mn_major, void* C, int c_bf16,
-                    const float* bias, int accumulate, long M, int N, long K, int flags, void* stream);
-
-/* cta_group::2 tiles (two CTAs of a cluster share one 256 x 256 tile, each staging half of the B operand) for the
- * bf16-output GEMMs with K-major A -- the joint's logits (+LSE) and d-hidden products -- and, on request only, for
- * split-K weight gradients with both operands MN-major.  mode -1 = automatic (bf16-output products with enough 256-row
- * blocks for every CTA pair), 0 = never, 1 = whenever legal; returns the previous mode.  Default: EDGEDICT_GEMM_PAIR. */
-int eb_gemm_pair_mode(int mode);
+                    const float* bias, int accumulate, long M, int N, long K, int flags, float* partials,
+                    long partial_floats, void* stream);
 
 /* C16[M,N] = bf16((A B) * (1 - hid16[M,N]^2)): the joint's d-hidden GEMM with the derivative of Joint.forward's Tanh
  * (rnnt/models.py:164) applied in the epilogue, so that d(pre-activation) leaves the GEMM directly. */
@@ -116,7 +116,7 @@ int eb_lstm_tc_bwd_chunks(const float* dy, const float* gates, const float* cseq
                           const void* whhT16, const float* dhT, const float* dcT, void* dg16, float* dh0, float* dc0,
                           void* scratch, int B, const int* chunk_lens, int nchunks, int H, void* stream);
 
-/* ---- LSTM layer on tcgen05 tensor cores inside thread-block clusters (bf16 mode; H % 256 == 0, H <= 1024) ----
+/* ---- LSTM layer on wgmma tensor cores inside thread-block clusters (bf16 mode; H % 256 == 0, H <= 1024) ------
  * csrc/lstm_c4.cu: W_hh slices resident in shared memory, h / dG exchanged through L2 with TMA pulls, partial gate
  * sums reduced across a cluster through distributed shared memory.  Same cell semantics as eb_lstm_tc_* with a
  * CTA-private layout of the forward saves:

@@ -5,7 +5,7 @@
  * load libedgedict_b200.so unchanged.
  *
  * Differences in behaviour (documented in INTEGRATION.md):
- *   - only RNNT_GPU is implemented (sm_100a); RNNT_CPU returns RNNT_STATUS_EXECUTION_FAILED;
+ *   - only RNNT_GPU is implemented (sm_90a); RNNT_CPU returns RNNT_STATUS_EXECUTION_FAILED;
  *   - get_workspace_size() reports this library's own requirement (5*T*U+2 scalars per
  *     utterance); callers already size the workspace through it;
  *   - as in the reference's GPU path, activations are raw logits, labels / lengths / workspace

@@ -4,7 +4,7 @@ baseline may import this; the product path is edgedict_b200/csrc/frontend.cu).
 Follows rnnt/features.py:33-152 (FilterbankFeatures: dither -> pre-emphasis -> torch.stft -> power -> mel
 matmul -> log(x + 1e-20) -> mask) and rnnt/transforms.py:30-51 (Downsample = frame stacking).
 
-Third-party arithmetic not under /root/reference (SURVEY 8c):
+Third-party arithmetic outside the reference project (SURVEY 8c):
   * torch.stft as the reference calls it (torch==1.4: center=True, pad_mode='reflect', onesided, window of
     win_length zero-padded symmetrically to n_fft).  PINNED in tests/test_oracle_features.py against this
     container's torch.stft (same arguments, return_complex=True).

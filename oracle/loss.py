@@ -17,7 +17,7 @@ _REF_SO = os.path.join(_HERE, "_ref", "libwarprnnt_ref.so")
 
 
 def build(quiet=True):
-    """Compile liboracle.so (and _ref/ when /root/reference is present)."""
+    """Compile liboracle.so and, where the reference's warp-transducer sources are (oracle/Makefile), _ref/."""
     out = subprocess.run(["make", "-C", _HERE], capture_output=True, text=True)
     if out.returncode != 0:
         raise RuntimeError("oracle build failed:\n" + out.stdout + out.stderr)

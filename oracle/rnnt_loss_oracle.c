@@ -9,7 +9,7 @@
  * Parity pin: checked against the reference's known-answer vectors
  * (warp-transducer/tests/test_cpu.cpp:12-179, pytorch_binding/test/test.py:51-161)
  * in tests/test_oracle_loss.py, and against oracle/_ref/libwarprnnt_ref.so
- * (the reference's own CPU library compiled from /root/reference) on random
+ * (the reference's own CPU library, tests/golden/ref_loss.npz) on random
  * problems.
  *
  * What follows what:

@@ -1,13 +1,12 @@
-"""Generates tests/golden/*.npz by running the REFERENCE itself (only possible in the build
-container, where /root/reference exists):
+"""Generates tests/golden/*.npz by running the REFERENCE itself (only possible where its sources are):
 
-    python tests/golden/make_golden.py
+    EDGEDICT_REFERENCE=<reference checkout> python tests/golden/make_golden.py [tiny|e4d1|ref_loss ...]
 
-* model: ``rnnt.models.Transducer`` imported from /root/reference (torch CPU fp32);
-* loss : the reference's CPU library compiled by oracle/Makefile (oracle/_ref), driven exactly
-  like warprnnt_pytorch._RNNT does on CPU tensors (log_softmax first, 'mean' = /B).
+* model: ``rnnt.models.Transducer`` imported from $EDGEDICT_REFERENCE (torch CPU fp32);
+* loss : the reference's CPU library compiled by oracle/Makefile (oracle/_ref, make WARP_TRANSDUCER_DIR=...),
+  driven exactly like warprnnt_pytorch._RNNT does on CPU tensors (log_softmax first, 'mean' = /B).
 
-The committed fixtures are what the GPU box sees; nothing at test time reads /root/reference.
+The committed fixtures are what the tests see; nothing at test time reads the reference.
 """
 import os
 import sys
@@ -18,12 +17,16 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference")
 
-from rnnt.models import Transducer  # noqa: E402  (the reference)
 from oracle import loss as ol  # noqa: E402
 
-assert ol.have_ref(), "build oracle/_ref first (make -C oracle)"
+assert ol.have_ref(), "build oracle/_ref first (make -C oracle WARP_TRANSDUCER_DIR=<warp-transducer tree>)"
+
+
+def Transducer(**kw):
+    sys.path.insert(0, os.environ["EDGEDICT_REFERENCE"])
+    from rnnt.models import Transducer as T  # (the reference)
+    return T(**kw)
 
 
 class RefLoss(torch.autograd.Function):
@@ -174,8 +177,39 @@ def e4d1():
     np.savez_compressed(os.path.join(HERE, "e4d1.npz"), **save)
 
 
+# problems of tests/test_oracle_loss.py: (B, T, U, V, ragged), inputs drawn there from RandomState(B * 1000 + T)
+REF_LOSS_CASES = [(1, 2, 3, 5, False), (3, 17, 6, 11, True), (2, 50, 16, 20, True), (4, 10, 6, 5, True)]
+
+
+def ref_loss_inputs(B, T, U, V, ragged):
+    rng = np.random.RandomState(B * 1000 + T)
+    acts = rng.uniform(0, 1, size=(B, T, U, V)).astype(np.float32)
+    labels = rng.randint(1, V, size=(B, U - 1)).astype(np.int32)
+    tl = np.full(B, T, np.int32)
+    ul = np.full(B, U - 1, np.int32)
+    if ragged:
+        tl[1:] = rng.randint(1, T + 1, size=B - 1)
+        ul[1:] = rng.randint(0, U, size=B - 1)
+    return acts, labels, tl, ul
+
+
+def ref_loss():
+    """Costs and log-prob gradients of the reference's CPU loss library on the problems of test_oracle_loss.py."""
+    from tests.golden import loss_kat as K
+    save = {}
+    for case in REF_LOSS_CASES:
+        acts, labels, tl, ul = ref_loss_inputs(*case)
+        lp, _ = ol.log_softmax(acts)
+        c, g = ol.ref_cpu(lp, labels, tl, ul)
+        tag = "%d_%d_%d_%d" % case[:4]
+        save[tag + ".costs"], save[tag + ".grads"] = c, g
+    lp, _ = ol.log_softmax(K.SMALL_ACTS)
+    save["small_kat.costs"], _ = ol.ref_cpu(lp, K.SMALL_LABELS, [2], [2])
+    np.savez_compressed(os.path.join(HERE, "ref_loss.npz"), **save)
+
+
 if __name__ == "__main__":
-    tiny()
-    e4d1()
-    for f in ("tiny.npz", "e4d1.npz"):
+    for name in sys.argv[1:] or ("tiny", "e4d1", "ref_loss"):
+        globals()[name]()
+    for f in ("tiny.npz", "e4d1.npz", "ref_loss.npz"):
         print(f, os.path.getsize(os.path.join(HERE, f)) // 1024, "KiB")

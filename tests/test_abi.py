@@ -112,7 +112,7 @@ def test_entry_points_reject_bad_arguments_before_touching_the_device(built):
     assert L.eb_gemm_bf16(None, 0, p, 0, p, 0, None, 0, 8, 8, 8, None) == 2
     assert L.eb_gemm_bf16(p, 0, p, 0, p, 0, None, 0, 8, 8, 12, None) == 2            # K-major rows must be 16-byte multiples
     assert L.eb_gemm_bf16(p + 2, 0, p, 0, p, 0, None, 0, 8, 8, 8, None) == 2         # misaligned operand
-    assert L.eb_gemm_bf16_ex(p, 1, p, 0, p, 0, None, 0, 8, 8, 8, 1, None) == 2       # co-resident config: K-major only
+    assert L.eb_gemm_bf16_ex(p, 1, p, 0, p, 0, None, 0, 8, 8, 8, 1, None, 0, None) == 2   # co-resident config: K-major only
     assert L.eb_gemm_bf16_dtanh(p, 0, p, 1, p, None, 8, 8, 8, None) == 2             # needs the hidden activations
     assert L.eb_gemm_bf16_dtanh(p, 0, p, 1, p, p, 8, 6, 8, None) == 2                # N % 4
     assert L.eb_joint_dpre_reduce(None, p, p, 1, 1, 1, 8, None) == 2
@@ -135,6 +135,3 @@ def test_entry_points_reject_bad_arguments_before_touching_the_device(built):
     lens0 = (ctypes.c_int * 2)(3, 0)
     assert L.eb_lstm_tc_bwd_chunks(p, p, p, None, p, None, None, p, p, p, p, 4, lens0, 2, 64, None) == 2  # empty chunk
     assert L.eb_lstm_tc_bwd_chunks(p, p, p, None, p, None, None, p, p, p, p, 4, lens, 2, 96, None) == 2   # H % 64
-    prev = L.eb_gemm_pair_mode(1)                                                    # policy switch: returns the previous mode
-    assert prev in (-1, 0, 1) and L.eb_gemm_pair_mode(0) == 1 and L.eb_gemm_pair_mode(prev) == 0
-    assert L.eb_gemm_pair_mode(prev) == prev

@@ -1,4 +1,4 @@
-"""End-to-end parity of the B200 engine (edgedict_b200.rnnt.models) against the golden fixtures
+"""End-to-end parity of the H100 engine (edgedict_b200.rnnt.models) against the golden fixtures
 produced by the reference itself (tests/golden/*.npz) and against the oracle restatements."""
 import numpy as np
 import pytest

@@ -64,7 +64,7 @@ def test_gemm_bf16_tcgen05_all_layouts(M, N, K):
 
 def test_gemm_bf16_persistent_many_tiles():
     from edgedict_b200 import ops
-    M, N, K = 128 * 40 + 17, 1024, 640                                   # > 148 tiles, ragged M
+    M, N, K = 128 * 40 + 17, 1024, 640                                   # > 132 tiles (one per SM), ragged M
     x, w = _r(M, K, seed=7).bfloat16(), _r(N, K, seed=8).bfloat16()
     y = ops.gemm_bf16(x.cuda(), 0, w.cuda(), 0, M, N, K)
     ref = x.float() @ w.float().t()
@@ -91,59 +91,46 @@ def test_gemm_bf16_wide_tiles_overhanging_the_last_columns():
     assert rel_err(y3.float().cpu(), ((dy.float() @ w_nn.float()) * (1 - hid.float() ** 2)).cpu()) < 1e-2
 
 
-def test_gemm_bf16_cta_pair_tiles_match_one_cta_tiles():
-    """cta_group::2 tiles (two CTAs of a cluster on one 256 x 256 tile, each staging half of B; eb_gemm_pair_mode) give
-    the bits of the one-CTA tiles -- same MMA order per output element -- for the three bf16-output products of the
-    joint: plain nt + bias (and accumulate), d-hidden with tanh' (B MN-major), logits + softmax statistics; odd row-block
-    counts (the peer CTA of the last pair has no rows), N = 256 k + 128 (128-wide MMAs on the last column tile)."""
+@pytest.mark.parametrize("M,N,K", [(1024, 640, 64 * 700 + 24), (320, 384, 64 * 97), (128, 128, 64 * 361)])
+def test_gemm_bf16_split_k_weight_gradients(M, N, K):
+    """fp32-output products with few output tiles and a long contraction split K across CTAs: each split's partial tile
+    goes to the workspace sized by eb_gemm_bf16_partials and splitk_reduce_kernel adds the splits in order.  Both operands
+    MN-major (the weight-gradient layout), with / without bias and accumulate, against fp64; a shrunk workspace (fewer
+    splits, and for the last shape 20 splits of 19 k-blocks over 361, so that the last split is empty) and no workspace
+    (no split) give the same product; repeated launches give the same bits."""
     from edgedict_b200 import ops
-    g = torch.Generator(device="cuda").manual_seed(11)
-    rn = lambda *s: torch.randn(*s, device="cuda", generator=g)
+    from edgedict_b200._lib import lib, check
+    g = torch.Generator(device="cuda").manual_seed(M + K)
+    a = (torch.randn(K, M, device="cuda", generator=g) * 0.1).bfloat16()       # A^T stored [K, M]
+    b = torch.randn(K, N, device="cuda", generator=g).bfloat16()               # B stored [K, N]
+    bias = torch.randn(N, device="cuda", generator=g)
+    want = a.double().t() @ b.double()
+    planned = int(lib().eb_gemm_bf16_partials(1, 0, 0, M, N, K, 0))
+    assert planned >= 2 * M * N, "this shape must take the split-K path"
+    y = ops.gemm_bf16(a, 1, b, 1, M, N, K)
+    assert rel_err(y.cpu(), want.cpu()) < 2e-5
+    assert torch.equal(ops.gemm_bf16(a, 1, b, 1, M, N, K), y)
+    yb = ops.gemm_bf16(a, 1, b, 1, M, N, K, bias=bias)
+    assert rel_err(yb.cpu(), (want + bias.double()).cpu()) < 2e-5
+    base = torch.randn(M, N, device="cuda", generator=g)
+    acc = base.clone()
+    ops.gemm_bf16(a, 1, b, 1, M, N, K, out=acc, accumulate=True)
+    assert rel_err(acc.cpu(), (want + base.double()).cpu()) < 2e-5
 
-    def both(fn):
-        prev = ops.gemm_pair_mode(0)
-        try:
-            one = fn()
-            ops.gemm_pair_mode(1)
-            two = fn()
-        finally:
-            ops.gemm_pair_mode(prev)
-        return one, two
-
-    for (M, N, K) in [(256 * 5, 512, 320), (128 * 7 + 40, 640, 192), (128 * 301, 1024, 640)]:
-        A, W, bias = (rn(M, K) * 0.5).bfloat16(), (rn(N, K) * 0.1).bfloat16(), rn(N)
-        one, two = both(lambda: ops.gemm_bf16(A, 0, W, 0, M, N, K, bias=bias, out_bf16=True))
-        assert torch.equal(one, two)
-        assert rel_err(two.float().cpu(), (A.float() @ W.float().t() + bias).cpu()) < 1e-2
-        base = rn(M, N).bfloat16()
-        one, two = both(lambda: ops.gemm_bf16(A, 0, W, 0, M, N, K, out=base.clone(), accumulate=True))
-        assert torch.equal(one, two)
-        Wn, hid = (rn(K, N) * 0.1).bfloat16(), torch.tanh(rn(M, N)).bfloat16()
-        one, two = both(lambda: ops.gemm_bf16_dtanh(A, Wn, True, hid, M, N, K))
-        assert torch.equal(one, two)
-        assert rel_err(two.float().cpu(), ((A.float() @ Wn.float()) * (1 - hid.float() ** 2)).cpu()) < 1e-2
-    # split-K weight gradient, both operands MN-major (fp32 atomics: compared with the fp32 product, not bit for bit)
-    for (M, N, K) in [(1024, 640, 64 * 700 + 24), (320, 384, 64 * 97)]:
-        dy, x = (rn(K, M) * 0.1).bfloat16(), rn(K, N).bfloat16()
-        one, two = both(lambda: ops.gemm_bf16(dy, 1, x, 1, M, N, K))
-        want = dy.float().t() @ x.float()
-        assert rel_err(two.cpu(), want.cpu()) < 2e-5 and rel_err(one.cpu(), want.cpu()) < 2e-5
-    for (B, T, U, V, J) in [(3, 37, 9, 512, 128), (2, 150, 33, 1024, 640)]:
-        hid, w2, b2 = torch.tanh(rn(B, T, U, J)).bfloat16(), (rn(V, J) * 0.2).bfloat16(), rn(V)
-        labels = torch.randint(1, V, (B, U - 1), dtype=torch.int32, device="cuda", generator=g)
-        xlen = torch.randint(T // 2, T + 1, (B,), dtype=torch.int32, device="cuda", generator=g)
-        ylen = torch.randint(1, U, (B,), dtype=torch.int32, device="cuda", generator=g)
-        xlen[0], ylen[0] = T, U - 1
-        (l0, w0), (l1, w1) = both(lambda: ops.joint_logits_lse(hid, w2, b2, labels, xlen, ylen, B, T, U, 0))
-        assert torch.equal(l0, l1)
-        n = B * T * U
-        ok = ((torch.arange(T, device="cuda")[None, :, None] < xlen[:, None, None]) &
-              (torch.arange(U, device="cuda")[None, None, :] <= ylen[:, None, None])).reshape(-1)
-        s0 = w0.view(torch.float32)[:3 * n].view(3, n)[:, ok]
-        s1 = w1.view(torch.float32)[:3 * n].view(3, n)[:, ok]
-        assert torch.equal(s0, s1)
-        den = -torch.logsumexp(hid.float().view(n, J) @ w2.float().t() + b2, dim=1)
-        assert float((s1[0] - den[ok]).abs().max()) < 2e-3
+    def with_ws(floats):
+        out = torch.full((M, N), 7.0, device="cuda")
+        ws = torch.empty(max(floats, 1), device="cuda")
+        check(lib().eb_gemm_bf16_ex(a.data_ptr(), 1, b.data_ptr(), 1, out.data_ptr(), 0, bias.data_ptr(), 0, M, N, K, 0,
+                                    ws.data_ptr() if floats else None, floats, None), "eb_gemm_bf16_ex")
+        torch.cuda.synchronize()
+        return out
+    shrunk = 20 if K == 64 * 361 else 2
+    assert planned >= shrunk * M * N
+    # fewer splits = longer fp32 accumulation chains per element (no workspace: one chain over all of K, up to 45 k
+    # terms): the rounding grows with the chain, so chains beyond 16 k terms get a wider bar
+    for splits, floats in ((shrunk, shrunk * M * N), (1, 0)):
+        bar = 2e-5 if K // splits <= 16384 else 1e-4
+        assert rel_err(with_ws(floats).cpu(), (want + bias.double()).cpu()) < bar, splits
 
 
 @pytest.mark.parametrize("rows,H,res", [(7, 12, False), (33, 240, False), (64, 320, True), (19, 1024, True), (5, 1500, True),
@@ -351,7 +338,7 @@ def test_gemm_dtanh_epilogue_and_dpre_reductions(M, N, K):
 
 @pytest.mark.parametrize("B,T,H", [(32, 9, 256), (5, 7, 512), (40, 4, 768), (32, 6, 1024)])
 def test_lstm_c4_cluster_kernels_vs_oracle(B, T, H):
-    """csrc/lstm_c4.cu directly (cluster / tcgen05 forward with both save layouts, tcgen05 BPTT) against an explicit fp64
+    """csrc/lstm_c4.cu directly (cluster / wgmma forward with both save layouts, wgmma BPTT) against an explicit fp64
     cell loop on the same bf16-rounded recurrent weights; remaining difference: h_{t-1} / dG_t exchanged in bf16 and
     the saved gates kept in bf16 (documented tolerances as for lstm_tc: 2e-2 forward, 5e-2 gradients)."""
     from edgedict_b200 import ops
@@ -381,7 +368,7 @@ def test_lstm_c4_cluster_kernels_vs_oracle(B, T, H):
     assert rel_err(y1.cpu(), y.detach()) < 2e-2 and rel_err(hT.cpu(), h.detach()) < 2e-2 and rel_err(cT.cpu(), c.detach()) < 2e-2
     want_hp = torch.cat([h0[:, None], y.detach().float()[:, :-1]], 1)
     assert rel_err(hp.float().cpu(), want_hp) < 2e-2
-    # standard-layout saves feed the mma.sync BPTT kernel, the CTA-private ones the tcgen05 BPTT kernel
+    # standard-layout saves feed the mma.sync BPTT kernel, the CTA-private ones the wgmma BPTT kernel
     y2, _, _, _, gstd, cstd = ops.lstm_c4_fwd(xg.to(dev), wg, h0.to(dev), c0.to(dev), True, std_saves=True)
     assert torch.equal(y1, y2)
     for name, (dg, dh0, dc0) in (("tc_bwd", ops.lstm_tc_bwd(dy.to(dev), gstd, cstd, c0.to(dev), whT, dhT.to(dev), dcT.to(dev))),

@@ -1,7 +1,7 @@
 """Parity of the BENCHMARKED mode -- set_precision("bf16"): layer wavefront + tensor-core recurrent kernels +
-tcgen05 GEMMs + the joint GEMM with the softmax statistics in its epilogue -- against (i) the fixtures the
+wgmma GEMMs + the joint GEMM with the softmax statistics in its epilogue -- against (i) the fixtures the
 reference itself produced for BASELINE configs[0] (tests/golden/e4d1.npz, made by tests/golden/make_golden.py
-importing /root/reference/rnnt/models.py) and (ii) the fp32 CPU oracle restatement at the hidden sizes of
+importing the reference's rnnt/models.py) and (ii) the fp32 CPU oracle restatement at the hidden sizes of
 BASELINE configs[1] (E6D2: H=1024, L=6, V=1024, J=640), run in-test.
 
 Bars.  north_star asks for "loss and encoder activations within 1e-3 rel fp32".  The fp32 mode of this engine

@@ -1,10 +1,16 @@
 """Pins the loss oracle (oracle/rnnt_loss_oracle.c) against the reference's own known-answer
-vectors and against the reference's CPU library compiled from /root/reference (oracle/_ref)."""
+vectors and against what the reference's CPU library computes (tests/golden/ref_loss.npz, written by
+tests/golden/make_golden.py from that library)."""
+import os
+
 import numpy as np
 import pytest
 
 from oracle import loss as ol
 from tests.golden import loss_kat as K
+from tests.util import GOLDEN
+
+REF_LOSS = os.path.join(GOLDEN, "ref_loss.npz")
 
 
 def test_small_kat_logits():
@@ -67,10 +73,8 @@ def test_numeric_gradient():
     assert np.allclose(g, num, atol=1e-7)
 
 
-@pytest.mark.skipif(not ol.have_ref(), reason="oracle/_ref not built")
-@pytest.mark.parametrize("B,T,U,V,ragged", [(1, 2, 3, 5, False), (3, 17, 6, 11, True),
-                                            (2, 50, 16, 20, True), (4, 10, 6, 5, True)])
-def test_against_reference_library(B, T, U, V, ragged):
+def _ref_inputs(B, T, U, V, ragged):
+    """the inputs tests/golden/make_golden.py fed the reference library for ref_loss.npz"""
     rng = np.random.RandomState(B * 1000 + T)
     acts = rng.uniform(0, 1, size=(B, T, U, V)).astype(np.float32)
     labels = rng.randint(1, V, size=(B, U - 1)).astype(np.int32)
@@ -79,8 +83,16 @@ def test_against_reference_library(B, T, U, V, ragged):
     if ragged:
         tl[1:] = rng.randint(1, T + 1, size=B - 1)
         ul[1:] = rng.randint(0, U, size=B - 1)
+    return acts, labels, tl, ul
+
+
+@pytest.mark.parametrize("B,T,U,V,ragged", [(1, 2, 3, 5, False), (3, 17, 6, 11, True),
+                                            (2, 50, 16, 20, True), (4, 10, 6, 5, True)])
+def test_against_reference_library(B, T, U, V, ragged):
+    acts, labels, tl, ul = _ref_inputs(B, T, U, V, ragged)
     lp, _ = ol.log_softmax(acts)
-    c_ref, g_ref = ol.ref_cpu(lp, labels, tl, ul)
+    z = np.load(REF_LOSS)
+    c_ref, g_ref = z["%d_%d_%d_%d.costs" % (B, T, U, V)], z["%d_%d_%d_%d.grads" % (B, T, U, V)]
     c_o, g_o = ol.logprobs(lp, labels, tl, ul)
     assert np.allclose(c_o, c_ref, rtol=1e-6)
     # both fp32; |alpha+beta| ~ 1e2 so one ulp of the exponent argument is ~1e-5 relative
@@ -93,8 +105,9 @@ def test_against_reference_library(B, T, U, V, ragged):
     assert np.allclose(g_l, g_chain, atol=1e-4)
 
 
-@pytest.mark.skipif(not ol.have_ref(), reason="oracle/_ref not built")
 def test_reference_library_reproduces_its_own_kat():
-    lp, _ = ol.log_softmax(K.SMALL_ACTS)
-    c, _ = ol.ref_cpu(lp, K.SMALL_LABELS, [2], [2])
+    c = np.load(REF_LOSS)["small_kat.costs"]
     assert abs(c[0] - K.SMALL_COST) < 1e-4
+    lp, _ = ol.log_softmax(K.SMALL_ACTS)                    # and the oracle's CPU-entry path agrees with the library
+    c_o, _ = ol.logprobs(lp, K.SMALL_LABELS, [2], [2])
+    assert np.allclose(c_o, c, rtol=1e-6)
