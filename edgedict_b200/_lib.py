@@ -44,6 +44,8 @@ SIGNATURES = {
     "eb_lstm_c4_csave_bytes": (Z, [I, I, I]),
     "eb_lstm_c4_fwd": (I, [P, P, P, P, P, P, P, P, P, P, P, P, P, I, I, I, P]),
     "eb_lstm_c4_bwd": (I, [P, P, P, P, P, P, P, P, P, P, P, I, I, I, P]),
+    "eb_lstm_c4_bwd_chunks_cluster": (I, [I]),
+    "eb_lstm_c4_bwd_chunks": (I, [P, P, P, P, P, P, P, P, P, P, P, I, P, I, I, P]),
     "eb_layernorm_fwd": (I, [P, P, P, P, P, P, P, P, L, I, F, P]),
     "eb_layernorm_bwd": (I, [P, P, P, P, P, P, P, P, P, L, I, P]),
     "eb_time_reduce_fwd": (I, [P, P, P, I, I, I, P]),

@@ -103,6 +103,16 @@ class Embedding(torch.autograd.Function):
         return None, ops.embedding_bwd(ids, _c(dout), V, prepend_bos, bos, pad), None, None, None
 
 
+# The K-split BPTT kernel (eb_lstm_c4_bwd_chunks) runs where it measured faster than lstm_tc_bwd on an H100 at B = 32:
+# H = 1024 (6.35 - 6.49 against 7.48 - 7.67 us per step).  At H = 512 it is slower (4.98 against 4.42), at the predictor's
+# H = 256 (two clusters) the two measure the same (3.90 - 4.04 against 3.89 - 4.00); those sizes keep lstm_tc_bwd.
+C4_BPTT_MIN_H = 1024
+
+
+def _c4_bptt(H):
+    return H >= C4_BPTT_MIN_H and ops.lstm_c4_bwd_chunks_supported(H)
+
+
 class LSTMLayer(torch.autograd.Function):
     """One unidirectional batch_first nn.LSTM layer (rnnt/models.py:45-46,64-65,145-147):
     bulk input GEMM + persistent recurrent kernel; backward = BPTT kernel + three bulk GEMMs."""
@@ -148,6 +158,10 @@ class LSTMLayer(torch.autograd.Function):
         ctx.consumed = True
         if ctx.c4_bwd:
             dg16, dh0, dc0 = ops.lstm_c4_bwd(dy, gates, cseq, c0, ops.transpose_to_bf16(_c(w_hh)), dhT, dcT)
+            dg2 = dg16.view(B * T, 4 * H)
+        elif ctx.c4 and _c4_bptt(H):
+            dg16, dh0, dc0 = ops.lstm_c4_bwd_chunks(dy, gates, cseq, ops.transpose_to_bf16(_c(w_hh)), [T], B,
+                                                    torch.empty(B, T, 4 * H, dtype=bf16, device=dy.device), c0, dhT, dcT)
             dg2 = dg16.view(B * T, 4 * H)
         elif ctx.tc or ctx.c4:
             dg16, dh0, dc0 = ops.lstm_tc_bwd(dy, gates, cseq, c0, ops.transpose_to_bf16(_c(w_hh)), dhT, dcT)
@@ -429,7 +443,9 @@ class LSTMStack(torch.autograd.Function):
             else:
                 hprev = y16[l] if c4 else k.new(H, bf16, dev)  # c4 forward: h_{t-1} already written by the kernel
                 one_launch = c4 and BPTT_ONE_LAUNCH and C <= 8
-                if one_launch:                                 # the kernel walks the chunk-major buffers itself
+                if one_launch and _c4_bptt(H):                 # the kernel walks the chunk-major buffers itself
+                    ops.lstm_c4_bwd_chunks(dz, gates[l], cseq[l], whhT16, k.lens, B, dg16)
+                elif one_launch:
                     ops.lstm_tc_bwd_chunks(dz, gates[l], cseq[l], whhT16, k.lens, B, dg16)
                 for c in (() if one_launch else range(C - 1, -1, -1)):
                     _, dh, dc = ops.lstm_tc_bwd(k.blk(dz, c), k.blk(gates[l], c), k.blk(cseq[l], c),

@@ -414,6 +414,33 @@ def lstm_c4_fwd(xg, whh16, h0, c0, save, out=None, std_saves=None):
     return y, hprev16, hT, cT, gsave, csave
 
 
+_c4_chunks_ok = {}
+
+
+def lstm_c4_bwd_chunks_supported(H):
+    """True when eb_lstm_c4_bwd_chunks can run hidden size H: H % 256 == 0, H <= 1024 and all clusters of 16 co-resident."""
+    v = _c4_chunks_ok.get(H)
+    if v is None:
+        v = _c4_chunks_ok[H] = lib().eb_lstm_c4_bwd_chunks_cluster(H) == 16
+    return v
+
+
+def lstm_c4_bwd_chunks(dy, gates, cseq, whhT16, lens, B, out, c0=None, dhT=None, dcT=None):
+    """lstm_tc_bwd_chunks on the K-split wgmma kernel (clusters of 16), same saves and buffers; returns (out, dh0, dc0).
+    c0 / dhT / dcT [B,H] are optional (zero)."""
+    import ctypes
+    H = dy.shape[-1]
+    dev = dy.device
+    dh0 = torch.empty(B, H, dtype=f32, device=dev)
+    dc0 = torch.empty(B, H, dtype=f32, device=dev)
+    arr = (ctypes.c_int * len(lens))(*[int(n) for n in lens])
+    with _timed("lstm_tc_bwd", 1, 0.0, 2.0 * B * sum(lens) * 4 * H * H):
+        check(lib().eb_lstm_c4_bwd_chunks(_p(dy), _p(gates), _p(cseq), _p(c0), _p(whhT16), _p(dhT), _p(dcT), _p(out),
+                                          _p(dh0), _p(dc0), _p(_lstm_c4_scratch(B, H, dev)), B, arr, len(lens), H, _s()),
+              "eb_lstm_c4_bwd_chunks")
+    return out, dh0, dc0
+
+
 def lstm_c4_bwd(dy, gsave, csave, c0, whhT16, dhT, dcT, out=None):
     B, T, H = dy.shape
     dev = dy.device

@@ -124,7 +124,7 @@ int eb_lstm_tc_bwd_chunks(const float* dy, const float* gates, const float* cseq
  *   hprev16 [B,T,H] bf16 = h_{t-1} for every step (frame 0 = h0): the operand of the dW_hh GEMM (optional).
  * eb_lstm_c4_supported also checks that all clusters of a launch are co-resident (cooperative cluster launch). */
 int eb_lstm_c4_supported(int B, int H);
-int eb_lstm_c4_max_clusters(int H, int which);        /* diagnostic: co-resident clusters (0 fwd, 4 / 8 bwd) */
+int eb_lstm_c4_max_clusters(int H, int which);        /* diagnostic: co-resident clusters (0 fwd, 4 / 8 / 16 bwd) */
 int eb_lstm_c4_bwd_cluster(int H);                      /* cluster size the BPTT kernel uses (8 / 4), 0 = cannot run */
 int eb_lstm_c4_set_trace(void* dev_buf, int steps);     /* debug: per-stage clock64 stamps of CTA 0 ([steps][16] int64) */
 size_t eb_lstm_c4_scratch_bytes(int B, int H);
@@ -136,6 +136,14 @@ int eb_lstm_c4_fwd(const float* xg, const void* whh16, const float* h0, const fl
 int eb_lstm_c4_bwd(const float* dy, const void* gsave, const void* csave, const float* c0, const void* whhT16,
                    const float* dhT, const float* dcT, void* dg16, float* dh0, float* dc0, void* scratch, int B,
                    int T, int H, void* stream);
+/* eb_lstm_tc_bwd_chunks on the wgmma kernel: same arguments and fp32 standard-layout saves (eb_lstm_c4_fwd's gates_std /
+ * cseq_std), scratch sized by eb_lstm_c4_scratch_bytes.  The contraction is split over clusters of 16 CTAs (non-portable
+ * cluster size); it runs when eb_lstm_c4_bwd_chunks_cluster(H) == 16 (all H/128 clusters co-resident), else returns
+ * EB_ERR_INVALID.  Only the summation order of dh = W_hh^T dG differs from eb_lstm_tc_bwd_chunks. */
+int eb_lstm_c4_bwd_chunks_cluster(int H);
+int eb_lstm_c4_bwd_chunks(const float* dy, const float* gates, const float* cseq, const float* c0,
+                          const void* whhT16, const float* dhT, const float* dcT, void* dg16, float* dh0, float* dc0,
+                          void* scratch, int B, const int* chunk_lens, int nchunks, int H, void* stream);
 
 /* ---- LayerNorm(x + res) fwd/bwd, TimeReduction, Embedding -------------------------------
  * rnnt/models.py:47,66-69,124 ; :21-29 ; :150-153.  *_bf16 outputs are optional side copies. */
