@@ -427,12 +427,18 @@ inline int row_grid(long ncells, int warps) {
     return (int)(blocks < cap ? (blocks < 1 ? 1 : blocks) : cap);
 }
 
+// The problem description every loss entry validates before it launches anything: the kernels dereference the
+// lengths (and the labels, for maxU > 1) on the device, and a blank outside [0, V) would silently skip its term.
+inline bool bad_problem(const int* labels, const int* xlen, const int* ylen, int B, int maxT, int maxU, int V,
+                        int blank) {
+    return (!labels && maxU > 1) || !xlen || !ylen || B <= 0 || maxT <= 0 || maxU <= 0 || V <= 0 || blank < 0 ||
+           blank >= V || maxU > 1024;
+}
+
 template <typename T>
 int loss_fwd(const T* logits, const int* labels, const int* xlen, const int* ylen, int B, int maxT,
              int maxU, int V, int blank, void* ws, int need_beta, cudaStream_t st) {
-    if (!logits || (!labels && maxU > 1) || !xlen || !ylen || !ws || B <= 0 || maxT <= 0 || maxU <= 0 || V <= 0 ||
-        blank < 0 || blank >= V || maxU > 1024)
-        return EB_ERR_INVALID;
+    if (!logits || !ws || bad_problem(labels, xlen, ylen, B, maxT, maxU, V, blank)) return EB_ERR_INVALID;
     Workspace<T> w(ws, B, maxT, maxU);
     const long ncells = (long)B * maxT * maxU;
     constexpr int WARPS = 8;
@@ -455,7 +461,7 @@ template <typename T, typename TO>
 int loss_bwd(const T* logits, TO* grads, const int* labels, const int* xlen, const int* ylen, int B,
              int maxT, int maxU, int V, int blank, void* ws, const T* gscale, int per_batch,
              T hscale, cudaStream_t st) {
-    if (!logits || !grads || !ws) return EB_ERR_INVALID;
+    if (!logits || !grads || !ws || bad_problem(labels, xlen, ylen, B, maxT, maxU, V, blank)) return EB_ERR_INVALID;
     Workspace<T> w(ws, B, maxT, maxU);
     const long ncells = (long)B * maxT * maxU;
     constexpr int WARPS = 8;
@@ -630,7 +636,8 @@ EB_API int eb_rnnt_loss_lattice(const int* xlen, const int* ylen, int B, int max
 EB_API int eb_rnnt_loss_bwd_bf16(const void* logits16, void* grads16, const int* labels, const int* xlen,
                                  const int* ylen, int B, int maxT, int maxU, int V, int blank, void* workspace,
                                  const float* gscale_dev, int gscale_per_batch, double host_scale, void* stream) {
-    if (!logits16 || !grads16 || !workspace) return EB_ERR_INVALID;
+    if (!logits16 || !grads16 || !workspace || bad_problem(labels, xlen, ylen, B, maxT, maxU, V, blank))
+        return EB_ERR_INVALID;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     Workspace<float> w(workspace, B, maxT, maxU);
     const long ncells = (long)B * maxT * maxU;

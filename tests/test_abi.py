@@ -135,3 +135,15 @@ def test_entry_points_reject_bad_arguments_before_touching_the_device(built):
     lens0 = (ctypes.c_int * 2)(3, 0)
     assert L.eb_lstm_tc_bwd_chunks(p, p, p, None, p, None, None, p, p, p, p, 4, lens0, 2, 64, None) == 2  # empty chunk
     assert L.eb_lstm_tc_bwd_chunks(p, p, p, None, p, None, None, p, p, p, p, 4, lens, 2, 96, None) == 2   # H % 64
+    # the two loss backward entries reject what eb_rnnt_loss_fwd rejects: the kernels would dereference the missing
+    # lengths / labels on the device, and a blank outside [0, V) would silently drop its gradient term
+    good = dict(labels=p, xlen=p, ylen=p, B=2, maxT=3, maxU=4, V=8, blank=0)
+    bad = [dict(xlen=None), dict(ylen=None), dict(labels=None), dict(B=0), dict(maxT=0), dict(maxU=0), dict(V=0),
+           dict(B=-1), dict(V=-8), dict(blank=-1), dict(blank=8), dict(maxU=1025)]
+    for change in bad:
+        a = dict(good, **change)
+        args = (a["labels"], a["xlen"], a["ylen"], a["B"], a["maxT"], a["maxU"], a["V"], a["blank"])
+        assert L.eb_rnnt_loss_bwd_bf16(p, p, *args, p, None, 0, 1.0, None) == 2, change
+        for dtype_size, out_bf16 in ((4, 0), (4, 1), (8, 0)):
+            assert L.eb_rnnt_loss_bwd(p, p, out_bf16, *args, dtype_size, p, None, 0, 1.0, None) == 2, (change, dtype_size)
+        assert L.eb_rnnt_loss_fwd(p, a["labels"], a["xlen"], a["ylen"], *args[3:], 4, p, None, 1, None) == 2, change
