@@ -14,7 +14,12 @@
 //   LINEAR  y = act(x1 W1^T (+ x2 W2^T) + b)         Linear / joint (models.py:129,148,163-167)
 //   ARGMAX  token = argmax(logits) with the <unk> rule (stream.py:105-108: logit := 0, re-argmax)
 //   COPY    y = x
+//   BEAM_SELECT  per utterance: log-softmax of its W rows, exact top-W of the live slots' candidates, merge of equal
+//           token sequences, new slot log p / tokens / gather sources / history (Transducer.beam_search, one frame)
+//   GATHER  y[l, r] = x1[l, src[r]] (and y2[r] = x2[src[r]]): survivors inherit their parent's predictor state
+//   BEAM_FINAL  per utterance: best live slot, back-pointer walk through the history, ids and -log p written out
 //
+// LINEAR's x1 row divisor (x1_div) lets the W rows of one utterance's beam share its encoder frame without copies.
 // fp32-accurate arithmetic throughout: the north star asks for token-for-token identical greedy output, which
 // bf16 (or plain tf32) near-ties would break.  The matrix products run on the tensor cores as 3xTF32 split
 // products with fp32 accumulation (see tile_mma); everything else is fp32 CUDA-core code.
@@ -252,7 +257,9 @@ __device__ void phase_linear(const EbPhase& p, float* red, float* outs) {
             for (int b = 0; b < 4; ++b)
 #pragma unroll
                 for (int c = 0; c < 4; ++c) acc[a][b][c] = 0.f;
-        auto x1row = [&](int r) -> const float* { return p.x1 + (long)(s0 + r) * p.ldx1; };
+        auto x1row = [&](int r) -> const float* {
+            return p.x1 + (long)(p.x1_div > 1 ? (s0 + r) / p.x1_div : s0 + r) * p.ldx1;
+        };
         auto w1row = [&](int n) -> const float* { return p.w1 + (long)(n0 + n) * p.ldw1; };
         int step = 0;
         tile_mma(acc, x1row, w1row, p.K1, nrows, ncols, a1vec, b1vec, step);
@@ -332,6 +339,328 @@ __device__ void phase_argmax(const EbPhase& p) {
     }
 }
 
+// ---- beam search: B utterances x W slots, row r = b*W + slot, T' = hist_ld frames.  Field use:
+//   BEAM_SELECT (S = B, aux = W, N = V, aux2 = blank, hist_col = t, flags 16 = merge): x1 logits [B*W, V] (ldx1);
+//     y slot log p [B*W] (in/out, dead slots -inf); tok_in frames [B]; tok_out token per row (blank for dead and
+//     frozen rows, so the masked predictor skips them); src gather source row [B*W]; seq_in / seq_out token
+//     sequences [B*W][T'+3] = {len, hash lo, hash hi, tokens} of frame t-1 / t (two buffers alternating by frame);
+//     hist = parent slot [B,T',W] | token [B,T',W] | log p (fp32 bits) [B,T',W] | live count [B,T'], back to back.
+//     Slots 0..live-1 are live.  Frozen frames (t >= frames[b]) write an identity history entry.
+//   BEAM_FINAL (S = B, aux = W, aux2 = blank): y slot log p; hist; tok_out ids [B][ldy], the non-blank tokens of the
+//     best live slot right-aligned in the row and -1 before them; y2 -log p of that slot [B].
+// Both run one CTA per utterance (grid-strided over B).  They are __noinline__ so that their registers do not
+// count against the tensor-core phases the streaming decode spends its time in.
+constexpr int BEAM_MAX_W = EB_BEAM_MAX_W;
+constexpr unsigned long long SEQ_HASH_MUL = 0x100000001b3ull;      // polynomial hash: h' = h * MUL + (token + 1)
+// BEAM_SELECT's shared memory (2 x u64 + 10 x 32-bit arrays of BEAM_MAX_W, histogram, scalars) lives in the dynamic
+// shared memory the matrix phases use
+static_assert(BEAM_MAX_W * (2 * 8 + 10 * 4) + 256 * 4 + 8 * 4 <= (RED_FLOATS + TR * OUT_LD) * 4, "beam smem");
+
+// order-preserving map of a float to uint32 (larger float -> larger key); -0 ranks with +0 as in a float compare
+__device__ __forceinline__ uint32_t order_key(float v) {
+    if (v == 0.f) v = 0.f;
+    const uint32_t b = __float_as_uint(v);
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ float key_value(uint32_t u) {
+    return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
+}
+// low half of a candidate's composite key: the lowest flat index ranks first (the map is its own inverse)
+__device__ __forceinline__ unsigned tie_key(unsigned flat) { return 0xffffffffu - flat; }
+// torch.logaddexp
+__device__ __forceinline__ float logaddexp_(float a, float b) {
+    const float m = fmaxf(a, b);
+    if (m == -INFINITY) return m;
+    return m + log1pf(expf(-fabsf(a - b)));
+}
+// s2 == s1 + [k1], exactly (rows of the sequence buffer)
+__device__ bool seq_extends(const int* s2, const int* s1, int k1) {
+    const int n1 = __ldcg(s1);
+    if (__ldcg(s2) != n1 + 1 || __ldcg(s2 + 3 + n1) != k1) return false;
+    for (int i = 0; i < n1; ++i)
+        if (__ldcg(s2 + 3 + i) != __ldcg(s1 + 3 + i)) return false;
+    return true;
+}
+
+// Selection: the candidates of one utterance are (slot q < live, token k) with value
+//   lp = ((x[q,k] - max_q) - log sum_k exp(x[q,k] - max_q)) + logp[q],
+// ranked by value descending, ties by the lowest flat index q*V + k.  Each candidate's 64-bit composite
+// (order_key(lp) << 32 | tie_key(flat)) is unique and orders exactly so; a radix select finds the min(W, live*V)-th largest
+// composite 8 bits at a time (a 256-bin shared-memory histogram per pass, stopping at the first pass whose chosen bin
+// holds exactly the remaining count: 3-4 passes without exact value ties, at most 8), one more pass collects the
+// survivors and a bitonic sort of those <= W composites gives the walk order.  Cost per frame and utterance: about
+// 4-5 passes over live*V candidates read from L2 (W = 64, V = 1024: 64 K candidates, 256 per thread per pass) and
+// O(W log^2 W) for the sort.  Merging (rule: a candidate whose token sequence equals an earlier survivor's is folded
+// into it by log-add) compares survivor i with every earlier one, O(W) per thread.  Because the previous beam was
+// already merged, two distinct candidates can only have equal sequences when one is the blank extension of a parent
+// q2 and the other the non-blank extension seq(q1) + [k]; length and a 64-bit hash reject the rest, and a hash match
+// is confirmed by an exact token-by-token comparison (seq_extends), never accepted on its own.
+__device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
+    const int W = p.aux, V = p.N, T = p.hist_ld, t = p.hist_col, blank = p.aux2;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nt = blockDim.x;
+    const bool merge = p.flags & 16;
+    const long BTW = (long)p.S * T * W;
+    int* hpar = p.hist;
+    int* htok = p.hist + BTW;
+    float* hlp = reinterpret_cast<float*>(p.hist + 2 * BTW);
+    int* hlive = p.hist + 3 * BTW;
+    const int LS = T + 3;
+    unsigned long long* comp = reinterpret_cast<unsigned long long*>(sm);       // [BEAM_MAX_W] (padded to 2^k)
+    unsigned long long* shash = comp + BEAM_MAX_W;
+    float* rowm = reinterpret_cast<float*>(shash + BEAM_MAX_W);
+    float* rowls = rowm + BEAM_MAX_W;
+    float* rowlp = rowls + BEAM_MAX_W;
+    float* sval = rowlp + BEAM_MAX_W;
+    float* smlp = sval + BEAM_MAX_W;
+    int* spar = reinterpret_cast<int*>(smlp + BEAM_MAX_W);
+    int* stok = spar + BEAM_MAX_W;
+    int* slen = stok + BEAM_MAX_W;
+    int* sfirst = slen + BEAM_MAX_W;
+    int* skept = sfirst + BEAM_MAX_W;                                           // slot -> survivor index
+    unsigned* rhist = reinterpret_cast<unsigned*>(skept + BEAM_MAX_W);          // [256]
+    int* misc = reinterpret_cast<int*>(rhist + 256);
+    for (int b = blockIdx.x; b < p.S; b += gridDim.x) {
+        const long r0 = (long)b * W, h0 = ((long)b * T + t) * W;
+        const int nlive = t == 0 ? 1 : __ldcg(hlive + (long)b * T + t - 1);
+        __syncthreads();                                     // the previous utterance is done with shared memory
+        if (t >= __ldg(p.tok_in + b)) {                      // frozen: the beam stays, the predictor rests
+            for (int j = tid; j < W; j += nt) {
+                hpar[h0 + j] = j;
+                htok[h0 + j] = blank;
+                hlp[h0 + j] = __ldcg(p.y + r0 + j);
+                p.tok_out[r0 + j] = blank;
+                p.src[r0 + j] = (int)(r0 + j);
+            }
+            if (tid == 0) hlive[(long)b * T + t] = nlive;
+            continue;
+        }
+        // per-row log-softmax statistics (warp per row)
+        for (int q = warp; q < nlive; q += nt >> 5) {
+            const float* x = p.x1 + (r0 + q) * p.ldx1;
+            float m = -INFINITY;
+            for (int k = lane; k < V; k += 32) m = fmaxf(m, __ldcg(x + k));
+            m = warp_max(m);
+            float s = 0.f;
+            for (int k = lane; k < V; k += 32) s += expf(__ldcg(x + k) - m);
+            s = warp_sum(s);
+            if (lane == 0) {
+                rowm[q] = m;
+                rowls[q] = logf(s);
+                rowlp[q] = __ldcg(p.y + r0 + q);
+            }
+        }
+        __syncthreads();
+        auto composite = [&](int q, int k, const float* x) -> unsigned long long {
+            const float v = ((__ldcg(x + k) - rowm[q]) - rowls[q]) + rowlp[q];
+            return ((unsigned long long)order_key(v) << 32) | tie_key((unsigned)(q * V + k));
+        };
+        const int nsel = (int)min((long)W, (long)nlive * V);
+        unsigned need = nsel;
+        unsigned long long prefix = 0, mask = 0;
+        for (int shift = 56; shift >= 0; shift -= 8) {
+            for (int i = tid; i < 256; i += nt) rhist[i] = 0;
+            __syncthreads();
+            for (int q = 0; q < nlive; ++q) {
+                const float* x = p.x1 + (r0 + q) * p.ldx1;
+                for (int k = tid; k < V; k += nt) {
+                    const unsigned long long c = composite(q, k, x);
+                    if ((c & mask) == prefix) atomicAdd(&rhist[(c >> shift) & 255], 1u);
+                }
+            }
+            __syncthreads();
+            if (warp == 0) {                                 // lane l owns bins 255-8l .. 248-8l, scanned from the top
+                unsigned cnt[8], s = 0;
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                    cnt[i] = rhist[255 - 8 * lane - i];
+                    s += cnt[i];
+                }
+                unsigned inc = s;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    const unsigned v = __shfl_up_sync(0xffffffffu, inc, o);
+                    if (lane >= o) inc += v;
+                }
+                unsigned above = inc - s;
+                if (above < need && need <= inc) {
+                    int i = 0;
+                    while (above + cnt[i] < need) above += cnt[i++];
+                    misc[0] = 255 - 8 * lane - i;
+                    misc[1] = (int)above;
+                    misc[2] = (int)cnt[i];
+                }
+            }
+            __syncthreads();
+            need -= (unsigned)misc[1];
+            prefix |= (unsigned long long)misc[0] << shift;
+            mask |= 0xffull << shift;
+            if ((unsigned)misc[2] == need) break;            // every candidate under this prefix survives
+        }
+        if (tid == 0) misc[3] = 0;
+        __syncthreads();
+        for (int q = 0; q < nlive; ++q) {
+            const float* x = p.x1 + (r0 + q) * p.ldx1;
+            for (int k = tid; k < V; k += nt) {
+                const unsigned long long c = composite(q, k, x);
+                if ((c & mask) >= prefix) {
+                    const int i = atomicAdd(&misc[3], 1);
+                    if (i < nsel) comp[i] = c;               // exactly nsel pass; the guard keeps smem safe regardless
+                }
+            }
+        }
+        int P = 1;
+        while (P < nsel) P <<= 1;
+        for (int i = nsel + tid; i < P; i += nt) comp[i] = 0;
+        __syncthreads();
+        for (int kk = 2; kk <= P; kk <<= 1)                  // bitonic sort, descending
+            for (int jj = kk >> 1; jj > 0; jj >>= 1) {
+                for (int i = tid; i < P; i += nt) {
+                    const int l = i ^ jj;
+                    if (l > i) {
+                        const unsigned long long a = comp[i], c = comp[l];
+                        if ((i & kk) == 0 ? a < c : a > c) {
+                            comp[i] = c;
+                            comp[l] = a;
+                        }
+                    }
+                }
+                __syncthreads();
+            }
+        // survivors in walk order: parent, token, value, and the length / hash of the extended sequence
+        for (int i = tid; i < nsel; i += nt) {
+            const unsigned long long c = comp[i];
+            const unsigned f = tie_key((unsigned)c);
+            const int q = (int)(f / V), k = (int)(f % V);
+            const int* ps = p.seq_in + (r0 + q) * LS;
+            int len = __ldcg(ps);
+            unsigned long long h = (unsigned)__ldcg(ps + 1) | ((unsigned long long)(unsigned)__ldcg(ps + 2) << 32);
+            if (k != blank) {
+                ++len;
+                h = h * SEQ_HASH_MUL + (unsigned)(k + 1);
+            }
+            spar[i] = q;
+            stok[i] = k;
+            sval[i] = key_value((unsigned)(c >> 32));
+            slen[i] = len;
+            shash[i] = h;
+        }
+        if (tid == 0) misc[4] = 0;
+        __syncthreads();
+        for (int i = tid; i < nsel; i += nt) {
+            int first = i;
+            if (merge) {
+                const bool ib = stok[i] == blank;
+                for (int j = 0; j < i; ++j) {
+                    if ((stok[j] == blank) == ib || slen[j] != slen[i] || shash[j] != shash[i]) continue;
+                    const int q2 = ib ? spar[i] : spar[j], q1 = ib ? spar[j] : spar[i], k1 = ib ? stok[j] : stok[i];
+                    if (seq_extends(p.seq_in + (r0 + q2) * LS, p.seq_in + (r0 + q1) * LS, k1)) {
+                        first = j;
+                        break;
+                    }
+                }
+            }
+            sfirst[i] = first;
+        }
+        __syncthreads();
+        for (int i = tid; i < nsel; i += nt) {
+            if (sfirst[i] != i) continue;
+            int slot = 0;
+            for (int j = 0; j < i; ++j) slot += sfirst[j] == j;
+            float lp = sval[i];
+            for (int j = i + 1; j < nsel; ++j)               // fold in walk order, as the host loop did
+                if (sfirst[j] == i) lp = logaddexp_(lp, sval[j]);
+            smlp[i] = lp;
+            skept[slot] = i;
+            atomicAdd(&misc[4], 1);
+        }
+        __syncthreads();
+        const int nkept = misc[4];
+        for (int s = tid; s < W; s += nt) {
+            const long h = h0 + s, r = r0 + s;
+            if (s < nkept) {
+                const int i = skept[s], k = stok[i];
+                p.y[r] = smlp[i];
+                p.tok_out[r] = k;
+                p.src[r] = (int)(r0 + spar[i]);
+                hpar[h] = spar[i];
+                htok[h] = k;
+                hlp[h] = smlp[i];
+                int* d = p.seq_out + r * LS;
+                d[0] = slen[i];
+                d[1] = (int)(unsigned)shash[i];
+                d[2] = (int)(unsigned)(shash[i] >> 32);
+            } else {
+                p.y[r] = -INFINITY;
+                p.tok_out[r] = blank;
+                p.src[r] = (int)r;
+                hpar[h] = s;
+                htok[h] = blank;
+                hlp[h] = -INFINITY;
+            }
+        }
+        if (tid == 0) hlive[(long)b * T + t] = nkept;
+        for (int s = 0; s < nkept; ++s) {                    // token sequences of the new beam
+            const int i = skept[s], len = slen[i];
+            const int* ps = p.seq_in + (r0 + spar[i]) * LS + 3;
+            int* d = p.seq_out + (r0 + s) * LS + 3;
+            for (int j = tid; j < len; j += nt) d[j] = (stok[i] != blank && j == len - 1) ? stok[i] : __ldcg(ps + j);
+        }
+    }
+}
+
+__device__ __noinline__ void phase_gather(const EbPhase& p) {
+    const long gtid = (long)blockIdx.x * blockDim.x + threadIdx.x, gn = (long)gridDim.x * blockDim.x;
+    const int S = p.S, N = p.N;
+    for (long e = gtid; e < (long)p.aux * S * N; e += gn) {
+        const long lr = e / N;
+        const int c = (int)(e - lr * N), r = (int)(lr % S);
+        p.y[e] = __ldcg(p.x1 + ((lr - r) + __ldcg(p.src + r)) * N + c);
+    }
+    if (p.x2)
+        for (long e = gtid; e < (long)S * p.K2; e += gn) {
+            const int r = (int)(e / p.K2), c = (int)(e % p.K2);
+            p.y2[e] = __ldcg(p.x2 + (long)__ldcg(p.src + r) * p.K2 + c);
+        }
+}
+
+__device__ __noinline__ void phase_beam_final(const EbPhase& p) {
+    const int W = p.aux, T = p.hist_ld, blank = p.aux2, lane = threadIdx.x & 31;
+    const long BTW = (long)p.S * T * W;
+    const int* hpar = p.hist;
+    const int* htok = p.hist + BTW;
+    const int* hlive = p.hist + 3 * BTW;
+    if (threadIdx.x >= 32) return;
+    for (int b = blockIdx.x; b < p.S; b += gridDim.x) {
+        const int nlive = T == 0 ? 1 : __ldcg(hlive + (long)b * T + T - 1);
+        float best = -INFINITY;
+        int bi = -1;
+        for (int j = lane; j < nlive; j += 32) {
+            const float v = __ldcg(p.y + (long)b * W + j);
+            if (bi < 0 || v > best) { best = v; bi = j; }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {                   // logp.argmax(): the lowest slot on ties
+            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+            if (oi >= 0 && (bi < 0 || ob > best || (ob == best && oi < bi))) { best = ob; bi = oi; }
+        }
+        int* ids = p.tok_out + (long)b * p.ldy;
+        int pos = T;
+        if (lane == 0) {
+            int slot = bi;
+            for (int tt = T - 1; tt >= 0; --tt) {
+                const long h = ((long)b * T + tt) * W + slot;
+                const int k = __ldcg(htok + h);
+                if (k != blank) ids[--pos] = k;
+                slot = __ldcg(hpar + h);
+            }
+            p.y2[b] = -best;
+        }
+        pos = __shfl_sync(0xffffffffu, pos, 0);
+        for (int j = lane; j < pos; j += 32) ids[j] = -1;
+    }
+}
+
 __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __restrict__ prog, int nphase, unsigned* bar) {
     extern __shared__ __align__(16) float dsm[];
     float* red = dsm;                                        // [8 warps][2048]
@@ -362,6 +691,9 @@ __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __re
             case EB_PH_COPY:
                 for (long k = gtid; k < (long)ph.S * ph.N; k += gn) ph.y[k] = __ldcg(ph.x1 + k);
                 break;
+            case EB_PH_BEAM_SELECT: phase_beam_select(ph, dsm); break;
+            case EB_PH_GATHER: phase_gather(ph); break;
+            case EB_PH_BEAM_FINAL: phase_beam_final(ph); break;
             default: break;
         }
         ++epoch;

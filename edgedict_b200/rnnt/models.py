@@ -12,6 +12,7 @@ precision: "fp32" (default; parity mode, CUDA-core GEMMs, matches torch-CPU fp32
 "bf16" (wgmma tensor-core GEMMs with fp32 accumulation; also selected automatically inside
 ``torch.autocast('cuda')``, the modern spelling of the reference's apex-O1 switch).
 """
+import operator
 import os
 
 import torch
@@ -328,53 +329,37 @@ class Transducer(nn.Module):
         legacy v0 stack holds a batch-1 Graves-style search (models.py:121-202, with no-op `sorted(...)` calls and a
         removed `volatile=` API).  This is a time-synchronous beam under the SAME emission constraint as
         `greedy_decode` (at most one symbol per encoder frame, rnnt/models.py:243-269): per frame every hypothesis is
-        scored against the whole vocabulary in one joint call, the W best continuations survive (hypotheses that
-        reach the same token sequence are merged by log-add when `merge`), and only the survivors that emitted a
-        non-blank take a predictor step (one batched call).  W = 1 reproduces `greedy_decode` token for token.
-        xs [B,T,F] -> (list of non-blank id lists, -log p [B]); utterances are searched one at a time like the
-        reference's beam."""
-        h_enc_all, _ = self.encoder(xs)
-        B, Tn = h_enc_all.shape[0], h_enc_all.shape[1]
-        dev = h_enc_all.device
-        outs, nlps = [], []
-        for b in range(B):
-            frames = Tn if xlen is None else min(Tn, int(scale_length(Tn, xlen)[b]))
-            dec_x, (dh, dc) = self.decoder(torch.zeros(1, 0, dtype=torch.long, device=dev))     # BOS prime
-            dec_x = dec_x[:, 0]                                                                   # [n, D]
-            seqs, logp = [[]], torch.zeros(1, device=dev)
-            for t in range(frames):
-                n = dec_x.shape[0]
-                he = h_enc_all[b, t][None].expand(n, -1).contiguous()
-                logits = self.joint(he, dec_x.contiguous())                                      # [n, V]
-                lp = torch.log_softmax(logits.float(), 1) + logp[:, None]                        # [n, V]
-                V = lp.shape[1]
-                top, idx = lp.reshape(-1).topk(min(W, n * V))                                   # ties: lowest index first
-                par, tok = (idx // V).tolist(), (idx % V).tolist()
-                new_seqs = [seqs[q] + ([k] if k != self.blank else []) for q, k in zip(par, tok)]
-                keep, merged_lp, seen = [], [], {}
-                for i, sq in enumerate(new_seqs):
-                    key = tuple(sq)
-                    if merge and key in seen:
-                        j = seen[key]
-                        merged_lp[j] = torch.logaddexp(merged_lp[j], top[i])
-                        continue
-                    seen[key] = len(keep)
-                    keep.append(i)
-                    merged_lp.append(top[i])
-                par_t = torch.tensor([par[i] for i in keep], device=dev)
-                tok_t = torch.tensor([tok[i] for i in keep], device=dev)
-                seqs = [new_seqs[i] for i in keep]
-                logp = torch.stack(merged_lp)
-                dec_x, dh, dc = dec_x[par_t], dh[:, par_t], dc[:, par_t]
-                nb = (tok_t != self.blank).nonzero()[:, 0]
-                if nb.numel():
-                    nx, (nh, nc) = self.decoder(tok_t[nb][:, None], (dh[:, nb].contiguous(), dc[:, nb].contiguous()))
-                    dec_x, dh, dc = dec_x.clone(), dh.clone(), dc.clone()
-                    dec_x[nb], dh[:, nb], dc[:, nb] = nx[:, 0], nh, nc
-            best = int(logp.argmax())
-            outs.append(seqs[best])
-            nlps.append(-logp[best])
-        return outs, torch.stack(nlps)
+        scored against the whole vocabulary, the W best continuations survive (ties to the lowest hypothesis, then
+        token index; hypotheses that reach the same token sequence are merged by log-add when `merge`), and only the
+        survivors that emitted a non-blank take a predictor step.  W = 1 reproduces `greedy_decode` token for token.
+        xs [B,T,F] -> (list of non-blank id lists, -log p [B]).  Utterance b decodes min(T', scale_length(xlen)[b])
+        encoder frames (all T' when xlen is None).
+
+        All utterances are searched together on the device after the encoder, in one persistent kernel launch
+        (stream_engine.BeamEngine); each utterance's result does not depend on the rest of the batch.  The joint and
+        the log-softmax run in fp32-accurate arithmetic (3xTF32 products, fp32 log-softmax) whatever `set_precision`
+        or autocast says, as in `greedy_decode`; only the encoder follows the precision setting."""
+        from ..stream_engine import BeamEngine, BEAM_MAX_W, param_fingerprint
+        W = operator.index(W)
+        if not 1 <= W <= BEAM_MAX_W:
+            raise ValueError("beam width W must be in [1, %d], got %d" % (BEAM_MAX_W, W))
+        h_enc, _ = self.encoder(xs)
+        B, T = h_enc.shape[0], h_enc.shape[1]
+        if xlen is None:
+            frames = torch.full((B,), T, dtype=torch.int32)
+        else:
+            frames = scale_length(T, xlen).clamp(max=T).to(torch.int32)
+        frames = _lens_to_device(frames.cpu(), h_enc.device)
+        # the phase program bakes raw weight pointers: re-homed parameters (FlatAdam, .to(), .float()) rebuild it
+        key = (B, T, W, bool(merge), h_enc.device, param_fingerprint(self))
+        cache = self.__dict__.setdefault("_beam_engines", {})
+        eng = cache.get(key)
+        if eng is None:
+            cache.clear()                                  # one resident program is enough
+            eng = cache[key] = BeamEngine(self, B, T, W, merge=bool(merge), blank=self.blank)
+        ids, nlogp = eng.run(h_enc, frames)
+        ids = ids.cpu().numpy()
+        return [[int(k) for k in row if k >= 0] for row in ids], nlogp.clone()
 
 
 def _i32(t):

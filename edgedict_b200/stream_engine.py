@@ -15,19 +15,40 @@ import torch
 from ._lib import lib, check
 from .rnnt.tokenizer import NUL, BOS, UNK
 
-PH_LN, PH_PAIR, PH_LSTM, PH_LINEAR, PH_ARGMAX, PH_COPY = range(6)
-F_TANH, F_EMBED, F_MASKED, F_LOGP = 1, 2, 4, 8
+PH_LN, PH_PAIR, PH_LSTM, PH_LINEAR, PH_ARGMAX, PH_COPY, PH_BEAM_SELECT, PH_GATHER, PH_BEAM_FINAL = range(9)
+F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE = 1, 2, 4, 8, 16
+BEAM_MAX_W = 1024                                     # EB_BEAM_MAX_W
 
 
 class EbPhase(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("type", "S", "K1", "K2", "N", "flags", "ldx1", "ldx2", "ldw1", "ldw2",
-                                         "ldy", "aux", "aux2", "hist_ld", "hist_col", "pad_")] + \
+                                         "ldy", "aux", "aux2", "hist_ld", "hist_col", "x1_div")] + \
                [(n, C.c_void_p) for n in ("x1", "x2", "w1", "w2", "b1", "b2", "y", "y2", "c", "tok_in", "tok_out",
-                                          "hist")]
+                                          "hist", "seq_in", "seq_out", "src")]
 
 
 def _ptr(t, off=0):
     return None if t is None else t.data_ptr() + off * t.element_size()
+
+
+def predictor_phases(prog, dec, S, h, c, htmp, x, tok, blank, masked):
+    """Append one predictor step for S rows to the phase list ``prog``: the embedding row of ``tok`` through every
+    LSTM layer (h, c, htmp [Ld, S, Hd]; with ``masked``, rows whose token is ``blank`` keep their state), then the
+    projection into x [S, D]."""
+    Ld, Hd = dec.lstm.num_layers, dec.lstm.hidden_size
+    Em, D = dec.embed.weight.shape[1], dec.proj.weight.shape[0]
+    fl = F_EMBED | (F_MASKED if masked else 0)
+    for k in range(Ld):
+        w = [getattr(dec.lstm, n % k) for n in ("weight_ih_l%d", "weight_hh_l%d", "bias_ih_l%d", "bias_hh_l%d")]
+        prog.append(EbPhase(type=PH_LSTM, S=S, N=Hd, K1=Em if k == 0 else Hd, K2=Hd,
+                            flags=fl if k == 0 else (fl & F_MASKED),
+                            x1=_ptr(dec.embed.weight) if k == 0 else _ptr(htmp[k - 1]), ldx1=Em if k == 0 else Hd,
+                            x2=_ptr(h[k]), ldx2=Hd, w1=_ptr(w[0]), ldw1=w[0].shape[1], w2=_ptr(w[1]), ldw2=Hd,
+                            b1=_ptr(w[2]), b2=_ptr(w[3]), c=_ptr(c[k]), y=_ptr(htmp[k]), ldy=Hd, tok_in=_ptr(tok),
+                            aux=blank))
+    prog.append(EbPhase(type=PH_COPY, S=Ld * S, N=Hd, x1=_ptr(htmp), y=_ptr(h)))
+    prog.append(EbPhase(type=PH_LINEAR, S=S, N=D, K1=Hd, x1=_ptr(h[Ld - 1]), ldx1=Hd, w1=_ptr(dec.proj.weight),
+                        ldw1=Hd, b1=_ptr(dec.proj.bias), y=_ptr(x), ldy=D))
 
 
 def param_fingerprint(module):
@@ -101,7 +122,6 @@ class StreamEngine:
             self.enc_out = X
         # ---- predictor + joint state
         Ld, Hd = dec.lstm.num_layers, dec.lstm.hidden_size
-        Em = dec.embed.weight.shape[1]
         D = dec.proj.weight.shape[0]
         J, V = joint[0].weight.shape[0], joint[2].weight.shape[0]
         assert joint[0].weight.shape[1] == E + D
@@ -109,19 +129,6 @@ class StreamEngine:
         self.dec_x, self.hidden, self.logits = z(S, D), z(S, J), z(S, V)
         self.tok = torch.zeros(S, dtype=torch.int32, device=self.dev)
         self.hist = torch.zeros(S, max(ni, 1), dtype=torch.int32, device=self.dev)
-
-        def predictor_phases(masked):
-            fl = F_EMBED | (F_MASKED if masked else 0)
-            for k in range(Ld):
-                w = [getattr(dec.lstm, s % k) for s in ("weight_ih_l%d", "weight_hh_l%d", "bias_ih_l%d", "bias_hh_l%d")]
-                ph(type=PH_LSTM, S=S, N=Hd, K1=Em if k == 0 else Hd, K2=Hd, flags=fl if k == 0 else (fl & F_MASKED),
-                   x1=_ptr(dec.embed.weight) if k == 0 else _ptr(self.dec_htmp[k - 1]), ldx1=Em if k == 0 else Hd,
-                   x2=_ptr(self.dec_h[k]), ldx2=Hd, w1=_ptr(w[0]), ldw1=w[0].shape[1], w2=_ptr(w[1]), ldw2=Hd,
-                   b1=_ptr(w[2]), b2=_ptr(w[3]), c=_ptr(self.dec_c[k]), y=_ptr(self.dec_htmp[k]), ldy=Hd,
-                   tok_in=_ptr(self.tok), aux=blank)
-            ph(type=PH_COPY, S=Ld * S, N=Hd, x1=_ptr(self.dec_htmp), y=_ptr(self.dec_h))
-            ph(type=PH_LINEAR, S=S, N=D, K1=Hd, x1=_ptr(self.dec_h[Ld - 1]), ldx1=Hd, w1=_ptr(dec.proj.weight), ldw1=Hd,
-               b1=_ptr(dec.proj.bias), y=_ptr(self.dec_x), ldy=D)
 
         w1 = joint[0].weight
         for k in range(ni):
@@ -132,12 +139,14 @@ class StreamEngine:
                b1=_ptr(joint[2].bias), y=_ptr(self.logits), ldy=V)
             ph(type=PH_ARGMAX, S=S, N=V, x1=_ptr(self.logits), ldx1=V, aux=blank, aux2=unk_id, tok_out=_ptr(self.tok),
                hist=_ptr(self.hist), hist_ld=self.hist.shape[1], hist_col=k)
-            predictor_phases(masked=True)
+            predictor_phases(prog, dec, S, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
+                             masked=True)
         ph(type=PH_COPY, S=L * S, N=H, x1=_ptr(self.enc_htmp), y=_ptr(self.enc_h))
         self.n_chunk_phases = len(prog)
         chunk_prog = prog
         prog = []
-        predictor_phases(masked=False)                  # priming program: tok = BOS from a zero state
+        predictor_phases(prog, dec, S, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
+                         masked=False)                  # priming program: tok = BOS from a zero state
         self.n_prime_phases = len(prog)
         self._chunk = self._upload(chunk_prog)
         self._prime = self._upload(prog)
@@ -197,7 +206,7 @@ class GreedyEngine:
         self.B, self.T, self.blank, self.max_ctas = B, T, blank, max_ctas
         z = lambda *shape: torch.zeros(*shape, dtype=f32, device=self.dev)
         Ld, Hd = dec.lstm.num_layers, dec.lstm.hidden_size
-        Em, D = dec.embed.weight.shape[1], dec.proj.weight.shape[0]
+        D = dec.proj.weight.shape[0]
         J, V = joint[0].weight.shape[0], joint[2].weight.shape[0]
         E = joint[0].weight.shape[1] - D
         self.h_enc = z(B, T, E)
@@ -215,20 +224,8 @@ class GreedyEngine:
                 setattr(q, k, v)
             prog.append(q)
 
-        def predictor(masked):
-            fl = F_EMBED | (F_MASKED if masked else 0)
-            for k in range(Ld):
-                w = [getattr(dec.lstm, n % k) for n in ("weight_ih_l%d", "weight_hh_l%d", "bias_ih_l%d", "bias_hh_l%d")]
-                ph(type=PH_LSTM, S=B, N=Hd, K1=Em if k == 0 else Hd, K2=Hd, flags=fl if k == 0 else (fl & F_MASKED),
-                   x1=_ptr(dec.embed.weight) if k == 0 else _ptr(self.dec_htmp[k - 1]), ldx1=Em if k == 0 else Hd,
-                   x2=_ptr(self.dec_h[k]), ldx2=Hd, w1=_ptr(w[0]), ldw1=w[0].shape[1], w2=_ptr(w[1]), ldw2=Hd,
-                   b1=_ptr(w[2]), b2=_ptr(w[3]), c=_ptr(self.dec_c[k]), y=_ptr(self.dec_htmp[k]), ldy=Hd,
-                   tok_in=_ptr(self.tok), aux=blank)
-            ph(type=PH_COPY, S=Ld * B, N=Hd, x1=_ptr(self.dec_htmp), y=_ptr(self.dec_h))
-            ph(type=PH_LINEAR, S=B, N=D, K1=Hd, x1=_ptr(self.dec_h[Ld - 1]), ldx1=Hd, w1=_ptr(dec.proj.weight), ldw1=Hd,
-               b1=_ptr(dec.proj.bias), y=_ptr(self.dec_x), ldy=D)
-
-        predictor(masked=False)                          # prime with BOS from the zero state
+        predictor_phases(prog, dec, B, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
+                         masked=False)                   # prime with BOS from the zero state
         w1 = joint[0].weight
         for k in range(T):
             ph(type=PH_LINEAR, S=B, N=J, flags=F_TANH, K1=E, x1=_ptr(self.h_enc, k * E), ldx1=T * E, w1=_ptr(w1),
@@ -238,7 +235,8 @@ class GreedyEngine:
                b1=_ptr(joint[2].bias), y=_ptr(self.logits), ldy=V)
             ph(type=PH_ARGMAX, S=B, N=V, flags=F_LOGP, x1=_ptr(self.logits), ldx1=V, aux=blank, aux2=-1,
                tok_out=_ptr(self.tok), hist=_ptr(self.hist), hist_ld=T, hist_col=k, y=_ptr(self.logp))
-            predictor(masked=True)
+            predictor_phases(prog, dec, B, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
+                             masked=True)
         self.nphase = len(prog)
         arr = (EbPhase * len(prog))(*prog)
         self._prog = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(self.dev)
@@ -254,3 +252,90 @@ class GreedyEngine:
         check(lib().eb_decode_run(self._prog.data_ptr(), self.nphase, self._bar.data_ptr(), self.max_ctas,
                                   torch.cuda.current_stream().cuda_stream), "eb_decode_run")
         return self.hist, self.logp
+
+
+class BeamEngine:
+    """Device-side batched beam search (Transducer.beam_search): the time-synchronous beam under greedy_decode's
+    emission rule (at most one symbol per encoder frame) for B utterances of W slots each, in ONE cooperative kernel
+    launch.  Row r = b*W + j holds slot j of utterance b.  Per frame: joint hidden (the encoder frame shared by the
+    utterance's W rows) and logits for every row, BEAM_SELECT (log-softmax, exact top-W of the live slots' candidates,
+    ties to the lowest flat index slot*V + token, merge of equal token sequences by log-add when ``merge``), GATHER of
+    the parents' predictor state, and the masked predictor step for the survivors that emitted a non-blank.  The
+    predictor state alternates between two buffers by frame parity (a permutation cannot be gathered in place).
+    BEAM_FINAL picks the best live slot of each utterance and walks its back-pointers.
+
+    ``hist_parent`` / ``hist_token`` / ``hist_logp`` [B, T', W] and ``hist_live`` [B, T'] keep the beam of every
+    frame (slots below the live count are live; frames at or past an utterance's length repeat its last beam)."""
+
+    def __init__(self, transducer, batch, t_out, W, merge=True, blank=NUL, max_ctas=0):
+        if not 1 <= W <= BEAM_MAX_W:
+            raise ValueError("beam width must be in [1, %d], got %r" % (BEAM_MAX_W, W))
+        dec, joint = transducer.decoder, transducer.joint.joint
+        self.dev = dec.embed.weight.device
+        if self.dev.type != "cuda":
+            raise RuntimeError("BeamEngine needs the model on a CUDA device")
+        f32, i32 = torch.float32, torch.int32
+        B, T, R = batch, t_out, batch * W
+        self.B, self.T, self.W, self.merge, self.blank, self.max_ctas = B, T, W, merge, blank, max_ctas
+        z = lambda *shape, dtype=f32: torch.zeros(*shape, dtype=dtype, device=self.dev)
+        Ld, Hd = dec.lstm.num_layers, dec.lstm.hidden_size
+        D = dec.proj.weight.shape[0]
+        J, V = joint[0].weight.shape[0], joint[2].weight.shape[0]
+        E = joint[0].weight.shape[1] - D
+        self.h_enc, self.frames = z(B, T, E), z(B, dtype=i32)
+        st = [z(2 * Ld, R, Hd), z(2 * Ld, R, Hd)]              # [h of every layer | c of every layer], per parity
+        self.dec_h, self.dec_c = [s[:Ld] for s in st], [s[Ld:] for s in st]
+        self.dec_x = [z(R, D), z(R, D)]
+        self.dec_htmp, self.hidden, self.logits = z(Ld, R, Hd), z(R, J), z(R, V)
+        self.tok, self.src, self.logp = z(R, dtype=i32), z(R, dtype=i32), z(R)
+        self.seqs = z(2, R, T + 3, dtype=i32)                  # {len, hash lo, hash hi, tokens} per row, per parity
+        n = B * T * W
+        self.hist = z(3 * n + B * T, dtype=i32)
+        self.hist_parent = self.hist[:n].view(B, T, W)
+        self.hist_token = self.hist[n:2 * n].view(B, T, W)
+        self.hist_logp = self.hist[2 * n:3 * n].view(f32).view(B, T, W)
+        self.hist_live = self.hist[3 * n:].view(B, T)
+        self.ids, self.nlogp = z(B, max(T, 1), dtype=i32), z(B)
+        self._keep = [p.detach() for p in transducer.parameters()]
+        prog = []
+        predictor_phases(prog, dec, R, self.dec_h[0], self.dec_c[0], self.dec_htmp, self.dec_x[0], self.tok, blank,
+                         masked=False)                         # prime every row with BOS from the zero state
+        w1 = joint[0].weight
+        for t in range(T):
+            p, q = t & 1, 1 - (t & 1)
+            prog.append(EbPhase(type=PH_LINEAR, S=R, N=J, flags=F_TANH, K1=E, x1=_ptr(self.h_enc, t * E), ldx1=T * E,
+                                x1_div=W, w1=_ptr(w1), ldw1=E + D, K2=D, x2=_ptr(self.dec_x[p]), ldx2=D,
+                                w2=_ptr(w1, E), ldw2=E + D, b1=_ptr(joint[0].bias), y=_ptr(self.hidden), ldy=J))
+            prog.append(EbPhase(type=PH_LINEAR, S=R, N=V, K1=J, x1=_ptr(self.hidden), ldx1=J,
+                                w1=_ptr(joint[2].weight), ldw1=J, b1=_ptr(joint[2].bias), y=_ptr(self.logits), ldy=V))
+            prog.append(EbPhase(type=PH_BEAM_SELECT, S=B, N=V, aux=W, aux2=blank, flags=F_MERGE if merge else 0,
+                                x1=_ptr(self.logits), ldx1=V, y=_ptr(self.logp), tok_in=_ptr(self.frames),
+                                tok_out=_ptr(self.tok), src=_ptr(self.src), hist=_ptr(self.hist), hist_ld=T,
+                                hist_col=t, seq_in=_ptr(self.seqs[p]), seq_out=_ptr(self.seqs[q])))
+            prog.append(EbPhase(type=PH_GATHER, S=R, N=Hd, aux=2 * Ld, x1=_ptr(st[p]), y=_ptr(st[q]), K2=D,
+                                x2=_ptr(self.dec_x[p]), y2=_ptr(self.dec_x[q]), src=_ptr(self.src)))
+            predictor_phases(prog, dec, R, self.dec_h[q], self.dec_c[q], self.dec_htmp, self.dec_x[q], self.tok, blank,
+                             masked=True)
+        prog.append(EbPhase(type=PH_BEAM_FINAL, S=B, aux=W, aux2=blank, y=_ptr(self.logp), hist=_ptr(self.hist),
+                            hist_ld=T, tok_out=_ptr(self.ids), ldy=self.ids.shape[1], y2=_ptr(self.nlogp)))
+        self._st0 = st[0]
+        self.nphase = len(prog)
+        arr = (EbPhase * len(prog))(*prog)
+        self._prog = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(self.dev)
+        self._bar = torch.zeros(64, dtype=torch.int32, device=self.dev)
+
+    @torch.no_grad()
+    def run(self, h_enc, frames):
+        """h_enc [B, T', E], frames int32 [B] on the device (encoder frames each utterance decodes, <= T') ->
+        (ids int32 [B, max(T', 1)]: the best hypothesis' non-blank tokens right-aligned, -1 before them;
+        -log p [B] of that hypothesis)."""
+        self.h_enc.copy_(h_enc)
+        self.frames.copy_(frames)
+        self._st0.zero_()
+        self.seqs[0].zero_()
+        self.logp.fill_(float("-inf"))
+        self.logp.view(self.B, self.W)[:, 0] = 0.0
+        self.tok.fill_(BOS)
+        check(lib().eb_decode_run(self._prog.data_ptr(), self.nphase, self._bar.data_ptr(), self.max_ctas,
+                                  torch.cuda.current_stream().cuda_stream), "eb_decode_run")
+        return self.ids, self.nlogp

@@ -171,18 +171,26 @@ int eb_joint_dpre_reduce(const void* dpre16, float* dep, float* ddp, int B, int 
 /* ---- streaming greedy decode: one persistent kernel per audio chunk -----------------------------
  * replaces PytorchStreamDecoder.decode's Python loop (rnnt/stream.py:93-120).  The host builds a
  * phase program once (edgedict_b200/stream_engine.py) and launches it per chunk; see decode.cu. */
-enum { EB_PH_LN = 0, EB_PH_PAIR = 1, EB_PH_LSTM = 2, EB_PH_LINEAR = 3, EB_PH_ARGMAX = 4, EB_PH_COPY = 5 };
+enum { EB_PH_LN = 0, EB_PH_PAIR = 1, EB_PH_LSTM = 2, EB_PH_LINEAR = 3, EB_PH_ARGMAX = 4, EB_PH_COPY = 5,
+       EB_PH_BEAM_SELECT = 6, EB_PH_GATHER = 7, EB_PH_BEAM_FINAL = 8 };
 typedef struct EbPhase {
-    int32_t type, S, K1, K2, N, flags, ldx1, ldx2, ldw1, ldw2, ldy, aux, aux2, hist_ld, hist_col, pad_;
+    int32_t type, S, K1, K2, N, flags, ldx1, ldx2, ldw1, ldw2, ldy, aux, aux2, hist_ld, hist_col, x1_div;
     const float *x1, *x2, *w1, *w2, *b1, *b2;
     float *y, *y2, *c;
     const int32_t* tok_in;
     int32_t* tok_out;
     int32_t* hist;
+    const int32_t* seq_in;
+    int32_t *seq_out, *src;
 } EbPhase;
 /* flags: 1 = tanh epilogue (LINEAR); 2 = x1 rows are embedding rows indexed by tok_in (LSTM);
  *        4 = masked update: streams whose tok_in equals aux (blank) keep their state (LSTM);
- *        8 = ARGMAX also accumulates log_softmax(x)[argmax] into y[s] (batched greedy decode). */
+ *        8 = ARGMAX also accumulates log_softmax(x)[argmax] into y[s] (batched greedy decode);
+ *       16 = BEAM_SELECT folds hypotheses with equal token sequences (log-add).
+ * x1_div (LINEAR): row r of x1 is x1[r / x1_div] (0 or 1: row r), the encoder frame a beam's W rows share.
+ * Beam search (batched, W slots per utterance, row r = b*W + slot; see decode.cu for the field use of each phase):
+ * at most EB_BEAM_MAX_W slots per utterance. */
+#define EB_BEAM_MAX_W 1024
 int eb_decode_phase_size(void);
 int eb_decode_run(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream);
 
