@@ -8,8 +8,11 @@
 //                                                 first Linear split as W1e*e + W1d*d + b1
 //   column sums (bias gradients), casts, Adam     torch autograd / torch.optim.Adam in
 //                                                 cli/baseline.py:141-156,239-245
+#include <cooperative_groups.h>
 #include "common.cuh"
 #include "../../include/edgedict_b200.h"
+
+namespace cg = cooperative_groups;
 
 namespace {
 
@@ -455,24 +458,32 @@ __global__ void __launch_bounds__(1024) colsum_kernel(const TI* __restrict__ x, 
     if (k == 0 && c < N) out[c] += t;
 }
 
-// bf16 rows with N % 8 == 0: a CTA owns 16 columns (two threads of 8 columns, one 16-byte load per row each) and 512
-// row lanes with four independent row loads in flight
-__global__ void __launch_bounds__(1024) colsum_bf16_vec_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ out,
-                                                               long rows, int N) {
-    __shared__ float sh[512][17];
-    const int half = threadIdx.x & 1, k = threadIdx.x >> 1;
+// bf16 rows with N % 8 == 0: a slab of 16 columns is summed by 512 row lanes (two threads of 8 columns per lane, one
+// 16-byte load per row each, eight row loads in flight); lane k adds rows k, k + 512, k + 1024, ... in order, then a
+// fixed-shape tree adds the 512 lane sums.  The lanes of a slab are spread over a cluster of COLSUM_CL CTAs so that the
+// 4 GB column sum of the joint's d logits (N = 1024: 64 slabs) streams from every SM instead of 64, and so that a CTA
+// needs only 8.7 KB of shared memory: it fits beside a CTA of the joint's d-hidden GEMM (198 KB), under which this sum
+// runs.  The first tree levels add lane sums across the cluster through distributed shared memory, the rest run in the
+// CTA of rank 0.  Same additions in the same order as one CTA of 512 lanes: the same bits.
+constexpr int COLSUM_LANES = 512, COLSUM_CL = 4, COLSUM_CTA_LANES = COLSUM_LANES / COLSUM_CL;   // (the tree below assumes 4)
+__global__ void __cluster_dims__(1, COLSUM_CL, 1) __launch_bounds__(2 * COLSUM_CTA_LANES)
+colsum_bf16_vec_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ out, long rows, int N) {
+    __shared__ float sh[COLSUM_CTA_LANES][17];
+    cg::cluster_group cluster = cg::this_cluster();
+    const unsigned rank = cluster.block_rank();
+    const int half = threadIdx.x & 1, kl = threadIdx.x >> 1, k = (int)rank * COLSUM_CTA_LANES + kl;
     const int c0 = blockIdx.x * 16 + half * 8;
     float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     if (c0 < N) {
         const __nv_bfloat16* p = x + (long)k * N + c0;
-        const long step = 512L * N;
+        const long step = (long)COLSUM_LANES * N;
         long r = k;
-        for (; r + 3 * 512 < rows; r += 4 * 512) {
-            uint4 v[4];
+        for (; r + 7 * COLSUM_LANES < rows; r += 8 * COLSUM_LANES) {
+            uint4 v[8];
 #pragma unroll
-            for (int q = 0; q < 4; ++q) v[q] = *reinterpret_cast<const uint4*>(p + q * step);
+            for (int q = 0; q < 8; ++q) v[q] = *reinterpret_cast<const uint4*>(p + q * step);
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
+            for (int q = 0; q < 8; ++q) {
                 const uint32_t w[4] = {v[q].x, v[q].y, v[q].z, v[q].w};
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
@@ -481,9 +492,9 @@ __global__ void __launch_bounds__(1024) colsum_bf16_vec_kernel(const __nv_bfloat
                     acc[2 * i + 1] += f.y;
                 }
             }
-            p += 4 * step;
+            p += 8 * step;
         }
-        for (; r < rows; r += 512, p += step) {
+        for (; r < rows; r += COLSUM_LANES, p += step) {
             const uint4 v = *reinterpret_cast<const uint4*>(p);
             const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
@@ -494,12 +505,28 @@ __global__ void __launch_bounds__(1024) colsum_bf16_vec_kernel(const __nv_bfloat
             }
         }
     }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) sh[kl][half * 8 + i] = acc[i];
+    // the tree of colsum_tree<512, 16> (at stride st, lane k < st adds lane k + st), its first two levels across the
+    // cluster: stride 256 adds rank r + 2 to rank r, stride 128 adds rank 1 to rank 0
+    cluster.sync();
+    if (rank < 2) {
+        const float* peer = cluster.map_shared_rank(&sh[0][0], rank + 2);
+        for (int e = threadIdx.x; e < COLSUM_CTA_LANES * 16; e += blockDim.x) sh[e >> 4][e & 15] += peer[(e >> 4) * 17 + (e & 15)];
+    }
+    cluster.sync();
+    if (rank == 0) {
+        const float* peer = cluster.map_shared_rank(&sh[0][0], 1);
+        for (int e = threadIdx.x; e < COLSUM_CTA_LANES * 16; e += blockDim.x) sh[e >> 4][e & 15] += peer[(e >> 4) * 17 + (e & 15)];
+    }
+    cluster.sync();                                          // (a CTA's shared memory stays valid until its peers have read it)
+    if (rank != 0) return;
 #pragma unroll 1
-    for (int i = 0; i < 8; ++i) {
-        const float t = colsum_tree<512, 16>(sh, acc[i], k, half * 8 + i);
-        if (k == 0 && c0 < N) out[c0 + i] += t;
+    for (int st = COLSUM_CTA_LANES / 2; st > 0; st >>= 1) {
+        for (int e = threadIdx.x; e < st * 16; e += blockDim.x) sh[e >> 4][e & 15] += sh[(e >> 4) + st][e & 15];
         __syncthreads();
     }
+    if (threadIdx.x < 16 && blockIdx.x * 16 + (int)threadIdx.x < N) out[blockIdx.x * 16 + threadIdx.x] += sh[0][threadIdx.x];
 }
 
 __global__ void cast_bf16_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, long n) {
@@ -737,7 +764,7 @@ EB_API int eb_joint_dpre_reduce(const void* dpre16, float* dep, float* ddp, int 
 EB_API int eb_colsum(const void* x, int x_bf16, float* out, long rows, int N, void* stream) {
     if (!x || !out || rows <= 0 || N <= 0) return EB_ERR_INVALID;
     if (x_bf16 && N % 8 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0)
-        colsum_bf16_vec_kernel<<<(N + 15) / 16, 1024, 0, ST(stream)>>>((const __nv_bfloat16*)x, out, rows, N);
+        colsum_bf16_vec_kernel<<<dim3((N + 15) / 16, COLSUM_CL), 2 * COLSUM_CTA_LANES, 0, ST(stream)>>>((const __nv_bfloat16*)x, out, rows, N);
     else if (x_bf16)
         colsum_kernel<__nv_bfloat16><<<(N + 31) / 32, 1024, 0, ST(stream)>>>((const __nv_bfloat16*)x, out, rows, N);
     else

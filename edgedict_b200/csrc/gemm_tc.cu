@@ -278,6 +278,27 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
             for (int h = 0; h < 2; ++h) {
                 const long row = m0 + r_in + 8 * h;
                 if (row >= M) continue;
+                // tanh' epilogue (eb_gemm_bf16_dtanh, always on the 128-wide tile): the row's aux operands are all loaded
+                // before its first store.  The compiler cannot move a load of aux above a store to C (they may alias), so
+                // loads placed between the stores waited one HBM round trip per 8 columns.  The other tiles have no
+                // registers to spare for this and keep the loads in place.
+                constexpr bool PRE = BN == 128 && !LOW_;
+                __nv_bfloat162 hx[PRE ? BN / 8 : 1];
+                if constexpr (PRE) {
+                    if (c_bf16 && lse.aux) {
+#pragma unroll
+                        for (int i = 0; i < BN / 8; ++i) {
+                            const int col = n0 + 8 * i + cq;
+                            const long off = row * N + col;
+                            hx[i] = __floats2bfloat162_rn(0.f, 0.f);
+                            if (col + 1 < N && vec2) hx[i] = __ldg(reinterpret_cast<const __nv_bfloat162*>(lse.aux + off));
+                            else if (col < N) {
+                                hx[i].x = lse.aux[off];
+                                if (col + 1 < N) hx[i].y = lse.aux[off + 1];
+                            }
+                        }
+                    }
+                }
 #pragma unroll
                 for (int i = 0; i < BN / 8; ++i) {
                     const int col = n0 + 8 * i + cq;
@@ -290,7 +311,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                         __nv_bfloat16* cp = Ch + off;
                         if (lse.aux) {
                             float h0, h1 = 0.f;
-                            if (pair) {
+                            if constexpr (PRE) {
+                                const float2 hh = __bfloat1622float2(hx[i]);
+                                h0 = hh.x;
+                                if (two) h1 = hh.y;
+                            } else if (pair) {
                                 const float2 hh = __bfloat1622float2(__ldg(reinterpret_cast<const __nv_bfloat162*>(lse.aux + off)));
                                 h0 = hh.x; h1 = hh.y;
                             } else {
@@ -397,8 +422,8 @@ void plan(int a_mn_major, int c_bf16, int accumulate, long M, int N, long K, int
     // (split-K weight gradients take their parallelism from K: the wide tile only has to exist a few times -- it
     //  moves 48 KB of operands per 128x256x64 block where two narrow tiles move 64 KB)
     wide = (N % 256 == 0) && (wide_tiles >= eb_num_sms() || (!c_bf16 && (K + BK - 1) / BK >= 64 && wide_tiles >= 8));
-    // N = 256 k + 128 with many row blocks (the joint's d-hidden GEMM, N = 640): wide tiles with a half-empty last
-    // column tile move 20 % fewer operand bytes than 128-wide tiles for 20 % more (idle anyway) MMA issue
+    // N = 256 k + 128 with many row blocks: wide tiles with a half-empty last column tile move 20 % fewer operand bytes
+    // than 128-wide tiles for 20 % more (idle anyway) MMA issue
     if (!wide && N % 256 == 128 && N >= 512 && (M + BM - 1) / BM >= 4L * eb_num_sms() && accumulate == 0) wide = true;
     if (force_bn == 128) wide = false;
     if (force_bn == 256 && N % 128 == 0) wide = true;
@@ -499,6 +524,10 @@ static int gemm_dispatch(const void* A, int a_mn_major, const void* B, int b_mn_
     bool wide;
     int ksplit;
     plan(a_mn_major, c_bf16, accumulate, M, N, K, flags, wide, ksplit);
+    // the tanh' epilogue (eb_gemm_bf16_dtanh: the joint's d-hidden GEMM, N = 640) runs on 128-wide tiles, which have the
+    // registers to load a row's aux operands ahead of its stores (the 128 x 256 tile's epilogue waits for each load in
+    // turn); bf16 output never splits K, so this only changes the tile width
+    if (aux) wide = false;
     // split-K needs its workspace: with less (or none) the split count shrinks to what fits, down to no split
     if (ksplit > 1) {
         const long fit = (partials && (reinterpret_cast<uintptr_t>(partials) & 7) == 0) ? partial_floats / (M * (long)N) : 0;
