@@ -28,6 +28,13 @@ SIGNATURES = {
     "eb_lstm_scratch_bytes": (Z, [I, I]),
     "eb_lstm_seq_fwd": (I, [P, P, P, P, P, P, P, P, P, P, I, I, I, P]),
     "eb_lstm_seq_bwd": (I, [P, P, P, P, P, P, P, P, P, P, P, I, I, I, P]),
+    "eb_gru_scratch_bytes": (Z, [I, I]),
+    "eb_gru_seq_fwd": (I, [P, P, P, P, P, P, P, P, I, I, I, P]),
+    "eb_gru_seq_bwd": (I, [P, P, P, P, P, P, P, P, P, P, I, I, I, P]),
+    "eb_gru_tc_supported": (I, [I, I]),
+    "eb_gru_tc_scratch_bytes": (Z, [I, I]),
+    "eb_gru_tc_fwd": (I, [P, P, P, P, P, P, P, P, I, I, I, P]),
+    "eb_gru_tc_bwd": (I, [P, P, P, P, P, P, P, P, P, P, I, I, I, P]),
     "eb_lstm_tc_supported": (I, [I, I]),
     "eb_lstm_tc_scratch_bytes": (Z, [I, I]),
     "eb_lstm_tc_max_clusters": (I, [I, I]),

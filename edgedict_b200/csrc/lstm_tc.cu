@@ -635,6 +635,287 @@ int pick_cs(int H) {
     return c;
 }
 
+// ---- GRU layer on tensor cores (nn.GRU, gate order r|z|n; bf16 operands, fp32 accumulation and state) -------------
+// Forward: CTA k owns the 16 hidden units [16k, 16k+16) as three m16 tiles of W_hh rows -- (r|z of units 0-7),
+// (r|z of units 8-15), (n of units 0-15) -- held in registers as A fragments (each warp a K-range of H/8 columns:
+// 3 x 8 x 4 = 96 registers at H = 1024); h_{t-1} is exchanged in bf16 as in lstm_tc_fwd_kernel, the fp32 state stays in
+// registers of the thread that owns the (unit, batch row) pair, and b_hn is added to the n-row sum inside the reset
+// product.  Saves r | z | n | gh_n (fp32, [B,T,4H]) as the fp32 kernel does.
+// BPTT: CTA k owns the same 16 units, now as the output rows of dh_rec = W_hh^T dgh; the contraction runs over all 3H
+// rows of dgh (each warp a K-range of 3H/8 rows: 24 k-steps x 4 = 96 registers at H = 1024).  dgh_t is exchanged in
+// bf16 ([NB][3H], gate-major), the direct term dh z is carried in fp32 registers.
+constexpr int GU = 16;           // hidden units per CTA
+constexpr int GRS = 33;          // padded lane stride of the cross-warp reduction buffer
+
+// the caller has pulled this warp's K-range into `tile`; the warp's partial products -> red[w][slot][lane],
+// slot = (mt * 4 + nt) * 4 + i
+template <int MT, int KSM>
+__device__ __forceinline__ void gru_contract(const uint32_t (&afr)[MT][KSM][4], const __nv_bfloat16* tile, int ld,
+                                             int ks0, int myks, float* red) {
+    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+    float acc[MT][4][4];
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) acc[mt][nt][i] = 0.f;
+#pragma unroll
+    for (int ks = 0; ks < KSM; ++ks) {
+        if (ks < myks) {
+            uint32_t b01[4], b23[4];
+            load_b<4>(b01, b23, tile, ld, ks0 + ks);
+#pragma unroll
+            for (int mt = 0; mt < MT; ++mt) {
+                mma_bf16(acc[mt][0], afr[mt][ks], b01[0], b01[1]);
+                mma_bf16(acc[mt][1], afr[mt][ks], b01[2], b01[3]);
+                mma_bf16(acc[mt][2], afr[mt][ks], b23[0], b23[1]);
+                mma_bf16(acc[mt][3], afr[mt][ks], b23[2], b23[3]);
+            }
+        }
+    }
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) red[(w * MT * 16 + (mt * 4 + nt) * 4 + i) * GRS + l] = acc[mt][nt][i];
+}
+
+// sum over the 8 warps of the accumulator element at (tile mt, tile row `row` 0-15, batch column b)
+__device__ __forceinline__ float gru_red_sum(const float* red, int MT, int mt, int row, int b) {
+    const int lane = (row & 7) * 4 + ((b & 7) >> 1);
+    const int slot = (mt * 4 + (b >> 3)) * 4 + (row >> 3) * 2 + (b & 1);
+    float s = 0.f;
+#pragma unroll
+    for (int sw = 0; sw < NW; ++sw) s += red[(sw * MT * 16 + slot) * GRS + lane];
+    return s;
+}
+
+struct GruFwdP {
+    const float* xg;              // [B,T,3H] fp32 (b_hr, b_hz folded in)
+    const __nv_bfloat16* whh;     // [3H,H] bf16
+    const float* bhn; const float* h0;
+    float* y; float* hT; float* save;
+    __nv_bfloat16* hx;            // [2][NB][H] exchange
+    unsigned* bar;
+    int B, T, H;
+};
+
+__global__ void __launch_bounds__(NW * 32, 1) gru_tc_fwd_kernel(GruFwdP p) {
+    extern __shared__ __align__(16) unsigned char smraw[];
+    const int H = p.H, B = p.B, T = p.T;
+    const long H3 = 3 * (long)H;
+    const int HP = H + PAD;
+    __nv_bfloat16* hs = reinterpret_cast<__nv_bfloat16*>(smraw);                 // [NB][HP]
+    float* red = reinterpret_cast<float*>(smraw + (size_t)NB * HP * 2);          // [NW][48][GRS]
+    __nv_bfloat16* sh_h = reinterpret_cast<__nv_bfloat16*>(red + NW * 48 * GRS);  // [NB][GU]
+    const int tid = threadIdx.x, w = tid >> 5, l = tid & 31;
+    const int j0 = blockIdx.x * GU;
+    const unsigned ncta = gridDim.x;
+    const int nks = H / 16;
+    const int ksper = (nks + NW - 1) / NW;                   // <= 8
+    const int ks0 = w * ksper;
+    const int myks = max(0, min(ksper, nks - ks0));
+    const size_t xstride = (size_t)NB * H;
+
+    // A fragments: tile mt rows lo (fragment row l/4) and hi (l/4 + 8) as W_hh rows
+    uint32_t afr[3][8][4];
+#pragma unroll
+    for (int mt = 0; mt < 3; ++mt)
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks) {
+            const int k = (ks0 + ks) * 16 + (l & 3) * 2;
+            const int u = l >> 2;
+            const long rlo = mt == 2 ? 2 * (long)H + j0 + u : (long)j0 + mt * 8 + u;
+            const long rhi = mt == 2 ? 2 * (long)H + j0 + 8 + u : (long)H + j0 + mt * 8 + u;
+            const bool ok = ks < myks;
+            afr[mt][ks][0] = ok ? ldg_u32(p.whh + rlo * H + k) : 0u;
+            afr[mt][ks][1] = ok ? ldg_u32(p.whh + rhi * H + k) : 0u;
+            afr[mt][ks][2] = ok ? ldg_u32(p.whh + rlo * H + k + 8) : 0u;
+            afr[mt][ks][3] = ok ? ldg_u32(p.whh + rhi * H + k + 8) : 0u;
+        }
+
+    // the two (unit, batch row) pairs this thread finalises every step: (w, l) and (w + 8, l)
+    const int bb = l;
+    const bool own = bb < B;
+    float h_state[2], bn[2];
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+        const int j = j0 + w + 8 * q;
+        h_state[q] = (own && p.h0) ? p.h0[(long)bb * H + j] : 0.f;
+        bn[q] = p.bhn ? p.bhn[j] : 0.f;
+        if (own) p.hx[xstride + (long)bb * H + j] = __float2bfloat16(h_state[q]);
+    }
+    __syncthreads();
+    if (tid == 0) { __threadfence(); atomicAdd(p.bar, 1u); }
+    unsigned epoch = 1;
+
+    for (int t = 0; t < T; ++t) {
+        const __nv_bfloat16* hprev = p.hx + ((t + 1) & 1) * xstride;
+        __nv_bfloat16* hnext = p.hx + (t & 1) * xstride;
+        float px[2][3];                                      // input pre-activations, loaded before the wait
+#pragma unroll
+        for (int q = 0; q < 2; ++q)
+#pragma unroll
+            for (int g = 0; g < 3; ++g)
+                px[q][g] = own ? __ldg(p.xg + ((long)bb * T + t) * H3 + (long)g * H + j0 + w + 8 * q) : 0.f;
+        if (tid == 0) spin_wait_ge(p.bar, epoch * ncta);
+        __syncthreads();
+        warp_pull(hs + ks0 * 16, HP, hprev + ks0 * 16, H, myks * 2, NB);
+        gru_contract<3, 8>(afr, hs, HP, ks0, myks, red);
+        __syncthreads();
+        float rg[2], zg[2], ng[2], ghn[2];
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+            const int u = w + 8 * q;                         // tile rows: r, z in tile u/8, n in tile 2
+            rg[q] = fast_sigmoid(gru_red_sum(red, 3, q, w, bb) + px[q][0]);
+            zg[q] = fast_sigmoid(gru_red_sum(red, 3, q, 8 + w, bb) + px[q][1]);
+            ghn[q] = gru_red_sum(red, 3, 2, u, bb) + bn[q];
+            ng[q] = fast_tanh(px[q][2] + rg[q] * ghn[q]);
+            h_state[q] = (1.f - zg[q]) * ng[q] + zg[q] * h_state[q];
+            sh_h[bb * GU + u] = __float2bfloat16(own ? h_state[q] : 0.f);
+        }
+        __syncthreads();
+        if (w == 0) {   // publish h_t: two 16-byte stores per batch row, then a single fence + arrive
+            const uint4* src = reinterpret_cast<const uint4*>(sh_h + l * GU);
+            uint4* dst = reinterpret_cast<uint4*>(hnext + (size_t)l * H + j0);
+            dst[0] = src[0];
+            dst[1] = src[1];
+            __syncwarp();
+            if (l == 0) { __threadfence(); atomicAdd(p.bar, 1u); }
+        }
+        ++epoch;
+        if (own) {
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+                const int j = j0 + w + 8 * q;
+                const long row = (long)bb * T + t;
+                p.y[row * H + j] = h_state[q];
+                if (p.save) {
+                    float* sp = p.save + row * 4 * H + j;
+                    sp[0] = rg[q]; sp[H] = zg[q]; sp[2 * (long)H] = ng[q]; sp[3 * (long)H] = ghn[q];
+                }
+                if (t == T - 1) p.hT[(long)bb * H + j] = h_state[q];
+            }
+        }
+    }
+}
+
+struct GruBwdP {
+    const float* dy; const float* save; const float* y; const float* h0;
+    const __nv_bfloat16* whhT;    // [H,3H] bf16 = W_hh^T
+    const float* dhT;
+    __nv_bfloat16* dgi16; __nv_bfloat16* dgh16;   // [B,T,3H] bf16 out
+    float* dh0;
+    __nv_bfloat16* gx;            // [2][NB][3H] exchange
+    unsigned* bar;
+    int B, T, H;
+};
+
+__global__ void __launch_bounds__(NW * 32, 1) gru_tc_bwd_kernel(GruBwdP p) {
+    constexpr int KSM = 24;                                  // k-steps per warp at H = 1024: 3H / 16 / NW
+    extern __shared__ __align__(16) unsigned char smraw[];
+    const int H = p.H, B = p.B, T = p.T;
+    const int H3 = 3 * H;
+    const int KP = H3 + PAD;
+    __nv_bfloat16* gs = reinterpret_cast<__nv_bfloat16*>(smraw);                 // [NB][KP]
+    float* red = reinterpret_cast<float*>(smraw + (size_t)NB * KP * 2);          // [NW][16][GRS]
+    __nv_bfloat16* sg = reinterpret_cast<__nv_bfloat16*>(red + NW * 16 * GRS);    // [NB][3][GU]
+    const int tid = threadIdx.x, w = tid >> 5, l = tid & 31;
+    const int j0 = blockIdx.x * GU;
+    const unsigned ncta = gridDim.x;
+    const int nks = H3 / 16;
+    const int ksper = (nks + NW - 1) / NW;                   // <= KSM
+    const int ks0 = w * ksper;
+    const int myks = max(0, min(ksper, nks - ks0));
+    const size_t xstride = (size_t)NB * H3;
+
+    // A(m = unit u, k = gate row r) = W_hh[r, j0 + u] = whhT[j0 + u][r]: consecutive k are contiguous in whhT
+    uint32_t afr[1][KSM][4];
+#pragma unroll
+    for (int ks = 0; ks < KSM; ++ks) {
+        const int k = (ks0 + ks) * 16 + (l & 3) * 2;
+        const long ulo = j0 + (l >> 2), uhi = ulo + 8;
+        const bool ok = ks < myks;
+        afr[0][ks][0] = ok ? ldg_u32(p.whhT + ulo * H3 + k) : 0u;
+        afr[0][ks][1] = ok ? ldg_u32(p.whhT + uhi * H3 + k) : 0u;
+        afr[0][ks][2] = ok ? ldg_u32(p.whhT + ulo * H3 + k + 8) : 0u;
+        afr[0][ks][3] = ok ? ldg_u32(p.whhT + uhi * H3 + k + 8) : 0u;
+    }
+
+    const int bb = l;
+    const bool own = bb < B;
+    float dh_rec[2];                                         // dh_{t} minus dy_t: dh_{t+1} z_{t+1} + W_hh^T dgh_{t+1}
+#pragma unroll
+    for (int q = 0; q < 2; ++q) dh_rec[q] = (own && p.dhT) ? p.dhT[(long)bb * H + j0 + w + 8 * q] : 0.f;
+    unsigned epoch = 0;
+
+    for (int t = T - 1; t >= 0; --t) {
+        __nv_bfloat16* gcur = p.gx + (t & 1) * xstride;
+        float carry[2];
+        // phase A: gate gradients of step t for the owned pairs
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+            const int u = w + 8 * q, j = j0 + u;
+            float dr = 0.f, dz = 0.f, dn = 0.f, dhn = 0.f;
+            carry[q] = 0.f;
+            if (own) {
+                const long row = (long)bb * T + t;
+                const float* sp = p.save + row * 4 * H + j;
+                const float rg = sp[0], zg = sp[H], ng = sp[2 * (long)H], ghn = sp[3 * (long)H];
+                const float hp = (t > 0) ? p.y[(row - 1) * H + j] : (p.h0 ? p.h0[(long)bb * H + j] : 0.f);
+                const float dh = p.dy[row * H + j] + dh_rec[q];
+                dn = dh * (1.f - zg) * (1.f - ng * ng);
+                dz = dh * (hp - ng) * zg * (1.f - zg);
+                dr = dn * ghn * rg * (1.f - rg);
+                dhn = rg * dn;
+                carry[q] = dh * zg;
+                __nv_bfloat16* gi = p.dgi16 + row * H3 + j;
+                __nv_bfloat16* gh = p.dgh16 + row * H3 + j;
+                gi[0] = gh[0] = __float2bfloat16(dr);
+                gi[H] = gh[H] = __float2bfloat16(dz);
+                gi[2 * (long)H] = __float2bfloat16(dn);
+                gh[2 * (long)H] = __float2bfloat16(dhn);
+            }
+            sg[(bb * 3 + 0) * GU + u] = __float2bfloat16(dr);
+            sg[(bb * 3 + 1) * GU + u] = __float2bfloat16(dz);
+            sg[(bb * 3 + 2) * GU + u] = __float2bfloat16(dhn);
+        }
+        __syncthreads();
+        if (tid < NB * 3 * 2) {   // publish dgh_t: rows b, gates g, two 16-byte halves of the 16 units
+            const int b = tid / 6, g = (tid >> 1) % 3, half = tid & 1;
+            *reinterpret_cast<uint4*>(gcur + (size_t)b * H3 + (size_t)g * H + j0 + half * 8) =
+                *reinterpret_cast<const uint4*>(sg + (b * 3 + g) * GU + half * 8);
+        }
+        __syncthreads();
+        ++epoch;
+        if (tid == 0) {
+            __threadfence();
+            atomicAdd(p.bar, 1u);
+            spin_wait_ge(p.bar, epoch * ncta);
+        }
+        __syncthreads();
+        // phase B: dh_rec = dh z + W_hh^T dgh_t for the owned pairs
+        warp_pull(gs + ks0 * 16, KP, gcur + ks0 * 16, H3, myks * 2, NB);
+        gru_contract<1, KSM>(afr, gs, KP, ks0, myks, red);
+        __syncthreads();
+#pragma unroll
+        for (int q = 0; q < 2; ++q) dh_rec[q] = carry[q] + gru_red_sum(red, 1, 0, w + 8 * q, bb);
+    }
+    if (own) {
+#pragma unroll
+        for (int q = 0; q < 2; ++q) p.dh0[(long)bb * H + j0 + w + 8 * q] = dh_rec[q];
+    }
+}
+
+inline size_t gru_tc_fwd_smem(int H) {
+    return (size_t)NB * (H + PAD) * 2 + sizeof(float) * NW * 48 * GRS + NB * GU * 2;
+}
+inline size_t gru_tc_bwd_smem(int H) {
+    return (size_t)NB * (3 * H + PAD) * 2 + sizeof(float) * NW * 16 * GRS + NB * 3 * GU * 2;
+}
+
 }  // namespace
 
 // debug: clock64 stamps of CTA 0 of the BPTT kernel for the first `steps` steps of subsequent launches ([steps][16] int64)
@@ -764,6 +1045,76 @@ static int tc_bwd_impl(const float* dy, const float* gates, const float* cseq, c
             void* args[] = {&p};
             EB_CUDA(cudaLaunchCooperativeKernel((void*)kern, dim3(H / 8), dim3(NW * 32), args, smem, st));
         }
+    }
+    return EB_OK;
+}
+
+// ---- GRU entry points (bf16 mode; H % 64 == 0, H <= 1024) -------------------------------------------------------------
+static inline bool gru_tc_ok(int B, int H) { return H > 0 && tc_ok(B, H); }
+
+EB_API int eb_gru_tc_supported(int B, int H) { return gru_tc_ok(B, H) ? 1 : 0; }
+
+EB_API size_t eb_gru_tc_scratch_bytes(int B, int H) {
+    if (!gru_tc_ok(B, H)) return 0;
+    return TC_HDR + sizeof(__nv_bfloat16) * (size_t)2 * NB * 3 * H;
+}
+
+// xg [B,T,3H] fp32 (b_hr, b_hz folded in); whh16 [3H,H] bf16; bhn [H] fp32 (NULL: zero).  B > 32: batch tiles of 32.
+EB_API int eb_gru_tc_fwd(const float* xg, const void* whh16, const float* bhn, const float* h0, float* y, float* hT,
+                         float* save, void* scratch, int B, int T, int H, void* stream) {
+    if (!xg || !whh16 || !y || !hT || !scratch || T <= 0 || !gru_tc_ok(B, H)) return EB_ERR_INVALID;
+    if ((reinterpret_cast<uintptr_t>(whh16) & 3) || (reinterpret_cast<uintptr_t>(scratch) & 15)) return EB_ERR_INVALID;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const size_t smem = gru_tc_fwd_smem(H);
+    EB_CUDA(cudaFuncSetAttribute(gru_tc_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    for (int b0 = 0; b0 < B; b0 += NB) {
+        const int nb = (B - b0 < NB) ? (B - b0) : NB;
+        GruFwdP p;
+        p.xg = xg + (size_t)b0 * T * 3 * H;
+        p.whh = reinterpret_cast<const __nv_bfloat16*>(whh16);
+        p.bhn = bhn;
+        p.h0 = h0 ? h0 + (size_t)b0 * H : nullptr;
+        p.y = y + (size_t)b0 * T * H;
+        p.hT = hT + (size_t)b0 * H;
+        p.save = save ? save + (size_t)b0 * T * 4 * H : nullptr;
+        p.bar = reinterpret_cast<unsigned*>(scratch);
+        p.hx = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<char*>(scratch) + TC_HDR);
+        p.B = nb; p.T = T; p.H = H;
+        EB_CUDA(cudaMemsetAsync(scratch, 0, TC_HDR + sizeof(__nv_bfloat16) * (size_t)2 * NB * H, st));
+        void* args[] = {&p};
+        EB_CUDA(cudaLaunchCooperativeKernel((void*)gru_tc_fwd_kernel, dim3(H / GU), dim3(NW * 32), args, smem, st));
+    }
+    return EB_OK;
+}
+
+// whhT16 [H,3H] bf16 (W_hh transposed); dgi16 / dgh16 [B,T,3H] bf16 out; dh0 [B,H] fp32 out.
+EB_API int eb_gru_tc_bwd(const float* dy, const float* save, const float* y, const float* h0, const void* whhT16,
+                         const float* dhT, void* dgi16, void* dgh16, float* dh0, void* scratch, int B, int T, int H,
+                         void* stream) {
+    if (!dy || !save || !y || !whhT16 || !dgi16 || !dgh16 || !dh0 || !scratch || T <= 0 || !gru_tc_ok(B, H))
+        return EB_ERR_INVALID;
+    if ((reinterpret_cast<uintptr_t>(whhT16) & 3) || (reinterpret_cast<uintptr_t>(scratch) & 15)) return EB_ERR_INVALID;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const size_t smem = gru_tc_bwd_smem(H);
+    EB_CUDA(cudaFuncSetAttribute(gru_tc_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    for (int b0 = 0; b0 < B; b0 += NB) {
+        const int nb = (B - b0 < NB) ? (B - b0) : NB;
+        GruBwdP p;
+        p.dy = dy + (size_t)b0 * T * H;
+        p.save = save + (size_t)b0 * T * 4 * H;
+        p.y = y + (size_t)b0 * T * H;
+        p.h0 = h0 ? h0 + (size_t)b0 * H : nullptr;
+        p.whhT = reinterpret_cast<const __nv_bfloat16*>(whhT16);
+        p.dhT = dhT ? dhT + (size_t)b0 * H : nullptr;
+        p.dgi16 = reinterpret_cast<__nv_bfloat16*>(dgi16) + (size_t)b0 * T * 3 * H;
+        p.dgh16 = reinterpret_cast<__nv_bfloat16*>(dgh16) + (size_t)b0 * T * 3 * H;
+        p.dh0 = dh0 + (size_t)b0 * H;
+        p.bar = reinterpret_cast<unsigned*>(scratch);
+        p.gx = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<char*>(scratch) + TC_HDR);
+        p.B = nb; p.T = T; p.H = H;
+        EB_CUDA(cudaMemsetAsync(scratch, 0, TC_HDR + sizeof(__nv_bfloat16) * (size_t)2 * NB * 3 * H, st));
+        void* args[] = {&p};
+        EB_CUDA(cudaLaunchCooperativeKernel((void*)gru_tc_bwd_kernel, dim3(H / GU), dim3(NW * 32), args, smem, st));
     }
     return EB_OK;
 }

@@ -190,6 +190,67 @@ class LSTMLayer(torch.autograd.Function):
                 dw_ih, dw_hh, db, db.clone(), None)
 
 
+class GRULayer(torch.autograd.Function):
+    """One unidirectional batch_first nn.GRU layer (rnnt/models.py:77-116, gate order r|z|n): bulk input GEMM with
+    b_hr and b_hz folded into its bias (b_hn stays inside the reset product and is added by the recurrent kernel) +
+    persistent recurrent kernel; backward = BPTT kernel + three bulk GEMMs (dx, dW_ih from the input-side gate gradient
+    [dr, dz, dn], dW_hh from the recurrent-side one [dr, dz, r dn]) and their column sums for the biases.  fp32 mode runs
+    the fp32 recurrence (eb_gru_seq_fwd/bwd); bf16 mode runs the tensor-core recurrence (eb_gru_tc_fwd/bwd) where it is
+    supported (H % 64 == 0, H <= 1024) and the fp32 one otherwise, and the three bulk GEMMs on tensor cores."""
+
+    @staticmethod
+    def forward(ctx, x, h0, w_ih, w_hh, b_ih, b_hh, precision):
+        B, T, I = x.shape
+        H = w_hh.shape[1]
+        x2 = _c(x).view(B * T, I)
+        x16 = ops.cast_bf16(x2) if precision == "bf16" else None
+        bias = torch.cat([b_ih[:2 * H] + b_hh[:2 * H], b_ih[2 * H:]])
+        xg = ops.mm_nt(x2, w_ih, bias, precision, x16=x16).view(B, T, 3 * H)
+        h0c = _c(h0) if h0 is not None else None
+        bhn = _c(b_hh[2 * H:])
+        need = any(ctx.needs_input_grad)     # (grad mode is off inside Function.forward)
+        tc = precision == "bf16" and ops.gru_tc_supported(B, H)
+        if tc:
+            y, hT, save = ops.gru_tc_fwd(xg, ops.cast_bf16(_c(w_hh)), bhn, h0c, need)
+        else:
+            y, hT, save = ops.gru_seq_fwd(xg, _c(w_hh), bhn, h0c, need)
+        if need:
+            ctx.save_for_backward(x2 if x16 is None else x16, h0c, w_ih, w_hh, y, save)
+            ctx.precision, ctx.dims, ctx.tc = precision, (B, T, I, H), tc
+        return y, hT
+
+    @staticmethod
+    def backward(ctx, dy, dhT):
+        xs, h0, w_ih, w_hh, y, save = ctx.saved_tensors
+        B, T, I, H = ctx.dims
+        p = ctx.precision
+        if getattr(ctx, "consumed", False):
+            raise RuntimeError("GRULayer.backward ran twice on the same graph (retain_graph is not supported by this "
+                               "node)")
+        ctx.consumed = True
+        dy = _c(dy) if dy is not None else torch.zeros(B, T, H, dtype=f32, device=y.device)
+        dhT = _c(dhT) if dhT is not None else None
+        if ctx.tc:
+            dgi, dgh, dh0 = ops.gru_tc_bwd(dy, save, y, h0, ops.transpose_to_bf16(_c(w_hh)), dhT)
+        else:
+            dgi, dgh, dh0 = ops.gru_seq_bwd(dy, save, y, h0, _c(w_hh), dhT)
+        dgi2, dgh2 = dgi.view(B * T, 3 * H), dgh.view(B * T, 3 * H)
+        dgi16 = (dgi2 if ctx.tc else ops.cast_bf16(dgi2)) if p == "bf16" else None
+        dgh16 = (dgh2 if ctx.tc else ops.cast_bf16(dgh2)) if p == "bf16" else None
+        # h_{t-1} for every step: y shifted right by one frame, h0 (or zeros) in front
+        hprev = torch.empty_like(y)
+        hprev[:, 1:] = y[:, :-1]
+        if h0 is not None:
+            hprev[:, 0] = h0
+        else:
+            hprev[:, 0].zero_()
+        hp2 = hprev.view(B * T, H)
+        dx = ops.mm_nn(dgi2, w_ih, p, dy16=dgi16).view(B, T, I) if ctx.needs_input_grad[0] else None
+        dw_ih = ops.mm_tn(dgi2, xs, p, dy16=dgi16, x16=xs if p == "bf16" else None)
+        dw_hh = ops.mm_tn(dgh2, hp2, p, dy16=dgh16)
+        return (dx, dh0 if ctx.needs_input_grad[1] else None, dw_ih, dw_hh, ops.colsum(dgi2), ops.colsum(dgh2), None)
+
+
 # ---- layer-wavefront schedule of the LSTM stack ------------------------------------------------------------
 # The recurrence of one layer is a chain of T grid-synchronous steps that is bound by exchange/barrier LATENCY
 # (DESIGN.md section 4a): one layer's persistent kernel leaves its SMs idle most of the time.  Layer l+1 at frame t

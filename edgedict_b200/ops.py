@@ -293,6 +293,86 @@ def lstm_seq_bwd(dy, gates, cseq, c0, whh, dhT, dcT):
     return gates, dh0, dc0
 
 
+# ---- GRU recurrent part --------------------------------------------------------------------------
+def _gru_scratch(B, H, device):
+    key = ("gru", B, H, device, _s())
+    t = _scratch.get(key)
+    if t is None:
+        n = lib().eb_gru_scratch_bytes(B, H)
+        if n == 0:
+            raise ValueError("GRU hidden size %d not supported by the persistent kernel" % H)
+        t = torch.zeros(n, dtype=torch.uint8, device=device)
+        _scratch[key] = t
+    return t
+
+
+def gru_seq_fwd(xg, whh, bhn, h0, save):
+    """xg [B,T,3H] (b_hr, b_hz folded in), whh [3H,H], bhn [H] -> (y, hT, save [B,T,4H] = r|z|n|gh_n or None)."""
+    B, T, H3 = xg.shape
+    H = H3 // 3
+    dev = xg.device
+    y = torch.empty(B, T, H, dtype=f32, device=dev)
+    hT = torch.empty(B, H, dtype=f32, device=dev)
+    sv = torch.empty(B, T, 4 * H, dtype=f32, device=dev) if save else None
+    with _timed("gru_seq_fwd", 1, 0.0, 2.0 * B * T * 3 * H * H):
+        check(lib().eb_gru_seq_fwd(_p(xg), _p(whh), _p(bhn), _p(h0), _p(y), _p(hT), _p(sv),
+                                   _p(_gru_scratch(B, H, dev)), B, T, H, _s()), "eb_gru_seq_fwd")
+    return y, hT, sv
+
+
+def gru_seq_bwd(dy, save, y, h0, whh, dhT):
+    """Returns (dgi, dgh [B,T,3H], dh0 [B,H])."""
+    B, T, H = dy.shape
+    dev = dy.device
+    dgi = torch.empty(B, T, 3 * H, dtype=f32, device=dev)
+    dgh = torch.empty(B, T, 3 * H, dtype=f32, device=dev)
+    dh0 = torch.empty(B, H, dtype=f32, device=dev)
+    with _timed("gru_seq_bwd", 1, 0.0, 2.0 * B * T * 3 * H * H):
+        check(lib().eb_gru_seq_bwd(_p(dy), _p(save), _p(y), _p(h0), _p(whh), _p(dhT), _p(dgi), _p(dgh), _p(dh0),
+                                   _p(_gru_scratch(B, H, dev)), B, T, H, _s()), "eb_gru_seq_bwd")
+    return dgi, dgh, dh0
+
+
+def gru_tc_supported(B, H):
+    return bool(lib().eb_gru_tc_supported(B, H))
+
+
+def _gru_tc_scratch(B, H, device):
+    key = ("gru_tc", H, device, _s())
+    t = _scratch.get(key)
+    if t is None:
+        t = torch.zeros(lib().eb_gru_tc_scratch_bytes(B, H), dtype=torch.uint8, device=device)
+        _scratch[key] = t
+    return t
+
+
+def gru_tc_fwd(xg, whh16, bhn, h0, save):
+    """bf16 tensor-core recurrence: xg [B,T,3H] fp32, whh16 [3H,H] bf16 -> (y, hT, save | None), as gru_seq_fwd."""
+    B, T, H3 = xg.shape
+    H = H3 // 3
+    dev = xg.device
+    y = torch.empty(B, T, H, dtype=f32, device=dev)
+    hT = torch.empty(B, H, dtype=f32, device=dev)
+    sv = torch.empty(B, T, 4 * H, dtype=f32, device=dev) if save else None
+    with _timed("gru_tc_fwd", 1, 0.0, 2.0 * B * T * 3 * H * H):
+        check(lib().eb_gru_tc_fwd(_p(xg), _p(whh16), _p(bhn), _p(h0), _p(y), _p(hT), _p(sv),
+                                  _p(_gru_tc_scratch(B, H, dev)), B, T, H, _s()), "eb_gru_tc_fwd")
+    return y, hT, sv
+
+
+def gru_tc_bwd(dy, save, y, h0, whhT16, dhT):
+    """Returns (dgi16, dgh16 [B,T,3H] bf16, dh0 [B,H] fp32)."""
+    B, T, H = dy.shape
+    dev = dy.device
+    dgi = torch.empty(B, T, 3 * H, dtype=bf16, device=dev)
+    dgh = torch.empty(B, T, 3 * H, dtype=bf16, device=dev)
+    dh0 = torch.empty(B, H, dtype=f32, device=dev)
+    with _timed("gru_tc_bwd", 1, 0.0, 2.0 * B * T * 3 * H * H):
+        check(lib().eb_gru_tc_bwd(_p(dy), _p(save), _p(y), _p(h0), _p(whhT16), _p(dhT), _p(dgi), _p(dgh), _p(dh0),
+                                  _p(_gru_tc_scratch(B, H, dev)), B, T, H, _s()), "eb_gru_tc_bwd")
+    return dgi, dgh, dh0
+
+
 def lstm_tc_supported(B, H):
     return bool(lib().eb_lstm_tc_supported(B, H))
 

@@ -126,10 +126,12 @@ class ResLayerNormLSTM(nn.Module):
 
 
 class ResLayerNormGRU(nn.Module):
-    """rnnt/models.py:77-116, the GRU encoder variant (`module_type='GRU'`, only cli/lightning.py:63 selects it).
-    SURVEY 8(a) a22: kept as a TORCH FALLBACK -- nn.GRU / nn.LayerNorm run through ATen (cuDNN on a GPU), not through
-    this library's kernels; same constructor, ``state_dict`` keys (`lstms.{i}`, `projs.{i}.0`) and return value
-    (xs, hs [L, B, H]) as the reference, so a GRU checkpoint loads and decodes."""
+    """rnnt/models.py:77-116, the GRU encoder variant (`module_type='GRU'`, cli/lightning.py selects it through
+    --enc_type).  Same constructor, ``state_dict`` keys (`lstms.{i}`, `projs.{i}.0`) and return value
+    (xs, hs [L, B, H]) as the reference.  The ``nn.GRU`` / ``nn.LayerNorm`` objects are parameter containers only: each
+    layer runs functional.GRULayer (persistent GRU recurrence: eb_gru_seq_fwd/bwd, in bf16 mode eb_gru_tc_fwd/bwd),
+    LayerNorm with the residual fused (functional.LayerNormRes) and the engine's TimeReduction, layer after layer, like
+    ResLayerNormLSTM's per-layer path."""
 
     def __init__(self, input_size, hidden_size, num_layers, dropout=0, time_reductions=[1], reduction_factor=2):
         super().__init__()
@@ -147,29 +149,24 @@ class ResLayerNormGRU(nn.Module):
             input_size = hidden_size
             self.projs.append(nn.Sequential(*proj))
 
-    @staticmethod
-    def _time_reduce(x, factor=2):
-        B, T, H = x.shape
-        pad = (factor - T % factor) % factor
-        if pad:
-            x = nn.functional.pad(x, [0, 0, 0, pad])
-        return x.reshape(B, -1, factor, H).mean(2)
-
     def forward(self, xs, hiddens=None):
-        hs = xs.new_zeros(len(self.lstms), xs.shape[0], self.hidden_size) if hiddens is None else hiddens
+        p = _precision(self)
         new_hs = []
-        for i, (gru, proj) in enumerate(zip(self.lstms, self.projs)):
-            ys, h = gru(xs, hs[i, None].contiguous())
-            xs = ys if i == 0 else xs + ys
-            for m in proj:                                   # torch modules, except the parameter-free reduction
-                xs = self._time_reduce(xs, m.reduction_factor) if isinstance(m, TimeReduction) else m(xs)
-            new_hs.append(h)
-        return xs, torch.cat(new_hs, dim=0)
+        for i, (gru, post) in enumerate(zip(self.lstms, self.projs)):
+            h0 = None if hiddens is None else hiddens[i]
+            y, hT = Fn.GRULayer.apply(xs, h0, gru.weight_ih_l0, gru.weight_hh_l0, gru.bias_ih_l0, gru.bias_hh_l0, p)
+            ln = post[0]
+            xs = Fn.LayerNormRes.apply(y, xs if i != 0 else None, ln.weight, ln.bias, ln.eps)
+            for extra in list(post)[1:]:
+                xs = extra(xs)
+            new_hs.append(hT)
+        return xs, torch.stack(new_hs, 0)
 
 
 class Encoder(nn.Module):
     """rnnt/models.py:119-136.  ``module`` defaults to the LSTM stack (the reference's default argument is the GRU
-    variant, but every caller that matters passes the LSTM one; ResLayerNormGRU above is the torch fallback)."""
+    variant, but every caller that matters passes the one it wants; Transducer passes ResLayerNormGRU for
+    ``module_type='GRU'``).  Both stacks run on this library's kernels."""
 
     def __init__(self, input_size, hidden_size, num_layers, dropout, proj_size,
                  module=ResLayerNormLSTM, time_reductions=[1], has_proj=True):
@@ -251,7 +248,7 @@ class Transducer(nn.Module):
         self.blank = blank
         if module_type not in ['GRU', 'LSTM']:
             raise ValueError('Unsupported module type')
-        # rnnt/models.py:196-205: the GRU variant runs as a torch fallback (SURVEY 8(a) a22), the LSTM one on this engine
+        # rnnt/models.py:196-205: GRU or LSTM encoder stack, both on this engine
         self.encoder = Encoder(input_size=input_size, hidden_size=enc_hidden_size, num_layers=enc_layers,
                                dropout=enc_dropout, proj_size=enc_proj_size,
                                time_reductions=enc_time_reductions,

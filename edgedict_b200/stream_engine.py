@@ -63,6 +63,10 @@ class StreamEngine:
     def __init__(self, transducer, n_streams, frames_per_chunk, unk_id=UNK, blank=NUL, max_ctas=0, state=None):
         assert C.sizeof(EbPhase) == lib().eb_decode_phase_size(), "EbPhase layout mismatch"
         enc, dec, joint = transducer.encoder, transducer.decoder, transducer.joint.joint
+        from .rnnt.models import ResLayerNormLSTM
+        if not isinstance(enc.lstm, ResLayerNormLSTM):
+            # the decode program's encoder phases are LSTM cells (4H-row weights); a GRU stack has 3H rows
+            raise ValueError("StreamEngine streams an LSTM encoder only, got %s" % type(enc.lstm).__name__)
         self.dev = enc.norm.weight.device
         if self.dev.type != "cuda":
             raise RuntimeError("StreamEngine needs the model on a CUDA device")

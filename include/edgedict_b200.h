@@ -95,6 +95,34 @@ int eb_lstm_seq_bwd(const float* dy, const float* gates, const float* cseq, cons
                     const float* whh, const float* dhT, const float* dcT, float* dgates, float* dh0,
                     float* dc0, void* scratch, int B, int T, int H, void* stream);
 
+/* ---- GRU layer, recurrent part (persistent kernel, fp32) ------------------------------------
+ * replaces the time loop of nn.GRU (rnnt/models.py:77-116, ResLayerNormGRU), gate order r|z|n:
+ *   r = s(xg_r + W_hr h), z = s(xg_z + W_hz h), n = tanh(xg_n + r (W_hn h + b_hn)), h' = (1-z) n + z h.
+ * xg [B,T,3H] = W_ih x + b_ih + (b_hr | b_hz | 0); whh [3H,H]; bhn [H] (NULL: zero); h0 may be NULL (zeros).
+ * save [B,T,4H] = r | z | n | gh_n (gh_n = W_hn h + b_hn), may be NULL for inference.
+ * scratch: eb_gru_scratch_bytes(B,H) bytes, 16-byte aligned (0: H not supported). */
+size_t eb_gru_scratch_bytes(int B, int H);
+int eb_gru_seq_fwd(const float* xg, const float* whh, const float* bhn, const float* h0, float* y, float* hT,
+                   float* save, void* scratch, int B, int T, int H, void* stream);
+/* BPTT: y [B,T,H] the forward output (h_{t-1} of step t is y[:, t-1], h0 at t = 0), dhT may be NULL.
+ * dgi [B,T,3H] = [dr, dz, dn] (input side: dx, dW_ih, db_ih), dgh [B,T,3H] = [dr, dz, r dn] (recurrent side:
+ * dW_hh, db_hh), dh0 [B,H] = d loss / d h0. */
+int eb_gru_seq_bwd(const float* dy, const float* save, const float* y, const float* h0, const float* whh,
+                   const float* dhT, float* dgi, float* dgh, float* dh0, void* scratch, int B, int T, int H,
+                   void* stream);
+
+/* ---- GRU layer on tensor cores (bf16 mode; H % 64 == 0, H <= 1024) ----------------------------
+ * same contract as eb_gru_seq_fwd/bwd with bf16 recurrent operands (fp32 accumulation, fp32 state): whh16 [3H,H] bf16,
+ * whhT16 [H,3H] bf16 (= W_hh^T), both 4-byte aligned; dgi16 / dgh16 [B,T,3H] bf16 out.  scratch:
+ * eb_gru_tc_scratch_bytes(B,H) bytes, 16-byte aligned. */
+int eb_gru_tc_supported(int B, int H);
+size_t eb_gru_tc_scratch_bytes(int B, int H);
+int eb_gru_tc_fwd(const float* xg, const void* whh16, const float* bhn, const float* h0, float* y, float* hT,
+                  float* save, void* scratch, int B, int T, int H, void* stream);
+int eb_gru_tc_bwd(const float* dy, const float* save, const float* y, const float* h0, const void* whhT16,
+                  const float* dhT, void* dgi16, void* dgh16, float* dh0, void* scratch, int B, int T, int H,
+                  void* stream);
+
 /* ---- LSTM layer on tensor cores (bf16 mode; H % 64 == 0, H <= 1024) ---------------------------
  * same contract as eb_lstm_seq_fwd/bwd with bf16 recurrent operands (fp32 accumulation, fp32 cell
  * state): whh16 [4H,H] bf16, whhT16 [H,4H] bf16 (= W_hh^T), y16 optional bf16 copy of y, dg16
