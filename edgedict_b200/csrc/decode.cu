@@ -302,6 +302,13 @@ __device__ void phase_ln(const EbPhase& p) {
     }
 }
 
+// (v, i) ranks above (b, bi) in torch.argmax's order: NaN above every number, then by value, ties to the lower index
+__device__ __forceinline__ bool argmax_before(float v, int i, float b, int bi) {
+    if (isnan(v)) return !isnan(b) || i < bi;
+    if (isnan(b)) return false;
+    return v > b || (v == b && i < bi);
+}
+
 __device__ void phase_argmax(const EbPhase& p) {
     const int lane = threadIdx.x & 31, V = p.N, blank = p.aux, unk = p.aux2;
     (void)blank;
@@ -309,18 +316,20 @@ __device__ void phase_argmax(const EbPhase& p) {
         const float* x = p.x1 + (long)s * p.ldx1;
         int pred = -1;
         for (int pass = 0; pass < 2; ++pass) {
+            // the sentinel index loses every tie, so an all -inf row gives index 0 and a lane without columns
+            // (V < 32) never wins: the token is always in [0, V)
             float best = -INFINITY;
             int bi = 0x7fffffff;
             for (int v = lane; v < V; v += 32) {
                 float val = __ldcg(x + v);
                 if (pass == 1 && v == pred) val = 0.f;              // stream.py:107 `prob[:, pred] = 0`
-                if (val > best) { best = val; bi = v; }             // strict >: first index wins ties
+                if (argmax_before(val, v, best, bi)) { best = val; bi = v; }
             }
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) {
                 float ob = __shfl_xor_sync(0xffffffffu, best, o);
                 int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-                if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }
+                if (argmax_before(ob, oi, best, bi)) { best = ob; bi = oi; }
             }
             pred = bi;
             if (pred != unk) break;

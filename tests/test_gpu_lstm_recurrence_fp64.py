@@ -89,16 +89,18 @@ def _report(name, items):
 
 
 # ---- fp64 references --------------------------------------------------------------------------------------------------
-def fwd_ref(xg, w, hin, cin, n_add, u_acc, eps):
+def fwd_ref(xg, w, hin, cin, n_add, u_acc, eps, dpre_in=0.0, dcin=0.0):
     """Teacher-forced forward, every step at once.  xg [B,T,4H], w [4H,H] (the values the kernel multiplies), hin [B,T,H]
     the h_{t-1} operand of each step as the kernel used it (bf16(h0) / hprev16 / y16 / y), cin [B,T,H] the c_{t-1} the
-    kernel carried (c0, then its fp32 cell save).  Returns {name: (value, bar)} for gates [B,T,4,H], c and y [B,T,H]."""
+    kernel carried (c0, then its fp32 cell save).  dpre_in [B,T,4H] and dcin [B,T,H] are bars the pre-activation and
+    c_{t-1} already carry (0 when every input is the kernel's own).  Returns {name: (value, bar)} for gates [B,T,4,H],
+    c and y [B,T,H]."""
     xg, w, hin, cin = (a.to(f64) for a in (xg, w, hin, cin))
     B, T, H4 = xg.shape
     H = H4 // 4
     s = hin @ w.t()
     pre = (xg + s).view(B, T, 4, H)
-    dpre = (n_add * u_acc * (hin.abs() @ w.abs().t()) + U24 * (s.abs() + xg.abs())).view(B, T, 4, H)
+    dpre = (n_add * u_acc * (hin.abs() @ w.abs().t()) + U24 * (s.abs() + xg.abs()) + dpre_in).view(B, T, 4, H)
     sg = torch.sigmoid(pre)
     tg = torch.tanh(pre)
     is_g = (torch.arange(4, device=pre.device) == 2).view(1, 1, 4, 1)
@@ -108,7 +110,7 @@ def fwd_ref(xg, w, hin, cin, n_add, u_acc, eps):
     i, f, g, o = act.unbind(2)
     di, df, dg, do = dact.unbind(2)
     c = f * cin + i * g
-    dc = df * cin.abs() + di * g.abs() + i * dg + 2 * U24 * ((f * cin).abs() + (i * g).abs())
+    dc = df * cin.abs() + f * dcin + di * g.abs() + i * dg + 2 * U24 * ((f * cin).abs() + (i * g).abs())
     tc = torch.tanh(c)
     y = o * tc
     dy = do * tc.abs() + o * ((1 - tc * tc) * dc + eps) + 2 * U24 * y.abs()
