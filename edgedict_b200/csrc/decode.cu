@@ -15,7 +15,8 @@
 //   ARGMAX  token = argmax(logits) with the <unk> rule (stream.py:105-108: logit := 0, re-argmax)
 //   COPY    y = x
 //   BEAM_SELECT  per utterance: log-softmax of its W rows, exact top-W of the live slots' candidates, merge of equal
-//           token sequences, new slot log p / tokens / gather sources / history (Transducer.beam_search, one frame)
+//           token sequences, new slot log p / tokens / gather sources / history (Transducer.beam_search, one frame);
+//           optionally with an LSTM language model's log-probs fused into the candidate values (shallow fusion)
 //   GATHER  y[l, r] = x1[l, src[r]] (and y2[r] = x2[src[r]]): survivors inherit their parent's predictor state
 //   BEAM_FINAL  per utterance: best live slot, back-pointer walk through the history, ids and -log p written out
 //
@@ -204,7 +205,10 @@ __device__ void phase_lstm(const EbPhase& p, float* red, float* outs) {
 #pragma unroll
                 for (int c = 0; c < 4; ++c) acc[a][b][c] = 0.f;
         auto x1row = [&](int r) -> const float* {
-            if (embed) return p.x1 + (long)__ldcg(p.tok_in + s0 + r) * p.ldx1;     // embedding row of the last token
+            if (embed) {                                     // embedding row of the last token; none (zeros) below 0
+                const int k = __ldcg(p.tok_in + s0 + r);
+                return k < 0 ? nullptr : p.x1 + (long)k * p.ldx1;
+            }
             return p.x1 + (long)(s0 + r) * p.ldx1;
         };
         auto hrow = [&](int r) -> const float* { return p.x2 + (long)(s0 + r) * p.ldx2; };
@@ -355,15 +359,17 @@ __device__ void phase_argmax(const EbPhase& p) {
 //     sequences [B*W][T'+3] = {len, hash lo, hash hi, tokens} of frame t-1 / t (two buffers alternating by frame);
 //     hist = parent slot [B,T',W] | token [B,T',W] | log p (fp32 bits) [B,T',W] | live count [B,T'], back to back.
 //     Slots 0..live-1 are live.  Frozen frames (t >= frames[b]) write an identity history entry.
+//     flags 32 = LM fusion: x2 LM logits [B*W, K2] (ldx2), fuse {lm_weight, length_bonus}, tok_map [V] -> LM token or
+//     -1, tok_out2 LM token per row (-1 where the LM rests, its masked step's sentinel).
 //   BEAM_FINAL (S = B, aux = W, aux2 = blank): y slot log p; hist; tok_out ids [B][ldy], the non-blank tokens of the
 //     best live slot right-aligned in the row and -1 before them; y2 -log p of that slot [B].
 // Both run one CTA per utterance (grid-strided over B).  They are __noinline__ so that their registers do not
 // count against the tensor-core phases the streaming decode spends its time in.
 constexpr int BEAM_MAX_W = EB_BEAM_MAX_W;
 constexpr unsigned long long SEQ_HASH_MUL = 0x100000001b3ull;      // polynomial hash: h' = h * MUL + (token + 1)
-// BEAM_SELECT's shared memory (2 x u64 + 10 x 32-bit arrays of BEAM_MAX_W, histogram, scalars) lives in the dynamic
+// BEAM_SELECT's shared memory (2 x u64 + 12 x 32-bit arrays of BEAM_MAX_W, histogram, scalars) lives in the dynamic
 // shared memory the matrix phases use
-static_assert(BEAM_MAX_W * (2 * 8 + 10 * 4) + 256 * 4 + 8 * 4 <= (RED_FLOATS + TR * OUT_LD) * 4, "beam smem");
+static_assert(BEAM_MAX_W * (2 * 8 + 12 * 4) + 256 * 4 + 8 * 4 <= (RED_FLOATS + TR * OUT_LD) * 4, "beam smem");
 
 // order-preserving map of a float to uint32 (larger float -> larger key); -0 ranks with +0 as in a float compare
 __device__ __forceinline__ uint32_t order_key(float v) {
@@ -393,6 +399,10 @@ __device__ bool seq_extends(const int* s2, const int* s1, int k1) {
 
 // Selection: the candidates of one utterance are (slot q < live, token k) with value
 //   lp = ((x[q,k] - max_q) - log sum_k exp(x[q,k] - max_q)) + logp[q],
+// or with LM fusion (flags 32) lp = (a + f) + logp[q] where a is the first term above and, for k != blank,
+//   f = lm_weight * ((l[q,j] - lmax_q) - log sum_i exp(l[q,i] - lmax_q)) + length_bonus   (j = tok_map[k] >= 0)
+//   f = length_bonus   (j < 0),
+// and f = 0 for blank (a + 0 is a bitwise, since a is never -0: lm_weight = length_bonus = 0 ranks as without LM).
 // ranked by value descending, ties by the lowest flat index q*V + k.  Each candidate's 64-bit composite
 // (order_key(lp) << 32 | tie_key(flat)) is unique and orders exactly so; a radix select finds the min(W, live*V)-th largest
 // composite 8 bits at a time (a 256-bin shared-memory histogram per pass, stopping at the first pass whose chosen bin
@@ -407,7 +417,7 @@ __device__ bool seq_extends(const int* s2, const int* s1, int k1) {
 __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
     const int W = p.aux, V = p.N, T = p.hist_ld, t = p.hist_col, blank = p.aux2;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nt = blockDim.x;
-    const bool merge = p.flags & 16;
+    const bool merge = p.flags & 16, lm = p.flags & 32;
     const long BTW = (long)p.S * T * W;
     int* hpar = p.hist;
     int* htok = p.hist + BTW;
@@ -426,8 +436,11 @@ __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
     int* slen = stok + BEAM_MAX_W;
     int* sfirst = slen + BEAM_MAX_W;
     int* skept = sfirst + BEAM_MAX_W;                                           // slot -> survivor index
-    unsigned* rhist = reinterpret_cast<unsigned*>(skept + BEAM_MAX_W);          // [256]
+    float* lmm = reinterpret_cast<float*>(skept + BEAM_MAX_W);                   // LM log-softmax statistics
+    float* lmls = lmm + BEAM_MAX_W;
+    unsigned* rhist = reinterpret_cast<unsigned*>(lmls + BEAM_MAX_W);           // [256]
     int* misc = reinterpret_cast<int*>(rhist + 256);
+    const float lm_weight = lm ? __ldg(p.fuse) : 0.f, length_bonus = lm ? __ldg(p.fuse + 1) : 0.f;
     for (int b = blockIdx.x; b < p.S; b += gridDim.x) {
         const long r0 = (long)b * W, h0 = ((long)b * T + t) * W;
         const int nlive = t == 0 ? 1 : __ldcg(hlive + (long)b * T + t - 1);
@@ -439,6 +452,7 @@ __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
                 hlp[h0 + j] = __ldcg(p.y + r0 + j);
                 p.tok_out[r0 + j] = blank;
                 p.src[r0 + j] = (int)(r0 + j);
+                if (lm) p.tok_out2[r0 + j] = -1;
             }
             if (tid == 0) hlive[(long)b * T + t] = nlive;
             continue;
@@ -457,10 +471,34 @@ __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
                 rowls[q] = logf(s);
                 rowlp[q] = __ldcg(p.y + r0 + q);
             }
+            if (lm) {
+                const float* l = p.x2 + (r0 + q) * p.ldx2;
+                float lmx = -INFINITY;
+                for (int k = lane; k < p.K2; k += 32) lmx = fmaxf(lmx, __ldcg(l + k));
+                lmx = warp_max(lmx);
+                float ls = 0.f;
+                for (int k = lane; k < p.K2; k += 32) ls += expf(__ldcg(l + k) - lmx);
+                ls = warp_sum(ls);
+                if (lane == 0) {
+                    lmm[q] = lmx;
+                    lmls[q] = logf(ls);
+                }
+            }
         }
         __syncthreads();
+        // the one expression every pass ranks by
         auto composite = [&](int q, int k, const float* x) -> unsigned long long {
-            const float v = ((__ldcg(x + k) - rowm[q]) - rowls[q]) + rowlp[q];
+            float v = (__ldcg(x + k) - rowm[q]) - rowls[q];
+            if (lm) {
+                float f = 0.f;
+                if (k != blank) {
+                    const int j = __ldg(p.tok_map + k);
+                    f = j >= 0 ? lm_weight * ((__ldcg(p.x2 + (r0 + q) * p.ldx2 + j) - lmm[q]) - lmls[q]) + length_bonus
+                               : length_bonus;
+                }
+                v = v + f;
+            }
+            v = v + rowlp[q];
             return ((unsigned long long)order_key(v) << 32) | tie_key((unsigned)(q * V + k));
         };
         const int nsel = (int)min((long)W, (long)nlive * V);
@@ -590,6 +628,7 @@ __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
                 const int i = skept[s], k = stok[i];
                 p.y[r] = smlp[i];
                 p.tok_out[r] = k;
+                if (lm) p.tok_out2[r] = k != blank ? __ldg(p.tok_map + k) : -1;
                 p.src[r] = (int)(r0 + spar[i]);
                 hpar[h] = spar[i];
                 htok[h] = k;
@@ -601,6 +640,7 @@ __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
             } else {
                 p.y[r] = -INFINITY;
                 p.tok_out[r] = blank;
+                if (lm) p.tok_out2[r] = -1;
                 p.src[r] = (int)r;
                 hpar[h] = s;
                 htok[h] = blank;
@@ -669,6 +709,9 @@ __device__ __noinline__ void phase_beam_final(const EbPhase& p) {
         for (int j = lane; j < pos; j += 32) ids[j] = -1;
     }
 }
+
+// the phase loader copies the struct as 32-bit words, one per thread of the 256-thread CTA
+static_assert(sizeof(EbPhase) % 4 == 0 && sizeof(EbPhase) / 4 <= 256, "EbPhase loader");
 
 __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __restrict__ prog, int nphase, unsigned* bar) {
     extern __shared__ __align__(16) float dsm[];

@@ -321,7 +321,8 @@ class Transducer(nn.Module):
 
 
     @torch.no_grad()
-    def beam_search(self, xs, xlen=None, W=4, merge=True):
+    def beam_search(self, xs, xlen=None, W=4, merge=True, *, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1,
+                    lm_token_map=None):
         """SURVEY 8(f) N4: beam decode.  The reference has no beam search in rnnt/ (north_star mentions one); its
         legacy v0 stack holds a batch-1 Graves-style search (models.py:121-202, with no-op `sorted(...)` calls and a
         removed `volatile=` API).  This is a time-synchronous beam under the SAME emission constraint as
@@ -335,11 +336,31 @@ class Transducer(nn.Module):
         All utterances are searched together on the device after the encoder, in one persistent kernel launch
         (stream_engine.BeamEngine); each utterance's result does not depend on the rest of the batch.  The joint and
         the log-softmax run in fp32-accurate arithmetic (3xTF32 products, fp32 log-softmax) whatever `set_precision`
-        or autocast says, as in `greedy_decode`; only the encoder follows the precision setting."""
-        from ..stream_engine import BeamEngine, BEAM_MAX_W, param_fingerprint
+        or autocast says, as in `greedy_decode`; only the encoder follows the precision setting.
+
+        Shallow fusion of a language model: `lm` is the reference's `LMModel` (models.py:224-261; an nn.Embedding
+        `encoder`, a batch_first one-direction nn.LSTM `rnn` without proj_size, an nn.Linear `decoder` over the same
+        tokens) or its state_dict (what cli/train_lm.py saves).  Per frame the candidate (slot q, token k) is ranked by
+        (a + f) + logp[q], with a the acoustic log-softmax value and, for k != blank,
+        f = lm_weight * log_softmax(LM logits of slot q)[map(k)] + length_bonus, or f = length_bonus when
+        map(k) = -1 (a token the LM does not score); f = 0 for blank.  `map` is the identity (the LM's tokens must be
+        the transducer's) or `lm_token_map`, an integer tensor [V] with values in [-1, ntoken).  Each hypothesis' LM
+        state starts from zeros with one step on `lm_bos` (<bos> = 1 in cli/train_lm.py's seq_collate) and steps on
+        map(k) only when the hypothesis emits a non-blank k with map(k) >= 0; there is no end-of-sentence term.  The LM
+        runs as in eval mode (no dropout), in the same fp32-accurate arithmetic as the predictor.  Ranking, merging
+        (log-add of the fused values) and the final pick are as without LM, and the returned -log p is the negated
+        fused score of the best hypothesis.  With lm_weight = length_bonus = 0 the result is bitwise that of lm=None."""
+        from ..stream_engine import BeamEngine, BEAM_MAX_W, check_lm_args, param_fingerprint
         W = operator.index(W)
         if not 1 <= W <= BEAM_MAX_W:
             raise ValueError("beam width W must be in [1, %d], got %d" % (BEAM_MAX_W, W))
+        fusion = check_lm_args(lm, self.joint.joint[2].weight.shape[0], lm_weight, length_bonus, lm_bos, lm_token_map)
+        lm_key = None
+        if fusion is not None:
+            lsd, lw, lb, bos, tmap = fusion
+            # a state_dict on another device is copied into the engine: its tensors' identity and version are the key
+            lm_key = (tuple((k, v.data_ptr(), v.device, v.dtype, v._version) for k, v in sorted(lsd.items())),
+                      lw, lb, bos, tuple(tmap.tolist()))
         h_enc, _ = self.encoder(xs)
         B, T = h_enc.shape[0], h_enc.shape[1]
         if xlen is None:
@@ -348,12 +369,14 @@ class Transducer(nn.Module):
             frames = scale_length(T, xlen).clamp(max=T).to(torch.int32)
         frames = _lens_to_device(frames.cpu(), h_enc.device)
         # the phase program bakes raw weight pointers: re-homed parameters (FlatAdam, .to(), .float()) rebuild it
-        key = (B, T, W, bool(merge), h_enc.device, param_fingerprint(self))
+        key = (B, T, W, bool(merge), h_enc.device, param_fingerprint(self), lm_key)
         cache = self.__dict__.setdefault("_beam_engines", {})
         eng = cache.get(key)
         if eng is None:
             cache.clear()                                  # one resident program is enough
-            eng = cache[key] = BeamEngine(self, B, T, W, merge=bool(merge), blank=self.blank)
+            eng = cache[key] = BeamEngine(self, B, T, W, merge=bool(merge), blank=self.blank, lm=lm,
+                                          lm_weight=lm_weight, length_bonus=length_bonus, lm_bos=lm_bos,
+                                          lm_token_map=lm_token_map)
         ids, nlogp = eng.run(h_enc, frames)
         ids = ids.cpu().numpy()
         return [[int(k) for k in row if k >= 0] for row in ids], nlogp.clone()

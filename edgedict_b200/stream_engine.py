@@ -9,6 +9,9 @@ PytorchStreamDecoder.reset/decode (reference rnnt/stream.py:78-120): at most one
 encoder frame, argmax over raw logits, predictor advanced only on non-blank.
 """
 import ctypes as C
+import math
+import numbers
+import operator
 
 import torch
 
@@ -16,7 +19,7 @@ from ._lib import lib, check
 from .rnnt.tokenizer import NUL, BOS, UNK
 
 PH_LN, PH_PAIR, PH_LSTM, PH_LINEAR, PH_ARGMAX, PH_COPY, PH_BEAM_SELECT, PH_GATHER, PH_BEAM_FINAL = range(9)
-F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE = 1, 2, 4, 8, 16
+F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE, F_LM = 1, 2, 4, 8, 16, 32
 BEAM_MAX_W = 1024                                     # EB_BEAM_MAX_W
 
 
@@ -24,31 +27,123 @@ class EbPhase(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("type", "S", "K1", "K2", "N", "flags", "ldx1", "ldx2", "ldw1", "ldw2",
                                          "ldy", "aux", "aux2", "hist_ld", "hist_col", "x1_div")] + \
                [(n, C.c_void_p) for n in ("x1", "x2", "w1", "w2", "b1", "b2", "y", "y2", "c", "tok_in", "tok_out",
-                                          "hist", "seq_in", "seq_out", "src")]
+                                          "hist", "seq_in", "seq_out", "src", "fuse", "tok_map", "tok_out2")]
 
 
 def _ptr(t, off=0):
     return None if t is None else t.data_ptr() + off * t.element_size()
 
 
-def predictor_phases(prog, dec, S, h, c, htmp, x, tok, blank, masked):
-    """Append one predictor step for S rows to the phase list ``prog``: the embedding row of ``tok`` through every
-    LSTM layer (h, c, htmp [Ld, S, Hd]; with ``masked``, rows whose token is ``blank`` keep their state), then the
-    projection into x [S, D]."""
-    Ld, Hd = dec.lstm.num_layers, dec.lstm.hidden_size
-    Em, D = dec.embed.weight.shape[1], dec.proj.weight.shape[0]
+def lstm_layers(lstm):
+    """[(weight_ih, weight_hh, bias_ih, bias_hh)] of every layer of an nn.LSTM."""
+    return [tuple(getattr(lstm, n % k) for n in ("weight_ih_l%d", "weight_hh_l%d", "bias_ih_l%d", "bias_hh_l%d"))
+            for k in range(lstm.num_layers)]
+
+
+def predictor_phases(prog, embed, layers, proj_w, proj_b, S, h, c, htmp, x, tok, rest, masked):
+    """Append one step of an embedding -> LSTM stack -> Linear network for S rows to the phase list ``prog``: the
+    embedding row (of table ``embed``) of ``tok`` through every LSTM layer (``layers`` as from lstm_layers; h, c, htmp
+    [Ld, S, Hd]; with ``masked``, rows whose token is ``rest`` keep their state), then the output Linear into x [S, D].
+    The transducer's predictor rests on blank, a fused language model on -1."""
+    Ld, Hd = len(layers), layers[0][1].shape[1]
+    Em, D = embed.shape[1], proj_w.shape[0]
     fl = F_EMBED | (F_MASKED if masked else 0)
-    for k in range(Ld):
-        w = [getattr(dec.lstm, n % k) for n in ("weight_ih_l%d", "weight_hh_l%d", "bias_ih_l%d", "bias_hh_l%d")]
+    for k, w in enumerate(layers):
         prog.append(EbPhase(type=PH_LSTM, S=S, N=Hd, K1=Em if k == 0 else Hd, K2=Hd,
                             flags=fl if k == 0 else (fl & F_MASKED),
-                            x1=_ptr(dec.embed.weight) if k == 0 else _ptr(htmp[k - 1]), ldx1=Em if k == 0 else Hd,
+                            x1=_ptr(embed) if k == 0 else _ptr(htmp[k - 1]), ldx1=Em if k == 0 else Hd,
                             x2=_ptr(h[k]), ldx2=Hd, w1=_ptr(w[0]), ldw1=w[0].shape[1], w2=_ptr(w[1]), ldw2=Hd,
                             b1=_ptr(w[2]), b2=_ptr(w[3]), c=_ptr(c[k]), y=_ptr(htmp[k]), ldy=Hd, tok_in=_ptr(tok),
-                            aux=blank))
+                            aux=rest))
     prog.append(EbPhase(type=PH_COPY, S=Ld * S, N=Hd, x1=_ptr(htmp), y=_ptr(h)))
-    prog.append(EbPhase(type=PH_LINEAR, S=S, N=D, K1=Hd, x1=_ptr(h[Ld - 1]), ldx1=Hd, w1=_ptr(dec.proj.weight),
-                        ldw1=Hd, b1=_ptr(dec.proj.bias), y=_ptr(x), ldy=D))
+    prog.append(EbPhase(type=PH_LINEAR, S=S, N=D, K1=Hd, x1=_ptr(h[Ld - 1]), ldx1=Hd, w1=_ptr(proj_w),
+                        ldw1=Hd, b1=_ptr(proj_b), y=_ptr(x), ldy=D))
+
+
+def _dec_phases(prog, dec, S, h, c, htmp, x, tok, blank, masked):
+    predictor_phases(prog, dec.embed.weight, lstm_layers(dec.lstm), dec.proj.weight, dec.proj.bias, S, h, c, htmp, x,
+                     tok, blank, masked)
+
+
+def lm_state_dict(lm):
+    """The fusion LM's weights as {key: tensor} in the layout of the reference's LMModel state_dict
+    (``encoder.weight``, ``rnn.{weight_ih,weight_hh,bias_ih,bias_hh}_l{k}``, ``decoder.{weight,bias}``), from the
+    module or from such a state_dict.  Raises TypeError / ValueError for anything else; touches no device."""
+    import torch.nn as nn
+    if isinstance(lm, nn.Module):
+        enc, rnn, dec = (getattr(lm, n, None) for n in ("encoder", "rnn", "decoder"))
+        if not (isinstance(enc, nn.Embedding) and isinstance(rnn, nn.LSTM) and isinstance(dec, nn.Linear)):
+            raise TypeError("lm must have encoder = nn.Embedding, rnn = nn.LSTM and decoder = nn.Linear (LMModel)")
+        if not rnn.batch_first or rnn.bidirectional or rnn.proj_size or not rnn.bias or dec.bias is None:
+            raise ValueError("lm.rnn must be a batch_first, one-direction LSTM with biases and no proj_size, and "
+                             "lm.decoder a Linear with bias")
+        sd = {"encoder.weight": enc.weight, "decoder.weight": dec.weight, "decoder.bias": dec.bias}
+        for k, w in enumerate(lstm_layers(rnn)):
+            for n, t in zip(("weight_ih", "weight_hh", "bias_ih", "bias_hh"), w):
+                sd["rnn.%s_l%d" % (n, k)] = t
+    elif isinstance(lm, dict):
+        sd = dict(lm)
+    else:
+        raise TypeError("lm must be an LMModel-like nn.Module or its state_dict, got %s" % type(lm).__name__)
+    L = 0
+    while "rnn.weight_ih_l%d" % L in sd:
+        L += 1
+    want = ["encoder.weight", "decoder.weight", "decoder.bias"] + \
+        ["rnn.%s_l%d" % (n, k) for k in range(L) for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh")]
+    if L == 0 or set(sd) != set(want):
+        raise ValueError("lm state_dict keys must be exactly %s, got %s" % (want if L else "encoder.weight, "
+                         "rnn.{weight_ih,weight_hh,bias_ih,bias_hh}_l{k}, decoder.{weight,bias}", sorted(sd)))
+    for k, t in sd.items():
+        if not isinstance(t, torch.Tensor) or not t.is_floating_point():
+            raise TypeError("lm weight %s must be a floating-point tensor" % k)
+    sd = {k: t.detach() for k, t in sd.items()}
+    ntok, ninp = sd["encoder.weight"].shape if sd["encoder.weight"].dim() == 2 else (0, 0)
+    H = sd["rnn.weight_hh_l0"].shape[-1]
+    shapes = {"encoder.weight": (ntok, ninp), "decoder.weight": (ntok, H), "decoder.bias": (ntok,)}
+    for k in range(L):
+        shapes.update({"rnn.weight_ih_l%d" % k: (4 * H, ninp if k == 0 else H), "rnn.weight_hh_l%d" % k: (4 * H, H),
+                       "rnn.bias_ih_l%d" % k: (4 * H,), "rnn.bias_hh_l%d" % k: (4 * H,)})
+    for k, s in shapes.items():
+        if tuple(sd[k].shape) != s or 0 in s:
+            raise ValueError("lm weight %s has shape %s, the layout needs %s" % (k, tuple(sd[k].shape), s))
+    return sd
+
+
+def check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map):
+    """Validate the shallow-fusion arguments of a beam search over a vocabulary of V tokens.  Returns
+    (lm state_dict, lm_weight, length_bonus, lm_bos, token map int64 [V] on the host) or None without ``lm``.
+    Raises TypeError / ValueError; touches no device."""
+    if lm is None:
+        if lm_weight != 0.0 or length_bonus != 0.0 or lm_token_map is not None:
+            raise ValueError("lm_weight, length_bonus and lm_token_map need an lm")
+        return None
+    sd = lm_state_dict(lm)
+    ntok = sd["encoder.weight"].shape[0]
+    vals = []
+    for name, v in (("lm_weight", lm_weight), ("length_bonus", length_bonus)):
+        if isinstance(v, bool) or not isinstance(v, numbers.Real):
+            raise TypeError("%s must be a real number, got %r" % (name, v))
+        v = float(v)
+        if not math.isfinite(v):
+            raise ValueError("%s must be finite, got %r" % (name, v))
+        vals.append(v)
+    lm_bos = operator.index(lm_bos)
+    if not 0 <= lm_bos < ntok:
+        raise ValueError("lm_bos must be in [0, %d), got %d" % (ntok, lm_bos))
+    if lm_token_map is None:
+        if ntok != V:
+            raise ValueError("the LM has %d tokens and the transducer %d: pass lm_token_map" % (ntok, V))
+        tmap = torch.arange(V)
+    else:
+        if not isinstance(lm_token_map, torch.Tensor) or lm_token_map.is_floating_point() or \
+                lm_token_map.is_complex() or lm_token_map.dtype == torch.bool:
+            raise TypeError("lm_token_map must be an integer tensor [%d]" % V)
+        if tuple(lm_token_map.shape) != (V,):
+            raise ValueError("lm_token_map must have shape [%d], got %s" % (V, tuple(lm_token_map.shape)))
+        tmap = lm_token_map.detach().to("cpu", torch.int64)
+        if bool(((tmap < -1) | (tmap >= ntok)).any()):
+            raise ValueError("lm_token_map values must be in [-1, %d)" % ntok)
+    return sd, vals[0], vals[1], lm_bos, tmap
 
 
 def param_fingerprint(module):
@@ -143,14 +238,14 @@ class StreamEngine:
                b1=_ptr(joint[2].bias), y=_ptr(self.logits), ldy=V)
             ph(type=PH_ARGMAX, S=S, N=V, x1=_ptr(self.logits), ldx1=V, aux=blank, aux2=unk_id, tok_out=_ptr(self.tok),
                hist=_ptr(self.hist), hist_ld=self.hist.shape[1], hist_col=k)
-            predictor_phases(prog, dec, S, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
-                             masked=True)
+            _dec_phases(prog, dec, S, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
+                        masked=True)
         ph(type=PH_COPY, S=L * S, N=H, x1=_ptr(self.enc_htmp), y=_ptr(self.enc_h))
         self.n_chunk_phases = len(prog)
         chunk_prog = prog
         prog = []
-        predictor_phases(prog, dec, S, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
-                         masked=False)                  # priming program: tok = BOS from a zero state
+        _dec_phases(prog, dec, S, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
+                    masked=False)                  # priming program: tok = BOS from a zero state
         self.n_prime_phases = len(prog)
         self._chunk = self._upload(chunk_prog)
         self._prime = self._upload(prog)
@@ -228,8 +323,8 @@ class GreedyEngine:
                 setattr(q, k, v)
             prog.append(q)
 
-        predictor_phases(prog, dec, B, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
-                         masked=False)                   # prime with BOS from the zero state
+        _dec_phases(prog, dec, B, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
+                    masked=False)                   # prime with BOS from the zero state
         w1 = joint[0].weight
         for k in range(T):
             ph(type=PH_LINEAR, S=B, N=J, flags=F_TANH, K1=E, x1=_ptr(self.h_enc, k * E), ldx1=T * E, w1=_ptr(w1),
@@ -239,8 +334,8 @@ class GreedyEngine:
                b1=_ptr(joint[2].bias), y=_ptr(self.logits), ldy=V)
             ph(type=PH_ARGMAX, S=B, N=V, flags=F_LOGP, x1=_ptr(self.logits), ldx1=V, aux=blank, aux2=-1,
                tok_out=_ptr(self.tok), hist=_ptr(self.hist), hist_ld=T, hist_col=k, y=_ptr(self.logp))
-            predictor_phases(prog, dec, B, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
-                             masked=True)
+            _dec_phases(prog, dec, B, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
+                        masked=True)
         self.nphase = len(prog)
         arr = (EbPhase * len(prog))(*prog)
         self._prog = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(self.dev)
@@ -269,11 +364,20 @@ class BeamEngine:
     BEAM_FINAL picks the best live slot of each utterance and walks its back-pointers.
 
     ``hist_parent`` / ``hist_token`` / ``hist_logp`` [B, T', W] and ``hist_live`` [B, T'] keep the beam of every
-    frame (slots below the live count are live; frames at or past an utterance's length repeat its last beam)."""
+    frame (slots below the live count are live; frames at or past an utterance's length repeat its last beam).
 
-    def __init__(self, transducer, batch, t_out, W, merge=True, blank=NUL, max_ctas=0):
+    With ``lm`` (the reference's LMModel or its state_dict, see check_lm_args) the LM is fused into the candidate
+    values (shallow fusion, decode.cu flag 32): each slot carries an LM state ``lm_h`` / ``lm_c`` (two parities, like
+    the predictor's), primed with ``lm_bos`` and stepped with ``lm_token_map[k]`` only when the slot emitted a
+    non-blank token k the LM scores; after the predictor step, the LM's output Linear recomputes ``lm_logits`` for all
+    rows (a row that did not step gets its parent's logits bit for bit, rows being independent)."""
+
+    def __init__(self, transducer, batch, t_out, W, merge=True, blank=NUL, max_ctas=0, lm=None, lm_weight=0.0,
+                 length_bonus=0.0, lm_bos=1, lm_token_map=None):
         if not 1 <= W <= BEAM_MAX_W:
             raise ValueError("beam width must be in [1, %d], got %r" % (BEAM_MAX_W, W))
+        fusion = check_lm_args(lm, transducer.joint.joint[2].weight.shape[0], lm_weight, length_bonus, lm_bos,
+                               lm_token_map)
         dec, joint = transducer.decoder, transducer.joint.joint
         self.dev = dec.embed.weight.device
         if self.dev.type != "cuda":
@@ -302,8 +406,29 @@ class BeamEngine:
         self.ids, self.nlogp = z(B, max(T, 1), dtype=i32), z(B)
         self._keep = [p.detach() for p in transducer.parameters()]
         prog = []
-        predictor_phases(prog, dec, R, self.dec_h[0], self.dec_c[0], self.dec_htmp, self.dec_x[0], self.tok, blank,
-                         masked=False)                         # prime every row with BOS from the zero state
+        _dec_phases(prog, dec, R, self.dec_h[0], self.dec_c[0], self.dec_htmp, self.dec_x[0], self.tok, blank,
+                    masked=False)                         # prime every row with BOS from the zero state
+        self.lm = fusion is not None
+        if self.lm:
+            lsd, lw, lb, self.lm_bos, tmap = fusion
+            # the weights are read in place when they already are fp32 on this device (tied weights stay tied)
+            lsd = {k: v.to(self.dev, f32).contiguous() for k, v in lsd.items()}
+            self._keep += list(lsd.values())
+            Ll = (len(lsd) - 3) // 4
+            lm_layers = [tuple(lsd["rnn.%s_l%d" % (n, k)] for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"))
+                         for k in range(Ll)]
+            Hl, ntok = lm_layers[0][1].shape[1], lsd["encoder.weight"].shape[0]
+            lst = [z(2 * Ll, R, Hl), z(2 * Ll, R, Hl)]         # as st, for the LM
+            self.lm_h, self.lm_c = [s[:Ll] for s in lst], [s[Ll:] for s in lst]
+            self.lm_htmp, self.lm_logits, self.lm_tok = z(Ll, R, Hl), z(R, ntok), z(R, dtype=i32)
+            self.lm_map = tmap.to(self.dev, i32)
+            self.lm_fuse = torch.tensor([lw, lb], dtype=f32, device=self.dev)
+            self._lst0 = lst[0]
+
+            def lm_phases(q, masked):
+                predictor_phases(prog, lsd["encoder.weight"], lm_layers, lsd["decoder.weight"], lsd["decoder.bias"],
+                                 R, self.lm_h[q], self.lm_c[q], self.lm_htmp, self.lm_logits, self.lm_tok, -1, masked)
+            lm_phases(0, masked=False)                           # prime every row with lm_bos from the zero state
         w1 = joint[0].weight
         for t in range(T):
             p, q = t & 1, 1 - (t & 1)
@@ -312,14 +437,24 @@ class BeamEngine:
                                 w2=_ptr(w1, E), ldw2=E + D, b1=_ptr(joint[0].bias), y=_ptr(self.hidden), ldy=J))
             prog.append(EbPhase(type=PH_LINEAR, S=R, N=V, K1=J, x1=_ptr(self.hidden), ldx1=J,
                                 w1=_ptr(joint[2].weight), ldw1=J, b1=_ptr(joint[2].bias), y=_ptr(self.logits), ldy=V))
-            prog.append(EbPhase(type=PH_BEAM_SELECT, S=B, N=V, aux=W, aux2=blank, flags=F_MERGE if merge else 0,
-                                x1=_ptr(self.logits), ldx1=V, y=_ptr(self.logp), tok_in=_ptr(self.frames),
-                                tok_out=_ptr(self.tok), src=_ptr(self.src), hist=_ptr(self.hist), hist_ld=T,
-                                hist_col=t, seq_in=_ptr(self.seqs[p]), seq_out=_ptr(self.seqs[q])))
+            sel = EbPhase(type=PH_BEAM_SELECT, S=B, N=V, aux=W, aux2=blank, flags=F_MERGE if merge else 0,
+                          x1=_ptr(self.logits), ldx1=V, y=_ptr(self.logp), tok_in=_ptr(self.frames),
+                          tok_out=_ptr(self.tok), src=_ptr(self.src), hist=_ptr(self.hist), hist_ld=T,
+                          hist_col=t, seq_in=_ptr(self.seqs[p]), seq_out=_ptr(self.seqs[q]))
+            if self.lm:
+                sel.flags |= F_LM
+                sel.x2, sel.ldx2, sel.K2 = _ptr(self.lm_logits), ntok, ntok
+                sel.fuse, sel.tok_map, sel.tok_out2 = _ptr(self.lm_fuse), _ptr(self.lm_map), _ptr(self.lm_tok)
+            prog.append(sel)
             prog.append(EbPhase(type=PH_GATHER, S=R, N=Hd, aux=2 * Ld, x1=_ptr(st[p]), y=_ptr(st[q]), K2=D,
                                 x2=_ptr(self.dec_x[p]), y2=_ptr(self.dec_x[q]), src=_ptr(self.src)))
-            predictor_phases(prog, dec, R, self.dec_h[q], self.dec_c[q], self.dec_htmp, self.dec_x[q], self.tok, blank,
-                             masked=True)
+            if self.lm:
+                prog.append(EbPhase(type=PH_GATHER, S=R, N=Hl, aux=2 * Ll, x1=_ptr(lst[p]), y=_ptr(lst[q]),
+                                    src=_ptr(self.src)))
+            _dec_phases(prog, dec, R, self.dec_h[q], self.dec_c[q], self.dec_htmp, self.dec_x[q], self.tok, blank,
+                        masked=True)
+            if self.lm:
+                lm_phases(q, masked=True)
         prog.append(EbPhase(type=PH_BEAM_FINAL, S=B, aux=W, aux2=blank, y=_ptr(self.logp), hist=_ptr(self.hist),
                             hist_ld=T, tok_out=_ptr(self.ids), ldy=self.ids.shape[1], y2=_ptr(self.nlogp)))
         self._st0 = st[0]
@@ -332,7 +467,7 @@ class BeamEngine:
     def run(self, h_enc, frames):
         """h_enc [B, T', E], frames int32 [B] on the device (encoder frames each utterance decodes, <= T') ->
         (ids int32 [B, max(T', 1)]: the best hypothesis' non-blank tokens right-aligned, -1 before them;
-        -log p [B] of that hypothesis)."""
+        -log p [B] of that hypothesis, the negated fused score with an LM)."""
         self.h_enc.copy_(h_enc)
         self.frames.copy_(frames)
         self._st0.zero_()
@@ -340,6 +475,9 @@ class BeamEngine:
         self.logp.fill_(float("-inf"))
         self.logp.view(self.B, self.W)[:, 0] = 0.0
         self.tok.fill_(BOS)
+        if self.lm:
+            self._lst0.zero_()
+            self.lm_tok.fill_(self.lm_bos)
         check(lib().eb_decode_run(self._prog.data_ptr(), self.nphase, self._bar.data_ptr(), self.max_ctas,
                                   torch.cuda.current_stream().cuda_stream), "eb_decode_run")
         return self.ids, self.nlogp

@@ -210,11 +210,19 @@ typedef struct EbPhase {
     int32_t* hist;
     const int32_t* seq_in;
     int32_t *seq_out, *src;
+    const float* fuse;
+    const int32_t* tok_map;
+    int32_t* tok_out2;
 } EbPhase;
-/* flags: 1 = tanh epilogue (LINEAR); 2 = x1 rows are embedding rows indexed by tok_in (LSTM);
- *        4 = masked update: streams whose tok_in equals aux (blank) keep their state (LSTM);
+/* flags: 1 = tanh epilogue (LINEAR); 2 = x1 rows are embedding rows indexed by tok_in, a negative token reading as a
+ *            zero row (LSTM);
+ *        4 = masked update: streams whose tok_in equals aux (blank, or -1 for a language model) keep their state (LSTM);
  *        8 = ARGMAX also accumulates log_softmax(x)[argmax] into y[s] (batched greedy decode);
- *       16 = BEAM_SELECT folds hypotheses with equal token sequences (log-add).
+ *       16 = BEAM_SELECT folds hypotheses with equal token sequences (log-add);
+ *       32 = BEAM_SELECT fuses a language model into the candidate values (shallow fusion): x2 [B*W, K2] (ldx2) holds
+ *            the LM logits of each slot, fuse = {lm_weight, length_bonus} on the device, tok_map [N] maps a token to
+ *            its LM token (-1: not scored by the LM), and tok_out2 [B*W] receives each new slot's LM token (-1 when the
+ *            LM does not step: blank, unmapped, empty slot or frozen utterance).
  * x1_div (LINEAR): row r of x1 is x1[r / x1_div] (0 or 1: row r), the encoder frame a beam's W rows share.
  * Beam search (batched, W slots per utterance, row r = b*W + slot; see decode.cu for the field use of each phase):
  * at most EB_BEAM_MAX_W slots per utterance. */
