@@ -19,6 +19,8 @@
 //           optionally with an LSTM language model's log-probs fused into the candidate values (shallow fusion)
 //   GATHER  y[l, r] = x1[l, src[r]] (and y2[r] = x2[src[r]]): survivors inherit their parent's predictor state
 //   BEAM_FINAL  per utterance: best live slot, back-pointer walk through the history, ids and -log p written out
+//   BEAM_COMMIT per stream, at the end of a streaming chunk: commit the live hypotheses' common prefix, collapse the
+//           beam to its best slot when a stored suffix would outgrow its capacity (or on a flush)
 //
 // LINEAR's x1 row divisor (x1_div) lets the W rows of one utterance's beam share its encoder frame without copies.
 // fp32-accurate arithmetic throughout: the north star asks for token-for-token identical greedy output, which
@@ -363,7 +365,11 @@ __device__ void phase_argmax(const EbPhase& p) {
 //     -1, tok_out2 LM token per row (-1 where the LM rests, its masked step's sentinel).
 //   BEAM_FINAL (S = B, aux = W, aux2 = blank): y slot log p; hist; tok_out ids [B][ldy], the non-blank tokens of the
 //     best live slot right-aligned in the row and -1 before them; y2 -log p of that slot [B].
-// Both run one CTA per utterance (grid-strided over B).  They are __noinline__ so that their registers do not
+//   BEAM_COMMIT (S = B streams, aux = W, N = max_pending, aux2 = max_pending - n_out, K1 = sequence row stride, hist_ld
+//     = T', flags 128 = collapse unconditionally): y slot log p (in/out); hist (reads and rewrites the live count of
+//     column T'-1); seq_in / seq_out sequence rows before / after the commit (distinct buffers); tok_out committed
+//     tokens [B][N]; tok_out2 committed count [B] | collapsed 0/1 [B]; src gather source row [B*W].
+// They run one CTA per utterance (grid-strided over B).  They are __noinline__ so that their registers do not
 // count against the tensor-core phases the streaming decode spends its time in.
 constexpr int BEAM_MAX_W = EB_BEAM_MAX_W;
 constexpr unsigned long long SEQ_HASH_MUL = 0x100000001b3ull;      // polynomial hash: h' = h * MUL + (token + 1)
@@ -414,16 +420,22 @@ __device__ bool seq_extends(const int* s2, const int* s1, int k1) {
 // already merged, two distinct candidates can only have equal sequences when one is the blank extension of a parent
 // q2 and the other the non-blank extension seq(q1) + [k]; length and a 64-bit hash reject the rest, and a hash match
 // is confirmed by an exact token-by-token comparison (seq_extends), never accepted on its own.
+//
+// Streaming (flags 64): the beam lives on across launches.  The live count at t = 0 is the one the previous launch left
+// in the last history column (hist_live[b, T'-1], set by BEAM_COMMIT or the host), and the sequence rows have stride K1
+// (max_pending + 3) whatever the frames per launch.  A row's length counts only the tokens stored since the stream's
+// last commit, while its hash keeps describing the whole sequence: every slot of a stream shares the committed prefix,
+// so equal whole sequences are exactly equal stored suffixes, and seq_extends and the merge stay exact.
 __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
     const int W = p.aux, V = p.N, T = p.hist_ld, t = p.hist_col, blank = p.aux2;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nt = blockDim.x;
-    const bool merge = p.flags & 16, lm = p.flags & 32;
+    const bool merge = p.flags & 16, lm = p.flags & 32, stream = p.flags & 64;
     const long BTW = (long)p.S * T * W;
     int* hpar = p.hist;
     int* htok = p.hist + BTW;
     float* hlp = reinterpret_cast<float*>(p.hist + 2 * BTW);
     int* hlive = p.hist + 3 * BTW;
-    const int LS = T + 3;
+    const int LS = stream ? p.K1 : T + 3;
     unsigned long long* comp = reinterpret_cast<unsigned long long*>(sm);       // [BEAM_MAX_W] (padded to 2^k)
     unsigned long long* shash = comp + BEAM_MAX_W;
     float* rowm = reinterpret_cast<float*>(shash + BEAM_MAX_W);
@@ -443,7 +455,7 @@ __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
     const float lm_weight = lm ? __ldg(p.fuse) : 0.f, length_bonus = lm ? __ldg(p.fuse + 1) : 0.f;
     for (int b = blockIdx.x; b < p.S; b += gridDim.x) {
         const long r0 = (long)b * W, h0 = ((long)b * T + t) * W;
-        const int nlive = t == 0 ? 1 : __ldcg(hlive + (long)b * T + t - 1);
+        const int nlive = t > 0 ? __ldcg(hlive + (long)b * T + t - 1) : stream ? __ldcg(hlive + (long)b * T + T - 1) : 1;
         __syncthreads();                                     // the previous utterance is done with shared memory
         if (t >= __ldg(p.tok_in + b)) {                      // frozen: the beam stays, the predictor rests
             for (int j = tid; j < W; j += nt) {
@@ -672,6 +684,86 @@ __device__ __noinline__ void phase_gather(const EbPhase& p) {
         }
 }
 
+// Chunk end of the streaming beam, one CTA per stream.  The live slots' stored suffixes (seq_in) share a longest common
+// prefix of c tokens; no later frame can change it, since every future hypothesis extends a current one, so it is
+// committed: written to tok_out row b and dropped from every live suffix (seq_out).  If a suffix then still holds more
+// than aux2 = max_pending - n_out tokens (or flags 128: always), the beam collapses: the best live slot (highest log p,
+// lowest slot on ties, as BEAM_FINAL) commits its whole suffix and becomes slot 0, the only live one, keeping its log p.
+// src receives the gather sources that move each kept slot's predictor / LM state into place (identity without a
+// collapse), tok_out2[b] the committed count and tok_out2[S + b] whether the beam collapsed.
+__device__ __noinline__ void phase_beam_commit(const EbPhase& p, float* sm) {
+    const int W = p.aux, T = p.hist_ld, LS = p.K1;
+    const int tid = threadIdx.x, nt = blockDim.x;
+    int* hlive = p.hist + 3 * (long)p.S * T * W;
+    int* misc = reinterpret_cast<int*>(sm);
+    for (int b = blockIdx.x; b < p.S; b += gridDim.x) {
+        const long r0 = (long)b * W;
+        const int nlive = __ldcg(hlive + (long)b * T + T - 1);
+        const int* seq0 = p.seq_in + r0 * LS;
+        __syncthreads();                                     // the previous stream is done with shared memory
+        if (tid == 0) {
+            misc[0] = 0x7fffffff;                            // shortest live suffix
+            misc[1] = 0;                                     // longest live suffix
+            misc[4] = 0x7fffffff;                            // first position where two live suffixes differ
+        }
+        __syncthreads();
+        for (int s = tid; s < nlive; s += nt) {
+            const int len = __ldcg(p.seq_in + (r0 + s) * LS);
+            atomicMin(&misc[0], len);
+            atomicMax(&misc[1], len);
+        }
+        __syncthreads();
+        const int lmin = misc[0];
+        for (long e = tid; e < (long)(nlive - 1) * lmin; e += nt) {
+            const int s = 1 + (int)(e / lmin), j = (int)(e % lmin);
+            if (__ldcg(p.seq_in + (r0 + s) * LS + 3 + j) != __ldcg(seq0 + 3 + j)) atomicMin(&misc[4], j);
+        }
+        __syncthreads();
+        const int c = min(lmin, misc[4]);
+        const bool collapse = (p.flags & 128) || misc[1] - c > p.aux2;
+        if (collapse && tid < 32) {                          // logp.argmax() over the live slots
+            float best = -INFINITY;
+            int bi = -1;
+            for (int j = tid; j < nlive; j += 32) {
+                const float v = __ldcg(p.y + r0 + j);
+                if (bi < 0 || v > best) { best = v; bi = j; }
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+                const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+                if (oi >= 0 && (bi < 0 || ob > best || (ob == best && oi < bi))) { best = ob; bi = oi; }
+            }
+            if (tid == 0) {
+                misc[2] = bi;
+                misc[3] = __float_as_int(best);
+            }
+        }
+        __syncthreads();
+        const int best = collapse ? misc[2] : 0, nkeep = collapse ? 1 : nlive;
+        const int* bs = p.seq_in + (r0 + best) * LS;
+        const int ncommit = collapse ? __ldcg(bs) : c;
+        int* out = p.tok_out + (long)b * p.N;
+        for (int j = tid; j < ncommit; j += nt) out[j] = __ldcg(bs + 3 + j);
+        for (long e = tid; e < (long)nkeep * LS; e += nt) {  // kept slot s: {length - ncommit, hash, shifted tokens}
+            const int s = (int)(e / LS), j = (int)(e % LS);
+            const int* ps = p.seq_in + (r0 + (collapse ? best : s)) * LS;
+            const int len = __ldcg(ps) - ncommit;
+            if (j >= len + 3) continue;
+            p.seq_out[(r0 + s) * LS + j] = j == 0 ? len : j < 3 ? __ldcg(ps + j) : __ldcg(ps + j + ncommit);
+        }
+        for (int s = tid; s < W; s += nt) {
+            p.src[r0 + s] = (int)(r0 + (s == 0 ? best : s));
+            if (collapse) p.y[r0 + s] = s == 0 ? __int_as_float(misc[3]) : -INFINITY;
+        }
+        if (tid == 0) {
+            p.tok_out2[b] = ncommit;
+            p.tok_out2[p.S + b] = collapse;
+            hlive[(long)b * T + T - 1] = nkeep;
+        }
+    }
+}
+
 __device__ __noinline__ void phase_beam_final(const EbPhase& p) {
     const int W = p.aux, T = p.hist_ld, blank = p.aux2, lane = threadIdx.x & 31;
     const long BTW = (long)p.S * T * W;
@@ -746,6 +838,7 @@ __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __re
             case EB_PH_BEAM_SELECT: phase_beam_select(ph, dsm); break;
             case EB_PH_GATHER: phase_gather(ph); break;
             case EB_PH_BEAM_FINAL: phase_beam_final(ph); break;
+            case EB_PH_BEAM_COMMIT: phase_beam_commit(ph, dsm); break;
             default: break;
         }
         ++epoch;

@@ -5,10 +5,13 @@
 joint_elapsed``, ``tokenizer`` -- so ``stream.py`` / ``youtube_live.py`` /
 ``cli/openvino_wav_inference.py`` drive it unchanged, but ``decode`` is ONE persistent-kernel
 launch per chunk (edgedict_b200/stream_engine.py) instead of a Python loop with a host sync per
-encoder frame.  The feature transform and the BPE tokenizer are host-side components outside the
+encoder frame.  With ``beam_width`` it decodes by streaming beam search instead (optionally with a fused LSTM
+language model): ``decode`` returns the text that became final in that chunk and ``flush()`` the rest.
+The feature transform and the BPE tokenizer are host-side components outside the
 hot path: they are taken from the caller (``transform=``, ``tokenizer=``) or, like the reference,
 built from FLAGS when the reference's ``rnnt.transforms`` / ``rnnt.tokenizer`` are importable.
 """
+import operator
 import os
 import time
 
@@ -16,7 +19,7 @@ import torch
 
 from .models import Transducer, convert_lightning2normal
 from .tokenizer import NUL, BOS, UNK
-from ..stream_engine import StreamEngine, param_fingerprint
+from ..stream_engine import BEAM_MAX_W, StreamBeamEngine, StreamEngine, check_lm_args, param_fingerprint
 
 
 class StreamTransducerDecoder:
@@ -33,8 +36,19 @@ class StreamTransducerDecoder:
 
 
 class PytorchStreamDecoder(StreamTransducerDecoder):
+    """``beam_width=None`` decodes greedily, as the reference does.  With a beam width W, every chunk runs the streaming
+    beam search of stream_engine.StreamBeamEngine (``merge``, ``lm``, ``lm_weight``, ``length_bonus``, ``lm_bos`` and
+    ``lm_token_map`` as in Transducer.beam_search; ``max_pending`` caps the uncommitted tokens a hypothesis stores).
+    ``decode`` then returns the text of the tokens that became final in that chunk: the common prefix of all live
+    hypotheses, which no later audio can change, so returned text is never revised.  ``flush()`` returns the rest of
+    the best hypothesis and continues decoding from it; call it at the end of an utterance or a segment.  Without a
+    forced collapse (a suffix outgrowing ``max_pending``), everything ``decode`` returned plus ``flush()`` is the
+    best hypothesis of Transducer.beam_search over the same encoder frames.  The beam does not apply the reference's
+    ``<unk>`` rule, which belongs to greedy argmax decoding; Transducer.beam_search does not apply it either."""
+
     def __init__(self, FLAGS, transducer=None, transform=None, tokenizer=None, device="cuda",
-                 frames_per_chunk=None, input_size=None):
+                 frames_per_chunk=None, input_size=None, *, beam_width=None, merge=True, lm=None, lm_weight=0.0,
+                 length_bonus=0.0, lm_bos=1, lm_token_map=None, max_pending=64):
         self.FLAGS = FLAGS
         self.device = torch.device(device)
         if tokenizer is None:
@@ -71,6 +85,14 @@ class PytorchStreamDecoder(StreamTransducerDecoder):
         self.encoder, self.decoder, self.joint = transducer.encoder, transducer.decoder, transducer.joint
         self._transducer = transducer
         self._unk = self._token_id('<unk>')
+        self._beam = None
+        if beam_width is not None:
+            W = operator.index(beam_width)
+            if not 1 <= W <= BEAM_MAX_W:
+                raise ValueError("beam_width must be in [1, %d], got %d" % (BEAM_MAX_W, W))
+            check_lm_args(lm, transducer.joint.joint[2].weight.shape[0], lm_weight, length_bonus, lm_bos, lm_token_map)
+            self._beam = dict(W=W, merge=bool(merge), lm=lm, lm_weight=lm_weight, length_bonus=length_bonus,
+                              lm_bos=lm_bos, lm_token_map=lm_token_map, max_pending=operator.index(max_pending))
         self._engine = None
         self._frames = frames_per_chunk
         self.reset_profile()
@@ -89,7 +111,10 @@ class PytorchStreamDecoder(StreamTransducerDecoder):
         # program, NOT a new utterance: the recurrent state moves over (rnnt/stream.py:94-120 carries it across
         # arbitrary chunk lengths); only reset() starts from the primed zero state
         st = self._engine.state() if self._engine is not None else None
-        self._engine = StreamEngine(self._transducer, 1, n, unk_id=self._unk, blank=NUL, state=st)
+        if self._beam is None:
+            self._engine = StreamEngine(self._transducer, 1, n, unk_id=self._unk, blank=NUL, state=st)
+        else:
+            self._engine = StreamBeamEngine(self._transducer, 1, n, blank=NUL, state=st, **self._beam)
         self._frames = n
 
     @torch.no_grad()
@@ -104,6 +129,11 @@ class PytorchStreamDecoder(StreamTransducerDecoder):
         if self._engine is None or xs.shape[1] != self._frames or \
                 self._engine.fingerprint != param_fingerprint(self._transducer):
             self._build(xs.shape[1])
+        if self._beam is not None:
+            ids, counts = self._engine.step(xs.to(self.device, non_blocking=True))  # one D2H per chunk
+            self.encoder_elapsed.append(time.time() - start)
+            self.joint_elapsed += [0.0] * self._engine.n_out      # fused into the chunk kernel
+            return self._text(ids[0, :int(counts[0])].tolist())
         ids = self._engine.step(xs.to(self.device, non_blocking=True))[0].tolist()   # one D2H per chunk
         self.encoder_elapsed.append(time.time() - start)
         tokens = []
@@ -114,3 +144,19 @@ class PytorchStreamDecoder(StreamTransducerDecoder):
                 seq = self.tokenizer.tokenizer.id_to_token(pred)
                 tokens.append(seq.replace('</w>', ' '))
         return "".join(tokens)
+
+    def _text(self, ids):
+        tokens = []
+        for pred in ids:
+            self.decoder_elapsed.append(0.0)
+            tokens.append(self.tokenizer.tokenizer.id_to_token(pred).replace('</w>', ' '))
+        return "".join(tokens)
+
+    @torch.no_grad()
+    def flush(self):
+        """Beam search: the text of the best hypothesis' tokens not yet returned by ``decode``; decoding continues
+        from that hypothesis.  Greedy decoding returns every token at once, so there is nothing to flush: ""."""
+        if self._beam is None or self._engine is None:
+            return ""
+        ids, counts, _ = self._engine.flush()
+        return self._text(ids[0, :int(counts[0])].tolist())

@@ -18,8 +18,9 @@ import torch
 from ._lib import lib, check
 from .rnnt.tokenizer import NUL, BOS, UNK
 
-PH_LN, PH_PAIR, PH_LSTM, PH_LINEAR, PH_ARGMAX, PH_COPY, PH_BEAM_SELECT, PH_GATHER, PH_BEAM_FINAL = range(9)
-F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE, F_LM = 1, 2, 4, 8, 16, 32
+PH_LN, PH_PAIR, PH_LSTM, PH_LINEAR, PH_ARGMAX, PH_COPY, PH_BEAM_SELECT, PH_GATHER, PH_BEAM_FINAL, PH_BEAM_COMMIT = \
+    range(10)
+F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE, F_LM, F_STREAM, F_FLUSH = 1, 2, 4, 8, 16, 32, 64, 128
 BEAM_MAX_W = 1024                                     # EB_BEAM_MAX_W
 
 
@@ -152,30 +153,106 @@ def param_fingerprint(module):
     return tuple(p.data_ptr() for p in module.parameters())
 
 
+def _check_lstm_encoder(enc, who):
+    from .rnnt.models import ResLayerNormLSTM
+    if not isinstance(enc.lstm, ResLayerNormLSTM):
+        # the decode program's encoder phases are LSTM cells (4H-row weights); a GRU stack has 3H rows
+        raise ValueError("%s streams an LSTM encoder only, got %s" % (who, type(enc.lstm).__name__))
+
+
+def _odd_chunk():
+    return ValueError("streaming chunks must hold an even number of frames before each time reduction "
+                      "(cli/export_onnx.py:20-21 asserts the same)")
+
+
+def stream_frames_out(enc, n):
+    """Encoder output frames of a streaming chunk of n input frames; ValueError when a time reduction meets an odd
+    count.  Touches no device."""
+    for i in range(len(enc.lstm.lstms)):
+        if i in enc.lstm.time_reductions:
+            if n % 2:
+                raise _odd_chunk()
+            n //= 2
+    return n
+
+
+def encoder_phases(prog, engine, enc, S, n):
+    """Append the stateful streaming encoder for S streams and chunks of n log-mel frames to the phase list ``prog``:
+    LayerNorm of the input, then per layer n LSTM cell steps from the carried (h, c), the residual LayerNorm and the
+    time reduction, then the projection.  Allocates on ``engine`` (whose ``dev`` is set) the chunk input ``xin``
+    [S, n, F], the carried state ``enc_h`` / ``enc_c`` [L, S, H] (with ``enc_htmp``, the last step's h, copied into
+    enc_h by the caller's final phase) and the output ``enc_out`` [S, n_out, E]; sets ``engine.n_out``."""
+    lstms = list(enc.lstm.lstms)
+    L = len(lstms)
+    H = enc.lstm.hidden_size
+    F = enc.norm.weight.shape[0]
+    reductions = enc.lstm.time_reductions
+    z = lambda *shape: torch.zeros(*shape, dtype=torch.float32, device=engine.dev)
+    engine.xin, engine.a0 = z(S, n, F), z(S, n, F)
+    engine.enc_h, engine.enc_c, engine.enc_htmp = z(L, S, H), z(L, S, H), z(L, S, H)
+
+    def ph(**kw):
+        p = EbPhase()
+        for k, v in kw.items():
+            setattr(p, k, v)
+        prog.append(p)
+
+    ph(type=PH_LN, S=S * n, N=F, x1=_ptr(engine.xin), ldx1=F, w1=_ptr(enc.norm.weight), b1=_ptr(enc.norm.bias),
+       y=_ptr(engine.a0), ldy=F)
+    X, I, ni = engine.a0, F, n
+    engine._bufs = []
+    for i, (cell, post) in enumerate(zip(lstms, enc.lstm.projs)):
+        yL, zL = z(S, ni, H), z(S, ni, H)
+        engine._bufs += [yL, zL]
+        for t in range(ni):
+            ph(type=PH_LSTM, S=S, N=H, K1=I, K2=H, x1=_ptr(X, t * I), ldx1=ni * I,
+               x2=_ptr(engine.enc_h[i]) if t == 0 else _ptr(yL, (t - 1) * H), ldx2=H if t == 0 else ni * H,
+               w1=_ptr(cell.weight_ih_l0), ldw1=I, w2=_ptr(cell.weight_hh_l0), ldw2=H,
+               b1=_ptr(cell.bias_ih_l0), b2=_ptr(cell.bias_hh_l0), c=_ptr(engine.enc_c[i]),
+               y=_ptr(yL, t * H), ldy=ni * H, y2=_ptr(engine.enc_htmp[i]) if t == ni - 1 else None)
+        ln = post[0]
+        ph(type=PH_LN, S=S * ni, N=H, x1=_ptr(yL), ldx1=H, x2=_ptr(X) if i > 0 else None, ldx2=H,
+           w1=_ptr(ln.weight), b1=_ptr(ln.bias), y=_ptr(zL), ldy=H)
+        X, I = zL, H
+        if i in reductions:
+            if ni % 2:
+                raise _odd_chunk()
+            zr = z(S, ni // 2, H)
+            engine._bufs.append(zr)
+            ph(type=PH_PAIR, S=S, N=H, aux=ni, x1=_ptr(zL), y=_ptr(zr))
+            X, ni = zr, ni // 2
+    engine.n_out = ni
+    E = enc.proj.weight.shape[0] if enc.has_proj else H
+    if enc.has_proj:
+        engine.enc_out = z(S, ni, E)
+        ph(type=PH_LINEAR, S=S * ni, N=E, K1=H, x1=_ptr(X), ldx1=H, w1=_ptr(enc.proj.weight), ldw1=H,
+           b1=_ptr(enc.proj.bias), y=_ptr(engine.enc_out), ldy=E)
+    else:
+        engine.enc_out = X
+    return E
+
+
+def _upload(prog, dev):
+    arr = (EbPhase * len(prog))(*prog)
+    return torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(dev)
+
+
 class StreamEngine:
     STATE = ("enc_h", "enc_c", "dec_h", "dec_c", "dec_x", "tok")
 
     def __init__(self, transducer, n_streams, frames_per_chunk, unk_id=UNK, blank=NUL, max_ctas=0, state=None):
         assert C.sizeof(EbPhase) == lib().eb_decode_phase_size(), "EbPhase layout mismatch"
         enc, dec, joint = transducer.encoder, transducer.decoder, transducer.joint.joint
-        from .rnnt.models import ResLayerNormLSTM
-        if not isinstance(enc.lstm, ResLayerNormLSTM):
-            # the decode program's encoder phases are LSTM cells (4H-row weights); a GRU stack has 3H rows
-            raise ValueError("StreamEngine streams an LSTM encoder only, got %s" % type(enc.lstm).__name__)
+        _check_lstm_encoder(enc, "StreamEngine")
         self.dev = enc.norm.weight.device
         if self.dev.type != "cuda":
             raise RuntimeError("StreamEngine needs the model on a CUDA device")
         f32 = torch.float32
         S, n = n_streams, frames_per_chunk
         self.S, self.n, self.blank, self.unk, self.max_ctas = S, n, blank, unk_id, max_ctas
-        lstms = list(enc.lstm.lstms)
-        L = len(lstms)
+        L = len(enc.lstm.lstms)
         H = enc.lstm.hidden_size
-        F = enc.norm.weight.shape[0]
-        reductions = enc.lstm.time_reductions
         z = lambda *shape: torch.zeros(*shape, dtype=f32, device=self.dev)
-        self.xin, self.a0 = z(S, n, F), z(S, n, F)
-        self.enc_h, self.enc_c, self.enc_htmp = z(L, S, H), z(L, S, H), z(L, S, H)
         self._keep = [p.detach() for p in transducer.parameters()]      # weights are read in place
         self.fingerprint = param_fingerprint(transducer)
         prog = []
@@ -186,39 +263,8 @@ class StreamEngine:
                 setattr(p, k, v)
             prog.append(p)
 
-        ph(type=PH_LN, S=S * n, N=F, x1=_ptr(self.xin), ldx1=F, w1=_ptr(enc.norm.weight), b1=_ptr(enc.norm.bias),
-           y=_ptr(self.a0), ldy=F)
-        X, I, ni = self.a0, F, n
-        self._bufs = []
-        for i, (cell, post) in enumerate(zip(lstms, enc.lstm.projs)):
-            yL, zL = z(S, ni, H), z(S, ni, H)
-            self._bufs += [yL, zL]
-            for t in range(ni):
-                ph(type=PH_LSTM, S=S, N=H, K1=I, K2=H, x1=_ptr(X, t * I), ldx1=ni * I,
-                   x2=_ptr(self.enc_h[i]) if t == 0 else _ptr(yL, (t - 1) * H), ldx2=H if t == 0 else ni * H,
-                   w1=_ptr(cell.weight_ih_l0), ldw1=I, w2=_ptr(cell.weight_hh_l0), ldw2=H,
-                   b1=_ptr(cell.bias_ih_l0), b2=_ptr(cell.bias_hh_l0), c=_ptr(self.enc_c[i]),
-                   y=_ptr(yL, t * H), ldy=ni * H, y2=_ptr(self.enc_htmp[i]) if t == ni - 1 else None)
-            ln = post[0]
-            ph(type=PH_LN, S=S * ni, N=H, x1=_ptr(yL), ldx1=H, x2=_ptr(X) if i > 0 else None, ldx2=H,
-               w1=_ptr(ln.weight), b1=_ptr(ln.bias), y=_ptr(zL), ldy=H)
-            X, I = zL, H
-            if i in reductions:
-                if ni % 2:
-                    raise ValueError("streaming chunks must hold an even number of frames before each time "
-                                     "reduction (cli/export_onnx.py:20-21 asserts the same)")
-                zr = z(S, ni // 2, H)
-                self._bufs.append(zr)
-                ph(type=PH_PAIR, S=S, N=H, aux=ni, x1=_ptr(zL), y=_ptr(zr))
-                X, ni = zr, ni // 2
-        self.n_out = ni
-        E = enc.proj.weight.shape[0] if enc.has_proj else H
-        if enc.has_proj:
-            self.enc_out = z(S, ni, E)
-            ph(type=PH_LINEAR, S=S * ni, N=E, K1=H, x1=_ptr(X), ldx1=H, w1=_ptr(enc.proj.weight), ldw1=H,
-               b1=_ptr(enc.proj.bias), y=_ptr(self.enc_out), ldy=E)
-        else:
-            self.enc_out = X
+        E = encoder_phases(prog, self, enc, S, n)
+        ni = self.n_out
         # ---- predictor + joint state
         Ld, Hd = dec.lstm.num_layers, dec.lstm.hidden_size
         D = dec.proj.weight.shape[0]
@@ -481,3 +527,268 @@ class BeamEngine:
         check(lib().eb_decode_run(self._prog.data_ptr(), self.nphase, self._bar.data_ptr(), self.max_ctas,
                                   torch.cuda.current_stream().cuda_stream), "eb_decode_run")
         return self.ids, self.nlogp
+
+
+class StreamBeamEngine:
+    """Streaming beam search: S streams of W hypotheses each, carried from one chunk to the next, one persistent kernel
+    launch per chunk.  The chunk program runs StreamEngine's stateful encoder, then per encoder output frame exactly
+    BeamEngine's frame (joint, BEAM_SELECT, GATHER, masked predictor and LM steps, with or without LM fusion), so how
+    the audio is cut into chunks does not change which hypotheses survive.  Row r = s*W + slot.
+
+    After the chunk's last frame BEAM_COMMIT commits each stream's longest common prefix of its live hypotheses' token
+    sequences: no later frame can change it, so it is final and ``step`` returns it while audio is still arriving.
+    Each slot stores only its uncommitted suffix, at most ``max_pending`` tokens.  If after the commit a live suffix
+    holds more than ``max_pending - n_out`` tokens (a chunk adds at most n_out), the beam collapses: the best live
+    slot (highest log p, lowest slot on ties) commits its whole suffix and becomes slot 0, the only live slot, with its
+    log p, predictor state and LM state.  ``flush()`` is that collapse done unconditionally.
+
+    The beam state (slot log p, token sequences, live counts, predictor and LM states) lives in the parity-0 buffers
+    between launches, whatever the parity of n_out: the chunk-end phases read the other parity (copied there first
+    when n_out is even, since GATHER is not in-place safe) and write parity 0.  ``state()`` / ``load_state()`` carry
+    it to an engine rebuilt for another chunk length or re-homed weights.  The carried beam was bounded for the old
+    n_out; load_state runs the chunk-end rule once with the new bound (a longer chunk may need a collapse) and the
+    tokens that commits come first in the next ``step``'s output.
+
+    The reference's ``<unk>`` rule (re-argmax when the argmax is ``<unk>``) is a device of the greedy loop; the beam,
+    like Transducer.beam_search, does not apply it."""
+
+    def __init__(self, transducer, n_streams, frames_per_chunk, W, merge=True, lm=None, lm_weight=0.0,
+                 length_bonus=0.0, lm_bos=1, lm_token_map=None, max_pending=64, state=None, blank=NUL, max_ctas=0):
+        W = operator.index(W)
+        if not 1 <= W <= BEAM_MAX_W:
+            raise ValueError("beam width must be in [1, %d], got %r" % (BEAM_MAX_W, W))
+        V = transducer.joint.joint[2].weight.shape[0]
+        fusion = check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map)
+        enc, dec, joint = transducer.encoder, transducer.decoder, transducer.joint.joint
+        _check_lstm_encoder(enc, "StreamBeamEngine")
+        S, n, P = operator.index(n_streams), operator.index(frames_per_chunk), operator.index(max_pending)
+        if S < 1 or n < 1:
+            raise ValueError("n_streams and frames_per_chunk must be positive, got %d and %d" % (S, n))
+        T = stream_frames_out(enc, n)
+        if T < 1:
+            raise ValueError("a chunk of %d frames gives no encoder output frame" % n)
+        if P < T:
+            raise ValueError("max_pending (%d) must be at least the encoder frames per chunk (%d): a chunk can add "
+                             "that many tokens to a hypothesis" % (P, T))
+        assert C.sizeof(EbPhase) == lib().eb_decode_phase_size(), "EbPhase layout mismatch"
+        self.dev = enc.norm.weight.device
+        if self.dev.type != "cuda":
+            raise RuntimeError("StreamBeamEngine needs the model on a CUDA device")
+        f32, i32 = torch.float32, torch.int32
+        R, LS = S * W, P + 3
+        self.S, self.n, self.W, self.merge, self.blank, self.max_ctas, self.max_pending = S, n, W, merge, blank, \
+            max_ctas, P
+        z = lambda *shape, dtype=f32: torch.zeros(*shape, dtype=dtype, device=self.dev)
+        self._keep = [p.detach() for p in transducer.parameters()]      # weights are read in place
+        self.fingerprint = param_fingerprint(transducer)
+        L, H = len(enc.lstm.lstms), enc.lstm.hidden_size
+        prog = []
+        E = encoder_phases(prog, self, enc, S, n)
+        assert self.n_out == T
+        Ld, Hd = dec.lstm.num_layers, dec.lstm.hidden_size
+        D = dec.proj.weight.shape[0]
+        J = joint[0].weight.shape[0]
+        st = [z(2 * Ld, R, Hd), z(2 * Ld, R, Hd)]              # [h of every layer | c of every layer], per parity
+        self.dec_h, self.dec_c = [s[:Ld] for s in st], [s[Ld:] for s in st]
+        self.dec_x = [z(R, D), z(R, D)]
+        self.dec_htmp, self.hidden, self.logits = z(Ld, R, Hd), z(R, J), z(R, V)
+        self.tok, self.src, self.logp = z(R, dtype=i32), z(R, dtype=i32), z(R)
+        self.frames = torch.full((S,), T, dtype=i32, device=self.dev)      # a stream never freezes
+        self.seqs = z(2, R, LS, dtype=i32)     # {suffix length, hash lo, hash hi, tokens since the last commit}
+        nh = S * T * W
+        self.hist = z(3 * nh + S * T, dtype=i32)
+        self.hist_live = self.hist[3 * nh:].view(S, T)        # column T-1 carries the live count between launches
+        self._out = z(S * P + 2 * S, dtype=i32)               # committed ids [S, P] | counts [S] | collapsed [S]
+        self._host = torch.zeros(self._out.shape, dtype=i32).pin_memory()
+        self.n_collapses = 0
+        self._st, self._lst = st, None
+        prime = []
+        _dec_phases(prime, dec, R, self.dec_h[0], self.dec_c[0], self.dec_htmp, self.dec_x[0], self.tok, blank,
+                    masked=False)
+        self.lm = fusion is not None
+        if self.lm:
+            lsd, lw, lb, self.lm_bos, tmap = fusion
+            lsd = {k: v.to(self.dev, f32).contiguous() for k, v in lsd.items()}
+            self._keep += list(lsd.values())
+            Ll = (len(lsd) - 3) // 4
+            lm_layers = [tuple(lsd["rnn.%s_l%d" % (nm, k)] for nm in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"))
+                         for k in range(Ll)]
+            Hl, ntok = lm_layers[0][1].shape[1], lsd["encoder.weight"].shape[0]
+            self._lst = [z(2 * Ll, R, Hl), z(2 * Ll, R, Hl)]
+            self.lm_h, self.lm_c = [s[:Ll] for s in self._lst], [s[Ll:] for s in self._lst]
+            self.lm_htmp, self.lm_logits, self.lm_tok = z(Ll, R, Hl), z(R, ntok), z(R, dtype=i32)
+            self._lm_logits_tmp = z(R, ntok)
+            self.lm_map = tmap.to(self.dev, i32)
+            self.lm_fuse = torch.tensor([lw, lb], dtype=f32, device=self.dev)
+
+            def lm_phases(pr, q, masked):
+                predictor_phases(pr, lsd["encoder.weight"], lm_layers, lsd["decoder.weight"], lsd["decoder.bias"],
+                                 R, self.lm_h[q], self.lm_c[q], self.lm_htmp, self.lm_logits, self.lm_tok, -1, masked)
+            lm_phases(prime, 0, masked=False)
+        w1 = joint[0].weight
+        for t in range(T):
+            p, q = t & 1, 1 - (t & 1)
+            prog.append(EbPhase(type=PH_LINEAR, S=R, N=J, flags=F_TANH, K1=E, x1=_ptr(self.enc_out, t * E), ldx1=T * E,
+                                x1_div=W, w1=_ptr(w1), ldw1=E + D, K2=D, x2=_ptr(self.dec_x[p]), ldx2=D,
+                                w2=_ptr(w1, E), ldw2=E + D, b1=_ptr(joint[0].bias), y=_ptr(self.hidden), ldy=J))
+            prog.append(EbPhase(type=PH_LINEAR, S=R, N=V, K1=J, x1=_ptr(self.hidden), ldx1=J,
+                                w1=_ptr(joint[2].weight), ldw1=J, b1=_ptr(joint[2].bias), y=_ptr(self.logits), ldy=V))
+            sel = EbPhase(type=PH_BEAM_SELECT, S=S, N=V, aux=W, aux2=blank, flags=F_STREAM | (F_MERGE if merge else 0),
+                          K1=LS, x1=_ptr(self.logits), ldx1=V, y=_ptr(self.logp), tok_in=_ptr(self.frames),
+                          tok_out=_ptr(self.tok), src=_ptr(self.src), hist=_ptr(self.hist), hist_ld=T,
+                          hist_col=t, seq_in=_ptr(self.seqs[p]), seq_out=_ptr(self.seqs[q]))
+            if self.lm:
+                sel.flags |= F_LM
+                sel.x2, sel.ldx2, sel.K2 = _ptr(self.lm_logits), ntok, ntok
+                sel.fuse, sel.tok_map, sel.tok_out2 = _ptr(self.lm_fuse), _ptr(self.lm_map), _ptr(self.lm_tok)
+            prog.append(sel)
+            prog.append(EbPhase(type=PH_GATHER, S=R, N=Hd, aux=2 * Ld, x1=_ptr(st[p]), y=_ptr(st[q]), K2=D,
+                                x2=_ptr(self.dec_x[p]), y2=_ptr(self.dec_x[q]), src=_ptr(self.src)))
+            if self.lm:
+                prog.append(EbPhase(type=PH_GATHER, S=R, N=Hl, aux=2 * Ll, x1=_ptr(self._lst[p]),
+                                    y=_ptr(self._lst[q]), src=_ptr(self.src)))
+            _dec_phases(prog, dec, R, self.dec_h[q], self.dec_c[q], self.dec_htmp, self.dec_x[q], self.tok, blank,
+                        masked=True)
+            if self.lm:
+                lm_phases(prog, q, masked=True)
+
+        def chunk_end(pr, in_parity0, flush):
+            """commit (and collapse) from parity 1 into parity 0; state found in parity 0 is copied over first"""
+            if in_parity0:
+                pr.append(EbPhase(type=PH_COPY, S=2 * Ld * R, N=Hd, x1=_ptr(st[0]), y=_ptr(st[1])))
+                pr.append(EbPhase(type=PH_COPY, S=R, N=D, x1=_ptr(self.dec_x[0]), y=_ptr(self.dec_x[1])))
+                pr.append(EbPhase(type=PH_COPY, S=R, N=LS, x1=_ptr(self.seqs[0]), y=_ptr(self.seqs[1])))
+                if self.lm:
+                    pr.append(EbPhase(type=PH_COPY, S=2 * Ll * R, N=Hl, x1=_ptr(self._lst[0]), y=_ptr(self._lst[1])))
+            if self.lm:
+                pr.append(EbPhase(type=PH_COPY, S=R, N=ntok, x1=_ptr(self.lm_logits), y=_ptr(self._lm_logits_tmp)))
+            pr.append(EbPhase(type=PH_BEAM_COMMIT, S=S, N=P, aux=W, aux2=P - T, K1=LS, flags=F_FLUSH if flush else 0,
+                              y=_ptr(self.logp), hist=_ptr(self.hist), hist_ld=T, seq_in=_ptr(self.seqs[1]),
+                              seq_out=_ptr(self.seqs[0]), tok_out=_ptr(self._out), tok_out2=_ptr(self._out, S * P),
+                              src=_ptr(self.src)))
+            pr.append(EbPhase(type=PH_GATHER, S=R, N=Hd, aux=2 * Ld, x1=_ptr(st[1]), y=_ptr(st[0]), K2=D,
+                              x2=_ptr(self.dec_x[1]), y2=_ptr(self.dec_x[0]), src=_ptr(self.src)))
+            if self.lm:
+                pr.append(EbPhase(type=PH_GATHER, S=R, N=Hl, aux=2 * Ll, x1=_ptr(self._lst[1]), y=_ptr(self._lst[0]),
+                                  K2=ntok, x2=_ptr(self._lm_logits_tmp), y2=_ptr(self.lm_logits), src=_ptr(self.src)))
+
+        chunk_end(prog, T % 2 == 0, flush=False)
+        prog.append(EbPhase(type=PH_COPY, S=L * S, N=H, x1=_ptr(self.enc_htmp), y=_ptr(self.enc_h)))
+        flush, rebound = [], []
+        chunk_end(flush, True, flush=True)
+        chunk_end(rebound, True, flush=False)          # a loaded beam under this engine's bound, max_pending - n_out
+        self.n_chunk_phases, self.n_prime_phases, self.n_flush_phases = len(prog), len(prime), len(flush)
+        self._chunk, self._prime, self._flush = _upload(prog, self.dev), _upload(prime, self.dev), \
+            _upload(flush, self.dev)
+        self._rebound, self.n_rebound_phases = _upload(rebound, self.dev), len(rebound)
+        self._bar = torch.zeros(64, dtype=torch.int32, device=self.dev)
+        self._unreturned = (torch.zeros(S, 0, dtype=i32), torch.zeros(S, dtype=i32))
+        if state is None:
+            self.reset()
+        else:
+            self.load_state(state)
+
+    def _state_views(self):
+        v = dict(enc_h=self.enc_h, enc_c=self.enc_c, dec_state=self._st[0], dec_x=self.dec_x[0], logp=self.logp,
+                 seqs=self.seqs[0], live=self.hist_live[:, -1])
+        if self.lm:
+            v.update(lm_state=self._lst[0], lm_logits=self.lm_logits)
+        return v
+
+    def state(self):
+        """Every stream's encoder state and beam (slot log p, stored token suffixes, live count, predictor and LM
+        states), as a dict of tensors, with the committed tokens not yet returned by ``step`` (host ids [S, K] and
+        counts [S])."""
+        st = {k: t.clone() for k, t in self._state_views().items()}
+        st["unreturned_ids"], st["unreturned_counts"] = (t.clone() for t in self._unreturned)
+        return st
+
+    @torch.no_grad()
+    def load_state(self, st):
+        """Continue from ``state()`` of an engine over the same model, LM, n_streams, W and max_pending, with any
+        chunk length.  The previous engine bounded every stored suffix by max_pending minus ITS n_out; when this
+        engine's chunks yield more encoder frames, that bound is too loose, so the chunk-end commit and collapse rule
+        runs once here with this engine's bound.  The tokens it commits are returned by the next ``step``."""
+        views = self._state_views()
+        carried = ("unreturned_ids", "unreturned_counts")
+        if set(st) != set(views) | set(carried):
+            raise ValueError("state keys %s do not match this engine's %s (same model, LM use, n_streams, W and "
+                             "max_pending are needed)" % (sorted(st), sorted(set(views) | set(carried))))
+        for k, t in views.items():
+            if tuple(st[k].shape) != tuple(t.shape):
+                raise ValueError("state %s has shape %s, this engine needs %s (same n_streams, W and max_pending)"
+                                 % (k, tuple(st[k].shape), tuple(t.shape)))
+            t.copy_(st[k])
+        self._unreturned = tuple(st[k].to("cpu", torch.int32) for k in carried)
+        self._run(self._rebound, self.n_rebound_phases)
+        ids, counts, collapsed = self._fetch()
+        self.n_collapses += int(collapsed.sum())
+        self._add_unreturned(ids, counts)
+
+    def _add_unreturned(self, ids, counts):
+        """Append committed tokens (ids [S, K], counts [S]) to those not yet returned."""
+        uids, ucounts = self._unreturned
+        n = ucounts + counts
+        out = torch.zeros(self.S, int(n.max()), dtype=torch.int32)
+        for s in range(self.S):
+            a, b = int(ucounts[s]), int(counts[s])
+            out[s, :a] = uids[s, :a]
+            out[s, a:a + b] = ids[s, :b]
+        self._unreturned = (out, n)
+
+    def _take(self, ids, counts):
+        """The tokens just committed, after any committed earlier and not yet returned."""
+        if int(self._unreturned[1].max()) > 0:
+            self._add_unreturned(ids, counts)
+            ids, counts = self._unreturned
+            self._unreturned = (ids[:, :0].clone(), torch.zeros_like(counts))
+        return ids, counts
+
+    def _run(self, prog, nphase):
+        check(lib().eb_decode_run(prog.data_ptr(), nphase, self._bar.data_ptr(), self.max_ctas,
+                                  torch.cuda.current_stream().cuda_stream), "eb_decode_run")
+
+    def _fetch(self):
+        S, P = self.S, self.max_pending
+        self._host.copy_(self._out, non_blocking=True)       # the chunk's only device-to-host copy
+        torch.cuda.current_stream().synchronize()
+        return self._host[:S * P].view(S, P).clone(), self._host[S * P:S * P + S].clone(), \
+            self._host[S * P + S:].clone()
+
+    @torch.no_grad()
+    def reset(self):
+        """Every stream starts a new utterance: zero encoder state, one live slot of log p 0 with the empty sequence,
+        predictor primed with <bos> and the LM with lm_bos from zeros."""
+        for t in (self.enc_h, self.enc_c, self._st[0], self.seqs[0]):
+            t.zero_()
+        self.logp.fill_(float("-inf"))
+        self.logp.view(self.S, self.W)[:, 0] = 0.0
+        self.hist_live[:, -1] = 1
+        self._unreturned = (torch.zeros(self.S, 0, dtype=torch.int32), torch.zeros(self.S, dtype=torch.int32))
+        self.tok.fill_(BOS)
+        if self.lm:
+            self._lst[0].zero_()
+            self.lm_tok.fill_(self.lm_bos)
+        self._run(self._prime, self.n_prime_phases)
+
+    @torch.no_grad()
+    def step(self, chunk):
+        """chunk [S, n, F] log-mel frames (device or pinned host) -> (committed ids int32 [S, K], counts int32 [S]) on
+        the host: row s holds in its first counts[s] entries the tokens stream s committed in this chunk.  K is
+        max_pending, or more on the first step after load_state had to commit carried tokens (they come first).
+        ``n_collapses`` counts the forced collapses so far."""
+        self.xin.copy_(chunk, non_blocking=True)
+        self._run(self._chunk, self.n_chunk_phases)
+        ids, counts, collapsed = self._fetch()
+        self.n_collapses += int(collapsed.sum())
+        return self._take(ids, counts)
+
+    @torch.no_grad()
+    def flush(self):
+        """Collapse every stream's beam to its best hypothesis and commit all of that hypothesis' remaining tokens;
+        decoding continues from it.  -> (ids int32 [S, K], counts int32 [S] as from ``step``, -log p [S] of the best
+        hypothesis, the negated fused score with an LM), on the host."""
+        self._run(self._flush, self.n_flush_phases)
+        ids, counts, _ = self._fetch()
+        ids, counts = self._take(ids, counts)
+        return ids, counts, -self.logp.view(self.S, self.W)[:, 0].cpu()

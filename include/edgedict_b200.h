@@ -200,7 +200,7 @@ int eb_joint_dpre_reduce(const void* dpre16, float* dep, float* ddp, int B, int 
  * replaces PytorchStreamDecoder.decode's Python loop (rnnt/stream.py:93-120).  The host builds a
  * phase program once (edgedict_b200/stream_engine.py) and launches it per chunk; see decode.cu. */
 enum { EB_PH_LN = 0, EB_PH_PAIR = 1, EB_PH_LSTM = 2, EB_PH_LINEAR = 3, EB_PH_ARGMAX = 4, EB_PH_COPY = 5,
-       EB_PH_BEAM_SELECT = 6, EB_PH_GATHER = 7, EB_PH_BEAM_FINAL = 8 };
+       EB_PH_BEAM_SELECT = 6, EB_PH_GATHER = 7, EB_PH_BEAM_FINAL = 8, EB_PH_BEAM_COMMIT = 9 };
 typedef struct EbPhase {
     int32_t type, S, K1, K2, N, flags, ldx1, ldx2, ldw1, ldw2, ldy, aux, aux2, hist_ld, hist_col, x1_div;
     const float *x1, *x2, *w1, *w2, *b1, *b2;
@@ -223,6 +223,15 @@ typedef struct EbPhase {
  *            the LM logits of each slot, fuse = {lm_weight, length_bonus} on the device, tok_map [N] maps a token to
  *            its LM token (-1: not scored by the LM), and tok_out2 [B*W] receives each new slot's LM token (-1 when the
  *            LM does not step: blank, unmapped, empty slot or frozen utterance).
+ *       64 = BEAM_SELECT streams: the beam carries over from the previous launch (live count at t = 0 read from the
+ *            last history column, hist_live[b, hist_ld - 1]) and the token-sequence rows have stride K1 (max_pending + 3)
+ *            and hold only the tokens since the stream's last commit (length = that count; the hash still covers the
+ *            whole sequence).  The offline beam search does not set it.
+ *      128 = BEAM_COMMIT collapses every stream's beam to its best slot unconditionally (a flush).
+ * BEAM_COMMIT (streaming beam, after a chunk's last frame, one CTA per stream): commits the common prefix of the live
+ * slots' stored suffixes to tok_out [S, N] with the count in tok_out2[s] (tok_out2[S + s] = 1 when the beam collapsed),
+ * shifts the suffixes left into seq_out, and, when a suffix still exceeds aux2 tokens or on flags 128, collapses the beam
+ * to its best slot; src receives the gather sources that move the kept slots' state into place.
  * x1_div (LINEAR): row r of x1 is x1[r / x1_div] (0 or 1: row r), the encoder frame a beam's W rows share.
  * Beam search (batched, W slots per utterance, row r = b*W + slot; see decode.cu for the field use of each phase):
  * at most EB_BEAM_MAX_W slots per utterance. */
