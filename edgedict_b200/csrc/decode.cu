@@ -12,8 +12,11 @@
 //           x rows may come from an embedding table indexed by the last token, and the update can
 //           be masked per stream (predictor advances only on non-blank, stream.py:111-116)
 //   LINEAR  y = act(x1 W1^T (+ x2 W2^T) + b)         Linear / joint (models.py:129,148,163-167)
-//   ARGMAX  token = argmax(logits) with the <unk> rule (stream.py:105-108: logit := 0, re-argmax)
+//   ARGMAX  token = argmax(logits) with the <unk> rule (stream.py:105-108: logit := 0, re-argmax); with flags 256 (a
+//           continuation round of a multi-symbol frame) rows whose tok_out already holds blank stay blank
 //   COPY    y = x
+//   SKIP    if no row of tok_in[0..S) differs from aux2 (blank), jump over the next aux phases: a frame's round j >= 1
+//           costs one read of S ints per CTA when no row is still emitting (greedy decoding with max_symbols > 1)
 //   BEAM_SELECT  per utterance: log-softmax of its W rows, exact top-W of the live slots' candidates, merge of equal
 //           token sequences, new slot log p / tokens / gather sources / history (Transducer.beam_search, one frame);
 //           optionally with an LSTM language model's log-probs fused into the candidate values (shallow fusion)
@@ -317,8 +320,14 @@ __device__ __forceinline__ bool argmax_before(float v, int i, float b, int bi) {
 
 __device__ void phase_argmax(const EbPhase& p) {
     const int lane = threadIdx.x & 31, V = p.N, blank = p.aux, unk = p.aux2;
-    (void)blank;
+    const bool cont = p.flags & 256;
     for (int s = blockIdx.x * 8 + (threadIdx.x >> 5); s < p.S; s += gridDim.x * 8) {
+        // continuation round of a multi-symbol frame (flags 256): a row whose frame already ended on blank stays blank,
+        // takes no argmax and adds no log p; its masked predictor phases then leave it untouched
+        if (cont && __ldcg(p.tok_out + s) == blank) {
+            if (lane == 0 && p.hist) p.hist[(long)s * p.hist_ld + p.hist_col] = blank;
+            continue;
+        }
         const float* x = p.x1 + (long)s * p.ldx1;
         int pred = -1;
         for (int pass = 0; pass < 2; ++pass) {
@@ -802,6 +811,14 @@ __device__ __noinline__ void phase_beam_final(const EbPhase& p) {
     }
 }
 
+// SKIP: does any row of tok_in[0..S) differ from aux2 (blank)?  tok_in is final at the preceding grid barrier, so every
+// thread of every CTA gets the same answer.
+__device__ __noinline__ bool phase_skip_live(const EbPhase& p) {
+    int live = 0;
+    for (int s = threadIdx.x; s < p.S; s += blockDim.x) live |= __ldcg(p.tok_in + s) != p.aux2;
+    return __syncthreads_or(live);
+}
+
 // the phase loader copies the struct as 32-bit words, one per thread of the 256-thread CTA
 static_assert(sizeof(EbPhase) % 4 == 0 && sizeof(EbPhase) / 4 <= 256, "EbPhase loader");
 
@@ -810,11 +827,15 @@ __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __re
     float* red = dsm;                                        // [8 warps][2048]
     float* outs = dsm + RED_FLOATS;                          // [64][33]
     __shared__ EbPhase ph;
+    // the next phase index lives in shared memory: a loop-carried register that SKIP could change costs the matrix
+    // phases (compiled at the 255-register cap) extra spills
+    __shared__ int next;
     unsigned epoch = 0;
-    for (int i = 0; i < nphase; ++i) {
+    for (int i = 0; i < nphase; i = next) {
         __syncthreads();
         if (threadIdx.x < sizeof(EbPhase) / 4)
             reinterpret_cast<int*>(&ph)[threadIdx.x] = reinterpret_cast<const int*>(prog + i)[threadIdx.x];
+        if (threadIdx.x == 0) next = i + 1;
         __syncthreads();
         const long gtid = (long)blockIdx.x * blockDim.x + threadIdx.x, gn = (long)gridDim.x * blockDim.x;
         switch (ph.type) {
@@ -839,10 +860,19 @@ __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __re
             case EB_PH_GATHER: phase_gather(ph); break;
             case EB_PH_BEAM_FINAL: phase_beam_final(ph); break;
             case EB_PH_BEAM_COMMIT: phase_beam_commit(ph, dsm); break;
+            case EB_PH_SKIP:
+                // writes nothing, so it takes no grid barrier (and no epoch) of its own, and neither do the phases it
+                // skips: every CTA counts the same barriers
+                if (!phase_skip_live(ph) && threadIdx.x == 0) next = i + 1 + ph.aux;
+                __syncthreads();                             // every thread reads the same next
+                continue;
             default: break;
         }
         ++epoch;
         if (i + 1 < nphase) grid_sync(bar, epoch * gridDim.x);
+        // redundant after grid_sync, but it costs nothing beside the grid barrier, and with it ptxas keeps this kernel's
+        // spills at 12 / 16 bytes (stores / loads); without it they grow to 20 / 28
+        __syncthreads();
     }
 }
 

@@ -300,23 +300,29 @@ class Transducer(nn.Module):
         return loss
 
     @torch.no_grad()
-    def greedy_decode(self, xs, xlen):
+    def greedy_decode(self, xs, xlen, max_symbols=1):
         """rnnt/models.py:243-269: at most one symbol per encoder frame; returns (list of id arrays
         incl. blanks, truncated by the UNSCALED xlen as the reference does, -sum log p).  The T'
-        per-frame iterations run device-side in one persistent kernel (stream_engine.GreedyEngine)."""
-        from ..stream_engine import GreedyEngine, param_fingerprint
+        per-frame iterations run device-side in one persistent kernel (stream_engine.GreedyEngine).
+
+        ``max_symbols`` = K (1 to 16) lets a frame emit up to K symbols, as the RNN-T lattice allows: the frame repeats
+        joint -> argmax -> predictor step until a blank or K non-blank tokens.  Each array then holds K entries per
+        frame (blank for rounds not taken) for the first xlen frames, and log p sums every round taken.  K = 1 is the
+        reference's decode, bit for bit."""
+        from ..stream_engine import GreedyEngine, check_max_symbols, param_fingerprint
+        K = check_max_symbols(max_symbols)
         h_enc, _ = self.encoder(xs)
         B, T = h_enc.shape[0], h_enc.shape[1]
         # the phase program bakes raw weight pointers: re-homed parameters (FlatAdam, .to(), .float()) rebuild it
-        key = (B, T, h_enc.device, param_fingerprint(self))
+        key = (B, T, K, h_enc.device, param_fingerprint(self))
         cache = self.__dict__.setdefault("_greedy_engines", {})
         eng = cache.get(key)
         if eng is None:
             cache.clear()                                  # one resident program is enough
-            eng = cache[key] = GreedyEngine(self, B, T, blank=self.blank)
+            eng = cache[key] = GreedyEngine(self, B, T, blank=self.blank, max_symbols=K)
         ids, logp = eng.run(h_enc)
         ids = ids.cpu().numpy()
-        out = [ids[i, :int(n)].astype("int64") for i, n in enumerate(xlen)]
+        out = [ids[i, :int(n) * K].astype("int64") for i, n in enumerate(xlen)]
         return out, -logp.clone()
 
 

@@ -19,7 +19,8 @@ import torch
 
 from .models import Transducer, convert_lightning2normal
 from .tokenizer import NUL, BOS, UNK
-from ..stream_engine import BEAM_MAX_W, StreamBeamEngine, StreamEngine, check_lm_args, param_fingerprint
+from ..stream_engine import BEAM_MAX_W, StreamBeamEngine, StreamEngine, check_lm_args, check_max_symbols, \
+    param_fingerprint
 
 
 class StreamTransducerDecoder:
@@ -44,11 +45,17 @@ class PytorchStreamDecoder(StreamTransducerDecoder):
     the best hypothesis and continues decoding from it; call it at the end of an utterance or a segment.  Without a
     forced collapse (a suffix outgrowing ``max_pending``), everything ``decode`` returned plus ``flush()`` is the
     best hypothesis of Transducer.beam_search over the same encoder frames.  The beam does not apply the reference's
-    ``<unk>`` rule, which belongs to greedy argmax decoding; Transducer.beam_search does not apply it either."""
+    ``<unk>`` rule, which belongs to greedy argmax decoding; Transducer.beam_search does not apply it either.
+
+    ``max_symbols`` = K (1 to 16, greedy decoding only) lets each encoder frame emit up to K symbols: the frame repeats
+    joint -> argmax (with the ``<unk>`` rule) -> predictor step until a blank or K non-blank tokens."""
 
     def __init__(self, FLAGS, transducer=None, transform=None, tokenizer=None, device="cuda",
                  frames_per_chunk=None, input_size=None, *, beam_width=None, merge=True, lm=None, lm_weight=0.0,
-                 length_bonus=0.0, lm_bos=1, lm_token_map=None, max_pending=64):
+                 length_bonus=0.0, lm_bos=1, lm_token_map=None, max_pending=64, max_symbols=1):
+        self._max_symbols = check_max_symbols(max_symbols)
+        if beam_width is not None and self._max_symbols != 1:
+            raise ValueError("max_symbols > 1 is a greedy decoding option; the beam search emits one symbol per frame")
         self.FLAGS = FLAGS
         self.device = torch.device(device)
         if tokenizer is None:
@@ -112,7 +119,8 @@ class PytorchStreamDecoder(StreamTransducerDecoder):
         # arbitrary chunk lengths); only reset() starts from the primed zero state
         st = self._engine.state() if self._engine is not None else None
         if self._beam is None:
-            self._engine = StreamEngine(self._transducer, 1, n, unk_id=self._unk, blank=NUL, state=st)
+            self._engine = StreamEngine(self._transducer, 1, n, unk_id=self._unk, blank=NUL, state=st,
+                                        max_symbols=self._max_symbols)
         else:
             self._engine = StreamBeamEngine(self._transducer, 1, n, blank=NUL, state=st, **self._beam)
         self._frames = n

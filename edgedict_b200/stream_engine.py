@@ -6,7 +6,8 @@ chunk's log-mel frames into a fixed input buffer and launches ONE cooperative ke
 stateful encoder, then for every encoder output frame joint -> argmax (with the ``<unk>`` rule) ->
 masked predictor step, for all streams at once.  Semantics per stream are exactly those of
 PytorchStreamDecoder.reset/decode (reference rnnt/stream.py:78-120): at most one symbol per
-encoder frame, argmax over raw logits, predictor advanced only on non-blank.
+encoder frame, argmax over raw logits, predictor advanced only on non-blank.  With ``max_symbols`` = K > 1 a frame
+repeats joint -> argmax -> predictor step until a blank or K symbols (GreedyEngine likewise).
 """
 import ctypes as C
 import math
@@ -18,10 +19,11 @@ import torch
 from ._lib import lib, check
 from .rnnt.tokenizer import NUL, BOS, UNK
 
-PH_LN, PH_PAIR, PH_LSTM, PH_LINEAR, PH_ARGMAX, PH_COPY, PH_BEAM_SELECT, PH_GATHER, PH_BEAM_FINAL, PH_BEAM_COMMIT = \
-    range(10)
-F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE, F_LM, F_STREAM, F_FLUSH = 1, 2, 4, 8, 16, 32, 64, 128
+PH_LN, PH_PAIR, PH_LSTM, PH_LINEAR, PH_ARGMAX, PH_COPY, PH_BEAM_SELECT, PH_GATHER, PH_BEAM_FINAL, PH_BEAM_COMMIT, \
+    PH_SKIP = range(11)
+F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE, F_LM, F_STREAM, F_FLUSH, F_CONT = 1, 2, 4, 8, 16, 32, 64, 128, 256
 BEAM_MAX_W = 1024                                     # EB_BEAM_MAX_W
+MAX_SYMBOLS = 16                                      # bounds the program: about (5 + L_dec) * K phases per frame
 
 
 class EbPhase(C.Structure):
@@ -64,6 +66,32 @@ def predictor_phases(prog, embed, layers, proj_w, proj_b, S, h, c, htmp, x, tok,
 def _dec_phases(prog, dec, S, h, c, htmp, x, tok, blank, masked):
     predictor_phases(prog, dec.embed.weight, lstm_layers(dec.lstm), dec.proj.weight, dec.proj.bias, S, h, c, htmp, x,
                      tok, blank, masked)
+
+
+def check_max_symbols(max_symbols):
+    """The per-frame symbol cap K of greedy decoding, an integer in [1, MAX_SYMBOLS].  Raises TypeError / ValueError;
+    touches no device."""
+    if isinstance(max_symbols, bool) or not isinstance(max_symbols, numbers.Integral):
+        raise TypeError("max_symbols must be an integer, got %r" % (max_symbols,))
+    K = int(max_symbols)
+    if not 1 <= K <= MAX_SYMBOLS:
+        raise ValueError("max_symbols must be in [1, %d], got %d" % (MAX_SYMBOLS, K))
+    return K
+
+
+def greedy_frame(prog, K, S, tok, blank, round_phases):
+    """Append one encoder frame of greedy decoding with at most K symbols for S rows.  ``round_phases(j)`` appends round
+    j: the joint, an ARGMAX into ``tok`` (with F_CONT for j >= 1: rows whose frame already ended stay blank) and the
+    predictor step masked on blank.  Each round j >= 1 opens with a SKIP to the end of the frame, taken when every row's
+    round j-1 token was blank.  With K = 1 this is round 0 alone, the one-symbol program."""
+    skips = []
+    for j in range(K):
+        if j:
+            skips.append(len(prog))
+            prog.append(EbPhase(type=PH_SKIP, S=S, aux2=blank, tok_in=_ptr(tok)))
+        round_phases(j)
+    for i in skips:
+        prog[i].aux = len(prog) - i - 1
 
 
 def lm_state_dict(lm):
@@ -240,7 +268,12 @@ def _upload(prog, dev):
 class StreamEngine:
     STATE = ("enc_h", "enc_c", "dec_h", "dec_c", "dec_x", "tok")
 
-    def __init__(self, transducer, n_streams, frames_per_chunk, unk_id=UNK, blank=NUL, max_ctas=0, state=None):
+    def __init__(self, transducer, n_streams, frames_per_chunk, unk_id=UNK, blank=NUL, max_ctas=0, state=None,
+                 max_symbols=1):
+        """``max_symbols`` = K: per output frame up to K rounds of joint -> argmax (with the <unk> rule) -> masked
+        predictor step; a stream's frame ends at its first blank or after K non-blank tokens.  ``step`` then returns
+        [S, n_out * K]: K entries per frame, blank for the rounds a stream did not take."""
+        K = check_max_symbols(max_symbols)
         assert C.sizeof(EbPhase) == lib().eb_decode_phase_size(), "EbPhase layout mismatch"
         enc, dec, joint = transducer.encoder, transducer.decoder, transducer.joint.joint
         _check_lstm_encoder(enc, "StreamEngine")
@@ -249,7 +282,7 @@ class StreamEngine:
             raise RuntimeError("StreamEngine needs the model on a CUDA device")
         f32 = torch.float32
         S, n = n_streams, frames_per_chunk
-        self.S, self.n, self.blank, self.unk, self.max_ctas = S, n, blank, unk_id, max_ctas
+        self.S, self.n, self.blank, self.unk, self.max_ctas, self.max_symbols = S, n, blank, unk_id, max_ctas, K
         L = len(enc.lstm.lstms)
         H = enc.lstm.hidden_size
         z = lambda *shape: torch.zeros(*shape, dtype=f32, device=self.dev)
@@ -273,19 +306,22 @@ class StreamEngine:
         self.dec_h, self.dec_c, self.dec_htmp = z(Ld, S, Hd), z(Ld, S, Hd), z(Ld, S, Hd)
         self.dec_x, self.hidden, self.logits = z(S, D), z(S, J), z(S, V)
         self.tok = torch.zeros(S, dtype=torch.int32, device=self.dev)
-        self.hist = torch.zeros(S, max(ni, 1), dtype=torch.int32, device=self.dev)
+        self.hist = torch.zeros(S, max(ni * K, 1), dtype=torch.int32, device=self.dev)
 
         w1 = joint[0].weight
         for k in range(ni):
-            ph(type=PH_LINEAR, S=S, N=J, flags=F_TANH, K1=E, x1=_ptr(self.enc_out, k * E), ldx1=ni * E, w1=_ptr(w1),
-               ldw1=E + D, K2=D, x2=_ptr(self.dec_x), ldx2=D, w2=_ptr(w1, E), ldw2=E + D, b1=_ptr(joint[0].bias),
-               y=_ptr(self.hidden), ldy=J)
-            ph(type=PH_LINEAR, S=S, N=V, K1=J, x1=_ptr(self.hidden), ldx1=J, w1=_ptr(joint[2].weight), ldw1=J,
-               b1=_ptr(joint[2].bias), y=_ptr(self.logits), ldy=V)
-            ph(type=PH_ARGMAX, S=S, N=V, x1=_ptr(self.logits), ldx1=V, aux=blank, aux2=unk_id, tok_out=_ptr(self.tok),
-               hist=_ptr(self.hist), hist_ld=self.hist.shape[1], hist_col=k)
-            _dec_phases(prog, dec, S, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
-                        masked=True)
+            def round_phases(j):
+                ph(type=PH_LINEAR, S=S, N=J, flags=F_TANH, K1=E, x1=_ptr(self.enc_out, k * E), ldx1=ni * E,
+                   w1=_ptr(w1), ldw1=E + D, K2=D, x2=_ptr(self.dec_x), ldx2=D, w2=_ptr(w1, E), ldw2=E + D,
+                   b1=_ptr(joint[0].bias), y=_ptr(self.hidden), ldy=J)
+                ph(type=PH_LINEAR, S=S, N=V, K1=J, x1=_ptr(self.hidden), ldx1=J, w1=_ptr(joint[2].weight), ldw1=J,
+                   b1=_ptr(joint[2].bias), y=_ptr(self.logits), ldy=V)
+                ph(type=PH_ARGMAX, S=S, N=V, flags=F_CONT if j else 0, x1=_ptr(self.logits), ldx1=V, aux=blank,
+                   aux2=unk_id, tok_out=_ptr(self.tok), hist=_ptr(self.hist), hist_ld=self.hist.shape[1],
+                   hist_col=k * K + j)
+                _dec_phases(prog, dec, S, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
+                            masked=True)
+            greedy_frame(prog, K, S, self.tok, blank, round_phases)
         ph(type=PH_COPY, S=L * S, N=H, x1=_ptr(self.enc_htmp), y=_ptr(self.enc_h))
         self.n_chunk_phases = len(prog)
         chunk_prog = prog
@@ -330,9 +366,11 @@ class StreamEngine:
 
     @torch.no_grad()
     def step(self, chunk):
-        """chunk [S, n, F] log-mel frames (device or pinned host) -> int32 [S, n_out] token ids
-        (blank = 0 means 'no symbol for this frame')."""
+        """chunk [S, n, F] log-mel frames (device or pinned host) -> int32 [S, n_out * max_symbols] token ids, the
+        max_symbols rounds of each frame in order (blank = 0 means 'no symbol in this round')."""
         self.xin.copy_(chunk, non_blocking=True)
+        if self.max_symbols > 1:
+            self.hist.fill_(self.blank)             # the columns of rounds skipped for every stream are not written
         self._run(self._chunk, self.n_chunk_phases)
         return self.hist
 
@@ -343,12 +381,16 @@ class GreedyEngine:
     the new state only where the prediction is non-blank) run inside ONE cooperative kernel launch as
     a phase program over the encoder output, instead of T' Python iterations of ~10 launches each."""
 
-    def __init__(self, transducer, batch, t_out, blank=NUL, max_ctas=0):
+    def __init__(self, transducer, batch, t_out, blank=NUL, max_ctas=0, max_symbols=1):
+        """``max_symbols`` = K: per encoder frame up to K rounds of joint -> argmax -> masked predictor step; a row's
+        frame ends at its first blank or after K non-blank tokens (the predictor has then stepped on the K-th).  log p
+        accumulates over every round taken; ``hist`` is [B, T' * K], frame-major, blank for rounds not taken."""
+        K = check_max_symbols(max_symbols)
         dec, joint = transducer.decoder, transducer.joint.joint
         self.dev = dec.embed.weight.device
         f32 = torch.float32
         B, T = batch, t_out
-        self.B, self.T, self.blank, self.max_ctas = B, T, blank, max_ctas
+        self.B, self.T, self.blank, self.max_ctas, self.max_symbols = B, T, blank, max_ctas, K
         z = lambda *shape: torch.zeros(*shape, dtype=f32, device=self.dev)
         Ld, Hd = dec.lstm.num_layers, dec.lstm.hidden_size
         D = dec.proj.weight.shape[0]
@@ -358,7 +400,7 @@ class GreedyEngine:
         self.dec_h, self.dec_c, self.dec_htmp = z(Ld, B, Hd), z(Ld, B, Hd), z(Ld, B, Hd)
         self.dec_x, self.hidden, self.logits = z(B, D), z(B, J), z(B, V)
         self.tok = torch.zeros(B, dtype=torch.int32, device=self.dev)
-        self.hist = torch.zeros(B, T, dtype=torch.int32, device=self.dev)
+        self.hist = torch.zeros(B, T * K, dtype=torch.int32, device=self.dev)
         self.logp = z(B)
         self._keep = [p.detach() for p in transducer.parameters()]
         prog = []
@@ -373,15 +415,18 @@ class GreedyEngine:
                     masked=False)                   # prime with BOS from the zero state
         w1 = joint[0].weight
         for k in range(T):
-            ph(type=PH_LINEAR, S=B, N=J, flags=F_TANH, K1=E, x1=_ptr(self.h_enc, k * E), ldx1=T * E, w1=_ptr(w1),
-               ldw1=E + D, K2=D, x2=_ptr(self.dec_x), ldx2=D, w2=_ptr(w1, E), ldw2=E + D, b1=_ptr(joint[0].bias),
-               y=_ptr(self.hidden), ldy=J)
-            ph(type=PH_LINEAR, S=B, N=V, K1=J, x1=_ptr(self.hidden), ldx1=J, w1=_ptr(joint[2].weight), ldw1=J,
-               b1=_ptr(joint[2].bias), y=_ptr(self.logits), ldy=V)
-            ph(type=PH_ARGMAX, S=B, N=V, flags=F_LOGP, x1=_ptr(self.logits), ldx1=V, aux=blank, aux2=-1,
-               tok_out=_ptr(self.tok), hist=_ptr(self.hist), hist_ld=T, hist_col=k, y=_ptr(self.logp))
-            _dec_phases(prog, dec, B, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
-                        masked=True)
+            def round_phases(j):
+                ph(type=PH_LINEAR, S=B, N=J, flags=F_TANH, K1=E, x1=_ptr(self.h_enc, k * E), ldx1=T * E, w1=_ptr(w1),
+                   ldw1=E + D, K2=D, x2=_ptr(self.dec_x), ldx2=D, w2=_ptr(w1, E), ldw2=E + D, b1=_ptr(joint[0].bias),
+                   y=_ptr(self.hidden), ldy=J)
+                ph(type=PH_LINEAR, S=B, N=V, K1=J, x1=_ptr(self.hidden), ldx1=J, w1=_ptr(joint[2].weight), ldw1=J,
+                   b1=_ptr(joint[2].bias), y=_ptr(self.logits), ldy=V)
+                ph(type=PH_ARGMAX, S=B, N=V, flags=F_LOGP | (F_CONT if j else 0), x1=_ptr(self.logits), ldx1=V,
+                   aux=blank, aux2=-1, tok_out=_ptr(self.tok), hist=_ptr(self.hist), hist_ld=T * K,
+                   hist_col=k * K + j, y=_ptr(self.logp))
+                _dec_phases(prog, dec, B, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
+                            masked=True)
+            greedy_frame(prog, K, B, self.tok, blank, round_phases)
         self.nphase = len(prog)
         arr = (EbPhase * len(prog))(*prog)
         self._prog = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(self.dev)
@@ -389,10 +434,12 @@ class GreedyEngine:
 
     @torch.no_grad()
     def run(self, h_enc):
-        """h_enc [B, T', E] -> (ids int32 [B, T'] incl. blanks, sum of log p [B])."""
+        """h_enc [B, T', E] -> (ids int32 [B, T' * max_symbols] incl. blanks, sum of log p [B])."""
         self.h_enc.copy_(h_enc)
         for t in (self.dec_h, self.dec_c, self.logp):
             t.zero_()
+        if self.max_symbols > 1:
+            self.hist.fill_(self.blank)             # the columns of rounds skipped for every row are not written
         self.tok.fill_(BOS)
         check(lib().eb_decode_run(self._prog.data_ptr(), self.nphase, self._bar.data_ptr(), self.max_ctas,
                                   torch.cuda.current_stream().cuda_stream), "eb_decode_run")

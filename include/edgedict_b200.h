@@ -200,7 +200,7 @@ int eb_joint_dpre_reduce(const void* dpre16, float* dep, float* ddp, int B, int 
  * replaces PytorchStreamDecoder.decode's Python loop (rnnt/stream.py:93-120).  The host builds a
  * phase program once (edgedict_b200/stream_engine.py) and launches it per chunk; see decode.cu. */
 enum { EB_PH_LN = 0, EB_PH_PAIR = 1, EB_PH_LSTM = 2, EB_PH_LINEAR = 3, EB_PH_ARGMAX = 4, EB_PH_COPY = 5,
-       EB_PH_BEAM_SELECT = 6, EB_PH_GATHER = 7, EB_PH_BEAM_FINAL = 8, EB_PH_BEAM_COMMIT = 9 };
+       EB_PH_BEAM_SELECT = 6, EB_PH_GATHER = 7, EB_PH_BEAM_FINAL = 8, EB_PH_BEAM_COMMIT = 9, EB_PH_SKIP = 10 };
 typedef struct EbPhase {
     int32_t type, S, K1, K2, N, flags, ldx1, ldx2, ldw1, ldw2, ldy, aux, aux2, hist_ld, hist_col, x1_div;
     const float *x1, *x2, *w1, *w2, *b1, *b2;
@@ -228,6 +228,11 @@ typedef struct EbPhase {
  *            and hold only the tokens since the stream's last commit (length = that count; the hash still covers the
  *            whole sequence).  The offline beam search does not set it.
  *      128 = BEAM_COMMIT collapses every stream's beam to its best slot unconditionally (a flush).
+ *      256 = ARGMAX continuation (round j >= 1 of a multi-symbol greedy frame): a row whose tok_out already holds aux
+ *            (blank: its frame ended) writes blank to its hist column, takes no argmax and adds nothing under flag 8;
+ *            the other rows run the plain ARGMAX, <unk> rule included.
+ * SKIP (no flags, writes nothing, no grid barrier): when no row of tok_in[0..S) differs from aux2 (blank), every CTA
+ * jumps over the next aux phases.  It reads only data final at the preceding barrier, so all CTAs take the same branch.
  * BEAM_COMMIT (streaming beam, after a chunk's last frame, one CTA per stream): commits the common prefix of the live
  * slots' stored suffixes to tok_out [S, N] with the count in tok_out2[s] (tok_out2[S + s] = 1 when the beam collapsed),
  * shifts the suffixes left into seq_out, and, when a suffix still exceeds aux2 tokens or on flags 128, collapses the beam
