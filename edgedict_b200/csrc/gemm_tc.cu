@@ -519,6 +519,8 @@ static int gemm_dispatch(const void* A, int a_mn_major, const void* B, int b_mn_
     const bool low = (flags & EB_GEMM_CORESIDENT) != 0;
     if (low && (a_mn_major || b_mn_major)) return EB_ERR_INVALID;
     if ((reinterpret_cast<uintptr_t>(A) & 15) || (reinterpret_cast<uintptr_t>(B) & 15)) return EB_ERR_INVALID;
+    // the epilogue stores column pairs as one float2 / __nv_bfloat162 whenever N is even
+    if (reinterpret_cast<uintptr_t>(C) & (c_bf16 ? 3 : 7)) return EB_ERR_INVALID;
     // contiguous dimension must keep row pitches 16-byte aligned
     if ((a_mn_major ? M : K) % 8 || (b_mn_major ? (long)N : K) % 8) return EB_ERR_INVALID;
     bool wide;

@@ -52,7 +52,8 @@ int eb_gemm_f32(const float* A, long sam, long sak, const float* B, long sbk, lo
 /* ---- bf16 tensor-core GEMM (wgmma + TMA), fp32 accumulate ----------------------------------
  * same call sites in bf16 mode.  A: [M,K] (a_mn_major=0, K contiguous) or [K,M] (a_mn_major=1);
  * B: [N,K] (b_mn_major=0) or [K,N] (b_mn_major=1); C row-major [M,N] fp32 or bf16;
- * C = A*B (+ bias[n]) (+ C when accumulate).  Pointers 16-byte aligned, contiguous dim % 8 == 0. */
+ * C = A*B (+ bias[n]) (+ C when accumulate).  A and B 16-byte aligned, contiguous dim % 8 == 0; C 8-byte aligned
+ * (fp32) or 4-byte aligned (bf16), the width of the epilogue's paired stores. */
 int eb_gemm_bf16(const void* A, int a_mn_major, const void* B, int b_mn_major, void* C, int c_bf16,
                  const float* bias, int accumulate, long M, int N, long K, void* stream);
 

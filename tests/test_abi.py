@@ -113,6 +113,11 @@ def test_entry_points_reject_bad_arguments_before_touching_the_device(built):
     assert L.eb_gemm_bf16(p, 0, p, 0, p, 0, None, 0, 8, 8, 12, None) == 2            # K-major rows must be 16-byte multiples
     assert L.eb_gemm_bf16(p + 2, 0, p, 0, p, 0, None, 0, 8, 8, 8, None) == 2         # misaligned operand
     assert L.eb_gemm_bf16_ex(p, 1, p, 0, p, 0, None, 0, 8, 8, 8, 1, None, 0, None) == 2   # co-resident config: K-major only
+    # the epilogue stores column pairs as float2 (fp32 C) / __nv_bfloat162 (bf16 C)
+    for c_bf16, off in ((0, 4), (0, 2), (0, 1), (1, 2), (1, 1)):
+        assert L.eb_gemm_bf16(p, 0, p, 0, p + off, c_bf16, None, 0, 8, 8, 8, None) == 2, (c_bf16, off)
+        assert L.eb_gemm_bf16(p, 1, p, 1, p + off, c_bf16, None, 1, 8, 8, 8, None) == 2, (c_bf16, off)
+        assert L.eb_gemm_bf16_ex(p, 0, p, 0, p + off, c_bf16, None, 0, 8, 8, 8, 1, None, 0, None) == 2, (c_bf16, off)
     assert L.eb_gemm_bf16_dtanh(p, 0, p, 1, p, None, 8, 8, 8, None) == 2             # needs the hidden activations
     assert L.eb_gemm_bf16_dtanh(p, 0, p, 1, p, p, 8, 6, 8, None) == 2                # N % 4
     assert L.eb_joint_dpre_reduce(None, p, p, 1, 1, 1, 8, None) == 2
