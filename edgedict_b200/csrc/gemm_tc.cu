@@ -1,5 +1,5 @@
 // gemm_tc.cu -- bf16 tensor-core GEMM for sm_90a: TMA -> shared (128B swizzle) -> wgmma.mma_async (fp32
-// accumulators in registers) -> epilogue straight from the accumulator fragments.  Hand-written PTX, no CUTLASS.
+// accumulators in registers) -> epilogue from the accumulator fragments.  Hand-written PTX, no CUTLASS.
 //
 // Used in bf16 mode for every dense contraction of the RNN-T path:
 //   LSTM input projections  xg = X * W_ih^T          (rnnt/models.py:45-46 -> nn.LSTM)
@@ -11,9 +11,13 @@
 //   warps 0-7   two consumer warpgroups: warpgroup g issues the wgmma (M64 N128|256 K16) of rows [64g, 64g+64) of the
 //               tile, four per stage; one stage of MMAs stays in flight and the stage before it is handed back to the
 //               producer.  At the end of the tile the warpgroup applies the epilogue (bias, + C, tanh', softmax
-//               statistics) to its own accumulators and stores them.
+//               statistics) to its own accumulators and stores them.  Staged-C configuration (SC: bf16 C written
+//               whole, 128-wide tile): the warpgroup converts its 64 x 128 half to bf16 into a swizzled shared tile,
+//               one thread hands it to a TMA store and the warpgroup goes on to the next tile's MMAs while it drains.
 //   warp 8      TMA producer: cp.async.bulk.tensor.2d into a STAGES-deep ring, mbarrier expect_tx.  It runs ahead into
-//               the next tile while the consumers are in the epilogue.
+//               the next tile while the consumers are in the epilogue.  SC with a tanh' operand: it also loads the
+//               tile's 128 x 128 block of that operand into the staging tile once the consumers have started the tile,
+//               so the load lands under the MMAs; the epilogue reads it there and overwrites it with C in place.
 #include <cuda.h>
 #include <stdlib.h>
 #include "common.cuh"
@@ -29,11 +33,15 @@ constexpr int NTHREADS = 2 * 128 + 32;                       // two consumer war
 // LOW_ = "co-resident" configuration: 3 stages of the narrow tile (97 KB of shared memory), so that a GEMM CTA fits on an
 // SM next to one CTA of a persistent recurrent kernel (lstm_c4.cu) -- used by the layer-wavefront schedule of the encoder
 // stack, where the input GEMM of one layer runs under the recurrence of another.
-template <int BN_, bool LOW_ = false> struct Cfg {
-    static constexpr int STAGES = LOW_ ? 3 : (BN_ == 256 ? 4 : 6);
+// SC_ = staged-C configuration: 5 stages + the 32 KB staging tile, the shared memory of the 6-stage one, so that the
+// joint's d-hidden GEMM still leaves room on each SM for a CTA of the bias column sum that runs beside it.
+template <int BN_, bool LOW_ = false, bool SC_ = false> struct Cfg {
+    static_assert(!SC_ || (BN_ == 128 && !LOW_), "the staged-C epilogue is built for the full-size 128-wide tile");
+    static constexpr int STAGES = LOW_ ? 3 : (BN_ == 256 ? 4 : (SC_ ? 5 : 6));
     static constexpr int B_BYTES = BN_ * BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 256;
+    static constexpr int X_BYTES = SC_ ? BM * BN_ * 2 : 0;    // staging tile: [warpgroup][64-column half][64 rows][128 B]
+    static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + X_BYTES + 256;
 };
 
 // Persistent tile schedule (identical in the producer and the consumers).  Work item j of CTA b:
@@ -80,24 +88,67 @@ __device__ __forceinline__ void st_bf16x2(__nv_bfloat16* p, float a, float b) {
     *reinterpret_cast<__nv_bfloat162*>(p) = __floats2bfloat162_rn(a, b);
 }
 
+// ---- staged-C epilogue (SC)
+// Byte offset of the thread's column pair of fragment column group i (tile columns 8i + cq, + 1) in row rr of its
+// warpgroup's staging tile.  The TMA 128B swizzle: 64-column halves of 8 KB, 128 B per row, the 16-byte chunk c of row r
+// at chunk c ^ (r % 8).  The 8 rows of a warp store land in 8 different chunks: no bank conflicts.
+__device__ __forceinline__ uint32_t x_off(int rr, int i, int lane) {
+    return (uint32_t)((i >> 3) * 8192 + rr * 128 + (((i & 7) ^ (rr & 7)) << 4) + 4 * (lane & 3));
+}
+__device__ __forceinline__ void st_shared_bf16x2(uint32_t a, float x, float y) {
+    const __nv_bfloat162 v = __floats2bfloat162_rn(x, y);
+    asm volatile("st.shared.b32 [%0], %1;" :: "r"(a), "r"(*reinterpret_cast<const uint32_t*>(&v)) : "memory");
+}
+__device__ __forceinline__ float2 ld_shared_bf16x2(uint32_t a) {
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+    return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&v));
+}
+__device__ __forceinline__ void wg_bar_sync(int wg) { asm volatile("bar.sync %0, 128;" :: "r"(1 + wg) : "memory"); }
+// the warpgroup's staging tile is free: its previous TMA stores have read it
+__device__ __forceinline__ void x_acquire(int wg, bool leader) {
+    if (leader) bulk_wait_read<0>();
+    wg_bar_sync(wg);
+}
+// the warpgroup's 64 x 128 half tile [r0, r0 + 64) x [n0, n0 + 128) leaves by TMA; rows >= M and columns >= N are clipped
+__device__ __forceinline__ void x_store(const CUtensorMap* map, uint32_t xw, int wg, bool leader, long r0, int n0, long M,
+                                        int N) {
+    fence_proxy_async_smem();                                // the st.shared above -> the TMA engine's reads
+    wg_bar_sync(wg);
+    if (leader) {
+        if (r0 < M) {
+            tma_store_2d(map, xw, n0, (int)r0);
+            if (n0 + 64 < N) tma_store_2d(map, xw + 8192, n0 + 64, (int)r0);
+        }
+        bulk_commit();
+    }
+}
+
 // A_MN / B_MN: operand stored with its M (resp. N) index contiguous ("MN-major"), else K contiguous.
 //   K-major tile in smem : [rows][64 k] bf16, 128 B per row, 128B swizzle; SBO = 1024 (8 rows)
 //   MN-major tile in smem: [64 k][64 mn] bf16 boxes of 8 KB, 128 B per k-row; SBO = 1024 (8 k-rows), LBO = 8192
 // LOW_ is also capped to 112 registers per thread (two CTAs' worth per SM): the register file has to hold a recurrent
 // CTA beside it as well.
-template <bool A_MN, bool B_MN, int BN_, bool LSE = false, bool LOW_ = false>
+// SC: staged-C epilogue (bf16 C, no accumulation, ksplit = 1, N % 8 == 0; tma_c / tma_x: C and lse.aux with 64 x 64
+// boxes), else tma_c / tma_x are unused.
+template <bool A_MN, bool B_MN, int BN_, bool LSE = false, bool LOW_ = false, bool SC = false>
 __global__ void __launch_bounds__(NTHREADS, LOW_ ? 2 : 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
+               const __grid_constant__ CUtensorMap tma_c, const __grid_constant__ CUtensorMap tma_x,
                void* __restrict__ Cout, int c_bf16, const float* __restrict__ bias, int accumulate,
                long M, int N, long K, int ksplit, LseArgs lse = LseArgs(), float* __restrict__ part = nullptr) {
-    using C_ = Cfg<BN_, LOW_>;
+    using C_ = Cfg<BN_, LOW_, SC>;
     constexpr int BN = BN_, STAGES = C_::STAGES, STAGE_BYTES = C_::STAGE_BYTES, NACC = BN / 2;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* tiles = smem;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
-    // bars: full[S], empty[S]
+    const uint32_t xtile = smem_u32(smem + STAGES * STAGE_BYTES);   // SC staging tile (1024-aligned)
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + C_::X_BYTES);
+    // bars: full[S], empty[S], xfull, xempty (SC with a tanh' operand: the operand has landed in the staging tile / the
+    // staging tile's stores have read it)
     const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + STAGES);
+    const uint32_t xfull = smem_u32(bars + 2 * STAGES), xempty = xfull + 8;
+    const bool has_x = SC && lse.aux != nullptr;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long num_m = (M + BM - 1) / BM;
@@ -111,9 +162,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 8); }   // 8 consumer warps
+        if (SC) { mbar_init(xfull, 1); mbar_init(xempty, 2); }                                          // 2 store leaders
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" :: "l"(&tma_a) : "memory");
         asm volatile("prefetch.tensormap [%0];" :: "l"(&tma_b) : "memory");
+        if (SC) asm volatile("prefetch.tensormap [%0];" :: "l"(&tma_c) : "memory");
+        if (has_x) asm volatile("prefetch.tensormap [%0];" :: "l"(&tma_x) : "memory");
     }
     __syncthreads();
 
@@ -126,6 +180,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
             for (long jj = 0; sch.get(jj, mb, nb, ksx); ++jj) {
                 const int kb0 = ksx * kb_per, kb1 = min(nkb_total, kb0 + kb_per);
                 const int m0 = (int)mb * BM, n0 = nb * BN;
+                // the tanh' operand of this tile: loaded once the wait for k-block kb0 + STAGES has shown that the
+                // consumers are into the tile, so that waiting for the staging tile does not stall the ring
+                const int kbx = min(kb0 + STAGES, kb1 - 1);
                 for (int kb = kb0; kb < kb1; ++kb) {
                     mbar_wait(empty0 + 8 * stage, phase ^ 1);
                     const uint32_t sa = smem_u32(tiles + stage * STAGE_BYTES), sb = sa + A_BYTES;
@@ -137,6 +194,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                     else {
 #pragma unroll
                         for (int bx = 0; bx < BN / 64; ++bx) tma_load_2d(sb + bx * 8192, &tma_b, n0 + bx * 64, kb * BK, fb);
+                    }
+                    if (has_x && kb == kbx) {
+                        if (jj > 0) mbar_wait(xempty, (uint32_t)(jj - 1) & 1u);   // the previous tile's stores read it
+                        mbar_expect_tx(xfull, C_::X_BYTES);
+#pragma unroll
+                        for (int q = 0; q < 4; ++q)                  // [warpgroup q / 2][64-column half q % 2]
+                            tma_load_2d(xtile + q * 8192, &tma_x, n0 + 64 * (q & 1), m0 + 64 * (q >> 1), xfull);
                     }
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
@@ -152,6 +216,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
     float* Cf = reinterpret_cast<float*>(Cout);
     __nv_bfloat16* const Ch = reinterpret_cast<__nv_bfloat16*>(Cout);
     const bool vec2 = (N % 2) == 0;
+    const uint32_t xw = xtile + (uint32_t)wg * 16384u;       // SC: this warpgroup's 64 rows of the staging tile
+    const bool leader = threadIdx.x == 128 * wg;             // SC: issues and waits for the warpgroup's TMA stores
+    uint32_t xph = 0;
     float acc[NACC];
     int stage = 0; uint32_t phase = 0;
     long mb; int nb, ks;
@@ -179,6 +246,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
             wgmma_commit();
             wgmma_wait<1>();                                 // the previous stage's MMAs have retired: hand it back
             if (prev >= 0 && lane == 0) mbar_arrive(empty0 + 8 * prev);
+            // the previous tile's stores have read the staging tile: the producer may load this tile's tanh' operand
+            if (has_x && kb == kb0 && jj > 0 && leader) { bulk_wait_read<0>(); mbar_arrive(xempty); }
             prev = stage;
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
@@ -203,6 +272,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                     }
                 }
             }
+            if constexpr (SC) x_acquire(wg, leader);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 // add the bias here (the statistics are over logits = acc + b2), then the online softmax
@@ -233,7 +303,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                     rm[h] = nm;
                 }
                 const long row = m0 + r_in + 8 * h;
-                if (row < M) {
+                if constexpr (SC) {
+                    const int rr = r_in - 64 * wg + 8 * h;
+#pragma unroll
+                    for (int i = 0; i < BN / 8; ++i) st_shared_bf16x2(xw + x_off(rr, i, lane), acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+                } else if (row < M) {
 #pragma unroll
                     for (int i = 0; i < BN / 8; ++i) {
                         const int col = n0 + 8 * i + cq;
@@ -246,6 +320,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                     }
                 }
             }
+            if constexpr (SC) x_store(&tma_c, xw, wg, leader, m0 + 64 * wg, n0, M, N);
             if (nb == num_n - 1) {                           // whole vocabulary seen: merge the quad, publish
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
@@ -268,6 +343,28 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                     }
                 }
             }
+        } else if constexpr (SC) {
+            // the register path's arithmetic in its order (bias, then tanh'), every row and column of the tile: the TMA
+            // store clips what lies outside C
+            if (has_x) { mbar_wait(xfull, xph); xph ^= 1; }   // (implies the previous stores have read the tile)
+            else x_acquire(wg, leader);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int rr = r_in - 64 * wg + 8 * h;
+#pragma unroll
+                for (int i = 0; i < BN / 8; ++i) {
+                    const int col = n0 + 8 * i + cq;
+                    float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+                    if (bias && col < N) { v0 += __ldg(bias + col); v1 += __ldg(bias + col + 1); }
+                    const uint32_t a = xw + x_off(rr, i, lane);
+                    if (has_x) {
+                        const float2 hh = ld_shared_bf16x2(a);
+                        v0 *= 1.f - hh.x * hh.x; v1 *= 1.f - hh.y * hh.y;
+                    }
+                    st_shared_bf16x2(a, v0, v1);
+                }
+            }
+            x_store(&tma_c, xw, wg, leader, m0 + 64 * wg, n0, M, N);
         } else {
             const bool add_bias = bias && ks == 0;
             // split-K: each split stores its partial tile in its own slice of the workspace (splitk_reduce_kernel adds
@@ -350,6 +447,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
             }
         }
     }
+    if constexpr (SC) {
+        if (leader) bulk_wait<0>();                          // the staging tile stays valid until the last store is done
+    }
 }
 
 // C[i] = (accumulate ? C[i] : 0) + part[0][i] + part[1][i] + ...: the split-K partial tiles added in split order
@@ -379,19 +479,36 @@ int choose_ksplit(long out_tiles, long nkb, long workers, double r) {
     return ksplit;
 }
 
-// one persistent launch over `work` items, at most one CTA per SM
-template <bool A_MN, bool B_MN, int BN_, bool LSE, bool LOW_>
-int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_bf16, const float* bias, int accumulate,
-                  long M, int N, long K, int ksplit, long work, const LseArgs& ea, cudaStream_t st, float* part = nullptr) {
-    using C_ = Cfg<BN_, LOW_>;
-    auto kern = gemm_tc_kernel<A_MN, B_MN, BN_, LSE, LOW_>;
+// Whether a product takes the staged-C epilogue (SC): bf16 C written whole by one K split, its rows (and those of the
+// tanh' operand) 16-byte aligned as a tensor map needs.  The caller adds: 128-wide tile, not co-resident.
+bool staged_c(const void* C, int c_bf16, int accumulate, int N, int ksplit, const void* aux) {
+    return c_bf16 && !accumulate && ksplit == 1 && N % 8 == 0 && (reinterpret_cast<uintptr_t>(C) & 15) == 0 &&
+           (reinterpret_cast<uintptr_t>(aux) & 15) == 0;
+}
+
+// C (and the tanh' operand) as TMA-store / load maps: [M][N] bf16, 64 x 64 boxes (one per 64 x 64 quarter of a
+// warpgroup's half tile), 128B swizzle
+bool make_c_maps(CUtensorMap* tc, CUtensorMap* tx, const void* C, const void* aux, long M, int N) {
+    return make_map(tc, C, (uint64_t)N, (uint64_t)M, 64) && (!aux || make_map(tx, aux, (uint64_t)N, (uint64_t)M, 64));
+}
+
+const CUtensorMap kNoMap = {};
+
+// one persistent launch over `work` items, at most one CTA per SM; tc / tx: the SC maps (SC instantiations only)
+template <bool A_MN, bool B_MN, int BN_, bool LSE, bool LOW_, bool SC = false>
+int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* tc, const CUtensorMap* tx, void* C,
+                  int c_bf16, const float* bias, int accumulate, long M, int N, long K, int ksplit, long work,
+                  const LseArgs& ea, cudaStream_t st, float* part = nullptr) {
+    using C_ = Cfg<BN_, LOW_, SC>;
+    auto kern = gemm_tc_kernel<A_MN, B_MN, BN_, LSE, LOW_, SC>;
     static bool attr_done = false;
     if (!attr_done) {
         EB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM_BYTES));
         attr_done = true;
     }
     const int grid = (int)(work < eb_num_sms() ? work : eb_num_sms());
-    kern<<<grid, NTHREADS, C_::SMEM_BYTES, st>>>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, ksplit, ea, part);
+    kern<<<grid, NTHREADS, C_::SMEM_BYTES, st>>>(ta, tb, tc ? *tc : kNoMap, tx ? *tx : kNoMap, C, c_bf16, bias,
+                                                 accumulate, M, N, K, ksplit, ea, part);
     EB_CHECK_LAUNCH();
     if (ksplit > 1) {
         const long mn = M * (long)N;
@@ -402,14 +519,21 @@ int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_b
     return EB_OK;
 }
 
+// tc non-null: the SC epilogue (128-wide tile only)
 template <bool A_MN, bool B_MN, int BN_>
-int launch(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_bf16, const float* bias, int accumulate,
-           long M, int N, long K, int ksplit, float* part, cudaStream_t st, const void* aux = nullptr) {
+int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* tc, const CUtensorMap* tx, void* C,
+           int c_bf16, const float* bias, int accumulate, long M, int N, long K, int ksplit, float* part,
+           cudaStream_t st, const void* aux = nullptr) {
     LseArgs ea = LseArgs();
     ea.aux = reinterpret_cast<const __nv_bfloat16*>(aux);
     const long out_tiles = ((M + BM - 1) / BM) * ((N + BN_ - 1) / BN_);
-    return launch_kernel<A_MN, B_MN, BN_, false, false>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, ksplit,
-                                                        out_tiles * ksplit, ea, st, part);
+    if constexpr (BN_ == 128) {
+        if (tc)
+            return launch_kernel<A_MN, B_MN, BN_, false, false, true>(ta, tb, tc, tx, C, c_bf16, bias, accumulate, M, N,
+                                                                      K, ksplit, out_tiles * ksplit, ea, st, part);
+    }
+    return launch_kernel<A_MN, B_MN, BN_, false, false>(ta, tb, nullptr, nullptr, C, c_bf16, bias, accumulate, M, N, K,
+                                                        ksplit, out_tiles * ksplit, ea, st, part);
 }
 
 // Tile width and split-K factor of a product (the one decision shared by eb_gemm_bf16_partials and the launch).
@@ -441,12 +565,17 @@ void plan(int a_mn_major, int c_bf16, int accumulate, long M, int N, long K, int
 int launch_low(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_bf16, const float* bias, int accumulate,
                long M, int N, long K, cudaStream_t st) {
     const long tiles = ((M + BM - 1) / BM) * ((N + 127) / 128);
-    return launch_kernel<false, false, 128, false, true>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, 1, tiles, LseArgs(), st);
+    return launch_kernel<false, false, 128, false, true>(ta, tb, nullptr, nullptr, C, c_bf16, bias, accumulate, M, N, K,
+                                                         1, tiles, LseArgs(), st);
 }
 
-int launch_lse(const CUtensorMap& ta, const CUtensorMap& tb, void* C, const float* bias, long M, int N, long K,
-               const LseArgs& lse, cudaStream_t st) {
-    return launch_kernel<false, false, 128, true, false>(ta, tb, C, 1, bias, 0, M, N, K, 1, (M + BM - 1) / BM, lse, st);
+int launch_lse(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* tc, void* C, const float* bias, long M,
+               int N, long K, const LseArgs& lse, cudaStream_t st) {
+    if (tc)
+        return launch_kernel<false, false, 128, true, false, true>(ta, tb, tc, nullptr, C, 1, bias, 0, M, N, K, 1,
+                                                                   (M + BM - 1) / BM, lse, st);
+    return launch_kernel<false, false, 128, true, false>(ta, tb, nullptr, nullptr, C, 1, bias, 0, M, N, K, 1,
+                                                         (M + BM - 1) / BM, lse, st);
 }
 
 }  // namespace
@@ -467,8 +596,10 @@ EB_API int eb_joint_logits_lse(const void* hidden16, const void* w2_16, const fl
         return EB_ERR_INVALID;
     const long M = (long)B * maxT * maxU;
     // 128-wide tiles: the softmax statistics of a 256-wide tile do not fit the registers beside its accumulators
-    CUtensorMap ta, tb;
-    if (!make_map(&ta, hidden16, (uint64_t)J, (uint64_t)M, 128) || !make_map(&tb, w2_16, (uint64_t)J, (uint64_t)V, 128)) {
+    CUtensorMap ta, tb, tc;
+    const bool sc = staged_c(logits16, 1, 0, V, 1, nullptr);
+    if (!make_map(&ta, hidden16, (uint64_t)J, (uint64_t)M, 128) || !make_map(&tb, w2_16, (uint64_t)J, (uint64_t)V, 128) ||
+        (sc && !make_c_maps(&tc, nullptr, logits16, nullptr, M, V))) {
         fprintf(stderr, "[edgedict_b200] cuTensorMapEncodeTiled failed\n");
         return EB_ERR_CUDA;
     }
@@ -476,7 +607,7 @@ EB_API int eb_joint_logits_lse(const void* hidden16, const void* w2_16, const fl
     lse.labels = labels; lse.xlen = xlen; lse.ylen = ylen; lse.denom = denom; lse.lpb = lpb; lse.lpl = lpl;
     lse.maxT = maxT; lse.maxU = maxU; lse.blank = blank; lse.aux = nullptr;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    return launch_lse(ta, tb, logits16, b2, M, V, J, lse, st);
+    return launch_lse(ta, tb, sc ? &tc : nullptr, logits16, b2, M, V, J, lse, st);
 }
 
 EB_API int eb_gemm_bf16(const void* A, int a_mn_major, const void* B, int b_mn_major, void* C, int c_bf16,
@@ -535,19 +666,24 @@ static int gemm_dispatch(const void* A, int a_mn_major, const void* B, int b_mn_
         const long fit = (partials && (reinterpret_cast<uintptr_t>(partials) & 7) == 0) ? partial_floats / (M * (long)N) : 0;
         if (fit < ksplit) ksplit = fit > 1 ? (int)fit : 1;
     }
-    CUtensorMap ta, tb;
+    CUtensorMap ta, tb, tc, tx;
+    const bool sc = !low && !wide && staged_c(C, c_bf16, accumulate, N, ksplit, aux);
     bool ok = a_mn_major ? make_map(&ta, A, (uint64_t)M, (uint64_t)K, 64) : make_map(&ta, A, (uint64_t)K, (uint64_t)M, 128);
     ok = ok && (b_mn_major ? make_map(&tb, B, (uint64_t)N, (uint64_t)K, 64)
                            : make_map(&tb, B, (uint64_t)K, (uint64_t)N, wide ? 256 : 128));
+    ok = ok && (!sc || make_c_maps(&tc, &tx, C, aux, M, N));
     if (!ok) {
         fprintf(stderr, "[edgedict_b200] cuTensorMapEncodeTiled failed\n");
         return EB_ERR_CUDA;
     }
+    const CUtensorMap* pc = sc ? &tc : nullptr;
+    const CUtensorMap* px = sc && aux ? &tx : nullptr;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (low) return launch_low(ta, tb, C, c_bf16, bias, accumulate, M, N, K, st);
-#define EB_GO(AM, BMN)                                                                                          \
-    return wide ? launch<AM, BMN, 256>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, ksplit, partials, st, aux) \
-                : launch<AM, BMN, 128>(ta, tb, C, c_bf16, bias, accumulate, M, N, K, ksplit, partials, st, aux)
+#define EB_GO(AM, BMN)                                                                                            \
+    return wide ? launch<AM, BMN, 256>(ta, tb, nullptr, nullptr, C, c_bf16, bias, accumulate, M, N, K, ksplit,    \
+                                       partials, st, aux)                                                         \
+                : launch<AM, BMN, 128>(ta, tb, pc, px, C, c_bf16, bias, accumulate, M, N, K, ksplit, partials, st, aux)
     if (a_mn_major) {
         if (b_mn_major) { EB_GO(true, true); }
         EB_GO(true, false);

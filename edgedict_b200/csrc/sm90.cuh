@@ -35,6 +35,19 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  :: "r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
+// shared -> global through the tensor map (its box and swizzle); elements outside the tensor are not written.  Tracked
+// by this thread's bulk async-groups: commit after the stores, wait before the source is overwritten or the CTA exits.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                 :: "l"(map), "r"(src), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// all but the N most recent bulk groups of this thread have read their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" :: "n"(N) : "memory"); }
+// all but the N most recent bulk groups of this thread have completed
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" :: "n"(N) : "memory"); }
 
 // ---- warpgroup MMA (wgmma) ------------------------------------------------------------------------------
 // D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 operands from shared memory, fp32 accumulators in registers.  All 128
