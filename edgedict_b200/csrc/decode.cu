@@ -19,7 +19,8 @@
 //           costs one read of S ints per CTA when no row is still emitting (greedy decoding with max_symbols > 1)
 //   BEAM_SELECT  per utterance: log-softmax of its W rows, exact top-W of the live slots' candidates, merge of equal
 //           token sequences, new slot log p / tokens / gather sources / history (Transducer.beam_search, one frame);
-//           optionally with an LSTM language model's log-probs fused into the candidate values (shallow fusion)
+//           optionally with an LSTM language model's log-probs fused into the candidate values (shallow fusion); with
+//           flags 512 one round of several per frame (beam search with max_symbols > 1: closed slots stay, open ones extend)
 //   GATHER  y[l, r] = x1[l, src[r]] (and y2[r] = x2[src[r]]): survivors inherit their parent's predictor state
 //   BEAM_FINAL  per utterance: best live slot, back-pointer walk through the history, ids and -log p written out
 //   BEAM_COMMIT per stream, at the end of a streaming chunk: commit the live hypotheses' common prefix, collapse the
@@ -378,13 +379,18 @@ __device__ void phase_argmax(const EbPhase& p) {
 //     = T', flags 128 = collapse unconditionally): y slot log p (in/out); hist (reads and rewrites the live count of
 //     column T'-1); seq_in / seq_out sequence rows before / after the commit (distinct buffers); tok_out committed
 //     tokens [B][N]; tok_out2 committed count [B] | collapsed 0/1 [B]; src gather source row [B*W].
+//   Several symbols per frame (BEAM_SELECT flags 512, ldw2 = K rounds per frame): hist_col = t*K + j is round j of
+//     frame t, hist_ld = T'*K columns.  The live count is read from and written to the last column, hist_live[b,
+//     hist_ld - 1], in every round (the host sets it before the launch), and each round a row takes also records it in
+//     its own column.  A round a row does not take (frozen, its frame ended, or SKIP jumped over it) writes no history:
+//     the host fills parent = slot, token = blank beforehand.  BEAM_FINAL and BEAM_COMMIT need no change.
 // They run one CTA per utterance (grid-strided over B).  They are __noinline__ so that their registers do not
 // count against the tensor-core phases the streaming decode spends its time in.
 constexpr int BEAM_MAX_W = EB_BEAM_MAX_W;
 constexpr unsigned long long SEQ_HASH_MUL = 0x100000001b3ull;      // polynomial hash: h' = h * MUL + (token + 1)
-// BEAM_SELECT's shared memory (2 x u64 + 12 x 32-bit arrays of BEAM_MAX_W, histogram, scalars) lives in the dynamic
+// BEAM_SELECT's shared memory (2 x u64 + 13 x 32-bit arrays of BEAM_MAX_W, histogram, scalars) lives in the dynamic
 // shared memory the matrix phases use
-static_assert(BEAM_MAX_W * (2 * 8 + 12 * 4) + 256 * 4 + 8 * 4 <= (RED_FLOATS + TR * OUT_LD) * 4, "beam smem");
+static_assert(BEAM_MAX_W * (2 * 8 + 13 * 4) + 256 * 4 + 8 * 4 <= (RED_FLOATS + TR * OUT_LD) * 4, "beam smem");
 
 // order-preserving map of a float to uint32 (larger float -> larger key); -0 ranks with +0 as in a float compare
 __device__ __forceinline__ uint32_t order_key(float v) {
@@ -411,6 +417,13 @@ __device__ bool seq_extends(const int* s2, const int* s1, int k1) {
         if (__ldcg(s2 + 3 + i) != __ldcg(s1 + 3 + i)) return false;
     return true;
 }
+// s1 + [e1] == s2 + [e2] exactly, where e < 0 appends nothing; the caller has checked that the lengths are equal
+__device__ bool seq_equal_ext(const int* s1, int e1, const int* s2, int e2) {
+    const int n1 = __ldcg(s1), n2 = __ldcg(s2), n = n1 + (e1 >= 0);
+    for (int i = 0; i < n; ++i)
+        if ((i < n1 ? __ldcg(s1 + 3 + i) : e1) != (i < n2 ? __ldcg(s2 + 3 + i) : e2)) return false;
+    return true;
+}
 
 // Selection: the candidates of one utterance are (slot q < live, token k) with value
 //   lp = ((x[q,k] - max_q) - log sum_k exp(x[q,k] - max_q)) + logp[q],
@@ -435,8 +448,21 @@ __device__ bool seq_extends(const int* s2, const int* s1, int k1) {
 // (max_pending + 3) whatever the frames per launch.  A row's length counts only the tokens stored since the stream's
 // last commit, while its hash keeps describing the whole sequence: every slot of a stream shares the committed prefix,
 // so equal whole sequences are exactly equal stored suffixes, and seq_extends and the merge stay exact.
-__device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
-    const int W = p.aux, V = p.N, T = p.hist_ld, t = p.hist_col, blank = p.aux2;
+//
+// Several symbols per frame (MULTI, flags 512, K = ldw2 rounds): round j of frame t.  A slot is open when its previous
+// round's token (tok_out, read before it is overwritten) is non-blank; every slot is open at round 0.  An open slot's
+// candidates are its V tokens as above: blank closes it, a non-blank token keeps it open unless j = K-1.  A closed slot
+// has one "stay" candidate of value logp[q] (nothing added) at flat index q*V + blank; it keeps its sequence and state,
+// so it is written exactly as a blank extension.  Merging needs equal sequences AND equal closedness (an open and a
+// closed hypothesis are different lattice states), and equal sequences can now come from parents with equal sequences
+// (a stay and a blank extension), so the exact check is the general seq_equal_ext.  A row with no open slot at j >= 1
+// has ended its frame and keeps its beam, as a frozen row does, and as SKIP does when no row is open: history, live
+// count and log p unwritten, the sequences copied to seq_out (the round's state moves back from there).
+template <bool MULTI>
+__device__ __forceinline__ void beam_select(const EbPhase& p, float* sm) {
+    const int W = p.aux, V = p.N, T = p.hist_ld, col = p.hist_col, blank = p.aux2;
+    const int KR = MULTI ? p.ldw2 : 1, t = MULTI ? col / KR : col, jr = MULTI ? col % KR : 0;
+    const bool last = jr == KR - 1;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nt = blockDim.x;
     const bool merge = p.flags & 16, lm = p.flags & 32, stream = p.flags & 64;
     const long BTW = (long)p.S * T * W;
@@ -459,14 +485,42 @@ __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
     int* skept = sfirst + BEAM_MAX_W;                                           // slot -> survivor index
     float* lmm = reinterpret_cast<float*>(skept + BEAM_MAX_W);                   // LM log-softmax statistics
     float* lmls = lmm + BEAM_MAX_W;
-    unsigned* rhist = reinterpret_cast<unsigned*>(lmls + BEAM_MAX_W);           // [256]
+    int* sopen = reinterpret_cast<int*>(lmls + BEAM_MAX_W);                      // slot open (MULTI)
+    unsigned* rhist = reinterpret_cast<unsigned*>(sopen + BEAM_MAX_W);          // [256]
     int* misc = reinterpret_cast<int*>(rhist + 256);
     const float lm_weight = lm ? __ldg(p.fuse) : 0.f, length_bonus = lm ? __ldg(p.fuse + 1) : 0.f;
     for (int b = blockIdx.x; b < p.S; b += gridDim.x) {
-        const long r0 = (long)b * W, h0 = ((long)b * T + t) * W;
-        const int nlive = t > 0 ? __ldcg(hlive + (long)b * T + t - 1) : stream ? __ldcg(hlive + (long)b * T + T - 1) : 1;
+        const long r0 = (long)b * W, h0 = ((long)b * T + col) * W;
+        const int nlive = MULTI ? __ldcg(hlive + (long)b * T + T - 1)
+                                : t > 0 ? __ldcg(hlive + (long)b * T + t - 1) : stream ? __ldcg(hlive + (long)b * T + T - 1) : 1;
         __syncthreads();                                     // the previous utterance is done with shared memory
-        if (t >= __ldg(p.tok_in + b)) {                      // frozen: the beam stays, the predictor rests
+        int nopen = nlive;
+        if (MULTI) {
+            if (tid == 0) misc[5] = 0;
+            __syncthreads();
+            int open = 0;
+            for (int q = tid; q < nlive; q += nt) {
+                sopen[q] = jr == 0 || __ldcg(p.tok_out + r0 + q) != blank;
+                open += sopen[q];
+            }
+            if (open) atomicAdd(&misc[5], open);
+            __syncthreads();
+            nopen = misc[5];
+            if (t >= __ldg(p.tok_in + b) || nopen == 0) {   // frozen, or the frame has ended: the beam stays as it is
+                for (int s = tid; s < W; s += nt) {
+                    p.tok_out[r0 + s] = blank;
+                    p.src[r0 + s] = (int)(r0 + s);
+                    if (lm) p.tok_out2[r0 + s] = -1;
+                }
+                for (int s = 0; s < nlive; ++s) {
+                    const int* ps = p.seq_in + (r0 + s) * LS;
+                    int* d = p.seq_out + (r0 + s) * LS;
+                    const int n = __ldcg(ps) + 3;
+                    for (int i = tid; i < n; i += nt) d[i] = __ldcg(ps + i);
+                }
+                continue;
+            }
+        } else if (t >= __ldg(p.tok_in + b)) {               // frozen: the beam stays, the predictor rests
             for (int j = tid; j < W; j += nt) {
                 hpar[h0 + j] = j;
                 htok[h0 + j] = blank;
@@ -480,6 +534,10 @@ __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
         }
         // per-row log-softmax statistics (warp per row)
         for (int q = warp; q < nlive; q += nt >> 5) {
+            if (MULTI && !sopen[q]) {                        // a stay needs only the slot's log p
+                if (lane == 0) rowlp[q] = __ldcg(p.y + r0 + q);
+                continue;
+            }
             const float* x = p.x1 + (r0 + q) * p.ldx1;
             float m = -INFINITY;
             for (int k = lane; k < V; k += 32) m = fmaxf(m, __ldcg(x + k));
@@ -522,7 +580,11 @@ __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
             v = v + rowlp[q];
             return ((unsigned long long)order_key(v) << 32) | tie_key((unsigned)(q * V + k));
         };
-        const int nsel = (int)min((long)W, (long)nlive * V);
+        // a closed slot's (MULTI) one candidate, its stay: value logp[q], flat index q*V + blank
+        auto stay = [&](int q) -> unsigned long long {
+            return ((unsigned long long)order_key(rowlp[q]) << 32) | tie_key((unsigned)(q * V + blank));
+        };
+        const int nsel = (int)min((long)W, (long)nopen * V + (nlive - nopen));
         unsigned need = nsel;
         unsigned long long prefix = 0, mask = 0;
         for (int shift = 56; shift >= 0; shift -= 8) {
@@ -530,6 +592,11 @@ __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
             __syncthreads();
             for (int q = 0; q < nlive; ++q) {
                 const float* x = p.x1 + (r0 + q) * p.ldx1;
+                if (MULTI && !sopen[q]) {                    // a closed slot: its stay alone
+                    const unsigned long long c = stay(q);
+                    if (tid == 0 && (c & mask) == prefix) atomicAdd(&rhist[(c >> shift) & 255], 1u);
+                    continue;
+                }
                 for (int k = tid; k < V; k += nt) {
                     const unsigned long long c = composite(q, k, x);
                     if ((c & mask) == prefix) atomicAdd(&rhist[(c >> shift) & 255], 1u);
@@ -568,6 +635,14 @@ __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
         __syncthreads();
         for (int q = 0; q < nlive; ++q) {
             const float* x = p.x1 + (r0 + q) * p.ldx1;
+            if (MULTI && !sopen[q]) {
+                const unsigned long long c = stay(q);
+                if (tid == 0 && (c & mask) >= prefix) {
+                    const int i = atomicAdd(&misc[3], 1);
+                    if (i < nsel) comp[i] = c;
+                }
+                continue;
+            }
             for (int k = tid; k < V; k += nt) {
                 const unsigned long long c = composite(q, k, x);
                 if ((c & mask) >= prefix) {
@@ -616,7 +691,17 @@ __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
         __syncthreads();
         for (int i = tid; i < nsel; i += nt) {
             int first = i;
-            if (merge) {
+            if (MULTI && merge) {                            // same sequence and same closedness
+                const bool ic = stok[i] == blank || last;
+                for (int j = 0; j < i; ++j) {
+                    if ((stok[j] == blank || last) != ic || slen[j] != slen[i] || shash[j] != shash[i]) continue;
+                    if (seq_equal_ext(p.seq_in + (r0 + spar[i]) * LS, stok[i] != blank ? stok[i] : -1,
+                                      p.seq_in + (r0 + spar[j]) * LS, stok[j] != blank ? stok[j] : -1)) {
+                        first = j;
+                        break;
+                    }
+                }
+            } else if (merge) {
                 const bool ib = stok[i] == blank;
                 for (int j = 0; j < i; ++j) {
                     if ((stok[j] == blank) == ib || slen[j] != slen[i] || shash[j] != shash[i]) continue;
@@ -668,7 +753,10 @@ __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
                 hlp[h] = -INFINITY;
             }
         }
-        if (tid == 0) hlive[(long)b * T + t] = nkept;
+        if (tid == 0) {
+            hlive[(long)b * T + col] = nkept;
+            if (MULTI) hlive[(long)b * T + T - 1] = nkept;  // the live count the next round reads
+        }
         for (int s = 0; s < nkept; ++s) {                    // token sequences of the new beam
             const int i = skept[s], len = slen[i];
             const int* ps = p.seq_in + (r0 + spar[i]) * LS + 3;
@@ -676,6 +764,12 @@ __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
             for (int j = tid; j < len; j += nt) d[j] = (stok[i] != blank && j == len - 1) ? stok[i] : __ldcg(ps + j);
         }
     }
+}
+
+// one call site in the kernel, as before the multi-symbol rounds: a second one costs the matrix phases spills
+__device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
+    if (p.flags & 512) beam_select<true>(p, sm);
+    else beam_select<false>(p, sm);
 }
 
 __device__ __noinline__ void phase_gather(const EbPhase& p) {

@@ -328,7 +328,7 @@ class Transducer(nn.Module):
 
     @torch.no_grad()
     def beam_search(self, xs, xlen=None, W=4, merge=True, *, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1,
-                    lm_token_map=None):
+                    lm_token_map=None, max_symbols=1):
         """SURVEY 8(f) N4: beam decode.  The reference has no beam search in rnnt/ (north_star mentions one); its
         legacy v0 stack holds a batch-1 Graves-style search (models.py:121-202, with no-op `sorted(...)` calls and a
         removed `volatile=` API).  This is a time-synchronous beam under the SAME emission constraint as
@@ -355,8 +355,19 @@ class Transducer(nn.Module):
         map(k) only when the hypothesis emits a non-blank k with map(k) >= 0; there is no end-of-sentence term.  The LM
         runs as in eval mode (no dropout), in the same fp32-accurate arithmetic as the predictor.  Ranking, merging
         (log-add of the fused values) and the final pick are as without LM, and the returned -log p is the negated
-        fused score of the best hypothesis.  With lm_weight = length_bonus = 0 the result is bitwise that of lm=None."""
-        from ..stream_engine import BeamEngine, BEAM_MAX_W, check_lm_args, param_fingerprint
+        fused score of the best hypothesis.  With lm_weight = length_bonus = 0 the result is bitwise that of lm=None.
+
+        Several symbols per frame: ``max_symbols`` = K (1 to 16, as in `greedy_decode`) runs rounds j = 0 .. K-1 in
+        every frame.  Every hypothesis is open at round 0.  An open hypothesis q offers every token k at the value above:
+        blank closes it, a non-blank k extends its sequence and keeps it open unless j = K-1 (the frame has then emitted
+        K symbols, greedy's rule).  A closed hypothesis offers one candidate, its "stay", of value logp[q] with nothing
+        added, ranked at flat index q*V + blank.  Each round keeps the W best candidates (ties as above); hypotheses
+        merge only when both their sequences and their closedness are equal.  A survivor that took a non-blank token
+        steps its predictor (and LM); the others keep their parent's state.  An utterance's frame ends after round K-1
+        or as soon as none of its hypotheses is open.  K = 1 is the search above, bit for bit, and W = 1 gives the
+        non-blank tokens of `greedy_decode(max_symbols=K)`."""
+        from ..stream_engine import BeamEngine, BEAM_MAX_W, check_lm_args, check_max_symbols, param_fingerprint
+        K = check_max_symbols(max_symbols)
         W = operator.index(W)
         if not 1 <= W <= BEAM_MAX_W:
             raise ValueError("beam width W must be in [1, %d], got %d" % (BEAM_MAX_W, W))
@@ -375,14 +386,14 @@ class Transducer(nn.Module):
             frames = scale_length(T, xlen).clamp(max=T).to(torch.int32)
         frames = _lens_to_device(frames.cpu(), h_enc.device)
         # the phase program bakes raw weight pointers: re-homed parameters (FlatAdam, .to(), .float()) rebuild it
-        key = (B, T, W, bool(merge), h_enc.device, param_fingerprint(self), lm_key)
+        key = (B, T, W, bool(merge), K, h_enc.device, param_fingerprint(self), lm_key)
         cache = self.__dict__.setdefault("_beam_engines", {})
         eng = cache.get(key)
         if eng is None:
             cache.clear()                                  # one resident program is enough
             eng = cache[key] = BeamEngine(self, B, T, W, merge=bool(merge), blank=self.blank, lm=lm,
                                           lm_weight=lm_weight, length_bonus=length_bonus, lm_bos=lm_bos,
-                                          lm_token_map=lm_token_map)
+                                          lm_token_map=lm_token_map, max_symbols=K)
         ids, nlogp = eng.run(h_enc, frames)
         ids = ids.cpu().numpy()
         return [[int(k) for k in row if k >= 0] for row in ids], nlogp.clone()

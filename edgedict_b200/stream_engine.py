@@ -21,7 +21,8 @@ from .rnnt.tokenizer import NUL, BOS, UNK
 
 PH_LN, PH_PAIR, PH_LSTM, PH_LINEAR, PH_ARGMAX, PH_COPY, PH_BEAM_SELECT, PH_GATHER, PH_BEAM_FINAL, PH_BEAM_COMMIT, \
     PH_SKIP = range(11)
-F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE, F_LM, F_STREAM, F_FLUSH, F_CONT = 1, 2, 4, 8, 16, 32, 64, 128, 256
+F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE, F_LM, F_STREAM, F_FLUSH, F_CONT, F_ROUNDS = 1, 2, 4, 8, 16, 32, 64, 128, \
+    256, 512
 BEAM_MAX_W = 1024                                     # EB_BEAM_MAX_W
 MAX_SYMBOLS = 16                                      # bounds the program: about (5 + L_dec) * K phases per frame
 
@@ -92,6 +93,69 @@ def greedy_frame(prog, K, S, tok, blank, round_phases):
         round_phases(j)
     for i in skips:
         prog[i].aux = len(prog) - i - 1
+
+
+def beam_state(e, R, Ld, Hd, D, LS, Ll=0, Hl=0):
+    """Allocate on engine ``e`` (its ``dev`` set) the per-slot state of a beam search over R rows, for each parity p
+    in one flat buffer ``e._home[p]``: the predictor state e._st[p] [2 Ld, R, Hd] (h of every layer, then c; views
+    e.dec_h[p] / e.dec_c[p]), its output e.dec_x[p] [R, D], the token sequences e.seqs[p] int32 [R, LS] and, with an LM
+    (Ll > 0), its state e._lst[p] [2 Ll, R, Hl] (e.lm_h[p] / e.lm_c[p]).  One COPY of e._home[1] into e._home[0] moves
+    all of it, which a round of a multi-symbol frame needs (beam_frame)."""
+    sizes = [2 * Ld * R * Hd, R * D, R * LS, 2 * Ll * R * Hl]
+    offs = [0]
+    for n in sizes:
+        offs.append(offs[-1] + -(-n // 64) * 64)           # 256-byte aligned segments
+    assert offs[-1] < 2 ** 31
+    e._home = torch.zeros(2, offs[-1], dtype=torch.float32, device=e.dev)
+    seg = lambda p, i: e._home[p, offs[i]:offs[i] + sizes[i]]
+    e._st = [seg(p, 0).view(2 * Ld, R, Hd) for p in (0, 1)]
+    e.dec_h, e.dec_c = [s[:Ld] for s in e._st], [s[Ld:] for s in e._st]
+    e.dec_x = [seg(p, 1).view(R, D) for p in (0, 1)]
+    e.seqs = [seg(p, 2).view(torch.int32).view(R, LS) for p in (0, 1)]
+    e._lst = [seg(p, 3).view(2 * Ll, R, Hl) for p in (0, 1)] if Ll else None
+    if Ll:
+        e.lm_h, e.lm_c = [s[:Ll] for s in e._lst], [s[Ll:] for s in e._lst]
+
+
+def beam_frame(prog, e, t, x_enc, ldx_enc, sel, step):
+    """Append encoder frame t of the beam search, the same for BeamEngine and StreamBeamEngine (engine ``e``): up to
+    K = e.max_symbols rounds of joint hidden (the encoder frame at x_enc, row stride ldx_enc, shared by an utterance's W
+    rows) and logits, BEAM_SELECT (``sel``: its fields common to every round), GATHER of the parents' predictor (and
+    LM) state, and ``step(h)``, which appends the masked predictor (and LM) steps on state buffer h.
+
+    K = 1 is the one-symbol frame: the state alternates between the buffers by frame parity.  For K > 1 the number of
+    rounds a frame runs is known only on the device (SKIP, greedy_frame), so the state ends every round in buffer 0:
+    GATHER writes buffer 1 and one COPY moves it back."""
+    K, R = e.max_symbols, e.R
+    w1, b1, w2, b2 = e._joint
+    J, V = w1.shape[0], w2.shape[0]
+    D = e.dec_x[0].shape[1]
+    E = w1.shape[1] - D
+
+    def round_phases(j):
+        p, q = (t & 1, 1 - (t & 1)) if K == 1 else (0, 1)
+        prog.append(EbPhase(type=PH_LINEAR, S=R, N=J, flags=F_TANH, K1=E, x1=x_enc, ldx1=ldx_enc, x1_div=e.W,
+                            w1=_ptr(w1), ldw1=E + D, K2=D, x2=_ptr(e.dec_x[p]), ldx2=D, w2=_ptr(w1, E), ldw2=E + D,
+                            b1=_ptr(b1), y=_ptr(e.hidden), ldy=J))
+        prog.append(EbPhase(type=PH_LINEAR, S=R, N=V, K1=J, x1=_ptr(e.hidden), ldx1=J, w1=_ptr(w2), ldw1=J,
+                            b1=_ptr(b2), y=_ptr(e.logits), ldy=V))
+        ph = EbPhase(hist_col=t * K + j, seq_in=_ptr(e.seqs[p]), seq_out=_ptr(e.seqs[q]), **sel)
+        if K > 1:
+            ph.flags |= F_ROUNDS
+            ph.ldw2 = K
+        prog.append(ph)
+        Ld, Hd = e._st[0].shape[0] // 2, e._st[0].shape[2]
+        prog.append(EbPhase(type=PH_GATHER, S=R, N=Hd, aux=2 * Ld, x1=_ptr(e._st[p]), y=_ptr(e._st[q]), K2=D,
+                            x2=_ptr(e.dec_x[p]), y2=_ptr(e.dec_x[q]), src=_ptr(e.src)))
+        if e._lst is not None:
+            prog.append(EbPhase(type=PH_GATHER, S=R, N=e._lst[0].shape[2], aux=e._lst[0].shape[0],
+                                x1=_ptr(e._lst[p]), y=_ptr(e._lst[q]), src=_ptr(e.src)))
+        if K > 1:
+            prog.append(EbPhase(type=PH_COPY, S=1, N=e._home.shape[1], x1=_ptr(e._home[1]), y=_ptr(e._home[0])))
+            q = 0
+        step(q)
+
+    greedy_frame(prog, K, R, e.tok, e.blank, round_phases)
 
 
 def lm_state_dict(lm):
@@ -448,12 +512,13 @@ class GreedyEngine:
 
 class BeamEngine:
     """Device-side batched beam search (Transducer.beam_search): the time-synchronous beam under greedy_decode's
-    emission rule (at most one symbol per encoder frame) for B utterances of W slots each, in ONE cooperative kernel
-    launch.  Row r = b*W + j holds slot j of utterance b.  Per frame: joint hidden (the encoder frame shared by the
-    utterance's W rows) and logits for every row, BEAM_SELECT (log-softmax, exact top-W of the live slots' candidates,
+    emission rule (at most one symbol per encoder frame, or K with ``max_symbols`` = K: see beam_frame and
+    Transducer.beam_search) for B utterances of W slots each, in ONE cooperative kernel launch.  Row r = b*W + j
+    holds slot j of utterance b.  Per frame: joint hidden (the encoder frame shared by the utterance's W rows) and logits for every row, BEAM_SELECT (log-softmax, exact top-W of the live slots' candidates,
     ties to the lowest flat index slot*V + token, merge of equal token sequences by log-add when ``merge``), GATHER of
     the parents' predictor state, and the masked predictor step for the survivors that emitted a non-blank.  The
-    predictor state alternates between two buffers by frame parity (a permutation cannot be gathered in place).
+    predictor state alternates between two buffers by frame parity (a permutation cannot be gathered in place; with
+    K > 1 every round gathers into buffer 1 and copies back to buffer 0).
     BEAM_FINAL picks the best live slot of each utterance and walks its back-pointers.
 
     ``hist_parent`` / ``hist_token`` / ``hist_logp`` [B, T', W] and ``hist_live`` [B, T'] keep the beam of every
@@ -466,7 +531,12 @@ class BeamEngine:
     rows (a row that did not step gets its parent's logits bit for bit, rows being independent)."""
 
     def __init__(self, transducer, batch, t_out, W, merge=True, blank=NUL, max_ctas=0, lm=None, lm_weight=0.0,
-                 length_bonus=0.0, lm_bos=1, lm_token_map=None):
+                 length_bonus=0.0, lm_bos=1, lm_token_map=None, max_symbols=1):
+        """``max_symbols`` = K: up to K rounds per encoder frame (Transducer.beam_search states the rule).  The history
+        then has one column per round, [B, T' * K, W] (column t*K + j; a round a row did not take holds parent = slot,
+        token = blank and live count 0, except the last column, which holds the final live count), and ``ids`` is
+        [B, T' * K]."""
+        K = check_max_symbols(max_symbols)
         if not 1 <= W <= BEAM_MAX_W:
             raise ValueError("beam width must be in [1, %d], got %r" % (BEAM_MAX_W, W))
         fusion = check_lm_args(lm, transducer.joint.joint[2].weight.shape[0], lm_weight, length_bonus, lm_bos,
@@ -477,80 +547,67 @@ class BeamEngine:
             raise RuntimeError("BeamEngine needs the model on a CUDA device")
         f32, i32 = torch.float32, torch.int32
         B, T, R = batch, t_out, batch * W
-        self.B, self.T, self.W, self.merge, self.blank, self.max_ctas = B, T, W, merge, blank, max_ctas
+        TK = T * K                                             # history columns: one per round
+        self.B, self.T, self.W, self.R, self.merge, self.blank, self.max_ctas, self.max_symbols = \
+            B, T, W, R, merge, blank, max_ctas, K
         z = lambda *shape, dtype=f32: torch.zeros(*shape, dtype=dtype, device=self.dev)
         Ld, Hd = dec.lstm.num_layers, dec.lstm.hidden_size
         D = dec.proj.weight.shape[0]
         J, V = joint[0].weight.shape[0], joint[2].weight.shape[0]
         E = joint[0].weight.shape[1] - D
         self.h_enc, self.frames = z(B, T, E), z(B, dtype=i32)
-        st = [z(2 * Ld, R, Hd), z(2 * Ld, R, Hd)]              # [h of every layer | c of every layer], per parity
-        self.dec_h, self.dec_c = [s[:Ld] for s in st], [s[Ld:] for s in st]
-        self.dec_x = [z(R, D), z(R, D)]
-        self.dec_htmp, self.hidden, self.logits = z(Ld, R, Hd), z(R, J), z(R, V)
-        self.tok, self.src, self.logp = z(R, dtype=i32), z(R, dtype=i32), z(R)
-        self.seqs = z(2, R, T + 3, dtype=i32)                  # {len, hash lo, hash hi, tokens} per row, per parity
-        n = B * T * W
-        self.hist = z(3 * n + B * T, dtype=i32)
-        self.hist_parent = self.hist[:n].view(B, T, W)
-        self.hist_token = self.hist[n:2 * n].view(B, T, W)
-        self.hist_logp = self.hist[2 * n:3 * n].view(f32).view(B, T, W)
-        self.hist_live = self.hist[3 * n:].view(B, T)
-        self.ids, self.nlogp = z(B, max(T, 1), dtype=i32), z(B)
-        self._keep = [p.detach() for p in transducer.parameters()]
-        prog = []
-        _dec_phases(prog, dec, R, self.dec_h[0], self.dec_c[0], self.dec_htmp, self.dec_x[0], self.tok, blank,
-                    masked=False)                         # prime every row with BOS from the zero state
         self.lm = fusion is not None
         if self.lm:
             lsd, lw, lb, self.lm_bos, tmap = fusion
             # the weights are read in place when they already are fp32 on this device (tied weights stay tied)
             lsd = {k: v.to(self.dev, f32).contiguous() for k, v in lsd.items()}
-            self._keep += list(lsd.values())
             Ll = (len(lsd) - 3) // 4
             lm_layers = [tuple(lsd["rnn.%s_l%d" % (n, k)] for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"))
                          for k in range(Ll)]
             Hl, ntok = lm_layers[0][1].shape[1], lsd["encoder.weight"].shape[0]
-            lst = [z(2 * Ll, R, Hl), z(2 * Ll, R, Hl)]         # as st, for the LM
-            self.lm_h, self.lm_c = [s[:Ll] for s in lst], [s[Ll:] for s in lst]
+        # per parity: predictor state, its output, {len, hash lo, hash hi, tokens} per row and the LM state
+        beam_state(self, R, Ld, Hd, D, TK + 3, *((Ll, Hl) if self.lm else ()))
+        self.dec_htmp, self.hidden, self.logits = z(Ld, R, Hd), z(R, J), z(R, V)
+        self.tok, self.src, self.logp = z(R, dtype=i32), z(R, dtype=i32), z(R)
+        n = B * TK * W
+        self.hist = z(3 * n + B * TK, dtype=i32)
+        self.hist_parent = self.hist[:n].view(B, TK, W)
+        self.hist_token = self.hist[n:2 * n].view(B, TK, W)
+        self.hist_logp = self.hist[2 * n:3 * n].view(f32).view(B, TK, W)
+        self.hist_live = self.hist[3 * n:].view(B, TK)
+        self._slots = torch.arange(W, dtype=i32, device=self.dev)
+        self.ids, self.nlogp = z(B, max(TK, 1), dtype=i32), z(B)
+        self._keep = [p.detach() for p in transducer.parameters()]
+        self._joint = (joint[0].weight, joint[0].bias, joint[2].weight, joint[2].bias)
+        prog = []
+        _dec_phases(prog, dec, R, self.dec_h[0], self.dec_c[0], self.dec_htmp, self.dec_x[0], self.tok, blank,
+                    masked=False)                         # prime every row with BOS from the zero state
+        if self.lm:
+            self._keep += list(lsd.values())
             self.lm_htmp, self.lm_logits, self.lm_tok = z(Ll, R, Hl), z(R, ntok), z(R, dtype=i32)
             self.lm_map = tmap.to(self.dev, i32)
             self.lm_fuse = torch.tensor([lw, lb], dtype=f32, device=self.dev)
-            self._lst0 = lst[0]
 
             def lm_phases(q, masked):
                 predictor_phases(prog, lsd["encoder.weight"], lm_layers, lsd["decoder.weight"], lsd["decoder.bias"],
                                  R, self.lm_h[q], self.lm_c[q], self.lm_htmp, self.lm_logits, self.lm_tok, -1, masked)
             lm_phases(0, masked=False)                           # prime every row with lm_bos from the zero state
-        w1 = joint[0].weight
-        for t in range(T):
-            p, q = t & 1, 1 - (t & 1)
-            prog.append(EbPhase(type=PH_LINEAR, S=R, N=J, flags=F_TANH, K1=E, x1=_ptr(self.h_enc, t * E), ldx1=T * E,
-                                x1_div=W, w1=_ptr(w1), ldw1=E + D, K2=D, x2=_ptr(self.dec_x[p]), ldx2=D,
-                                w2=_ptr(w1, E), ldw2=E + D, b1=_ptr(joint[0].bias), y=_ptr(self.hidden), ldy=J))
-            prog.append(EbPhase(type=PH_LINEAR, S=R, N=V, K1=J, x1=_ptr(self.hidden), ldx1=J,
-                                w1=_ptr(joint[2].weight), ldw1=J, b1=_ptr(joint[2].bias), y=_ptr(self.logits), ldy=V))
-            sel = EbPhase(type=PH_BEAM_SELECT, S=B, N=V, aux=W, aux2=blank, flags=F_MERGE if merge else 0,
-                          x1=_ptr(self.logits), ldx1=V, y=_ptr(self.logp), tok_in=_ptr(self.frames),
-                          tok_out=_ptr(self.tok), src=_ptr(self.src), hist=_ptr(self.hist), hist_ld=T,
-                          hist_col=t, seq_in=_ptr(self.seqs[p]), seq_out=_ptr(self.seqs[q]))
-            if self.lm:
-                sel.flags |= F_LM
-                sel.x2, sel.ldx2, sel.K2 = _ptr(self.lm_logits), ntok, ntok
-                sel.fuse, sel.tok_map, sel.tok_out2 = _ptr(self.lm_fuse), _ptr(self.lm_map), _ptr(self.lm_tok)
-            prog.append(sel)
-            prog.append(EbPhase(type=PH_GATHER, S=R, N=Hd, aux=2 * Ld, x1=_ptr(st[p]), y=_ptr(st[q]), K2=D,
-                                x2=_ptr(self.dec_x[p]), y2=_ptr(self.dec_x[q]), src=_ptr(self.src)))
-            if self.lm:
-                prog.append(EbPhase(type=PH_GATHER, S=R, N=Hl, aux=2 * Ll, x1=_ptr(lst[p]), y=_ptr(lst[q]),
-                                    src=_ptr(self.src)))
+        sel = dict(type=PH_BEAM_SELECT, S=B, N=V, aux=W, aux2=blank, flags=F_MERGE if merge else 0,
+                   x1=_ptr(self.logits), ldx1=V, y=_ptr(self.logp), tok_in=_ptr(self.frames), tok_out=_ptr(self.tok),
+                   src=_ptr(self.src), hist=_ptr(self.hist), hist_ld=TK)
+        if self.lm:
+            sel.update(flags=sel["flags"] | F_LM, x2=_ptr(self.lm_logits), ldx2=ntok, K2=ntok, fuse=_ptr(self.lm_fuse),
+                       tok_map=_ptr(self.lm_map), tok_out2=_ptr(self.lm_tok))
+
+        def step(q):
             _dec_phases(prog, dec, R, self.dec_h[q], self.dec_c[q], self.dec_htmp, self.dec_x[q], self.tok, blank,
                         masked=True)
             if self.lm:
                 lm_phases(q, masked=True)
+        for t in range(T):
+            beam_frame(prog, self, t, _ptr(self.h_enc, t * E), T * E, sel, step)
         prog.append(EbPhase(type=PH_BEAM_FINAL, S=B, aux=W, aux2=blank, y=_ptr(self.logp), hist=_ptr(self.hist),
-                            hist_ld=T, tok_out=_ptr(self.ids), ldy=self.ids.shape[1], y2=_ptr(self.nlogp)))
-        self._st0 = st[0]
+                            hist_ld=TK, tok_out=_ptr(self.ids), ldy=self.ids.shape[1], y2=_ptr(self.nlogp)))
         self.nphase = len(prog)
         arr = (EbPhase * len(prog))(*prog)
         self._prog = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(self.dev)
@@ -563,13 +620,18 @@ class BeamEngine:
         -log p [B] of that hypothesis, the negated fused score with an LM)."""
         self.h_enc.copy_(h_enc)
         self.frames.copy_(frames)
-        self._st0.zero_()
+        self._st[0].zero_()
         self.seqs[0].zero_()
         self.logp.fill_(float("-inf"))
         self.logp.view(self.B, self.W)[:, 0] = 0.0
         self.tok.fill_(BOS)
+        if self.max_symbols > 1 and self.T > 0:  # what a round a row does not take leaves: parent = slot, token = blank
+            self.hist_parent.copy_(self._slots.expand_as(self.hist_parent))
+            self.hist_token.fill_(self.blank)
+            self.hist_live.zero_()
+            self.hist_live[:, -1] = 1                           # the live count every round reads and writes
         if self.lm:
-            self._lst0.zero_()
+            self._lst[0].zero_()
             self.lm_tok.fill_(self.lm_bos)
         check(lib().eb_decode_run(self._prog.data_ptr(), self.nphase, self._bar.data_ptr(), self.max_ctas,
                                   torch.cuda.current_stream().cuda_stream), "eb_decode_run")
@@ -600,7 +662,9 @@ class StreamBeamEngine:
     like Transducer.beam_search, does not apply it."""
 
     def __init__(self, transducer, n_streams, frames_per_chunk, W, merge=True, lm=None, lm_weight=0.0,
-                 length_bonus=0.0, lm_bos=1, lm_token_map=None, max_pending=64, state=None, blank=NUL, max_ctas=0):
+                 length_bonus=0.0, lm_bos=1, lm_token_map=None, max_pending=64, state=None, blank=NUL, max_ctas=0,
+                 max_symbols=1):
+        K = check_max_symbols(max_symbols)
         W = operator.index(W)
         if not 1 <= W <= BEAM_MAX_W:
             raise ValueError("beam width must be in [1, %d], got %r" % (BEAM_MAX_W, W))
@@ -614,17 +678,17 @@ class StreamBeamEngine:
         T = stream_frames_out(enc, n)
         if T < 1:
             raise ValueError("a chunk of %d frames gives no encoder output frame" % n)
-        if P < T:
-            raise ValueError("max_pending (%d) must be at least the encoder frames per chunk (%d): a chunk can add "
-                             "that many tokens to a hypothesis" % (P, T))
+        if P < T * K:
+            raise ValueError("max_pending (%d) must be at least the encoder frames per chunk times max_symbols (%d x %d):"
+                             " a chunk can add that many tokens to a hypothesis" % (P, T, K))
         assert C.sizeof(EbPhase) == lib().eb_decode_phase_size(), "EbPhase layout mismatch"
         self.dev = enc.norm.weight.device
         if self.dev.type != "cuda":
             raise RuntimeError("StreamBeamEngine needs the model on a CUDA device")
         f32, i32 = torch.float32, torch.int32
-        R, LS = S * W, P + 3
-        self.S, self.n, self.W, self.merge, self.blank, self.max_ctas, self.max_pending = S, n, W, merge, blank, \
-            max_ctas, P
+        R, LS, TK = S * W, P + 3, T * K
+        self.S, self.n, self.W, self.R, self.merge, self.blank, self.max_ctas, self.max_pending, self.max_symbols = \
+            S, n, W, R, merge, blank, max_ctas, P, K
         z = lambda *shape, dtype=f32: torch.zeros(*shape, dtype=dtype, device=self.dev)
         self._keep = [p.detach() for p in transducer.parameters()]      # weights are read in place
         self.fingerprint = param_fingerprint(transducer)
@@ -635,23 +699,6 @@ class StreamBeamEngine:
         Ld, Hd = dec.lstm.num_layers, dec.lstm.hidden_size
         D = dec.proj.weight.shape[0]
         J = joint[0].weight.shape[0]
-        st = [z(2 * Ld, R, Hd), z(2 * Ld, R, Hd)]              # [h of every layer | c of every layer], per parity
-        self.dec_h, self.dec_c = [s[:Ld] for s in st], [s[Ld:] for s in st]
-        self.dec_x = [z(R, D), z(R, D)]
-        self.dec_htmp, self.hidden, self.logits = z(Ld, R, Hd), z(R, J), z(R, V)
-        self.tok, self.src, self.logp = z(R, dtype=i32), z(R, dtype=i32), z(R)
-        self.frames = torch.full((S,), T, dtype=i32, device=self.dev)      # a stream never freezes
-        self.seqs = z(2, R, LS, dtype=i32)     # {suffix length, hash lo, hash hi, tokens since the last commit}
-        nh = S * T * W
-        self.hist = z(3 * nh + S * T, dtype=i32)
-        self.hist_live = self.hist[3 * nh:].view(S, T)        # column T-1 carries the live count between launches
-        self._out = z(S * P + 2 * S, dtype=i32)               # committed ids [S, P] | counts [S] | collapsed [S]
-        self._host = torch.zeros(self._out.shape, dtype=i32).pin_memory()
-        self.n_collapses = 0
-        self._st, self._lst = st, None
-        prime = []
-        _dec_phases(prime, dec, R, self.dec_h[0], self.dec_c[0], self.dec_htmp, self.dec_x[0], self.tok, blank,
-                    masked=False)
         self.lm = fusion is not None
         if self.lm:
             lsd, lw, lb, self.lm_bos, tmap = fusion
@@ -661,8 +708,24 @@ class StreamBeamEngine:
             lm_layers = [tuple(lsd["rnn.%s_l%d" % (nm, k)] for nm in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"))
                          for k in range(Ll)]
             Hl, ntok = lm_layers[0][1].shape[1], lsd["encoder.weight"].shape[0]
-            self._lst = [z(2 * Ll, R, Hl), z(2 * Ll, R, Hl)]
-            self.lm_h, self.lm_c = [s[:Ll] for s in self._lst], [s[Ll:] for s in self._lst]
+        # per parity: predictor state, its output, {suffix length, hash lo, hash hi, tokens since the last commit} per
+        # row and the LM state
+        beam_state(self, R, Ld, Hd, D, LS, *((Ll, Hl) if self.lm else ()))
+        st = self._st
+        self.dec_htmp, self.hidden, self.logits = z(Ld, R, Hd), z(R, J), z(R, V)
+        self.tok, self.src, self.logp = z(R, dtype=i32), z(R, dtype=i32), z(R)
+        self.frames = torch.full((S,), T, dtype=i32, device=self.dev)      # a stream never freezes
+        nh = S * TK * W
+        self.hist = z(3 * nh + S * TK, dtype=i32)
+        self.hist_live = self.hist[3 * nh:].view(S, TK)       # the last column carries the live count between launches
+        self._out = z(S * P + 2 * S, dtype=i32)               # committed ids [S, P] | counts [S] | collapsed [S]
+        self._host = torch.zeros(self._out.shape, dtype=i32).pin_memory()
+        self.n_collapses = 0
+        self._joint = (joint[0].weight, joint[0].bias, joint[2].weight, joint[2].bias)
+        prime = []
+        _dec_phases(prime, dec, R, self.dec_h[0], self.dec_c[0], self.dec_htmp, self.dec_x[0], self.tok, blank,
+                    masked=False)
+        if self.lm:
             self.lm_htmp, self.lm_logits, self.lm_tok = z(Ll, R, Hl), z(R, ntok), z(R, dtype=i32)
             self._lm_logits_tmp = z(R, ntok)
             self.lm_map = tmap.to(self.dev, i32)
@@ -672,32 +735,20 @@ class StreamBeamEngine:
                 predictor_phases(pr, lsd["encoder.weight"], lm_layers, lsd["decoder.weight"], lsd["decoder.bias"],
                                  R, self.lm_h[q], self.lm_c[q], self.lm_htmp, self.lm_logits, self.lm_tok, -1, masked)
             lm_phases(prime, 0, masked=False)
-        w1 = joint[0].weight
-        for t in range(T):
-            p, q = t & 1, 1 - (t & 1)
-            prog.append(EbPhase(type=PH_LINEAR, S=R, N=J, flags=F_TANH, K1=E, x1=_ptr(self.enc_out, t * E), ldx1=T * E,
-                                x1_div=W, w1=_ptr(w1), ldw1=E + D, K2=D, x2=_ptr(self.dec_x[p]), ldx2=D,
-                                w2=_ptr(w1, E), ldw2=E + D, b1=_ptr(joint[0].bias), y=_ptr(self.hidden), ldy=J))
-            prog.append(EbPhase(type=PH_LINEAR, S=R, N=V, K1=J, x1=_ptr(self.hidden), ldx1=J,
-                                w1=_ptr(joint[2].weight), ldw1=J, b1=_ptr(joint[2].bias), y=_ptr(self.logits), ldy=V))
-            sel = EbPhase(type=PH_BEAM_SELECT, S=S, N=V, aux=W, aux2=blank, flags=F_STREAM | (F_MERGE if merge else 0),
-                          K1=LS, x1=_ptr(self.logits), ldx1=V, y=_ptr(self.logp), tok_in=_ptr(self.frames),
-                          tok_out=_ptr(self.tok), src=_ptr(self.src), hist=_ptr(self.hist), hist_ld=T,
-                          hist_col=t, seq_in=_ptr(self.seqs[p]), seq_out=_ptr(self.seqs[q]))
-            if self.lm:
-                sel.flags |= F_LM
-                sel.x2, sel.ldx2, sel.K2 = _ptr(self.lm_logits), ntok, ntok
-                sel.fuse, sel.tok_map, sel.tok_out2 = _ptr(self.lm_fuse), _ptr(self.lm_map), _ptr(self.lm_tok)
-            prog.append(sel)
-            prog.append(EbPhase(type=PH_GATHER, S=R, N=Hd, aux=2 * Ld, x1=_ptr(st[p]), y=_ptr(st[q]), K2=D,
-                                x2=_ptr(self.dec_x[p]), y2=_ptr(self.dec_x[q]), src=_ptr(self.src)))
-            if self.lm:
-                prog.append(EbPhase(type=PH_GATHER, S=R, N=Hl, aux=2 * Ll, x1=_ptr(self._lst[p]),
-                                    y=_ptr(self._lst[q]), src=_ptr(self.src)))
+        sel = dict(type=PH_BEAM_SELECT, S=S, N=V, aux=W, aux2=blank, flags=F_STREAM | (F_MERGE if merge else 0),
+                   K1=LS, x1=_ptr(self.logits), ldx1=V, y=_ptr(self.logp), tok_in=_ptr(self.frames),
+                   tok_out=_ptr(self.tok), src=_ptr(self.src), hist=_ptr(self.hist), hist_ld=TK)
+        if self.lm:
+            sel.update(flags=sel["flags"] | F_LM, x2=_ptr(self.lm_logits), ldx2=ntok, K2=ntok, fuse=_ptr(self.lm_fuse),
+                       tok_map=_ptr(self.lm_map), tok_out2=_ptr(self.lm_tok))
+
+        def step(q):
             _dec_phases(prog, dec, R, self.dec_h[q], self.dec_c[q], self.dec_htmp, self.dec_x[q], self.tok, blank,
                         masked=True)
             if self.lm:
                 lm_phases(prog, q, masked=True)
+        for t in range(T):
+            beam_frame(prog, self, t, _ptr(self.enc_out, t * E), T * E, sel, step)
 
         def chunk_end(pr, in_parity0, flush):
             """commit (and collapse) from parity 1 into parity 0; state found in parity 0 is copied over first"""
@@ -709,8 +760,8 @@ class StreamBeamEngine:
                     pr.append(EbPhase(type=PH_COPY, S=2 * Ll * R, N=Hl, x1=_ptr(self._lst[0]), y=_ptr(self._lst[1])))
             if self.lm:
                 pr.append(EbPhase(type=PH_COPY, S=R, N=ntok, x1=_ptr(self.lm_logits), y=_ptr(self._lm_logits_tmp)))
-            pr.append(EbPhase(type=PH_BEAM_COMMIT, S=S, N=P, aux=W, aux2=P - T, K1=LS, flags=F_FLUSH if flush else 0,
-                              y=_ptr(self.logp), hist=_ptr(self.hist), hist_ld=T, seq_in=_ptr(self.seqs[1]),
+            pr.append(EbPhase(type=PH_BEAM_COMMIT, S=S, N=P, aux=W, aux2=P - TK, K1=LS, flags=F_FLUSH if flush else 0,
+                              y=_ptr(self.logp), hist=_ptr(self.hist), hist_ld=TK, seq_in=_ptr(self.seqs[1]),
                               seq_out=_ptr(self.seqs[0]), tok_out=_ptr(self._out), tok_out2=_ptr(self._out, S * P),
                               src=_ptr(self.src)))
             pr.append(EbPhase(type=PH_GATHER, S=R, N=Hd, aux=2 * Ld, x1=_ptr(st[1]), y=_ptr(st[0]), K2=D,
@@ -719,11 +770,11 @@ class StreamBeamEngine:
                 pr.append(EbPhase(type=PH_GATHER, S=R, N=Hl, aux=2 * Ll, x1=_ptr(self._lst[1]), y=_ptr(self._lst[0]),
                                   K2=ntok, x2=_ptr(self._lm_logits_tmp), y2=_ptr(self.lm_logits), src=_ptr(self.src)))
 
-        chunk_end(prog, T % 2 == 0, flush=False)
+        chunk_end(prog, K > 1 or T % 2 == 0, flush=False)     # where the frames left the state
         prog.append(EbPhase(type=PH_COPY, S=L * S, N=H, x1=_ptr(self.enc_htmp), y=_ptr(self.enc_h)))
         flush, rebound = [], []
         chunk_end(flush, True, flush=True)
-        chunk_end(rebound, True, flush=False)          # a loaded beam under this engine's bound, max_pending - n_out
+        chunk_end(rebound, True, flush=False)   # a loaded beam under this engine's bound, max_pending - n_out * K
         self.n_chunk_phases, self.n_prime_phases, self.n_flush_phases = len(prog), len(prime), len(flush)
         self._chunk, self._prime, self._flush = _upload(prog, self.dev), _upload(prime, self.dev), \
             _upload(flush, self.dev)

@@ -232,6 +232,11 @@ typedef struct EbPhase {
  *      256 = ARGMAX continuation (round j >= 1 of a multi-symbol greedy frame): a row whose tok_out already holds aux
  *            (blank: its frame ended) writes blank to its hist column, takes no argmax and adds nothing under flag 8;
  *            the other rows run the plain ARGMAX, <unk> rule included.
+ *      512 = BEAM_SELECT runs round j of several per frame (beam search with max_symbols K = ldw2 > 1): hist_col =
+ *            t*K + j over hist_ld = T'*K columns; a slot whose previous round's tok_out is blank is closed and has one
+ *            candidate, its stay (value log p, flat index slot*N + blank); a non-blank token at j = K-1 closes; only
+ *            hypotheses of equal closedness merge; the live count lives in the last history column; a row with no open
+ *            slot (or frozen) keeps its beam and writes no history.
  * SKIP (no flags, writes nothing, no grid barrier): when no row of tok_in[0..S) differs from aux2 (blank), every CTA
  * jumps over the next aux phases.  It reads only data final at the preceding barrier, so all CTAs take the same branch.
  * BEAM_COMMIT (streaming beam, after a chunk's last frame, one CTA per stream): commits the common prefix of the live
