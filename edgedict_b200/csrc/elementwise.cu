@@ -543,20 +543,24 @@ __global__ void cast_bf16_kernel(const float* __restrict__ x, __nv_bfloat16* __r
     if (i < n) for (long k = i; k < n && k < i + 4; ++k) y[k] = __float2bfloat16(x[k]);
 }
 
-// y[c, r] = x[r, c]  (bf16 or fp32 -> bf16), 32x32 tiles through shared memory
+// y[c, r] = x[r, c]  (bf16 or fp32 -> bf16), 32x32 tiles through shared memory.  Column tiles on x, row tiles on y,
+// looped with stride gridDim.y: gridDim.y is capped at 65535, so rows beyond 65535 * 32 take more than one pass.
 template <typename TI>
 __global__ void transpose_to_bf16_kernel(const TI* __restrict__ x, __nv_bfloat16* __restrict__ y,
                                          long rows, long cols) {
     __shared__ float tile[32][33];
-    long c0 = (long)blockIdx.x * 32, r0 = (long)blockIdx.y * 32;
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-        long r = r0 + i, c = c0 + threadIdx.x;
-        tile[i][threadIdx.x] = (r < rows && c < cols) ? (float)x[r * cols + c] : 0.f;
-    }
-    __syncthreads();
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-        long c = c0 + i, r = r0 + threadIdx.x;
-        if (r < rows && c < cols) y[c * rows + r] = __float2bfloat16(tile[threadIdx.x][i]);
+    const long c0 = (long)blockIdx.x * 32;
+    for (long r0 = (long)blockIdx.y * 32; r0 < rows; r0 += (long)gridDim.y * 32) {
+        for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+            long r = r0 + i, c = c0 + threadIdx.x;
+            tile[i][threadIdx.x] = (r < rows && c < cols) ? (float)x[r * cols + c] : 0.f;
+        }
+        __syncthreads();
+        for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+            long c = c0 + i, r = r0 + threadIdx.x;
+            if (r < rows && c < cols) y[c * rows + r] = __float2bfloat16(tile[threadIdx.x][i]);
+        }
+        __syncthreads();                                   // the tile is refilled by the next pass
     }
 }
 
@@ -647,9 +651,9 @@ EB_API int eb_layernorm_fwd(const float* x, const float* res, const float* gamma
 EB_API int eb_layernorm_bwd(const float* dy, const float* x, const float* res, const float* gamma,
                             const float* mean, const float* rstd, float* dz, float* dgamma,
                             float* dbeta, long rows, int H, void* stream) {
-    if (!dy || !x || !gamma || !mean || !rstd || !dz || !dgamma || !dbeta || H > 2048)
+    if (!dy || !x || !gamma || !mean || !rstd || !dz || !dgamma || !dbeta || rows <= 0 || H <= 0 || H > 2048)
         return EB_ERR_INVALID;
-    const bool vec_ok = H % 128 == 0 && H <= 1024 && rows > 0 &&
+    const bool vec_ok = H % 128 == 0 && H <= 1024 &&
                         ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dz) |
                           reinterpret_cast<uintptr_t>(gamma) | (res ? reinterpret_cast<uintptr_t>(res) : 0)) & 15) == 0;
     if (vec_ok) {
@@ -676,13 +680,19 @@ EB_API int eb_layernorm_bwd(const float* dy, const float* x, const float* res, c
 }
 
 EB_API int eb_time_reduce_fwd(const float* x, float* y, void* y_bf16, int B, int T, int H, void* stream) {
+    if (B < 0 || T < 0 || H < 0) return EB_ERR_INVALID;
     long n = (long)B * ((T + 1) / 2) * H;
+    if (n == 0) return EB_OK;
+    if (!x || !y) return EB_ERR_INVALID;
     time_reduce_fwd_kernel<<<ew_grid(n, 256), 256, 0, ST(stream)>>>(x, y, (__nv_bfloat16*)y_bf16, B, T, H);
     EB_CHECK_LAUNCH();
     return EB_OK;
 }
 EB_API int eb_time_reduce_bwd(const float* dy, float* dx, int B, int T, int H, void* stream) {
+    if (B < 0 || T < 0 || H < 0) return EB_ERR_INVALID;
     long n = (long)B * T * H;
+    if (n == 0) return EB_OK;
+    if (!dy || !dx) return EB_ERR_INVALID;
     time_reduce_bwd_kernel<<<ew_grid(n, 256), 256, 0, ST(stream)>>>(dy, dx, B, T, H);
     EB_CHECK_LAUNCH();
     return EB_OK;
@@ -690,8 +700,10 @@ EB_API int eb_time_reduce_bwd(const float* dy, float* dx, int B, int T, int H, v
 
 EB_API int eb_embedding_fwd(const void* ids, int ids_are_int64, const float* W, float* out,
                             void* out_bf16, int B, int U, int E, int prepend_bos, int bos, void* stream) {
+    if (B < 0 || U < 0 || E < 0 || (prepend_bos && bos < 0)) return EB_ERR_INVALID;
     long n = (long)B * (U + (prepend_bos ? 1 : 0)) * E;
-    if (n <= 0) return EB_OK;
+    if (n == 0) return EB_OK;
+    if (!W || !out || (U > 0 && !ids)) return EB_ERR_INVALID;    // U = 0 (priming): ids is never read
     if (ids_are_int64)
         embedding_fwd_kernel<long long><<<ew_grid(n, 256), 256, 0, ST(stream)>>>(
             (const long long*)ids, W, out, (__nv_bfloat16*)out_bf16, B, U, E, prepend_bos ? 1 : 0, bos);
@@ -703,8 +715,10 @@ EB_API int eb_embedding_fwd(const void* ids, int ids_are_int64, const float* W, 
 }
 EB_API int eb_embedding_bwd(const void* ids, int ids_are_int64, const float* dout, float* dW, int B,
                             int U, int E, int prepend_bos, int bos, int pad, void* stream) {
+    if (B < 0 || U < 0 || E < 0 || (prepend_bos && bos < 0)) return EB_ERR_INVALID;
     const long npos = (long)B * (U + (prepend_bos ? 1 : 0));
-    if (npos <= 0 || E <= 0) return EB_OK;
+    if (npos == 0 || E == 0) return EB_OK;
+    if (!dout || !dW || (U > 0 && !ids)) return EB_ERR_INVALID;
     const long n = npos * 32;                                // one warp per position
     if (ids_are_int64)
         embedding_bwd_kernel<long long><<<ew_grid(n, 256), 256, 0, ST(stream)>>>(
@@ -719,8 +733,10 @@ EB_API int eb_embedding_bwd(const void* ids, int ids_are_int64, const float* dou
 EB_API int eb_joint_hidden_fwd(const float* ep, const float* dp, void* hidden, int hidden_bf16, int B,
                                int T, int U, int J, void* stream) {
     if (!ep || !dp || !hidden) return EB_ERR_INVALID;
-    if (hidden_bf16) {
-        if (J % 8) return EB_ERR_INVALID;
+    if (hidden_bf16) {       // 16-byte loads of ep / dp and stores of hidden
+        if (J % 8 || ((reinterpret_cast<uintptr_t>(ep) | reinterpret_cast<uintptr_t>(dp) |
+                       reinterpret_cast<uintptr_t>(hidden)) & 15))
+            return EB_ERR_INVALID;
         joint_hidden_fwd_bf16_kernel<<<B * T, 96, 0, ST(stream)>>>(ep, dp, (__nv_bfloat16*)hidden, T, U, J);
     } else {
         joint_hidden_fwd_f32_kernel<<<B * T, 256, 0, ST(stream)>>>(ep, dp, (float*)hidden, T, U, J);
@@ -732,8 +748,10 @@ EB_API int eb_joint_hidden_fwd(const float* ep, const float* dp, void* hidden, i
 EB_API int eb_joint_hidden_bwd(void* dhidden_inout, const void* hidden, int is_bf16, float* dep,
                                float* ddp, int B, int T, int U, int J, void* stream) {
     if (!dhidden_inout || !hidden || !dep || !ddp) return EB_ERR_INVALID;
-    if (is_bf16) {
-        if (J % 8) return EB_ERR_INVALID;
+    if (is_bf16) {           // 16-byte accesses of every operand
+        if (J % 8 || ((reinterpret_cast<uintptr_t>(dhidden_inout) | reinterpret_cast<uintptr_t>(hidden) |
+                       reinterpret_cast<uintptr_t>(dep) | reinterpret_cast<uintptr_t>(ddp)) & 15))
+            return EB_ERR_INVALID;
         joint_hidden_bwd_t_bf16_kernel<<<B * T, 96, 0, ST(stream)>>>(
             (__nv_bfloat16*)dhidden_inout, (const __nv_bfloat16*)hidden, dep, T, U, J);
         EB_CHECK_LAUNCH();
@@ -752,7 +770,7 @@ EB_API int eb_joint_hidden_bwd(void* dhidden_inout, const void* hidden, int is_b
 // dep[b,t,:] = sum_u, ddp[b,u,:] = sum_t  (backward of the e_t + d_u broadcast add of Joint.forward).
 EB_API int eb_joint_dpre_reduce(const void* dpre16, float* dep, float* ddp, int B, int T, int U, int J, void* stream) {
     if (!dpre16 || !dep || !ddp || B <= 0 || T <= 0 || U <= 0 || J <= 0 || J % 8 ||
-        (reinterpret_cast<uintptr_t>(dpre16) & 15) || (reinterpret_cast<uintptr_t>(dep) & 15))
+        ((reinterpret_cast<uintptr_t>(dpre16) | reinterpret_cast<uintptr_t>(dep) | reinterpret_cast<uintptr_t>(ddp)) & 15))
         return EB_ERR_INVALID;
     joint_dep_reduce_bf16_kernel<<<B * T, 96, 0, ST(stream)>>>((const __nv_bfloat16*)dpre16, dep, U, J);
     EB_CHECK_LAUNCH();
@@ -782,7 +800,11 @@ EB_API int eb_cast_bf16(const float* x, void* y, long n, void* stream) {
 }
 
 EB_API int eb_transpose_to_bf16(const void* x, int x_bf16, void* y, long rows, long cols, void* stream) {
-    dim3 grid((unsigned)((cols + 31) / 32), (unsigned)((rows + 31) / 32));
+    if (rows < 0 || cols < 0 || (cols + 31) / 32 > 0x7fffffffL) return EB_ERR_INVALID;
+    if (rows == 0 || cols == 0) return EB_OK;
+    if (!x || !y) return EB_ERR_INVALID;
+    const long row_tiles = (rows + 31) / 32;
+    dim3 grid((unsigned)((cols + 31) / 32), (unsigned)(row_tiles < 65535 ? row_tiles : 65535));
     if (x_bf16)
         transpose_to_bf16_kernel<__nv_bfloat16><<<grid, dim3(32, 8), 0, ST(stream)>>>(
             (const __nv_bfloat16*)x, (__nv_bfloat16*)y, rows, cols);
@@ -815,6 +837,9 @@ EB_API int eb_adam_step_ex(float* p, const float* g, float* m, float* v, long n,
 }
 
 EB_API int eb_sumsq(const float* x, long n, float* out_accum, void* stream) {
+    if (n < 0 || !out_accum) return EB_ERR_INVALID;
+    if (n == 0) return EB_OK;
+    if (!x) return EB_ERR_INVALID;
     sumsq_kernel<<<ew_grid(n, 256), 256, 0, ST(stream)>>>(x, n, out_accum);
     EB_CHECK_LAUNCH();
     return EB_OK;

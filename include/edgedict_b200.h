@@ -175,7 +175,9 @@ int eb_lstm_c4_bwd_chunks(const float* dy, const float* gates, const float* cseq
                           void* scratch, int B, const int* chunk_lens, int nchunks, int H, void* stream);
 
 /* ---- LayerNorm(x + res) fwd/bwd, TimeReduction, Embedding -------------------------------
- * rnnt/models.py:47,66-69,124 ; :21-29 ; :150-153.  *_bf16 outputs are optional side copies. */
+ * rnnt/models.py:47,66-69,124 ; :21-29 ; :150-153.  *_bf16 outputs are optional side copies.
+ * LayerNorm: rows > 0 and 0 < H <= 2048.  Time reduction and embedding: negative sizes are EB_ERR_INVALID, an empty
+ * output is a no-op, and ids may be NULL when U == 0 (the BOS-only priming input). */
 int eb_layernorm_fwd(const float* x, const float* res, const float* gamma, const float* beta, float* y,
                      void* y_bf16, float* mean, float* rstd, long rows, int H, float eps, void* stream);
 int eb_layernorm_bwd(const float* dy, const float* x, const float* res, const float* gamma,
@@ -189,12 +191,16 @@ int eb_embedding_bwd(const void* ids, int ids_are_int64, const float* dout, floa
                      int U, int E, int prepend_bos, int bos, int pad, void* stream);
 
 /* ---- Joint network pieces (rnnt/models.py:169-179) --------------------------------------
- * hidden[b,t,u,:] = tanh(ep[b,t,:] + dp[b,u,:]) with ep = W1e*h_enc + b1, dp = W1d*h_dec. */
+ * hidden[b,t,u,:] = tanh(ep[b,t,:] + dp[b,u,:]) with ep = W1e*h_enc + b1, dp = W1d*h_dec.
+ * bf16 (hidden_bf16 / is_bf16 = 1, tanh.approx): J % 8 == 0 and every pointer 16-byte aligned, else EB_ERR_INVALID.
+ * In the bf16 backward ddp sums the stored (bf16-rounded) dpre over t, while dep sums the unrounded fp32 products
+ * dh * (1 - h^2) over u: the two reductions do not see the same addends. */
 int eb_joint_hidden_fwd(const float* ep, const float* dp, void* hidden, int hidden_bf16, int B, int T,
                         int U, int J, void* stream);
 int eb_joint_hidden_bwd(void* dhidden_inout, const void* hidden, int is_bf16, float* dep, float* ddp,
                         int B, int T, int U, int J, void* stream);
-/* the same two reductions when d(pre-activation) [B,T,U,J] bf16 is already available (eb_gemm_bf16_dtanh) */
+/* the same two reductions when d(pre-activation) [B,T,U,J] bf16 is already available (eb_gemm_bf16_dtanh);
+ * J % 8 == 0 and dpre16, dep, ddp 16-byte aligned, else EB_ERR_INVALID */
 int eb_joint_dpre_reduce(const void* dpre16, float* dep, float* ddp, int B, int T, int U, int J, void* stream);
 
 /* ---- streaming greedy decode: one persistent kernel per audio chunk -----------------------------
@@ -253,6 +259,7 @@ int eb_decode_run(const void* phases_dev, int nphase, void* barrier_dev, int max
 /* ---- reductions, casts, optimizer -------------------------------------------------------- */
 int eb_colsum(const void* x, int x_bf16, float* out_accum, long rows, int N, void* stream);
 int eb_cast_bf16(const float* x, void* y, long n, void* stream);
+/* eb_transpose_to_bf16: y [cols, rows] = x^T for any rows, cols >= 0 (an empty matrix is a no-op). */
 int eb_transpose_to_bf16(const void* x, int x_bf16, void* y, long rows, long cols, void* stream);
 int eb_adam_step(float* p, const float* g, float* m, float* v, long n, float lr, float beta1,
                  float beta2, float eps, float weight_decay, int step, float grad_scale, void* stream);

@@ -124,6 +124,58 @@ def test_entry_points_reject_bad_arguments_before_touching_the_device(built):
     assert L.eb_joint_dpre_reduce(p, p, p, 1, 1, 1, 12, None) == 2                   # J % 8
     assert L.eb_joint_logits_lse(p, p, None, p, p, p, p, p, p, p, 1, 1, 1, 8, 12, 0, None) == 2   # J % 8
     assert L.eb_joint_logits_lse(p, p, None, p, p, p, p, p, p, p, 1, 1, 1, 8, 8, 9, None) == 2    # blank >= V
+    # the bf16 joint kernels load and store 16 bytes at a time: every operand must be 16-byte aligned
+    for off in (2, 4, 8):
+        assert L.eb_joint_dpre_reduce(p, p, p + off, 1, 1, 1, 8, None) == 2, off          # ddp
+        assert L.eb_joint_dpre_reduce(p, p + off, p, 1, 1, 1, 8, None) == 2, off          # dep
+        for i in range(3):
+            a = [p, p, p]
+            a[i] += off
+            assert L.eb_joint_hidden_fwd(a[0], a[1], a[2], 1, 1, 1, 1, 8, None) == 2, (i, off)
+        for i in range(4):
+            a = [p, p, p, p]
+            a[i] += off
+            assert L.eb_joint_hidden_bwd(a[0], a[1], 1, a[2], a[3], 1, 1, 1, 8, None) == 2, (i, off)
+    assert L.eb_joint_hidden_fwd(p, p, p, 1, 1, 1, 1, 12, None) == 2                  # J % 8
+    assert L.eb_joint_hidden_bwd(p, p, 1, p, p, 1, 1, 1, 12, None) == 2
+    # LayerNorm backward rejects what the forward rejects
+    assert L.eb_layernorm_fwd(p, None, p, p, p, None, p, p, 0, 64, 1e-5, None) == 2
+    assert L.eb_layernorm_bwd(p, p, None, p, p, p, p, p, p, 0, 64, None) == 2          # rows <= 0
+    assert L.eb_layernorm_bwd(p, p, None, p, p, p, p, p, p, -3, 64, None) == 2
+    assert L.eb_layernorm_bwd(p, p, None, p, p, p, p, p, p, 4, 0, None) == 2           # H <= 0
+    assert L.eb_layernorm_bwd(p, p, None, p, p, p, p, p, p, 4, 2049, None) == 2
+    assert L.eb_layernorm_fwd(p, None, p, p, p, None, p, p, 4, 2049, 1e-5, None) == 2
+    # NULL operands and negative sizes; the optional y_bf16 / out_bf16 copies stay optional (an empty output returns
+    # 0 without a launch, which is also what these calls with the copies omitted would reach on a GPU)
+    assert L.eb_time_reduce_fwd(None, p, None, 2, 3, 4, None) == 2
+    assert L.eb_time_reduce_fwd(p, None, p, 2, 3, 4, None) == 2
+    assert L.eb_time_reduce_fwd(p, p, None, -1, 3, 4, None) == 2
+    assert L.eb_time_reduce_fwd(p, p, None, 2, -3, 4, None) == 2
+    assert L.eb_time_reduce_fwd(p, p, None, 2, 3, -4, None) == 2
+    assert L.eb_time_reduce_fwd(None, None, None, 2, 0, 4, None) == 0                # empty: nothing to do
+    assert L.eb_time_reduce_bwd(None, p, 2, 3, 4, None) == 2
+    assert L.eb_time_reduce_bwd(p, None, 2, 3, 4, None) == 2
+    assert L.eb_time_reduce_bwd(p, p, 2, -3, 4, None) == 2
+    assert L.eb_embedding_fwd(None, 0, p, p, None, 2, 3, 4, 1, 2, None) == 2
+    assert L.eb_embedding_fwd(p, 0, None, p, None, 2, 3, 4, 1, 2, None) == 2
+    assert L.eb_embedding_fwd(p, 1, p, None, p, 2, 3, 4, 0, 2, None) == 2
+    assert L.eb_embedding_fwd(p, 0, p, p, None, -2, 3, 4, 1, 2, None) == 2
+    assert L.eb_embedding_fwd(p, 0, p, p, None, 2, -3, 4, 1, 2, None) == 2
+    assert L.eb_embedding_fwd(p, 0, p, p, None, 2, 3, -4, 1, 2, None) == 2
+    assert L.eb_embedding_fwd(p, 0, p, p, None, 2, 3, 4, 1, -1, None) == 2           # BOS row < 0
+    assert L.eb_embedding_bwd(None, 0, p, p, 2, 3, 4, 1, 2, 1, None) == 2
+    assert L.eb_embedding_bwd(p, 0, None, p, 2, 3, 4, 1, 2, 1, None) == 2
+    assert L.eb_embedding_bwd(p, 0, p, None, 2, 3, 4, 1, 2, 1, None) == 2
+    assert L.eb_embedding_bwd(p, 0, p, p, 2, -3, 4, 1, 2, 1, None) == 2
+    assert L.eb_embedding_bwd(p, 0, p, p, 2, 3, 4, 1, -2, 1, None) == 2
+    assert L.eb_transpose_to_bf16(None, 0, p, 8, 8, None) == 2
+    assert L.eb_transpose_to_bf16(p, 1, None, 8, 8, None) == 2
+    assert L.eb_transpose_to_bf16(p, 0, p, -8, 8, None) == 2
+    assert L.eb_transpose_to_bf16(p, 0, p, 8, -8, None) == 2
+    assert L.eb_transpose_to_bf16(None, 0, None, 0, 8, None) == 0                    # empty: nothing to do
+    assert L.eb_sumsq(None, 8, p, None) == 2
+    assert L.eb_sumsq(p, 8, None, None) == 2
+    assert L.eb_sumsq(p, -8, p, None) == 2
     assert L.eb_fe_preemph_pad(None, p, 1, 100, 400, 8, 0.97, 1, None) == 2
     assert L.eb_fe_preemph_pad(p, p, 1, 100, 100, 8, 0.97, 1, None) == 2             # Lp < L + 2*pad
     assert L.eb_fe_power(p, None, 4, 4, None) == 2
