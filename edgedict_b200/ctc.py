@@ -1,0 +1,121 @@
+"""CTC loss on the engine: ``CTCLoss`` / ``ctc_loss`` with the signature and semantics of ``torch.nn.CTCLoss`` /
+``torch.nn.functional.ctc_loss``, computed by this library's kernels (csrc/ctc.cu).
+
+Unlike torch's CUDA ctc_loss, the backward pass is deterministic: the gradient of every utterance is bitwise the same on
+every run and does not depend on the other utterances of the batch, so it may run under
+``torch.use_deterministic_algorithms(True)``.
+
+Accepted inputs:
+  * log_probs: fp32 CUDA tensor (T, N, C), or (T, C) for one unbatched utterance.  Any strides over T and N (the
+    ``.transpose(0, 1)`` view of a [N, T, C] tensor is used without a copy).  Other dtypes raise TypeError, CPU tensors
+    RuntimeError: there is no fallback.
+  * targets: integer tensor, padded (N, S) or the labels of all utterances concatenated (sum(target_lengths),);
+    (S,) for an unbatched input.  Labels are expected in [0, C) and different from blank.  A label outside [0, C) gives
+    the utterance no alignment (cost +inf).
+  * input_lengths / target_lengths: integer tensors or sequences with one entry per utterance (a scalar when
+    unbatched).  They are read on the host; every length is checked there, before anything is launched.
+  * target lengths up to 1023.
+
+reduction: 'none' (per-utterance costs), 'sum', or 'mean' (each cost divided by max(target_length, 1), then the mean over
+the batch).  zero_infinity sets infinite costs (no alignment exists) and their gradients to zero.
+"""
+import operator
+
+import torch
+from torch import nn
+
+from . import functional as Fn
+
+MAX_TARGET_LENGTH = 1023          # 2S+1 lattice states, at most 2047
+
+
+def _lengths(x, n, name):
+    if isinstance(x, torch.Tensor):
+        if x.is_floating_point() or x.is_complex() or x.dtype == torch.bool:
+            raise TypeError("%s must hold integers, got %s" % (name, x.dtype))
+        x = x.detach().reshape(-1).cpu().to(torch.int64)
+    else:
+        if not hasattr(x, "__len__"):
+            x = [x]
+        x = torch.tensor([operator.index(v) for v in x], dtype=torch.int64)
+    if x.numel() != n:
+        raise ValueError("%s must have one entry per utterance (%d), got %d" % (name, n, x.numel()))
+    return x
+
+
+def ctc_loss(log_probs, targets, input_lengths, target_lengths, blank=0, reduction="mean", zero_infinity=False):
+    """torch.nn.functional.ctc_loss on the engine's kernels; see the module docstring."""
+    if not isinstance(log_probs, torch.Tensor) or not isinstance(targets, torch.Tensor):
+        raise TypeError("log_probs and targets must be tensors")
+    if log_probs.dtype != torch.float32:
+        raise TypeError("edgedict_b200 ctc_loss takes fp32 log_probs, got %s (there is no fallback)" % log_probs.dtype)
+    if reduction not in ("none", "mean", "sum"):
+        raise ValueError("reduction must be 'none', 'mean' or 'sum', got %r" % (reduction,))
+    if targets.is_floating_point() or targets.is_complex() or targets.dtype == torch.bool:
+        raise TypeError("targets must hold integers, got %s" % targets.dtype)
+    unbatched = log_probs.dim() == 2
+    if unbatched:
+        if targets.dim() != 1:
+            raise ValueError("an unbatched (T, C) input takes 1-D targets, got shape %s" % (tuple(targets.shape),))
+        log_probs, targets = log_probs.unsqueeze(1), targets.unsqueeze(0)
+    elif log_probs.dim() != 3:
+        raise ValueError("log_probs must be (T, N, C) or (T, C), got shape %s" % (tuple(log_probs.shape),))
+    T, N, V = log_probs.shape
+    if T < 1 or N < 1 or V < 1:
+        raise ValueError("log_probs must not be empty, got shape %s"
+                         % (tuple(log_probs.shape),))
+    blank = operator.index(blank)
+    if not 0 <= blank < V:
+        raise ValueError("blank must lie in [0, %d), got %d" % (V, blank))
+    il = _lengths(input_lengths, N, "input_lengths")
+    tl = _lengths(target_lengths, N, "target_lengths")
+    if bool((il < 0).any()) or bool((il > T).any()):
+        raise ValueError("input_lengths must lie in [0, T = %d], got %s" % (T, il.tolist()))
+    if bool((tl < 0).any()):
+        raise ValueError("target_lengths must be >= 0, got %s" % tl.tolist())
+    if targets.dim() == 2:
+        if targets.shape[0] != N:
+            raise ValueError("padded targets must have %d rows, got %d" % (N, targets.shape[0]))
+        if bool((tl > targets.shape[1]).any()):
+            raise ValueError("target_lengths exceed the padded target length %d" % targets.shape[1])
+        offsets = torch.arange(N, dtype=torch.int64) * targets.shape[1]
+    elif targets.dim() == 1:
+        if int(tl.sum()) != targets.numel():
+            raise ValueError("concatenated targets hold %d labels, target_lengths sum to %d"
+                             % (targets.numel(), int(tl.sum())))
+        offsets = torch.cumsum(tl, 0) - tl
+    else:
+        raise ValueError("targets must be (N, S) or 1-D, got shape %s" % (tuple(targets.shape),))
+    S = int(tl.max())
+    if S > MAX_TARGET_LENGTH:
+        raise ValueError("target lengths above %d are not supported, got %d" % (MAX_TARGET_LENGTH, S))
+    if not log_probs.is_cuda:                  # checked last: every argument error above is found without a GPU
+        raise RuntimeError("edgedict_b200 ctc_loss needs CUDA log_probs (got a %s tensor); there is no CPU path"
+                           % log_probs.device)
+    dev = log_probs.device
+    lens = torch.empty(3, N, dtype=torch.int32, pin_memory=True)
+    lens[0], lens[1], lens[2] = offsets, tl, il
+    lens = lens.to(dev, non_blocking=True)
+    tg = targets.reshape(-1).to(device=dev, dtype=torch.int32).contiguous()
+    if log_probs.stride(-1) != 1:
+        log_probs = log_probs.contiguous()
+    costs = Fn.CTCLossFn.apply(log_probs, tg, lens[0], lens[1], lens[2], (S, blank, bool(zero_infinity)))
+    if reduction == "mean":
+        costs = (costs / lens[1].clamp(min=1).to(costs.dtype)).mean()
+    elif reduction == "sum":
+        costs = costs.sum()
+    elif unbatched:
+        costs = costs[0]
+    return costs
+
+
+class CTCLoss(nn.Module):
+    """torch.nn.CTCLoss on the engine's kernels (see ctc_loss)."""
+
+    def __init__(self, blank=0, reduction="mean", zero_infinity=False):
+        super().__init__()
+        self.blank, self.reduction, self.zero_infinity = blank, reduction, zero_infinity
+
+    def forward(self, log_probs, targets, input_lengths, target_lengths):
+        return ctc_loss(log_probs, targets, input_lengths, target_lengths, self.blank, self.reduction,
+                        self.zero_infinity)

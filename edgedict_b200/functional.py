@@ -668,6 +668,42 @@ class RNNTLossFn(torch.autograd.Function):
         return grads, None, None, None, None, None
 
 
+class LogSoftmax(torch.autograd.Function):
+    """nn.LogSoftmax(dim=-1) of CTCEncoder.tovocab (rnnt/models.py:284-287), fp32 in every precision mode."""
+
+    @staticmethod
+    def forward(ctx, x):
+        y = ops.log_softmax_fwd(_c(x))
+        ctx.save_for_backward(y)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (y,) = ctx.saved_tensors
+        return ops.log_softmax_bwd(_c(dy), y)
+
+
+class CTCLossFn(torch.autograd.Function):
+    """Per-utterance CTC costs [N] of log_probs (T, N, V) (torch.nn.functional.ctc_loss with reduction='none'); the
+    reductions are taken by the caller (edgedict_b200/ctc.py), and autograd hands their per-utterance factors to
+    backward, where the gradient kernel applies them.  meta = (S, blank, zero_infinity)."""
+
+    @staticmethod
+    def forward(ctx, log_probs, targets, offsets, tlen, ilen, meta):
+        S, blank, zero_inf = meta
+        costs, ws = ops.ctc_loss_fwd(log_probs, targets, offsets, tlen, ilen, S, blank, zero_inf)
+        ctx.save_for_backward(log_probs, tlen, ilen, ws)
+        ctx.meta = meta
+        return costs
+
+    @staticmethod
+    def backward(ctx, gcosts):
+        log_probs, tlen, ilen, ws = ctx.saved_tensors
+        S, blank, zero_inf = ctx.meta
+        grad = ops.ctc_loss_bwd(log_probs, tlen, ilen, S, blank, zero_inf, ws, _c(gcosts.to(f32)))
+        return grad, None, None, None, None, None
+
+
 class JointLoss(torch.autograd.Function):
     """Transducer.forward's joint + loss (rnnt/models.py:234-239) as one autograd node: logits are
     produced, consumed by the loss, and their gradient is written IN PLACE over them (fp32 mode)

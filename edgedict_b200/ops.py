@@ -641,6 +641,63 @@ def rnnt_loss_bwd_bf16(logits16, labels, xlen, ylen, blank, ws, gscale, host_sca
     return logits16
 
 
+# ---- CTC (csrc/ctc.cu) -------------------------------------------------------------------------------
+def log_softmax_fwd(x):
+    """Row log-softmax over the last dim of a contiguous fp32 tensor."""
+    _need(x, f32, "x")
+    y = torch.empty_like(x)
+    V = x.shape[-1]
+    with _timed("log_softmax_fwd", 1, 8.0 * x.numel(), 0.0):
+        check(lib().eb_log_softmax_fwd(_p(x), _p(y), x.numel() // V, V, _s()), "eb_log_softmax_fwd")
+    return y
+
+
+def log_softmax_bwd(dy, y):
+    """dx = dy - exp(y) * sum(dy) per row; contiguous fp32 tensors of one shape."""
+    _need(dy, f32, "dy")
+    _need(y, f32, "y")
+    dx = torch.empty_like(y)
+    V = y.shape[-1]
+    with _timed("log_softmax_bwd", 1, 12.0 * y.numel(), 0.0):
+        check(lib().eb_log_softmax_bwd(_p(dy), _p(y), _p(dx), y.numel() // V, V, _s()), "eb_log_softmax_bwd")
+    return dx
+
+
+def ctc_loss_fwd(lp, targets, offsets, tlen, ilen, S, blank, zero_infinity):
+    """lp (T, N, V) fp32 with unit stride over V (any T / N strides); targets int32 (device, 1-D storage of the labels);
+    offsets / tlen / ilen int32 [N] on the device; S >= max(tlen).  Returns (costs [N], workspace)."""
+    T, N, V = lp.shape
+    ws = torch.empty(lib().eb_ctc_workspace_size(N, T, S), dtype=torch.uint8, device=lp.device)
+    costs = torch.empty(N, dtype=f32, device=lp.device)
+    with _timed("ctc_loss_fwd", 1, 4.0 * N * T * (2 * S + 1) * 2, 0.0):
+        check(lib().eb_ctc_loss_fwd(_p(lp), lp.stride(1), lp.stride(0), N, T, V, _p(targets), targets.numel(),
+                                    _p(offsets), _p(tlen), _p(ilen), S, blank, int(zero_infinity), _p(ws), _p(costs),
+                                    _s()), "eb_ctc_loss_fwd")
+    return costs, ws
+
+
+def ctc_loss_bwd(lp, tlen, ilen, S, blank, zero_infinity, ws, gscale):
+    """Gradient for log_probs (same shape and strides as lp), scaled per utterance by gscale [N] (device fp32)."""
+    T, N, V = lp.shape
+    grad = torch.empty_like(lp)
+    with _timed("ctc_loss_bwd", 1, 8.0 * lp.numel(), 0.0):
+        check(lib().eb_ctc_loss_bwd(_p(lp), lp.stride(1), lp.stride(0), _p(grad), grad.stride(1), grad.stride(0), N, T,
+                                    V, _p(tlen), _p(ilen), S, blank, int(zero_infinity), _p(ws), _p(gscale), _s()),
+              "eb_ctc_loss_bwd")
+    return grad
+
+
+def ctc_greedy(lp, xlen, blank):
+    """lp [B, T, V] fp32 (unit stride over V), xlen int32 [B] on the device -> one int32 device buffer
+    [B*T ids | B counts | B neg-scores (fp32 bits)], so that the host needs one copy."""
+    B, T, V = lp.shape
+    out = torch.empty(B * T + 2 * B, dtype=torch.int32, device=lp.device)
+    with _timed("ctc_greedy", 1, 4.0 * lp.numel(), 0.0):
+        check(lib().eb_ctc_greedy(_p(lp), lp.stride(0), lp.stride(1), B, T, V, _p(xlen), blank, _p(out),
+                                  _p(out[B * T:]), _p(out[B * T + B:]), _s()), "eb_ctc_greedy")
+    return out
+
+
 def adam_step(p, g, m, v, lr, beta1, beta2, eps, weight_decay, step, grad_scale=1.0):
     check(lib().eb_adam_step(_p(p), _p(g), _p(m), _p(v), p.numel(), lr, beta1, beta2, eps, weight_decay, step,
                              grad_scale, _s()), "eb_adam_step")

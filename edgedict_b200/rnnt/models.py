@@ -1,7 +1,7 @@
 """H100-native mirror of the reference's ``rnnt/models.py`` hot path.
 
 Same class names, constructor arguments, ``forward`` signatures, return values and
-``state_dict`` keys as the reference's rnnt/models.py:16-269, so ``cli/train.py``,
+``state_dict`` keys as the reference's rnnt/models.py:16-310, so ``cli/train.py``,
 ``cli/baseline.py``, ``cli/lightning.py`` and ``rnnt/stream.py`` can import this module
 unchanged.  The torch ``nn.LSTM`` / ``nn.LayerNorm`` / ``nn.Linear`` / ``nn.Embedding`` objects
 below are PARAMETER CONTAINERS ONLY (identical default initialisation and checkpoint keys); their
@@ -397,6 +397,49 @@ class Transducer(nn.Module):
         ids, nlogp = eng.run(h_enc, frames)
         ids = ids.cpu().numpy()
         return [[int(k) for k in row if k >= 0] for row in ids], nlogp.clone()
+
+
+class CTCEncoder(nn.Module):
+    """rnnt/models.py:272-310: the GRU encoder stack (``model.*``) and a ``Linear(proj_size, vocab_size)`` + LogSoftmax
+    head (``tovocab.0.*``), same constructor and ``state_dict`` keys as the reference.  ``Encoder`` gets
+    ``module=ResLayerNormGRU`` explicitly: that is the reference's default argument, which our ``Encoder`` does not share.
+    Train it with ``edgedict_b200.ctc.CTCLoss`` on ``forward(xs).transpose(0, 1)``.
+
+    Follows ``set_precision``: in bf16 mode the encoder and the projection GEMM run bf16; the log-softmax is fp32 in both
+    modes (csrc/ctc.cu)."""
+
+    def __init__(self, vocab_size, input_size, enc_hidden_size, enc_layers, enc_dropout, proj_size, blank=NUL):
+        super().__init__()
+        self.blank = blank
+        self.model = Encoder(input_size=input_size, hidden_size=enc_hidden_size, num_layers=enc_layers,
+                             dropout=enc_dropout, proj_size=proj_size, module=ResLayerNormGRU)
+        self.tovocab = nn.Sequential(nn.Linear(proj_size, vocab_size), nn.LogSoftmax(dim=-1))
+
+    def set_precision(self, precision):
+        return _set_precision(self, precision)
+
+    def forward(self, xs):
+        """xs [B, T, F] -> log-probs [B, T', V] (fp32)."""
+        xs, _ = self.model(xs)
+        lin = self.tovocab[0]
+        return Fn.LogSoftmax.apply(Fn.Linear.apply(xs, lin.weight, lin.bias, _precision(self)))
+
+    @torch.no_grad()
+    def greedy_decode(self, xs, xlen):
+        """rnnt/models.py:294-310 -> (list of int64 id arrays, -score [B] on the device).  Per frame the argmax (NaN first,
+        ties to the lowest id); frames repeating the previous frame's argmax and blanks are dropped, after truncation to
+        the first xlen frames -- the xlen as passed, not scaled to T' (the reference's behaviour).  The score keeps the
+        reference's quirk: it sums the WHOLE log-prob rows of the kept frames, not the chosen ids' log-probs.  One kernel
+        (eb_ctc_greedy) and one device-to-host copy."""
+        lp = self.forward(xs)
+        B, T = lp.shape[0], lp.shape[1]
+        xl = torch.as_tensor(xlen).reshape(-1).to(torch.int64).clamp(0, T).to(torch.int32)
+        if xl.numel() != B:
+            raise ValueError("xlen must have one entry per utterance (%d), got %d" % (B, xl.numel()))
+        out = ops.ctc_greedy(lp, _lens_to_device(xl.cpu(), lp.device), self.blank)
+        host = out.cpu().numpy()
+        ids, counts = host[:B * T].reshape(B, T), host[B * T:B * T + B]
+        return [ids[i, :int(counts[i])].astype("int64") for i in range(B)], out[B * T + B:].view(torch.float32).clone()
 
 
 def _i32(t):

@@ -41,6 +41,38 @@ int eb_rnnt_loss_bwd_bf16(const void* logits16, void* grads16, const int* labels
 int eb_rnnt_workspace_views(void* workspace, int B, int maxT, int maxU, int dtype_size,
                             void** denom, void** alphas, void** betas, void** ll_fwd, void** ll_bwd);
 
+/* ---- CTC: CTCEncoder's head, loss and greedy decode (csrc/ctc.cu) ------------------------------
+ * replaces tovocab's LogSoftmax and greedy_decode of CTCEncoder (rnnt/models.py:272-310) and torch.nn.CTCLoss.
+ * eb_log_softmax_fwd: y[r,:] = x[r,:] - logsumexp(x[r,:]) over contiguous rows of V floats (y may alias x);
+ * eb_log_softmax_bwd: dx = dy - exp(y) * sum(dy) per row (dx may alias dy).  Fixed reduction order: bitwise repeatable.
+ * eb_ctc_loss_fwd: log_probs element (n, t, v) at log_probs[n*stride_n + t*stride_t + v] (torch's (T, N, C) layout or
+ * the transposed [N, T, V] view); the labels of utterance n are targets[target_offsets[n] + k], k < target_lengths[n]
+ * (padded (N, S) rows: offset n*S; concatenated: the running sum), ntargets the size of `targets`.  S >= every
+ * target length, 0 <= S <= 1023 (2S+1 lattice states); lengths are clamped to [0, T] / [0, S], and a label outside
+ * [0, V) (or an index outside `targets`) has no emission, so nothing outside the buffers is read.  costs [N] = -log p
+ * (+inf when no alignment exists; 0 then when zero_infinity).  workspace: eb_ctc_workspace_size(N, T, S) bytes,
+ * 8-byte aligned (0: unsupported sizes).
+ * eb_ctc_loss_bwd (after the forward, same workspace): grad (strides grad_stride_n / _t, not aliasing log_probs) =
+ * gscale[n] * (exp(lp) - sum_{s: l'_s = v} exp(alpha_t(s) + beta_t(s) + nll - lp_v)), the gradient torch's ctc_loss
+ * returns for log_probs; zero for t >= input_lengths[n], and for the whole utterance when zero_infinity and its cost is
+ * +inf.  gscale [N] may be NULL (1).  The states of one label are summed in increasing s: every value is bitwise
+ * repeatable and independent of the other utterances of the batch.  alpha / beta are computed and kept in fp64.
+ * eb_ctc_greedy: log_probs [B, T, V] (strides stride_b / stride_t); per frame t < min(xlen[b], T) the argmax in
+ * torch.argmax order (NaN first, ties to the lowest index); frames equal to the previous frame's argmax and blanks are
+ * dropped: ids [B, T] row b holds counts[b] ids; neg_score[b] = -(sum of the WHOLE log-prob rows of the kept frames),
+ * the reference's score. */
+int eb_log_softmax_fwd(const float* x, float* y, long rows, int V, void* stream);
+int eb_log_softmax_bwd(const float* dy, const float* y, float* dx, long rows, int V, void* stream);
+size_t eb_ctc_workspace_size(int N, int T, int S);
+int eb_ctc_loss_fwd(const float* log_probs, long stride_n, long stride_t, int N, int T, int V, const int* targets,
+                    long ntargets, const int* target_offsets, const int* target_lengths, const int* input_lengths,
+                    int S, int blank, int zero_infinity, void* workspace, float* costs, void* stream);
+int eb_ctc_loss_bwd(const float* log_probs, long stride_n, long stride_t, float* grad, long grad_stride_n,
+                    long grad_stride_t, int N, int T, int V, const int* target_lengths, const int* input_lengths,
+                    int S, int blank, int zero_infinity, const void* workspace, const float* gscale, void* stream);
+int eb_ctc_greedy(const float* log_probs, long stride_b, long stride_t, int B, int T, int V, const int* xlen, int blank,
+                  int* ids, int* counts, float* neg_score, void* stream);
+
 /* ---- fp32 GEMM (parity mode of every Linear / LSTM input projection) ----------------------
  * replaces the cuBLAS/MKL calls behind nn.Linear and nn.LSTM's input GEMM (rnnt/models.py:45-46,
  * 129,148,163-167).  C = alpha*A'B' + beta*C + bias[n], A'(m,k)=A[m*sam+k*sak],
