@@ -905,6 +905,296 @@ __device__ __noinline__ void phase_beam_final(const EbPhase& p) {
     }
 }
 
+// ---- CTC prefix beam search (CTCBeamEngine, Hannun et al. 2014): B utterances x W slots, row r = b*W + slot, T' =
+// hist_ld frames.  Field use of CTC_BEAM:
+//   S = B, N = V, aux = W, aux2 = blank, hist_col = first frame t0, ldw1 = frames this phase runs (>= 1), K1 = LS =
+//   T' + 5; x1 log-probs [B, T', V] contiguous; tok_in frames [B]; c per-slot state [2 parities][pb | pnb | f][B*W]
+//   (frame t reads parity t&1 and writes the other); seq_out token rows [2 parities][B*W][LS] = {len, hash lo, hash hi,
+//   parent hash lo, parent hash hi, tokens} (the parent hash is the hash of the prefix without its last token); y the
+//   ranking value (pb (+) pnb) + f of each slot [B*W] (dead slots -inf), what BEAM_FINAL picks by; hist as BEAM_SELECT's,
+//   a stay recorded with token blank; src the parent row [B*W].  Flag 32 (LM fusion): x2 / ldx2 / K2 LM logits, fuse,
+//   tok_map and tok_out2 (LM token of each new slot, -1 for a stay) as BEAM_SELECT's.
+// A frame t < frames[b] of one utterance, for its live slots q (prefix l, last token e or none), with (+) = logaddexp_:
+//   stay       pb' = (pb (+) pnb) + y[blank], pnb' = pnb + y[e] (-inf for the empty prefix), f' = f;
+//   extension  by a non-blank c: pb' = -inf, pnb' = (c == e ? pb : pb (+) pnb) + y[c], f' = f + fusion term;
+//   merge      when l + c is the prefix of another live slot q2 (q2's prefix minus its last token is l: length, hash,
+//              then an exact token comparison, never the hash alone), that extension is no candidate of its own: its
+//              pnb' is log-added into q2's stay pnb' after q2's own repeat term;
+//   ranking    by (pb' (+) pnb') + f' descending, ties to the lowest flat index q*V + k (a stay at k = blank), the same
+//              64-bit composites, radix select and bitonic sort as BEAM_SELECT; min(W, candidates) survive.
+// The previous beam holds distinct prefixes, so the merge is the only way two candidates can share one.  An extension's
+// value is pnb' + f', which is (-inf (+) pnb') + f' bit for bit for every non-NaN pnb'.  Frames t >= frames[b] write an
+// identity history entry and touch no state: a frozen utterance is never read again.  NaN log-probs are outside the
+// contract; a NaN value gets a composite like any other (order_key keeps every key distinct), so the select still ends
+// after at most 8 passes and reads nothing out of bounds.  Without an LM nothing runs between frames, and one phase
+// walks all frames of its utterances with no grid barrier; with an LM the program runs one frame per phase.
+constexpr int CTC_SEQ_HEAD = 5;
+// CTC_BEAM's shared memory (2 x u64 + 11 x 32-bit arrays of BEAM_MAX_W, histogram, scalars) in the dynamic shared memory
+static_assert(BEAM_MAX_W * (2 * 8 + 11 * 4) + 256 * 4 + 8 * 4 <= (RED_FLOATS + TR * OUT_LD) * 4, "ctc beam smem");
+
+__device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
+    const int W = p.aux, V = p.N, T = p.hist_ld, blank = p.aux2, LS = p.K1;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nt = blockDim.x;
+    const bool lm = p.flags & 32;
+    const long R = (long)p.S * W, BTW = R * T;
+    int* hpar = p.hist;
+    int* htok = p.hist + BTW;
+    float* hlp = reinterpret_cast<float*>(p.hist + 2 * BTW);
+    int* hlive = p.hist + 3 * BTW;
+    unsigned long long* comp = reinterpret_cast<unsigned long long*>(sm);       // [BEAM_MAX_W] (padded to 2^k)
+    unsigned long long* shash = comp + BEAM_MAX_W;                             // prefix hash
+    float* sA = reinterpret_cast<float*>(shash + BEAM_MAX_W);                   // pb (+) pnb
+    float* sB = sA + BEAM_MAX_W;                                                // pb
+    float* sf = sB + BEAM_MAX_W;                                                // f
+    float* sstay = sf + BEAM_MAX_W;                                             // the stay's value
+    float* lmm = sstay + BEAM_MAX_W;                                            // LM log-softmax statistics
+    float* lmls = lmm + BEAM_MAX_W;
+    int* se = reinterpret_cast<int*>(lmls + BEAM_MAX_W);                        // last token, -1 for the empty prefix
+    int* slen = se + BEAM_MAX_W;
+    int* mpar = slen + BEAM_MAX_W;                                              // slot whose extension merges in, or -1
+    int* chead = mpar + BEAM_MAX_W;                                             // slots merging from this one: a list
+    int* cnext = chead + BEAM_MAX_W;
+    unsigned* rhist = reinterpret_cast<unsigned*>(cnext + BEAM_MAX_W);          // [256]
+    int* misc = reinterpret_cast<int*>(rhist + 256);
+    const float lm_weight = lm ? __ldg(p.fuse) : 0.f, length_bonus = lm ? __ldg(p.fuse + 1) : 0.f;
+    for (int b = blockIdx.x; b < p.S; b += gridDim.x) {
+        const long r0 = (long)b * W;
+        const int frames = __ldg(p.tok_in + b);
+        for (int t = p.hist_col; t < p.hist_col + p.ldw1; ++t) {
+            __syncthreads();                                 // the previous frame's shared and global writes are done
+            const long h0 = ((long)b * T + t) * W;
+            const int nlive = t > 0 ? __ldcg(hlive + (long)b * T + t - 1) : 1;
+            if (t >= frames) {                               // frozen: the beam stays, the LM rests
+                for (int j = tid; j < W; j += nt) {
+                    hpar[h0 + j] = j;
+                    htok[h0 + j] = blank;
+                    hlp[h0 + j] = __ldcg(p.y + r0 + j);
+                    p.src[r0 + j] = (int)(r0 + j);
+                    if (lm) p.tok_out2[r0 + j] = -1;
+                }
+                if (tid == 0) hlive[(long)b * T + t] = nlive;
+                continue;
+            }
+            const float* st_in = p.c + (t & 1) * 3 * R;
+            float* st_out = p.c + ((t + 1) & 1) * 3 * R;
+            const int* seq_in = p.seq_out + (t & 1) * R * LS;
+            int* seq_out = p.seq_out + ((t + 1) & 1) * R * LS;
+            const float* y = p.x1 + ((long)b * T + t) * V;
+            if (tid < 8) misc[tid] = 0;
+            for (int q = tid; q < nlive; q += nt) {
+                const float pb = __ldcg(st_in + r0 + q), pnb = __ldcg(st_in + R + r0 + q);
+                const int* ps = seq_in + (r0 + q) * LS;
+                const int len = __ldcg(ps);
+                sA[q] = logaddexp_(pb, pnb);
+                sB[q] = pb;
+                sf[q] = __ldcg(st_in + 2 * R + r0 + q);
+                slen[q] = len;
+                shash[q] = (unsigned)__ldcg(ps + 1) | ((unsigned long long)(unsigned)__ldcg(ps + 2) << 32);
+                se[q] = len > 0 ? __ldcg(ps + CTC_SEQ_HEAD + len - 1) : -1;
+                chead[q] = -1;
+            }
+            __syncthreads();
+            // merges: the slot whose prefix is slot q2's minus its last token
+            for (int q2 = tid; q2 < nlive; q2 += nt) {
+                int par = -1;
+                const int len = slen[q2];
+                if (len > 0) {
+                    const int* s2 = seq_in + (r0 + q2) * LS;
+                    const unsigned long long ph =
+                        (unsigned)__ldcg(s2 + 3) | ((unsigned long long)(unsigned)__ldcg(s2 + 4) << 32);
+                    for (int q = 0; q < nlive && par < 0; ++q) {
+                        if (slen[q] != len - 1 || shash[q] != ph) continue;
+                        const int* s1 = seq_in + (r0 + q) * LS + CTC_SEQ_HEAD;
+                        bool eq = true;
+                        for (int i = 0; i < len - 1 && eq; ++i) eq = __ldcg(s1 + i) == __ldcg(s2 + CTC_SEQ_HEAD + i);
+                        if (eq) par = q;
+                    }
+                }
+                mpar[q2] = par;
+                if (par >= 0) {
+                    cnext[q2] = atomicExch(&chead[par], q2);
+                    atomicAdd(&misc[6], 1);
+                }
+            }
+            __syncthreads();
+            // the stay of slot q, with the extension that merges into it
+            auto stay_of = [&](int q, float& pb2, float& pnb2) {
+                const int e = se[q], par = mpar[q];
+                pb2 = sA[q] + __ldg(y + blank);
+                pnb2 = e >= 0 ? __ldcg(st_in + R + r0 + q) + __ldg(y + e) : -INFINITY;
+                if (par >= 0) pnb2 = logaddexp_(pnb2, (e == se[par] ? sB[par] : sA[par]) + __ldg(y + e));
+            };
+            for (int q = tid; q < nlive; q += nt) {
+                float pb2, pnb2;
+                stay_of(q, pb2, pnb2);
+                sstay[q] = logaddexp_(pb2, pnb2) + sf[q];
+            }
+            if (lm)                                          // per-row LM log-softmax statistics (warp per row)
+                for (int q = warp; q < nlive; q += nt >> 5) {
+                    const float* l = p.x2 + (r0 + q) * p.ldx2;
+                    float lmx = -INFINITY;
+                    for (int k = lane; k < p.K2; k += 32) lmx = fmaxf(lmx, __ldcg(l + k));
+                    lmx = warp_max(lmx);
+                    float ls = 0.f;
+                    for (int k = lane; k < p.K2; k += 32) ls += expf(__ldcg(l + k) - lmx);
+                    ls = warp_sum(ls);
+                    if (lane == 0) {
+                        lmm[q] = lmx;
+                        lmls[q] = logf(ls);
+                    }
+                }
+            __syncthreads();
+            // extension (q, k), k != blank: pnb' and f'
+            auto ext_of = [&](int q, int k, float& pnb2, float& f2) {
+                pnb2 = (k == se[q] ? sB[q] : sA[q]) + __ldg(y + k);
+                f2 = sf[q];
+                if (lm) {
+                    const int j = __ldg(p.tok_map + k);
+                    f2 = f2 + (j >= 0 ? lm_weight * ((__ldcg(p.x2 + (r0 + q) * p.ldx2 + j) - lmm[q]) - lmls[q]) +
+                                            length_bonus
+                                      : length_bonus);
+                }
+            };
+            // candidate flat index e = q*V + k; false when it merged into a live slot's stay
+            auto cand = [&](long e, unsigned long long& c) -> bool {
+                const int q = (int)(e / V), k = (int)(e - (long)q * V);
+                float v;
+                if (k == blank) {
+                    v = sstay[q];
+                } else {
+                    for (int q2 = chead[q]; q2 >= 0; q2 = cnext[q2])
+                        if (se[q2] == k) return false;
+                    float pnb2, f2;
+                    ext_of(q, k, pnb2, f2);
+                    v = pnb2 + f2;
+                }
+                c = ((unsigned long long)order_key(v) << 32) | tie_key((unsigned)e);
+                return true;
+            };
+            const long ncand = (long)nlive * V;
+            const int nsel = (int)min((long)W, ncand - misc[6]);
+            unsigned need = nsel;
+            unsigned long long prefix = 0, mask = 0;
+            for (int shift = 56; shift >= 0; shift -= 8) {
+                for (int i = tid; i < 256; i += nt) rhist[i] = 0;
+                __syncthreads();
+                for (long e = tid; e < ncand; e += nt) {
+                    unsigned long long c;
+                    if (cand(e, c) && (c & mask) == prefix) atomicAdd(&rhist[(c >> shift) & 255], 1u);
+                }
+                __syncthreads();
+                if (warp == 0) {                             // lane l owns bins 255-8l .. 248-8l, scanned from the top
+                    unsigned cnt[8], s = 0;
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        cnt[i] = rhist[255 - 8 * lane - i];
+                        s += cnt[i];
+                    }
+                    unsigned inc = s;
+#pragma unroll
+                    for (int o = 1; o < 32; o <<= 1) {
+                        const unsigned v = __shfl_up_sync(0xffffffffu, inc, o);
+                        if (lane >= o) inc += v;
+                    }
+                    unsigned above = inc - s;
+                    if (above < need && need <= inc) {
+                        int i = 0;
+                        while (above + cnt[i] < need) above += cnt[i++];
+                        misc[0] = 255 - 8 * lane - i;
+                        misc[1] = (int)above;
+                        misc[2] = (int)cnt[i];
+                    }
+                }
+                __syncthreads();
+                need -= (unsigned)misc[1];
+                prefix |= (unsigned long long)misc[0] << shift;
+                mask |= 0xffull << shift;
+                if ((unsigned)misc[2] == need) break;        // every candidate under this prefix survives
+            }
+            for (long e = tid; e < ncand; e += nt) {
+                unsigned long long c;
+                if (cand(e, c) && (c & mask) >= prefix) {
+                    const int i = atomicAdd(&misc[3], 1);
+                    if (i < nsel) comp[i] = c;               // exactly nsel pass; the guard keeps smem safe regardless
+                }
+            }
+            int P = 1;
+            while (P < nsel) P <<= 1;
+            for (int i = nsel + tid; i < P; i += nt) comp[i] = 0;
+            __syncthreads();
+            for (int kk = 2; kk <= P; kk <<= 1)              // bitonic sort, descending
+                for (int jj = kk >> 1; jj > 0; jj >>= 1) {
+                    for (int i = tid; i < P; i += nt) {
+                        const int l = i ^ jj;
+                        if (l > i) {
+                            const unsigned long long a = comp[i], c = comp[l];
+                            if ((i & kk) == 0 ? a < c : a > c) {
+                                comp[i] = c;
+                                comp[l] = a;
+                            }
+                        }
+                    }
+                    __syncthreads();
+                }
+            // the new beam in walk order
+            for (int s = tid; s < W; s += nt) {
+                const long r = r0 + s, h = h0 + s;
+                if (s < nsel) {
+                    const unsigned f = tie_key((unsigned)comp[s]);
+                    const int q = (int)(f / V), k = (int)(f % V);
+                    float pb2, pnb2, f2, v;
+                    if (k == blank) {
+                        stay_of(q, pb2, pnb2);
+                        f2 = sf[q];
+                        v = sstay[q];
+                    } else {
+                        pb2 = -INFINITY;
+                        ext_of(q, k, pnb2, f2);
+                        v = pnb2 + f2;
+                    }
+                    st_out[r] = pb2;
+                    st_out[R + r] = pnb2;
+                    st_out[2 * R + r] = f2;
+                    p.y[r] = v;
+                    p.src[r] = (int)(r0 + q);
+                    if (lm) p.tok_out2[r] = k != blank ? __ldg(p.tok_map + k) : -1;
+                    hpar[h] = q;
+                    htok[h] = k;
+                    hlp[h] = v;
+                } else {
+                    st_out[r] = -INFINITY;
+                    st_out[R + r] = -INFINITY;
+                    st_out[2 * R + r] = 0.f;
+                    p.y[r] = -INFINITY;
+                    p.src[r] = (int)r;
+                    if (lm) p.tok_out2[r] = -1;
+                    hpar[h] = s;
+                    htok[h] = blank;
+                    hlp[h] = -INFINITY;
+                }
+            }
+            if (tid == 0) hlive[(long)b * T + t] = nsel;
+            for (int s = 0; s < nsel; ++s) {                 // token rows of the new beam
+                const unsigned f = tie_key((unsigned)comp[s]);
+                const int q = (int)(f / V), k = (int)(f % V), len = slen[q];
+                const bool ext = k != blank;
+                const int* ps = seq_in + (r0 + q) * LS;
+                int* d = seq_out + (r0 + s) * LS;
+                const unsigned long long hn = shash[q] * SEQ_HASH_MUL + (unsigned)(k + 1);
+                for (int j = tid; j < CTC_SEQ_HEAD + len + ext; j += nt) {
+                    int v;
+                    if (j >= CTC_SEQ_HEAD) v = j - CTC_SEQ_HEAD < len ? __ldcg(ps + j) : k;
+                    else if (!ext) v = __ldcg(ps + j);
+                    else if (j == 0) v = len + 1;
+                    else if (j < 3) v = (int)(unsigned)((j == 1 ? hn : hn >> 32));
+                    else v = (int)(unsigned)((j == 3 ? shash[q] : shash[q] >> 32));
+                    d[j] = v;
+                }
+            }
+        }
+    }
+}
+
 // SKIP: does any row of tok_in[0..S) differ from aux2 (blank)?  tok_in is final at the preceding grid barrier, so every
 // thread of every CTA gets the same answer.
 __device__ __noinline__ bool phase_skip_live(const EbPhase& p) {
@@ -916,6 +1206,10 @@ __device__ __noinline__ bool phase_skip_live(const EbPhase& p) {
 // the phase loader copies the struct as 32-bit words, one per thread of the 256-thread CTA
 static_assert(sizeof(EbPhase) % 4 == 0 && sizeof(EbPhase) / 4 <= 256, "EbPhase loader");
 
+// Two instantiations: CTC = false runs every phase but CTC_BEAM (which it skips), CTC = true adds CTC_BEAM.  Any reachable
+// call to phase_ctc_beam, whatever the call site, takes this kernel from 12 / 16 to 44 / 136 bytes of spill stores / loads,
+// some of them inside the matrix phases' tile loops; the programs that do not search CTC beams keep the kernel without it.
+template <bool CTC>
 __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __restrict__ prog, int nphase, unsigned* bar) {
     extern __shared__ __align__(16) float dsm[];
     float* red = dsm;                                        // [8 warps][2048]
@@ -951,6 +1245,9 @@ __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __re
                 for (long k = gtid; k < (long)ph.S * ph.N; k += gn) ph.y[k] = __ldcg(ph.x1 + k);
                 break;
             case EB_PH_BEAM_SELECT: phase_beam_select(ph, dsm); break;
+            case EB_PH_CTC_BEAM:
+                if constexpr (CTC) phase_ctc_beam(ph, dsm);
+                break;
             case EB_PH_GATHER: phase_gather(ph); break;
             case EB_PH_BEAM_FINAL: phase_beam_final(ph); break;
             case EB_PH_BEAM_COMMIT: phase_beam_commit(ph, dsm); break;
@@ -972,7 +1269,8 @@ __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __re
 
 }  // namespace
 
-EB_API int eb_decode_run(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream) {
+template <bool CTC>
+int decode_run(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream) {
     if (!phases_dev || nphase <= 0 || !barrier_dev) return EB_ERR_INVALID;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     EB_CUDA(cudaMemsetAsync(barrier_dev, 0, 4, st));
@@ -982,9 +1280,17 @@ EB_API int eb_decode_run(const void* phases_dev, int nphase, void* barrier_dev, 
     unsigned* bar = reinterpret_cast<unsigned*>(barrier_dev);
     void* args[] = {(void*)&prog, (void*)&nphase, (void*)&bar};
     const size_t smem = sizeof(float) * (RED_FLOATS + TR * OUT_LD);
-    EB_CUDA(cudaFuncSetAttribute(decode_program_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    EB_CUDA(cudaLaunchCooperativeKernel((void*)decode_program_kernel, dim3(grid), dim3(256), args, smem, st));
+    EB_CUDA(cudaFuncSetAttribute(decode_program_kernel<CTC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    EB_CUDA(cudaLaunchCooperativeKernel((void*)decode_program_kernel<CTC>, dim3(grid), dim3(256), args, smem, st));
     return EB_OK;
+}
+
+EB_API int eb_decode_run(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream) {
+    return decode_run<false>(phases_dev, nphase, barrier_dev, max_ctas, stream);
+}
+
+EB_API int eb_decode_run_ctc(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream) {
+    return decode_run<true>(phases_dev, nphase, barrier_dev, max_ctas, stream);
 }
 
 EB_API int eb_decode_phase_size(void) { return (int)sizeof(EbPhase); }

@@ -119,3 +119,74 @@ class CTCLoss(nn.Module):
     def forward(self, log_probs, targets, input_lengths, target_lengths):
         return ctc_loss(log_probs, targets, input_lengths, target_lengths, self.blank, self.reduction,
                         self.zero_infinity)
+
+
+# beam_search keeps the program of its last call (one engine: its log-prob copy [B, T, V], history [B, T, W] x 3,
+# token rows [2, B*W, T + 5], state and, with an LM, the LM's weights on the device); free_beam_search() releases it
+_beam_engines = {}
+
+
+def free_beam_search():
+    """Release the device memory beam_search keeps for its next call with the same shapes and LM."""
+    _beam_engines.clear()
+
+
+def beam_search(log_probs, input_lengths, beam_width, blank=0, *, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1,
+                lm_token_map=None):
+    """CTC prefix beam search (Hannun et al., 2014) on the device, optionally with shallow fusion of the reference's
+    LSTM language model (LMModel, or its state_dict).  ``CTCEncoder.beam_search`` states the rule.
+
+      * log_probs: fp32 CUDA tensor [B, T, V] of log-softmax rows, batch first (what ``CTCEncoder.forward`` returns),
+        any strides.  ``ctc_loss``'s (T, N, C) layout is not taken as such: pass its ``.transpose(0, 1)``.
+      * input_lengths: integers or an integer tensor, one per utterance, in log-prob frames, each in [0, T].
+      * beam_width: W in [1, 1024]; blank in [0, V).
+      * lm, lm_weight, length_bonus, lm_bos, lm_token_map: as ``Transducer.beam_search``'s fusion arguments.
+
+    Returns (list of B int64 arrays: the best prefix of each utterance, -score [B] on the device: its negated
+    (pb (+) pnb) + f).  Every argument is checked on the host before any device work (TypeError / ValueError, and
+    RuntimeError for CPU log_probs: there is no CPU path).  One persistent kernel launch (stream_engine.CTCBeamEngine)
+    and one device-to-host copy of the ids.  The engine stays resident for the next call with the same shapes and LM
+    (about 4·B·T·(V + 4·W) bytes and the LM's weights); ``free_beam_search()`` releases it."""
+    import numbers
+    from .stream_engine import BEAM_MAX_W, CTCBeamEngine, check_lm_args, lm_cache_key
+    if not isinstance(log_probs, torch.Tensor):
+        raise TypeError("log_probs must be a tensor")
+    if log_probs.dtype != torch.float32:
+        raise TypeError("edgedict_b200 ctc beam_search takes fp32 log_probs, got %s (there is no fallback)"
+                        % log_probs.dtype)
+    if log_probs.dim() != 3:
+        raise ValueError("log_probs must be [B, T, V], got shape %s" % (tuple(log_probs.shape),))
+    B, T, V = log_probs.shape
+    if B < 1 or T < 1 or V < 1:
+        raise ValueError("log_probs must not be empty, got shape %s" % (tuple(log_probs.shape),))
+    if isinstance(beam_width, bool) or not isinstance(beam_width, numbers.Integral):
+        raise TypeError("beam_width must be an integer, got %r" % (beam_width,))
+    W = int(beam_width)
+    if not 1 <= W <= BEAM_MAX_W:
+        raise ValueError("beam_width must be in [1, %d], got %d" % (BEAM_MAX_W, W))
+    if W * V >= 2 ** 31:
+        raise ValueError("beam_width x V must stay below 2^31, got %d x %d" % (W, V))
+    blank = operator.index(blank)
+    if not 0 <= blank < V:
+        raise ValueError("blank must lie in [0, %d), got %d" % (V, blank))
+    il = _lengths(input_lengths, B, "input_lengths")
+    if bool((il < 0).any()) or bool((il > T).any()):
+        raise ValueError("input_lengths must lie in [0, T = %d], got %s" % (T, il.tolist()))
+    fusion = check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map)
+    if not log_probs.is_cuda:
+        raise RuntimeError("edgedict_b200 ctc beam_search needs CUDA log_probs (got a %s tensor); there is no CPU path"
+                           % log_probs.device)
+    dev = log_probs.device
+    key = (B, T, V, W, blank, dev, lm_cache_key(fusion))
+    eng = _beam_engines.get(key)
+    if eng is None:
+        _beam_engines.clear()                                  # one resident program is enough
+        eng = _beam_engines[key] = CTCBeamEngine(B, T, V, W, blank, lm=lm, lm_weight=lm_weight,
+                                                 length_bonus=length_bonus, lm_bos=lm_bos, lm_token_map=lm_token_map,
+                                                 device=dev)
+    lens = torch.empty(B, dtype=torch.int32, pin_memory=True)
+    lens.copy_(il)
+    with torch.no_grad():
+        ids, nlogp = eng.run(log_probs, lens.to(dev, non_blocking=True))
+        ids = ids.cpu().numpy()
+    return [row[row >= 0].astype("int64") for row in ids], nlogp.clone()

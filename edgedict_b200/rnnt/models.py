@@ -366,18 +366,14 @@ class Transducer(nn.Module):
         steps its predictor (and LM); the others keep their parent's state.  An utterance's frame ends after round K-1
         or as soon as none of its hypotheses is open.  K = 1 is the search above, bit for bit, and W = 1 gives the
         non-blank tokens of `greedy_decode(max_symbols=K)`."""
-        from ..stream_engine import BeamEngine, BEAM_MAX_W, check_lm_args, check_max_symbols, param_fingerprint
+        from ..stream_engine import (BeamEngine, BEAM_MAX_W, check_lm_args, check_max_symbols, lm_cache_key,
+                                     param_fingerprint)
         K = check_max_symbols(max_symbols)
         W = operator.index(W)
         if not 1 <= W <= BEAM_MAX_W:
             raise ValueError("beam width W must be in [1, %d], got %d" % (BEAM_MAX_W, W))
         fusion = check_lm_args(lm, self.joint.joint[2].weight.shape[0], lm_weight, length_bonus, lm_bos, lm_token_map)
-        lm_key = None
-        if fusion is not None:
-            lsd, lw, lb, bos, tmap = fusion
-            # a state_dict on another device is copied into the engine: its tensors' identity and version are the key
-            lm_key = (tuple((k, v.data_ptr(), v.device, v.dtype, v._version) for k, v in sorted(lsd.items())),
-                      lw, lb, bos, tuple(tmap.tolist()))
+        lm_key = lm_cache_key(fusion)
         h_enc, _ = self.encoder(xs)
         B, T = h_enc.shape[0], h_enc.shape[1]
         if xlen is None:
@@ -440,6 +436,53 @@ class CTCEncoder(nn.Module):
         host = out.cpu().numpy()
         ids, counts = host[:B * T].reshape(B, T), host[B * T:B * T + B]
         return [ids[i, :int(counts[i])].astype("int64") for i in range(B)], out[B * T + B:].view(torch.float32).clone()
+
+    @torch.no_grad()
+    def beam_search(self, xs, xlen=None, W=4, *, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1, lm_token_map=None):
+        """CTC prefix beam search (Hannun et al., 2014) after ``forward`` (which follows ``set_precision``), optionally
+        with shallow fusion of the reference's LSTM language model.  xs [B, T, F] -> (list of B int64 id arrays, -score
+        [B] on the device).  Utterance b decodes min(T', scale_length(xlen)[b]) log-prob frames (all T' when xlen is
+        None): xlen is in input frames and is scaled to T' as in ``Transducer.beam_search``.  This is deliberately not
+        ``greedy_decode``'s behaviour, which truncates to the unscaled xlen as the reference does.
+
+        A hypothesis is a prefix l (non-blank ids) with pb = log P(l, the path so far ends in blank), pnb = log P(l, it
+        ends in a non-blank) and a fusion term f; it starts as l = (), pb = 0, pnb = -inf, f = 0.  With (+) the log-add
+        m + log1p(exp(-|a - b|)), m = max(a, b) (-inf when m is), frame t of log-probs y, for each live prefix l with
+        last token e:
+          * stay: pb' = (pb (+) pnb) + y[blank], pnb' = pnb + y[e] (-inf for l = ()), f' = f;
+          * extension by a non-blank c to l + c: pb' = -inf, pnb' = (c == e ? pb : pb (+) pnb) + y[c], and
+            f' = f + lm_weight * log_softmax(LM logits of l)[map(c)] + length_bonus (f + length_bonus when
+            map(c) = -1; f' = f without an LM);
+          * when l + c is the prefix of another live hypothesis l2, the extension is no candidate of its own: its pnb'
+            is log-added into l2's stay pnb' (after l2's repeat term), and l2 keeps its f and LM state;
+          * candidates are ranked by (pb' (+) pnb') + f' descending, ties to the lowest flat index q*V + k (a stay at
+            k = blank, q the slot); the min(W, candidates) best survive, -inf candidates included.
+        The result is the best live hypothesis by (pb (+) pnb) + f (lowest slot on ties) and -score is its negated
+        value.  An utterance of length 0 gives an empty prefix and score 0.  The LM (as in ``Transducer.beam_search``:
+        primed on lm_bos, stepped on map(c) when a hypothesis extends by a c the LM scores, no end-of-sentence term)
+        runs in fp32-accurate arithmetic whatever the precision setting.  lm_weight = length_bonus = 0 gives the
+        result of lm=None bit for bit.  NaN log-probs are outside the contract: the search still ends and stays in
+        bounds, but which hypotheses a NaN keeps is unspecified.  See ``edgedict_b200.ctc.beam_search`` (this search on
+        log-probs you already have) for the arguments."""
+        from .. import ctc
+        from ..stream_engine import BEAM_MAX_W, check_lm_args
+        W = operator.index(W)
+        if not 1 <= W <= BEAM_MAX_W:
+            raise ValueError("beam width W must be in [1, %d], got %d" % (BEAM_MAX_W, W))
+        check_lm_args(lm, self.tovocab[0].weight.shape[0], lm_weight, length_bonus, lm_bos, lm_token_map)
+        lp = self.forward(xs)
+        B, T = lp.shape[0], lp.shape[1]
+        if xlen is None:
+            frames = torch.full((B,), T, dtype=torch.int64)
+        else:
+            xl = torch.as_tensor(xlen).reshape(-1).cpu()
+            if xl.numel() != B:
+                raise ValueError("xlen must have one entry per utterance (%d), got %d" % (B, xl.numel()))
+            frames = torch.zeros(B, dtype=torch.int64)            # scale_length divides by the longest xlen
+            if int(xl.max()) > 0:
+                frames = scale_length(T, xl).clamp(0, T).to(torch.int64)
+        return ctc.beam_search(lp, frames, W, self.blank, lm=lm, lm_weight=lm_weight, length_bonus=length_bonus,
+                               lm_bos=lm_bos, lm_token_map=lm_token_map)
 
 
 def _i32(t):

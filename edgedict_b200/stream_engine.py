@@ -20,7 +20,7 @@ from ._lib import lib, check
 from .rnnt.tokenizer import NUL, BOS, UNK
 
 PH_LN, PH_PAIR, PH_LSTM, PH_LINEAR, PH_ARGMAX, PH_COPY, PH_BEAM_SELECT, PH_GATHER, PH_BEAM_FINAL, PH_BEAM_COMMIT, \
-    PH_SKIP = range(11)
+    PH_SKIP, PH_CTC_BEAM = range(12)
 F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE, F_LM, F_STREAM, F_FLUSH, F_CONT, F_ROUNDS = 1, 2, 4, 8, 16, 32, 64, 128, \
     256, 512
 BEAM_MAX_W = 1024                                     # EB_BEAM_MAX_W
@@ -890,3 +890,128 @@ class StreamBeamEngine:
         ids, counts, _ = self._fetch()
         ids, counts = self._take(ids, counts)
         return ids, counts, -self.logp.view(self.S, self.W)[:, 0].cpu()
+
+
+def lm_cache_key(fusion):
+    """What a phase program built for the fusion arguments ``fusion`` (check_lm_args' result, or None) depends on: the
+    LM tensors' identity and version (a state_dict on another device is copied into the engine) and the scalars."""
+    if fusion is None:
+        return None
+    lsd, lw, lb, bos, tmap = fusion
+    return (tuple((k, v.data_ptr(), v.device, v.dtype, v._version) for k, v in sorted(lsd.items())), lw, lb, bos,
+            tuple(tmap.tolist()))
+
+
+class CTCBeamEngine:
+    """Device-side CTC prefix beam search (Hannun et al., 2014) over log-probs [B, T', V], optionally with shallow
+    fusion of the reference's LSTM language model, in ONE cooperative kernel launch (decode.cu, CTC_BEAM, which states
+    the rule).  Row r = b*W + j holds slot j of utterance b; each slot carries a prefix with log P(prefix, path ends in
+    blank) ``pb``, log P(prefix, ends in a non-blank) ``pnb`` and its accumulated fusion term ``f``.
+
+    Without an LM nothing runs between frames but the selection, so the program is ``frames_per_phase`` frames per
+    CTC_BEAM phase (0: all T' frames in one phase, no grid barrier per frame) and BEAM_FINAL.  With an LM every frame
+    is one CTC_BEAM phase, the GATHER of the LM state by parent and the masked LM step and output Linear
+    (predictor_phases resting on -1, as BeamEngine's LM), after a priming step on ``lm_bos``; frames_per_phase must
+    then be 0 or 1.  BEAM_FINAL picks the best live slot by (pb (+) pnb) + f, lowest slot on ties, and walks the
+    history, where a stay is recorded as blank."""
+
+    def __init__(self, batch, t_out, V, W, blank=0, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1,
+                 lm_token_map=None, max_ctas=0, device=None, frames_per_phase=0):
+        B, T, V, W, blank = (operator.index(v) for v in (batch, t_out, V, W, blank))
+        if not 1 <= W <= BEAM_MAX_W:
+            raise ValueError("beam width must be in [1, %d], got %d" % (BEAM_MAX_W, W))
+        if B < 1 or T < 1 or V < 1:
+            raise ValueError("batch, t_out and V must be positive, got %d, %d, %d" % (B, T, V))
+        if not 0 <= blank < V:
+            raise ValueError("blank must lie in [0, %d), got %d" % (V, blank))
+        if W * V >= 2 ** 31:
+            raise ValueError("beam width x vocabulary must stay below 2^31 (flat candidate index), got %d x %d" % (W, V))
+        fusion = check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map)
+        n = operator.index(frames_per_phase)
+        if n < 0 or (fusion is not None and n > 1):
+            raise ValueError("frames_per_phase must be >= 0 (0: all), and 0 or 1 with an lm; got %d" % n)
+        n = 1 if fusion is not None else (n or T)
+        assert C.sizeof(EbPhase) == lib().eb_decode_phase_size(), "EbPhase layout mismatch"
+        self.dev = torch.device("cuda") if device is None else torch.device(device)
+        if self.dev.type != "cuda":
+            raise RuntimeError("CTCBeamEngine runs on a CUDA device")
+        f32, i32 = torch.float32, torch.int32
+        R, LS = B * W, T + 5
+        self.B, self.T, self.V, self.W, self.R, self.blank, self.max_ctas = B, T, V, W, R, blank, max_ctas
+        z = lambda *shape, dtype=f32: torch.zeros(*shape, dtype=dtype, device=self.dev)
+        self.lp, self.frames = z(B, T, V), z(B, dtype=i32)
+        self.state = z(2, 3, R)                      # per parity: pb | pnb | f
+        self.seqs = z(2, R, LS, dtype=i32)           # per parity: {len, hash lo / hi, parent hash lo / hi, tokens}
+        self.score, self.src = z(R), z(R, dtype=i32)
+        nh = B * T * W
+        self.hist = z(3 * nh + B * T, dtype=i32)
+        self.hist_parent = self.hist[:nh].view(B, T, W)
+        self.hist_token = self.hist[nh:2 * nh].view(B, T, W)
+        self.hist_live = self.hist[3 * nh:].view(B, T)
+        self.ids, self.nlogp = z(B, T, dtype=i32), z(B)
+        self.lm = fusion is not None
+        prog = []
+        sel = dict(type=PH_CTC_BEAM, S=B, N=V, aux=W, aux2=blank, K1=LS, x1=_ptr(self.lp), tok_in=_ptr(self.frames),
+                   c=_ptr(self.state), seq_out=_ptr(self.seqs), y=_ptr(self.score), src=_ptr(self.src),
+                   hist=_ptr(self.hist), hist_ld=T)
+        if self.lm:
+            lsd, lw, lb, self.lm_bos, tmap = fusion
+            lsd = {k: v.to(self.dev, f32).contiguous() for k, v in lsd.items()}
+            self._keep = list(lsd.values())
+            Ll = (len(lsd) - 3) // 4
+            layers = [tuple(lsd["rnn.%s_l%d" % (nm, k)] for nm in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"))
+                      for k in range(Ll)]
+            Hl, ntok = layers[0][1].shape[1], lsd["encoder.weight"].shape[0]
+            self.lm_state = z(2, 2 * Ll, R, Hl)      # per parity: h of every layer, then c
+            self.lm_htmp, self.lm_logits, self.lm_tok = z(Ll, R, Hl), z(R, ntok), z(R, dtype=i32)
+            self.lm_map = tmap.to(self.dev, i32)
+            self.lm_fuse = torch.tensor([lw, lb], dtype=f32, device=self.dev)
+            sel.update(flags=F_LM, x2=_ptr(self.lm_logits), ldx2=ntok, K2=ntok, fuse=_ptr(self.lm_fuse),
+                       tok_map=_ptr(self.lm_map), tok_out2=_ptr(self.lm_tok))
+
+            def lm_step(q, masked):
+                st = self.lm_state[q]
+                predictor_phases(prog, lsd["encoder.weight"], layers, lsd["decoder.weight"], lsd["decoder.bias"], R,
+                                 st[:Ll], st[Ll:], self.lm_htmp, self.lm_logits, self.lm_tok, -1, masked)
+            lm_step(0, masked=False)                 # prime every row with lm_bos from the zero state
+        for t0 in range(0, T, n):
+            prog.append(EbPhase(hist_col=t0, ldw1=min(n, T - t0), **sel))
+            if self.lm:                              # survivors inherit their parent's LM state, extensions step it
+                p, q = t0 & 1, 1 - (t0 & 1)
+                prog.append(EbPhase(type=PH_GATHER, S=R, N=Hl, aux=2 * Ll, x1=_ptr(self.lm_state[p]),
+                                    y=_ptr(self.lm_state[q]), src=_ptr(self.src)))
+                lm_step(q, masked=True)
+        prog.append(EbPhase(type=PH_BEAM_FINAL, S=B, aux=W, aux2=blank, y=_ptr(self.score), hist=_ptr(self.hist),
+                            hist_ld=T, tok_out=_ptr(self.ids), ldy=T, y2=_ptr(self.nlogp)))
+        self.nphase = len(prog)
+        self._prog = _upload(prog, self.dev)
+        self._bar = torch.zeros(64, dtype=torch.int32, device=self.dev)
+
+    @torch.no_grad()
+    def run(self, log_probs, lengths):
+        """log_probs [B, T', V] fp32 on the device (any strides), lengths int32 [B] on the device (frames each utterance
+        decodes, clamped to [0, T']) -> (ids int32 [B, T']: the best prefix right-aligned, -1 before it; -score [B],
+        the negated (pb (+) pnb) + f of that prefix).  Both stay on the device."""
+        self.lp.copy_(log_probs)
+        self.frames.copy_(lengths.clamp(0, self.T))
+        self.state.zero_()
+        self.state[0, :2].fill_(float("-inf"))
+        self.state[0, 0].view(self.B, self.W)[:, 0] = 0.0        # the empty prefix: pb = 0, pnb = -inf, f = 0
+        self.score.fill_(float("-inf"))
+        self.score.view(self.B, self.W)[:, 0] = 0.0
+        self.seqs[0].zero_()
+        if self.lm:
+            self.lm_state[0].zero_()
+            self.lm_tok.fill_(self.lm_bos)
+        check(lib().eb_decode_run_ctc(self._prog.data_ptr(), self.nphase, self._bar.data_ptr(), self.max_ctas,
+                                      torch.cuda.current_stream().cuda_stream), "eb_decode_run_ctc")
+        return self.ids, self.nlogp
+
+    def hypotheses(self, b):
+        """The live slots of utterance b after ``run``, in slot order: [(prefix tuple, pb, pnb, f)] on the host."""
+        n = int(self.frames[b])
+        live = int(self.hist_live[b, -1])
+        st = self.state[n & 1, :, b * self.W:b * self.W + live].cpu()
+        rows = self.seqs[n & 1, b * self.W:b * self.W + live].cpu()
+        return [(tuple(int(x) for x in rows[j, 5:5 + int(rows[j, 0])]), float(st[0, j]), float(st[1, j]),
+                 float(st[2, j])) for j in range(live)]

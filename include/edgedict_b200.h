@@ -239,7 +239,8 @@ int eb_joint_dpre_reduce(const void* dpre16, float* dep, float* ddp, int B, int 
  * replaces PytorchStreamDecoder.decode's Python loop (rnnt/stream.py:93-120).  The host builds a
  * phase program once (edgedict_b200/stream_engine.py) and launches it per chunk; see decode.cu. */
 enum { EB_PH_LN = 0, EB_PH_PAIR = 1, EB_PH_LSTM = 2, EB_PH_LINEAR = 3, EB_PH_ARGMAX = 4, EB_PH_COPY = 5,
-       EB_PH_BEAM_SELECT = 6, EB_PH_GATHER = 7, EB_PH_BEAM_FINAL = 8, EB_PH_BEAM_COMMIT = 9, EB_PH_SKIP = 10 };
+       EB_PH_BEAM_SELECT = 6, EB_PH_GATHER = 7, EB_PH_BEAM_FINAL = 8, EB_PH_BEAM_COMMIT = 9, EB_PH_SKIP = 10,
+       EB_PH_CTC_BEAM = 11 };
 typedef struct EbPhase {
     int32_t type, S, K1, K2, N, flags, ldx1, ldx2, ldw1, ldw2, ldy, aux, aux2, hist_ld, hist_col, x1_div;
     const float *x1, *x2, *w1, *w2, *b1, *b2;
@@ -283,10 +284,18 @@ typedef struct EbPhase {
  * to its best slot; src receives the gather sources that move the kept slots' state into place.
  * x1_div (LINEAR): row r of x1 is x1[r / x1_div] (0 or 1: row r), the encoder frame a beam's W rows share.
  * Beam search (batched, W slots per utterance, row r = b*W + slot; see decode.cu for the field use of each phase):
- * at most EB_BEAM_MAX_W slots per utterance. */
+ * at most EB_BEAM_MAX_W slots per utterance.
+ * CTC_BEAM (CTC prefix beam search over log-probs, one CTA per utterance; see decode.cu for the field use): frames
+ * hist_col .. hist_col + ldw1 - 1 in one phase; each slot carries log P(prefix, ends in blank / non-blank) and a fusion
+ * term in an engine-owned state buffer (c), an extension that reaches another live slot's prefix is log-added into that
+ * slot's stay before the ranking, the history is BEAM_SELECT's (a stay recorded as blank) and BEAM_FINAL reads it.
+ * Programs with CTC_BEAM run through eb_decode_run_ctc. */
 #define EB_BEAM_MAX_W 1024
 int eb_decode_phase_size(void);
 int eb_decode_run(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream);
+/* eb_decode_run with CTC_BEAM phases: the same kernel in an instantiation that also runs CTC_BEAM (eb_decode_run skips
+ * them: the extra phase costs the matrix phases register spills, which the other programs do not pay). */
+int eb_decode_run_ctc(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream);
 
 /* ---- reductions, casts, optimizer -------------------------------------------------------- */
 int eb_colsum(const void* x, int x_bf16, float* out_accum, long rows, int N, void* stream);
