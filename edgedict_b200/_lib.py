@@ -61,6 +61,8 @@ SIGNATURES = {
     "eb_lstm_c4_bwd_chunks": (I, [P, P, P, P, P, P, P, P, P, P, P, I, P, I, I, P]),
     "eb_layernorm_fwd": (I, [P, P, P, P, P, P, P, P, L, I, F, P]),
     "eb_layernorm_bwd": (I, [P, P, P, P, P, P, P, P, P, L, I, P]),
+    "eb_layernorm_bwd_dz": (I, [P, P, P, P, P, P, P, L, I, P]),
+    "eb_layernorm_bwd_params": (I, [P, P, P, P, P, P, P, L, I, P]),
     "eb_time_reduce_fwd": (I, [P, P, P, I, I, I, P]),
     "eb_time_reduce_bwd": (I, [P, P, I, I, I, P]),
     "eb_embedding_fwd": (I, [P, I, P, P, P, I, I, I, I, I, P]),

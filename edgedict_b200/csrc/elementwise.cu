@@ -648,11 +648,13 @@ EB_API int eb_layernorm_fwd(const float* x, const float* res, const float* gamma
     return EB_OK;
 }
 
-EB_API int eb_layernorm_bwd(const float* dy, const float* x, const float* res, const float* gamma,
-                            const float* mean, const float* rstd, float* dz, float* dgamma,
-                            float* dbeta, long rows, int H, void* stream) {
-    if (!dy || !x || !gamma || !mean || !rstd || !dz || !dgamma || !dbeta || rows <= 0 || H <= 0 || H > 2048)
-        return EB_ERR_INVALID;
+// The two passes of eb_layernorm_bwd, for callers that run them apart (the layer wavefront of the LSTM stack's backward:
+// dz per time chunk on the critical path, the parameter gradients once per layer beside it).  Rows are independent in
+// the dz pass and the parameter pass sums in a fixed order over all rows it is given, so dz of a row block is the same
+// bits as the rows of a whole-buffer call, and the parameter pass over the whole buffer is the same bits as inside it.
+EB_API int eb_layernorm_bwd_dz(const float* dy, const float* x, const float* res, const float* gamma, const float* mean,
+                               const float* rstd, float* dz, long rows, int H, void* stream) {
+    if (!dy || !x || !gamma || !mean || !rstd || !dz || rows <= 0 || H <= 0 || H > 2048) return EB_ERR_INVALID;
     const bool vec_ok = H % 128 == 0 && H <= 1024 &&
                         ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dz) |
                           reinterpret_cast<uintptr_t>(gamma) | (res ? reinterpret_cast<uintptr_t>(res) : 0)) & 15) == 0;
@@ -674,9 +676,26 @@ EB_API int eb_layernorm_bwd(const float* dy, const float* x, const float* res, c
 #undef LN_BWD
     }
     EB_CHECK_LAUNCH();
+    return EB_OK;
+}
+
+// dgamma += sum_r dy*xhat, dbeta += sum_r dy (the caller zeroes them)
+EB_API int eb_layernorm_bwd_params(const float* dy, const float* x, const float* res, const float* mean,
+                                   const float* rstd, float* dgamma, float* dbeta, long rows, int H, void* stream) {
+    if (!dy || !x || !mean || !rstd || !dgamma || !dbeta || rows <= 0 || H <= 0 || H > 2048) return EB_ERR_INVALID;
     layernorm_param_grad_kernel<<<(H + 7) / 8, 1024, 0, ST(stream)>>>(dy, x, res, mean, rstd, dgamma, dbeta, rows, H);
     EB_CHECK_LAUNCH();
     return EB_OK;
+}
+
+EB_API int eb_layernorm_bwd(const float* dy, const float* x, const float* res, const float* gamma,
+                            const float* mean, const float* rstd, float* dz, float* dgamma,
+                            float* dbeta, long rows, int H, void* stream) {
+    if (!dy || !x || !gamma || !mean || !rstd || !dz || !dgamma || !dbeta || rows <= 0 || H <= 0 || H > 2048)
+        return EB_ERR_INVALID;
+    const int st = eb_layernorm_bwd_dz(dy, x, res, gamma, mean, rstd, dz, rows, H, stream);
+    if (st != EB_OK) return st;
+    return eb_layernorm_bwd_params(dy, x, res, mean, rstd, dgamma, dbeta, rows, H, stream);
 }
 
 EB_API int eb_time_reduce_fwd(const float* x, float* y, void* y_bf16, int B, int T, int H, void* stream) {

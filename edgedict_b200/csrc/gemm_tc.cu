@@ -552,12 +552,15 @@ void plan(int a_mn_major, int c_bf16, int accumulate, long M, int N, long K, int
     if (force_bn == 128) wide = false;
     if (force_bn == 256 && N % 128 == 0) wide = true;
     if (low) wide = false;
+    // fixed K order: the plan depends on N alone, so that a product computed in row blocks gives the bits of the whole
+    const bool fixed = (flags & EB_GEMM_FIXED_K) != 0;
+    if (fixed) wide = N % 256 == 0;
     (void)a_mn_major;
     const int BN = wide ? 256 : 128;
     const long out_tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
     const long nkb = (K + BK - 1) / BK;
     ksplit = 1;
-    if (!low && !c_bf16 && nkb >= 64 && out_tiles < eb_num_sms())
+    if (!low && !fixed && !c_bf16 && nkb >= 64 && out_tiles < eb_num_sms())
         ksplit = choose_ksplit(out_tiles, nkb, eb_num_sms(), BN == 256 ? 32.0 : 16.0);
 }
 

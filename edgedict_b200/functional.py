@@ -338,6 +338,24 @@ class _Chunks:
 
 
 BPTT_ONE_LAUNCH = __import__("os").environ.get("EDGEDICT_BPTT_ONE_LAUNCH", "1") != "0"   # one BPTT launch per layer (else per chunk)
+# Chunked backward (LSTMStack._backward_wave): the BPTT of every layer runs in groups of BPTT_GROUP time chunks, and the
+# input of a group (dgrad GEMM of the layer above, TimeReduction and LayerNorm backward) is prepared on other streams
+# while the recurrence of the layer above is still running, so that the recurrences follow each other without the
+# serial schedule's gap between layers.  Tests set it to False to take the serial schedule, which gives the same bits.
+BPTT_WAVEFRONT = True
+BPTT_GROUP = 3          # time chunks per BPTT launch of the chunked backward (fewer launches, each ~45 us of prologue)
+_bwd_streams = {}
+
+
+def _wave_bwd_streams(device):
+    """Streams of the chunked backward: one for the recurrence and two for the group inputs at high priority (their
+    blocks are dispatched first when a BPTT grid ends, so the next group's grid is not held up behind a GEMM), and one
+    for the weight gradients at the default priority."""
+    st = _bwd_streams.get(device)
+    if st is None:
+        st = _bwd_streams[device] = tuple(torch.cuda.Stream(device, priority=-1) for _ in range(3)) + (
+            torch.cuda.Stream(device),)
+    return st
 
 
 class LSTMStack(torch.autograd.Function):
@@ -479,6 +497,8 @@ class LSTMStack(torch.autograd.Function):
         P = [params[6 * l:6 * l + 6] for l in range(L)]
         ck = [_Chunks(B, lens) for lens in plan]
         dev = dout.device
+        if BPTT_WAVEFRONT and BPTT_ONE_LAUNCH and C <= 8 and c4 and not c4b and _c4_bptt(H):
+            return LSTMStack._backward_wave(ctx, dout, P, ck, hT, cT, x16, xs, y, y16, gates, cseq, mean, rstd)
         main = torch.cuda.current_stream(dev)
         side = _side_streams(dev)[0]
         side.wait_stream(main)
@@ -524,7 +544,8 @@ class LSTMStack(torch.autograd.Function):
             wih16 = ops.cast_bf16(_c(P[l][0]))
             M, I_l = dg16.shape[0], P[l][0].shape[1]
             if l > 0:
-                g = ops.gemm_bf16(dg16, 0, wih16, 1, M, I_l, 4 * H, out=dz, accumulate=True, tag="gemm_bf16_nn")
+                g = ops.gemm_bf16(dg16, 0, wih16, 1, M, I_l, 4 * H, out=dz, accumulate=True, tag="gemm_bf16_nn",
+                                  flags=ops.GEMM_FIXED_K)
             elif ctx.needs_input_grad[0]:
                 g = ops.gemm_bf16(dg16, 0, wih16, 1, M, I_l, 4 * H, tag="gemm_bf16_nn")
             else:
@@ -545,6 +566,101 @@ class LSTMStack(torch.autograd.Function):
                     t_.record_stream(main)
             grads[6 * l + 4], grads[6 * l + 5] = dgamma, dbeta
         main.wait_stream(side)
+        dxin = ck[0].gather(g) if g is not None else None
+        return (dxin, None, *grads)
+
+    @staticmethod
+    def _backward_wave(ctx, dout, P, ck, hT, cT, x16, xs, y, y16, gates, cseq, mean, rstd):
+        """The backward pass in reverse time, in groups of BPTT_GROUP consecutive time chunks of the forward's plan:
+        group (l, q), q = NG-1 .. 0, runs its BPTT in one launch over the group's chunk segments with the (dh, dc) carry
+        of group q+1.  Its input dz_l[q] is prepared on prep[l % 2] as soon as layer l+1 has finished group q: the dgrad
+        GEMM of layer l+1's rows of the group accumulated into dz_{l+1} (the residual branch), TimeReduction backward,
+        the dz pass of the LayerNorm backward.  Every BPTT launch runs on one stream, in the order of the diagonals of
+        forward's wavefront, so the inputs of layer l are prepared under the recurrence of layer l+1 and the recurrences
+        follow each other without a gap.  (Two layers' recurrences at once, as in the forward, would need two grids of a
+        BPTT kernel co-resident at H = 1024: the clusters-of-16 kernel fits 14 clusters where two grids need 16, and a
+        clusters-of-8 variant 30 where two need 32, on an H100 SXM -- DESIGN.md section 4a.)  The dgrad GEMM runs in the
+        co-resident configuration, beside the BPTT grid's CTAs on every SM instead of on the few SMs it leaves free.
+        Every kernel computes what the serial schedule's does on a row block (the dgrad GEMMs of both sum each element's
+        K in one order, the LayerNorm's parameter pass runs once per layer over all rows), so the gradients are the same
+        bits.  The weight, bias and LayerNorm parameter gradients wait for layer 1's last group and run under the
+        recurrence of layer 0: earlier, they slow down the recurrences they run beside.  All cross-stream dependencies
+        are events; one BPTT grid is in flight at a time, and it completes once all its own CTAs are resident."""
+        reductions, eps, plan = ctx.cfg
+        B, T, I0, H, L, C = ctx.dims
+        dev = dout.device
+        main = torch.cuda.current_stream(dev)
+        st = _wave_bwd_streams(dev)
+        rec, prep, wgs = st[0], st[1:3], st[3]
+        gtop = ck[L].scatter(_c(dout))                       # d xs[L], chunk-major
+        whhT16 = [ops.transpose_to_bf16(_c(p[1])) for p in P]
+        wihT16 = [ops.transpose_to_bf16(_c(p[0])) for p in P]
+        for s_ in st:
+            s_.wait_stream(main)
+        dz = [ck[l].new(H, f32, dev) for l in range(L)]      # LayerNorm dz; layer l > 0: + the dgrad GEMM = d xs[l]
+        gz = [ck[l].new(H, f32, dev) if reductions[l] else None for l in range(L)]
+        dg16 = [ck[l].new(4 * H, bf16, dev) for l in range(L)]
+        # units of the schedule: groups of BPTT_GROUP consecutive chunks, one BPTT launch each (it walks their segments)
+        G = [list(range(max(0, e - BPTT_GROUP), e)) for e in range(C, 0, -BPTT_GROUP)][::-1]
+        NG = len(G)
+        ev = lambda: torch.cuda.Event()
+        prep_done = [[ev() for _ in range(NG)] for _ in range(L)]
+        rec_done = [[ev() for _ in range(NG)] for _ in range(L)]
+        carry = [(None, None)] * L
+        grads = [None] * (6 * L)
+        wg = []
+        for d in range(L + NG - 1):
+            for l in range(L - 1, -1, -1):
+                q = NG - 1 - (d - (L - 1 - l))
+                if not 0 <= q < NG:
+                    continue
+                k, kn = ck[l], ck[l + 1]
+                c0, c1 = G[q][0], G[q][-1] + 1
+                a, b = k.B * k.off[c0], k.B * k.off[c1]       # rows of the group on layer l's axis
+                with torch.cuda.stream(prep[l % 2]):
+                    if l + 1 < L:
+                        prep[l % 2].wait_event(rec_done[l + 1][q])
+                        an, bn = kn.B * kn.off[c0], kn.B * kn.off[c1]
+                        # the co-resident configuration shares the SMs of the running BPTT grid; the same bits as the
+                        # serial schedule's whole-layer GEMM (both sum each element's K in one order)
+                        ops.gemm_bf16(dg16[l + 1][an:bn], 0, wihT16[l + 1], 0, bn - an, H, 4 * H, out=dz[l + 1][an:bn],
+                                      accumulate=True, tag="gemm_bf16_nn", flags=ops.GEMM_CORESIDENT)
+                        gin = dz[l + 1]
+                    else:
+                        gin = gtop
+                    if reductions[l]:
+                        for c in G[q]:
+                            ops.time_reduce_bwd(kn.blk(gin, c), k.lens[c], out=k.blk(gz[l], c))
+                    gl = gz[l] if reductions[l] else gin
+                    ops.layernorm_bwd_dz(gl[a:b], y[l][a:b], xs[l][a:b] if l else None, P[l][4], mean[l][a:b],
+                                         rstd[l][a:b], out=dz[l][a:b])
+                    prep_done[l][q].record(prep[l % 2])
+                with torch.cuda.stream(rec):
+                    rec.wait_event(prep_done[l][q])
+                    _, dh, dc = ops.lstm_c4_bwd_chunks(dz[l][a:b], gates[l][a:b], cseq[l][a:b], whhT16[l],
+                                                       k.lens[c0:c1], B, dg16[l][a:b], cT[l, c0 - 1] if c0 else None,
+                                                       *carry[l])
+                    carry[l] = (dh, dc)
+                    rec_done[l][q].record(rec)
+                if q == 0:
+                    wg.append((l, gl))
+        # off the critical path: the weight, bias and LayerNorm parameter gradients, once layers L-1 .. 1 are done (under
+        # the recurrence of layer 0; earlier they would slow the recurrence of the layers they wait for)
+        with torch.cuda.stream(wgs):
+            for l, gl in wg:
+                wgs.wait_event(rec_done[min(l, 1)][0])
+                grads[6 * l + 0] = ops.mm_tn(dg16[l], x16[l], "bf16", dy16=dg16[l], x16=x16[l])
+                grads[6 * l + 1] = ops.mm_tn(dg16[l], y16[l], "bf16", dy16=dg16[l], x16=y16[l])
+                db = ops.colsum(dg16[l])
+                grads[6 * l + 2], grads[6 * l + 3] = db, db.clone()
+                grads[6 * l + 4], grads[6 * l + 5] = ops.layernorm_bwd_params(gl, y[l], xs[l], mean[l], rstd[l])
+        for s_ in st:
+            main.wait_stream(s_)
+        for t_ in grads:
+            t_.record_stream(main)
+        g = None
+        if ctx.needs_input_grad[0]:
+            g = ops.gemm_bf16(dg16[0], 0, ops.cast_bf16(_c(P[0][0])), 1, dg16[0].shape[0], I0, 4 * H, tag="gemm_bf16_nn")
         dxin = ck[0].gather(g) if g is not None else None
         return (dxin, None, *grads)
 

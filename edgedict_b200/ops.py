@@ -122,6 +122,7 @@ def gemm_f32(A, sam, sak, B, sbk, sbn, M, N, K, bias=None, out=None, beta=0.0, a
 
 
 GEMM_CORESIDENT = 1      # include/edgedict_b200.h EB_GEMM_CORESIDENT
+GEMM_FIXED_K = 2         # EB_GEMM_FIXED_K: row blocks of a product give the bits of the whole
 
 
 def gemm_bf16(A, a_mn, B, b_mn, M, N, K, bias=None, out=None, out_bf16=False, accumulate=False, tag=None, flags=0):
@@ -199,6 +200,24 @@ def layernorm_fwd(x, res, gamma, beta, eps=1e-5, want_bf16=False, out=None):
     check(lib().eb_layernorm_fwd(_p(x), _p(res), _p(gamma), _p(beta), _p(y), _p(y16), _p(mean), _p(rstd),
                                  rows, H, eps, _s()), "eb_layernorm_fwd")
     return y, y16, mean, rstd
+
+
+def layernorm_bwd_dz(dy, x, res, gamma, mean, rstd, out):
+    """The dz pass of layernorm_bwd alone, into out (rows independent: a row block gives the rows of the whole)."""
+    H = x.shape[-1]
+    check(lib().eb_layernorm_bwd_dz(_p(dy), _p(x), _p(res), _p(gamma), _p(mean), _p(rstd), _p(out), x.numel() // H, H,
+                                    _s()), "eb_layernorm_bwd_dz")
+    return out
+
+
+def layernorm_bwd_params(dy, x, res, mean, rstd):
+    """The parameter pass of layernorm_bwd alone: (dgamma, dbeta), the same bits as layernorm_bwd's."""
+    H = x.shape[-1]
+    dgamma = torch.zeros(H, dtype=f32, device=x.device)
+    dbeta = torch.zeros(H, dtype=f32, device=x.device)
+    check(lib().eb_layernorm_bwd_params(_p(dy), _p(x), _p(res), _p(mean), _p(rstd), _p(dgamma), _p(dbeta),
+                                        x.numel() // H, H, _s()), "eb_layernorm_bwd_params")
+    return dgamma, dbeta
 
 
 def layernorm_bwd(dy, x, res, gamma, mean, rstd):

@@ -97,6 +97,9 @@ int eb_gemm_bf16(const void* A, int a_mn_major, const void* B, int b_mn_major, v
  * bits on every run.  With a smaller workspace the split count shrinks to what fits (NULL / 0: no split; eb_gemm_bf16
  * passes none). */
 #define EB_GEMM_CORESIDENT 1
+/* EB_GEMM_FIXED_K: the tile width follows N alone (256 when N % 256 == 0) and K is never split, so every element's K
+ * order is independent of M: a product computed in row blocks gives the bits of the whole product. */
+#define EB_GEMM_FIXED_K 2
 long eb_gemm_bf16_partials(int a_mn_major, int c_bf16, int accumulate, long M, int N, long K, int flags);
 int eb_gemm_bf16_ex(const void* A, int a_mn_major, const void* B, int b_mn_major, void* C, int c_bf16,
                     const float* bias, int accumulate, long M, int N, long K, int flags, float* partials,
@@ -205,7 +208,6 @@ int eb_lstm_c4_bwd_chunks_cluster(int H);
 int eb_lstm_c4_bwd_chunks(const float* dy, const float* gates, const float* cseq, const float* c0,
                           const void* whhT16, const float* dhT, const float* dcT, void* dg16, float* dh0, float* dc0,
                           void* scratch, int B, const int* chunk_lens, int nchunks, int H, void* stream);
-
 /* ---- LayerNorm(x + res) fwd/bwd, TimeReduction, Embedding -------------------------------
  * rnnt/models.py:47,66-69,124 ; :21-29 ; :150-153.  *_bf16 outputs are optional side copies.
  * LayerNorm: rows > 0 and 0 < H <= 2048.  Time reduction and embedding: negative sizes are EB_ERR_INVALID, an empty
@@ -215,6 +217,11 @@ int eb_layernorm_fwd(const float* x, const float* res, const float* gamma, const
 int eb_layernorm_bwd(const float* dy, const float* x, const float* res, const float* gamma,
                      const float* mean, const float* rstd, float* dz, float* dgamma_accum,
                      float* dbeta_accum, long rows, int H, void* stream);
+/* the two passes of eb_layernorm_bwd apart: dz (rows independent) and the parameter gradients (fixed order over rows) */
+int eb_layernorm_bwd_dz(const float* dy, const float* x, const float* res, const float* gamma, const float* mean,
+                        const float* rstd, float* dz, long rows, int H, void* stream);
+int eb_layernorm_bwd_params(const float* dy, const float* x, const float* res, const float* mean, const float* rstd,
+                            float* dgamma_accum, float* dbeta_accum, long rows, int H, void* stream);
 int eb_time_reduce_fwd(const float* x, float* y, void* y_bf16, int B, int T, int H, void* stream);
 int eb_time_reduce_bwd(const float* dy, float* dx, int B, int T, int H, void* stream);
 int eb_embedding_fwd(const void* ids, int ids_are_int64, const float* W, float* out, void* out_bf16,
