@@ -368,6 +368,11 @@ class LSTMStack(torch.autograd.Function):
     returns y [B,T',H], h_T [L,B,H], c_T [L,B,H] (final states: not differentiated through)."""
 
     collect = None      # tests: set to a list to receive every layer's output [B,T_l,H] (parity of the per-layer activations)
+    # tests: set to a list to receive, per backward and per layer l = 0 .. L-1, a dict of [B,T_l,.] tensors: "dln" the
+    # LayerNorm's incoming gradient (after TimeReduction backward), "dy" the BPTT's input (the LayerNorm dz, before the dgrad
+    # GEMM accumulates into it), "dg16" the bf16 dG of the BPTT, "dxs" d xs[l] (dy + the dgrad GEMM; None for l = 0, whose
+    # product is the returned dx).  Off (None): nothing is copied or ordered.
+    collect_bwd = None
 
     @staticmethod
     def forward(ctx, x, cfg, *params):
@@ -504,6 +509,8 @@ class LSTMStack(torch.autograd.Function):
         side.wait_stream(main)
         g = ck[L].scatter(_c(dout))                           # d xs[L], chunk-major
         grads = [None] * (6 * L)
+        hook = LSTMStack.collect_bwd
+        recs = [None] * L
         for l in range(L - 1, -1, -1):
             k, kn = ck[l], ck[l + 1]
             if reductions[l]:
@@ -512,6 +519,8 @@ class LSTMStack(torch.autograd.Function):
                     ops.time_reduce_bwd(kn.blk(g, c), k.lens[c], out=k.blk(gz, c))
                 g = gz
             dz, dgamma, dbeta = ops.layernorm_bwd(g, y[l], xs[l], P[l][4], mean[l], rstd[l])
+            if hook is not None:
+                recs[l] = dict(dln=k.gather(g), dy=k.gather(dz))
             whhT16 = ops.transpose_to_bf16(_c(P[l][1]))
             dg16 = k.new(4 * H, bf16, dev)
             dh = dc = None
@@ -550,6 +559,8 @@ class LSTMStack(torch.autograd.Function):
                 g = ops.gemm_bf16(dg16, 0, wih16, 1, M, I_l, 4 * H, tag="gemm_bf16_nn")
             else:
                 g = None
+            if hook is not None:
+                recs[l].update(dg16=k.gather(dg16), dxs=k.gather(g) if l > 0 else None)
             # off the critical path: the weight / bias gradients of this layer run on a side stream under the BPTT
             # recurrence of the next layer (which leaves 20 SMs idle and the tensor pipe nearly so)
             ready = torch.cuda.Event()
@@ -566,6 +577,8 @@ class LSTMStack(torch.autograd.Function):
                     t_.record_stream(main)
             grads[6 * l + 4], grads[6 * l + 5] = dgamma, dbeta
         main.wait_stream(side)
+        if hook is not None:
+            hook.extend(recs)
         dxin = ck[0].gather(g) if g is not None else None
         return (dxin, None, *grads)
 
@@ -600,6 +613,8 @@ class LSTMStack(torch.autograd.Function):
         dz = [ck[l].new(H, f32, dev) for l in range(L)]      # LayerNorm dz; layer l > 0: + the dgrad GEMM = d xs[l]
         gz = [ck[l].new(H, f32, dev) if reductions[l] else None for l in range(L)]
         dg16 = [ck[l].new(4 * H, bf16, dev) for l in range(L)]
+        hook = LSTMStack.collect_bwd
+        dyc = [ck[l].new(H, f32, dev) for l in range(L)] if hook is not None else None
         # units of the schedule: groups of BPTT_GROUP consecutive chunks, one BPTT launch each (it walks their segments)
         G = [list(range(max(0, e - BPTT_GROUP), e)) for e in range(C, 0, -BPTT_GROUP)][::-1]
         NG = len(G)
@@ -634,6 +649,10 @@ class LSTMStack(torch.autograd.Function):
                     gl = gz[l] if reductions[l] else gin
                     ops.layernorm_bwd_dz(gl[a:b], y[l][a:b], xs[l][a:b] if l else None, P[l][4], mean[l][a:b],
                                          rstd[l][a:b], out=dz[l][a:b])
+                    if dyc is not None:
+                        # the copy is ordered before prep_done[l][q]; the BPTT of the group waits for that event and the
+                        # dgrad GEMM of layer l-1 that adds into these rows waits for rec_done[l][q], recorded after it
+                        dyc[l][a:b].copy_(dz[l][a:b])
                     prep_done[l][q].record(prep[l % 2])
                 with torch.cuda.stream(rec):
                     rec.wait_event(prep_done[l][q])
@@ -661,6 +680,10 @@ class LSTMStack(torch.autograd.Function):
         g = None
         if ctx.needs_input_grad[0]:
             g = ops.gemm_bf16(dg16[0], 0, ops.cast_bf16(_c(P[0][0])), 1, dg16[0].shape[0], I0, 4 * H, tag="gemm_bf16_nn")
+        if hook is not None:
+            gls = dict(wg)
+            hook.extend(dict(dln=ck[l].gather(gls[l]), dy=ck[l].gather(dyc[l]), dg16=ck[l].gather(dg16[l]),
+                             dxs=ck[l].gather(dz[l]) if l else None) for l in range(L))
         dxin = ck[0].gather(g) if g is not None else None
         return (dxin, None, *grads)
 

@@ -48,6 +48,7 @@ U24 = 2.0 ** -24          # fp32 unit roundoff, round to nearest (the FMA chains
 TINY = 2.0 ** -120        # absolute floor of every bar
 BM, BK = 128, 64          # gemm_tc.cu: rows of a tile, k per k-block
 CORESIDENT = 1            # include/edgedict_b200.h EB_GEMM_CORESIDENT
+FIXED_K = 2               # EB_GEMM_FIXED_K
 
 
 def _lib():
@@ -134,10 +135,13 @@ def _plan(M, N, K, c16=0, acc=0, flags=0):
     low = bool(flags & CORESIDENT)
     if low:
         wide = False
+    fixed = bool(flags & FIXED_K)            # the tile width follows N alone and K is never split
+    if fixed:
+        wide = N % 256 == 0
     bn = 256 if wide else 128
     out_tiles = num_m * _cdiv(N, bn)
     ks = 1
-    if not low and not c16 and nkb >= 64 and out_tiles < nsm:
+    if not low and not fixed and not c16 and nkb >= 64 and out_tiles < nsm:
         ks = _choose_ksplit(out_tiles, nkb, nsm, 32.0 if bn == 256 else 16.0)
     return bn, ks
 
@@ -431,6 +435,50 @@ def test_gemm_bf16_split_k(name):
           _split_sum(c, ksplit, bias, c0))
     # no workspace: one chain over all of K
     c.check_raw("no split", c.gemm("no split"))
+
+
+# ---- EB_GEMM_FIXED_K: the serial encoder backward's dgrad GEMM ----------------------------------------------------------
+# (name, M, N, K): A K-major, B MN-major (dG [rows, 4H] times W_ih [4H, I]).  N = 1024 at M = 300 would be split at the
+# default plan (12 wide tiles, 64 k-blocks); FIXED_K keeps one chain over K.
+FIXED_K_CASES = [("fixedk-M300-N1024-K4096", 300, 1024, 4096), ("fixedk-M200-N240-K4096", 200, 240, 4096),
+                 ("fixedk-M129-N640-K72", 129, 640, 72)]
+
+
+@pytest.mark.parametrize("name,M,N,K", FIXED_K_CASES, ids=[c[0] for c in FIXED_K_CASES])
+def test_gemm_bf16_fixed_k(name, M, N, K):
+    """EB_GEMM_FIXED_K: the tile width follows N alone (256 when N % 256 == 0) and K is never split.  The raw product is
+    within the fp64 bar of one chain over K, and the epilogue relations hold on it."""
+    bn, ks, _ = _config(0, M, N, K, flags=FIXED_K)
+    assert (bn, ks) == (256 if N % 256 == 0 else 128, 1), (name, bn, ks)
+    c = Case(name, M, N, K, 0, 1, "normal", seed=M + N + K)
+    P = c.gemm("raw", flags=FIXED_K)
+    c.check_raw("raw", P)
+    _same(name + " repeated launch", c.gemm("raw", flags=FIXED_K), P)
+    _relations(c, P, flags=FIXED_K, tag=" (fixed K)")
+
+
+@pytest.mark.parametrize("N", [1024, 240])
+def test_gemm_bf16_fixed_k_equals_coresident_row_blocks(N):
+    """The invariant both encoder backward schedules rest on: the serial schedule's whole-layer dgrad GEMM (FIXED_K, A
+    K-major, B MN-major, accumulated onto fp32 C) is bitwise the chunked schedule's co-resident GEMMs (B transposed to
+    K-major) on row blocks accumulated onto the same C: one row, blocks that are not a multiple of 128, and the
+    wavefront's group sizes at B = 32 (3 x 168 and 2 x 168 + 160 frames, 3 x 84 on the reduced axis)."""
+    K = 4096
+    blocks = [1, 77, 333, 32 * 504, 32 * 496, 32 * 252]
+    M = sum(blocks)
+    g = torch.Generator(device=DEV).manual_seed(N)
+    A = (torch.randn(M, K, device=DEV, generator=g) * 0.1).bfloat16()
+    Bt = (torch.randn(N, K, device=DEV, generator=g) / 32).bfloat16()         # W_ih^T: [I, 4H], K-major
+    Bn = Bt.t().contiguous()                                                  # W_ih: [4H, I], MN-major
+    C0 = torch.randn(M, N, device=DEV, generator=g)
+    assert _partials(0, 0, 1, M, N, K, FIXED_K) == 0
+    whole = _gemm("fixed-K whole", A, 0, Bn, 1, M, N, K, init=C0, flags=FIXED_K)
+    a = 0
+    for n in blocks:
+        part = _gemm("co-resident rows [%d, %d)" % (a, a + n), A[a:a + n], 0, Bt, 0, n, N, K, init=C0[a:a + n],
+                     flags=CORESIDENT)
+        _same("N%d: co-resident rows [%d, %d) vs fixed-K whole" % (N, a, a + n), part, whole[a:a + n])
+        a += n
 
 
 # ---- the joint's logits ----------------------------------------------------------------------------------------------

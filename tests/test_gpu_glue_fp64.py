@@ -182,10 +182,10 @@ def _ln_inputs(rows, H, with_res, offset, seed, scale=1.0):
 
 
 def _ln_ref(z, mean_k, rstd_k, gamma, beta, eps, H):
-    """fp64 LayerNorm of z and the bars of the kernel's mean, rstd and y (module docstring)."""
-    zd = z.double().cpu()
-    mk, rk = mean_k.double().cpu(), rstd_k.double().cpu()
-    gd, bd = gamma.double().cpu(), beta.double().cpu()
+    """fp64 LayerNorm of z and the bars of the kernel's mean, rstd and y (module docstring), on the device of z."""
+    zd = z.double()
+    mk, rk = mean_k.double(), rstd_k.double()
+    gd, bd = gamma.double(), beta.double()
     n_add = _pl(H) + 5
     mu = zd.mean(1)
     bar_mu = n_add * U24 * zd.abs().sum(1) / H + U24 * mu.abs()
@@ -265,6 +265,27 @@ def _dbeta_order(dy, H):
     return acc[0]
 
 
+def ln_bwd_ref(z, mean_k, rstd_k, dy, gamma, dg0=None):
+    """Teacher-forced fp64 LayerNorm backward from the kernel's mean / rstd, on the device of the inputs (module
+    docstring): (dz, its bar, the magnitude sum |g| + |s1| + |xhat s2| of each dz, dgamma = dg0 + sum dy xhat, its bar)."""
+    zd, mk, rk, dyd, gd = (t.double() for t in (z, mean_k, rstd_k, dy, gamma))
+    rows, H = zd.shape
+    xh = (zd - mk[:, None]) * rk[:, None]
+    gg = dyd * gd
+    s1 = gg.mean(1, keepdim=True)
+    s2 = (gg * xh).mean(1, keepdim=True)
+    dz = rk[:, None] * (gg - s1 - xh * s2)
+    n_add = -(-H // 32) + 8
+    e1 = (n_add + 3) * U24 * gg.abs().mean(1, keepdim=True)
+    e2 = (n_add + 6) * U24 * (gg * xh).abs().mean(1, keepdim=True)
+    mag = gg.abs() + s1.abs() + (xh * s2).abs()
+    bar = rk[:, None] * (5 * U24 * mag + e1 + xh.abs() * e2) + U24 * dz.abs()
+    dg0 = torch.zeros(H, dtype=torch.float64, device=zd.device) if dg0 is None else dg0.double()
+    dgam = dg0 + (dyd * xh).sum(0)
+    bar_dgam = (3 + -(-rows // 128) + 8) * U24 * (dyd * xh).abs().sum(0) + U24 * (dg0.abs() + dgam.abs())
+    return dz, bar, mag, dgam, bar_dgam
+
+
 # (name, rows, H, residual): H % 128 == 0 and H <= 1024 reach both dz kernels (aligned vs a view offset by one float);
 # rows < 128 and rows % 128 != 0 (the param-grad row lanes), H % 8 != 0 (the last CTA's partial column group),
 # rows > 4 x 3 x #SMs (the vectorised kernel's grid-stride loop)
@@ -292,28 +313,15 @@ def test_layernorm_bwd(name, rows, H, with_res):
     dg0 = torch.randn(H, device=DEV, generator=g)
     db0 = torch.randn(H, device=DEV, generator=g)
     z = (x + res if with_res else x).double().cpu()
-    mk, rk = mean.double().cpu(), rstd.double().cpu()
-    dyd, gd = dy.double().cpu(), gamma.double().cpu()
-    # teacher-forced fp64 dz and its bar
-    xh = (z - mk[:, None]) * rk[:, None]
-    gg = dyd * gd
-    s1 = gg.mean(1, keepdim=True)
-    s2 = (gg * xh).mean(1, keepdim=True)
-    dz_tf = rk[:, None] * (gg - s1 - xh * s2)
-    n_add = -(-H // 32) + 8
-    e1 = (n_add + 3) * U24 * gg.abs().mean(1, keepdim=True)
-    e2 = (n_add + 6) * U24 * (gg * xh).abs().mean(1, keepdim=True)
-    mag = gg.abs() + s1.abs() + (xh * s2).abs()
-    bar_tf = rk[:, None] * (5 * U24 * mag + e1 + xh.abs() * e2) + U24 * dz_tf.abs()
+    rk = rstd.double().cpu()
+    # teacher-forced fp64 dz and its bar; dgamma teacher-forced, barred
+    dz_tf, bar_tf, mag, dgam_tf, bar_dgam = ln_bwd_ref(z, mean.cpu(), rstd.cpu(), dy.cpu(), gamma.cpu(), dg0.cpu())
     # end to end: fp64 torch.layer_norm autograd
     zr = z.clone().requires_grad_(True)
-    torch.nn.functional.layer_norm(zr, (H,), gd, None, eps).backward(dyd)
+    torch.nn.functional.layer_norm(zr, (H,), gamma.double().cpu(), None, eps).backward(dy.double().cpu())
     dz_e2e = zr.grad
     bar_e2e = 4 * bar_tf + 64 * U24 * rk[:, None] * mag
-    # parameter gradients: dgamma teacher-forced, barred; dbeta bitwise in the kernel's order
-    dgam_tf = dg0.double().cpu() + (dyd * xh).sum(0)
-    bar_dgam = (3 + -(-rows // 128) + 8) * U24 * (dyd * xh).abs().sum(0) + U24 * (dg0.double().cpu().abs()
-                                                                                  + dgam_tf.abs())
+    # dbeta bitwise in the kernel's order
     dbeta_want = torch.from_numpy(db0.cpu().numpy() + _dbeta_order(dy, H))
 
     L = _lib()
@@ -341,6 +349,44 @@ def test_layernorm_bwd(name, rows, H, with_res):
         results[kern] = dgb[:H].clone()
     if len(results) == 2:
         _same(name + " dgamma: vectorised vs generic dz kernel", results["vectorised"], results["generic"])
+
+
+@pytest.mark.parametrize("H,off", [(1024, 0), (1024, 1), (1000, 0)], ids=["H1024-vectorised", "H1024-offset-generic",
+                                                                          "H1000-generic"])
+@pytest.mark.parametrize("with_res", [False, True])
+def test_layernorm_bwd_split_entry_points(H, off, with_res):
+    """The two halves of eb_layernorm_bwd that the chunked encoder backward calls separately: eb_layernorm_bwd_dz on row
+    sub-ranges (one row, a ragged block, the wavefront's group sizes) gives bitwise the matching rows of eb_layernorm_bwd's
+    dz, on the vectorised kernel (H = 1024, aligned) and the generic one (x offset by one float, or H % 128 != 0); and
+    eb_layernorm_bwd_params over all rows gives bitwise its dgamma / dbeta."""
+    rows, eps = 2300, 1e-5
+    x, res, gamma, beta = _ln_inputs(rows, H, with_res, 0.0, seed=H + off + 3 * with_res)
+    dy = torch.randn(rows, H, device=DEV, generator=_gen(rows + H))
+    _, _, mean, rstd = _ln_fwd(x, res, gamma, beta, rows, H, eps)
+    xv = _offset_copy(x, off) if off else x
+    L = _lib()
+    dz = _nan(rows * H)
+    dg, db = torch.zeros(H, device=DEV), torch.zeros(H, device=DEV)
+    _ok(L.eb_layernorm_bwd(_p(dy), _p(xv), _p(res), _p(gamma), _p(mean), _p(rstd), _p(dz), _p(dg), _p(db), rows, H,
+                           _stream()), "eb_layernorm_bwd")
+    dz = dz[:rows * H].view(rows, H)
+    vec = _ln_bwd_vec(H, [dy.data_ptr(), xv.data_ptr(), dz.data_ptr(), gamma.data_ptr(), res.data_ptr() if with_res else 0])
+    assert vec == (H == 1024 and off == 0)
+    name = "layernorm_bwd H%d %s%s" % (H, "vectorised" if vec else "generic", " res" if with_res else "")
+    blocks = [(0, 1), (1, 127), (128, 32 * 5 + 3), (291, 5 * 96), (771, 1529)]      # a partition of the rows
+    assert blocks[-1][0] + blocks[-1][1] == rows
+    for a, n in blocks:
+        out = _nan(n * H)
+        r = res[a:a + n] if with_res else None
+        _ok(L.eb_layernorm_bwd_dz(_p(dy[a:a + n]), _p(xv[a:a + n]), _p(r), _p(gamma), _p(mean[a:a + n]),
+                                  _p(rstd[a:a + n]), _p(out), n, H, _stream()), "eb_layernorm_bwd_dz")
+        _guard(name, out, n * H)
+        _same("%s dz rows [%d, %d)" % (name, a, a + n), out[:n * H].view(n, H), dz[a:a + n])
+    dg2, db2 = torch.zeros(H, device=DEV), torch.zeros(H, device=DEV)
+    _ok(L.eb_layernorm_bwd_params(_p(dy), _p(xv), _p(res), _p(mean), _p(rstd), _p(dg2), _p(db2), rows, H, _stream()),
+        "eb_layernorm_bwd_params")
+    _same(name + " dgamma of the parameter pass", dg2, dg)
+    _same(name + " dbeta of the parameter pass", db2, db)
 
 
 # ---- time reduction ---------------------------------------------------------------------------------------------------
