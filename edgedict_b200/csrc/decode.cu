@@ -25,6 +25,8 @@
 //   BEAM_FINAL  per utterance: best live slot, back-pointer walk through the history, ids and -log p written out
 //   BEAM_COMMIT per stream, at the end of a streaming chunk: commit the live hypotheses' common prefix, collapse the
 //           beam to its best slot when a stored suffix would outgrow its capacity (or on a flush)
+//   GRU     one nn.GRU cell step for S streams (ResLayerNormGRU, models.py:77-116): CTCEncoder's streaming encoder
+//   CTC_EMIT per stream: log-softmax, argmax, repeats (carried across chunks) and blanks dropped (CTCEncoder.greedy_decode)
 //
 // LINEAR's x1 row divisor (x1_div) lets the W rows of one utterance's beam share its encoder frame without copies.
 // fp32-accurate arithmetic throughout: the north star asks for token-for-token identical greedy output, which
@@ -251,6 +253,61 @@ __device__ void phase_lstm(const EbPhase& p, float* red, float* outs) {
     }
 }
 
+// GRU: one nn.GRU cell step for S rows, gate order r|z|n (w1 = W_ih [3H, K1], w2 = W_hh [3H, K2 = H], b1 = b_ih,
+// b2 = b_hh, h read from x2).  LSTM's tile: each of a tile's 8 units takes 4 columns, r, z, n_x (x W_in alone) and n_h
+// (h W_hn alone); the rows a column does not use are nullptr, which tile_mma reads as zeros, so a step streams the
+// 3H (K1 + K2) weights once.  r and z add b1 then b2 as LSTM's gates do; n = tanh((n_x + b_in) + r (n_h + b_hn)) keeps
+// b_hn inside the reset product (nn.GRU); h' = (1 - z) n + z h.
+__device__ void phase_gru(const EbPhase& p, float* red, float* outs) {
+    const int S = p.S, H = p.N;
+    const int ctiles = (H + 7) / 8, rtiles = (S + TR - 1) / TR;
+    const int tid = threadIdx.x;
+    const bool a1vec = vec_ok(p.x1, p.ldx1, p.K1), a2vec = vec_ok(p.x2, p.ldx2, p.K2);
+    const bool b1vec = vec_ok(p.w1, p.ldw1, p.K1), b2vec = vec_ok(p.w2, p.ldw2, p.K2);
+    for (int tile = blockIdx.x; tile < ctiles * rtiles; tile += gridDim.x) {
+        const int s0 = (tile / ctiles) * TR, j0 = (tile % ctiles) * 8;
+        const int nrows = min(TR, S - s0), nunits = min(8, H - j0);
+        float acc[4][4][4];
+#pragma unroll
+        for (int a = 0; a < 4; ++a)
+#pragma unroll
+            for (int b = 0; b < 4; ++b)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) acc[a][b][c] = 0.f;
+        auto x1row = [&](int r) -> const float* { return p.x1 + (long)(s0 + r) * p.ldx1; };
+        auto hrow = [&](int r) -> const float* { return p.x2 + (long)(s0 + r) * p.ldx2; };
+        // column n = 4 u + g: g = 0 r, 1 z, 2 n_x (W_ih rows only), 3 n_h (W_hh rows only)
+        auto w1row = [&](int n) -> const float* {
+            const int g = n & 3;
+            return g == 3 ? nullptr : p.w1 + ((long)g * H + j0 + (n >> 2)) * p.ldw1;
+        };
+        auto w2row = [&](int n) -> const float* {
+            const int g = n & 3;
+            return g == 2 ? nullptr : p.w2 + ((long)(g == 3 ? 2 : g) * H + j0 + (n >> 2)) * p.ldw2;
+        };
+        int step = 0;
+        tile_mma(acc, x1row, w1row, p.K1, nrows, nunits * 4, a1vec, b1vec, step);
+        tile_mma(acc, hrow, w2row, p.K2, nrows, nunits * 4, a2vec, b2vec, step);
+        tile_reduce(acc, red, outs);
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+            const int e = q * 256 + tid;
+            const int r = e >> 3, u = e & 7;
+            const int s = s0 + r;
+            if (r >= nrows || u >= nunits) continue;
+            const int j = j0 + u;
+            const float* o = outs + r * OUT_LD + u * 4;
+            const float rg = sigmoidf_(o[0] + p.b1[j] + p.b2[j]);
+            const float zg = sigmoidf_(o[1] + p.b1[(long)H + j] + p.b2[(long)H + j]);
+            const float ng = tanhf((o[2] + p.b1[2L * H + j]) + rg * (o[3] + p.b2[2L * H + j]));
+            const float hp = __ldcg(p.x2 + (long)s * p.ldx2 + j);
+            const float hn = (1.f - zg) * ng + zg * hp;
+            p.y[(long)s * p.ldy + j] = hn;
+            if (p.y2) p.y2[(long)s * H + j] = hn;
+        }
+    }
+}
+
 __device__ void phase_linear(const EbPhase& p, float* red, float* outs) {
     const int S = p.S, N = p.N;
     const int ctiles = (N + TC - 1) / TC, rtiles = (S + TR - 1) / TR;
@@ -360,6 +417,60 @@ __device__ void phase_argmax(const EbPhase& p) {
         if (lane == 0) {
             p.tok_out[s] = pred;
             if (p.hist) p.hist[(long)s * p.hist_ld + p.hist_col] = pred;
+        }
+    }
+}
+
+// CTC_EMIT: greedy CTC emission of one streaming chunk (CTCEncoder.greedy_decode, rnnt/models.py:294-310, carried across
+// chunks), one warp per stream.  Field use: S streams, aux = n frames (row s*n + t), N = V, aux2 = blank; x1 logits
+// (ldx1); y log-probs out (ldy), each row as eb_log_softmax_fwd forms it, (x - max) - log(sum exp(x - max)); tok_out [S]
+// the previous frame's argmax (in / out; a negative value after a reset matches no token); hist ids [S, hist_ld] and
+// tok_out2 counts [S]; y2 the running score [S] as DOUBLE, += the fp32 whole-row sum of every kept frame's log-probs;
+// seq_out (optional) the argmax of every frame [S, n].  A frame is kept when its argmax (torch.argmax order over the
+// log-probs: NaN first, ties to the lowest id) is not blank and differs from the previous frame's.
+__device__ __noinline__ void phase_ctc_emit(const EbPhase& p) {
+    const int lane = threadIdx.x & 31, V = p.N, n = p.aux, blank = p.aux2;
+    double* score = reinterpret_cast<double*>(p.y2);
+    for (int s = blockIdx.x * 8 + (threadIdx.x >> 5); s < p.S; s += gridDim.x * 8) {
+        int prev = __ldcg(p.tok_out + s), cnt = 0;
+        double acc = 0.0;
+        for (int t = 0; t < n; ++t) {
+            const long row = (long)s * n + t;
+            const float* x = p.x1 + row * p.ldx1;
+            float* lp = p.y + row * p.ldy;
+            float m = -INFINITY;
+            for (int v = lane; v < V; v += 32) m = fmaxf(m, __ldcg(x + v));
+            m = warp_max(m);
+            float e = 0.f;
+            for (int v = lane; v < V; v += 32) e += expf(__ldcg(x + v) - m);
+            const float ls = logf(warp_sum(e));
+            float best = -INFINITY, sum = 0.f;
+            int bi = 0x7fffffff;
+            for (int v = lane; v < V; v += 32) {
+                const float val = (__ldcg(x + v) - m) - ls;
+                lp[v] = val;
+                if (argmax_before(val, v, best, bi)) { best = val; bi = v; }
+                sum += val;
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+                const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+                if (argmax_before(ob, oi, best, bi)) { best = ob; bi = oi; }
+            }
+            sum = warp_sum(sum);
+            if (bi != blank && bi != prev) {
+                if (lane == 0) p.hist[(long)s * p.hist_ld + cnt] = bi;
+                ++cnt;
+                acc += (double)sum;
+            }
+            if (lane == 0 && p.seq_out) p.seq_out[row] = bi;
+            prev = bi;
+        }
+        if (lane == 0) {
+            p.tok_out[s] = prev;
+            p.tok_out2[s] = cnt;
+            score[s] += acc;
         }
     }
 }
@@ -1209,7 +1320,10 @@ static_assert(sizeof(EbPhase) % 4 == 0 && sizeof(EbPhase) / 4 <= 256, "EbPhase l
 // Two instantiations: CTC = false runs every phase but CTC_BEAM (which it skips), CTC = true adds CTC_BEAM.  Any reachable
 // call to phase_ctc_beam, whatever the call site, takes this kernel from 12 / 16 to 44 / 136 bytes of spill stores / loads,
 // some of them inside the matrix phases' tile loops; the programs that do not search CTC beams keep the kernel without it.
-template <bool CTC>
+// A third, CTC_STREAM = true (eb_decode_run_ctc_stream), adds GRU and CTC_EMIT, the phases of a streaming CTC chunk, and
+// skips LSTM (with it, 28 / 52 bytes of spills instead of 16 / 28); the other two skip GRU and CTC_EMIT like any unknown
+// type, so their code and registers are what they were without these phases.
+template <bool CTC, bool CTC_STREAM>
 __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __restrict__ prog, int nphase, unsigned* bar) {
     extern __shared__ __align__(16) float dsm[];
     float* red = dsm;                                        // [8 warps][2048]
@@ -1238,7 +1352,9 @@ __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __re
                     ph.y[k] = 0.5f * (__ldcg(x) + __ldcg(x + H));
                 }
             } break;
-            case EB_PH_LSTM: phase_lstm(ph, red, outs); break;
+            case EB_PH_LSTM:
+                if constexpr (!CTC_STREAM) phase_lstm(ph, red, outs);
+                break;
             case EB_PH_LINEAR: phase_linear(ph, red, outs); break;
             case EB_PH_ARGMAX: phase_argmax(ph); break;
             case EB_PH_COPY:
@@ -1257,7 +1373,12 @@ __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __re
                 if (!phase_skip_live(ph) && threadIdx.x == 0) next = i + 1 + ph.aux;
                 __syncthreads();                             // every thread reads the same next
                 continue;
-            default: break;
+            default:
+                if constexpr (CTC_STREAM) {
+                    if (ph.type == EB_PH_GRU) phase_gru(ph, red, outs);
+                    else if (ph.type == EB_PH_CTC_EMIT) phase_ctc_emit(ph);
+                }
+                break;
         }
         ++epoch;
         if (i + 1 < nphase) grid_sync(bar, epoch * gridDim.x);
@@ -1269,7 +1390,7 @@ __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __re
 
 }  // namespace
 
-template <bool CTC>
+template <bool CTC, bool CTC_STREAM>
 int decode_run(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream) {
     if (!phases_dev || nphase <= 0 || !barrier_dev) return EB_ERR_INVALID;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -1280,17 +1401,23 @@ int decode_run(const void* phases_dev, int nphase, void* barrier_dev, int max_ct
     unsigned* bar = reinterpret_cast<unsigned*>(barrier_dev);
     void* args[] = {(void*)&prog, (void*)&nphase, (void*)&bar};
     const size_t smem = sizeof(float) * (RED_FLOATS + TR * OUT_LD);
-    EB_CUDA(cudaFuncSetAttribute(decode_program_kernel<CTC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    EB_CUDA(cudaLaunchCooperativeKernel((void*)decode_program_kernel<CTC>, dim3(grid), dim3(256), args, smem, st));
+    EB_CUDA(cudaFuncSetAttribute(decode_program_kernel<CTC, CTC_STREAM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)smem));
+    EB_CUDA(cudaLaunchCooperativeKernel((void*)decode_program_kernel<CTC, CTC_STREAM>, dim3(grid), dim3(256), args, smem,
+                                        st));
     return EB_OK;
 }
 
 EB_API int eb_decode_run(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream) {
-    return decode_run<false>(phases_dev, nphase, barrier_dev, max_ctas, stream);
+    return decode_run<false, false>(phases_dev, nphase, barrier_dev, max_ctas, stream);
 }
 
 EB_API int eb_decode_run_ctc(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream) {
-    return decode_run<true>(phases_dev, nphase, barrier_dev, max_ctas, stream);
+    return decode_run<true, false>(phases_dev, nphase, barrier_dev, max_ctas, stream);
+}
+
+EB_API int eb_decode_run_ctc_stream(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream) {
+    return decode_run<false, true>(phases_dev, nphase, barrier_dev, max_ctas, stream);
 }
 
 EB_API int eb_decode_phase_size(void) { return (int)sizeof(EbPhase); }

@@ -190,3 +190,63 @@ def beam_search(log_probs, input_lengths, beam_width, blank=0, *, lm=None, lm_we
         ids, nlogp = eng.run(log_probs, lens.to(dev, non_blocking=True))
         ids = ids.cpu().numpy()
     return [row[row >= 0].astype("int64") for row in ids], nlogp.clone()
+
+
+class CTCStreamDecoder:
+    """Streaming greedy CTC decoding of a ``CTCEncoder`` with ``PytorchStreamDecoder``'s surface (rnnt/stream.py:15-120):
+    ``reset()``, ``decode(frame) -> str``, ``reset_profile()``, the ``encoder_elapsed`` / ``decoder_elapsed`` /
+    ``joint_elapsed`` lists and ``tokenizer``.  ``decode`` runs one persistent kernel launch per chunk
+    (stream_engine.CTCStreamEngine, one stream) and returns the text of the ids emitted in that chunk, ``'</w>'`` turned
+    into a space.  The ids of all chunks together are ``CTCEncoder.greedy_decode``'s on the concatenated frames: a token
+    held across a chunk boundary is emitted once.
+
+    ``transform`` maps a chunk of audio to log-mel features [1, F, n] (the reference's feature transform);
+    ``tokenizer`` is the reference's HuggingFaceTokenizer (``tokenizer.tokenizer.id_to_token``).  A chunk whose frame
+    count differs from the previous one's (a short last chunk), or weights that moved (``.to()``, an optimizer's flat
+    bucket), rebuild the program and carry the state over; only ``reset()`` starts a new utterance.  Chunks must hold an
+    even number of frames before each time reduction."""
+
+    def __init__(self, model, transform, tokenizer, device="cuda", frames_per_chunk=None):
+        from .rnnt.models import CTCEncoder
+        if not isinstance(model, CTCEncoder):
+            raise TypeError("CTCStreamDecoder decodes a CTCEncoder, got %s" % type(model).__name__)
+        self.device = torch.device(device)
+        self.transform, self.tokenizer = transform, tokenizer
+        model.eval()
+        model.to(self.device)
+        self.model = model
+        self._engine = None
+        self._frames = frames_per_chunk
+        self.reset_profile()
+        if frames_per_chunk is not None:
+            self._build(operator.index(frames_per_chunk))
+
+    def reset_profile(self):
+        self.encoder_elapsed = []
+        self.decoder_elapsed = []
+        self.joint_elapsed = []
+
+    def _build(self, n):
+        from .stream_engine import CTCStreamEngine
+        st = self._engine.state() if self._engine is not None else None
+        self._engine = CTCStreamEngine(self.model, 1, n, blank=self.model.blank, state=st)
+        self._frames = n
+
+    @torch.no_grad()
+    def reset(self):
+        if self._engine is not None:
+            self._engine.reset()
+
+    @torch.no_grad()
+    def decode(self, frame):
+        import time
+        from .stream_engine import param_fingerprint
+        start = time.time()
+        xs = self.transform(frame).transpose(1, 2)                 # [1, n, F] log-mel
+        if self._engine is None or xs.shape[1] != self._frames or \
+                self._engine.fingerprint != param_fingerprint(self.model):
+            self._build(xs.shape[1])
+        ids, counts = self._engine.step(xs.to(self.device, non_blocking=True))   # one D2H per chunk
+        self.encoder_elapsed.append(time.time() - start)
+        return "".join(self.tokenizer.tokenizer.id_to_token(int(k)).replace('</w>', ' ')
+                       for k in ids[0, :int(counts[0])].tolist())

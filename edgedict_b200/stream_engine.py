@@ -20,7 +20,7 @@ from ._lib import lib, check
 from .rnnt.tokenizer import NUL, BOS, UNK
 
 PH_LN, PH_PAIR, PH_LSTM, PH_LINEAR, PH_ARGMAX, PH_COPY, PH_BEAM_SELECT, PH_GATHER, PH_BEAM_FINAL, PH_BEAM_COMMIT, \
-    PH_SKIP, PH_CTC_BEAM = range(12)
+    PH_SKIP, PH_CTC_BEAM, PH_GRU, PH_CTC_EMIT = range(14)
 F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE, F_LM, F_STREAM, F_FLUSH, F_CONT, F_ROUNDS = 1, 2, 4, 8, 16, 32, 64, 128, \
     256, 512
 BEAM_MAX_W = 1024                                     # EB_BEAM_MAX_W
@@ -273,7 +273,11 @@ def encoder_phases(prog, engine, enc, S, n):
     LayerNorm of the input, then per layer n LSTM cell steps from the carried (h, c), the residual LayerNorm and the
     time reduction, then the projection.  Allocates on ``engine`` (whose ``dev`` is set) the chunk input ``xin``
     [S, n, F], the carried state ``enc_h`` / ``enc_c`` [L, S, H] (with ``enc_htmp``, the last step's h, copied into
-    enc_h by the caller's final phase) and the output ``enc_out`` [S, n_out, E]; sets ``engine.n_out``."""
+    enc_h by the caller's final phase) and the output ``enc_out`` [S, n_out, E]; sets ``engine.n_out``.
+    A GRU encoder (ResLayerNormGRU) gets GRU cell steps instead, and its carried state is ``enc_h`` alone (``enc_c``
+    is None); its programs run through eb_decode_run_ctc_stream."""
+    from .rnnt.models import ResLayerNormGRU
+    gru = isinstance(enc.lstm, ResLayerNormGRU)
     lstms = list(enc.lstm.lstms)
     L = len(lstms)
     H = enc.lstm.hidden_size
@@ -281,7 +285,7 @@ def encoder_phases(prog, engine, enc, S, n):
     reductions = enc.lstm.time_reductions
     z = lambda *shape: torch.zeros(*shape, dtype=torch.float32, device=engine.dev)
     engine.xin, engine.a0 = z(S, n, F), z(S, n, F)
-    engine.enc_h, engine.enc_c, engine.enc_htmp = z(L, S, H), z(L, S, H), z(L, S, H)
+    engine.enc_h, engine.enc_c, engine.enc_htmp = z(L, S, H), None if gru else z(L, S, H), z(L, S, H)
 
     def ph(**kw):
         p = EbPhase()
@@ -297,10 +301,10 @@ def encoder_phases(prog, engine, enc, S, n):
         yL, zL = z(S, ni, H), z(S, ni, H)
         engine._bufs += [yL, zL]
         for t in range(ni):
-            ph(type=PH_LSTM, S=S, N=H, K1=I, K2=H, x1=_ptr(X, t * I), ldx1=ni * I,
+            ph(type=PH_GRU if gru else PH_LSTM, S=S, N=H, K1=I, K2=H, x1=_ptr(X, t * I), ldx1=ni * I,
                x2=_ptr(engine.enc_h[i]) if t == 0 else _ptr(yL, (t - 1) * H), ldx2=H if t == 0 else ni * H,
                w1=_ptr(cell.weight_ih_l0), ldw1=I, w2=_ptr(cell.weight_hh_l0), ldw2=H,
-               b1=_ptr(cell.bias_ih_l0), b2=_ptr(cell.bias_hh_l0), c=_ptr(engine.enc_c[i]),
+               b1=_ptr(cell.bias_ih_l0), b2=_ptr(cell.bias_hh_l0), c=None if gru else _ptr(engine.enc_c[i]),
                y=_ptr(yL, t * H), ldy=ni * H, y2=_ptr(engine.enc_htmp[i]) if t == ni - 1 else None)
         ln = post[0]
         ph(type=PH_LN, S=S * ni, N=H, x1=_ptr(yL), ldx1=H, x2=_ptr(X) if i > 0 else None, ldx2=H,
@@ -1015,3 +1019,111 @@ class CTCBeamEngine:
         rows = self.seqs[n & 1, b * self.W:b * self.W + live].cpu()
         return [(tuple(int(x) for x in rows[j, 5:5 + int(rows[j, 0])]), float(st[0, j]), float(st[1, j]),
                  float(st[2, j])) for j in range(live)]
+
+
+class CTCStreamEngine:
+    """Streaming greedy CTC decoding of a ``CTCEncoder`` (rnnt/models.py:272-310): S streams, one persistent kernel
+    launch per chunk (eb_decode_run_ctc_stream).  The chunk program is encoder_phases' GRU encoder (LayerNorm, per layer
+    n GRU cell steps from the carried h, residual LayerNorm, time reduction), the projection, the ``tovocab`` Linear
+    over the chunk's n_out output frames, and CTC_EMIT.
+
+    Per stream the emitted ids are those of ``CTCEncoder.greedy_decode`` on the concatenated chunks (every layer is a
+    unidirectional GRU, LayerNorm works per frame and the time reduction pairs frames inside a chunk of even length, so
+    streaming the chunks with h carried gives the offline log-probs): per frame the argmax of the log-probs (NaN first,
+    ties to the lowest id), a frame equal to the previous frame's argmax dropped, including across a chunk boundary, and
+    blanks dropped.  ``score()`` keeps greedy_decode's quirk: the sum of the WHOLE log-prob rows of the kept frames.
+    The matrix products are fp32-accurate (3xTF32) whatever the model's precision setting.
+
+    The carried state is ``enc_h`` [L, S, H], the previous frame's argmax ``prev`` [S] (-1 after ``reset``: it matches
+    no token) and the running score ``score`` (fp64 on the device).  ``state()`` / ``load_state()`` move it to an engine
+    rebuilt for another chunk length or for re-homed weights (``fingerprint``)."""
+    def __init__(self, ctc_model, n_streams, frames_per_chunk, blank=0, max_ctas=0, state=None):
+        from .rnnt.models import CTCEncoder
+        if not isinstance(ctc_model, CTCEncoder):
+            raise TypeError("CTCStreamEngine streams a CTCEncoder, got %s" % type(ctc_model).__name__)
+        S, n, blank = operator.index(n_streams), operator.index(frames_per_chunk), operator.index(blank)
+        if S < 1 or n < 1:
+            raise ValueError("n_streams and frames_per_chunk must be positive, got %d and %d" % (S, n))
+        enc, lin = ctc_model.model, ctc_model.tovocab[0]
+        V = lin.weight.shape[0]
+        if not 0 <= blank < V:
+            raise ValueError("blank must lie in [0, %d), got %d" % (V, blank))
+        T = stream_frames_out(enc, n)
+        if T < 1:
+            raise ValueError("a chunk of %d frames gives no encoder output frame" % n)
+        self.dev = lin.weight.device
+        if self.dev.type != "cuda":
+            raise RuntimeError("CTCStreamEngine needs the model on a CUDA device")
+        assert C.sizeof(EbPhase) == lib().eb_decode_phase_size(), "EbPhase layout mismatch"
+        i32 = torch.int32
+        self.S, self.n, self.V, self.blank, self.max_ctas = S, n, V, blank, max_ctas
+        self._keep = [p.detach() for p in ctc_model.parameters()]       # weights are read in place
+        self.fingerprint = param_fingerprint(ctc_model)
+        prog = []
+        E = encoder_phases(prog, self, enc, S, n)
+        assert self.n_out == T and lin.weight.shape[1] == E
+        L, H = self.enc_h.shape[0], self.enc_h.shape[2]
+        z = lambda *shape, dtype=torch.float32: torch.zeros(*shape, dtype=dtype, device=self.dev)
+        self.logits, self.logprobs = z(S * T, V), z(S * T, V)
+        self.argmax = z(S, T, dtype=i32)                        # every frame's argmax (CTC_EMIT's seq_out)
+        self.prev, self._score = z(S, dtype=i32), z(S, dtype=torch.float64)
+        self._out = z(S * T + S, dtype=i32)                    # emitted ids [S, n_out] | counts [S]
+        self._host = torch.zeros(self._out.shape, dtype=i32).pin_memory()
+        prog.append(EbPhase(type=PH_LINEAR, S=S * T, N=V, K1=E, x1=_ptr(self.enc_out), ldx1=E, w1=_ptr(lin.weight),
+                            ldw1=E, b1=_ptr(lin.bias), y=_ptr(self.logits), ldy=V))
+        prog.append(EbPhase(type=PH_CTC_EMIT, S=S, N=V, aux=T, aux2=blank, x1=_ptr(self.logits), ldx1=V,
+                            y=_ptr(self.logprobs), ldy=V, tok_out=_ptr(self.prev), hist=_ptr(self._out), hist_ld=T,
+                            tok_out2=_ptr(self._out, S * T), y2=_ptr(self._score), seq_out=_ptr(self.argmax)))
+        prog.append(EbPhase(type=PH_COPY, S=L * S, N=H, x1=_ptr(self.enc_htmp), y=_ptr(self.enc_h)))
+        self.n_chunk_phases = len(prog)
+        self._chunk = _upload(prog, self.dev)
+        self._bar = torch.zeros(64, dtype=i32, device=self.dev)
+        if state is None:
+            self.reset()
+        else:
+            self.load_state(state)
+
+    def _state_views(self):
+        return dict(enc_h=self.enc_h, prev=self.prev, score=self._score)
+
+    def state(self):
+        """Every stream's carried state (encoder h, previous argmax, running score) as a dict of device tensors."""
+        return {k: t.clone() for k, t in self._state_views().items()}
+
+    @torch.no_grad()
+    def load_state(self, st):
+        """Continue from ``state()`` of an engine over the same model and n_streams, with any chunk length."""
+        views = self._state_views()
+        if set(st) != set(views):
+            raise ValueError("state keys %s do not match this engine's %s" % (sorted(st), sorted(views)))
+        for k, t in views.items():
+            if tuple(st[k].shape) != tuple(t.shape):
+                raise ValueError("state %s has shape %s, this engine needs %s (same model and n_streams)"
+                                 % (k, tuple(st[k].shape), tuple(t.shape)))
+            t.copy_(st[k])
+
+    @torch.no_grad()
+    def reset(self):
+        """Every stream starts a new utterance: zero encoder state, no previous frame, score 0."""
+        self.enc_h.zero_()
+        self.prev.fill_(-1)
+        self._score.zero_()
+
+    def score(self):
+        """The running score of every stream [S] (fp64, on the device): the sum of the whole log-prob rows of every
+        frame kept since ``reset``, what ``CTCEncoder.greedy_decode`` returns negated."""
+        return self._score
+
+    @torch.no_grad()
+    def step(self, chunk):
+        """chunk [S, n, F] log-mel frames (device or pinned host) -> (ids int32 [S, n_out], counts int32 [S]) on the
+        host: row s holds in its first counts[s] entries the ids stream s emitted in this chunk.  One device-to-host
+        copy per chunk."""
+        self.xin.copy_(chunk, non_blocking=True)
+        check(lib().eb_decode_run_ctc_stream(self._chunk.data_ptr(), self.n_chunk_phases, self._bar.data_ptr(),
+                                             self.max_ctas, torch.cuda.current_stream().cuda_stream),
+              "eb_decode_run_ctc_stream")
+        self._host.copy_(self._out, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        S, T = self.S, self.n_out
+        return self._host[:S * T].view(S, T).clone(), self._host[S * T:].clone()

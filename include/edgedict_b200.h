@@ -247,7 +247,7 @@ int eb_joint_dpre_reduce(const void* dpre16, float* dep, float* ddp, int B, int 
  * phase program once (edgedict_b200/stream_engine.py) and launches it per chunk; see decode.cu. */
 enum { EB_PH_LN = 0, EB_PH_PAIR = 1, EB_PH_LSTM = 2, EB_PH_LINEAR = 3, EB_PH_ARGMAX = 4, EB_PH_COPY = 5,
        EB_PH_BEAM_SELECT = 6, EB_PH_GATHER = 7, EB_PH_BEAM_FINAL = 8, EB_PH_BEAM_COMMIT = 9, EB_PH_SKIP = 10,
-       EB_PH_CTC_BEAM = 11 };
+       EB_PH_CTC_BEAM = 11, EB_PH_GRU = 12, EB_PH_CTC_EMIT = 13 };
 typedef struct EbPhase {
     int32_t type, S, K1, K2, N, flags, ldx1, ldx2, ldw1, ldw2, ldy, aux, aux2, hist_ld, hist_col, x1_div;
     const float *x1, *x2, *w1, *w2, *b1, *b2;
@@ -303,6 +303,18 @@ int eb_decode_run(const void* phases_dev, int nphase, void* barrier_dev, int max
 /* eb_decode_run with CTC_BEAM phases: the same kernel in an instantiation that also runs CTC_BEAM (eb_decode_run skips
  * them: the extra phase costs the matrix phases register spills, which the other programs do not pay). */
 int eb_decode_run_ctc(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream);
+/* Streaming CTC (stream_engine.CTCStreamEngine, see decode.cu for the field use):
+ * GRU       one nn.GRU cell step for S rows (gate order r|z|n): w1 = W_ih [3N, K1], w2 = W_hh [3N, K2], b1 = b_ih,
+ *           b2 = b_hh, h from x2; y (ldy) = h', y2 (optional, [S, N]) a copy.  No flags.
+ * CTC_EMIT  greedy CTC emission of a chunk, one warp per stream: S streams of aux frames (logits x1 row s*aux + t), V = N,
+ *           blank = aux2; per frame the log-probs y = (x - max) - log(sum exp(x - max)), their argmax in torch.argmax
+ *           order (NaN first, ties to the lowest id); a frame equal to the previous frame's argmax (tok_out [S], carried
+ *           across launches; negative after a reset) or to blank is dropped; the kept ids go to hist [S, hist_ld] with
+ *           their count in tok_out2 [S]; y2, a DOUBLE [S], accumulates the whole-row log-prob sum of every kept frame;
+ *           seq_out (optional) [S, aux] receives every frame's argmax.
+ * eb_decode_run and eb_decode_run_ctc skip both; programs with them run through eb_decode_run_ctc_stream, the kernel
+ * in a third instantiation (the two others keep their code and registers), which skips LSTM and CTC_BEAM. */
+int eb_decode_run_ctc_stream(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream);
 
 /* ---- reductions, casts, optimizer -------------------------------------------------------- */
 int eb_colsum(const void* x, int x_bf16, float* out_accum, long rows, int N, void* stream);
