@@ -1323,7 +1323,9 @@ static_assert(sizeof(EbPhase) % 4 == 0 && sizeof(EbPhase) / 4 <= 256, "EbPhase l
 // A third, CTC_STREAM = true (eb_decode_run_ctc_stream), adds GRU and CTC_EMIT, the phases of a streaming CTC chunk, and
 // skips LSTM (with it, 28 / 52 bytes of spills instead of 16 / 28); the other two skip GRU and CTC_EMIT like any unknown
 // type, so their code and registers are what they were without these phases.
-template <bool CTC, bool CTC_STREAM>
+// A fourth, GRU_RNNT = true (eb_decode_run_gru_rnnt), is the default one plus GRU: the phases of a streaming GRU
+// transducer chunk (GRU encoder, LSTM predictor and LM, greedy and beam frames).  It skips CTC_BEAM and CTC_EMIT.
+template <bool CTC, bool CTC_STREAM, bool GRU_RNNT>
 __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __restrict__ prog, int nphase, unsigned* bar) {
     extern __shared__ __align__(16) float dsm[];
     float* red = dsm;                                        // [8 warps][2048]
@@ -1377,6 +1379,8 @@ __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __re
                 if constexpr (CTC_STREAM) {
                     if (ph.type == EB_PH_GRU) phase_gru(ph, red, outs);
                     else if (ph.type == EB_PH_CTC_EMIT) phase_ctc_emit(ph);
+                } else if constexpr (GRU_RNNT) {
+                    if (ph.type == EB_PH_GRU) phase_gru(ph, red, outs);
                 }
                 break;
         }
@@ -1390,7 +1394,7 @@ __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __re
 
 }  // namespace
 
-template <bool CTC, bool CTC_STREAM>
+template <bool CTC, bool CTC_STREAM, bool GRU_RNNT>
 int decode_run(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream) {
     if (!phases_dev || nphase <= 0 || !barrier_dev) return EB_ERR_INVALID;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -1401,23 +1405,27 @@ int decode_run(const void* phases_dev, int nphase, void* barrier_dev, int max_ct
     unsigned* bar = reinterpret_cast<unsigned*>(barrier_dev);
     void* args[] = {(void*)&prog, (void*)&nphase, (void*)&bar};
     const size_t smem = sizeof(float) * (RED_FLOATS + TR * OUT_LD);
-    EB_CUDA(cudaFuncSetAttribute(decode_program_kernel<CTC, CTC_STREAM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    EB_CUDA(cudaFuncSetAttribute(decode_program_kernel<CTC, CTC_STREAM, GRU_RNNT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)smem));
-    EB_CUDA(cudaLaunchCooperativeKernel((void*)decode_program_kernel<CTC, CTC_STREAM>, dim3(grid), dim3(256), args, smem,
+    EB_CUDA(cudaLaunchCooperativeKernel((void*)decode_program_kernel<CTC, CTC_STREAM, GRU_RNNT>, dim3(grid), dim3(256), args, smem,
                                         st));
     return EB_OK;
 }
 
 EB_API int eb_decode_run(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream) {
-    return decode_run<false, false>(phases_dev, nphase, barrier_dev, max_ctas, stream);
+    return decode_run<false, false, false>(phases_dev, nphase, barrier_dev, max_ctas, stream);
 }
 
 EB_API int eb_decode_run_ctc(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream) {
-    return decode_run<true, false>(phases_dev, nphase, barrier_dev, max_ctas, stream);
+    return decode_run<true, false, false>(phases_dev, nphase, barrier_dev, max_ctas, stream);
 }
 
 EB_API int eb_decode_run_ctc_stream(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream) {
-    return decode_run<false, true>(phases_dev, nphase, barrier_dev, max_ctas, stream);
+    return decode_run<false, true, false>(phases_dev, nphase, barrier_dev, max_ctas, stream);
+}
+
+EB_API int eb_decode_run_gru_rnnt(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream) {
+    return decode_run<false, false, true>(phases_dev, nphase, barrier_dev, max_ctas, stream);
 }
 
 EB_API int eb_decode_phase_size(void) { return (int)sizeof(EbPhase); }

@@ -17,10 +17,10 @@ import time
 
 import torch
 
-from .models import Transducer, convert_lightning2normal
+from .models import ResLayerNormGRU, Transducer, convert_lightning2normal
 from .tokenizer import NUL, BOS, UNK
-from ..stream_engine import BEAM_MAX_W, StreamBeamEngine, StreamEngine, check_lm_args, check_max_symbols, \
-    param_fingerprint
+from ..stream_engine import BEAM_MAX_W, GRUStreamBeamEngine, GRUStreamEngine, StreamBeamEngine, StreamEngine, \
+    check_lm_args, check_max_symbols, param_fingerprint
 
 
 class StreamTransducerDecoder:
@@ -48,7 +48,13 @@ class PytorchStreamDecoder(StreamTransducerDecoder):
     ``<unk>`` rule, which belongs to greedy argmax decoding; Transducer.beam_search does not apply it either.
 
     ``max_symbols`` = K (1 to 16, greedy decoding only) lets each encoder frame emit up to K symbols: the frame repeats
-    joint -> argmax (with the ``<unk>`` rule) -> predictor step until a blank or K non-blank tokens."""
+    joint -> argmax (with the ``<unk>`` rule) -> predictor step until a blank or K non-blank tokens.
+
+    A transducer with a GRU encoder (``Transducer(module_type='GRU')``; from FLAGS, ``enc_type='GRU'`` as
+    cli/lightning.py --enc_type GRU trains it) streams through stream_engine.GRUStreamEngine / GRUStreamBeamEngine,
+    greedily or by beam search, with the same ``decode`` / ``flush`` / ``max_symbols`` / beam and LM arguments.  The
+    reference cannot stream such a model (its decode hands an LSTM's (h, c) to the GRU stack): this is an addition, not
+    a mirror of rnnt/stream.py."""
 
     def __init__(self, FLAGS, transducer=None, transform=None, tokenizer=None, device="cuda",
                  frames_per_chunk=None, input_size=None, *, beam_width=None, merge=True, lm=None, lm_weight=0.0,
@@ -85,7 +91,8 @@ class PytorchStreamDecoder(StreamTransducerDecoder):
                 input_size=input_size, enc_hidden_size=FLAGS.enc_hidden_size, enc_layers=FLAGS.enc_layers,
                 enc_dropout=FLAGS.enc_dropout, enc_proj_size=FLAGS.enc_proj_size,
                 dec_hidden_size=FLAGS.dec_hidden_size, dec_layers=FLAGS.dec_layers, dec_dropout=FLAGS.dec_dropout,
-                dec_proj_size=FLAGS.dec_proj_size, joint_size=FLAGS.joint_size, output_loss=False)
+                dec_proj_size=FLAGS.dec_proj_size, joint_size=FLAGS.joint_size,
+                module_type=getattr(FLAGS, "enc_type", "LSTM"), output_loss=False)
             transducer.load_state_dict(convert_lightning2normal(checkpoint)['model'])
         transducer.eval()
         transducer.to(self.device)
@@ -118,11 +125,14 @@ class PytorchStreamDecoder(StreamTransducerDecoder):
         # program, NOT a new utterance: the recurrent state moves over (rnnt/stream.py:94-120 carries it across
         # arbitrary chunk lengths); only reset() starts from the primed zero state
         st = self._engine.state() if self._engine is not None else None
+        gru = isinstance(self.encoder.lstm, ResLayerNormGRU)
         if self._beam is None:
-            self._engine = StreamEngine(self._transducer, 1, n, unk_id=self._unk, blank=NUL, state=st,
-                                        max_symbols=self._max_symbols)
+            self._engine = (GRUStreamEngine if gru else StreamEngine)(self._transducer, 1, n, unk_id=self._unk,
+                                                                      blank=NUL, state=st,
+                                                                      max_symbols=self._max_symbols)
         else:
-            self._engine = StreamBeamEngine(self._transducer, 1, n, blank=NUL, state=st, **self._beam)
+            self._engine = (GRUStreamBeamEngine if gru else StreamBeamEngine)(self._transducer, 1, n, blank=NUL,
+                                                                              state=st, **self._beam)
         self._frames = n
 
     @torch.no_grad()

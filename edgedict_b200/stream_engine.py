@@ -252,6 +252,13 @@ def _check_lstm_encoder(enc, who):
         raise ValueError("%s streams an LSTM encoder only, got %s" % (who, type(enc.lstm).__name__))
 
 
+def _check_gru_encoder(enc, who):
+    from .rnnt.models import ResLayerNormGRU
+    if not isinstance(enc.lstm, ResLayerNormGRU):
+        # the GRU engines' encoder programs are GRU cells (3H-row weights)
+        raise ValueError("%s streams a GRU encoder only, got %s" % (who, type(enc.lstm).__name__))
+
+
 def _odd_chunk():
     return ValueError("streaming chunks must hold an even number of frames before each time reduction "
                       "(cli/export_onnx.py:20-21 asserts the same)")
@@ -268,6 +275,18 @@ def stream_frames_out(enc, n):
     return n
 
 
+def check_stream_shape(enc, n_streams, frames_per_chunk):
+    """(S, n, encoder output frames per chunk) of a streaming engine; ValueError for S < 1, n < 1, an odd count before
+    a time reduction or a chunk that gives no output frame.  Touches no device."""
+    S, n = operator.index(n_streams), operator.index(frames_per_chunk)
+    if S < 1 or n < 1:
+        raise ValueError("n_streams and frames_per_chunk must be positive, got %d and %d" % (S, n))
+    T = stream_frames_out(enc, n)
+    if T < 1:
+        raise ValueError("a chunk of %d frames gives no encoder output frame" % n)
+    return S, n, T
+
+
 def encoder_phases(prog, engine, enc, S, n):
     """Append the stateful streaming encoder for S streams and chunks of n log-mel frames to the phase list ``prog``:
     LayerNorm of the input, then per layer n LSTM cell steps from the carried (h, c), the residual LayerNorm and the
@@ -275,7 +294,7 @@ def encoder_phases(prog, engine, enc, S, n):
     [S, n, F], the carried state ``enc_h`` / ``enc_c`` [L, S, H] (with ``enc_htmp``, the last step's h, copied into
     enc_h by the caller's final phase) and the output ``enc_out`` [S, n_out, E]; sets ``engine.n_out``.
     A GRU encoder (ResLayerNormGRU) gets GRU cell steps instead, and its carried state is ``enc_h`` alone (``enc_c``
-    is None); its programs run through eb_decode_run_ctc_stream."""
+    is None); its programs run through eb_decode_run_ctc_stream (CTC) or eb_decode_run_gru_rnnt (transducer)."""
     from .rnnt.models import ResLayerNormGRU
     gru = isinstance(enc.lstm, ResLayerNormGRU)
     lstms = list(enc.lstm.lstms)
@@ -335,6 +354,10 @@ def _upload(prog, dev):
 
 class StreamEngine:
     STATE = ("enc_h", "enc_c", "dec_h", "dec_c", "dec_x", "tok")
+    RUN = "eb_decode_run"                     # the decode kernel entry every program of the engine runs through
+
+    def _check_encoder(self, enc, n_streams, frames_per_chunk):
+        _check_lstm_encoder(enc, "StreamEngine")
 
     def __init__(self, transducer, n_streams, frames_per_chunk, unk_id=UNK, blank=NUL, max_ctas=0, state=None,
                  max_symbols=1):
@@ -344,10 +367,10 @@ class StreamEngine:
         K = check_max_symbols(max_symbols)
         assert C.sizeof(EbPhase) == lib().eb_decode_phase_size(), "EbPhase layout mismatch"
         enc, dec, joint = transducer.encoder, transducer.decoder, transducer.joint.joint
-        _check_lstm_encoder(enc, "StreamEngine")
+        self._check_encoder(enc, n_streams, frames_per_chunk)
         self.dev = enc.norm.weight.device
         if self.dev.type != "cuda":
-            raise RuntimeError("StreamEngine needs the model on a CUDA device")
+            raise RuntimeError("%s needs the model on a CUDA device" % type(self).__name__)
         f32 = torch.float32
         S, n = n_streams, frames_per_chunk
         self.S, self.n, self.blank, self.unk, self.max_ctas, self.max_symbols = S, n, blank, unk_id, max_ctas, K
@@ -411,6 +434,9 @@ class StreamEngine:
 
     @torch.no_grad()
     def load_state(self, st):
+        if set(st) != set(self.STATE):
+            raise ValueError("state keys %s do not match this engine's %s (an LSTM encoder carries enc_h and enc_c, a "
+                             "GRU encoder enc_h alone)" % (sorted(st), sorted(self.STATE)))
         for k in self.STATE:
             getattr(self, k).copy_(st[k])
 
@@ -421,14 +447,15 @@ class StreamEngine:
         return t
 
     def _run(self, prog, nphase):
-        check(lib().eb_decode_run(prog.data_ptr(), nphase, self._bar.data_ptr(), self.max_ctas,
-                                  torch.cuda.current_stream().cuda_stream), "eb_decode_run")
+        check(getattr(lib(), self.RUN)(prog.data_ptr(), nphase, self._bar.data_ptr(), self.max_ctas,
+                                       torch.cuda.current_stream().cuda_stream), self.RUN)
 
     @torch.no_grad()
     def reset(self):
         """PytorchStreamDecoder.reset (rnnt/stream.py:78-91) for every stream."""
         for t in (self.enc_h, self.enc_c, self.dec_h, self.dec_c):
-            t.zero_()
+            if t is not None:
+                t.zero_()
         self.tok.fill_(BOS)
         self._run(self._prime, self.n_prime_phases)
 
@@ -664,6 +691,10 @@ class StreamBeamEngine:
 
     The reference's ``<unk>`` rule (re-argmax when the argmax is ``<unk>``) is a device of the greedy loop; the beam,
     like Transducer.beam_search, does not apply it."""
+    RUN = "eb_decode_run"                     # the decode kernel entry every program of the engine runs through
+
+    def _check_encoder(self, enc):
+        _check_lstm_encoder(enc, "StreamBeamEngine")
 
     def __init__(self, transducer, n_streams, frames_per_chunk, W, merge=True, lm=None, lm_weight=0.0,
                  length_bonus=0.0, lm_bos=1, lm_token_map=None, max_pending=64, state=None, blank=NUL, max_ctas=0,
@@ -675,20 +706,16 @@ class StreamBeamEngine:
         V = transducer.joint.joint[2].weight.shape[0]
         fusion = check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map)
         enc, dec, joint = transducer.encoder, transducer.decoder, transducer.joint.joint
-        _check_lstm_encoder(enc, "StreamBeamEngine")
-        S, n, P = operator.index(n_streams), operator.index(frames_per_chunk), operator.index(max_pending)
-        if S < 1 or n < 1:
-            raise ValueError("n_streams and frames_per_chunk must be positive, got %d and %d" % (S, n))
-        T = stream_frames_out(enc, n)
-        if T < 1:
-            raise ValueError("a chunk of %d frames gives no encoder output frame" % n)
+        self._check_encoder(enc)
+        P = operator.index(max_pending)
+        S, n, T = check_stream_shape(enc, n_streams, frames_per_chunk)
         if P < T * K:
             raise ValueError("max_pending (%d) must be at least the encoder frames per chunk times max_symbols (%d x %d):"
                              " a chunk can add that many tokens to a hypothesis" % (P, T, K))
         assert C.sizeof(EbPhase) == lib().eb_decode_phase_size(), "EbPhase layout mismatch"
         self.dev = enc.norm.weight.device
         if self.dev.type != "cuda":
-            raise RuntimeError("StreamBeamEngine needs the model on a CUDA device")
+            raise RuntimeError("%s needs the model on a CUDA device" % type(self).__name__)
         f32, i32 = torch.float32, torch.int32
         R, LS, TK = S * W, P + 3, T * K
         self.S, self.n, self.W, self.R, self.merge, self.blank, self.max_ctas, self.max_pending, self.max_symbols = \
@@ -793,6 +820,8 @@ class StreamBeamEngine:
     def _state_views(self):
         v = dict(enc_h=self.enc_h, enc_c=self.enc_c, dec_state=self._st[0], dec_x=self.dec_x[0], logp=self.logp,
                  seqs=self.seqs[0], live=self.hist_live[:, -1])
+        if self.enc_c is None:                               # a GRU encoder carries h alone
+            del v["enc_c"]
         if self.lm:
             v.update(lm_state=self._lst[0], lm_logits=self.lm_logits)
         return v
@@ -847,8 +876,8 @@ class StreamBeamEngine:
         return ids, counts
 
     def _run(self, prog, nphase):
-        check(lib().eb_decode_run(prog.data_ptr(), nphase, self._bar.data_ptr(), self.max_ctas,
-                                  torch.cuda.current_stream().cuda_stream), "eb_decode_run")
+        check(getattr(lib(), self.RUN)(prog.data_ptr(), nphase, self._bar.data_ptr(), self.max_ctas,
+                                       torch.cuda.current_stream().cuda_stream), self.RUN)
 
     def _fetch(self):
         S, P = self.S, self.max_pending
@@ -862,7 +891,8 @@ class StreamBeamEngine:
         """Every stream starts a new utterance: zero encoder state, one live slot of log p 0 with the empty sequence,
         predictor primed with <bos> and the LM with lm_bos from zeros."""
         for t in (self.enc_h, self.enc_c, self._st[0], self.seqs[0]):
-            t.zero_()
+            if t is not None:
+                t.zero_()
         self.logp.fill_(float("-inf"))
         self.logp.view(self.S, self.W)[:, 0] = 0.0
         self.hist_live[:, -1] = 1
@@ -894,6 +924,38 @@ class StreamBeamEngine:
         ids, counts, _ = self._fetch()
         ids, counts = self._take(ids, counts)
         return ids, counts, -self.logp.view(self.S, self.W)[:, 0].cpu()
+
+
+class GRUStreamEngine(StreamEngine):
+    """StreamEngine for a transducer with a GRU encoder (``Transducer(module_type='GRU')``, ResLayerNormGRU): the same
+    arguments, ``step`` / ``reset`` / ``state`` / ``load_state`` / ``fingerprint`` / ``n_out`` and ``max_symbols``
+    rounds with the ``<unk>`` rule.  The chunk program is encoder_phases' GRU encoder (per layer n GRU cell steps from
+    the carried h) followed by StreamEngine's frames; the predictor stays an LSTM.  Every program runs through
+    eb_decode_run_gru_rnnt, the decode kernel's instantiation with both cell phases.  The carried encoder state is
+    ``enc_h`` alone: the state of an LSTM-encoder engine does not load here, nor this one's there.
+
+    Per stream the ids are those of Transducer.greedy_decode (with the <unk> rule) on the concatenated chunks: every
+    layer is a unidirectional GRU and the time reduction pairs frames inside a chunk of even length, so the chunks with
+    h carried give the offline encoder output.  The matrix products are fp32-accurate (3xTF32)."""
+    STATE = ("enc_h", "dec_h", "dec_c", "dec_x", "tok")
+    RUN = "eb_decode_run_gru_rnnt"
+
+    def _check_encoder(self, enc, n_streams, frames_per_chunk):
+        _check_gru_encoder(enc, "GRUStreamEngine")
+        check_stream_shape(enc, n_streams, frames_per_chunk)
+
+
+class GRUStreamBeamEngine(StreamBeamEngine):
+    """StreamBeamEngine for a transducer with a GRU encoder: the same signature and contract (W, merge, the LM fusion
+    arguments, max_pending and the forced collapse, max_symbols, ``step`` / ``flush`` / ``reset`` / ``state`` /
+    ``load_state`` with the re-bound).  The chunk program is encoder_phases' GRU encoder followed by StreamBeamEngine's
+    beam frames and chunk end; every program (chunk, prime, flush, re-bound) runs through eb_decode_run_gru_rnnt.  The
+    state carries ``enc_h`` and no ``enc_c``, so the state of an LSTM-encoder engine does not load here, nor this one's
+    there."""
+    RUN = "eb_decode_run_gru_rnnt"
+
+    def _check_encoder(self, enc):
+        _check_gru_encoder(enc, "GRUStreamBeamEngine")
 
 
 def lm_cache_key(fusion):

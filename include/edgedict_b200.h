@@ -315,6 +315,10 @@ int eb_decode_run_ctc(const void* phases_dev, int nphase, void* barrier_dev, int
  * eb_decode_run and eb_decode_run_ctc skip both; programs with them run through eb_decode_run_ctc_stream, the kernel
  * in a third instantiation (the two others keep their code and registers), which skips LSTM and CTC_BEAM. */
 int eb_decode_run_ctc_stream(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream);
+/* Streaming GRU transducer (stream_engine.GRUStreamEngine / GRUStreamBeamEngine): the kernel in a fourth instantiation,
+ * eb_decode_run's plus GRU, so one program holds a GRU encoder, an LSTM predictor and LM, and the greedy and beam frame
+ * phases.  It skips CTC_BEAM and CTC_EMIT; the three other instantiations keep their code and registers. */
+int eb_decode_run_gru_rnnt(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream);
 
 /* ---- reductions, casts, optimizer -------------------------------------------------------- */
 int eb_colsum(const void* x, int x_bf16, float* out_accum, long rows, int N, void* stream);
