@@ -10,6 +10,7 @@ encoder frame, argmax over raw logits, predictor advanced only on non-blank.  Wi
 repeats joint -> argmax -> predictor step until a blank or K symbols (GreedyEngine likewise).
 """
 import ctypes as C
+import functools
 import math
 import numbers
 import operator
@@ -95,12 +96,41 @@ def greedy_frame(prog, K, S, tok, blank, round_phases):
         prog[i].aux = len(prog) - i - 1
 
 
-def beam_state(e, R, Ld, Hd, D, LS, Ll=0, Hl=0):
+def joint_phases(prog, joint, S, x_enc, ldx_enc, dec_x, hidden, logits, x1_div=0):
+    """Append the joint for S rows: hidden [S, J] = tanh(W1 [encoder frame | dec_x] + b1), then logits [S, V] =
+    W2 hidden + b2, ``joint`` being (W1, b1, W2, b2).  The encoder frame of row r is at x_enc, row stride ldx_enc; with
+    x1_div = W the W rows of a beam's utterance share row r // W."""
+    w1, b1, w2, b2 = joint
+    J, V, D = w1.shape[0], w2.shape[0], dec_x.shape[1]
+    E = w1.shape[1] - D
+    prog.append(EbPhase(type=PH_LINEAR, S=S, N=J, flags=F_TANH, K1=E, x1=x_enc, ldx1=ldx_enc, x1_div=x1_div,
+                        w1=_ptr(w1), ldw1=E + D, K2=D, x2=_ptr(dec_x), ldx2=D, w2=_ptr(w1, E), ldw2=E + D, b1=_ptr(b1),
+                        y=_ptr(hidden), ldy=J))
+    prog.append(EbPhase(type=PH_LINEAR, S=S, N=V, K1=J, x1=_ptr(hidden), ldx1=J, w1=_ptr(w2), ldw1=J, b1=_ptr(b2),
+                        y=_ptr(logits), ldy=V))
+
+
+def greedy_round(prog, e, dec, h_enc, k, j, flags, unk, logp=None):
+    """Append round j of encoder frame k of greedy decoding on engine ``e`` (GreedyEngine, StreamEngine): the joint of
+    frame k of h_enc [rows, T', E] with the predictor output e.dec_x, an ARGMAX of the logits into e.tok and history
+    column k * K + j (``flags``, F_CONT added for j >= 1; ``unk`` the token re-argmaxed when it wins, -1 for none; the
+    log p of every row added into ``logp`` with F_LOGP), then the predictor step masked on blank."""
+    S, T, E = h_enc.shape
+    V = e.logits.shape[1]
+    joint_phases(prog, e._joint, S, _ptr(h_enc, k * E), T * E, e.dec_x, e.hidden, e.logits)
+    prog.append(EbPhase(type=PH_ARGMAX, S=S, N=V, flags=flags | (F_CONT if j else 0), x1=_ptr(e.logits), ldx1=V,
+                        aux=e.blank, aux2=unk, tok_out=_ptr(e.tok), hist=_ptr(e.hist), hist_ld=e.hist.shape[1],
+                        hist_col=k * e.max_symbols + j, y=_ptr(logp)))
+    _dec_phases(prog, dec, S, e.dec_h, e.dec_c, e.dec_htmp, e.dec_x, e.tok, e.blank, masked=True)
+
+
+def beam_state(e, R, Ld, Hd, D, LS):
     """Allocate on engine ``e`` (its ``dev`` set) the per-slot state of a beam search over R rows, for each parity p
     in one flat buffer ``e._home[p]``: the predictor state e._st[p] [2 Ld, R, Hd] (h of every layer, then c; views
     e.dec_h[p] / e.dec_c[p]), its output e.dec_x[p] [R, D], the token sequences e.seqs[p] int32 [R, LS] and, with an LM
-    (Ll > 0), its state e._lst[p] [2 Ll, R, Hl] (e.lm_h[p] / e.lm_c[p]).  One COPY of e._home[1] into e._home[0] moves
-    all of it, which a round of a multi-symbol frame needs (beam_frame)."""
+    (``e.lm``, lm_fusion done), its state e._lst[p] [2 Ll, R, Hl] (e.lm_h[p] / e.lm_c[p]).  One COPY of e._home[1]
+    into e._home[0] moves all of it, which a round of a multi-symbol frame needs (beam_frame)."""
+    Ll, _, Hl = e.lm_htmp.shape if e.lm else (0, 0, 0)
     sizes = [2 * Ld * R * Hd, R * D, R * LS, 2 * Ll * R * Hl]
     offs = [0]
     for n in sizes:
@@ -117,28 +147,46 @@ def beam_state(e, R, Ld, Hd, D, LS, Ll=0, Hl=0):
         e.lm_h, e.lm_c = [s[:Ll] for s in e._lst], [s[Ll:] for s in e._lst]
 
 
-def beam_frame(prog, e, t, x_enc, ldx_enc, sel, step):
+def beam_history(e, B, T, W):
+    """Allocate on engine ``e`` the beam history of B utterances over T columns, which BEAM_SELECT / CTC_BEAM write
+    and BEAM_FINAL / BEAM_COMMIT read: one int32 buffer ``e.hist``, parent | token | log p | live, with the views
+    e.hist_parent / e.hist_token [B, T, W], e.hist_logp (fp32) [B, T, W] and e.hist_live [B, T]."""
+    n = B * T * W
+    e.hist = torch.zeros(3 * n + B * T, dtype=torch.int32, device=e.dev)
+    e.hist_parent, e.hist_token = e.hist[:n].view(B, T, W), e.hist[n:2 * n].view(B, T, W)
+    e.hist_logp = e.hist[2 * n:3 * n].view(torch.float32).view(B, T, W)
+    e.hist_live = e.hist[3 * n:].view(B, T)
+
+
+def beam_reset(e):
+    """Start a new utterance in every beam of engine ``e`` (BeamEngine, StreamBeamEngine): one live slot of log p 0
+    (the others -inf) with the empty sequence and the zero predictor state primed with <bos>, and with an LM the zero
+    LM state primed with lm_bos."""
+    e._st[0].zero_()
+    e.seqs[0].zero_()
+    e.logp.fill_(float("-inf"))
+    e.logp.view(-1, e.W)[:, 0] = 0.0
+    e.tok.fill_(BOS)
+    if e.lm:
+        e._lst[0].zero_()
+        e.lm_tok.fill_(e.lm_bos)
+
+
+def beam_frame(prog, e, dec, t, x_enc, ldx_enc, sel, lm_step):
     """Append encoder frame t of the beam search, the same for BeamEngine and StreamBeamEngine (engine ``e``): up to
     K = e.max_symbols rounds of joint hidden (the encoder frame at x_enc, row stride ldx_enc, shared by an utterance's W
     rows) and logits, BEAM_SELECT (``sel``: its fields common to every round), GATHER of the parents' predictor (and
-    LM) state, and ``step(h)``, which appends the masked predictor (and LM) steps on state buffer h.
+    LM) state, and the masked steps of the predictor ``dec`` and, with an LM, of the LM (``lm_step`` from lm_fusion).
 
     K = 1 is the one-symbol frame: the state alternates between the buffers by frame parity.  For K > 1 the number of
     rounds a frame runs is known only on the device (SKIP, greedy_frame), so the state ends every round in buffer 0:
     GATHER writes buffer 1 and one COPY moves it back."""
     K, R = e.max_symbols, e.R
-    w1, b1, w2, b2 = e._joint
-    J, V = w1.shape[0], w2.shape[0]
     D = e.dec_x[0].shape[1]
-    E = w1.shape[1] - D
 
     def round_phases(j):
         p, q = (t & 1, 1 - (t & 1)) if K == 1 else (0, 1)
-        prog.append(EbPhase(type=PH_LINEAR, S=R, N=J, flags=F_TANH, K1=E, x1=x_enc, ldx1=ldx_enc, x1_div=e.W,
-                            w1=_ptr(w1), ldw1=E + D, K2=D, x2=_ptr(e.dec_x[p]), ldx2=D, w2=_ptr(w1, E), ldw2=E + D,
-                            b1=_ptr(b1), y=_ptr(e.hidden), ldy=J))
-        prog.append(EbPhase(type=PH_LINEAR, S=R, N=V, K1=J, x1=_ptr(e.hidden), ldx1=J, w1=_ptr(w2), ldw1=J,
-                            b1=_ptr(b2), y=_ptr(e.logits), ldy=V))
+        joint_phases(prog, e._joint, R, x_enc, ldx_enc, e.dec_x[p], e.hidden, e.logits, x1_div=e.W)
         ph = EbPhase(hist_col=t * K + j, seq_in=_ptr(e.seqs[p]), seq_out=_ptr(e.seqs[q]), **sel)
         if K > 1:
             ph.flags |= F_ROUNDS
@@ -153,7 +201,9 @@ def beam_frame(prog, e, t, x_enc, ldx_enc, sel, step):
         if K > 1:
             prog.append(EbPhase(type=PH_COPY, S=1, N=e._home.shape[1], x1=_ptr(e._home[1]), y=_ptr(e._home[0])))
             q = 0
-        step(q)
+        _dec_phases(prog, dec, R, e.dec_h[q], e.dec_c[q], e.dec_htmp, e.dec_x[q], e.tok, e.blank, masked=True)
+        if lm_step is not None:
+            lm_step(prog, e.lm_h[q], e.lm_c[q], masked=True)
 
     greedy_frame(prog, K, R, e.tok, e.blank, round_phases)
 
@@ -239,24 +289,36 @@ def check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map):
     return sd, vals[0], vals[1], lm_bos, tmap
 
 
+def lm_fusion(e, fusion, R):
+    """Shallow fusion on beam engine ``e`` (its ``dev`` and ``_keep`` set) over R rows, from check_lm_args' result:
+    keeps the LM weights in e._keep (read in place when they already are fp32 on e.dev, so tied weights stay tied),
+    allocates the LM scratch e.lm_htmp [Ll, R, Hl], e.lm_logits [R, ntok] and e.lm_tok, the token map e.lm_map and
+    e.lm_fuse = (lm_weight, length_bonus), and sets e.lm_bos.  Returns the fields a BEAM_SELECT / CTC_BEAM phase reads
+    the LM through (besides flag F_LM) and ``step(prog, h, c, masked)``, which appends one LM step on state h, c
+    [Ll, R, Hl] (predictor_phases resting on -1)."""
+    lsd, lw, lb, e.lm_bos, tmap = fusion
+    lsd = {k: v.to(e.dev, torch.float32).contiguous() for k, v in lsd.items()}
+    e._keep += list(lsd.values())
+    Ll = (len(lsd) - 3) // 4
+    layers = [tuple(lsd["rnn.%s_l%d" % (n, k)] for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"))
+              for k in range(Ll)]
+    Hl, ntok = layers[0][1].shape[1], lsd["encoder.weight"].shape[0]
+    z = lambda *shape, dtype=torch.float32: torch.zeros(*shape, dtype=dtype, device=e.dev)
+    e.lm_htmp, e.lm_logits, e.lm_tok = z(Ll, R, Hl), z(R, ntok), z(R, dtype=torch.int32)
+    e.lm_map = tmap.to(e.dev, torch.int32)
+    e.lm_fuse = torch.tensor([lw, lb], dtype=torch.float32, device=e.dev)
+
+    def step(prog, h, c, masked):
+        predictor_phases(prog, lsd["encoder.weight"], layers, lsd["decoder.weight"], lsd["decoder.bias"], R, h, c,
+                         e.lm_htmp, e.lm_logits, e.lm_tok, -1, masked)
+    return dict(x2=_ptr(e.lm_logits), ldx2=ntok, K2=ntok, fuse=_ptr(e.lm_fuse), tok_map=_ptr(e.lm_map),
+                tok_out2=_ptr(e.lm_tok)), step
+
+
 def param_fingerprint(module):
     """Identity of the parameter storage a phase program was built over: the programs bake raw device pointers, so a
     re-homed parameter (FlatAdam bucket, .to(), .float(), p.data = ...) must trigger a rebuild."""
     return tuple(p.data_ptr() for p in module.parameters())
-
-
-def _check_lstm_encoder(enc, who):
-    from .rnnt.models import ResLayerNormLSTM
-    if not isinstance(enc.lstm, ResLayerNormLSTM):
-        # the decode program's encoder phases are LSTM cells (4H-row weights); a GRU stack has 3H rows
-        raise ValueError("%s streams an LSTM encoder only, got %s" % (who, type(enc.lstm).__name__))
-
-
-def _check_gru_encoder(enc, who):
-    from .rnnt.models import ResLayerNormGRU
-    if not isinstance(enc.lstm, ResLayerNormGRU):
-        # the GRU engines' encoder programs are GRU cells (3H-row weights)
-        raise ValueError("%s streams a GRU encoder only, got %s" % (who, type(enc.lstm).__name__))
 
 
 def _odd_chunk():
@@ -291,10 +353,11 @@ def encoder_phases(prog, engine, enc, S, n):
     """Append the stateful streaming encoder for S streams and chunks of n log-mel frames to the phase list ``prog``:
     LayerNorm of the input, then per layer n LSTM cell steps from the carried (h, c), the residual LayerNorm and the
     time reduction, then the projection.  Allocates on ``engine`` (whose ``dev`` is set) the chunk input ``xin``
-    [S, n, F], the carried state ``enc_h`` / ``enc_c`` [L, S, H] (with ``enc_htmp``, the last step's h, copied into
-    enc_h by the caller's final phase) and the output ``enc_out`` [S, n_out, E]; sets ``engine.n_out``.
-    A GRU encoder (ResLayerNormGRU) gets GRU cell steps instead, and its carried state is ``enc_h`` alone (``enc_c``
-    is None); its programs run through eb_decode_run_ctc_stream (CTC) or eb_decode_run_gru_rnnt (transducer)."""
+    [S, n, F], the carried state ``enc_h`` / ``enc_c`` [L, S, H] (with ``enc_htmp``, the last step's h, which the
+    chunk program's last phase copies into enc_h: _ChunkEngine._finish) and the output ``enc_out`` [S, n_out, E]; sets
+    ``engine.n_out``.  A GRU encoder (ResLayerNormGRU) gets GRU cell steps instead, and its carried state is ``enc_h``
+    alone (``enc_c`` is None); its programs run through eb_decode_run_ctc_stream (CTC) or eb_decode_run_gru_rnnt
+    (transducer)."""
     from .rnnt.models import ResLayerNormGRU
     gru = isinstance(enc.lstm, ResLayerNormGRU)
     lstms = list(enc.lstm.lstms)
@@ -305,59 +368,146 @@ def encoder_phases(prog, engine, enc, S, n):
     z = lambda *shape: torch.zeros(*shape, dtype=torch.float32, device=engine.dev)
     engine.xin, engine.a0 = z(S, n, F), z(S, n, F)
     engine.enc_h, engine.enc_c, engine.enc_htmp = z(L, S, H), None if gru else z(L, S, H), z(L, S, H)
-
-    def ph(**kw):
-        p = EbPhase()
-        for k, v in kw.items():
-            setattr(p, k, v)
-        prog.append(p)
-
-    ph(type=PH_LN, S=S * n, N=F, x1=_ptr(engine.xin), ldx1=F, w1=_ptr(enc.norm.weight), b1=_ptr(enc.norm.bias),
-       y=_ptr(engine.a0), ldy=F)
+    prog.append(EbPhase(type=PH_LN, S=S * n, N=F, x1=_ptr(engine.xin), ldx1=F, w1=_ptr(enc.norm.weight),
+                        b1=_ptr(enc.norm.bias), y=_ptr(engine.a0), ldy=F))
     X, I, ni = engine.a0, F, n
     engine._bufs = []
     for i, (cell, post) in enumerate(zip(lstms, enc.lstm.projs)):
         yL, zL = z(S, ni, H), z(S, ni, H)
         engine._bufs += [yL, zL]
         for t in range(ni):
-            ph(type=PH_GRU if gru else PH_LSTM, S=S, N=H, K1=I, K2=H, x1=_ptr(X, t * I), ldx1=ni * I,
-               x2=_ptr(engine.enc_h[i]) if t == 0 else _ptr(yL, (t - 1) * H), ldx2=H if t == 0 else ni * H,
-               w1=_ptr(cell.weight_ih_l0), ldw1=I, w2=_ptr(cell.weight_hh_l0), ldw2=H,
-               b1=_ptr(cell.bias_ih_l0), b2=_ptr(cell.bias_hh_l0), c=None if gru else _ptr(engine.enc_c[i]),
-               y=_ptr(yL, t * H), ldy=ni * H, y2=_ptr(engine.enc_htmp[i]) if t == ni - 1 else None)
+            prog.append(EbPhase(type=PH_GRU if gru else PH_LSTM, S=S, N=H, K1=I, K2=H, x1=_ptr(X, t * I), ldx1=ni * I,
+                                x2=_ptr(engine.enc_h[i]) if t == 0 else _ptr(yL, (t - 1) * H),
+                                ldx2=H if t == 0 else ni * H, w1=_ptr(cell.weight_ih_l0), ldw1=I,
+                                w2=_ptr(cell.weight_hh_l0), ldw2=H, b1=_ptr(cell.bias_ih_l0), b2=_ptr(cell.bias_hh_l0),
+                                c=None if gru else _ptr(engine.enc_c[i]), y=_ptr(yL, t * H), ldy=ni * H,
+                                y2=_ptr(engine.enc_htmp[i]) if t == ni - 1 else None))
         ln = post[0]
-        ph(type=PH_LN, S=S * ni, N=H, x1=_ptr(yL), ldx1=H, x2=_ptr(X) if i > 0 else None, ldx2=H,
-           w1=_ptr(ln.weight), b1=_ptr(ln.bias), y=_ptr(zL), ldy=H)
+        prog.append(EbPhase(type=PH_LN, S=S * ni, N=H, x1=_ptr(yL), ldx1=H, x2=_ptr(X) if i > 0 else None, ldx2=H,
+                            w1=_ptr(ln.weight), b1=_ptr(ln.bias), y=_ptr(zL), ldy=H))
         X, I = zL, H
         if i in reductions:
             if ni % 2:
                 raise _odd_chunk()
             zr = z(S, ni // 2, H)
             engine._bufs.append(zr)
-            ph(type=PH_PAIR, S=S, N=H, aux=ni, x1=_ptr(zL), y=_ptr(zr))
+            prog.append(EbPhase(type=PH_PAIR, S=S, N=H, aux=ni, x1=_ptr(zL), y=_ptr(zr)))
             X, ni = zr, ni // 2
     engine.n_out = ni
     E = enc.proj.weight.shape[0] if enc.has_proj else H
     if enc.has_proj:
         engine.enc_out = z(S, ni, E)
-        ph(type=PH_LINEAR, S=S * ni, N=E, K1=H, x1=_ptr(X), ldx1=H, w1=_ptr(enc.proj.weight), ldw1=H,
-           b1=_ptr(enc.proj.bias), y=_ptr(engine.enc_out), ldy=E)
+        prog.append(EbPhase(type=PH_LINEAR, S=S * ni, N=E, K1=H, x1=_ptr(X), ldx1=H, w1=_ptr(enc.proj.weight),
+                            ldw1=H, b1=_ptr(enc.proj.bias), y=_ptr(engine.enc_out), ldy=E))
     else:
         engine.enc_out = X
     return E
 
 
 def _upload(prog, dev):
+    """The phase list ``prog`` as the device bytes a decode kernel entry reads."""
+    assert C.sizeof(EbPhase) == lib().eb_decode_phase_size(), "EbPhase layout mismatch"
     arr = (EbPhase * len(prog))(*prog)
     return torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(dev)
 
 
-class StreamEngine:
-    STATE = ("enc_h", "enc_c", "dec_h", "dec_c", "dec_x", "tok")
-    RUN = "eb_decode_run"                     # the decode kernel entry every program of the engine runs through
+def _launch(entry, prog, nphase, bar, max_ctas):
+    """Run the first nphase phases of the uploaded program ``prog`` through the decode kernel entry ``entry`` on the
+    current stream; ``bar`` is the engine's grid barrier, which the entry zeroes at every launch."""
+    check(getattr(lib(), entry)(prog.data_ptr(), nphase, bar.data_ptr(), max_ctas,
+                                torch.cuda.current_stream().cuda_stream), entry)
 
-    def _check_encoder(self, enc, n_streams, frames_per_chunk):
-        _check_lstm_encoder(enc, "StreamEngine")
+
+class _ChunkEngine:
+    """What the streaming engines (StreamEngine, StreamBeamEngine, CTCStreamEngine) share: the host-side checks in a
+    fixed order (the encoder kind, check_stream_shape, then the CUDA device), the stateful encoder at the head of the
+    chunk program and the COPY that closes it, the launches, and ``state()`` / ``load_state()`` over
+    ``_state_views()``."""
+    GRU = False          # the encoder kind: ResLayerNormGRU cells, carrying enc_h alone, or ResLayerNormLSTM cells
+    HOST_STATE = ()      # keys of state() that are host tensors, outside _state_views
+
+    @functools.cached_property
+    def RUN(self):
+        """The decode kernel entry every program of the engine runs through (an instance may set another)."""
+        return "eb_decode_run_gru_rnnt" if self.GRU else "eb_decode_run"
+
+    def _check_shape(self, enc, n_streams, frames_per_chunk):
+        """check_stream_shape's (S, n, encoder output frames per chunk), after refusing an encoder of the other kind
+        with ValueError.  Touches no device."""
+        from .rnnt.models import ResLayerNormGRU, ResLayerNormLSTM
+        if not isinstance(enc.lstm, ResLayerNormGRU if self.GRU else ResLayerNormLSTM):
+            # the encoder phases are cells of one kind: LSTM (4H-row weights) or GRU (3H rows)
+            who, kind, got = type(self).__name__, "a GRU" if self.GRU else "an LSTM", type(enc.lstm).__name__
+            raise ValueError("%s streams %s encoder only, got %s" % (who, kind, got))
+        return check_stream_shape(enc, n_streams, frames_per_chunk)
+
+    def _build_encoder(self, prog, model, enc, S, n, T):
+        """After every other check, the CUDA device check; then encoder_phases into ``prog`` (T output frames per
+        chunk).  The program reads ``model``'s weights in place: they are kept, and ``fingerprint`` tells when they
+        move.  Returns the encoder output width E."""
+        self.dev = enc.norm.weight.device
+        if self.dev.type != "cuda":
+            raise RuntimeError("%s needs the model on a CUDA device" % type(self).__name__)
+        self._keep = [p.detach() for p in model.parameters()]
+        self.fingerprint = param_fingerprint(model)
+        E = encoder_phases(prog, self, enc, S, n)
+        assert self.n_out == T
+        return E
+
+    def _finish(self, prog, state):
+        """Close the chunk program ``prog`` with the COPY of the encoder's last h into the carried enc_h and upload it;
+        then start every stream from ``state`` (a rebuilt program continues the utterance, rnnt/stream.py:97-98), or
+        from ``reset()`` without one."""
+        L, S, H = self.enc_h.shape
+        prog.append(EbPhase(type=PH_COPY, S=L * S, N=H, x1=_ptr(self.enc_htmp), y=_ptr(self.enc_h)))
+        self._chunk, self.n_chunk_phases = _upload(prog, self.dev), len(prog)
+        self._bar = torch.zeros(64, dtype=torch.int32, device=self.dev)
+        if state is None:
+            self.reset()
+        else:
+            self.load_state(state)
+
+    def _run(self, prog, nphase):
+        _launch(self.RUN, prog, nphase, self._bar, self.max_ctas)
+
+    def _fetch(self, width):
+        """Copy ``_out`` (ids [S, width] | counts [S] | any further values) to the pinned ``_host``: the chunk's only
+        device-to-host copy.  -> (ids [S, width], counts [S], the further values) on the host."""
+        S = self.S
+        self._host.copy_(self._out, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        rest = self._host[S * width:].clone()
+        return self._host[:S * width].view(S, width).clone(), rest[:S], rest[S:]
+
+    def _state_views(self):
+        v = dict(enc_h=self.enc_h)
+        if self.enc_c is not None:                           # a GRU encoder carries h alone
+            v["enc_c"] = self.enc_c
+        return v
+
+    def state(self):
+        """The recurrent state of every stream (what PytorchStreamDecoder carries between chunks, rnnt/stream.py:78-91),
+        as a dict of device tensors."""
+        return {k: t.clone() for k, t in self._state_views().items()}
+
+    @torch.no_grad()
+    def load_state(self, st):
+        """Continue from ``state()`` of an engine of the same kind over the same model and n_streams, with any chunk
+        length or re-homed weights."""
+        views = self._state_views()
+        if set(st) != set(views) | set(self.HOST_STATE):
+            raise ValueError("state keys %s do not match this engine's %s (an LSTM encoder carries enc_h and enc_c, a "
+                             "GRU encoder enc_h alone; a beam needs the same LM use)"
+                             % (sorted(st), sorted(set(views) | set(self.HOST_STATE))))
+        for k, t in views.items():
+            if tuple(st[k].shape) != tuple(t.shape):
+                raise ValueError("state %s has shape %s, this engine needs %s (same model and n_streams, and for a "
+                                 "beam the same W and max_pending)" % (k, tuple(st[k].shape), tuple(t.shape)))
+            t.copy_(st[k])
+
+
+class StreamEngine(_ChunkEngine):
+    STATE = ("enc_h", "enc_c", "dec_h", "dec_c", "dec_x", "tok")   # the carried state (enc_c: None for a GRU encoder)
 
     def __init__(self, transducer, n_streams, frames_per_chunk, unk_id=UNK, blank=NUL, max_ctas=0, state=None,
                  max_symbols=1):
@@ -365,31 +515,13 @@ class StreamEngine:
         predictor step; a stream's frame ends at its first blank or after K non-blank tokens.  ``step`` then returns
         [S, n_out * K]: K entries per frame, blank for the rounds a stream did not take."""
         K = check_max_symbols(max_symbols)
-        assert C.sizeof(EbPhase) == lib().eb_decode_phase_size(), "EbPhase layout mismatch"
         enc, dec, joint = transducer.encoder, transducer.decoder, transducer.joint.joint
-        self._check_encoder(enc, n_streams, frames_per_chunk)
-        self.dev = enc.norm.weight.device
-        if self.dev.type != "cuda":
-            raise RuntimeError("%s needs the model on a CUDA device" % type(self).__name__)
-        f32 = torch.float32
-        S, n = n_streams, frames_per_chunk
+        S, n, T = self._check_shape(enc, n_streams, frames_per_chunk)
         self.S, self.n, self.blank, self.unk, self.max_ctas, self.max_symbols = S, n, blank, unk_id, max_ctas, K
-        L = len(enc.lstm.lstms)
-        H = enc.lstm.hidden_size
-        z = lambda *shape: torch.zeros(*shape, dtype=f32, device=self.dev)
-        self._keep = [p.detach() for p in transducer.parameters()]      # weights are read in place
-        self.fingerprint = param_fingerprint(transducer)
         prog = []
-
-        def ph(**kw):
-            p = EbPhase()
-            for k, v in kw.items():
-                setattr(p, k, v)
-            prog.append(p)
-
-        E = encoder_phases(prog, self, enc, S, n)
-        ni = self.n_out
+        E = self._build_encoder(prog, transducer, enc, S, n, T)
         # ---- predictor + joint state
+        z = lambda *shape: torch.zeros(*shape, dtype=torch.float32, device=self.dev)
         Ld, Hd = dec.lstm.num_layers, dec.lstm.hidden_size
         D = dec.proj.weight.shape[0]
         J, V = joint[0].weight.shape[0], joint[2].weight.shape[0]
@@ -397,58 +529,19 @@ class StreamEngine:
         self.dec_h, self.dec_c, self.dec_htmp = z(Ld, S, Hd), z(Ld, S, Hd), z(Ld, S, Hd)
         self.dec_x, self.hidden, self.logits = z(S, D), z(S, J), z(S, V)
         self.tok = torch.zeros(S, dtype=torch.int32, device=self.dev)
-        self.hist = torch.zeros(S, max(ni * K, 1), dtype=torch.int32, device=self.dev)
-
-        w1 = joint[0].weight
-        for k in range(ni):
-            def round_phases(j):
-                ph(type=PH_LINEAR, S=S, N=J, flags=F_TANH, K1=E, x1=_ptr(self.enc_out, k * E), ldx1=ni * E,
-                   w1=_ptr(w1), ldw1=E + D, K2=D, x2=_ptr(self.dec_x), ldx2=D, w2=_ptr(w1, E), ldw2=E + D,
-                   b1=_ptr(joint[0].bias), y=_ptr(self.hidden), ldy=J)
-                ph(type=PH_LINEAR, S=S, N=V, K1=J, x1=_ptr(self.hidden), ldx1=J, w1=_ptr(joint[2].weight), ldw1=J,
-                   b1=_ptr(joint[2].bias), y=_ptr(self.logits), ldy=V)
-                ph(type=PH_ARGMAX, S=S, N=V, flags=F_CONT if j else 0, x1=_ptr(self.logits), ldx1=V, aux=blank,
-                   aux2=unk_id, tok_out=_ptr(self.tok), hist=_ptr(self.hist), hist_ld=self.hist.shape[1],
-                   hist_col=k * K + j)
-                _dec_phases(prog, dec, S, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
-                            masked=True)
-            greedy_frame(prog, K, S, self.tok, blank, round_phases)
-        ph(type=PH_COPY, S=L * S, N=H, x1=_ptr(self.enc_htmp), y=_ptr(self.enc_h))
-        self.n_chunk_phases = len(prog)
-        chunk_prog = prog
-        prog = []
-        _dec_phases(prog, dec, S, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
+        self.hist = torch.zeros(S, T * K, dtype=torch.int32, device=self.dev)
+        self._joint = (joint[0].weight, joint[0].bias, joint[2].weight, joint[2].bias)
+        for k in range(T):
+            greedy_frame(prog, K, S, self.tok, blank,
+                         lambda j: greedy_round(prog, self, dec, self.enc_out, k, j, 0, unk_id))
+        prime = []
+        _dec_phases(prime, dec, S, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
                     masked=False)                  # priming program: tok = BOS from a zero state
-        self.n_prime_phases = len(prog)
-        self._chunk = self._upload(chunk_prog)
-        self._prime = self._upload(prog)
-        self._bar = torch.zeros(64, dtype=torch.int32, device=self.dev)
-        if state is None:
-            self.reset()
-        else:
-            self.load_state(state)                      # a rebuilt program continues the utterance (rnnt/stream.py:97-98)
+        self._prime, self.n_prime_phases = _upload(prime, self.dev), len(prime)
+        self._finish(prog, state)
 
-    def state(self):
-        """The recurrent state of every stream (what PytorchStreamDecoder carries between chunks, rnnt/stream.py:78-91)."""
-        return {k: getattr(self, k).clone() for k in self.STATE}
-
-    @torch.no_grad()
-    def load_state(self, st):
-        if set(st) != set(self.STATE):
-            raise ValueError("state keys %s do not match this engine's %s (an LSTM encoder carries enc_h and enc_c, a "
-                             "GRU encoder enc_h alone)" % (sorted(st), sorted(self.STATE)))
-        for k in self.STATE:
-            getattr(self, k).copy_(st[k])
-
-    def _upload(self, prog):
-        arr = (EbPhase * len(prog))(*prog)
-        raw = bytes(arr)
-        t = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(self.dev)
-        return t
-
-    def _run(self, prog, nphase):
-        check(getattr(lib(), self.RUN)(prog.data_ptr(), nphase, self._bar.data_ptr(), self.max_ctas,
-                                       torch.cuda.current_stream().cuda_stream), self.RUN)
+    def _state_views(self):
+        return {k: getattr(self, k) for k in self.STATE if getattr(self, k) is not None}
 
     @torch.no_grad()
     def reset(self):
@@ -483,6 +576,8 @@ class GreedyEngine:
         K = check_max_symbols(max_symbols)
         dec, joint = transducer.decoder, transducer.joint.joint
         self.dev = dec.embed.weight.device
+        if self.dev.type != "cuda":
+            raise RuntimeError("GreedyEngine needs the model on a CUDA device")
         f32 = torch.float32
         B, T = batch, t_out
         self.B, self.T, self.blank, self.max_ctas, self.max_symbols = B, T, blank, max_ctas, K
@@ -498,33 +593,15 @@ class GreedyEngine:
         self.hist = torch.zeros(B, T * K, dtype=torch.int32, device=self.dev)
         self.logp = z(B)
         self._keep = [p.detach() for p in transducer.parameters()]
+        self._joint = (joint[0].weight, joint[0].bias, joint[2].weight, joint[2].bias)
         prog = []
-
-        def ph(**kw):
-            q = EbPhase()
-            for k, v in kw.items():
-                setattr(q, k, v)
-            prog.append(q)
-
         _dec_phases(prog, dec, B, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
                     masked=False)                   # prime with BOS from the zero state
-        w1 = joint[0].weight
         for k in range(T):
-            def round_phases(j):
-                ph(type=PH_LINEAR, S=B, N=J, flags=F_TANH, K1=E, x1=_ptr(self.h_enc, k * E), ldx1=T * E, w1=_ptr(w1),
-                   ldw1=E + D, K2=D, x2=_ptr(self.dec_x), ldx2=D, w2=_ptr(w1, E), ldw2=E + D, b1=_ptr(joint[0].bias),
-                   y=_ptr(self.hidden), ldy=J)
-                ph(type=PH_LINEAR, S=B, N=V, K1=J, x1=_ptr(self.hidden), ldx1=J, w1=_ptr(joint[2].weight), ldw1=J,
-                   b1=_ptr(joint[2].bias), y=_ptr(self.logits), ldy=V)
-                ph(type=PH_ARGMAX, S=B, N=V, flags=F_LOGP | (F_CONT if j else 0), x1=_ptr(self.logits), ldx1=V,
-                   aux=blank, aux2=-1, tok_out=_ptr(self.tok), hist=_ptr(self.hist), hist_ld=T * K,
-                   hist_col=k * K + j, y=_ptr(self.logp))
-                _dec_phases(prog, dec, B, self.dec_h, self.dec_c, self.dec_htmp, self.dec_x, self.tok, blank,
-                            masked=True)
-            greedy_frame(prog, K, B, self.tok, blank, round_phases)
+            greedy_frame(prog, K, B, self.tok, blank,
+                         lambda j: greedy_round(prog, self, dec, self.h_enc, k, j, F_LOGP, -1, self.logp))
         self.nphase = len(prog)
-        arr = (EbPhase * len(prog))(*prog)
-        self._prog = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(self.dev)
+        self._prog = _upload(prog, self.dev)
         self._bar = torch.zeros(64, dtype=torch.int32, device=self.dev)
 
     @torch.no_grad()
@@ -536,8 +613,7 @@ class GreedyEngine:
         if self.max_symbols > 1:
             self.hist.fill_(self.blank)             # the columns of rounds skipped for every row are not written
         self.tok.fill_(BOS)
-        check(lib().eb_decode_run(self._prog.data_ptr(), self.nphase, self._bar.data_ptr(), self.max_ctas,
-                                  torch.cuda.current_stream().cuda_stream), "eb_decode_run")
+        _launch("eb_decode_run", self._prog, self.nphase, self._bar, self.max_ctas)
         return self.hist, self.logp
 
 
@@ -587,61 +663,32 @@ class BeamEngine:
         J, V = joint[0].weight.shape[0], joint[2].weight.shape[0]
         E = joint[0].weight.shape[1] - D
         self.h_enc, self.frames = z(B, T, E), z(B, dtype=i32)
+        self._keep = [p.detach() for p in transducer.parameters()]
         self.lm = fusion is not None
-        if self.lm:
-            lsd, lw, lb, self.lm_bos, tmap = fusion
-            # the weights are read in place when they already are fp32 on this device (tied weights stay tied)
-            lsd = {k: v.to(self.dev, f32).contiguous() for k, v in lsd.items()}
-            Ll = (len(lsd) - 3) // 4
-            lm_layers = [tuple(lsd["rnn.%s_l%d" % (n, k)] for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"))
-                         for k in range(Ll)]
-            Hl, ntok = lm_layers[0][1].shape[1], lsd["encoder.weight"].shape[0]
+        lm_sel, lm_step = lm_fusion(self, fusion, R) if self.lm else ({}, None)
         # per parity: predictor state, its output, {len, hash lo, hash hi, tokens} per row and the LM state
-        beam_state(self, R, Ld, Hd, D, TK + 3, *((Ll, Hl) if self.lm else ()))
+        beam_state(self, R, Ld, Hd, D, TK + 3)
         self.dec_htmp, self.hidden, self.logits = z(Ld, R, Hd), z(R, J), z(R, V)
         self.tok, self.src, self.logp = z(R, dtype=i32), z(R, dtype=i32), z(R)
-        n = B * TK * W
-        self.hist = z(3 * n + B * TK, dtype=i32)
-        self.hist_parent = self.hist[:n].view(B, TK, W)
-        self.hist_token = self.hist[n:2 * n].view(B, TK, W)
-        self.hist_logp = self.hist[2 * n:3 * n].view(f32).view(B, TK, W)
-        self.hist_live = self.hist[3 * n:].view(B, TK)
+        beam_history(self, B, TK, W)
         self._slots = torch.arange(W, dtype=i32, device=self.dev)
         self.ids, self.nlogp = z(B, max(TK, 1), dtype=i32), z(B)
-        self._keep = [p.detach() for p in transducer.parameters()]
         self._joint = (joint[0].weight, joint[0].bias, joint[2].weight, joint[2].bias)
         prog = []
         _dec_phases(prog, dec, R, self.dec_h[0], self.dec_c[0], self.dec_htmp, self.dec_x[0], self.tok, blank,
                     masked=False)                         # prime every row with BOS from the zero state
         if self.lm:
-            self._keep += list(lsd.values())
-            self.lm_htmp, self.lm_logits, self.lm_tok = z(Ll, R, Hl), z(R, ntok), z(R, dtype=i32)
-            self.lm_map = tmap.to(self.dev, i32)
-            self.lm_fuse = torch.tensor([lw, lb], dtype=f32, device=self.dev)
-
-            def lm_phases(q, masked):
-                predictor_phases(prog, lsd["encoder.weight"], lm_layers, lsd["decoder.weight"], lsd["decoder.bias"],
-                                 R, self.lm_h[q], self.lm_c[q], self.lm_htmp, self.lm_logits, self.lm_tok, -1, masked)
-            lm_phases(0, masked=False)                           # prime every row with lm_bos from the zero state
-        sel = dict(type=PH_BEAM_SELECT, S=B, N=V, aux=W, aux2=blank, flags=F_MERGE if merge else 0,
-                   x1=_ptr(self.logits), ldx1=V, y=_ptr(self.logp), tok_in=_ptr(self.frames), tok_out=_ptr(self.tok),
-                   src=_ptr(self.src), hist=_ptr(self.hist), hist_ld=TK)
-        if self.lm:
-            sel.update(flags=sel["flags"] | F_LM, x2=_ptr(self.lm_logits), ldx2=ntok, K2=ntok, fuse=_ptr(self.lm_fuse),
-                       tok_map=_ptr(self.lm_map), tok_out2=_ptr(self.lm_tok))
-
-        def step(q):
-            _dec_phases(prog, dec, R, self.dec_h[q], self.dec_c[q], self.dec_htmp, self.dec_x[q], self.tok, blank,
-                        masked=True)
-            if self.lm:
-                lm_phases(q, masked=True)
+            lm_step(prog, self.lm_h[0], self.lm_c[0], masked=False)    # prime every row with lm_bos from zeros
+        sel = dict(type=PH_BEAM_SELECT, S=B, N=V, aux=W, aux2=blank,
+                   flags=(F_MERGE if merge else 0) | (F_LM if self.lm else 0), x1=_ptr(self.logits), ldx1=V,
+                   y=_ptr(self.logp), tok_in=_ptr(self.frames), tok_out=_ptr(self.tok), src=_ptr(self.src),
+                   hist=_ptr(self.hist), hist_ld=TK, **lm_sel)
         for t in range(T):
-            beam_frame(prog, self, t, _ptr(self.h_enc, t * E), T * E, sel, step)
+            beam_frame(prog, self, dec, t, _ptr(self.h_enc, t * E), T * E, sel, lm_step)
         prog.append(EbPhase(type=PH_BEAM_FINAL, S=B, aux=W, aux2=blank, y=_ptr(self.logp), hist=_ptr(self.hist),
                             hist_ld=TK, tok_out=_ptr(self.ids), ldy=self.ids.shape[1], y2=_ptr(self.nlogp)))
         self.nphase = len(prog)
-        arr = (EbPhase * len(prog))(*prog)
-        self._prog = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(self.dev)
+        self._prog = _upload(prog, self.dev)
         self._bar = torch.zeros(64, dtype=torch.int32, device=self.dev)
 
     @torch.no_grad()
@@ -651,25 +698,17 @@ class BeamEngine:
         -log p [B] of that hypothesis, the negated fused score with an LM)."""
         self.h_enc.copy_(h_enc)
         self.frames.copy_(frames)
-        self._st[0].zero_()
-        self.seqs[0].zero_()
-        self.logp.fill_(float("-inf"))
-        self.logp.view(self.B, self.W)[:, 0] = 0.0
-        self.tok.fill_(BOS)
+        beam_reset(self)
         if self.max_symbols > 1 and self.T > 0:  # what a round a row does not take leaves: parent = slot, token = blank
             self.hist_parent.copy_(self._slots.expand_as(self.hist_parent))
             self.hist_token.fill_(self.blank)
             self.hist_live.zero_()
             self.hist_live[:, -1] = 1                           # the live count every round reads and writes
-        if self.lm:
-            self._lst[0].zero_()
-            self.lm_tok.fill_(self.lm_bos)
-        check(lib().eb_decode_run(self._prog.data_ptr(), self.nphase, self._bar.data_ptr(), self.max_ctas,
-                                  torch.cuda.current_stream().cuda_stream), "eb_decode_run")
+        _launch("eb_decode_run", self._prog, self.nphase, self._bar, self.max_ctas)
         return self.ids, self.nlogp
 
 
-class StreamBeamEngine:
+class StreamBeamEngine(_ChunkEngine):
     """Streaming beam search: S streams of W hypotheses each, carried from one chunk to the next, one persistent kernel
     launch per chunk.  The chunk program runs StreamEngine's stateful encoder, then per encoder output frame exactly
     BeamEngine's frame (joint, BEAM_SELECT, GATHER, masked predictor and LM steps, with or without LM fusion), so how
@@ -691,10 +730,7 @@ class StreamBeamEngine:
 
     The reference's ``<unk>`` rule (re-argmax when the argmax is ``<unk>``) is a device of the greedy loop; the beam,
     like Transducer.beam_search, does not apply it."""
-    RUN = "eb_decode_run"                     # the decode kernel entry every program of the engine runs through
-
-    def _check_encoder(self, enc):
-        _check_lstm_encoder(enc, "StreamBeamEngine")
+    HOST_STATE = ("unreturned_ids", "unreturned_counts")
 
     def __init__(self, transducer, n_streams, frames_per_chunk, W, merge=True, lm=None, lm_weight=0.0,
                  length_bonus=0.0, lm_bos=1, lm_token_map=None, max_pending=64, state=None, blank=NUL, max_ctas=0,
@@ -706,49 +742,31 @@ class StreamBeamEngine:
         V = transducer.joint.joint[2].weight.shape[0]
         fusion = check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map)
         enc, dec, joint = transducer.encoder, transducer.decoder, transducer.joint.joint
-        self._check_encoder(enc)
+        S, n, T = self._check_shape(enc, n_streams, frames_per_chunk)
         P = operator.index(max_pending)
-        S, n, T = check_stream_shape(enc, n_streams, frames_per_chunk)
         if P < T * K:
             raise ValueError("max_pending (%d) must be at least the encoder frames per chunk times max_symbols (%d x %d):"
                              " a chunk can add that many tokens to a hypothesis" % (P, T, K))
-        assert C.sizeof(EbPhase) == lib().eb_decode_phase_size(), "EbPhase layout mismatch"
-        self.dev = enc.norm.weight.device
-        if self.dev.type != "cuda":
-            raise RuntimeError("%s needs the model on a CUDA device" % type(self).__name__)
         f32, i32 = torch.float32, torch.int32
         R, LS, TK = S * W, P + 3, T * K
         self.S, self.n, self.W, self.R, self.merge, self.blank, self.max_ctas, self.max_pending, self.max_symbols = \
             S, n, W, R, merge, blank, max_ctas, P, K
-        z = lambda *shape, dtype=f32: torch.zeros(*shape, dtype=dtype, device=self.dev)
-        self._keep = [p.detach() for p in transducer.parameters()]      # weights are read in place
-        self.fingerprint = param_fingerprint(transducer)
-        L, H = len(enc.lstm.lstms), enc.lstm.hidden_size
         prog = []
-        E = encoder_phases(prog, self, enc, S, n)
-        assert self.n_out == T
+        E = self._build_encoder(prog, transducer, enc, S, n, T)
+        z = lambda *shape, dtype=f32: torch.zeros(*shape, dtype=dtype, device=self.dev)
         Ld, Hd = dec.lstm.num_layers, dec.lstm.hidden_size
         D = dec.proj.weight.shape[0]
         J = joint[0].weight.shape[0]
         self.lm = fusion is not None
-        if self.lm:
-            lsd, lw, lb, self.lm_bos, tmap = fusion
-            lsd = {k: v.to(self.dev, f32).contiguous() for k, v in lsd.items()}
-            self._keep += list(lsd.values())
-            Ll = (len(lsd) - 3) // 4
-            lm_layers = [tuple(lsd["rnn.%s_l%d" % (nm, k)] for nm in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"))
-                         for k in range(Ll)]
-            Hl, ntok = lm_layers[0][1].shape[1], lsd["encoder.weight"].shape[0]
+        lm_sel, lm_step = lm_fusion(self, fusion, R) if self.lm else ({}, None)
         # per parity: predictor state, its output, {suffix length, hash lo, hash hi, tokens since the last commit} per
         # row and the LM state
-        beam_state(self, R, Ld, Hd, D, LS, *((Ll, Hl) if self.lm else ()))
+        beam_state(self, R, Ld, Hd, D, LS)
         st = self._st
         self.dec_htmp, self.hidden, self.logits = z(Ld, R, Hd), z(R, J), z(R, V)
         self.tok, self.src, self.logp = z(R, dtype=i32), z(R, dtype=i32), z(R)
         self.frames = torch.full((S,), T, dtype=i32, device=self.dev)      # a stream never freezes
-        nh = S * TK * W
-        self.hist = z(3 * nh + S * TK, dtype=i32)
-        self.hist_live = self.hist[3 * nh:].view(S, TK)       # the last column carries the live count between launches
+        beam_history(self, S, TK, W)                          # hist_live's last column: the live count between launches
         self._out = z(S * P + 2 * S, dtype=i32)               # committed ids [S, P] | counts [S] | collapsed [S]
         self._host = torch.zeros(self._out.shape, dtype=i32).pin_memory()
         self.n_collapses = 0
@@ -757,29 +775,16 @@ class StreamBeamEngine:
         _dec_phases(prime, dec, R, self.dec_h[0], self.dec_c[0], self.dec_htmp, self.dec_x[0], self.tok, blank,
                     masked=False)
         if self.lm:
-            self.lm_htmp, self.lm_logits, self.lm_tok = z(Ll, R, Hl), z(R, ntok), z(R, dtype=i32)
+            Ll, _, Hl = self.lm_htmp.shape
+            ntok = self.lm_logits.shape[1]
             self._lm_logits_tmp = z(R, ntok)
-            self.lm_map = tmap.to(self.dev, i32)
-            self.lm_fuse = torch.tensor([lw, lb], dtype=f32, device=self.dev)
-
-            def lm_phases(pr, q, masked):
-                predictor_phases(pr, lsd["encoder.weight"], lm_layers, lsd["decoder.weight"], lsd["decoder.bias"],
-                                 R, self.lm_h[q], self.lm_c[q], self.lm_htmp, self.lm_logits, self.lm_tok, -1, masked)
-            lm_phases(prime, 0, masked=False)
-        sel = dict(type=PH_BEAM_SELECT, S=S, N=V, aux=W, aux2=blank, flags=F_STREAM | (F_MERGE if merge else 0),
-                   K1=LS, x1=_ptr(self.logits), ldx1=V, y=_ptr(self.logp), tok_in=_ptr(self.frames),
-                   tok_out=_ptr(self.tok), src=_ptr(self.src), hist=_ptr(self.hist), hist_ld=TK)
-        if self.lm:
-            sel.update(flags=sel["flags"] | F_LM, x2=_ptr(self.lm_logits), ldx2=ntok, K2=ntok, fuse=_ptr(self.lm_fuse),
-                       tok_map=_ptr(self.lm_map), tok_out2=_ptr(self.lm_tok))
-
-        def step(q):
-            _dec_phases(prog, dec, R, self.dec_h[q], self.dec_c[q], self.dec_htmp, self.dec_x[q], self.tok, blank,
-                        masked=True)
-            if self.lm:
-                lm_phases(prog, q, masked=True)
+            lm_step(prime, self.lm_h[0], self.lm_c[0], masked=False)
+        sel = dict(type=PH_BEAM_SELECT, S=S, N=V, aux=W, aux2=blank,
+                   flags=F_STREAM | (F_MERGE if merge else 0) | (F_LM if self.lm else 0), K1=LS, x1=_ptr(self.logits),
+                   ldx1=V, y=_ptr(self.logp), tok_in=_ptr(self.frames), tok_out=_ptr(self.tok), src=_ptr(self.src),
+                   hist=_ptr(self.hist), hist_ld=TK, **lm_sel)
         for t in range(T):
-            beam_frame(prog, self, t, _ptr(self.enc_out, t * E), T * E, sel, step)
+            beam_frame(prog, self, dec, t, _ptr(self.enc_out, t * E), T * E, sel, lm_step)
 
         def chunk_end(pr, in_parity0, flush):
             """commit (and collapse) from parity 1 into parity 0; state found in parity 0 is copied over first"""
@@ -802,26 +807,17 @@ class StreamBeamEngine:
                                   K2=ntok, x2=_ptr(self._lm_logits_tmp), y2=_ptr(self.lm_logits), src=_ptr(self.src)))
 
         chunk_end(prog, K > 1 or T % 2 == 0, flush=False)     # where the frames left the state
-        prog.append(EbPhase(type=PH_COPY, S=L * S, N=H, x1=_ptr(self.enc_htmp), y=_ptr(self.enc_h)))
         flush, rebound = [], []
         chunk_end(flush, True, flush=True)
         chunk_end(rebound, True, flush=False)   # a loaded beam under this engine's bound, max_pending - n_out * K
-        self.n_chunk_phases, self.n_prime_phases, self.n_flush_phases = len(prog), len(prime), len(flush)
-        self._chunk, self._prime, self._flush = _upload(prog, self.dev), _upload(prime, self.dev), \
-            _upload(flush, self.dev)
-        self._rebound, self.n_rebound_phases = _upload(rebound, self.dev), len(rebound)
-        self._bar = torch.zeros(64, dtype=torch.int32, device=self.dev)
-        self._unreturned = (torch.zeros(S, 0, dtype=i32), torch.zeros(S, dtype=i32))
-        if state is None:
-            self.reset()
-        else:
-            self.load_state(state)
+        self._prime, self._flush, self._rebound = _upload(prime, self.dev), _upload(flush, self.dev), \
+            _upload(rebound, self.dev)
+        self.n_prime_phases, self.n_flush_phases, self.n_rebound_phases = len(prime), len(flush), len(rebound)
+        self._finish(prog, state)
 
     def _state_views(self):
-        v = dict(enc_h=self.enc_h, enc_c=self.enc_c, dec_state=self._st[0], dec_x=self.dec_x[0], logp=self.logp,
-                 seqs=self.seqs[0], live=self.hist_live[:, -1])
-        if self.enc_c is None:                               # a GRU encoder carries h alone
-            del v["enc_c"]
+        v = dict(super()._state_views(), dec_state=self._st[0], dec_x=self.dec_x[0], logp=self.logp, seqs=self.seqs[0],
+                 live=self.hist_live[:, -1])
         if self.lm:
             v.update(lm_state=self._lst[0], lm_logits=self.lm_logits)
         return v
@@ -830,7 +826,7 @@ class StreamBeamEngine:
         """Every stream's encoder state and beam (slot log p, stored token suffixes, live count, predictor and LM
         states), as a dict of tensors, with the committed tokens not yet returned by ``step`` (host ids [S, K] and
         counts [S])."""
-        st = {k: t.clone() for k, t in self._state_views().items()}
+        st = super().state()
         st["unreturned_ids"], st["unreturned_counts"] = (t.clone() for t in self._unreturned)
         return st
 
@@ -840,19 +836,10 @@ class StreamBeamEngine:
         chunk length.  The previous engine bounded every stored suffix by max_pending minus ITS n_out; when this
         engine's chunks yield more encoder frames, that bound is too loose, so the chunk-end commit and collapse rule
         runs once here with this engine's bound.  The tokens it commits are returned by the next ``step``."""
-        views = self._state_views()
-        carried = ("unreturned_ids", "unreturned_counts")
-        if set(st) != set(views) | set(carried):
-            raise ValueError("state keys %s do not match this engine's %s (same model, LM use, n_streams, W and "
-                             "max_pending are needed)" % (sorted(st), sorted(set(views) | set(carried))))
-        for k, t in views.items():
-            if tuple(st[k].shape) != tuple(t.shape):
-                raise ValueError("state %s has shape %s, this engine needs %s (same n_streams, W and max_pending)"
-                                 % (k, tuple(st[k].shape), tuple(t.shape)))
-            t.copy_(st[k])
-        self._unreturned = tuple(st[k].to("cpu", torch.int32) for k in carried)
+        super().load_state(st)
+        self._unreturned = tuple(st[k].to("cpu", torch.int32) for k in self.HOST_STATE)
         self._run(self._rebound, self.n_rebound_phases)
-        ids, counts, collapsed = self._fetch()
+        ids, counts, collapsed = self._fetch(self.max_pending)
         self.n_collapses += int(collapsed.sum())
         self._add_unreturned(ids, counts)
 
@@ -875,32 +862,16 @@ class StreamBeamEngine:
             self._unreturned = (ids[:, :0].clone(), torch.zeros_like(counts))
         return ids, counts
 
-    def _run(self, prog, nphase):
-        check(getattr(lib(), self.RUN)(prog.data_ptr(), nphase, self._bar.data_ptr(), self.max_ctas,
-                                       torch.cuda.current_stream().cuda_stream), self.RUN)
-
-    def _fetch(self):
-        S, P = self.S, self.max_pending
-        self._host.copy_(self._out, non_blocking=True)       # the chunk's only device-to-host copy
-        torch.cuda.current_stream().synchronize()
-        return self._host[:S * P].view(S, P).clone(), self._host[S * P:S * P + S].clone(), \
-            self._host[S * P + S:].clone()
-
     @torch.no_grad()
     def reset(self):
         """Every stream starts a new utterance: zero encoder state, one live slot of log p 0 with the empty sequence,
         predictor primed with <bos> and the LM with lm_bos from zeros."""
-        for t in (self.enc_h, self.enc_c, self._st[0], self.seqs[0]):
+        for t in (self.enc_h, self.enc_c):
             if t is not None:
                 t.zero_()
-        self.logp.fill_(float("-inf"))
-        self.logp.view(self.S, self.W)[:, 0] = 0.0
+        beam_reset(self)
         self.hist_live[:, -1] = 1
         self._unreturned = (torch.zeros(self.S, 0, dtype=torch.int32), torch.zeros(self.S, dtype=torch.int32))
-        self.tok.fill_(BOS)
-        if self.lm:
-            self._lst[0].zero_()
-            self.lm_tok.fill_(self.lm_bos)
         self._run(self._prime, self.n_prime_phases)
 
     @torch.no_grad()
@@ -911,7 +882,7 @@ class StreamBeamEngine:
         ``n_collapses`` counts the forced collapses so far."""
         self.xin.copy_(chunk, non_blocking=True)
         self._run(self._chunk, self.n_chunk_phases)
-        ids, counts, collapsed = self._fetch()
+        ids, counts, collapsed = self._fetch(self.max_pending)
         self.n_collapses += int(collapsed.sum())
         return self._take(ids, counts)
 
@@ -921,7 +892,7 @@ class StreamBeamEngine:
         decoding continues from it.  -> (ids int32 [S, K], counts int32 [S] as from ``step``, -log p [S] of the best
         hypothesis, the negated fused score with an LM), on the host."""
         self._run(self._flush, self.n_flush_phases)
-        ids, counts, _ = self._fetch()
+        ids, counts, _ = self._fetch(self.max_pending)
         ids, counts = self._take(ids, counts)
         return ids, counts, -self.logp.view(self.S, self.W)[:, 0].cpu()
 
@@ -937,12 +908,7 @@ class GRUStreamEngine(StreamEngine):
     Per stream the ids are those of Transducer.greedy_decode (with the <unk> rule) on the concatenated chunks: every
     layer is a unidirectional GRU and the time reduction pairs frames inside a chunk of even length, so the chunks with
     h carried give the offline encoder output.  The matrix products are fp32-accurate (3xTF32)."""
-    STATE = ("enc_h", "dec_h", "dec_c", "dec_x", "tok")
-    RUN = "eb_decode_run_gru_rnnt"
-
-    def _check_encoder(self, enc, n_streams, frames_per_chunk):
-        _check_gru_encoder(enc, "GRUStreamEngine")
-        check_stream_shape(enc, n_streams, frames_per_chunk)
+    GRU = True
 
 
 class GRUStreamBeamEngine(StreamBeamEngine):
@@ -952,10 +918,7 @@ class GRUStreamBeamEngine(StreamBeamEngine):
     beam frames and chunk end; every program (chunk, prime, flush, re-bound) runs through eb_decode_run_gru_rnnt.  The
     state carries ``enc_h`` and no ``enc_c``, so the state of an LSTM-encoder engine does not load here, nor this one's
     there."""
-    RUN = "eb_decode_run_gru_rnnt"
-
-    def _check_encoder(self, enc):
-        _check_gru_encoder(enc, "GRUStreamBeamEngine")
+    GRU = True
 
 
 def lm_cache_key(fusion):
@@ -997,7 +960,6 @@ class CTCBeamEngine:
         if n < 0 or (fusion is not None and n > 1):
             raise ValueError("frames_per_phase must be >= 0 (0: all), and 0 or 1 with an lm; got %d" % n)
         n = 1 if fusion is not None else (n or T)
-        assert C.sizeof(EbPhase) == lib().eb_decode_phase_size(), "EbPhase layout mismatch"
         self.dev = torch.device("cuda") if device is None else torch.device(device)
         if self.dev.type != "cuda":
             raise RuntimeError("CTCBeamEngine runs on a CUDA device")
@@ -1009,44 +971,26 @@ class CTCBeamEngine:
         self.state = z(2, 3, R)                      # per parity: pb | pnb | f
         self.seqs = z(2, R, LS, dtype=i32)           # per parity: {len, hash lo / hi, parent hash lo / hi, tokens}
         self.score, self.src = z(R), z(R, dtype=i32)
-        nh = B * T * W
-        self.hist = z(3 * nh + B * T, dtype=i32)
-        self.hist_parent = self.hist[:nh].view(B, T, W)
-        self.hist_token = self.hist[nh:2 * nh].view(B, T, W)
-        self.hist_live = self.hist[3 * nh:].view(B, T)
+        beam_history(self, B, T, W)
         self.ids, self.nlogp = z(B, T, dtype=i32), z(B)
         self.lm = fusion is not None
+        self._keep = []
+        lm_sel, lm_step = lm_fusion(self, fusion, R) if self.lm else ({}, None)
         prog = []
-        sel = dict(type=PH_CTC_BEAM, S=B, N=V, aux=W, aux2=blank, K1=LS, x1=_ptr(self.lp), tok_in=_ptr(self.frames),
-                   c=_ptr(self.state), seq_out=_ptr(self.seqs), y=_ptr(self.score), src=_ptr(self.src),
-                   hist=_ptr(self.hist), hist_ld=T)
+        sel = dict(type=PH_CTC_BEAM, S=B, N=V, aux=W, aux2=blank, K1=LS, flags=F_LM if self.lm else 0,
+                   x1=_ptr(self.lp), tok_in=_ptr(self.frames), c=_ptr(self.state), seq_out=_ptr(self.seqs),
+                   y=_ptr(self.score), src=_ptr(self.src), hist=_ptr(self.hist), hist_ld=T, **lm_sel)
         if self.lm:
-            lsd, lw, lb, self.lm_bos, tmap = fusion
-            lsd = {k: v.to(self.dev, f32).contiguous() for k, v in lsd.items()}
-            self._keep = list(lsd.values())
-            Ll = (len(lsd) - 3) // 4
-            layers = [tuple(lsd["rnn.%s_l%d" % (nm, k)] for nm in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"))
-                      for k in range(Ll)]
-            Hl, ntok = layers[0][1].shape[1], lsd["encoder.weight"].shape[0]
+            Ll, _, Hl = self.lm_htmp.shape
             self.lm_state = z(2, 2 * Ll, R, Hl)      # per parity: h of every layer, then c
-            self.lm_htmp, self.lm_logits, self.lm_tok = z(Ll, R, Hl), z(R, ntok), z(R, dtype=i32)
-            self.lm_map = tmap.to(self.dev, i32)
-            self.lm_fuse = torch.tensor([lw, lb], dtype=f32, device=self.dev)
-            sel.update(flags=F_LM, x2=_ptr(self.lm_logits), ldx2=ntok, K2=ntok, fuse=_ptr(self.lm_fuse),
-                       tok_map=_ptr(self.lm_map), tok_out2=_ptr(self.lm_tok))
-
-            def lm_step(q, masked):
-                st = self.lm_state[q]
-                predictor_phases(prog, lsd["encoder.weight"], layers, lsd["decoder.weight"], lsd["decoder.bias"], R,
-                                 st[:Ll], st[Ll:], self.lm_htmp, self.lm_logits, self.lm_tok, -1, masked)
-            lm_step(0, masked=False)                 # prime every row with lm_bos from the zero state
+            lm_step(prog, self.lm_state[0, :Ll], self.lm_state[0, Ll:], masked=False)   # prime with lm_bos from zeros
         for t0 in range(0, T, n):
             prog.append(EbPhase(hist_col=t0, ldw1=min(n, T - t0), **sel))
             if self.lm:                              # survivors inherit their parent's LM state, extensions step it
                 p, q = t0 & 1, 1 - (t0 & 1)
                 prog.append(EbPhase(type=PH_GATHER, S=R, N=Hl, aux=2 * Ll, x1=_ptr(self.lm_state[p]),
                                     y=_ptr(self.lm_state[q]), src=_ptr(self.src)))
-                lm_step(q, masked=True)
+                lm_step(prog, self.lm_state[q, :Ll], self.lm_state[q, Ll:], masked=True)
         prog.append(EbPhase(type=PH_BEAM_FINAL, S=B, aux=W, aux2=blank, y=_ptr(self.score), hist=_ptr(self.hist),
                             hist_ld=T, tok_out=_ptr(self.ids), ldy=T, y2=_ptr(self.nlogp)))
         self.nphase = len(prog)
@@ -1069,8 +1013,7 @@ class CTCBeamEngine:
         if self.lm:
             self.lm_state[0].zero_()
             self.lm_tok.fill_(self.lm_bos)
-        check(lib().eb_decode_run_ctc(self._prog.data_ptr(), self.nphase, self._bar.data_ptr(), self.max_ctas,
-                                      torch.cuda.current_stream().cuda_stream), "eb_decode_run_ctc")
+        _launch("eb_decode_run_ctc", self._prog, self.nphase, self._bar, self.max_ctas)
         return self.ids, self.nlogp
 
     def hypotheses(self, b):
@@ -1083,7 +1026,7 @@ class CTCBeamEngine:
                  float(st[2, j])) for j in range(live)]
 
 
-class CTCStreamEngine:
+class CTCStreamEngine(_ChunkEngine):
     """Streaming greedy CTC decoding of a ``CTCEncoder`` (rnnt/models.py:272-310): S streams, one persistent kernel
     launch per chunk (eb_decode_run_ctc_stream).  The chunk program is encoder_phases' GRU encoder (LayerNorm, per layer
     n GRU cell steps from the carried h, residual LayerNorm, time reduction), the projection, the ``tovocab`` Linear
@@ -1099,32 +1042,23 @@ class CTCStreamEngine:
     The carried state is ``enc_h`` [L, S, H], the previous frame's argmax ``prev`` [S] (-1 after ``reset``: it matches
     no token) and the running score ``score`` (fp64 on the device).  ``state()`` / ``load_state()`` move it to an engine
     rebuilt for another chunk length or for re-homed weights (``fingerprint``)."""
+    GRU = True
+    RUN = "eb_decode_run_ctc_stream"
+
     def __init__(self, ctc_model, n_streams, frames_per_chunk, blank=0, max_ctas=0, state=None):
         from .rnnt.models import CTCEncoder
         if not isinstance(ctc_model, CTCEncoder):
             raise TypeError("CTCStreamEngine streams a CTCEncoder, got %s" % type(ctc_model).__name__)
-        S, n, blank = operator.index(n_streams), operator.index(frames_per_chunk), operator.index(blank)
-        if S < 1 or n < 1:
-            raise ValueError("n_streams and frames_per_chunk must be positive, got %d and %d" % (S, n))
         enc, lin = ctc_model.model, ctc_model.tovocab[0]
-        V = lin.weight.shape[0]
+        S, n, T = self._check_shape(enc, n_streams, frames_per_chunk)
+        V, blank = lin.weight.shape[0], operator.index(blank)
         if not 0 <= blank < V:
             raise ValueError("blank must lie in [0, %d), got %d" % (V, blank))
-        T = stream_frames_out(enc, n)
-        if T < 1:
-            raise ValueError("a chunk of %d frames gives no encoder output frame" % n)
-        self.dev = lin.weight.device
-        if self.dev.type != "cuda":
-            raise RuntimeError("CTCStreamEngine needs the model on a CUDA device")
-        assert C.sizeof(EbPhase) == lib().eb_decode_phase_size(), "EbPhase layout mismatch"
         i32 = torch.int32
         self.S, self.n, self.V, self.blank, self.max_ctas = S, n, V, blank, max_ctas
-        self._keep = [p.detach() for p in ctc_model.parameters()]       # weights are read in place
-        self.fingerprint = param_fingerprint(ctc_model)
         prog = []
-        E = encoder_phases(prog, self, enc, S, n)
-        assert self.n_out == T and lin.weight.shape[1] == E
-        L, H = self.enc_h.shape[0], self.enc_h.shape[2]
+        E = self._build_encoder(prog, ctc_model, enc, S, n, T)
+        assert lin.weight.shape[1] == E
         z = lambda *shape, dtype=torch.float32: torch.zeros(*shape, dtype=dtype, device=self.dev)
         self.logits, self.logprobs = z(S * T, V), z(S * T, V)
         self.argmax = z(S, T, dtype=i32)                        # every frame's argmax (CTC_EMIT's seq_out)
@@ -1136,33 +1070,10 @@ class CTCStreamEngine:
         prog.append(EbPhase(type=PH_CTC_EMIT, S=S, N=V, aux=T, aux2=blank, x1=_ptr(self.logits), ldx1=V,
                             y=_ptr(self.logprobs), ldy=V, tok_out=_ptr(self.prev), hist=_ptr(self._out), hist_ld=T,
                             tok_out2=_ptr(self._out, S * T), y2=_ptr(self._score), seq_out=_ptr(self.argmax)))
-        prog.append(EbPhase(type=PH_COPY, S=L * S, N=H, x1=_ptr(self.enc_htmp), y=_ptr(self.enc_h)))
-        self.n_chunk_phases = len(prog)
-        self._chunk = _upload(prog, self.dev)
-        self._bar = torch.zeros(64, dtype=i32, device=self.dev)
-        if state is None:
-            self.reset()
-        else:
-            self.load_state(state)
+        self._finish(prog, state)
 
     def _state_views(self):
-        return dict(enc_h=self.enc_h, prev=self.prev, score=self._score)
-
-    def state(self):
-        """Every stream's carried state (encoder h, previous argmax, running score) as a dict of device tensors."""
-        return {k: t.clone() for k, t in self._state_views().items()}
-
-    @torch.no_grad()
-    def load_state(self, st):
-        """Continue from ``state()`` of an engine over the same model and n_streams, with any chunk length."""
-        views = self._state_views()
-        if set(st) != set(views):
-            raise ValueError("state keys %s do not match this engine's %s" % (sorted(st), sorted(views)))
-        for k, t in views.items():
-            if tuple(st[k].shape) != tuple(t.shape):
-                raise ValueError("state %s has shape %s, this engine needs %s (same model and n_streams)"
-                                 % (k, tuple(st[k].shape), tuple(t.shape)))
-            t.copy_(st[k])
+        return dict(super()._state_views(), prev=self.prev, score=self._score)
 
     @torch.no_grad()
     def reset(self):
@@ -1182,10 +1093,6 @@ class CTCStreamEngine:
         host: row s holds in its first counts[s] entries the ids stream s emitted in this chunk.  One device-to-host
         copy per chunk."""
         self.xin.copy_(chunk, non_blocking=True)
-        check(lib().eb_decode_run_ctc_stream(self._chunk.data_ptr(), self.n_chunk_phases, self._bar.data_ptr(),
-                                             self.max_ctas, torch.cuda.current_stream().cuda_stream),
-              "eb_decode_run_ctc_stream")
-        self._host.copy_(self._out, non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        S, T = self.S, self.n_out
-        return self._host[:S * T].view(S, T).clone(), self._host[S * T:].clone()
+        self._run(self._chunk, self.n_chunk_phases)
+        ids, counts, _ = self._fetch(self.n_out)
+        return ids, counts

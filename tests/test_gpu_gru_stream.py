@@ -275,6 +275,10 @@ def test_greedy_state_survives_rebuilds_and_refuses_the_other_kind():
         eng.load_state(lstm.state())
     with pytest.raises(ValueError, match="state keys"):
         GRUStreamEngine(m, 1, 2, state=lstm.state())
+    with pytest.raises(ValueError, match="has shape"):     # one stream's state is not broadcast to four
+        StreamEngine(lstm_tiny()[0], 4, 2, state=lstm.state())
+    with pytest.raises(ValueError, match="has shape"):
+        GRUStreamEngine(m, 4, 2).load_state(eng.state())
 
 
 @pytest.mark.parametrize("with_lm", [False, True])

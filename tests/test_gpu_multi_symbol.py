@@ -105,6 +105,8 @@ def test_max_symbols_checked_before_device_work():
             PytorchStreamDecoder(None, transducer=m, transform=lambda f: f, tokenizer=object(), device="cpu",
                                  max_symbols=bad)
     assert check_max_symbols(1) == 1 and check_max_symbols(np.int64(16)) == 16
+    with pytest.raises(RuntimeError, match="CUDA"):           # the arguments are fine: the device is what is missing
+        GreedyEngine(m, 1, 2)
     with pytest.raises(ValueError):
         PytorchStreamDecoder(None, transducer=m, transform=lambda f: f, tokenizer=object(), device="cpu",
                              beam_width=4, max_symbols=2)

@@ -45,22 +45,23 @@ class Tok:
 
 # ---- refusals --------------------------------------------------------------------------------------------------------
 def test_greedy_engine_refusals_come_before_any_device_work():
-    from edgedict_b200.stream_engine import GRUStreamEngine
+    """GRUStreamEngine, and StreamEngine on an LSTM encoder with the same checks in the same order."""
+    from edgedict_b200.stream_engine import GRUStreamEngine, StreamEngine
     cuda_before = torch.cuda.is_initialized()
-    gru = _cpu()
-    with pytest.raises(ValueError, match="GRU encoder"):
-        GRUStreamEngine(_cpu("LSTM"), 1, 2)
-    for S, n in ((0, 2), (-1, 2), (2, 0), (2, -2)):
-        with pytest.raises(ValueError, match="positive"):
-            GRUStreamEngine(gru, S, n)
-    for n in (1, 3, 7):                                   # the time reduction after layer 1 pairs frames
-        with pytest.raises(ValueError, match="even number of frames"):
-            GRUStreamEngine(gru, 2, n)
-    for K in (0, 17):
-        with pytest.raises(ValueError, match="max_symbols"):
-            GRUStreamEngine(gru, 2, 2, max_symbols=K)
-    with pytest.raises(RuntimeError, match="CUDA"):        # a CPU model, every other argument valid
-        GRUStreamEngine(gru, 2, 4)
+    for engine, model, other in ((GRUStreamEngine, _cpu(), "GRU"), (StreamEngine, _cpu("LSTM"), "LSTM")):
+        with pytest.raises(ValueError, match=other + " encoder"):
+            engine(_cpu("LSTM" if other == "GRU" else "GRU"), 1, 2)
+        for S, n in ((0, 2), (-1, 2), (2, 0), (2, -2)):
+            with pytest.raises(ValueError, match="positive"):
+                engine(model, S, n)
+        for n in (1, 3, 7):                               # the time reduction after layer 1 pairs frames
+            with pytest.raises(ValueError, match="even number of frames"):
+                engine(model, 2, n)
+        for K in (0, 17):
+            with pytest.raises(ValueError, match="max_symbols"):
+                engine(model, 2, 2, max_symbols=K)
+        with pytest.raises(RuntimeError, match="CUDA"):    # a CPU model, every other argument valid
+            engine(model, 2, 4)
     assert torch.cuda.is_initialized() == cuda_before
 
 
