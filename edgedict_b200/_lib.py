@@ -19,12 +19,16 @@ SIGNATURES = {
     "eb_rnnt_loss_bwd_bf16": (I, [P, P, P, P, P, I, I, I, I, I, P, P, I, D, P]),
     "eb_joint_logits_lse": (I, [P, P, P, P, P, P, P, P, P, P, I, I, I, I, I, I, P]),
     "eb_rnnt_workspace_views": (I, [P, I, I, I, I, P, P, P, P, P]),
+    "eb_rnnt_align_bytes": (Z, [I, I, I]),
+    "eb_rnnt_viterbi": (I, [P, P, I, I, I, I, P, P, P, P, P, P]),
     "eb_log_softmax_fwd": (I, [P, P, L, I, P]),
     "eb_log_softmax_bwd": (I, [P, P, P, L, I, P]),
     "eb_ctc_workspace_size": (Z, [I, I, I]),
     "eb_ctc_loss_fwd": (I, [P, L, L, I, I, I, P, L, P, P, P, I, I, I, P, P, P]),
     "eb_ctc_loss_bwd": (I, [P, L, L, P, L, L, I, I, I, P, P, I, I, I, P, P, P]),
     "eb_ctc_greedy": (I, [P, L, L, I, I, I, P, I, P, P, P, P]),
+    "eb_ctc_align_workspace_size": (Z, [I, I, I]),
+    "eb_ctc_align": (I, [P, L, L, I, I, I, P, L, P, P, P, I, I, P, P, P, P]),
     "eb_gemm_f32": (I, [P, L, L, P, L, L, P, L, P, I, I, I, F, F, P]),
     "eb_gemm_bf16": (I, [P, I, P, I, P, I, P, I, L, I, L, P]),
     "eb_gemm_bf16_ex": (I, [P, I, P, I, P, I, P, I, L, I, L, I, P, L, P]),

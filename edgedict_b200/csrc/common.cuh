@@ -61,6 +61,20 @@ __device__ __forceinline__ T warp_sum(T v) {
     return v;
 }
 
+// n bytes from global to shared memory by threads tid = 0 .. nt-1, sixteen independent loads in flight per thread
+// before their stores (a plain byte loop waits out one global load latency per byte it copies)
+__device__ __forceinline__ void block_copy_bytes(unsigned char* dst, const unsigned char* src, int n, int tid, int nt) {
+    constexpr int K = 16;
+    for (int i0 = tid; i0 < n; i0 += K * nt) {
+        unsigned char r[K];
+#pragma unroll
+        for (int k = 0; k < K; ++k) r[k] = i0 + k * nt < n ? src[i0 + k * nt] : 0;
+#pragma unroll
+        for (int k = 0; k < K; ++k)
+            if (i0 + k * nt < n) dst[i0 + k * nt] = r[k];
+    }
+}
+
 // block-wide sum for blockDim.x <= 1024 (result valid in every thread)
 template <typename T>
 __device__ __forceinline__ T block_sum(T v, T* sh /* >= 33 entries */) {

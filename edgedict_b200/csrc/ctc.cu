@@ -12,6 +12,8 @@
 //                                  one label summed in increasing s (the lattice kernel links them)
 //   5. ctc_greedy_kernel           one CTA per utterance: per-frame argmax, repeats and blanks dropped, the reference's
 //                                  whole-row score
+//   ctc_viterbi_kernel             forced alignment: the alpha recurrence of 3. with max in place of log-add, one
+//                                  back-pointer byte per (t, s), then the backtrace in the same CTA
 //
 // Arithmetic follows torch's CPU ctc_loss (aten/src/ATen/native/LossCTC.cpp): alpha and beta include the frame's
 // emission, a step log-adds its (up to) three predecessors around their maximum, nll = -log p from alpha.  The lattice
@@ -214,6 +216,146 @@ ctc_lattice_kernel(const float* __restrict__ lp, long sn, long st, int T, int V,
 }
 
 // ---------------------------------------------------------------------------------------------
+// 3b. Viterbi alignment: the alpha recurrence of ctc_lattice_kernel with max in place of log-add, in fp64, and one
+//     back-pointer byte per (t, s): how many states back the best predecessor lies (0, 1 or 2).  Predecessors are
+//     taken in the order s, s-1, s-2, a later one replacing the current only when strictly greater.  At the last frame
+//     the last label state L-2 wins unless the final blank L-1 is strictly greater.  Then one thread walks the
+//     back-pointers and writes alignment[b, t]; every thread fills frame_logp[b, t] from it.  grid = N; the
+//     back-pointers live in shared memory after the states when bp == nullptr, else at bp + b*T*Lmax.
+// ---------------------------------------------------------------------------------------------
+template <int SLOTS>
+__global__ void __launch_bounds__(512, 1)
+ctc_viterbi_kernel(const float* __restrict__ lp, long sn, long st, int T, int V, const int* __restrict__ targets,
+                   long ntargets, const int* __restrict__ tg_off, const int* __restrict__ tg_len,
+                   const int* __restrict__ in_len, int S, int blank, unsigned char* __restrict__ bp_global,
+                   int rows, int* __restrict__ alignment, float* __restrict__ frame_logp) {
+    extern __shared__ double sm[];
+    const int Lmax = 2 * S + 1;
+    double* buf = sm;                                    // [2][Lmax]
+    int* lab = reinterpret_cast<int*>(sm + 2 * Lmax);   // [Lmax]
+    int* ctl = lab + Lmax;                               // [4]: feasible, walk, t, s (no static shared memory)
+    unsigned char* stage = reinterpret_cast<unsigned char*>(ctl + 4);   // [rows][Lmax] back-pointer bytes
+    unsigned char* bp = bp_global ? bp_global + (long)blockIdx.x * T * Lmax : stage;
+    const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+    int Tb, L;
+    ctc_lens(in_len, tg_len, b, T, S, Tb, L);
+    const long off = tg_off[b];
+    for (int s = tid; s < L; s += nt) {
+        int c = blank;
+        if (s & 1) {
+            const long i = off + (s >> 1);
+            c = (i >= 0 && i < ntargets) ? targets[i] : -1;
+        }
+        lab[s] = c;
+    }
+    __syncthreads();
+    int col[SLOTS];
+    bool skip[SLOTS];
+#pragma unroll
+    for (int k = 0; k < SLOTS; ++k) {
+        const int s = tid + k * nt;
+        const int c = s < L ? lab[s] : -1;
+        col[k] = (c >= 0 && c < V) ? c : -1;
+        skip[k] = s < L && (s & 1) && s >= 2 && lab[s] != lab[s - 2];
+    }
+    const float* row0 = lp + (long)b * sn;
+#define CTC_EMIT(k, n) ((col[k] >= 0 && (n) < Tb) ? __ldg(row0 + (long)(n) * st + col[k]) : -INFINITY)
+    float e[SLOTS][CTC_PF], en[SLOTS][CTC_PF];
+#pragma unroll
+    for (int k = 0; k < SLOTS; ++k)
+#pragma unroll
+        for (int i = 0; i < CTC_PF; ++i) e[k][i] = CTC_EMIT(k, i);
+    for (int n0 = 0; n0 < Tb; n0 += CTC_PF) {
+#pragma unroll
+        for (int k = 0; k < SLOTS; ++k)
+#pragma unroll
+            for (int i = 0; i < CTC_PF; ++i) en[k][i] = CTC_EMIT(k, n0 + CTC_PF + i);
+#pragma unroll
+        for (int i = 0; i < CTC_PF; ++i) {
+            const int n = n0 + i;
+            if (n >= Tb) break;                          // uniform across the CTA
+            const double* pv = buf + ((n - 1) & 1) * Lmax;
+            double* cur = buf + (n & 1) * Lmax;
+#pragma unroll
+            for (int k = 0; k < SLOTS; ++k) {
+                const int s = tid + k * nt;
+                if (s >= L) continue;
+                double v;
+                if (n == 0) {
+                    v = (s <= 1) ? (double)e[k][i] : -INFINITY;
+                } else {
+                    double best = pv[s];
+                    int back = 0;
+                    if (s >= 1 && pv[s - 1] > best) { best = pv[s - 1]; back = 1; }
+                    if (skip[k] && pv[s - 2] > best) { best = pv[s - 2]; back = 2; }
+                    v = best + (double)e[k][i];
+                    bp[(long)n * Lmax + s] = (unsigned char)back;
+                }
+                cur[s] = v;
+            }
+            __syncthreads();
+        }
+#pragma unroll
+        for (int k = 0; k < SLOTS; ++k)
+#pragma unroll
+            for (int i = 0; i < CTC_PF; ++i) e[k][i] = en[k][i];
+    }
+#undef CTC_EMIT
+    int* al = alignment + (long)b * T;
+    float* fl = frame_logp + (long)b * T;
+    if (tid == 0) {
+        bool ok = Tb > 0;
+        int s = 0;
+        if (ok) {
+            const double* last = buf + ((Tb - 1) & 1) * Lmax;
+            s = L - 1;
+            if (L >= 2 && !(last[L - 1] > last[L - 2])) s = L - 2;
+            ok = last[s] > -INFINITY;
+        }
+        ctl[0] = ok || (Tb == 0 && L == 1);              // an empty input aligns only the empty target
+        ctl[1] = ok;
+        ctl[2] = Tb - 1;
+        ctl[3] = s;
+    }
+    __syncthreads();
+    const int ok = ctl[0];
+    // Backtrace by thread 0 over the back-pointers in shared memory.  When they are in the caller's buffer
+    // (rows < T), the CTA first copies the band of the `rows` frames at and below the current t into shared memory, so
+    // the walk makes no dependent global load; a band's frames are contiguous bytes.  t is the same in every thread.
+    int t = ctl[1] ? ctl[2] : -1;
+    while (t >= 0) {
+        const int lo = max(0, t - rows + 1);
+        if (bp_global) {
+            block_copy_bytes(stage, bp + (long)lo * Lmax, (t - lo + 1) * Lmax, tid, nt);
+            __syncthreads();
+        }
+        if (tid == 0) {
+            int s = ctl[3];
+            for (; t >= lo; --t) {
+                al[t] = lab[s];
+                if (t > 0) s -= stage[(t - lo) * Lmax + s];
+            }
+            ctl[2] = t;
+            ctl[3] = s;
+        }
+        __syncthreads();
+        t = ctl[2];
+        __syncthreads();                                 // every thread has read t before the next band
+    }
+    for (int t = tid; t < T; t += nt) {
+        if (!ok) {
+            al[t] = -1;
+            fl[t] = -INFINITY;
+        } else if (t < Tb) {
+            fl[t] = __ldg(row0 + (long)t * st + al[t]);
+        } else {
+            al[t] = -1;
+            fl[t] = 0.f;
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
 // 4. gradient
 // ---------------------------------------------------------------------------------------------
 template <int THREADS>
@@ -400,6 +542,63 @@ EB_API int eb_ctc_loss_bwd(const float* log_probs, long stride_n, long stride_t,
     ctc_grad_kernel<THREADS><<<dim3(T, N), THREADS, 0, (cudaStream_t)stream>>>(
         log_probs, stride_n, stride_t, grad, grad_stride_n, grad_stride_t, T, V, target_lengths, input_lengths, S,
         zero_infinity, w, gscale);
+    EB_CHECK_LAUNCH();
+    return EB_OK;
+}
+
+namespace {
+
+constexpr size_t ALIGN_SMEM_MAX = 227 * 1024;           // opt-in dynamic shared memory per CTA on sm_90
+
+// frames of back-pointers the backtrace stages at a time when they do not all fit in shared memory
+constexpr size_t ALIGN_STAGE_BYTES = 64 * 1024;
+
+// dynamic shared memory of ctc_viterbi_kernel: states [2][Lmax] doubles, labels [Lmax] ints, four control ints and
+// [rows][Lmax] back-pointer bytes: all T frames when they fit (the back-pointers then live there), else a staging band
+// of the caller's buffer.  The kernel has no static shared memory, so the whole opt-in limit is available to this
+// buffer.
+inline size_t ctc_viterbi_smem(int T, int S, int* rows) {
+    const size_t L = 2 * (size_t)S + 1;
+    const size_t fixed = L * (2 * sizeof(double) + sizeof(int)) + 4 * sizeof(int);
+    *rows = fixed + (size_t)T * L <= ALIGN_SMEM_MAX ? T : (int)(ALIGN_STAGE_BYTES / L);
+    return fixed + (size_t)*rows * L;
+}
+
+}  // namespace
+
+EB_API size_t eb_ctc_align_workspace_size(int B, int T, int S) {
+    if (B <= 0 || T < 0 || S < 0 || S > CTC_MAX_S) return 0;
+    int rows;
+    ctc_viterbi_smem(T, S, &rows);
+    return rows == T ? 0 : (size_t)B * T * (2 * (size_t)S + 1);
+}
+
+EB_API int eb_ctc_align(const float* log_probs, long stride_b, long stride_t, int B, int T, int V, const int* targets,
+                        long ntargets, const int* tg_off, const int* tg_len, const int* in_len, int S, int blank,
+                        void* workspace, int* alignment, float* frame_logp, void* stream) {
+    if (!log_probs || !tg_off || !tg_len || !in_len || !alignment || !frame_logp || B <= 0 || B > 65535 || T < 0 ||
+        V <= 0 || S < 0 || S > CTC_MAX_S || blank < 0 || blank >= V || ntargets < 0 || (!targets && ntargets > 0) ||
+        stride_b < 0 || stride_t < 0)
+        return EB_ERR_INVALID;
+    int rows;
+    const size_t smem = ctc_viterbi_smem(T, S, &rows);
+    const bool in_smem = rows == T;
+    if (!in_smem && !workspace) return EB_ERR_INVALID;
+    if (T == 0) return EB_OK;
+    unsigned char* bp = in_smem ? nullptr : reinterpret_cast<unsigned char*>(workspace);
+    const int Lmax = 2 * S + 1;
+    const int slots = Lmax <= 1024 ? 2 : 4;
+    const int threads = ((Lmax + slots - 1) / slots + 31) / 32 * 32;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (Lmax <= 1024) {
+        EB_CUDA(cudaFuncSetAttribute(ctc_viterbi_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ctc_viterbi_kernel<2><<<B, threads, smem, st>>>(log_probs, stride_b, stride_t, T, V, targets, ntargets, tg_off,
+                                                        tg_len, in_len, S, blank, bp, rows, alignment, frame_logp);
+    } else {
+        EB_CUDA(cudaFuncSetAttribute(ctc_viterbi_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ctc_viterbi_kernel<4><<<B, threads, smem, st>>>(log_probs, stride_b, stride_t, T, V, targets, ntargets, tg_off,
+                                                        tg_len, in_len, S, blank, bp, rows, alignment, frame_logp);
+    }
     EB_CHECK_LAUNCH();
     return EB_OK;
 }

@@ -12,6 +12,9 @@
 //                          (fp32 or bf16, optionally in place), zero on padded cells, scaled
 //                          by the upstream gradient on the device               (2*s*N bytes)
 //
+// and, for forced alignment, rnnt_viterbi_kernel: the alpha wavefront with max in place of
+// log-add and a decision byte per cell, then the backtrace in the same CTA (eb_rnnt_viterbi).
+//
 // No host synchronisation anywhere except in the warp-transducer compatible entry point
 // compute_rnnt_loss(), whose contract returns costs in HOST memory (include/rnnt.h).
 //
@@ -241,6 +244,116 @@ __global__ void rnnt_lattice_kernel(const T* __restrict__ lpb, const T* __restri
             for (int i = 0; i < PF; ++i) { cb[i] = nb[i]; cl[i] = nl[i]; }
         }
         if (u == 0) ll_bwd[b] = self;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// 2b. Viterbi alignment: the alpha wavefront with max in place of log-add, in fp64, one decision
+//    byte per cell (1: emit, 0: stay; an exact tie takes stay), then a backtrace in the same CTA.
+//    grid = B, blockDim.x = maxU rounded up to a warp.  The decisions live in shared memory after
+//    the two delta diagonals when dec == nullptr (rows == maxT), else at dec + b*maxT*maxU and the
+//    backtrace stages them `rows` rows at a time; row stride maxU.
+// ---------------------------------------------------------------------------------------------
+template <typename T, int PF>
+__global__ void __launch_bounds__(1024) rnnt_viterbi_kernel(const T* __restrict__ lpb, const T* __restrict__ lpl,
+                                    const int* __restrict__ xlen, const int* __restrict__ ylen,
+                                    unsigned char* __restrict__ dec_global, int* __restrict__ frames,
+                                    T* __restrict__ label_logp, T* __restrict__ score, int maxT, int maxU,
+                                    int rows) {
+    extern __shared__ double dsm[];
+    const int W = blockDim.x;
+    double* sh = dsm;                                    // [2][W] delta of the last two diagonals
+    int* fr = reinterpret_cast<int*>(dsm + 2 * W);       // [W] frame of each label, from the backtrace
+    int* pos = fr + W;                                   // [2] the backtrace's (t, u) between bands
+    unsigned char* stage = reinterpret_cast<unsigned char*>(pos + 2);   // [rows][maxU] decision bytes
+    const int b = blockIdx.x, u = threadIdx.x;
+    const int Tn = min(max(xlen[b], 0), maxT), Un = min(max(ylen[b], 0) + 1, maxU);
+    const long base = (long)b * maxT * maxU;
+    unsigned char* dec = dec_global ? dec_global + base : stage;
+    const T* pb = lpb + base;
+    const T* pl = lpl + base;
+    const int ND = Tn + Un - 1;
+    const bool act = u < Un;
+    double self = -INFINITY;                             // delta(t-1,u)
+    T cb[PF], cl[PF], nb[PF], nl[PF];
+#pragma unroll
+    for (int i = 0; i < PF; ++i) {
+        int t = i - u;
+        cb[i] = (act && t >= 1 && t < Tn) ? pb[(long)(t - 1) * maxU + u] : T(0);
+        cl[i] = (act && u >= 1 && t >= 0 && t < Tn) ? pl[(long)t * maxU + u - 1] : T(0);
+    }
+    for (int n0 = 0; n0 < ND; n0 += PF) {
+#pragma unroll
+        for (int i = 0; i < PF; ++i) {
+            int t = n0 + PF + i - u;
+            nb[i] = (act && t >= 1 && t < Tn) ? pb[(long)(t - 1) * maxU + u] : T(0);
+            nl[i] = (act && u >= 1 && t >= 0 && t < Tn) ? pl[(long)t * maxU + u - 1] : T(0);
+        }
+#pragma unroll
+        for (int i = 0; i < PF; ++i) {
+            const int n = n0 + i;
+            if (n < ND) {
+                const int t = n - u;
+                if (act && t >= 0 && t < Tn) {
+                    double d = 0.0;
+                    if (n > 0) {
+                        const double stay = (t > 0) ? self + (double)cb[i] : -INFINITY;
+                        const double emit = (u > 0) ? sh[((n - 1) & 1) * W + u - 1] + (double)cl[i] : -INFINITY;
+                        const bool e = emit > stay;
+                        d = e ? emit : stay;
+                        dec[(long)t * maxU + u] = e;
+                    }
+                    self = d;
+                    sh[(n & 1) * W + u] = d;
+                }
+            }
+            __syncthreads();
+        }
+#pragma unroll
+        for (int i = 0; i < PF; ++i) { cb[i] = nb[i]; cl[i] = nl[i]; }
+    }
+    if (u == 0) {
+        if (Tn == 0) {
+            score[b] = T(-INFINITY);
+        } else {
+            // self of thread 0 is delta(Tn-1, 0); the corner's delta sits in the last diagonal's buffer
+            const double last = sh[((ND - 1) & 1) * W + Un - 1];
+            score[b] = (T)(last + (double)pb[(long)(Tn - 1) * maxU + Un - 1]);
+        }
+    }
+    // Backtrace by thread 0 over the decisions in shared memory.  When they are in the caller's buffer (rows < maxT),
+    // the CTA first copies the band of the `rows` rows at and below the current t into shared memory, so the walk
+    // makes no dependent global load; a band's rows are contiguous bytes.  t and u are the same in every thread.
+    int t = Tn - 1, v = Tn > 0 ? Un - 1 : 0;
+    while (v > 0) {
+        const int lo = max(0, t - rows + 1);
+        if (dec_global) {
+            block_copy_bytes(stage, dec + (long)lo * maxU, (t - lo + 1) * maxU, u, W);
+            __syncthreads();
+        }
+        if (u == 0) {
+            while (v > 0 && t >= lo) {                   // at t == 0 only emit is possible
+                if (t == 0 || stage[(t - lo) * maxU + v]) fr[--v] = t;
+                else --t;
+            }
+            pos[0] = t;
+            pos[1] = v;
+        }
+        __syncthreads();
+        t = pos[0];
+        v = pos[1];
+        __syncthreads();                                 // every thread has read pos before the next band
+    }
+    __syncthreads();
+    for (int k = u; k < maxU - 1; k += W) {
+        const long o = (long)b * (maxU - 1) + k;
+        if (k < Un - 1 && Tn > 0) {
+            frames[o] = fr[k];
+            label_logp[o] = pl[(long)fr[k] * maxU + k];
+        } else {
+            frames[o] = -1;
+            label_logp[o] = (k < Un - 1) ? T(-INFINITY) : T(0);
+        }
     }
 }
 
@@ -630,6 +743,63 @@ EB_API int eb_rnnt_loss_lattice(const int* xlen, const int* ylen, int B, int max
     if (costs_dev) neg_copy_kernel<float><<<(B + 127) / 128, 128, 0, st>>>(w.ll_fwd, costs_dev, B);
     EB_CHECK_LAUNCH();
     return EB_OK;
+}
+
+namespace {
+
+constexpr size_t ALIGN_SMEM_MAX = 227 * 1024;           // opt-in dynamic shared memory per CTA on sm_90
+// frames of the prefetch ring: 1024 threads leave 64 registers each, which eight fp64 pairs in flight would overrun
+template <typename T> constexpr int VITERBI_PF = sizeof(T) == 8 ? 4 : 8;
+
+// rows of decisions the backtrace stages at a time when they do not all fit in shared memory
+constexpr size_t ALIGN_STAGE_BYTES = 64 * 1024;
+
+// dynamic shared memory of rnnt_viterbi_kernel: delta [2][W] doubles, frames [W] ints, (t, u) and [rows][maxU] decision
+// bytes: all maxT rows when they fit (the decisions then live there), else a staging band of the caller's buffer.  The
+// kernel has no static shared memory, so the whole opt-in limit is available to this buffer.
+inline size_t viterbi_smem(int maxT, int maxU, int* rows) {
+    const size_t W = ((size_t)maxU + 31) / 32 * 32;
+    const size_t fixed = W * (2 * sizeof(double) + sizeof(int)) + 2 * sizeof(int);
+    *rows = fixed + (size_t)maxT * maxU <= ALIGN_SMEM_MAX ? maxT : (int)(ALIGN_STAGE_BYTES / maxU);
+    return fixed + (size_t)*rows * maxU;
+}
+
+template <typename T>
+int viterbi(const int* xlen, const int* ylen, int B, int maxT, int maxU, void* ws, unsigned char* decisions,
+            int* frames, void* label_logp, void* score, cudaStream_t st) {
+    int rows;
+    const size_t smem = viterbi_smem(maxT, maxU, &rows);
+    const bool in_smem = rows == maxT;
+    if (!in_smem && !decisions) return EB_ERR_INVALID;
+    Workspace<T> w(ws, B, maxT, maxU);
+    EB_CUDA(cudaFuncSetAttribute(rnnt_viterbi_kernel<T, VITERBI_PF<T>>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    rnnt_viterbi_kernel<T, VITERBI_PF<T>><<<B, ((maxU + 31) / 32) * 32, smem, st>>>(
+        w.lpb, w.lpl, xlen, ylen, in_smem ? nullptr : decisions, frames, (T*)label_logp, (T*)score, maxT, maxU, rows);
+    EB_CHECK_LAUNCH();
+    return EB_OK;
+}
+
+}  // namespace
+
+EB_API size_t eb_rnnt_align_bytes(int B, int maxT, int maxU) {
+    if (B <= 0 || maxT <= 0 || maxU <= 0 || maxU > 1024) return 0;
+    int rows;
+    viterbi_smem(maxT, maxU, &rows);
+    return rows == maxT ? 0 : (size_t)B * maxT * maxU;
+}
+
+EB_API int eb_rnnt_viterbi(const int* xlen, const int* ylen, int B, int maxT, int maxU, int dtype_size,
+                           const void* workspace, void* decisions, int* frames, void* label_logp, void* score,
+                           void* stream) {
+    if (!xlen || !ylen || !workspace || ((!frames || !label_logp) && maxU > 1) || !score || B <= 0 || maxT <= 0 ||
+        maxU <= 0 || maxU > 1024)
+        return EB_ERR_INVALID;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    void* ws = const_cast<void*>(workspace);
+    unsigned char* dec = reinterpret_cast<unsigned char*>(decisions);
+    if (dtype_size == 4) return viterbi<float>(xlen, ylen, B, maxT, maxU, ws, dec, frames, label_logp, score, st);
+    if (dtype_size == 8) return viterbi<double>(xlen, ylen, B, maxT, maxU, ws, dec, frames, label_logp, score, st);
+    return EB_ERR_INVALID;
 }
 
 // Gradient wrt bf16 logits, written as bf16 (grads16 may alias logits16: in place).

@@ -25,6 +25,7 @@ import torch
 from torch import nn
 
 from . import functional as Fn
+from . import ops
 
 MAX_TARGET_LENGTH = 1023          # 2S+1 lattice states, at most 2047
 
@@ -41,6 +42,33 @@ def _lengths(x, n, name):
     if x.numel() != n:
         raise ValueError("%s must have one entry per utterance (%d), got %d" % (name, n, x.numel()))
     return x
+
+
+def _targets_and_lengths(targets, input_lengths, target_lengths, N, T):
+    """The host checks of the lengths and the target layout -> (input lengths, target lengths, offsets, S)."""
+    il = _lengths(input_lengths, N, "input_lengths")
+    tl = _lengths(target_lengths, N, "target_lengths")
+    if bool((il < 0).any()) or bool((il > T).any()):
+        raise ValueError("input_lengths must lie in [0, T = %d], got %s" % (T, il.tolist()))
+    if bool((tl < 0).any()):
+        raise ValueError("target_lengths must be >= 0, got %s" % tl.tolist())
+    if targets.dim() == 2:
+        if targets.shape[0] != N:
+            raise ValueError("padded targets must have %d rows, got %d" % (N, targets.shape[0]))
+        if bool((tl > targets.shape[1]).any()):
+            raise ValueError("target_lengths exceed the padded target length %d" % targets.shape[1])
+        offsets = torch.arange(N, dtype=torch.int64) * targets.shape[1]
+    elif targets.dim() == 1:
+        if int(tl.sum()) != targets.numel():
+            raise ValueError("concatenated targets hold %d labels, target_lengths sum to %d"
+                             % (targets.numel(), int(tl.sum())))
+        offsets = torch.cumsum(tl, 0) - tl
+    else:
+        raise ValueError("targets must be (N, S) or 1-D, got shape %s" % (tuple(targets.shape),))
+    S = int(tl.max())
+    if S > MAX_TARGET_LENGTH:
+        raise ValueError("target lengths above %d are not supported, got %d" % (MAX_TARGET_LENGTH, S))
+    return il, tl, offsets, S
 
 
 def ctc_loss(log_probs, targets, input_lengths, target_lengths, blank=0, reduction="mean", zero_infinity=False):
@@ -67,28 +95,7 @@ def ctc_loss(log_probs, targets, input_lengths, target_lengths, blank=0, reducti
     blank = operator.index(blank)
     if not 0 <= blank < V:
         raise ValueError("blank must lie in [0, %d), got %d" % (V, blank))
-    il = _lengths(input_lengths, N, "input_lengths")
-    tl = _lengths(target_lengths, N, "target_lengths")
-    if bool((il < 0).any()) or bool((il > T).any()):
-        raise ValueError("input_lengths must lie in [0, T = %d], got %s" % (T, il.tolist()))
-    if bool((tl < 0).any()):
-        raise ValueError("target_lengths must be >= 0, got %s" % tl.tolist())
-    if targets.dim() == 2:
-        if targets.shape[0] != N:
-            raise ValueError("padded targets must have %d rows, got %d" % (N, targets.shape[0]))
-        if bool((tl > targets.shape[1]).any()):
-            raise ValueError("target_lengths exceed the padded target length %d" % targets.shape[1])
-        offsets = torch.arange(N, dtype=torch.int64) * targets.shape[1]
-    elif targets.dim() == 1:
-        if int(tl.sum()) != targets.numel():
-            raise ValueError("concatenated targets hold %d labels, target_lengths sum to %d"
-                             % (targets.numel(), int(tl.sum())))
-        offsets = torch.cumsum(tl, 0) - tl
-    else:
-        raise ValueError("targets must be (N, S) or 1-D, got shape %s" % (tuple(targets.shape),))
-    S = int(tl.max())
-    if S > MAX_TARGET_LENGTH:
-        raise ValueError("target lengths above %d are not supported, got %d" % (MAX_TARGET_LENGTH, S))
+    il, tl, offsets, S = _targets_and_lengths(targets, input_lengths, target_lengths, N, T)
     if not log_probs.is_cuda:                  # checked last: every argument error above is found without a GPU
         raise RuntimeError("edgedict_b200 ctc_loss needs CUDA log_probs (got a %s tensor); there is no CPU path"
                            % log_probs.device)
@@ -119,6 +126,53 @@ class CTCLoss(nn.Module):
     def forward(self, log_probs, targets, input_lengths, target_lengths):
         return ctc_loss(log_probs, targets, input_lengths, target_lengths, self.blank, self.reduction,
                         self.zero_infinity)
+
+
+def forced_align(log_probs, targets, input_lengths, target_lengths, blank=0):
+    """Forced (Viterbi) alignment of known transcripts, batched: torchaudio.functional.forced_align's signature and
+    return, for a whole batch in one kernel launch (csrc/ctc.cu).
+
+      * log_probs: fp32 CUDA tensor [B, T, V] of log-softmax rows, batch first (what ``CTCEncoder.forward`` returns),
+        any strides over B and T.
+      * targets: integer tensor, padded (B, S) or all labels concatenated (sum(target_lengths),), as in ``ctc_loss``;
+        S up to 1023.
+      * input_lengths / target_lengths: integers or integer tensors, one per utterance, read on the host.
+
+    Returns (alignments [B, T] in targets' dtype, scores [B, T] fp32), on the device.  Frame t < input_lengths[b]
+    holds the label (or blank) the best path emits there and its log-prob; later frames hold -1 and 0.  An utterance
+    without any alignment (its input too short for its labels and repeats, or a label outside [0, V)) holds -1 and -inf
+    in every frame.  The path maximises the sum of the frame log-probs, accumulated in fp64; ties between predecessors
+    go to the state itself, then s-1, then s-2, and the path ends in the last label unless the final blank is strictly
+    better (include/edgedict_b200.h, eb_ctc_align).  Arguments are checked on the host before any launch, with
+    ``ctc_loss``'s errors and order; CPU log_probs raise RuntimeError."""
+    if not isinstance(log_probs, torch.Tensor) or not isinstance(targets, torch.Tensor):
+        raise TypeError("log_probs and targets must be tensors")
+    if log_probs.dtype != torch.float32:
+        raise TypeError("edgedict_b200 forced_align takes fp32 log_probs, got %s (there is no fallback)" % log_probs.dtype)
+    if targets.is_floating_point() or targets.is_complex() or targets.dtype == torch.bool:
+        raise TypeError("targets must hold integers, got %s" % targets.dtype)
+    if log_probs.dim() != 3:
+        raise ValueError("log_probs must be [B, T, V], got shape %s" % (tuple(log_probs.shape),))
+    B, T, V = log_probs.shape
+    if T < 1 or B < 1 or V < 1:
+        raise ValueError("log_probs must not be empty, got shape %s" % (tuple(log_probs.shape),))
+    blank = operator.index(blank)
+    if not 0 <= blank < V:
+        raise ValueError("blank must lie in [0, %d), got %d" % (V, blank))
+    il, tl, offsets, S = _targets_and_lengths(targets, input_lengths, target_lengths, B, T)
+    if not log_probs.is_cuda:
+        raise RuntimeError("edgedict_b200 forced_align needs CUDA log_probs (got a %s tensor); there is no CPU path"
+                           % log_probs.device)
+    dev = log_probs.device
+    lens = torch.empty(3, B, dtype=torch.int32, pin_memory=True)
+    lens[0], lens[1], lens[2] = offsets, tl, il
+    lens = lens.to(dev, non_blocking=True)
+    tg = targets.reshape(-1).to(device=dev, dtype=torch.int32).contiguous()
+    if log_probs.stride(-1) != 1:
+        log_probs = log_probs.contiguous()
+    with torch.no_grad():
+        alignment, scores = ops.ctc_align(log_probs, tg, lens[0], lens[1], lens[2], S, blank)
+    return alignment.to(targets.dtype), scores
 
 
 # beam_search keeps the program of its last call (one engine: its log-prob copy [B, T, V], history [B, T, W] x 3,

@@ -688,6 +688,31 @@ class LSTMStack(torch.autograd.Function):
         return (dxin, None, *grads)
 
 
+def _fused_lse(precision, J, U):
+    """bf16 mode takes the softmax statistics from the logits GEMM's epilogue when its tiles allow it."""
+    return precision == "bf16" and FUSE_JOINT_LSE and J % 8 == 0 and U <= 1024
+
+
+def joint_align(h_enc, h_dec, w1, b1, w2, b2, labels, act_lens, label_lens, blank, precision):
+    """Transducer.align's joint: the logits and the loss workspace exactly as JointLoss.forward makes them, then the
+    Viterbi alignment over it (ops.rnnt_viterbi).  The logits are freed before the alignment runs."""
+    B, T, _ = h_enc.shape
+    U = h_dec.shape[1]
+    J = w1.shape[0]
+    _, _, ep, dp = _joint_pre(h_enc, h_dec, w1, b1, precision)
+    hid2 = ops.joint_hidden_fwd(ep, dp, precision == "bf16").view(B * T * U, J)
+    del ep, dp
+    if _fused_lse(precision, J, U):
+        b2a = b2 if (b2.is_contiguous() and b2.data_ptr() % 16 == 0) else b2.clone()
+        logits, ws = ops.joint_logits_lse(hid2, ops.cast_bf16(w2.contiguous()), b2a, labels, act_lens, label_lens,
+                                          B, T, U, blank)
+    else:
+        logits = ops.mm_nt(hid2, w2, b2, precision, x16=hid2 if precision == "bf16" else None).view(B, T, U, -1)
+        _, ws = ops.rnnt_loss_fwd(logits, labels, act_lens, label_lens, blank, need_beta=False)
+    del logits, hid2
+    return ops.rnnt_viterbi(act_lens, label_lens, B, T, U, ws, torch.float32)
+
+
 def _joint_pre(h_enc, h_dec, w1, b1, precision):
     """ep = W1[:, :E] h_enc + b1, dp = W1[:, E:] h_dec  -- exact split of Linear(cat[e, d])."""
     B, T, E = h_enc.shape
@@ -856,7 +881,7 @@ class JointLoss(torch.autograd.Function):
         he2, hd2, ep, dp = _joint_pre(h_enc, h_dec, w1, b1, precision)
         hid = ops.joint_hidden_fwd(ep, dp, precision == "bf16")
         hid2 = hid.view(B * T * U, J)
-        fused = precision == "bf16" and FUSE_JOINT_LSE and J % 8 == 0 and U <= 1024
+        fused = _fused_lse(precision, J, U)
         if fused:
             # bf16 mode: the logits GEMM epilogue also produces the softmax statistics (fp32, from the
             # register accumulators) and writes bf16 logits; the denominator pass over 8 GB disappears

@@ -650,6 +650,21 @@ def rnnt_lattice(xlen, ylen, B, T, U, ws, need_beta=True):
     return costs
 
 
+def rnnt_viterbi(xlen, ylen, B, T, U, ws, dtype):
+    """Forced alignment over a loss workspace of `dtype` (fp32 / fp64) that rnnt_loss_fwd or joint_logits_lse filled.
+    Returns (frames int32 [B, U-1], label_logp [B, U-1], score [B]) on the device (include/edgedict_b200.h)."""
+    dev = ws.device
+    dec = torch.empty(lib().eb_rnnt_align_bytes(B, T, U), dtype=torch.uint8, device=dev)
+    frames = torch.empty(B, U - 1, dtype=torch.int32, device=dev)
+    label_logp = torch.empty(B, U - 1, dtype=dtype, device=dev)
+    score = torch.empty(B, dtype=dtype, device=dev)
+    with _timed("rnnt_viterbi", 1, 0.0, 0.0):
+        check(lib().eb_rnnt_viterbi(_p(xlen), _p(ylen), B, T, U, 8 if dtype == torch.float64 else 4, _p(ws),
+                                    _p(dec) if dec.numel() else None, _p(frames), _p(label_logp), _p(score), _s()),
+              "eb_rnnt_viterbi")
+    return frames, label_logp, score
+
+
 def rnnt_loss_bwd_bf16(logits16, labels, xlen, ylen, blank, ws, gscale, host_scale):
     """In place: logits16 becomes d loss / d logits (bf16)."""
     B, T, U, V = logits16.shape
@@ -715,6 +730,20 @@ def ctc_greedy(lp, xlen, blank):
         check(lib().eb_ctc_greedy(_p(lp), lp.stride(0), lp.stride(1), B, T, V, _p(xlen), blank, _p(out),
                                   _p(out[B * T:]), _p(out[B * T + B:]), _s()), "eb_ctc_greedy")
     return out
+
+
+def ctc_align(lp, targets, offsets, tlen, ilen, S, blank):
+    """lp [B, T, V] fp32 (unit stride over V, any B / T strides); targets / offsets / tlen / ilen as ctc_loss_fwd.
+    Returns (alignment int32 [B, T], frame_logp fp32 [B, T]) on the device (include/edgedict_b200.h)."""
+    B, T, V = lp.shape
+    ws = torch.empty(lib().eb_ctc_align_workspace_size(B, T, S), dtype=torch.uint8, device=lp.device)
+    alignment = torch.empty(B, T, dtype=torch.int32, device=lp.device)
+    frame_logp = torch.empty(B, T, dtype=f32, device=lp.device)
+    with _timed("ctc_align", 1, 4.0 * B * T * (2 * S + 1), 0.0):
+        check(lib().eb_ctc_align(_p(lp), lp.stride(0), lp.stride(1), B, T, V, _p(targets), targets.numel(), _p(offsets),
+                                 _p(tlen), _p(ilen), S, blank, _p(ws) if ws.numel() else None, _p(alignment),
+                                 _p(frame_logp), _s()), "eb_ctc_align")
+    return alignment, frame_logp
 
 
 def adam_step(p, g, m, v, lr, beta1, beta2, eps, weight_decay, step, grad_scale=1.0):

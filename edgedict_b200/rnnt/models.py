@@ -271,6 +271,19 @@ class Transducer(nn.Module):
         return scale_length(logits.shape[1], xlen)
 
     def forward(self, xs, ys, xlen, ylen):
+        h_enc, h_dec = self._encode(xs, ys, xlen, ylen)
+        if not self.output_loss:
+            return self.joint(h_enc, h_dec)
+        xl = _lens_to_device(_i32(scale_length(h_enc.shape[1], xlen)), h_enc.device)
+        yl = _lens_to_device(_i32(ylen), h_enc.device)
+        l0, l2 = self.joint.joint[0], self.joint.joint[2]
+        loss, costs = Fn.JointLoss.apply(h_enc, h_dec, l0.weight, l0.bias, l2.weight, l2.bias,
+                                         _i32(ys[:, :int(ylen.max())]), xl, yl, self.blank, _precision(self))
+        self.last_costs = costs
+        return loss
+
+    def _encode(self, xs, ys, xlen, ylen):
+        """The encoder and the prediction network of forward / align on xs[:, :max xlen] and ys[:, :max ylen]."""
         xs = xs[:, :int(xlen.max())].contiguous()
         ys = ys[:, :int(ylen.max())].contiguous()
         if xs.is_cuda and _PREDICTOR_STREAM:
@@ -289,15 +302,34 @@ class Transducer(nn.Module):
         else:
             h_enc, _ = self.encoder(xs)
             h_dec, _ = self.decoder(ys)
-        if not self.output_loss:
-            return self.joint(h_enc, h_dec)
+        return h_enc, h_dec
+
+    @torch.no_grad()
+    def align(self, xs, ys, xlen, ylen):
+        """Forced alignment of the transcripts ys to the audio xs: the best (Viterbi) path through the RNN-T lattice,
+        which gives the encoder frame at which each label is emitted.  Takes ``forward``'s arguments and runs the
+        encoder, the predictor and the joint as ``forward`` does, following ``set_precision`` / autocast: bf16 mode
+        takes the softmax statistics from the logits GEMM, fp32 mode runs the fp32 logits GEMM and the loss's
+        statistics pass.  Utterance b covers scale_length(xlen)[b] encoder frames, as in the loss.
+
+        Returns (list of B int64 arrays: the frame of each of the ylen[b] labels, non-decreasing; list of B arrays of
+        their log-probs at those frames; -score [B] on the device, the negated log-prob of the best path, which is at
+        least the loss's cost).  On an exact tie a cell takes the blank step (include/edgedict_b200.h, eb_rnnt_viterbi).
+
+        Frames are encoder-output frames, after the time reductions.  Frame f starts at
+        f * 2**len(reductions) * downsample * hop / sample_rate seconds of audio (the feature front end's hop and
+        sample rate, its frame stacking / downsampling factor, and one factor 2 per time reduction of the encoder).
+        The logits are freed on return."""
+        h_enc, h_dec = self._encode(xs, ys, xlen, ylen)
         xl = _lens_to_device(_i32(scale_length(h_enc.shape[1], xlen)), h_enc.device)
         yl = _lens_to_device(_i32(ylen), h_enc.device)
         l0, l2 = self.joint.joint[0], self.joint.joint[2]
-        loss, costs = Fn.JointLoss.apply(h_enc, h_dec, l0.weight, l0.bias, l2.weight, l2.bias,
-                                         _i32(ys), xl, yl, self.blank, _precision(self))
-        self.last_costs = costs
-        return loss
+        frames, logp, score = Fn.joint_align(h_enc, h_dec, l0.weight, l0.bias, l2.weight, l2.bias,
+                                             _i32(ys[:, :int(ylen.max())]), xl, yl, self.blank, _precision(self))
+        frames, logp = frames.cpu().numpy(), logp.cpu().numpy()
+        n = [int(k) for k in ylen]
+        return ([frames[b, :n[b]].astype("int64") for b in range(len(n))], [logp[b, :n[b]] for b in range(len(n))],
+                -score)
 
     @torch.no_grad()
     def greedy_decode(self, xs, xlen, max_symbols=1):
@@ -472,17 +504,30 @@ class CTCEncoder(nn.Module):
         check_lm_args(lm, self.tovocab[0].weight.shape[0], lm_weight, length_bonus, lm_bos, lm_token_map)
         lp = self.forward(xs)
         B, T = lp.shape[0], lp.shape[1]
-        if xlen is None:
-            frames = torch.full((B,), T, dtype=torch.int64)
-        else:
-            xl = torch.as_tensor(xlen).reshape(-1).cpu()
-            if xl.numel() != B:
-                raise ValueError("xlen must have one entry per utterance (%d), got %d" % (B, xl.numel()))
-            frames = torch.zeros(B, dtype=torch.int64)            # scale_length divides by the longest xlen
-            if int(xl.max()) > 0:
-                frames = scale_length(T, xl).clamp(0, T).to(torch.int64)
+        frames = torch.full((B,), T, dtype=torch.int64) if xlen is None else _ctc_frames(T, xlen, B)
         return ctc.beam_search(lp, frames, W, self.blank, lm=lm, lm_weight=lm_weight, length_bonus=length_bonus,
                                lm_bos=lm_bos, lm_token_map=lm_token_map)
+
+    @torch.no_grad()
+    def align(self, xs, ys, xlen, ylen):
+        """Forced alignment of the transcripts ys (padded [B, S] or concatenated, ylen labels each) to the audio xs:
+        ``forward`` (which follows ``set_precision``), then ``edgedict_b200.ctc.forced_align`` over
+        min(T', scale_length(xlen)[b]) log-prob frames, xlen scaled to T' as in ``beam_search``.  Returns
+        (alignments [B, T'] in ys' dtype, per-frame log-probs [B, T'] fp32) on the device; see ``forced_align``."""
+        from .. import ctc
+        lp = self.forward(xs)
+        return ctc.forced_align(lp, ys, _ctc_frames(lp.shape[1], xlen, lp.shape[0]), ylen, self.blank)
+
+
+def _ctc_frames(T, xlen, B):
+    """CTCEncoder's log-prob frames per utterance: xlen (input frames, host) scaled to T' and clamped to [0, T]."""
+    xl = torch.as_tensor(xlen).reshape(-1).cpu()
+    if xl.numel() != B:
+        raise ValueError("xlen must have one entry per utterance (%d), got %d" % (B, xl.numel()))
+    frames = torch.zeros(B, dtype=torch.int64)                    # scale_length divides by the longest xlen
+    if int(xl.max()) > 0:
+        frames = scale_length(T, xl).clamp(0, T).to(torch.int64)
+    return frames
 
 
 def _i32(t):

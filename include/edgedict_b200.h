@@ -40,6 +40,22 @@ int eb_rnnt_loss_bwd_bf16(const void* logits16, void* grads16, const int* labels
                           int gscale_per_batch, double host_scale, void* stream);
 int eb_rnnt_workspace_views(void* workspace, int B, int maxT, int maxU, int dtype_size,
                             void** denom, void** alphas, void** betas, void** ll_fwd, void** ll_bwd);
+/* Forced (Viterbi) alignment over a workspace that eb_rnnt_loss_fwd (any need_beta) or eb_joint_logits_lse filled;
+ * dtype_size 4 or 8 as it was filled, 1 <= maxU <= 1024.  The workspace holds lpb = log p(blank) and lpl =
+ * log p(label u) for cell (b, t, u) at [(b*maxT + t)*maxU + u] of its second and third n = B*maxT*maxU arrays.  With
+ * T = min(xlen[b], maxT), U = min(ylen[b], maxU-1) + 1 and delta in fp64:
+ *   delta(0,0) = 0;  delta(t,u) = max(stay, emit), stay = delta(t-1,u) + lpb(t-1,u), emit = delta(t,u-1) + lpl(t,u-1),
+ *   a term -inf when it leaves the lattice; on an exact tie the cell takes stay.
+ *   score[b] = delta(T-1,U-1) + lpb(T-1,U-1), rounded to the workspace's dtype.
+ * The best path is backtraced from (T-1, U-1): frames [B, maxU-1] int32 holds the frame t at which label u is emitted
+ * (the step (t,u) -> (t,u+1)) and label_logp [B, maxU-1] (workspace dtype) lpl(t,u); past ylen[b] they are -1 and 0
+ * (both may be NULL when maxU = 1).
+ * T = 0 has no alignment: score -inf, frames -1 and label_logp -inf for every label.
+ * decisions: eb_rnnt_align_bytes(B, maxT, maxU) bytes of scratch, NULL allowed when that is 0 (the decisions then stay
+ * in shared memory).  No host synchronisation. */
+size_t eb_rnnt_align_bytes(int B, int maxT, int maxU);
+int eb_rnnt_viterbi(const int* xlen, const int* ylen, int B, int maxT, int maxU, int dtype_size, const void* workspace,
+                    void* decisions, int* frames, void* label_logp, void* score, void* stream);
 
 /* ---- CTC: CTCEncoder's head, loss and greedy decode (csrc/ctc.cu) ------------------------------
  * replaces tovocab's LogSoftmax and greedy_decode of CTCEncoder (rnnt/models.py:272-310) and torch.nn.CTCLoss.
@@ -72,6 +88,20 @@ int eb_ctc_loss_bwd(const float* log_probs, long stride_n, long stride_t, float*
                     int S, int blank, int zero_infinity, const void* workspace, const float* gscale, void* stream);
 int eb_ctc_greedy(const float* log_probs, long stride_b, long stride_t, int B, int T, int V, const int* xlen, int blank,
                   int* ids, int* counts, float* neg_score, void* stream);
+/* eb_ctc_align: forced (Viterbi) alignment.  log_probs [B, T, V] at log_probs[b*stride_b + t*stride_t + v] (strides
+ * >= 0); targets, offsets and lengths as eb_ctc_loss_fwd, 0 <= S <= 1023, lengths clamped the same way.  Over the
+ * extended sequence l' of L = 2*tg_len+1 states, with delta in fp64 and e_t(s) = log_probs[b, t, l'_s]:
+ *   delta_0(s) = e_0(s) for s <= 1;  delta_t(s) = max(delta_{t-1}(s), delta_{t-1}(s-1), delta_{t-1}(s-2) when l'_s is
+ *   a label different from l'_{s-2}) + e_t(s), the predecessors taken in that order, a later one replacing the current
+ *   only when strictly greater.  The path ends in the last label state L-2 unless the final blank L-1 is strictly
+ *   greater.  alignment [B, T] int32 = l'_s of the path's state at frame t and frame_logp [B, T] its log-prob, -1 and 0
+ *   for t >= in_len[b].  An utterance with no alignment (too short for its labels and repeats, a label outside [0, V))
+ *   gets -1 and -inf for every frame.  workspace: eb_ctc_align_workspace_size(B, T, S) bytes of back-pointers, NULL
+ *   allowed when that is 0 (they then stay in shared memory).  No host synchronisation. */
+size_t eb_ctc_align_workspace_size(int B, int T, int S);
+int eb_ctc_align(const float* log_probs, long stride_b, long stride_t, int B, int T, int V, const int* targets,
+                 long ntargets, const int* tg_off, const int* tg_len, const int* in_len, int S, int blank, void* workspace,
+                 int* alignment, float* frame_logp, void* stream);
 
 /* ---- fp32 GEMM (parity mode of every Linear / LSTM input projection) ----------------------
  * replaces the cuBLAS/MKL calls behind nn.Linear and nn.LSTM's input GEMM (rnnt/models.py:45-46,
