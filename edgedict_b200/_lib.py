@@ -78,6 +78,7 @@ SIGNATURES = {
     "eb_decode_run_ctc": (I, [P, I, P, I, P]),
     "eb_decode_run_ctc_stream": (I, [P, I, P, I, P]),
     "eb_decode_run_gru_rnnt": (I, [P, I, P, I, P]),
+    "eb_decode_run_ctc_stream_beam": (I, [P, I, P, I, P]),
     "eb_colsum": (I, [P, I, P, L, I, P]),
     "eb_cast_bf16": (I, [P, P, L, P]),
     "eb_transpose_to_bf16": (I, [P, I, P, L, L, P]),

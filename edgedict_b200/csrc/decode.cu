@@ -486,10 +486,12 @@ __device__ __noinline__ void phase_ctc_emit(const EbPhase& p) {
 //     -1, tok_out2 LM token per row (-1 where the LM rests, its masked step's sentinel).
 //   BEAM_FINAL (S = B, aux = W, aux2 = blank): y slot log p; hist; tok_out ids [B][ldy], the non-blank tokens of the
 //     best live slot right-aligned in the row and -1 before them; y2 -log p of that slot [B].
-//   BEAM_COMMIT (S = B streams, aux = W, N = max_pending, aux2 = max_pending - n_out, K1 = sequence row stride, hist_ld
-//     = T', flags 128 = collapse unconditionally): y slot log p (in/out); hist (reads and rewrites the live count of
-//     column T'-1); seq_in / seq_out sequence rows before / after the commit (distinct buffers); tok_out committed
-//     tokens [B][N]; tok_out2 committed count [B] | collapsed 0/1 [B]; src gather source row [B*W].
+//   BEAM_COMMIT (S = B streams, aux = W, N = max_pending, aux2 = max_pending - n_out, K1 = sequence row stride, K2 = the
+//     row's head before its tokens (0: 3, BEAM_SELECT's {len, hash lo, hash hi}; CTC_SEQ_HEAD = 5 for CTC_BEAM's rows),
+//     hist_ld = T', flags 128 = collapse unconditionally): y slot value (in/out: log p, or CTC_BEAM's ranking value);
+//     hist (reads and rewrites the live count of column T'-1); seq_in / seq_out sequence rows before / after the commit
+//     (distinct buffers); tok_out committed tokens [B][N]; tok_out2 committed count [B] | collapsed 0/1 [B]; src gather
+//     source row [B*W]; y2 (optional, int32 [B]) each stream's last committed token, rewritten when it commits any.
 //   Several symbols per frame (BEAM_SELECT flags 512, ldw2 = K rounds per frame): hist_col = t*K + j is round j of
 //     frame t, hist_ld = T'*K columns.  The live count is read from and written to the last column, hist_live[b,
 //     hist_ld - 1], in every round (the host sets it before the launch), and each round a row takes also records it in
@@ -901,12 +903,15 @@ __device__ __noinline__ void phase_gather(const EbPhase& p) {
 // Chunk end of the streaming beam, one CTA per stream.  The live slots' stored suffixes (seq_in) share a longest common
 // prefix of c tokens; no later frame can change it, since every future hypothesis extends a current one, so it is
 // committed: written to tok_out row b and dropped from every live suffix (seq_out).  If a suffix then still holds more
-// than aux2 = max_pending - n_out tokens (or flags 128: always), the beam collapses: the best live slot (highest log p,
-// lowest slot on ties, as BEAM_FINAL) commits its whole suffix and becomes slot 0, the only live one, keeping its log p.
-// src receives the gather sources that move each kept slot's predictor / LM state into place (identity without a
-// collapse), tok_out2[b] the committed count and tok_out2[S + b] whether the beam collapsed.
+// than aux2 = max_pending - n_out tokens (or flags 128: always), the beam collapses: the best live slot (highest y,
+// lowest slot on ties, as BEAM_FINAL) commits its whole suffix and becomes slot 0, the only live one, keeping its y.
+// src receives the gather sources that move each kept slot's state (predictor / LM, or CTC's pb | pnb | f) into place
+// (identity without a collapse), tok_out2[b] the committed count and tok_out2[S + b] whether the beam collapsed.  The
+// row head (K2) is copied unchanged: the hashes describe the whole sequence, committed part included.  With y2, the last
+// token committed is kept per stream: a CTC slot whose stored suffix is empty takes it as its last token.
 __device__ __noinline__ void phase_beam_commit(const EbPhase& p, float* sm) {
-    const int W = p.aux, T = p.hist_ld, LS = p.K1;
+    const int W = p.aux, T = p.hist_ld, LS = p.K1, HEAD = p.K2 > 0 ? p.K2 : 3;
+    int* last = reinterpret_cast<int*>(p.y2);
     const int tid = threadIdx.x, nt = blockDim.x;
     int* hlive = p.hist + 3 * (long)p.S * T * W;
     int* misc = reinterpret_cast<int*>(sm);
@@ -930,7 +935,7 @@ __device__ __noinline__ void phase_beam_commit(const EbPhase& p, float* sm) {
         const int lmin = misc[0];
         for (long e = tid; e < (long)(nlive - 1) * lmin; e += nt) {
             const int s = 1 + (int)(e / lmin), j = (int)(e % lmin);
-            if (__ldcg(p.seq_in + (r0 + s) * LS + 3 + j) != __ldcg(seq0 + 3 + j)) atomicMin(&misc[4], j);
+            if (__ldcg(p.seq_in + (r0 + s) * LS + HEAD + j) != __ldcg(seq0 + HEAD + j)) atomicMin(&misc[4], j);
         }
         __syncthreads();
         const int c = min(lmin, misc[4]);
@@ -958,13 +963,13 @@ __device__ __noinline__ void phase_beam_commit(const EbPhase& p, float* sm) {
         const int* bs = p.seq_in + (r0 + best) * LS;
         const int ncommit = collapse ? __ldcg(bs) : c;
         int* out = p.tok_out + (long)b * p.N;
-        for (int j = tid; j < ncommit; j += nt) out[j] = __ldcg(bs + 3 + j);
+        for (int j = tid; j < ncommit; j += nt) out[j] = __ldcg(bs + HEAD + j);
         for (long e = tid; e < (long)nkeep * LS; e += nt) {  // kept slot s: {length - ncommit, hash, shifted tokens}
             const int s = (int)(e / LS), j = (int)(e % LS);
             const int* ps = p.seq_in + (r0 + (collapse ? best : s)) * LS;
             const int len = __ldcg(ps) - ncommit;
-            if (j >= len + 3) continue;
-            p.seq_out[(r0 + s) * LS + j] = j == 0 ? len : j < 3 ? __ldcg(ps + j) : __ldcg(ps + j + ncommit);
+            if (j >= len + HEAD) continue;
+            p.seq_out[(r0 + s) * LS + j] = j == 0 ? len : j < HEAD ? __ldcg(ps + j) : __ldcg(ps + j + ncommit);
         }
         for (int s = tid; s < W; s += nt) {
             p.src[r0 + s] = (int)(r0 + (s == 0 ? best : s));
@@ -974,6 +979,7 @@ __device__ __noinline__ void phase_beam_commit(const EbPhase& p, float* sm) {
             p.tok_out2[b] = ncommit;
             p.tok_out2[p.S + b] = collapse;
             hlive[(long)b * T + T - 1] = nkeep;
+            if (last && ncommit > 0) last[b] = __ldcg(bs + HEAD + ncommit - 1);
         }
     }
 }
@@ -1024,7 +1030,8 @@ __device__ __noinline__ void phase_beam_final(const EbPhase& p) {
 //   parent hash lo, parent hash hi, tokens} (the parent hash is the hash of the prefix without its last token); y the
 //   ranking value (pb (+) pnb) + f of each slot [B*W] (dead slots -inf), what BEAM_FINAL picks by; hist as BEAM_SELECT's,
 //   a stay recorded with token blank; src the parent row [B*W].  Flag 32 (LM fusion): x2 / ldx2 / K2 LM logits, fuse,
-//   tok_map and tok_out2 (LM token of each new slot, -1 for a stay) as BEAM_SELECT's.
+//   tok_map and tok_out2 (LM token of each new slot, -1 for a stay) as BEAM_SELECT's.  Flag 64 (streaming): K1 =
+//   max_pending + 5, the live count at t = 0 from hist_live[b, T'-1], y2 the last committed token [B] (int32, read).
 // A frame t < frames[b] of one utterance, for its live slots q (prefix l, last token e or none), with (+) = logaddexp_:
 //   stay       pb' = (pb (+) pnb) + y[blank], pnb' = pnb + y[e] (-inf for the empty prefix), f' = f;
 //   extension  by a non-blank c: pb' = -inf, pnb' = (c == e ? pb : pb (+) pnb) + y[c], f' = f + fusion term;
@@ -1039,6 +1046,14 @@ __device__ __noinline__ void phase_beam_final(const EbPhase& p) {
 // contract; a NaN value gets a composite like any other (order_key keeps every key distinct), so the select still ends
 // after at most 8 passes and reads nothing out of bounds.  Without an LM nothing runs between frames, and one phase
 // walks all frames of its utterances with no grid barrier; with an LM the program runs one frame per phase.
+// Streaming (flags 64, CTCStreamBeamEngine): the beam lives on across launches, as BEAM_SELECT's does.  The live count at
+// t = 0 is the one the previous launch left in the last history column (hist_live[b, T'-1], where BEAM_COMMIT reads and
+// rewrites it), K1 = max_pending + 5 whatever the frames per launch, and a row stores only the tokens since the stream's
+// last commit while its hash and parent hash keep describing the whole prefix, so the merge test stays exact (every
+// live slot of a stream shares the committed part, and no slot shorter than it is live).  y2 (int32 [B]) holds each
+// stream's last committed token, -1 before any: a slot whose stored suffix is empty takes it as its last token e, so the
+// stay's repeat term and the extension rule see the real last token across a commit.  Without the flag e is -1 there,
+// which is the same thing at the start of an utterance.
 constexpr int CTC_SEQ_HEAD = 5;
 // CTC_BEAM's shared memory (2 x u64 + 11 x 32-bit arrays of BEAM_MAX_W, histogram, scalars) in the dynamic shared memory
 static_assert(BEAM_MAX_W * (2 * 8 + 11 * 4) + 256 * 4 + 8 * 4 <= (RED_FLOATS + TR * OUT_LD) * 4, "ctc beam smem");
@@ -1046,7 +1061,7 @@ static_assert(BEAM_MAX_W * (2 * 8 + 11 * 4) + 256 * 4 + 8 * 4 <= (RED_FLOATS + T
 __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
     const int W = p.aux, V = p.N, T = p.hist_ld, blank = p.aux2, LS = p.K1;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nt = blockDim.x;
-    const bool lm = p.flags & 32;
+    const bool lm = p.flags & 32, stream = p.flags & 64;
     const long R = (long)p.S * W, BTW = R * T;
     int* hpar = p.hist;
     int* htok = p.hist + BTW;
@@ -1071,10 +1086,11 @@ __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
     for (int b = blockIdx.x; b < p.S; b += gridDim.x) {
         const long r0 = (long)b * W;
         const int frames = __ldg(p.tok_in + b);
+        const int e0 = stream ? __ldcg(reinterpret_cast<const int*>(p.y2) + b) : -1;   // last token of an empty suffix
         for (int t = p.hist_col; t < p.hist_col + p.ldw1; ++t) {
             __syncthreads();                                 // the previous frame's shared and global writes are done
             const long h0 = ((long)b * T + t) * W;
-            const int nlive = t > 0 ? __ldcg(hlive + (long)b * T + t - 1) : 1;
+            const int nlive = t > 0 ? __ldcg(hlive + (long)b * T + t - 1) : stream ? __ldcg(hlive + (long)b * T + T - 1) : 1;
             if (t >= frames) {                               // frozen: the beam stays, the LM rests
                 for (int j = tid; j < W; j += nt) {
                     hpar[h0 + j] = j;
@@ -1101,7 +1117,7 @@ __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
                 sf[q] = __ldcg(st_in + 2 * R + r0 + q);
                 slen[q] = len;
                 shash[q] = (unsigned)__ldcg(ps + 1) | ((unsigned long long)(unsigned)__ldcg(ps + 2) << 32);
-                se[q] = len > 0 ? __ldcg(ps + CTC_SEQ_HEAD + len - 1) : -1;
+                se[q] = len > 0 ? __ldcg(ps + CTC_SEQ_HEAD + len - 1) : e0;
                 chead[q] = -1;
             }
             __syncthreads();
@@ -1325,7 +1341,11 @@ static_assert(sizeof(EbPhase) % 4 == 0 && sizeof(EbPhase) / 4 <= 256, "EbPhase l
 // type, so their code and registers are what they were without these phases.
 // A fourth, GRU_RNNT = true (eb_decode_run_gru_rnnt), is the default one plus GRU: the phases of a streaming GRU
 // transducer chunk (GRU encoder, LSTM predictor and LM, greedy and beam frames).  It skips CTC_BEAM and CTC_EMIT.
-template <bool CTC, bool CTC_STREAM, bool GRU_RNNT>
+// A fifth, CTC_STREAM_BEAM = true (eb_decode_run_ctc_stream_beam), holds the phases of a streaming CTC beam chunk: the
+// GRU encoder, CTC_EMIT for the log-probs, CTC_BEAM, the LM's LSTM step, GATHER and BEAM_COMMIT.  It has to be a kernel
+// of its own: with CTC_BEAM reachable from any of the four above, their matrix phases would pay its spills.  It skips
+// ARGMAX, BEAM_SELECT and BEAM_FINAL, which no CTC program uses: with them, 68 / 200 bytes of spills instead of 36 / 148.
+template <bool CTC, bool CTC_STREAM, bool GRU_RNNT, bool CTC_STREAM_BEAM>
 __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __restrict__ prog, int nphase, unsigned* bar) {
     extern __shared__ __align__(16) float dsm[];
     float* red = dsm;                                        // [8 warps][2048]
@@ -1358,16 +1378,22 @@ __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __re
                 if constexpr (!CTC_STREAM) phase_lstm(ph, red, outs);
                 break;
             case EB_PH_LINEAR: phase_linear(ph, red, outs); break;
-            case EB_PH_ARGMAX: phase_argmax(ph); break;
+            case EB_PH_ARGMAX:
+                if constexpr (!CTC_STREAM_BEAM) phase_argmax(ph);
+                break;
             case EB_PH_COPY:
                 for (long k = gtid; k < (long)ph.S * ph.N; k += gn) ph.y[k] = __ldcg(ph.x1 + k);
                 break;
-            case EB_PH_BEAM_SELECT: phase_beam_select(ph, dsm); break;
+            case EB_PH_BEAM_SELECT:
+                if constexpr (!CTC_STREAM_BEAM) phase_beam_select(ph, dsm);
+                break;
             case EB_PH_CTC_BEAM:
-                if constexpr (CTC) phase_ctc_beam(ph, dsm);
+                if constexpr (CTC || CTC_STREAM_BEAM) phase_ctc_beam(ph, dsm);
                 break;
             case EB_PH_GATHER: phase_gather(ph); break;
-            case EB_PH_BEAM_FINAL: phase_beam_final(ph); break;
+            case EB_PH_BEAM_FINAL:
+                if constexpr (!CTC_STREAM_BEAM) phase_beam_final(ph);
+                break;
             case EB_PH_BEAM_COMMIT: phase_beam_commit(ph, dsm); break;
             case EB_PH_SKIP:
                 // writes nothing, so it takes no grid barrier (and no epoch) of its own, and neither do the phases it
@@ -1376,7 +1402,7 @@ __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __re
                 __syncthreads();                             // every thread reads the same next
                 continue;
             default:
-                if constexpr (CTC_STREAM) {
+                if constexpr (CTC_STREAM || CTC_STREAM_BEAM) {
                     if (ph.type == EB_PH_GRU) phase_gru(ph, red, outs);
                     else if (ph.type == EB_PH_CTC_EMIT) phase_ctc_emit(ph);
                 } else if constexpr (GRU_RNNT) {
@@ -1394,7 +1420,7 @@ __global__ void __launch_bounds__(256) decode_program_kernel(const EbPhase* __re
 
 }  // namespace
 
-template <bool CTC, bool CTC_STREAM, bool GRU_RNNT>
+template <bool CTC, bool CTC_STREAM, bool GRU_RNNT, bool CTC_STREAM_BEAM = false>
 int decode_run(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream) {
     if (!phases_dev || nphase <= 0 || !barrier_dev) return EB_ERR_INVALID;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -1405,9 +1431,9 @@ int decode_run(const void* phases_dev, int nphase, void* barrier_dev, int max_ct
     unsigned* bar = reinterpret_cast<unsigned*>(barrier_dev);
     void* args[] = {(void*)&prog, (void*)&nphase, (void*)&bar};
     const size_t smem = sizeof(float) * (RED_FLOATS + TR * OUT_LD);
-    EB_CUDA(cudaFuncSetAttribute(decode_program_kernel<CTC, CTC_STREAM, GRU_RNNT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    EB_CUDA(cudaFuncSetAttribute(decode_program_kernel<CTC, CTC_STREAM, GRU_RNNT, CTC_STREAM_BEAM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)smem));
-    EB_CUDA(cudaLaunchCooperativeKernel((void*)decode_program_kernel<CTC, CTC_STREAM, GRU_RNNT>, dim3(grid), dim3(256), args, smem,
+    EB_CUDA(cudaLaunchCooperativeKernel((void*)decode_program_kernel<CTC, CTC_STREAM, GRU_RNNT, CTC_STREAM_BEAM>, dim3(grid), dim3(256), args, smem,
                                         st));
     return EB_OK;
 }
@@ -1426,6 +1452,11 @@ EB_API int eb_decode_run_ctc_stream(const void* phases_dev, int nphase, void* ba
 
 EB_API int eb_decode_run_gru_rnnt(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream) {
     return decode_run<false, false, true>(phases_dev, nphase, barrier_dev, max_ctas, stream);
+}
+
+EB_API int eb_decode_run_ctc_stream_beam(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas,
+                                         void* stream) {
+    return decode_run<false, false, false, true>(phases_dev, nphase, barrier_dev, max_ctas, stream);
 }
 
 EB_API int eb_decode_phase_size(void) { return (int)sizeof(EbPhase); }

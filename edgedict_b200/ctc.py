@@ -247,23 +247,52 @@ def beam_search(log_probs, input_lengths, beam_width, blank=0, *, lm=None, lm_we
 
 
 class CTCStreamDecoder:
-    """Streaming greedy CTC decoding of a ``CTCEncoder`` with ``PytorchStreamDecoder``'s surface (rnnt/stream.py:15-120):
-    ``reset()``, ``decode(frame) -> str``, ``reset_profile()``, the ``encoder_elapsed`` / ``decoder_elapsed`` /
-    ``joint_elapsed`` lists and ``tokenizer``.  ``decode`` runs one persistent kernel launch per chunk
-    (stream_engine.CTCStreamEngine, one stream) and returns the text of the ids emitted in that chunk, ``'</w>'`` turned
-    into a space.  The ids of all chunks together are ``CTCEncoder.greedy_decode``'s on the concatenated frames: a token
-    held across a chunk boundary is emitted once.
+    """Streaming CTC decoding of a ``CTCEncoder`` with ``PytorchStreamDecoder``'s surface (rnnt/stream.py:15-120):
+    ``reset()``, ``decode(frame) -> str``, ``flush() -> str``, ``reset_profile()``, the ``encoder_elapsed`` /
+    ``decoder_elapsed`` / ``joint_elapsed`` lists and ``tokenizer``.  ``decode`` runs one persistent kernel launch per
+    chunk (one stream) and returns the text of the ids that became final in that chunk, ``'</w>'`` turned into a space.
+
+    Greedy (``beam_width=None``, stream_engine.CTCStreamEngine): the ids of all chunks together are
+    ``CTCEncoder.greedy_decode``'s on the concatenated frames (a token held across a chunk boundary is emitted once), and
+    ``flush()`` returns ``""``.  Beam search (``beam_width`` = W, stream_engine.CTCStreamBeamEngine): a chunk's text is
+    the common prefix of all live prefixes that became final in it, never revised; ``flush()`` returns the rest of the
+    best prefix, and decoding goes on from it.  ``lm``, ``lm_weight``, ``length_bonus``, ``lm_bos`` and
+    ``lm_token_map`` fuse the reference's LSTM LM as ``CTCEncoder.beam_search`` does; ``max_pending`` bounds the
+    uncommitted tokens a prefix may hold before the beam collapses to its best prefix.
 
     ``transform`` maps a chunk of audio to log-mel features [1, F, n] (the reference's feature transform);
     ``tokenizer`` is the reference's HuggingFaceTokenizer (``tokenizer.tokenizer.id_to_token``).  A chunk whose frame
     count differs from the previous one's (a short last chunk), or weights that moved (``.to()``, an optimizer's flat
-    bucket), rebuild the program and carry the state over; only ``reset()`` starts a new utterance.  Chunks must hold an
-    even number of frames before each time reduction."""
+    bucket), rebuild the program and carry the state (the beam included) over; only ``reset()`` starts a new utterance.
+    Chunks must hold an even number of frames before each time reduction.  Every argument is checked before any device
+    work."""
 
-    def __init__(self, model, transform, tokenizer, device="cuda", frames_per_chunk=None):
+    def __init__(self, model, transform, tokenizer, device="cuda", frames_per_chunk=None, *, beam_width=None, lm=None,
+                 lm_weight=0.0, length_bonus=0.0, lm_bos=1, lm_token_map=None, max_pending=64):
+        import numbers
         from .rnnt.models import CTCEncoder
+        from .stream_engine import BEAM_MAX_W, check_lm_args, check_stream_shape
         if not isinstance(model, CTCEncoder):
             raise TypeError("CTCStreamDecoder decodes a CTCEncoder, got %s" % type(model).__name__)
+        self._beam = None
+        if beam_width is not None:
+            if isinstance(beam_width, bool) or not isinstance(beam_width, numbers.Integral):
+                raise TypeError("beam_width must be an integer or None, got %r" % (beam_width,))
+            W, V = int(beam_width), model.tovocab[0].weight.shape[0]
+            if not 1 <= W <= BEAM_MAX_W:
+                raise ValueError("beam_width must be in [1, %d], got %d" % (BEAM_MAX_W, W))
+            if W * V >= 2 ** 31:
+                raise ValueError("beam_width x V must stay below 2^31, got %d x %d" % (W, V))
+            check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map)
+            P = operator.index(max_pending)
+            if frames_per_chunk is not None:
+                _, _, T = check_stream_shape(model.model, 1, frames_per_chunk)
+                if P < T:
+                    raise ValueError("max_pending (%d) must be at least the encoder frames per chunk (%d)" % (P, T))
+            self._beam = dict(W=W, lm=lm, lm_weight=lm_weight, length_bonus=length_bonus, lm_bos=lm_bos,
+                              lm_token_map=lm_token_map, max_pending=P)
+        elif lm is not None or lm_weight != 0.0 or length_bonus != 0.0 or lm_token_map is not None:
+            raise ValueError("lm, lm_weight, length_bonus and lm_token_map need beam_width")
         self.device = torch.device(device)
         self.transform, self.tokenizer = transform, tokenizer
         model.eval()
@@ -281,10 +310,18 @@ class CTCStreamDecoder:
         self.joint_elapsed = []
 
     def _build(self, n):
-        from .stream_engine import CTCStreamEngine
+        from .stream_engine import CTCStreamBeamEngine, CTCStreamEngine
         st = self._engine.state() if self._engine is not None else None
-        self._engine = CTCStreamEngine(self.model, 1, n, blank=self.model.blank, state=st)
+        if self._beam is None:
+            self._engine = CTCStreamEngine(self.model, 1, n, blank=self.model.blank, state=st)
+        else:
+            b = dict(self._beam)
+            self._engine = CTCStreamBeamEngine(self.model, 1, n, b.pop("W"), blank=self.model.blank, state=st, **b)
         self._frames = n
+
+    def _text(self, ids, counts):
+        return "".join(self.tokenizer.tokenizer.id_to_token(int(k)).replace('</w>', ' ')
+                       for k in ids[0, :int(counts[0])].tolist())
 
     @torch.no_grad()
     def reset(self):
@@ -302,5 +339,13 @@ class CTCStreamDecoder:
             self._build(xs.shape[1])
         ids, counts = self._engine.step(xs.to(self.device, non_blocking=True))   # one D2H per chunk
         self.encoder_elapsed.append(time.time() - start)
-        return "".join(self.tokenizer.tokenizer.id_to_token(int(k)).replace('</w>', ' ')
-                       for k in ids[0, :int(counts[0])].tolist())
+        return self._text(ids, counts)
+
+    @torch.no_grad()
+    def flush(self):
+        """The rest of the best prefix (beam search), after which decoding continues from it; ``""`` for greedy
+        decoding, whose every id is final when its chunk is decoded."""
+        if self._beam is None or self._engine is None:
+            return ""
+        ids, counts, _ = self._engine.flush()
+        return self._text(ids, counts)

@@ -25,6 +25,7 @@ PH_LN, PH_PAIR, PH_LSTM, PH_LINEAR, PH_ARGMAX, PH_COPY, PH_BEAM_SELECT, PH_GATHE
 F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE, F_LM, F_STREAM, F_FLUSH, F_CONT, F_ROUNDS = 1, 2, 4, 8, 16, 32, 64, 128, \
     256, 512
 BEAM_MAX_W = 1024                                     # EB_BEAM_MAX_W
+CTC_SEQ_HEAD = 5                                      # CTC_BEAM's token rows: {len, hash lo / hi, parent hash lo / hi}
 MAX_SYMBOLS = 16                                      # bounds the program: about (5 + L_dec) * K phases per frame
 
 
@@ -506,6 +507,112 @@ class _ChunkEngine:
             t.copy_(st[k])
 
 
+class _CommitEngine(_ChunkEngine):
+    """What the streaming beams (StreamBeamEngine, CTCStreamBeamEngine) share beyond _ChunkEngine: the chunk end that
+    commits each stream's common prefix with BEAM_COMMIT (``_chunk_end``, which each engine appends for its own state),
+    the flush and re-bound programs built from it, and the host bookkeeping of committed tokens: ``step`` / ``flush``
+    return them, ``state()`` carries those not yet returned, and ``load_state`` re-bounds the carried beam.  The beam
+    rests in the parity-0 buffers between launches; ``logp`` [S*W] is the value BEAM_COMMIT collapses by."""
+    HOST_STATE = ("unreturned_ids", "unreturned_counts")
+
+    def _chunk_end(self, pr, in_parity0, flush):
+        """Append the chunk end to ``pr``: commit (and collapse) from parity 1 into parity 0, the state found in parity 0
+        (``in_parity0``) copied over first; ``flush`` collapses unconditionally."""
+        raise NotImplementedError
+
+    def _commit_buffers(self):
+        """The chunk end's output, committed ids [S, max_pending] | counts [S] | collapsed [S], and its host copy."""
+        S, P = self.S, self.max_pending
+        self._out = torch.zeros(S * P + 2 * S, dtype=torch.int32, device=self.dev)
+        self._host = torch.zeros(self._out.shape, dtype=torch.int32).pin_memory()
+        self.n_collapses = 0
+
+    def _commit_phase(self, flush, n_add, **kw):
+        """BEAM_COMMIT of every stream from parity 1 into parity 0, for chunks that add up to ``n_add`` tokens to a
+        hypothesis; ``kw`` adds the row head (K2) and the last-token buffer (y2) of CTC rows."""
+        S, P = self.S, self.max_pending
+        return EbPhase(type=PH_BEAM_COMMIT, S=S, N=P, aux=self.W, aux2=P - n_add, K1=self.seqs[0].shape[1],
+                       flags=F_FLUSH if flush else 0, y=_ptr(self.logp), hist=_ptr(self.hist),
+                       hist_ld=self.hist_live.shape[1], seq_in=_ptr(self.seqs[1]), seq_out=_ptr(self.seqs[0]),
+                       tok_out=_ptr(self._out), tok_out2=_ptr(self._out, S * P), src=_ptr(self.src), **kw)
+
+    def _commit_programs(self, prog, in_parity0):
+        """Close the chunk program ``prog`` with the chunk end (the frames left the state in parity 0 when
+        ``in_parity0``) and build the flush and the re-bound programs, which find the state in parity 0."""
+        self._chunk_end(prog, in_parity0, flush=False)
+        flush, rebound = [], []
+        self._chunk_end(flush, True, flush=True)
+        self._chunk_end(rebound, True, flush=False)   # a loaded beam under this engine's bound
+        self._flush, self._rebound = _upload(flush, self.dev), _upload(rebound, self.dev)
+        self.n_flush_phases, self.n_rebound_phases = len(flush), len(rebound)
+
+    def _reset_commits(self):
+        """One live slot per stream (the caller starts its state) and nothing committed but not returned."""
+        self.hist_live[:, -1] = 1
+        self._unreturned = (torch.zeros(self.S, 0, dtype=torch.int32), torch.zeros(self.S, dtype=torch.int32))
+
+    def state(self):
+        """Every stream's encoder state and beam, as a dict of tensors, with the committed tokens not yet returned by
+        ``step`` (host ids [S, K] and counts [S])."""
+        st = super().state()
+        st["unreturned_ids"], st["unreturned_counts"] = (t.clone() for t in self._unreturned)
+        return st
+
+    @torch.no_grad()
+    def load_state(self, st):
+        """Continue from ``state()`` of an engine of the same kind over the same model, LM, n_streams, W and max_pending,
+        with any chunk length.  The previous engine bounded every stored suffix by max_pending minus ITS n_out; when
+        this engine's chunks yield more encoder frames, that bound is too loose, so the chunk-end commit and collapse
+        rule runs once here with this engine's bound.  The tokens it commits are returned by the next ``step``."""
+        super().load_state(st)
+        self._unreturned = tuple(st[k].to("cpu", torch.int32) for k in self.HOST_STATE)
+        self._run(self._rebound, self.n_rebound_phases)
+        ids, counts, collapsed = self._fetch(self.max_pending)
+        self.n_collapses += int(collapsed.sum())
+        self._add_unreturned(ids, counts)
+
+    def _add_unreturned(self, ids, counts):
+        """Append committed tokens (ids [S, K], counts [S]) to those not yet returned."""
+        uids, ucounts = self._unreturned
+        n = ucounts + counts
+        out = torch.zeros(self.S, int(n.max()), dtype=torch.int32)
+        for s in range(self.S):
+            a, b = int(ucounts[s]), int(counts[s])
+            out[s, :a] = uids[s, :a]
+            out[s, a:a + b] = ids[s, :b]
+        self._unreturned = (out, n)
+
+    def _take(self, ids, counts):
+        """The tokens just committed, after any committed earlier and not yet returned."""
+        if int(self._unreturned[1].max()) > 0:
+            self._add_unreturned(ids, counts)
+            ids, counts = self._unreturned
+            self._unreturned = (ids[:, :0].clone(), torch.zeros_like(counts))
+        return ids, counts
+
+    @torch.no_grad()
+    def step(self, chunk):
+        """chunk [S, n, F] log-mel frames (device or pinned host) -> (committed ids int32 [S, K], counts int32 [S]) on
+        the host: row s holds in its first counts[s] entries the tokens stream s committed in this chunk.  K is
+        max_pending, or more on the first step after load_state had to commit carried tokens (they come first).
+        ``n_collapses`` counts the forced collapses so far."""
+        self.xin.copy_(chunk, non_blocking=True)
+        self._run(self._chunk, self.n_chunk_phases)
+        ids, counts, collapsed = self._fetch(self.max_pending)
+        self.n_collapses += int(collapsed.sum())
+        return self._take(ids, counts)
+
+    @torch.no_grad()
+    def flush(self):
+        """Collapse every stream's beam to its best hypothesis and commit all of that hypothesis' remaining tokens;
+        decoding continues from it.  -> (ids int32 [S, K], counts int32 [S] as from ``step``, -log p [S] of the best
+        hypothesis, the negated fused score with an LM), on the host."""
+        self._run(self._flush, self.n_flush_phases)
+        ids, counts, _ = self._fetch(self.max_pending)
+        ids, counts = self._take(ids, counts)
+        return ids, counts, -self.logp.view(self.S, self.W)[:, 0].cpu()
+
+
 class StreamEngine(_ChunkEngine):
     STATE = ("enc_h", "enc_c", "dec_h", "dec_c", "dec_x", "tok")   # the carried state (enc_c: None for a GRU encoder)
 
@@ -708,7 +815,7 @@ class BeamEngine:
         return self.ids, self.nlogp
 
 
-class StreamBeamEngine(_ChunkEngine):
+class StreamBeamEngine(_CommitEngine):
     """Streaming beam search: S streams of W hypotheses each, carried from one chunk to the next, one persistent kernel
     launch per chunk.  The chunk program runs StreamEngine's stateful encoder, then per encoder output frame exactly
     BeamEngine's frame (joint, BEAM_SELECT, GATHER, masked predictor and LM steps, with or without LM fusion), so how
@@ -730,7 +837,6 @@ class StreamBeamEngine(_ChunkEngine):
 
     The reference's ``<unk>`` rule (re-argmax when the argmax is ``<unk>``) is a device of the greedy loop; the beam,
     like Transducer.beam_search, does not apply it."""
-    HOST_STATE = ("unreturned_ids", "unreturned_counts")
 
     def __init__(self, transducer, n_streams, frames_per_chunk, W, merge=True, lm=None, lm_weight=0.0,
                  length_bonus=0.0, lm_bos=1, lm_token_map=None, max_pending=64, state=None, blank=NUL, max_ctas=0,
@@ -762,22 +868,17 @@ class StreamBeamEngine(_ChunkEngine):
         # per parity: predictor state, its output, {suffix length, hash lo, hash hi, tokens since the last commit} per
         # row and the LM state
         beam_state(self, R, Ld, Hd, D, LS)
-        st = self._st
         self.dec_htmp, self.hidden, self.logits = z(Ld, R, Hd), z(R, J), z(R, V)
         self.tok, self.src, self.logp = z(R, dtype=i32), z(R, dtype=i32), z(R)
         self.frames = torch.full((S,), T, dtype=i32, device=self.dev)      # a stream never freezes
         beam_history(self, S, TK, W)                          # hist_live's last column: the live count between launches
-        self._out = z(S * P + 2 * S, dtype=i32)               # committed ids [S, P] | counts [S] | collapsed [S]
-        self._host = torch.zeros(self._out.shape, dtype=i32).pin_memory()
-        self.n_collapses = 0
+        self._commit_buffers()
         self._joint = (joint[0].weight, joint[0].bias, joint[2].weight, joint[2].bias)
         prime = []
         _dec_phases(prime, dec, R, self.dec_h[0], self.dec_c[0], self.dec_htmp, self.dec_x[0], self.tok, blank,
                     masked=False)
         if self.lm:
-            Ll, _, Hl = self.lm_htmp.shape
-            ntok = self.lm_logits.shape[1]
-            self._lm_logits_tmp = z(R, ntok)
+            self._lm_logits_tmp = z(R, self.lm_logits.shape[1])           # the chunk end gathers the LM logits
             lm_step(prime, self.lm_h[0], self.lm_c[0], masked=False)
         sel = dict(type=PH_BEAM_SELECT, S=S, N=V, aux=W, aux2=blank,
                    flags=F_STREAM | (F_MERGE if merge else 0) | (F_LM if self.lm else 0), K1=LS, x1=_ptr(self.logits),
@@ -785,35 +886,30 @@ class StreamBeamEngine(_ChunkEngine):
                    hist=_ptr(self.hist), hist_ld=TK, **lm_sel)
         for t in range(T):
             beam_frame(prog, self, dec, t, _ptr(self.enc_out, t * E), T * E, sel, lm_step)
-
-        def chunk_end(pr, in_parity0, flush):
-            """commit (and collapse) from parity 1 into parity 0; state found in parity 0 is copied over first"""
-            if in_parity0:
-                pr.append(EbPhase(type=PH_COPY, S=2 * Ld * R, N=Hd, x1=_ptr(st[0]), y=_ptr(st[1])))
-                pr.append(EbPhase(type=PH_COPY, S=R, N=D, x1=_ptr(self.dec_x[0]), y=_ptr(self.dec_x[1])))
-                pr.append(EbPhase(type=PH_COPY, S=R, N=LS, x1=_ptr(self.seqs[0]), y=_ptr(self.seqs[1])))
-                if self.lm:
-                    pr.append(EbPhase(type=PH_COPY, S=2 * Ll * R, N=Hl, x1=_ptr(self._lst[0]), y=_ptr(self._lst[1])))
-            if self.lm:
-                pr.append(EbPhase(type=PH_COPY, S=R, N=ntok, x1=_ptr(self.lm_logits), y=_ptr(self._lm_logits_tmp)))
-            pr.append(EbPhase(type=PH_BEAM_COMMIT, S=S, N=P, aux=W, aux2=P - TK, K1=LS, flags=F_FLUSH if flush else 0,
-                              y=_ptr(self.logp), hist=_ptr(self.hist), hist_ld=TK, seq_in=_ptr(self.seqs[1]),
-                              seq_out=_ptr(self.seqs[0]), tok_out=_ptr(self._out), tok_out2=_ptr(self._out, S * P),
-                              src=_ptr(self.src)))
-            pr.append(EbPhase(type=PH_GATHER, S=R, N=Hd, aux=2 * Ld, x1=_ptr(st[1]), y=_ptr(st[0]), K2=D,
-                              x2=_ptr(self.dec_x[1]), y2=_ptr(self.dec_x[0]), src=_ptr(self.src)))
-            if self.lm:
-                pr.append(EbPhase(type=PH_GATHER, S=R, N=Hl, aux=2 * Ll, x1=_ptr(self._lst[1]), y=_ptr(self._lst[0]),
-                                  K2=ntok, x2=_ptr(self._lm_logits_tmp), y2=_ptr(self.lm_logits), src=_ptr(self.src)))
-
-        chunk_end(prog, K > 1 or T % 2 == 0, flush=False)     # where the frames left the state
-        flush, rebound = [], []
-        chunk_end(flush, True, flush=True)
-        chunk_end(rebound, True, flush=False)   # a loaded beam under this engine's bound, max_pending - n_out * K
-        self._prime, self._flush, self._rebound = _upload(prime, self.dev), _upload(flush, self.dev), \
-            _upload(rebound, self.dev)
-        self.n_prime_phases, self.n_flush_phases, self.n_rebound_phases = len(prime), len(flush), len(rebound)
+        self._prime, self.n_prime_phases = _upload(prime, self.dev), len(prime)
+        self._commit_programs(prog, K > 1 or T % 2 == 0)     # where the frames left the state
         self._finish(prog, state)
+
+    def _chunk_end(self, pr, in_parity0, flush):
+        st, R = self._st, self.R
+        Ld, Hd, D, LS = st[0].shape[0] // 2, st[0].shape[2], self.dec_x[0].shape[1], self.seqs[0].shape[1]
+        if in_parity0:
+            pr.append(EbPhase(type=PH_COPY, S=2 * Ld * R, N=Hd, x1=_ptr(st[0]), y=_ptr(st[1])))
+            pr.append(EbPhase(type=PH_COPY, S=R, N=D, x1=_ptr(self.dec_x[0]), y=_ptr(self.dec_x[1])))
+            pr.append(EbPhase(type=PH_COPY, S=R, N=LS, x1=_ptr(self.seqs[0]), y=_ptr(self.seqs[1])))
+            if self.lm:
+                pr.append(EbPhase(type=PH_COPY, S=self._lst[0].shape[0] * R, N=self._lst[0].shape[2],
+                                  x1=_ptr(self._lst[0]), y=_ptr(self._lst[1])))
+        if self.lm:
+            ntok = self.lm_logits.shape[1]
+            pr.append(EbPhase(type=PH_COPY, S=R, N=ntok, x1=_ptr(self.lm_logits), y=_ptr(self._lm_logits_tmp)))
+        pr.append(self._commit_phase(flush, self.n_out * self.max_symbols))
+        pr.append(EbPhase(type=PH_GATHER, S=R, N=Hd, aux=2 * Ld, x1=_ptr(st[1]), y=_ptr(st[0]), K2=D,
+                          x2=_ptr(self.dec_x[1]), y2=_ptr(self.dec_x[0]), src=_ptr(self.src)))
+        if self.lm:
+            pr.append(EbPhase(type=PH_GATHER, S=R, N=self._lst[0].shape[2], aux=self._lst[0].shape[0],
+                              x1=_ptr(self._lst[1]), y=_ptr(self._lst[0]), K2=ntok, x2=_ptr(self._lm_logits_tmp),
+                              y2=_ptr(self.lm_logits), src=_ptr(self.src)))
 
     def _state_views(self):
         v = dict(super()._state_views(), dec_state=self._st[0], dec_x=self.dec_x[0], logp=self.logp, seqs=self.seqs[0],
@@ -821,46 +917,6 @@ class StreamBeamEngine(_ChunkEngine):
         if self.lm:
             v.update(lm_state=self._lst[0], lm_logits=self.lm_logits)
         return v
-
-    def state(self):
-        """Every stream's encoder state and beam (slot log p, stored token suffixes, live count, predictor and LM
-        states), as a dict of tensors, with the committed tokens not yet returned by ``step`` (host ids [S, K] and
-        counts [S])."""
-        st = super().state()
-        st["unreturned_ids"], st["unreturned_counts"] = (t.clone() for t in self._unreturned)
-        return st
-
-    @torch.no_grad()
-    def load_state(self, st):
-        """Continue from ``state()`` of an engine over the same model, LM, n_streams, W and max_pending, with any
-        chunk length.  The previous engine bounded every stored suffix by max_pending minus ITS n_out; when this
-        engine's chunks yield more encoder frames, that bound is too loose, so the chunk-end commit and collapse rule
-        runs once here with this engine's bound.  The tokens it commits are returned by the next ``step``."""
-        super().load_state(st)
-        self._unreturned = tuple(st[k].to("cpu", torch.int32) for k in self.HOST_STATE)
-        self._run(self._rebound, self.n_rebound_phases)
-        ids, counts, collapsed = self._fetch(self.max_pending)
-        self.n_collapses += int(collapsed.sum())
-        self._add_unreturned(ids, counts)
-
-    def _add_unreturned(self, ids, counts):
-        """Append committed tokens (ids [S, K], counts [S]) to those not yet returned."""
-        uids, ucounts = self._unreturned
-        n = ucounts + counts
-        out = torch.zeros(self.S, int(n.max()), dtype=torch.int32)
-        for s in range(self.S):
-            a, b = int(ucounts[s]), int(counts[s])
-            out[s, :a] = uids[s, :a]
-            out[s, a:a + b] = ids[s, :b]
-        self._unreturned = (out, n)
-
-    def _take(self, ids, counts):
-        """The tokens just committed, after any committed earlier and not yet returned."""
-        if int(self._unreturned[1].max()) > 0:
-            self._add_unreturned(ids, counts)
-            ids, counts = self._unreturned
-            self._unreturned = (ids[:, :0].clone(), torch.zeros_like(counts))
-        return ids, counts
 
     @torch.no_grad()
     def reset(self):
@@ -870,31 +926,8 @@ class StreamBeamEngine(_ChunkEngine):
             if t is not None:
                 t.zero_()
         beam_reset(self)
-        self.hist_live[:, -1] = 1
-        self._unreturned = (torch.zeros(self.S, 0, dtype=torch.int32), torch.zeros(self.S, dtype=torch.int32))
+        self._reset_commits()
         self._run(self._prime, self.n_prime_phases)
-
-    @torch.no_grad()
-    def step(self, chunk):
-        """chunk [S, n, F] log-mel frames (device or pinned host) -> (committed ids int32 [S, K], counts int32 [S]) on
-        the host: row s holds in its first counts[s] entries the tokens stream s committed in this chunk.  K is
-        max_pending, or more on the first step after load_state had to commit carried tokens (they come first).
-        ``n_collapses`` counts the forced collapses so far."""
-        self.xin.copy_(chunk, non_blocking=True)
-        self._run(self._chunk, self.n_chunk_phases)
-        ids, counts, collapsed = self._fetch(self.max_pending)
-        self.n_collapses += int(collapsed.sum())
-        return self._take(ids, counts)
-
-    @torch.no_grad()
-    def flush(self):
-        """Collapse every stream's beam to its best hypothesis and commit all of that hypothesis' remaining tokens;
-        decoding continues from it.  -> (ids int32 [S, K], counts int32 [S] as from ``step``, -log p [S] of the best
-        hypothesis, the negated fused score with an LM), on the host."""
-        self._run(self._flush, self.n_flush_phases)
-        ids, counts, _ = self._fetch(self.max_pending)
-        ids, counts = self._take(ids, counts)
-        return ids, counts, -self.logp.view(self.S, self.W)[:, 0].cpu()
 
 
 class GRUStreamEngine(StreamEngine):
@@ -1096,3 +1129,147 @@ class CTCStreamEngine(_ChunkEngine):
         self._run(self._chunk, self.n_chunk_phases)
         ids, counts, _ = self._fetch(self.n_out)
         return ids, counts
+
+
+class CTCStreamBeamEngine(_CommitEngine):
+    """Streaming CTC prefix beam search of a ``CTCEncoder``, optionally with shallow fusion of the reference's LSTM
+    language model: S streams of W prefixes each, carried from one chunk to the next, one persistent kernel launch per
+    chunk (eb_decode_run_ctc_stream_beam).  Row r = s*W + slot; each slot carries its prefix with log P(prefix, ends in
+    blank) ``pb``, log P(prefix, ends in a non-blank) ``pnb`` and its accumulated fusion term ``f`` (``beam`` [2][3][R],
+    by parity).
+
+    The chunk program is CTCStreamEngine's encoder and ``tovocab`` Linear, CTC_EMIT for the log-probs (``logprobs``
+    [S*n_out, V]; its greedy outputs go to scratch), then CTCBeamEngine's search in streaming mode: without an LM one
+    CTC_BEAM phase over the chunk's n_out frames, with an LM per frame CTC_BEAM, the GATHER of the LM state by parent and
+    the masked LM step.  So how the audio is cut into chunks does not change which prefixes survive.
+
+    After the chunk's last frame BEAM_COMMIT commits each stream's longest common prefix of its live prefixes, as
+    StreamBeamEngine does: each slot stores only its uncommitted suffix, at most ``max_pending`` tokens, while its hash
+    and parent hash describe the whole prefix.  When a suffix would hold more than ``max_pending - n_out`` tokens the
+    beam collapses to its best slot (highest (pb (+) pnb) + f, lowest slot on ties), whose pb | pnb | f and LM state
+    move to slot 0.  Each stream keeps its last committed token ``last`` [S] (-1 after ``reset``): a slot whose stored
+    suffix is empty takes it as its last token, so a token held across a commit is not emitted twice.  ``flush()``,
+    ``state()`` / ``load_state()`` (with the re-bound) and ``n_collapses`` are StreamBeamEngine's."""
+    GRU = True
+    RUN = "eb_decode_run_ctc_stream_beam"
+
+    def __init__(self, ctc_model, n_streams, frames_per_chunk, W, *, lm=None, lm_weight=0.0, length_bonus=0.0,
+                 lm_bos=1, lm_token_map=None, max_pending=64, blank=0, max_ctas=0, state=None):
+        from .rnnt.models import CTCEncoder
+        if not isinstance(ctc_model, CTCEncoder):
+            raise TypeError("CTCStreamBeamEngine streams a CTCEncoder, got %s" % type(ctc_model).__name__)
+        enc, lin = ctc_model.model, ctc_model.tovocab[0]
+        V, W, blank = lin.weight.shape[0], operator.index(W), operator.index(blank)
+        if not 1 <= W <= BEAM_MAX_W:
+            raise ValueError("beam width must be in [1, %d], got %d" % (BEAM_MAX_W, W))
+        if W * V >= 2 ** 31:
+            raise ValueError("beam width x vocabulary must stay below 2^31 (flat candidate index), got %d x %d" % (W, V))
+        if not 0 <= blank < V:
+            raise ValueError("blank must lie in [0, %d), got %d" % (V, blank))
+        fusion = check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map)
+        S, n, T = self._check_shape(enc, n_streams, frames_per_chunk)
+        P = operator.index(max_pending)
+        if P < T:
+            raise ValueError("max_pending (%d) must be at least the encoder frames per chunk (%d): a chunk can add that "
+                             "many tokens to a prefix" % (P, T))
+        f32, i32 = torch.float32, torch.int32
+        R, LS = S * W, P + 5
+        self.S, self.n, self.V, self.W, self.R, self.blank, self.max_ctas, self.max_pending = \
+            S, n, V, W, R, blank, max_ctas, P
+        prog = []
+        E = self._build_encoder(prog, ctc_model, enc, S, n, T)
+        assert lin.weight.shape[1] == E
+        z = lambda *shape, dtype=f32: torch.zeros(*shape, dtype=dtype, device=self.dev)
+        self.logits, self.logprobs = z(S * T, V), z(S * T, V)
+        self._emit = (z(S, dtype=i32), z(S, T, dtype=i32), z(S, dtype=i32), z(S, dtype=torch.float64))
+        self.beam = z(2, 3, R)                       # per parity: pb | pnb | f
+        self.seqs = z(2, R, LS, dtype=i32)           # per parity: {len, hash lo / hi, parent hash lo / hi, suffix}
+        self.logp, self.src = z(R), z(R, dtype=i32)  # logp: the ranking value (pb (+) pnb) + f
+        self.last = z(S, dtype=i32)
+        self.frames = torch.full((S,), T, dtype=i32, device=self.dev)      # a stream never freezes
+        beam_history(self, S, T, W)                  # hist_live's last column: the live count between launches
+        self._commit_buffers()
+        self.lm = fusion is not None
+        lm_sel, lm_step = lm_fusion(self, fusion, R) if self.lm else ({}, None)
+        prog.append(EbPhase(type=PH_LINEAR, S=S * T, N=V, K1=E, x1=_ptr(self.enc_out), ldx1=E, w1=_ptr(lin.weight),
+                            ldw1=E, b1=_ptr(lin.bias), y=_ptr(self.logits), ldy=V))
+        prev, ids, counts, score = self._emit
+        prog.append(EbPhase(type=PH_CTC_EMIT, S=S, N=V, aux=T, aux2=blank, x1=_ptr(self.logits), ldx1=V,
+                            y=_ptr(self.logprobs), ldy=V, tok_out=_ptr(prev), hist=_ptr(ids), hist_ld=T,
+                            tok_out2=_ptr(counts), y2=_ptr(score)))
+        sel = dict(type=PH_CTC_BEAM, S=S, N=V, aux=W, aux2=blank, K1=LS, flags=F_STREAM | (F_LM if self.lm else 0),
+                   x1=_ptr(self.logprobs), tok_in=_ptr(self.frames), c=_ptr(self.beam), seq_out=_ptr(self.seqs),
+                   y=_ptr(self.logp), src=_ptr(self.src), hist=_ptr(self.hist), hist_ld=T, y2=_ptr(self.last), **lm_sel)
+        prime = []
+        if self.lm:
+            Ll, _, Hl = self.lm_htmp.shape
+            self.lm_state = z(2, 2 * Ll, R, Hl)      # per parity: h of every layer, then c
+            self._lm_logits_tmp = z(R, self.lm_logits.shape[1])
+            lm_step(prime, self.lm_state[0, :Ll], self.lm_state[0, Ll:], masked=False)   # lm_bos from zeros
+            for t in range(T):
+                prog.append(EbPhase(hist_col=t, ldw1=1, **sel))
+                p, q = t & 1, 1 - (t & 1)
+                prog.append(EbPhase(type=PH_GATHER, S=R, N=Hl, aux=2 * Ll, x1=_ptr(self.lm_state[p]),
+                                    y=_ptr(self.lm_state[q]), src=_ptr(self.src)))
+                lm_step(prog, self.lm_state[q, :Ll], self.lm_state[q, Ll:], masked=True)
+        else:
+            prog.append(EbPhase(hist_col=0, ldw1=T, **sel))
+        self._prime, self.n_prime_phases = (_upload(prime, self.dev), len(prime)) if prime else (None, 0)
+        self._commit_programs(prog, T % 2 == 0)      # where the frames left the state
+        self._finish(prog, state)
+
+    def _chunk_end(self, pr, in_parity0, flush):
+        R, LS = self.R, self.seqs.shape[2]
+        if in_parity0:
+            pr.append(EbPhase(type=PH_COPY, S=3, N=R, x1=_ptr(self.beam[0]), y=_ptr(self.beam[1])))
+            pr.append(EbPhase(type=PH_COPY, S=R, N=LS, x1=_ptr(self.seqs[0]), y=_ptr(self.seqs[1])))
+            if self.lm:
+                pr.append(EbPhase(type=PH_COPY, S=self.lm_state.shape[1] * R, N=self.lm_state.shape[3],
+                                  x1=_ptr(self.lm_state[0]), y=_ptr(self.lm_state[1])))
+        if self.lm:
+            ntok = self.lm_logits.shape[1]
+            pr.append(EbPhase(type=PH_COPY, S=R, N=ntok, x1=_ptr(self.lm_logits), y=_ptr(self._lm_logits_tmp)))
+        pr.append(self._commit_phase(flush, self.n_out, K2=CTC_SEQ_HEAD, y2=_ptr(self.last)))
+        pr.append(EbPhase(type=PH_GATHER, S=R, N=1, aux=3, x1=_ptr(self.beam[1]), y=_ptr(self.beam[0]),
+                          src=_ptr(self.src)))
+        if self.lm:
+            pr.append(EbPhase(type=PH_GATHER, S=R, N=self.lm_state.shape[3], aux=self.lm_state.shape[1],
+                              x1=_ptr(self.lm_state[1]), y=_ptr(self.lm_state[0]), K2=ntok, x2=_ptr(self._lm_logits_tmp),
+                              y2=_ptr(self.lm_logits), src=_ptr(self.src)))
+
+    def _state_views(self):
+        v = dict(super()._state_views(), beam=self.beam[0], logp=self.logp, seqs=self.seqs[0],
+                 live=self.hist_live[:, -1], last=self.last)
+        if self.lm:
+            v.update(lm_state=self.lm_state[0], lm_logits=self.lm_logits)
+        return v
+
+    @torch.no_grad()
+    def reset(self):
+        """Every stream starts a new utterance: zero encoder state, one live slot holding the empty prefix (pb = 0,
+        pnb = -inf, f = 0), no committed token (last = -1), and the LM primed with lm_bos from zeros."""
+        S, W = self.S, self.W
+        self.enc_h.zero_()
+        self.beam[0].zero_()
+        self.beam[0, :2].fill_(float("-inf"))
+        self.beam[0, 0].view(S, W)[:, 0] = 0.0
+        self.logp.fill_(float("-inf"))
+        self.logp.view(S, W)[:, 0] = 0.0
+        self.seqs[0].zero_()
+        self.last.fill_(-1)
+        self._reset_commits()
+        if self.lm:
+            self.lm_state[0].zero_()
+            self.lm_tok.fill_(self.lm_bos)
+            self._run(self._prime, self.n_prime_phases)
+
+    def hypotheses(self, s):
+        """The live slots of stream s between chunks, in slot order: [(stored suffix tuple, pb, pnb, f, hash, parent
+        hash)] on the host; the committed tokens precede every suffix."""
+        W, live = self.W, int(self.hist_live[s, -1])
+        st = self.beam[0, :, s * W:s * W + live].cpu()
+        rows = self.seqs[0, s * W:s * W + live].cpu()
+        u = lambda lo, hi: (int(lo) & 0xffffffff) | ((int(hi) & 0xffffffff) << 32)
+        return [(tuple(int(x) for x in rows[j, CTC_SEQ_HEAD:CTC_SEQ_HEAD + int(rows[j, 0])]), float(st[0, j]),
+                 float(st[1, j]), float(st[2, j]), u(rows[j, 1], rows[j, 2]), u(rows[j, 3], rows[j, 4]))
+                for j in range(live)]

@@ -303,7 +303,9 @@ typedef struct EbPhase {
  *       64 = BEAM_SELECT streams: the beam carries over from the previous launch (live count at t = 0 read from the
  *            last history column, hist_live[b, hist_ld - 1]) and the token-sequence rows have stride K1 (max_pending + 3)
  *            and hold only the tokens since the stream's last commit (length = that count; the hash still covers the
- *            whole sequence).  The offline beam search does not set it.
+ *            whole sequence).  The offline beam search does not set it.  CTC_BEAM streams with the same flag (rows of
+ *            stride K1 = max_pending + 5, hashes and parent hashes of the whole prefix) and reads y2 as int32 [S], each
+ *            stream's last committed token (-1 before any), the last token of a slot whose stored suffix is empty.
  *      128 = BEAM_COMMIT collapses every stream's beam to its best slot unconditionally (a flush).
  *      256 = ARGMAX continuation (round j >= 1 of a multi-symbol greedy frame): a row whose tok_out already holds aux
  *            (blank: its frame ended) writes blank to its hist column, takes no argmax and adds nothing under flag 8;
@@ -318,7 +320,9 @@ typedef struct EbPhase {
  * BEAM_COMMIT (streaming beam, after a chunk's last frame, one CTA per stream): commits the common prefix of the live
  * slots' stored suffixes to tok_out [S, N] with the count in tok_out2[s] (tok_out2[S + s] = 1 when the beam collapsed),
  * shifts the suffixes left into seq_out, and, when a suffix still exceeds aux2 tokens or on flags 128, collapses the beam
- * to its best slot; src receives the gather sources that move the kept slots' state into place.
+ * to its best slot by y; src receives the gather sources that move the kept slots' state into place.  K2 is the rows'
+ * head before their tokens (0 for BEAM_SELECT's 3, 5 for CTC_BEAM's); y2, when set, int32 [S], receives each stream's
+ * last committed token whenever it commits any.
  * x1_div (LINEAR): row r of x1 is x1[r / x1_div] (0 or 1: row r), the encoder frame a beam's W rows share.
  * Beam search (batched, W slots per utterance, row r = b*W + slot; see decode.cu for the field use of each phase):
  * at most EB_BEAM_MAX_W slots per utterance.
@@ -349,6 +353,10 @@ int eb_decode_run_ctc_stream(const void* phases_dev, int nphase, void* barrier_d
  * eb_decode_run's plus GRU, so one program holds a GRU encoder, an LSTM predictor and LM, and the greedy and beam frame
  * phases.  It skips CTC_BEAM and CTC_EMIT; the three other instantiations keep their code and registers. */
 int eb_decode_run_gru_rnnt(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream);
+/* Streaming CTC beam search (stream_engine.CTCStreamBeamEngine): the kernel in a fifth instantiation with GRU, LINEAR,
+ * CTC_EMIT, CTC_BEAM (streaming, flag 64), LSTM (the fused LM's step), GATHER, COPY and BEAM_COMMIT.  It skips ARGMAX,
+ * BEAM_SELECT and BEAM_FINAL; the four other instantiations keep their code and registers. */
+int eb_decode_run_ctc_stream_beam(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream);
 
 /* ---- reductions, casts, optimizer -------------------------------------------------------- */
 int eb_colsum(const void* x, int x_bf16, float* out_accum, long rows, int N, void* stream);
