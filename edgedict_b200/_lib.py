@@ -18,6 +18,10 @@ SIGNATURES = {
     "eb_rnnt_loss_lattice": (I, [P, P, I, I, I, P, P, I, P]),
     "eb_rnnt_loss_bwd_bf16": (I, [P, P, P, P, P, I, I, I, I, I, P, P, I, D, P]),
     "eb_joint_logits_lse": (I, [P, P, P, P, P, P, P, P, P, P, I, I, I, I, I, I, P]),
+    "eb_lm_logits_ce": (I, [P, P, P, P, P, I, P, P, L, I, I, P]),
+    "eb_lm_ce_rows": (I, [P, P, I, P, P, L, I, P]),
+    "eb_lm_ce_loss": (I, [P, P, P, I, L, L, I, I, P, P, P, P]),
+    "eb_lm_ce_bwd": (I, [P, P, I, P, P, I, L, L, I, P, I, P, P]),
     "eb_rnnt_workspace_views": (I, [P, I, I, I, I, P, P, P, P, P]),
     "eb_rnnt_align_bytes": (Z, [I, I, I]),
     "eb_rnnt_viterbi": (I, [P, P, I, I, I, I, P, P, P, P, P, P]),

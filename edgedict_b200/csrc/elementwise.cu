@@ -241,8 +241,12 @@ __global__ void embedding_fwd_kernel(const I* __restrict__ ids, const float* __r
         if (out16) out16[i] = __float2bfloat16(v);
     }
 }
-// dW[id] += sum of dout over the positions with that id.  The thread of the FIRST position of an id owns its row and
-// adds the positions in order (no atomics: the same bits on every run); E is walked by the threads of a warp.
+// dW[id] += sum of dout over the positions with that id.  The warp of the FIRST position of an id owns its row and adds
+// the positions in order (no atomics: the same bits on every run).  Both walks read 32 consecutive positions per step
+// (one coalesced load of ids and a ballot): a warp whose id occurs earlier stops at the first 32-position step that holds
+// it, and the owner walks the positions from its own in n / 32 steps, adding only the rows of the matches, lowest first.
+// E is walked by the lanes, EMB_EC columns per lane and pass.
+constexpr int EMB_EC = 4;
 template <typename I>
 __device__ __forceinline__ long emb_id(const I* ids, long pos, int U, int U1, int prepend, int bos) {
     const long b = pos / U1;
@@ -260,13 +264,33 @@ __global__ void embedding_bwd_kernel(const I* __restrict__ ids, const float* __r
         const long id = emb_id(ids, i, U, U1, prepend, bos);
         if (id == pad) continue;                              // padding_idx row gets no gradient
         bool first = true;
-        for (long j = lane; j < i && first; j += 32) first = emb_id(ids, j, U, U1, prepend, bos) != id;
-        if (!__all_sync(0xffffffffu, first)) continue;
-        for (int e = lane; e < E; e += 32) {
-            float acc = 0.f;
-            for (long j = i; j < n; ++j)
-                if (emb_id(ids, j, U, U1, prepend, bos) == id) acc += dout[j * E + e];
-            dW[id * E + e] += acc;
+        for (long j0 = 0; j0 < i; j0 += 32) {
+            const long j = j0 + lane;
+            if (__any_sync(0xffffffffu, j < i && emb_id(ids, j, U, U1, prepend, bos) == id)) { first = false; break; }
+        }
+        if (!first) continue;
+        for (int e0 = 0; e0 < E; e0 += 32 * EMB_EC) {
+            float acc[EMB_EC];
+#pragma unroll
+            for (int c = 0; c < EMB_EC; ++c) acc[c] = 0.f;
+            for (long j0 = i; j0 < n; j0 += 32) {
+                const long j = j0 + lane;
+                unsigned m = __ballot_sync(0xffffffffu, j < n && emb_id(ids, j, U, U1, prepend, bos) == id);
+                while (m) {
+                    const float* dr = dout + (j0 + __ffs(m) - 1) * E;
+                    m &= m - 1;
+#pragma unroll
+                    for (int c = 0; c < EMB_EC; ++c) {
+                        const int e = e0 + lane + 32 * c;
+                        if (e < E) acc[c] += dr[e];
+                    }
+                }
+            }
+#pragma unroll
+            for (int c = 0; c < EMB_EC; ++c) {
+                const int e = e0 + lane + 32 * c;
+                if (e < E) dW[id * E + e] += acc[c];
+            }
         }
     }
 }

@@ -75,6 +75,10 @@ struct Sched {
 // its columns of the whole vocabulary across the consecutive column tiles of its row block, plus the blank and label
 // logits; the four threads that share a row merge them at the end -- everything rnnt_denom_kernel would otherwise
 // re-read the logits for.
+// LSE_ROWS is the same epilogue for the language model's output layer (eb_lm_logits_ce): row r has its own target
+// targets[r], denom[r] receives the row's log-sum-exp and lpl[r] the target's logit (0 for a target outside [0, N),
+// which is never used to index anything).
+constexpr int LSE_NONE = 0, LSE_RNNT = 1, LSE_ROWS = 2;
 struct LseArgs {
     const int* labels; const int* xlen; const int* ylen;     // [B,maxU-1], [B], [B]
     float* denom; float* lpb; float* lpl;                     // [B*maxT*maxU] each (loss workspace)
@@ -82,6 +86,7 @@ struct LseArgs {
     // (not LSE) optional epilogue multiplier for bf16 outputs: C = (A B) * (1 - aux^2), aux bf16 [M,N] -- the tanh'
     // of the joint's hidden layer applied where d hidden is produced (eb_gemm_bf16_dtanh)
     const __nv_bfloat16* aux;
+    const void* targets; int targets64;                       // LSE_ROWS: [M] int32 or int64
 };
 
 __device__ __forceinline__ void st_bf16x2(__nv_bfloat16* p, float a, float b) {
@@ -131,7 +136,7 @@ __device__ __forceinline__ void x_store(const CUtensorMap* map, uint32_t xw, int
 // CTA beside it as well.
 // SC: staged-C epilogue (bf16 C, no accumulation, ksplit = 1, N % 8 == 0; tma_c / tma_x: C and lse.aux with 64 x 64
 // boxes), else tma_c / tma_x are unused.
-template <bool A_MN, bool B_MN, int BN_, bool LSE = false, bool LOW_ = false, bool SC = false>
+template <bool A_MN, bool B_MN, int BN_, int LSE = LSE_NONE, bool LOW_ = false, bool SC = false>
 __global__ void __launch_bounds__(NTHREADS, LOW_ ? 2 : 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                const __grid_constant__ CUtensorMap tma_c, const __grid_constant__ CUtensorMap tma_x,
@@ -262,7 +267,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                 for (int h = 0; h < 2; ++h) {
                     rm[h] = -INFINITY; rs[h] = 0.f; xb[h] = 0.f; xl[h] = 0.f; lab[h] = -1; cell_ok[h] = false;
                     const long cell = m0 + r_in + 8 * h;
-                    if (cell < M) {
+                    if constexpr (LSE == LSE_ROWS) {
+                        if (cell < M) {
+                            const long t = lse.targets64 ? static_cast<const long long*>(lse.targets)[cell]
+                                                         : (long)static_cast<const int*>(lse.targets)[cell];
+                            lab[h] = (t >= 0 && t < N) ? (int)t : -1;
+                            cell_ok[h] = true;
+                        }
+                    } else if (cell < M) {
                         const int u = (int)(cell % lse.maxU);
                         const long bt = cell / lse.maxU;
                         const int t = (int)(bt % lse.maxT), b = (int)(bt / lse.maxT);
@@ -334,7 +346,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                                 (m2 == -INFINITY ? 0.f : s2 * fast_ex2((m2 - m) * LOG2E));
                         rm[h] = m;
                     }
-                    if ((lane & 3) == 0 && cell_ok[h]) {
+                    if constexpr (LSE == LSE_ROWS) {
+                        if ((lane & 3) == 0 && cell_ok[h]) {
+                            const long row = m0 + r_in + 8 * h;
+                            lse.denom[row] = rm[h] + logf(rs[h]);
+                            lse.lpl[row] = xl[h];
+                        }
+                    } else if ((lane & 3) == 0 && cell_ok[h]) {
                         const long cell = m0 + r_in + 8 * h;
                         const float d = -(rm[h] + logf(rs[h]));
                         lse.denom[cell] = d;
@@ -495,7 +513,7 @@ bool make_c_maps(CUtensorMap* tc, CUtensorMap* tx, const void* C, const void* au
 const CUtensorMap kNoMap = {};
 
 // one persistent launch over `work` items, at most one CTA per SM; tc / tx: the SC maps (SC instantiations only)
-template <bool A_MN, bool B_MN, int BN_, bool LSE, bool LOW_, bool SC = false>
+template <bool A_MN, bool B_MN, int BN_, int LSE, bool LOW_, bool SC = false>
 int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* tc, const CUtensorMap* tx, void* C,
                   int c_bf16, const float* bias, int accumulate, long M, int N, long K, int ksplit, long work,
                   const LseArgs& ea, cudaStream_t st, float* part = nullptr) {
@@ -529,10 +547,10 @@ int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* tc, 
     const long out_tiles = ((M + BM - 1) / BM) * ((N + BN_ - 1) / BN_);
     if constexpr (BN_ == 128) {
         if (tc)
-            return launch_kernel<A_MN, B_MN, BN_, false, false, true>(ta, tb, tc, tx, C, c_bf16, bias, accumulate, M, N,
+            return launch_kernel<A_MN, B_MN, BN_, LSE_NONE, false, true>(ta, tb, tc, tx, C, c_bf16, bias, accumulate, M, N,
                                                                       K, ksplit, out_tiles * ksplit, ea, st, part);
     }
-    return launch_kernel<A_MN, B_MN, BN_, false, false>(ta, tb, nullptr, nullptr, C, c_bf16, bias, accumulate, M, N, K,
+    return launch_kernel<A_MN, B_MN, BN_, LSE_NONE, false>(ta, tb, nullptr, nullptr, C, c_bf16, bias, accumulate, M, N, K,
                                                         ksplit, out_tiles * ksplit, ea, st, part);
 }
 
@@ -568,17 +586,18 @@ void plan(int a_mn_major, int c_bf16, int accumulate, long M, int N, long K, int
 int launch_low(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_bf16, const float* bias, int accumulate,
                long M, int N, long K, cudaStream_t st) {
     const long tiles = ((M + BM - 1) / BM) * ((N + 127) / 128);
-    return launch_kernel<false, false, 128, false, true>(ta, tb, nullptr, nullptr, C, c_bf16, bias, accumulate, M, N, K,
+    return launch_kernel<false, false, 128, LSE_NONE, true>(ta, tb, nullptr, nullptr, C, c_bf16, bias, accumulate, M, N, K,
                                                          1, tiles, LseArgs(), st);
 }
 
+template <int LSE>
 int launch_lse(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* tc, void* C, const float* bias, long M,
                int N, long K, const LseArgs& lse, cudaStream_t st) {
     if (tc)
-        return launch_kernel<false, false, 128, true, false, true>(ta, tb, tc, nullptr, C, 1, bias, 0, M, N, K, 1,
-                                                                   (M + BM - 1) / BM, lse, st);
-    return launch_kernel<false, false, 128, true, false>(ta, tb, nullptr, nullptr, C, 1, bias, 0, M, N, K, 1,
-                                                         (M + BM - 1) / BM, lse, st);
+        return launch_kernel<false, false, 128, LSE, false, true>(ta, tb, tc, nullptr, C, 1, bias, 0, M, N, K, 1,
+                                                                  (M + BM - 1) / BM, lse, st);
+    return launch_kernel<false, false, 128, LSE, false>(ta, tb, nullptr, nullptr, C, 1, bias, 0, M, N, K, 1,
+                                                        (M + BM - 1) / BM, lse, st);
 }
 
 }  // namespace
@@ -609,8 +628,33 @@ EB_API int eb_joint_logits_lse(const void* hidden16, const void* w2_16, const fl
     LseArgs lse;
     lse.labels = labels; lse.xlen = xlen; lse.ylen = ylen; lse.denom = denom; lse.lpb = lpb; lse.lpl = lpl;
     lse.maxT = maxT; lse.maxU = maxU; lse.blank = blank; lse.aux = nullptr;
+    lse.targets = nullptr; lse.targets64 = 0;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    return launch_lse(ta, tb, sc ? &tc : nullptr, logits16, b2, M, V, J, lse, st);
+    return launch_lse<LSE_RNNT>(ta, tb, sc ? &tc : nullptr, logits16, b2, M, V, J, lse, st);
+}
+
+// The language model's output layer with the statistics of its cross-entropy (LMModel.loss, bf16 mode): the joint's
+// epilogue above with one target per row (LSE_ROWS).
+//   logits16[r, v] = bf16(hidden16[r, :] . w16[v, :] + b[v]),  lse[r] = logsumexp_v(logits fp32),
+//   tlogit[r] = the fp32 logit of targets[r] when it lies in [0, V), else 0
+EB_API int eb_lm_logits_ce(const void* hidden16, const void* w16, const float* b, void* logits16, const void* targets,
+                           int targets_int64, float* lse, float* tlogit, long M, int V, int K, void* stream) {
+    if (!hidden16 || !w16 || !logits16 || !targets || !lse || !tlogit || M <= 0 || V <= 0 || K <= 0 || K % 8 ||
+        M > INT32_MAX)
+        return EB_ERR_INVALID;
+    if ((reinterpret_cast<uintptr_t>(hidden16) & 15) || (reinterpret_cast<uintptr_t>(w16) & 15) ||
+        (b && (reinterpret_cast<uintptr_t>(b) & 15)) || (reinterpret_cast<uintptr_t>(logits16) & 3))
+        return EB_ERR_INVALID;
+    CUtensorMap ta, tb, tc;
+    const bool sc = staged_c(logits16, 1, 0, V, 1, nullptr);
+    if (!make_map(&ta, hidden16, (uint64_t)K, (uint64_t)M, 128) || !make_map(&tb, w16, (uint64_t)K, (uint64_t)V, 128) ||
+        (sc && !make_c_maps(&tc, nullptr, logits16, nullptr, M, V))) {
+        fprintf(stderr, "[edgedict_b200] cuTensorMapEncodeTiled failed\n");
+        return EB_ERR_CUDA;
+    }
+    LseArgs a = LseArgs();
+    a.denom = lse; a.lpl = tlogit; a.blank = -1; a.targets = targets; a.targets64 = targets_int64 ? 1 : 0;
+    return launch_lse<LSE_ROWS>(ta, tb, sc ? &tc : nullptr, logits16, b, M, V, K, a, reinterpret_cast<cudaStream_t>(stream));
 }
 
 EB_API int eb_gemm_bf16(const void* A, int a_mn_major, const void* B, int b_mn_major, void* C, int c_bf16,

@@ -847,6 +847,50 @@ class LogSoftmax(torch.autograd.Function):
         return ops.log_softmax_bwd(_c(dy), y)
 
 
+class LMLoss(torch.autograd.Function):
+    """nn.NLLLoss(ignore_index, reduction)(F.log_softmax(x W^T + b), targets) -- the reference LMModel's decoder and
+    log-softmax (models.py:224-261) under cli/train_lm.py's criterion -- as one node: the log-probs are never written.
+    bf16 mode: the logits GEMM writes bf16 logits and takes each row's log-sum-exp and target logit from its fp32
+    accumulators (ops.lm_logits_ce); fp32 mode: the fp32 GEMM and a row pass (ops.lm_ce_rows).  The loss kernel sums
+    the costs and counts the targets on the device; backward writes d logits over the saved logits (bf16 or fp32) and
+    runs the three GEMMs of Linear.  x [M, K], targets [M] int32 / int64.  reduction "mean" / "sum" -> [], "none" -> the
+    per-token costs [M] (0 at ignored targets).  A target outside [0, V) that is not ignore_index gives a NaN cost."""
+
+    @staticmethod
+    def forward(ctx, x, w, b, targets, ignore_index, reduction, precision):
+        M, K = x.shape
+        V = w.shape[0]
+        targets = _c(targets)
+        if precision == "bf16":
+            x16 = ops.cast_bf16(_c(x))
+            ba = b if (b is None or (b.is_contiguous() and b.data_ptr() % 16 == 0)) else b.clone()
+            logits, lse, tl = ops.lm_logits_ce(x16, ops.cast_bf16(_c(w)), ba, targets)
+            xs = x16
+        else:
+            xs = _c(x)
+            logits = ops.mm_nt(xs, w, b, "fp32")
+            lse, tl = ops.lm_ce_rows(logits, targets)
+        cost, loss, scale = ops.lm_ce_loss(lse, tl, targets, ignore_index, V, reduction == "mean")
+        ctx.save_for_backward(xs, w, logits, lse, targets, scale)
+        ctx.meta = (precision, ignore_index, b is not None)
+        return cost if reduction == "none" else loss
+
+    @staticmethod
+    def backward(ctx, go):
+        xs, w, logits, lse, targets, scale = ctx.saved_tensors
+        p, ignore_index, has_b = ctx.meta
+        if getattr(ctx, "consumed", False):
+            raise RuntimeError("LMLoss.backward ran twice on the same graph: the gradient is written in place over the "
+                               "saved logits (retain_graph is not supported by this node)")
+        ctx.consumed = True
+        dl = ops.lm_ce_bwd(logits, lse, targets, ignore_index, _c(go.to(f32)).reshape(-1), scale, out=logits)
+        dl16 = dl if p == "bf16" else None
+        dx = ops.mm_nn(dl, w, p, dy16=dl16) if ctx.needs_input_grad[0] else None
+        dw = ops.mm_tn(dl, xs, p, dy16=dl16, x16=xs if p == "bf16" else None) if ctx.needs_input_grad[1] else None
+        db = ops.colsum(dl) if has_b and ctx.needs_input_grad[2] else None
+        return dx, dw, db, None, None, None, None
+
+
 class CTCLossFn(torch.autograd.Function):
     """Per-utterance CTC costs [N] of log_probs (T, N, V) (torch.nn.functional.ctc_loss with reduction='none'); the
     reductions are taken by the caller (edgedict_b200/ctc.py), and autograd hands their per-utterance factors to

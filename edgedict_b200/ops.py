@@ -264,8 +264,9 @@ def embedding_bwd(ids, dout, V, prepend_bos, bos, pad):
     E = dout.shape[-1]
     dW = torch.zeros(V, E, dtype=f32, device=dout.device)
     if dout.numel():
-        check(lib().eb_embedding_bwd(_p(ids), int(ids.dtype == torch.int64), _p(dout), _p(dW), B, U, E,
-                                     int(prepend_bos), bos, pad, _s()), "eb_embedding_bwd")
+        with _timed("embedding_bwd"):
+            check(lib().eb_embedding_bwd(_p(ids), int(ids.dtype == torch.int64), _p(dout), _p(dW), B, U, E,
+                                         int(prepend_bos), bos, pad, _s()), "eb_embedding_bwd")
     return dW
 
 
@@ -673,6 +674,68 @@ def rnnt_loss_bwd_bf16(logits16, labels, xlen, ylen, blank, ws, gscale, host_sca
         check(lib().eb_rnnt_loss_bwd_bf16(_p(logits16), _p(logits16), _p(labels), _p(xlen), _p(ylen), B, T, U, V, blank,
                                           _p(ws), _p(gscale), per_batch, float(host_scale), _s()), "eb_rnnt_loss_bwd_bf16")
     return logits16
+
+
+# ---- language-model cross-entropy (csrc/lm.cu, csrc/gemm_tc.cu) ---------------------------------------
+def _targets(t):
+    _need(t, None, "targets")
+    if t.dtype not in (torch.int32, torch.int64):
+        raise TypeError("targets must be int32 or int64, got %s" % t.dtype)
+    return int(t.dtype == torch.int64)
+
+
+def lm_logits_ce(hid16, w16, b, targets):
+    """bf16 logits [M, V] of hid16 [M, K] @ w16[V, K]^T + b, with each row's lse and target logit (fp32 [M]) from the
+    GEMM's accumulators."""
+    M, K = hid16.shape
+    V = w16.shape[0]
+    t64 = _targets(targets)
+    logits16 = torch.empty(M, V, dtype=bf16, device=hid16.device)
+    lse = torch.empty(M, dtype=f32, device=hid16.device)
+    tl = torch.empty(M, dtype=f32, device=hid16.device)
+    with _timed("lm_logits_ce", 1, 2.0 * (M * K + V * K) + 2.0 * M * V, 2.0 * M * V * K):
+        check(lib().eb_lm_logits_ce(_p(hid16), _p(w16), _p(b), _p(logits16), _p(targets), t64, _p(lse), _p(tl), M, V, K,
+                                    _s()), "eb_lm_logits_ce")
+    return logits16, lse, tl
+
+
+def lm_ce_rows(logits, targets):
+    """(lse, target logit) [M] of fp32 logit rows [M, V]."""
+    _need(logits, f32, "logits")
+    M, V = logits.shape
+    t64 = _targets(targets)
+    lse = torch.empty(M, dtype=f32, device=logits.device)
+    tl = torch.empty(M, dtype=f32, device=logits.device)
+    with _timed("lm_ce_rows", 1, 4.0 * M * V, 0.0):
+        check(lib().eb_lm_ce_rows(_p(logits), _p(targets), t64, _p(lse), _p(tl), M, V, _s()), "eb_lm_ce_rows")
+    return lse, tl
+
+
+def lm_ce_loss(lse, tl, targets, ignore_index, V, mean):
+    """(cost [M], loss [] , scale [1]): per-token costs, their sum or mean over non-ignored targets, and the gradient
+    scale (1 or 1 / count), all on the device."""
+    M = lse.shape[0]
+    t64 = _targets(targets)
+    cost = torch.empty(M, dtype=f32, device=lse.device)
+    loss = torch.empty((), dtype=f32, device=lse.device)
+    scale = torch.empty(1, dtype=f32, device=lse.device)
+    with _timed("lm_ce_loss", 1, 12.0 * M, 0.0):
+        check(lib().eb_lm_ce_loss(_p(lse), _p(tl), _p(targets), t64, int(ignore_index), M, V, int(mean), _p(cost),
+                                  _p(loss), _p(scale), _s()), "eb_lm_ce_loss")
+    return cost, loss, scale
+
+
+def lm_ce_bwd(logits, lse, targets, ignore_index, g, scale=None, out=None):
+    """d logits (same dtype as logits, written into `out`, which may be logits itself) of sum_r g[r] * scale * cost_r
+    (g [M]) or of g * scale * sum_r cost_r (g one element)."""
+    M, V = logits.shape
+    t64 = _targets(targets)
+    _need(g, f32, "g")
+    out = torch.empty_like(logits) if out is None else out
+    with _timed("lm_ce_bwd", 1, 2.0 * logits.element_size() * M * V, 0.0):
+        check(lib().eb_lm_ce_bwd(_p(logits), _p(out), int(logits.dtype == bf16), _p(lse), _p(targets), t64,
+                                 int(ignore_index), M, V, _p(g), int(g.numel() > 1), _p(scale), _s()), "eb_lm_ce_bwd")
+    return out
 
 
 # ---- CTC (csrc/ctc.cu) -------------------------------------------------------------------------------

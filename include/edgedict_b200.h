@@ -147,6 +147,30 @@ int eb_joint_logits_lse(const void* hidden16, const void* w2_16, const float* b2
                         const int* xlen, const int* ylen, float* denom, float* lpb, float* lpl, int B, int maxT,
                         int maxU, int V, int J, int blank, void* stream);
 
+/* ---- language model: the output layer's cross-entropy (csrc/lm.cu, csrc/gemm_tc.cu) -------------------------------
+ * replaces decoder + F.log_softmax of the reference's LMModel (models.py:224-261) under cli/train_lm.py's
+ * nn.NLLLoss(ignore_index); the [M, V] log-probs are never written.  targets [M] int32 or int64 (targets_int64).
+ * eb_lm_logits_ce (bf16 mode): logits16[r, v] = bf16(hidden16[r, :] . w16[v, :] + b[v]) (hidden16 [M, K], w16 [V, K]
+ *   bf16, b [V] fp32 or NULL, all 16-byte aligned, K % 8 == 0), with lse[r] = logsumexp_v of the fp32 logits and
+ *   tlogit[r] = the fp32 logit of targets[r] (0 when the target lies outside [0, V)) from the GEMM's accumulators.
+ * eb_lm_ce_rows (fp32 mode): lse and tlogit of contiguous fp32 logit rows [M, V] (expf / logf, fixed order).
+ * eb_lm_ce_loss: cost[r] = lse[r] - tlogit[r], 0 where targets[r] == ignore_index, NaN where the target is neither
+ *   ignore_index nor in [0, V) (never used as an index); cost may be NULL.  loss[0] = sum of the costs (mean = 0) or
+ *   that sum over the count of non-ignored targets (mean = 1: NaN when every target is ignored), and scale[0] = 1 or
+ *   1 / count, the factor of eb_lm_ce_bwd.  One CTA sums in a fixed order: bitwise repeatable, no atomics.
+ * eb_lm_ce_bwd: grad[r, k] = g[r or 0] * scale[0] * (exp(logits[r, k] - lse[r]) - [k == targets[r]]) (scale NULL: 1,
+ *   g [M] when g_per_row else [1], both device fp32), 0 on ignored rows, NaN on rows with an out-of-range target.
+ *   logits and grad both bf16 (bf16 = 1) or both fp32; grad may alias logits (in place).
+ * No host synchronisation. */
+int eb_lm_logits_ce(const void* hidden16, const void* w16, const float* b, void* logits16, const void* targets,
+                    int targets_int64, float* lse, float* tlogit, long M, int V, int K, void* stream);
+int eb_lm_ce_rows(const float* logits, const void* targets, int targets_int64, float* lse, float* tlogit, long M, int V,
+                  void* stream);
+int eb_lm_ce_loss(const float* lse, const float* tlogit, const void* targets, int targets_int64, long ignore_index,
+                  long M, int V, int mean, float* cost, float* loss, float* scale, void* stream);
+int eb_lm_ce_bwd(const void* logits, void* grad, int bf16, const float* lse, const void* targets, int targets_int64,
+                 long ignore_index, long M, int V, const float* g, int g_per_row, const float* scale, void* stream);
+
 /* ---- LSTM layer, recurrent part (persistent kernel) ---------------------------------------
  * replaces the time loop of nn.LSTM (rnnt/models.py:45-46,64-65,145-147,154-155).
  * xg [B,T,4H] = W_ih x + b_ih + b_hh (gate order i|f|g|o); whh [4H,H]; h0/c0 may be NULL (zeros).
