@@ -93,6 +93,14 @@ SIGNATURES = {
     "eb_fe_power": (I, [P, P, L, I, P]),
     "eb_fe_log_stack": (I, [P, P, I, I, I, I, I, I, I, I, P]),
     "eb_fe_mask": (I, [P, P, I, I, I, I, I, F, P]),
+    "eb_conv_rows_per_split": (I, [I]),
+    "eb_conv1d_first_fwd": (I, [P, P, P, P, I, I, I, I, I, I, P]),
+    "eb_conv1d_first_dw": (I, [P, P, P, I, L, I, I, I, I, I, I, P]),
+    "eb_gn_stats": (I, [P, L, I, I, I, P, P, P, F, P]),
+    "eb_gn_apply": (I, [P, L, I, I, I, P, P, P, P, P, I, I, L, L, P]),
+    "eb_gn_bwd": (I, [P, L, I, I, I, P, P, P, P, L, P, P, P, P, P, L, P, P]),
+    "eb_conv1d_bf16": (I, [P, L, I, I, I, P, I, I, P, P, L, L, P]),
+    "eb_gemm_f32_splitk": (I, [P, L, L, P, L, L, P, I, I, I, I, P]),
     # warp-transducer compatible ABI (include/rnnt.h)
     "get_warprnnt_version": (I, []),
     "rnntGetStatusString": (C.c_char_p, [I]),

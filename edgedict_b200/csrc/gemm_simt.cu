@@ -16,7 +16,15 @@ constexpr int BM = 64, BN = 64, BK = 16, TM = 4, TN = 4;
 __global__ void __launch_bounds__(256)
 sgemm_kernel(const float* __restrict__ A, long sam, long sak, const float* __restrict__ B, long sbk,
              long sbn, float* __restrict__ C, long ldc, const float* __restrict__ bias, int M, int N,
-             int K, float alpha, float beta) {
+             int K, float alpha, float beta, int kchunk = 0, long ldz = 0) {
+    // split-K (blockIdx.z): slice z contracts k in [z*kchunk, (z+1)*kchunk) into its own C slice z*ldz apart
+    if (kchunk > 0) {
+        const long z = blockIdx.z;
+        A += z * kchunk * sak;
+        B += z * kchunk * sbk;
+        C += z * ldz;
+        K = min((long)kchunk, (long)K - z * kchunk);
+    }
     __shared__ float As[2][BK][BM + 4];
     __shared__ float Bs[2][BK][BN + 4];
     const int tid = threadIdx.x;
@@ -97,6 +105,21 @@ EB_API int eb_gemm_f32(const float* A, long sam, long sak, const float* B, long 
     dim3 grid((M + BM - 1) / BM, (N + BN - 1) / BN);
     sgemm_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(A, sam, sak, B, sbk, sbn, C,
                                                                            ldc, bias, M, N, K, alpha, beta);
+    EB_CHECK_LAUNCH();
+    return EB_OK;
+}
+
+// C = A B as eb_gemm_f32 (alpha 1, no bias), its contraction split into ceil(K / kchunk) slices: slice z writes
+// part[z] ([M, N], row-major) and the caller adds the slices in slice order (eb_colsum).  For the weight gradients of the
+// front end's convolutions, whose K (rows) runs to about a million against a 128 x 384 output.
+EB_API int eb_gemm_f32_splitk(const float* A, long sam, long sak, const float* B, long sbk, long sbn, float* part,
+                              int M, int N, int K, int kchunk, void* stream) {
+    if (!A || !B || !part || M <= 0 || N <= 0 || K <= 0 || kchunk <= 0) return EB_ERR_INVALID;
+    const int nz = (K + kchunk - 1) / kchunk;
+    if (nz > 65535) return EB_ERR_INVALID;
+    dim3 grid((M + BM - 1) / BM, (N + BN - 1) / BN, nz);
+    sgemm_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(A, sam, sak, B, sbk, sbn, part, N, nullptr,
+                                                                           M, N, K, 1.f, 0.f, kchunk, (long)M * N);
     EB_CHECK_LAUNCH();
     return EB_OK;
 }

@@ -963,3 +963,163 @@ class JointLoss(torch.autograd.Function):
             dl = ops.rnnt_loss_bwd(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B, out=logits)
         dhe, dhd, dw1, db1, dw2, db2 = _joint_bwd(p, dl.view(B * T * U, V), hid, he2, hd2, w1, w2, ctx.dims)
         return dhe, dhd, dw1, db1, dw2, db2, None, None, None, None, None
+
+
+def conv_out_len(T, k, s):
+    """Output length of a FrontEnd conv (pad k - 1 on both sides, stride s, the last k - 1 outputs dropped)."""
+    return (T + k - 2) // s + 2 - k
+
+
+class FrontEndStack(torch.autograd.Function):
+    """FrontEnd.forward (rnnt/models.py:348-360) channels-last: the first conv (C_in = 1), then per DilatedConvBlock
+    (rnnt/models.py:319-334) conv(GroupNorm(1, C_in)(GELU(y))) with the trim, then LayerNorm(C_last).
+
+    spec = (first, blocks, ln_eps): first = (k, s, C, has_bias) or None (then x is a [B, T, C] block input, which takes
+    a gradient), blocks = ((k, s, C_in, C_out, has_bias, gn_eps), ...), ln_eps = the LayerNorm's eps or None (no
+    LayerNorm).  params in that order: first w [, b]; per block conv w [, b], gn weight, gn bias; ln weight, ln bias.
+
+    Each strided conv reads a padded operand buffer (csrc/conv.cu) that the GroupNorm pass writes; the backward
+    rebuilds it from the saved conv outputs and per-utterance statistics instead of keeping it."""
+
+    @staticmethod
+    def forward(ctx, x, spec, precision, *params):
+        first, blocks, ln_eps = spec
+        bf = precision == "bf16"
+        B = x.shape[0]
+        it = iter(params)
+        saves, meta = [], []
+        if first is not None:
+            k, s, C, hb = first
+            w0 = next(it)
+            b0 = next(it) if hb else None
+            T = conv_out_len(x.shape[1], k, s)
+            y = ops.conv1d_first_fwd(x, _c(w0.view(C, k)), b0, k, s, T)
+        else:
+            y, T, C = x, x.shape[1], x.shape[2]
+        ustride = T * C
+        for (k, s, Cin, Cout, hb, eps) in blocks:
+            w = next(it)
+            b = next(it) if hb else None
+            g, be = next(it), next(it)
+            mean, rstd = ops.gn_stats(y, ustride, B, T, Cin, eps)
+            Q = (k - 1 + T + s - 1) // s
+            rows = B * Q + (k + s - 1) // s
+            xp = torch.empty(rows * s * Cin, dtype=bf16 if bf else f32, device=x.device)
+            ops.gn_apply(y, ustride, B, T, Cin, mean, rstd, g, be, xp, k - 1, Q * s)
+            wp = w.permute(0, 2, 1).contiguous()                       # [C_out, k, C_in]
+            yo = torch.empty(B * Q, Cout, dtype=f32, device=x.device)
+            if bf:
+                ops.conv1d_bf16(xp, 0, rows, s, Cin, 0, ops.cast_bf16(wp), k, Cout, b, yo, 0, Cout, B * Q)
+            else:
+                ops.gemm_f32_at(xp, 0, s * Cin, 1, wp, 1, k * Cin, yo, 0, Cout, B * Q, Cout, k * Cin, bias=b)
+            saves.append((y, mean, rstd))
+            meta.append((ustride, T))
+            y, ustride, T, C = yo, Q * Cout, conv_out_len(T, k, s), Cout
+        out = y.view(B, -1, C)[:, :T].contiguous()
+        ctx.meta, ctx.spec, ctx.precision, ctx.B, ctx.nparams = meta, spec, precision, B, len(params)
+        ln_saves = ()
+        if ln_eps is not None:
+            lw, lb = next(it), next(it)
+            pre_ln = out
+            out, _, lm, lr = ops.layernorm_fwd(pre_ln, None, lw, lb, ln_eps)
+            ln_saves = (pre_ln, lm, lr)
+        ctx.save_for_backward(x, *params, *[t for blk in saves for t in blk], *ln_saves)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        first, blocks, ln_eps = ctx.spec
+        bf = ctx.precision == "bf16"
+        B, n = ctx.B, ctx.nparams
+        st = ctx.saved_tensors
+        first_in, params = st[0], st[1:1 + n]
+        saves = [(st[1 + n + 3 * i],) + ctx.meta[i] + st[2 + n + 3 * i:4 + n + 3 * i] for i in range(len(blocks))]
+        dev = dout.device
+        grads = [None] * len(params)
+        # parameter index of each piece
+        idx = 0
+        if first is not None:
+            i_first = idx
+            idx += 2 if first[3] else 1
+        i_blocks = []
+        for blk in blocks:
+            i_blocks.append(idx)
+            idx += 4 if blk[4] else 3
+        dz = _c(dout)
+        if ln_eps is not None:
+            pre_ln, lm, lr = st[1 + n + 3 * len(blocks):]
+            dz, grads[idx], grads[idx + 1] = ops.layernorm_bwd(dz, pre_ln, None, params[idx], lm, lr)
+        C = dz.shape[-1]
+        dx_in = None
+        # the gradient of the last conv output in the layout of its dY buffer: [lead + B*Q, C_out], zero rows besides
+        # the T_out valid ones of each utterance, lead = k - 1 zero rows in front (the dX phase GEMMs read above row 0)
+        db_next = None
+        if blocks:
+            k, s, Cin, Cout, hb, _ = blocks[-1]
+            T = saves[-1][2]
+            Q, To = (k - 1 + T + s - 1) // s, conv_out_len(T, k, s)
+            dyb = torch.zeros((k - 1 + B * Q) * Cout, dtype=f32, device=dev)
+            dyb[(k - 1) * Cout:].view(B, Q, Cout)[:, :To] = dz
+            dy16 = ops.cast_bf16(dyb) if bf else None
+            dy32 = dyb
+            db_next = ops.colsum(dz.view(-1, Cout)) if hb else None
+        for bi in range(len(blocks) - 1, -1, -1):
+            k, s, Cin, Cout, hb, _ = blocks[bi]
+            y, ustride, T, mean, rstd = saves[bi]
+            pi = i_blocks[bi]
+            w = params[pi]
+            gi = pi + (2 if hb else 1)
+            g, be = params[gi], params[gi + 1]
+            if hb:
+                grads[pi + 1] = db_next
+            Q = (k - 1 + T + s - 1) // s
+            rows = B * Q + (k + s - 1) // s
+            lead = (k - 1) * Cout
+            xp = torch.empty(rows * s * Cin, dtype=bf16 if bf else f32, device=dev)
+            ops.gn_apply(y, ustride, B, T, Cin, mean, rstd, g, be, xp, k - 1, Q * s)
+            # dW[n, j, c] = sum_m dY[m, n] X[m*s + j, c]
+            if bf:
+                nd = (k + s - 1) // s
+                parts = [ops.gemm_bf16(dy16[lead:], 1, xp[d * s * Cin:], 1, Cout, s * Cin, B * Q) for d in range(nd)]
+                dwp = torch.cat(parts, 1)[:, :k * Cin]
+            else:
+                dwp = ops.gemm_f32_rows(dy32, lead, 1, Cout, xp, s * Cin, 1, Cout, k * Cin, B * Q)
+            grads[pi] = dwp.reshape(Cout, k, Cin).permute(0, 2, 1).contiguous()
+            # dX per phase r: padded row q*s + r = sum_m dY[q - m] W[:, :, r + m*s], as a stride-1 conv over dY with the
+            # taps in reverse (m' = mr - 1 - m) starting mr - 1 rows above q
+            dxp = (torch.zeros if s > k else torch.empty)(B * Q * s * Cin, dtype=f32, device=dev)
+            for r in range(min(s, k)):
+                mr = len(range(r, k, s))
+                taps = [r + (mr - 1 - m) * s for m in range(mr)]
+                wr = w[:, :, taps].permute(1, 2, 0).contiguous()          # [C_in, mr, C_out]
+                if bf:
+                    ops.conv1d_bf16(dy16, lead, B * Q, 1, Cout, -(mr - 1), ops.cast_bf16(wr), mr, Cin, None, dxp, r * Cin,
+                                    s * Cin, B * Q)
+                else:
+                    ops.gemm_f32_at(dy32, lead - (mr - 1) * Cout, Cout, 1, wr, 1, mr * Cout, dxp, r * Cin, s * Cin,
+                                    B * Q, Cin, mr * Cout)
+            # GroupNorm + GELU backward into the gradient of this block's input
+            if bi > 0:
+                kp, sp, _, _, hbp, _ = blocks[bi - 1]
+                Tp = saves[bi - 1][2]
+                Qp = (kp - 1 + Tp + sp - 1) // sp
+                nxt = (kp - 1 + B * Qp) * Cin
+                dy32 = None if bf else torch.zeros(nxt, dtype=f32, device=dev)
+                dy16 = torch.zeros(nxt, dtype=bf16, device=dev) if bf else None
+                off, dstride, want_db = (kp - 1) * Cin, Qp * Cin, hbp
+            else:
+                dy32, dy16 = torch.empty(B * T * Cin, dtype=f32, device=dev), None
+                off, dstride, want_db = 0, T * Cin, False
+            grads[gi], grads[gi + 1], db_next = ops.gn_bwd(y, ustride, B, T, Cin, mean, rstd, g, dxp, (k - 1) * Cin,
+                                                           Q * s * Cin, dy32, dy16, off, dstride, want_db)
+            if bi == 0:
+                dx_in = dy32.view(B, T, Cin)
+        if first is not None:
+            k, s, C0, hb = first
+            dy0 = dx_in if blocks else dz.view(B, -1, C0)
+            dw0, db0 = ops.conv1d_first_dw(first_in, _c(dy0), k, s)
+            grads[i_first] = dw0.view(C0, 1, k)
+            if hb:
+                grads[i_first + 1] = db0
+            dx_in = None
+        return (dx_in, None, None) + tuple(grads)

@@ -859,3 +859,105 @@ def fe_mask(x, spans, axis, fill=0.0):
     B, D1, D2 = x.shape
     check(lib().eb_fe_mask(_p(x), _p(spans), B, D1, D2, spans.shape[1], axis, float(fill), _s()), "eb_fe_mask")
     return x
+
+
+# ---- raw-waveform front end (csrc/conv.cu) ----------------------------------------------------------------------------
+def _gn_slices(B, T, C):
+    """(per-channel partial slices, fp64 per-utterance partial slices) of eb_gn_stats / eb_gn_bwd."""
+    rps = int(lib().eb_conv_rows_per_split(C))
+    ns = B * ((T + rps - 1) // rps)
+    return ns, ns * ((C + 255) // 256)
+
+
+def conv1d_first_fwd(x, w, b, k, s, T):
+    """y [B, T, C] = the first layer (C_in = 1) of FrontEnd on x [B, L]; w [C, k]."""
+    B, L = x.shape
+    C = w.shape[0]
+    y = torch.empty(B, T, C, dtype=f32, device=x.device)
+    with _timed("conv1d_first_fwd", 1, 4.0 * (x.numel() + y.numel()), 2.0 * y.numel() * k):
+        check(lib().eb_conv1d_first_fwd(_p(x), _p(w), _p(b), _p(y), B, L, C, k, s, T, _s()), "eb_conv1d_first_fwd")
+    return y
+
+
+def conv1d_first_dw(x, dy, k, s):
+    """(dW [C, k], db [C]) of the first layer from dy [B, T, C]: row splits summed in order."""
+    B, L = x.shape
+    _, T, C = dy.shape
+    rows = B * T
+    rps = max(256, -(-rows // 1024))
+    ns = -(-rows // rps)
+    part = torch.empty(ns, (k + 1) * C, dtype=f32, device=x.device)
+    with _timed("conv1d_first_dw", 2, 4.0 * dy.numel(), 2.0 * dy.numel() * (k + 1)):
+        check(lib().eb_conv1d_first_dw(_p(x), _p(dy), _p(part), ns, rps, B, L, C, k, s, T, _s()), "eb_conv1d_first_dw")
+        tot = colsum(part)
+    tot = tot.view(k + 1, C)
+    return tot[:k].t().contiguous(), tot[k].contiguous()
+
+
+def gn_stats(y, ustride, B, T, C, eps=1e-5):
+    dpart = torch.empty(_gn_slices(B, T, C)[1], 2, dtype=torch.float64, device=y.device)
+    mean = torch.empty(B, dtype=f32, device=y.device)
+    rstd = torch.empty(B, dtype=f32, device=y.device)
+    with _timed("gn_stats", 2, 4.0 * B * T * C):
+        check(lib().eb_gn_stats(_p(y), ustride, B, T, C, _p(dpart), _p(mean), _p(rstd), eps, _s()), "eb_gn_stats")
+    return mean, rstd
+
+
+def gn_apply(y, ustride, B, T, C, mean, rstd, gamma, beta, out, p, rows_per_utt):
+    """The padded conv operand (out: flat fp32 or bf16, a whole number of C-rows) from y."""
+    total = out.numel() // C
+    with _timed("gn_apply", 1, 4.0 * B * T * C + out.element_size() * out.numel()):
+        check(lib().eb_gn_apply(_p(y), ustride, B, T, C, _p(mean), _p(rstd), _p(gamma), _p(beta), _p(out),
+                                int(out.dtype == bf16), p, rows_per_utt, total, _s()), "eb_gn_apply")
+    return out
+
+
+def gn_bwd(y, ustride, B, T, C, mean, rstd, gamma, dz, dz_off, dz_ustride, dy, dy16, dy_off, dy_ustride, want_db):
+    """GroupNorm(1, C) + GELU backward.  dz / dy / dy16 are flat buffers read / written from element offsets dz_off /
+    dy_off.  Returns (dgamma, dbeta, db | None): db = the column sums of dy (the bias gradient of the conv below)."""
+    ns, nd = _gn_slices(B, T, C)
+    dev = y.device
+    pg = torch.empty(ns, C, dtype=f32, device=dev)
+    pb = torch.empty(ns, C, dtype=f32, device=dev)
+    pdb = torch.empty(ns, C, dtype=f32, device=dev) if want_db else None
+    dpart = torch.empty(nd, 2, dtype=torch.float64, device=dev)
+
+    def at(t, off):
+        return None if t is None else t.data_ptr() + off * t.element_size()
+
+    with _timed("gn_bwd", 5, 8.0 * B * T * C + 6.0 * B * T * C):
+        check(lib().eb_gn_bwd(_p(y), ustride, B, T, C, _p(mean), _p(rstd), _p(gamma), at(dz, dz_off), dz_ustride,
+                              _p(pg), _p(pb), _p(dpart), at(dy, dy_off), at(dy16, dy_off), dy_ustride, _p(pdb), _s()),
+              "eb_gn_bwd")
+        dg, dbe = colsum(pg), colsum(pb)
+        db = colsum(pdb) if want_db else None
+    return dg, dbe, db
+
+
+def conv1d_bf16(x16, x_off, x_rows, s, C, row0, w16, taps, N, bias, out, out_off, ldc, M):
+    """out[m, n] (row pitch ldc, from element out_off) = bias + sum_j X[m + row0 + j/s][j%s] . W[n, j]  (eb_conv1d_bf16)."""
+    _need(w16, bf16, "w16")
+    with _timed("conv1d_bf16", 1, 2.0 * x_rows * s * C + 4.0 * M * N, 2.0 * M * N * taps * C):
+        check(lib().eb_conv1d_bf16(x16.data_ptr() + 2 * x_off, x_rows, s, C, row0, _p(w16), taps, N, _p(bias),
+                                   out.data_ptr() + 4 * out_off, ldc, M, _s()), "eb_conv1d_bf16")
+    return out
+
+
+def gemm_f32_at(A, a_off, sam, sak, B, sbk, sbn, out, out_off, ldc, M, N, K, bias=None):
+    """eb_gemm_f32 on views starting at element offsets of flat fp32 storage, output row pitch ldc."""
+    with _timed("gemm_f32", 1, 0.0, 2.0 * M * N * K):
+        check(lib().eb_gemm_f32(A.data_ptr() + 4 * a_off, sam, sak, _p(B), sbk, sbn, out.data_ptr() + 4 * out_off, ldc,
+                                _p(bias), M, N, K, 1.0, 0.0, _s()), "eb_gemm_f32")
+    return out
+
+
+def gemm_f32_rows(A, a_off, sam, sak, B, sbk, sbn, M, N, K):
+    """[M, N] = A' B' with a long contraction (weight gradients over rows): split in slices, added in order."""
+    kchunk = max(1024, -(-K // 128))
+    nz = -(-K // kchunk)
+    part = torch.empty(nz, M * N, dtype=f32, device=A.device)
+    with _timed("gemm_f32_splitk", 2, 0.0, 2.0 * M * N * K):
+        check(lib().eb_gemm_f32_splitk(A.data_ptr() + 4 * a_off, sam, sak, _p(B), sbk, sbn, _p(part), M, N, K, kchunk,
+                                       _s()), "eb_gemm_f32_splitk")
+        out = colsum(part)
+    return out.view(M, N)

@@ -551,6 +551,142 @@ def scale_length(T_out, xlen):
     return (xlen / scale).ceil().int()
 
 
+def CausalConv1d(in_channels, out_channels, kernel_size, dilation=1, **kwargs):
+    """rnnt/models.py:313-317: nn.Conv1d padded by (kernel_size - 1) * dilation, kaiming-normal weight."""
+    pad = (kernel_size - 1) * dilation
+    conv = nn.Conv1d(in_channels, out_channels, kernel_size, padding=pad, dilation=dilation, **kwargs)
+    nn.init.kaiming_normal_(conv.weight)
+    return conv
+
+
+def _conv_spec(conv):
+    k, s, d = conv.kernel_size[0], conv.stride[0], conv.dilation[0]
+    if d != 1:
+        raise ValueError("edgedict_b200's front end implements dilation 1 only (FrontEnd always passes 1)")
+    if k == 1:
+        raise ValueError("kernel_size 1: the reference's trim x[:, :, :-0] returns an empty tensor")
+    return k, s
+
+
+def _check_wave(x, what):
+    if not isinstance(x, torch.Tensor) or not x.is_cuda:
+        raise ValueError("%s needs a CUDA tensor (there is no CPU path)" % what)
+    if x.dtype != torch.float32:
+        raise ValueError("%s needs float32 input, got %s" % (what, x.dtype))
+
+
+def _check_lengths(T, specs):
+    for k, s in specs:
+        T = Fn.conv_out_len(T, k, s)
+        if T < 1:
+            raise ValueError("the front end's input is too short: a conv layer (k=%d, s=%d) has no output frame" % (k, s))
+    return T
+
+
+def _check_bf16_channels(chans):
+    if any(c % 16 for c in chans):
+        raise ValueError("bf16 mode needs the channel count of every conv block to be a multiple of 16 (got %s); use "
+                         "set_precision('fp32')" % (list(chans),))
+
+
+class DilatedConvBlock(nn.Module):
+    """rnnt/models.py:319-334: conv(GroupNorm(1, C_in)(GELU(x))) and the trim; x [B, C_in, T] -> [B, C_out, T_out]."""
+
+    def __init__(self, in_channels, out_channels, kernel_size, dilation=1, group_norm_size=1, **kwargs):
+        super().__init__()
+        pad = (kernel_size - 1) * dilation
+        self.conv = nn.Conv1d(in_channels, out_channels, kernel_size, padding=pad, dilation=dilation, **kwargs)
+        nn.init.kaiming_normal_(self.conv.weight)
+        self.gn = nn.GroupNorm(group_norm_size, in_channels)
+        self.act = nn.GELU()
+
+    def set_precision(self, precision):
+        return _set_precision(self, precision)
+
+    def _spec(self):
+        if self.gn.num_groups != 1 or self.conv.groups != 1 or not isinstance(self.act, nn.GELU) or \
+                self.act.approximate != "none":
+            raise ValueError("edgedict_b200 implements DilatedConvBlock with GroupNorm(1, C), groups=1 and exact GELU")
+        k, s = _conv_spec(self.conv)
+        return (k, s, self.conv.in_channels, self.conv.out_channels, self.conv.bias is not None, float(self.gn.eps))
+
+    def _params(self):
+        c = self.conv
+        return [c.weight] + ([c.bias] if c.bias is not None else []) + [self.gn.weight, self.gn.bias]
+
+    def forward(self, x):
+        _check_wave(x, "DilatedConvBlock")
+        spec = self._spec()
+        _check_lengths(x.shape[-1], [spec[:2]])
+        p = _precision(self)
+        if p == "bf16":
+            _check_bf16_channels(spec[2:4])
+        y = Fn.FrontEndStack.apply(x.transpose(1, 2).contiguous(), (None, (spec,), None), p, *self._params())
+        return y.transpose(1, 2)
+
+
+class FrontEnd(nn.Module):
+    """rnnt/models.py:336-365: the learned front end on raw audio.  x [B, L] or [B, 1, L] fp32 -> [B, T, C_last]
+    (the reference's return value), every step through the C-ABI: causal strided convs (bf16 mode: TMA + wgmma),
+    GELU + GroupNorm(1, C) with statistics over the whole padded batch row, LayerNorm(C_last)."""
+
+    def __init__(self, frontend_params=[(10, 5, 16)] + [(8, 4, 32)] + [(4, 2, 128)] * 3, bias=True):
+        super().__init__()
+        kernel_sizes = [p[0] for p in frontend_params]
+        strides = [p[1] for p in frontend_params]
+        channels = [p[2] for p in frontend_params]
+        assert len(kernel_sizes) == len(strides)
+        self.conv1 = CausalConv1d(1, channels[0], kernel_size=kernel_sizes[0], dilation=1, stride=strides[0], bias=bias)
+        self.encode = nn.Sequential(*[
+            DilatedConvBlock(channels[idx - 1], channels[idx], kernel_size=kernel_sizes[idx], dilation=1,
+                             stride=strides[idx], group_norm_size=1, bias=bias)
+            for idx in range(1, len(strides))
+        ])
+        self.layer_norm = nn.LayerNorm(frontend_params[-1][-1])
+
+    def set_precision(self, precision):
+        return _set_precision(self, precision)
+
+    def output_length(self, L):
+        """Frames of the output for L input samples (16 s at 16 kHz: 399 with cli/train.py's parameters)."""
+        specs = [_conv_spec(self.conv1)] + [blk._spec()[:2] for blk in self.encode]
+        return _check_lengths(L, specs)
+
+    def forward(self, x):
+        if isinstance(x, torch.Tensor) and x.dim() == 3:
+            if x.shape[1] != 1:
+                raise ValueError("FrontEnd takes [B, L] or [B, 1, L] audio, got %s" % (tuple(x.shape),))
+            x = x[:, 0]
+        _check_wave(x, "FrontEnd")
+        if x.dim() != 2:
+            raise ValueError("FrontEnd takes [B, L] or [B, 1, L] audio, got %s" % (tuple(x.shape),))
+        c1 = self.conv1
+        if c1.in_channels != 1:
+            raise ValueError("FrontEnd's first conv takes one channel")
+        k0, s0 = _conv_spec(c1)
+        blocks = tuple(blk._spec() for blk in self.encode)
+        self.output_length(x.shape[1])
+        p = _precision(self)
+        if p == "bf16":
+            _check_bf16_channels([c1.out_channels] + [b[3] for b in blocks])
+        params = [c1.weight] + ([c1.bias] if c1.bias is not None else [])
+        for blk in self.encode:
+            params += blk._params()
+        params += [self.layer_norm.weight, self.layer_norm.bias]
+        if self.layer_norm.normalized_shape != (blocks[-1][3] if blocks else c1.out_channels,) or \
+                not self.layer_norm.elementwise_affine:
+            raise ValueError("FrontEnd's layer_norm must be an affine LayerNorm over the last conv's channels")
+        spec = ((k0, s0, c1.out_channels, c1.bias is not None), blocks, float(self.layer_norm.eps))
+        return Fn.FrontEndStack.apply(x.contiguous(), spec, p, *params)
+
+
+def frontend_lengths(xlen, T):
+    """cli/train.py:236-238's frame lengths of FrontEnd's output: floor(xlen / (max(xlen) / T)), T = the output's time
+    axis (dimension 1 of FrontEnd's [B, T, C] output)."""
+    max_length = xlen.max()
+    return torch.floor(xlen.float() / (max_length.item() / T)).int()
+
+
 def convert_lightning2normal(checkpoint):
     """rnnt/models.py:368-380: unwrap a Lightning checkpoint; when its keys carry the ``model.``
     prefix, drop it and re-wrap as {'model': state_dict}."""

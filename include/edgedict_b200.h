@@ -417,6 +417,46 @@ int eb_fe_log_stack(const float* mel, float* out, int B, int rows_per_utt, int n
  * along axis 1 (frequency) or 2 (time); masked elements := fill. */
 int eb_fe_mask(float* x, const int* spans, int B, int D1, int D2, int nmask, int axis, float fill, void* stream);
 
+/* ---- raw-waveform front end: FrontEnd (rnnt/models.py:313-365), csrc/conv.cu ------------------------------------
+ * Activations channels-last.  y buffers are [B][rows][C] fp32 with `ustride` elements between utterances, the T valid
+ * rows first.  A strided conv (k, s, p = k - 1) over an input of T rows reads a padded operand buffer of Q = ceil((p+T)/s)
+ * rows of s*C_in per utterance (p zero rows, the input, zeros) plus ceil(k/s) zero rows of s*C_in at the end; its output
+ * row b*Q + t is valid for t < T_out = floor((T + k - 2) / s) + 2 - k.
+ * eb_conv_rows_per_split : rows of a [T, C] utterance per partial slice in eb_gn_stats / eb_gn_bwd.  With
+ *                          ns = B * ceil(T / rows): the per-channel partials (pg, pb, pdb) have ns slices of C, the fp64
+ *                          per-utterance partials (dpart) ns * ceil(C / 256) slices of 2.
+ * eb_conv1d_first_fwd    : the first layer (C_in = 1): y[b, t, c] = bias[c] + sum_j w[c, j] x[b, t*s + j - p], T as above.
+ * eb_conv1d_first_dw     : part[z][j][c] (j = k: the bias) over rows [z*rows_per_split, ...) of the B*T rows of dy;
+ *                          dW, db = the slices summed in order (eb_colsum).
+ * eb_gn_stats            : mean / rstd of GELU(y) per utterance over all T x C (GroupNorm(1, C), biased variance, eps),
+ *                          fp64 partial sums in dpart [slices][2].
+ * eb_gn_apply            : out row r = b*rows_per_utt + u (r < total_rows): (GELU(y[b, u-p]) - mean) rstd gamma + beta
+ *                          for p <= u < p + T, else 0; out fp32 or bf16.
+ * eb_gn_bwd              : dz (gradient of eb_gn_apply's valid rows, dz_ustride apart) -> pg / pb [slices][C] partials
+ *                          of dgamma / dbeta, dy = d y (fp32 and / or bf16, dy_ustride apart), pdb [slices][C] partials
+ *                          of sum dy (NULL: none); dpart [slices][2] fp64 scratch.
+ * eb_conv1d_bf16         : out[m, n] (row pitch ldc) = bias[n] + sum_{j<taps} sum_c X[m + row0 + j/s][j%s][c] W[n][j*C + c]
+ *                          on the tensor cores (TMA + wgmma, fp32 accumulation); X bf16 [x_rows][s][C], W bf16
+ *                          [N][taps*C]; rows outside [0, x_rows) read as zeros.  C % 16 == 0, N % 16 == 0. */
+int eb_conv_rows_per_split(int C);
+int eb_conv1d_first_fwd(const float* x, const float* w, const float* bias, float* y, int B, int L, int C, int k, int s,
+                        int T, void* stream);
+int eb_conv1d_first_dw(const float* x, const float* dy, float* part, int nsplit, long rows_per_split, int B, int L,
+                       int C, int k, int s, int T, void* stream);
+int eb_gn_stats(const float* y, long ustride, int B, int T, int C, double* dpart, float* mean, float* rstd, float eps,
+                void* stream);
+int eb_gn_apply(const float* y, long ustride, int B, int T, int C, const float* mean, const float* rstd,
+                const float* gamma, const float* beta, void* out, int out_bf16, int p, long rows_per_utt,
+                long total_rows, void* stream);
+int eb_gn_bwd(const float* y, long ustride, int B, int T, int C, const float* mean, const float* rstd,
+              const float* gamma, const float* dz, long dz_ustride, float* pg, float* pb, double* dpart, float* dy,
+              void* dy16, long dy_ustride, float* pdb, void* stream);
+int eb_conv1d_bf16(const void* x16, long x_rows, int s, int C, int row0, const void* w16, int taps, int N,
+                   const float* bias, float* out, long ldc, long M, void* stream);
+/* eb_gemm_f32 (alpha 1, beta 0, no bias) with the contraction split in slices of kchunk: part[z] = [M, N] of slice z */
+int eb_gemm_f32_splitk(const float* A, long sam, long sak, const float* B, long sbk, long sbn, float* part, int M,
+                       int N, int K, int kchunk, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
