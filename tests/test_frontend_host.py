@@ -45,6 +45,23 @@ def test_restatement_reproduces_the_reference(tag):
         np.testing.assert_allclose(g, want, rtol=0, atol=1e-5 * np.abs(want).max(), err_msg=k)
 
 
+@pytest.mark.parametrize("tag", TAGS)
+def test_bf16_restatement_without_rounding_is_the_fp64_restatement(tag):
+    """The bf16-mode restatement with every rounding switched off is bit for bit the fp64 one; with the roundings on it
+    moves the output and every gradient but the LayerNorm bias's (the sum of R), by no more than bf16 operands can."""
+    z, params, m = _seeded(tag)
+    sd = m.state_dict()
+    out, grads = fo.forward_and_grads(sd, z["x"], params, z[tag + ".R"])
+    out0, grads0 = fo.forward_and_grads(sd, z["x"], params, z[tag + ".R"], bf16=True, rounding=False)
+    assert torch.equal(out0, out)
+    for k, _ in m.named_parameters():
+        assert torch.equal(grads0[k], grads[k]), k
+    out1, grads1 = fo.forward_and_grads(sd, z["x"], params, z[tag + ".R"], bf16=True)
+    for k, a, b in [("out", out1, out)] + [(k, grads1[k], grads[k]) for k, _ in m.named_parameters()]:
+        rel = float((a - b).abs().max() / b.abs().max())
+        assert (rel > 0 or k == "layer_norm.bias") and rel < 5e-2, (k, rel)
+
+
 def test_length_arithmetic():
     from edgedict_b200.functional import conv_out_len
     from edgedict_b200.rnnt.models import FrontEnd
