@@ -38,6 +38,7 @@ SIGNATURES = {
     "eb_gemm_bf16_ex": (I, [P, I, P, I, P, I, P, I, L, I, L, I, P, L, P]),
     "eb_gemm_bf16_partials": (L, [I, I, I, L, I, L, I]),
     "eb_gemm_bf16_dtanh": (I, [P, I, P, I, P, P, L, I, L, P]),
+    "eb_gemm_tc_set_trace": (I, [P, I]),
     "eb_joint_dpre_reduce": (I, [P, P, P, I, I, I, I, P]),
     "eb_lstm_scratch_bytes": (Z, [I, I]),
     "eb_lstm_seq_fwd": (I, [P, P, P, P, P, P, P, P, P, P, I, I, I, P]),

@@ -29,6 +29,15 @@ namespace {
 constexpr int BM = 128, BK = 64, UMMA_K = 16;
 constexpr int A_BYTES = BM * BK * 2;
 constexpr int NTHREADS = 2 * 128 + 32;                       // two consumer warpgroups + the producer warp
+
+// Debug trace (eb_gemm_tc_set_trace): clock64 stamps of CTA 0 for its first trace_tiles work items, [item][8] int64.
+// Consumer thread 0: [0] tile start, [1] its first `full` wait satisfied, [2] the last wgmma_wait<0>, [3] epilogue end,
+// [4] cycles spent in its `full` waits, [6] the staging tile ready (staged-C epilogue: its previous stores have read it,
+// and the tanh' operand has landed); the producer: [5] cycles spent in its `empty` waits for that item.
+constexpr int TRACE_SLOTS = 8;
+long long* g_trace = nullptr;
+int g_trace_tiles = 0;
+
 // Tile width BN_ = 128 (6 stages) or 256 (4 stages): ~193 KB of shared memory either way.
 // LOW_ = "co-resident" configuration: 3 stages of the narrow tile (97 KB of shared memory), so that a GEMM CTA fits on an
 // SM next to one CTA of a persistent recurrent kernel (lstm_c4.cu) -- used by the layer-wavefront schedule of the encoder
@@ -141,7 +150,8 @@ __global__ void __launch_bounds__(NTHREADS, LOW_ ? 2 : 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                const __grid_constant__ CUtensorMap tma_c, const __grid_constant__ CUtensorMap tma_x,
                void* __restrict__ Cout, int c_bf16, const float* __restrict__ bias, int accumulate,
-               long M, int N, long K, int ksplit, LseArgs lse = LseArgs(), float* __restrict__ part = nullptr) {
+               long M, int N, long K, int ksplit, LseArgs lse = LseArgs(), float* __restrict__ part = nullptr,
+               long long* trace = nullptr, int trace_tiles = 0) {
     using C_ = Cfg<BN_, LOW_, SC>;
     constexpr int BN = BN_, STAGES = C_::STAGES, STAGE_BYTES = C_::STAGE_BYTES, NACC = BN / 2;
     extern __shared__ uint8_t smem_raw[];
@@ -188,8 +198,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                 // the tanh' operand of this tile: loaded once the wait for k-block kb0 + STAGES has shown that the
                 // consumers are into the tile, so that waiting for the staging tile does not stall the ring
                 const int kbx = min(kb0 + STAGES, kb1 - 1);
+                const bool tr = trace && blockIdx.x == 0 && jj < trace_tiles;
+                long long twait = 0;
                 for (int kb = kb0; kb < kb1; ++kb) {
+                    const long long tw = tr ? clock64() : 0;
                     mbar_wait(empty0 + 8 * stage, phase ^ 1);
+                    if (tr) twait += clock64() - tw;
                     const uint32_t sa = smem_u32(tiles + stage * STAGE_BYTES), sb = sa + A_BYTES;
                     const uint32_t fb = full0 + 8 * stage;
                     mbar_expect_tx(fb, TX);
@@ -209,6 +223,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                     }
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
+                if (tr) trace[jj * TRACE_SLOTS + 5] = twait;
             }
         }
         return;
@@ -234,11 +249,21 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
         const int kb0 = ks * kb_per, kb1 = min(nkb_total, kb0 + kb_per);
         const long m0 = mb * BM;
         const int n0 = nb * BN;
+        long long* const tr = (trace && blockIdx.x == 0 && threadIdx.x == 0 && jj < trace_tiles) ? trace + jj * TRACE_SLOTS
+                                                                                                  : nullptr;
+        long long twait = 0;
+        if (tr) tr[0] = clock64();
 #pragma unroll
         for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
         int prev = -1;
         for (int kb = kb0; kb < kb1; ++kb) {
+            const long long tw = tr ? clock64() : 0;
             mbar_wait(full0 + 8 * stage, phase);
+            if (tr) {
+                const long long t = clock64();
+                twait += t - tw;
+                if (kb == kb0) tr[1] = t;
+            }
             const uint32_t sa = smem_u32(tiles + stage * STAGE_BYTES) + (uint32_t)wg * 8192u, sb = smem_u32(tiles + stage * STAGE_BYTES) + A_BYTES;
             wgmma_fence();
 #pragma unroll
@@ -258,10 +283,22 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
         }
         wgmma_wait<0>();
         wgmma_fence_regs(acc);
+        if (tr) { tr[2] = clock64(); tr[4] = twait; }
         if (prev >= 0 && lane == 0) mbar_arrive(empty0 + 8 * prev);
 
         if constexpr (LSE) {
             constexpr float LOG2E = 1.4426950408889634f;
+            // The bias of the thread's 32 columns, shared by its two rows: all loads issued here, unconditionally (a
+            // column past N reads bias[N - 1] and is never used), so that their latency overlaps and is paid once.
+            // Loaded under a `col < N` branch at the point of use, each load's latency was exposed in turn.
+            float bb[BN / 4];
+            if (bias) {
+#pragma unroll
+                for (int i = 0; i < BN / 4; ++i) bb[i] = __ldg(bias + min(n0 + 8 * (i >> 1) + cq + (i & 1), N - 1));
+            } else {
+#pragma unroll
+                for (int i = 0; i < BN / 4; ++i) bb[i] = 0.f;
+            }
             if (nb == 0) {                                   // new row block: reset, decode (b,t,u) of my two rows
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
@@ -285,6 +322,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                 }
             }
             if constexpr (SC) x_acquire(wg, leader);
+            if (tr) tr[6] = clock64();
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 // add the bias here (the statistics are over logits = acc + b2), then the online softmax
@@ -293,8 +331,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                 for (int i = 0; i < BN / 8; ++i) {
                     const int col = n0 + 8 * i + cq;
                     float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
-                    v0 = col < N ? v0 + (bias ? __ldg(bias + col) : 0.f) : -INFINITY;
-                    v1 = col + 1 < N ? v1 + (bias ? __ldg(bias + col + 1) : 0.f) : -INFINITY;
+                    v0 = col < N ? v0 + bb[2 * i] : -INFINITY;
+                    v1 = col + 1 < N ? v1 + bb[2 * i + 1] : -INFINITY;
                     acc[4 * i + 2 * h] = v0; acc[4 * i + 2 * h + 1] = v1;
                     cm = fmaxf(cm, fmaxf(v0, v1));
                     if (col == lse.blank) xb[h] = v0;
@@ -366,6 +404,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
             // store clips what lies outside C
             if (has_x) { mbar_wait(xfull, xph); xph ^= 1; }   // (implies the previous stores have read the tile)
             else x_acquire(wg, leader);
+            if (tr) tr[6] = clock64();
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int rr = r_in - 64 * wg + 8 * h;
@@ -464,6 +503,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                 }
             }
         }
+        if (tr) tr[3] = clock64();
     }
     if constexpr (SC) {
         if (leader) bulk_wait<0>();                          // the staging tile stays valid until the last store is done
@@ -526,7 +566,7 @@ int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMa
     }
     const int grid = (int)(work < eb_num_sms() ? work : eb_num_sms());
     kern<<<grid, NTHREADS, C_::SMEM_BYTES, st>>>(ta, tb, tc ? *tc : kNoMap, tx ? *tx : kNoMap, C, c_bf16, bias,
-                                                 accumulate, M, N, K, ksplit, ea, part);
+                                                 accumulate, M, N, K, ksplit, ea, part, g_trace, g_trace_tiles);
     EB_CHECK_LAUNCH();
     if (ksplit > 1) {
         const long mn = M * (long)N;
@@ -655,6 +695,13 @@ EB_API int eb_lm_logits_ce(const void* hidden16, const void* w16, const float* b
     LseArgs a = LseArgs();
     a.denom = lse; a.lpl = tlogit; a.blank = -1; a.targets = targets; a.targets64 = targets_int64 ? 1 : 0;
     return launch_lse<LSE_ROWS>(ta, tb, sc ? &tc : nullptr, logits16, b, M, V, K, a, reinterpret_cast<cudaStream_t>(stream));
+}
+
+// debug: per-tile clock64 stamps of CTA 0 of subsequent wgmma GEMM launches ([tiles][8] int64, see TRACE_SLOTS; null = off)
+EB_API int eb_gemm_tc_set_trace(void* dev_buf, int tiles) {
+    g_trace = reinterpret_cast<long long*>(dev_buf);
+    g_trace_tiles = dev_buf ? tiles : 0;
+    return EB_OK;
 }
 
 EB_API int eb_gemm_bf16(const void* A, int a_mn_major, const void* B, int b_mn_major, void* C, int c_bf16,

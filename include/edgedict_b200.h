@@ -134,6 +134,9 @@ long eb_gemm_bf16_partials(int a_mn_major, int c_bf16, int accumulate, long M, i
 int eb_gemm_bf16_ex(const void* A, int a_mn_major, const void* B, int b_mn_major, void* C, int c_bf16,
                     const float* bias, int accumulate, long M, int N, long K, int flags, float* partials,
                     long partial_floats, void* stream);
+/* debug: per-tile clock64 stamps of CTA 0 of the wgmma GEMM ([tiles][8] int64: tile start, first operand stage ready,
+ * last MMA retired, epilogue end, consumer operand-wait cycles, producer empty-wait cycles; NULL = off) */
+int eb_gemm_tc_set_trace(void* dev_buf, int tiles);
 
 /* C16[M,N] = bf16((A B) * (1 - hid16[M,N]^2)): the joint's d-hidden GEMM with the derivative of Joint.forward's Tanh
  * (rnnt/models.py:164) applied in the epilogue, so that d(pre-activation) leaves the GEMM directly. */
