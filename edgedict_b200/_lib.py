@@ -102,6 +102,18 @@ SIGNATURES = {
     "eb_gn_bwd": (I, [P, L, I, I, I, P, P, P, P, L, P, P, P, P, P, L, P, P]),
     "eb_conv1d_bf16": (I, [P, L, I, I, I, P, I, I, P, P, L, L, P]),
     "eb_gemm_f32_splitk": (I, [P, L, L, P, L, L, P, I, I, I, I, P]),
+    "eb_w2v_mask_fwd": (I, [P, P, P, P, L, I, P]),
+    "eb_w2v_keep_rows": (I, [P, P, P, L, I, P]),
+    "eb_w2v_gather": (I, [P, P, P, I, I, I, I, P]),
+    "eb_w2v_scatter": (I, [P, P, P, I, I, I, I, P]),
+    "eb_w2v_sq_mean": (I, [P, L, P, P]),
+    "eb_w2v_scale": (I, [P, P, F, L, P, P]),
+    "eb_w2v_quant_fwd": (I, [P, P, P, I, I, I, I, F, P, P, P, P, P, P, P, P]),
+    "eb_w2v_quant_stats": (I, [P, P, I, I, I, P, P, P, P]),
+    "eb_w2v_quant_bwd": (I, [P, P, P, P, P, I, I, I, F, P, P]),
+    "eb_w2v_logits_fwd": (I, [P, P, P, I, I, I, I, F, F, P, P, P, P, P, P, P]),
+    "eb_w2v_logits_bwd": (I, [P, P, P, P, P, P, P, P, P, I, I, I, I, F, F, P, P, P, P, P]),
+    "eb_w2v_ce": (I, [P, I, I, I, P, P, P]),
     # warp-transducer compatible ABI (include/rnnt.h)
     "get_warprnnt_version": (I, []),
     "rnntGetStatusString": (C.c_char_p, [I]),

@@ -1123,3 +1123,140 @@ class FrontEndStack(torch.autograd.Function):
                 grads[i_first + 1] = db0
             dx_in = None
         return (dx_in, None, None) + tuple(grads)
+
+
+# ---- wav2vec pre-training head (rnnt/wav2vec.py, modules/softmax_vector_quantizer.py; csrc/w2v.cu) ----------------
+class W2VMask(torch.autograd.Function):
+    """Wav2Vec.apply_mask's ``x[mask_indices] = mask_emb`` (rnnt/wav2vec.py:165-181), out of place: x [B, T, D] with
+    mask_emb in the masked rows.  Backward: the masked rows of dx are zero and d mask_emb is the column sum of the
+    masked rows of dout, gathered and added in row order (eb_colsum)."""
+
+    @staticmethod
+    def forward(ctx, x, mask_emb, idx, inv):
+        ctx.save_for_backward(idx, inv)
+        return ops.w2v_mask_fwd(_c(x), _c(mask_emb), inv)
+
+    @staticmethod
+    def backward(ctx, dout):
+        idx, inv = ctx.saved_tensors
+        dout = _c(dout)
+        dx = ops.w2v_keep_rows(dout, inv) if ctx.needs_input_grad[0] else None
+        demb = None
+        if ctx.needs_input_grad[1]:
+            demb = ops.colsum(ops.w2v_gather(dout, idx).view(-1, dout.shape[-1]))
+        return dx, demb, None, None
+
+
+class W2VGather(torch.autograd.Function):
+    """x[mask_indices].view(B, M, D) (rnnt/wav2vec.py:308, 358): the masked rows of each utterance in frame order.
+    Backward writes them back and zeros elsewhere; the rows are unique, so no sum is involved."""
+
+    @staticmethod
+    def forward(ctx, x, idx, inv):
+        ctx.save_for_backward(inv)
+        return ops.w2v_gather(_c(x), idx)
+
+    @staticmethod
+    def backward(ctx, dy):
+        (inv,) = ctx.saved_tensors
+        return ops.w2v_scatter(_c(dy), inv), None, None
+
+
+class W2VSqMean(torch.autograd.Function):
+    """features.float().pow(2).mean() (rnnt/wav2vec.py:269), added in a fixed order by one CTA."""
+
+    @staticmethod
+    def forward(ctx, x):
+        x = _c(x)
+        ctx.save_for_backward(x)
+        return ops.w2v_sq_mean(x)
+
+    @staticmethod
+    def backward(ctx, g):
+        (x,) = ctx.saved_tensors
+        return ops.w2v_scale(x, _c(g.to(f32)).reshape(1), 2.0 / x.numel())
+
+
+class W2VQuantize(torch.autograd.Function):
+    """GumbelVectorQuantizer.forward after weight_proj (modules/softmax_vector_quantizer.py:140-201) for
+    combine_groups=False: logits [N, G*V], vars [1, G*V, vd], noise [N, G*V] (training) or None (eval) ->
+    (q [N, G*vd], prob_perplexity, code_perplexity, k [N, G] int32).  Training: q[r, g] = st * vars[g*V + k] with k the
+    hard Gumbel index and st = (1 - s_k) + s_k in fp32, as torch's straight-through F.gumbel_softmax(hard=True) gives it;
+    eval: q = vars[k0], k0 the clean argmax.  Backward: d soft = dq_g vars_g^T and d vars_g = X_g^T dq_g (eb_gemm_f32,
+    X the straight-through matrix), then the noisy and the clean softmax Jacobians (eb_w2v_quant_bwd)."""
+
+    @staticmethod
+    def forward(ctx, logits, vars, noise, G, tau):
+        logits = _c(logits)
+        v2 = _c(vars).view(-1, vars.shape[-1])
+        q, p, s, X, k0, k, st = ops.w2v_quant_fwd(logits, noise, v2, G, tau)
+        stats, coef = ops.w2v_quant_stats(p, k0, G)
+        ctx.save_for_backward(v2, p, X, coef, *([s] if s is not None else []))
+        ctx.meta = (G, tau, s is not None, vars.shape)
+        pp, cp = stats[0].clone(), stats[1].clone()
+        ctx.mark_non_differentiable(cp, k)
+        return q, pp, cp, k
+
+    @staticmethod
+    def backward(ctx, dq, dpp, _dcp, _dk):
+        G, tau, noisy, vshape = ctx.meta
+        v2, p, X, coef = ctx.saved_tensors[:4]
+        s = ctx.saved_tensors[4] if noisy else None
+        N, GV = p.shape
+        V, vd = GV // G, v2.shape[1]
+        dq = _c(dq)
+        dsoft = None
+        if ctx.needs_input_grad[0] and noisy:
+            dsoft = torch.empty(N, GV, dtype=f32, device=p.device)
+            for g in range(G):
+                ops.gemm_f32_at(dq, g * vd, G * vd, 1, v2[g * V:(g + 1) * V], 1, vd, dsoft, g * V, GV, N, V, vd)
+        dl = None
+        if ctx.needs_input_grad[0]:
+            dl = ops.w2v_quant_bwd(dsoft, s, p, coef, _c(dpp.to(f32)).reshape(1), G, tau)
+        dvars = None
+        if ctx.needs_input_grad[1]:
+            dvars = torch.empty(GV, vd, dtype=f32, device=p.device)
+            for g in range(G):
+                ops.gemm_f32_at(X, g * V, 1, GV, dq[:, g * vd:], G * vd, 1, dvars, g * V * vd, vd, V, vd, N)
+            dvars = dvars.view(vshape)
+        return dl, dvars, None, None, None
+
+
+class W2VLogits(torch.autograd.Function):
+    """Wav2Vec.compute_preds (rnnt/wav2vec.py:381-395) with the negatives of sample_negatives as frame indices:
+    xp, yp [B, M, D], neg [B, M, K] int32 -> logits [K+1, B, M] = cos(xp[b, m], candidate) / logit_temp, candidate 0 =
+    yp[b, m] and candidate 1 + k = yp[b, neg[b, m, k]]; -inf (and no gradient) where a negative equals the positive in
+    every element.  torch.cosine_similarity's semantics: each row over max(|row|, 1e-8), then the dot product.  The
+    [K+1, B, M, D] candidate tensor is never written."""
+
+    @staticmethod
+    def forward(ctx, xp, yp, neg, temp):
+        xp, yp = _c(xp), _c(yp)
+        logits, saved = ops.w2v_logits_fwd(xp, yp, neg, temp)
+        ctx.save_for_backward(xp, yp, neg, *saved)
+        ctx.temp = temp
+        return logits
+
+    @staticmethod
+    def backward(ctx, dlogits):
+        xp, yp, neg, xh, yh, xn, yn, cos = ctx.saved_tensors
+        dxp, dyp = ops.w2v_logits_bwd(_c(dlogits), cos, neg, xh, yh, xp, yp, xn, yn, ctx.temp)
+        return dxp, dyp, None, None
+
+
+class W2VCrossEntropy(torch.autograd.Function):
+    """ConstrastiveCriterion's F.cross_entropy(get_logits(x), 0, reduction='sum') and its correct count
+    (rnnt/wav2vec.py:445-461, 512-523) on logits [K+1, B, M], rows in get_logits' (m, b) order -> (loss, correct)."""
+
+    @staticmethod
+    def forward(ctx, logits):
+        grad, out = ops.w2v_ce(_c(logits))
+        ctx.save_for_backward(grad)
+        loss, correct = out[0].clone(), out[1].clone()
+        ctx.mark_non_differentiable(correct)
+        return loss, correct
+
+    @staticmethod
+    def backward(ctx, go, _dc):
+        (grad,) = ctx.saved_tensors
+        return ops.w2v_scale(grad, _c(go.to(f32)).reshape(1))

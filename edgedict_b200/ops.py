@@ -961,3 +961,138 @@ def gemm_f32_rows(A, a_off, sam, sak, B, sbk, sbn, M, N, K):
                                        _s()), "eb_gemm_f32_splitk")
         out = colsum(part)
     return out.view(M, N)
+
+
+# ---- wav2vec pre-training head (csrc/w2v.cu) -----------------------------------------------------
+def w2v_mask_fwd(x, mask_emb, inv):
+    """x [B, T, D] with mask_emb in the masked rows (inv [B, T] int32 >= 0), out of place."""
+    _need(x, f32, "x"), _need(mask_emb, f32, "mask_emb"), _need(inv, torch.int32, "inv")
+    out = torch.empty_like(x)
+    check(lib().eb_w2v_mask_fwd(_p(x), _p(mask_emb), _p(inv), _p(out), inv.numel(), x.shape[-1], _s()),
+          "eb_w2v_mask_fwd")
+    return out
+
+
+def w2v_keep_rows(x, inv):
+    _need(x, f32, "x"), _need(inv, torch.int32, "inv")
+    out = torch.empty_like(x)
+    check(lib().eb_w2v_keep_rows(_p(x), _p(inv), _p(out), inv.numel(), x.shape[-1], _s()), "eb_w2v_keep_rows")
+    return out
+
+
+def w2v_gather(x, idx):
+    """x [B, T, D], idx [B, M] int32 -> [B, M, D]."""
+    _need(x, f32, "x"), _need(idx, torch.int32, "idx")
+    B, T, D = x.shape
+    M = idx.shape[1]
+    out = torch.empty(B, M, D, dtype=f32, device=x.device)
+    check(lib().eb_w2v_gather(_p(x), _p(idx), _p(out), B, T, M, D, _s()), "eb_w2v_gather")
+    return out
+
+
+def w2v_scatter(x, inv):
+    """x [B, M, D], inv [B, T] int32 -> [B, T, D] (zeros in unmasked rows)."""
+    _need(x, f32, "x"), _need(inv, torch.int32, "inv")
+    B, M, D = x.shape
+    T = inv.shape[1]
+    out = torch.empty(B, T, D, dtype=f32, device=x.device)
+    check(lib().eb_w2v_scatter(_p(x), _p(inv), _p(out), B, T, M, D, _s()), "eb_w2v_scatter")
+    return out
+
+
+def w2v_sq_mean(x):
+    _need(x, f32, "x")
+    out = torch.empty((), dtype=f32, device=x.device)
+    check(lib().eb_w2v_sq_mean(_p(x), x.numel(), _p(out), _s()), "eb_w2v_sq_mean")
+    return out
+
+
+def w2v_scale(x, g, alpha=1.0, out=None):
+    """x * g (a device scalar) * alpha."""
+    _need(x, f32, "x"), _need(g, f32, "g")
+    out = torch.empty_like(x) if out is None else out
+    check(lib().eb_w2v_scale(_p(x), _p(g), float(alpha), x.numel(), _p(out), _s()), "eb_w2v_scale")
+    return out
+
+
+def w2v_quant_fwd(logits, noise, vars, G, tau):
+    """logits [N, G*V], noise like logits or None (eval), vars [G*V, vd] -> q [N, G*vd], p, s (None in eval), X,
+    k0, k [N, G] int32, st [N, G]."""
+    _need(logits, f32, "logits"), _need(vars, f32, "vars")
+    if noise is not None:
+        _need(noise, f32, "noise")
+    N, GV = logits.shape
+    V, vd = GV // G, vars.shape[-1]
+    dev = logits.device
+    q = torch.empty(N, G * vd, dtype=f32, device=dev)
+    p, X = torch.empty_like(logits), torch.empty_like(logits)
+    s = torch.empty_like(logits) if noise is not None else None
+    k0 = torch.empty(N, G, dtype=torch.int32, device=dev)
+    k = torch.empty(N, G, dtype=torch.int32, device=dev)
+    st = torch.empty(N, G, dtype=f32, device=dev)
+    check(lib().eb_w2v_quant_fwd(_p(logits), _p(noise), _p(vars), N, G, V, vd, float(tau), _p(q), _p(p), _p(s), _p(X),
+                                 _p(k0), _p(k), _p(st), _s()), "eb_w2v_quant_fwd")
+    return q, p, s, X, k0, k, st
+
+
+def w2v_quant_stats(p, k0, G):
+    """-> (out [2] = prob_perplexity, code_perplexity; coef [G*V])."""
+    N, GV = p.shape
+    psum = colsum(p)
+    out = torch.empty(2, dtype=f32, device=p.device)
+    coef = torch.empty(GV, dtype=f32, device=p.device)
+    counts = torch.empty(GV, dtype=torch.int32, device=p.device)
+    check(lib().eb_w2v_quant_stats(_p(psum), _p(k0), N, G, GV // G, _p(out), _p(coef), _p(counts), _s()),
+          "eb_w2v_quant_stats")
+    return out, coef
+
+
+def w2v_quant_bwd(dsoft, s, p, coef, g_ppl, G, tau):
+    ref = dsoft if dsoft is not None else p
+    N, GV = ref.shape
+    dl = torch.empty(N, GV, dtype=f32, device=ref.device)
+    check(lib().eb_w2v_quant_bwd(_p(dsoft), _p(s), _p(p), _p(coef), _p(g_ppl), N, G, GV // G, float(tau), _p(dl), _s()),
+          "eb_w2v_quant_bwd")
+    return dl
+
+
+COS_EPS = 1e-8          # torch.cosine_similarity's default eps
+
+
+def w2v_logits_fwd(xp, yp, neg, temp):
+    """xp, yp [B, M, D], neg [B, M, K] int32 -> logits [K+1, B, M] and the saved (xh, yh, xn, yn, cos)."""
+    _need(xp, f32, "xp"), _need(yp, f32, "yp"), _need(neg, torch.int32, "neg")
+    B, M, D = xp.shape
+    K = neg.shape[-1]
+    dev = xp.device
+    xh, yh = torch.empty_like(xp), torch.empty_like(yp)
+    xn = torch.empty(B, M, dtype=f32, device=dev)
+    yn = torch.empty(B, M, dtype=f32, device=dev)
+    cos = torch.empty(K + 1, B, M, dtype=f32, device=dev)
+    logits = torch.empty(K + 1, B, M, dtype=f32, device=dev)
+    check(lib().eb_w2v_logits_fwd(_p(xp), _p(yp), _p(neg), B, M, D, K, float(temp), COS_EPS, _p(xh), _p(yh), _p(xn),
+                                  _p(yn), _p(cos), _p(logits), _s()), "eb_w2v_logits_fwd")
+    return logits, (xh, yh, xn, yn, cos)
+
+
+def w2v_logits_bwd(dlogits, cos, neg, xh, yh, xp, yp, xn, yn, temp):
+    _need(dlogits, f32, "dlogits")
+    B, M, D = xp.shape
+    K = neg.shape[-1]
+    A = torch.empty(B, M, M, dtype=f32, device=xp.device)
+    AC = torch.empty_like(A)
+    dxp, dyp = torch.empty_like(xp), torch.empty_like(yp)
+    check(lib().eb_w2v_logits_bwd(_p(dlogits), _p(cos), _p(neg), _p(xh), _p(yh), _p(xp), _p(yp), _p(xn), _p(yn), B, M,
+                                  D, K, float(temp), COS_EPS, _p(A), _p(AC), _p(dxp), _p(dyp), _s()),
+          "eb_w2v_logits_bwd")
+    return dxp, dyp
+
+
+def w2v_ce(logits):
+    """logits [C, B, M] -> (grad [C, B, M] of the summed cross-entropy, out [2] = summed loss, correct rows)."""
+    _need(logits, f32, "logits")
+    C, B, M = logits.shape
+    grad = torch.empty_like(logits)
+    out = torch.empty(2, dtype=f32, device=logits.device)
+    check(lib().eb_w2v_ce(_p(logits), B, M, C, _p(grad), _p(out), _s()), "eb_w2v_ce")
+    return grad, out

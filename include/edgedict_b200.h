@@ -460,6 +460,46 @@ int eb_conv1d_bf16(const void* x16, long x_rows, int s, int C, int row0, const v
 int eb_gemm_f32_splitk(const float* A, long sam, long sak, const float* B, long sbk, long sbn, float* part, int M,
                        int N, int K, int kchunk, void* stream);
 
+/* ---- wav2vec pre-training head: Wav2Vec / ConstrastiveCriterion (rnnt/wav2vec.py), GumbelVectorQuantizer
+ * (modules/softmax_vector_quantizer.py), csrc/w2v.cu.  Masked frames per utterance: idx int32 [B, M] (ascending frame
+ * numbers) and inv int32 [B, T] (m of a masked frame, -1 otherwise).  Fixed-order reductions, no float atomics.
+ * eb_w2v_mask_fwd    : out[r] = inv[r] >= 0 ? mask_emb : x[r] over rows = B*T rows of D (x[mask] = mask_emb, out of place).
+ * eb_w2v_keep_rows   : out[r] = inv[r] >= 0 ? 0 : x[r].
+ * eb_w2v_gather      : out[b, m] = x[b, idx[b, m]];  eb_w2v_scatter: out[b, t] = inv[b, t] >= 0 ? x[b, inv[b, t]] : 0.
+ * eb_w2v_sq_mean     : out[0] = sum(x^2) / n (one CTA, fixed order).  eb_w2v_scale: out = x * g[0] * alpha (may alias).
+ * eb_w2v_quant_fwd   : logits, noise (NULL: eval), p, s, X [N, G*V], vars [G*V, vd], q [N, G*vd], k0, k, st [N*G]:
+ *                      k0 = argmax logits, p = softmax(logits), s = softmax((logits + noise) / tau), k = argmax s (first
+ *                      on ties), st = (1 - s_k) + s_k (fp32), X = st at k and 0 elsewhere, q[r, g] = st * vars[g*V + k].
+ *                      Eval: k = k0, st = 1, q = vars[k0] exactly; s is not written.
+ * eb_w2v_quant_stats : psum [G*V] = sum_r p, k0 -> out[0] = prob_perplexity, out[1] = code_perplexity, coef [G*V] =
+ *                      d prob_perplexity / d mean_r p; counts int [G*V] scratch.
+ * eb_w2v_quant_bwd   : dlogits = (1/tau) s (dsoft - <s, dsoft>) + (g_ppl[0] / N) p (coef - <p, coef>) per (row, group);
+ *                      dsoft or g_ppl may be NULL (that term is dropped).
+ * eb_w2v_logits_fwd  : xp, yp [B, M, D], neg int32 [B, M, K] (frames of the same utterance) -> xh, yh (rows over
+ *                      max(|row|, eps)), xn, yn [B*M] (|row|), cosv and logits [K+1, B, M]: candidate 0 is row m of yp,
+ *                      candidate 1 + k row neg[b, m, k]; logits = cos / temp, -inf where a negative equals yp[b, m].
+ * eb_w2v_logits_bwd  : dlogits [K+1, B, M] -> dxp, dyp; A, AC [B, M, M] scratch.
+ * eb_w2v_ce          : logits [C, B, M], rows (m, b) -> grad (softmax - onehot(0)), out[0] = sum of lse - logit 0,
+ *                      out[1] = rows whose argmax is 0 and argmin is not (first index on ties). */
+int eb_w2v_mask_fwd(const float* x, const float* mask_emb, const int* inv, float* out, long rows, int D, void* stream);
+int eb_w2v_keep_rows(const float* x, const int* inv, float* out, long rows, int D, void* stream);
+int eb_w2v_gather(const float* x, const int* idx, float* out, int B, int T, int M, int D, void* stream);
+int eb_w2v_scatter(const float* x, const int* inv, float* out, int B, int T, int M, int D, void* stream);
+int eb_w2v_sq_mean(const float* x, long n, float* out, void* stream);
+int eb_w2v_scale(const float* x, const float* g, float alpha, long n, float* out, void* stream);
+int eb_w2v_quant_fwd(const float* logits, const float* noise, const float* vars, int N, int G, int V, int vd,
+                     float tau, float* q, float* p, float* s, float* X, int* k0, int* k, float* st, void* stream);
+int eb_w2v_quant_stats(const float* psum, const int* k0, int N, int G, int V, float* out, float* coef, int* counts,
+                       void* stream);
+int eb_w2v_quant_bwd(const float* dsoft, const float* s, const float* p, const float* coef, const float* g_ppl, int N,
+                     int G, int V, float tau, float* dlogits, void* stream);
+int eb_w2v_logits_fwd(const float* xp, const float* yp, const int* neg, int B, int M, int D, int K, float temp,
+                      float eps, float* xh, float* yh, float* xn, float* yn, float* cosv, float* logits, void* stream);
+int eb_w2v_logits_bwd(const float* dlogits, const float* cosv, const int* neg, const float* xh, const float* yh,
+                      const float* xp, const float* yp, const float* xn, const float* yn, int B, int M, int D, int K,
+                      float temp, float eps, float* A, float* AC, float* dxp, float* dyp, void* stream);
+int eb_w2v_ce(const float* logits, int B, int M, int C, float* grad, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
