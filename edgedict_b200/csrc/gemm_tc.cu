@@ -315,7 +315,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                         const int u = (int)(cell % lse.maxU);
                         const long bt = cell / lse.maxU;
                         const int t = (int)(bt % lse.maxT), b = (int)(bt / lse.maxT);
-                        const int Tn = lse.xlen[b], Un = lse.ylen[b] + 1;
+                        const int Tn = min(max(lse.xlen[b], 0), lse.maxT);       // clamped as in loss.cu
+                        const int Un = min(max(lse.ylen[b], 0) + 1, lse.maxU);
                         cell_ok[h] = t < Tn && u < Un;
                         if (cell_ok[h] && u < Un - 1) lab[h] = lse.labels[b * (lse.maxU - 1) + u];
                     }

@@ -19,6 +19,8 @@
 // compute_rnnt_loss(), whose contract returns costs in HOST memory (include/rnnt.h).
 //
 // Arithmetic follows include/detail/gpu_rnnt_kernel.h:5-179 and rnnt_helper.h:17-24.
+#include <atomic>
+
 #include "common.cuh"
 #include "../../include/rnnt.h"
 #include "../../include/edgedict_b200.h"
@@ -47,6 +49,11 @@ __device__ __forceinline__ T lse2(T a, T b) {   // rnnt_helper.h:17-24
     if (b == M<T>::ninf()) return a;
     return (a > b) ? M<T>::log1p_acc(M<T>::exp_acc(b - a)) + a : M<T>::log1p_acc(M<T>::exp_acc(a - b)) + b;
 }
+
+// The lengths every kernel here uses: the valid cells of utterance b are t < Tn, u < Un, which never leave its own
+// [maxT, maxU] block whatever xlen / ylen hold (include/edgedict_b200.h).
+__device__ __forceinline__ int clamp_T(int xlen, int maxT) { return min(max(xlen, 0), maxT); }
+__device__ __forceinline__ int clamp_U(int ylen, int maxU) { return min(max(ylen, 0) + 1, maxU); }
 
 // 4-wide row access; VEC=true requires V % 4 == 0 (row starts are then 16-byte aligned for fp32)
 template <typename T, bool VEC> struct Row4 {
@@ -101,7 +108,7 @@ rnnt_denom_kernel(const T* __restrict__ logits, const int* __restrict__ labels,
         const long bt = cell / maxU;
         const int t = (int)(bt % maxT);
         const int b = (int)(bt / maxT);
-        const int Tn = xlen[b], Un = ylen[b] + 1;
+        const int Tn = clamp_T(xlen[b], maxT), Un = clamp_U(ylen[b], maxU);
         if (t >= Tn || u >= Un) continue;                // padded cell: never read
         const T* row = logits + cell * (long)V;
         const int lab = (u < Un - 1) ? labels[b * (maxU - 1) + u] : -1;
@@ -139,22 +146,23 @@ rnnt_denom_kernel(const T* __restrict__ logits, const int* __restrict__ labels,
 
 // ---------------------------------------------------------------------------------------------
 // 2. alpha / beta wavefronts.  grid = (B, 2): y == 0 -> alphas, y == 1 -> betas.
-//    blockDim.x = maxU rounded up to a warp.  Thread u walks its own column t = n - u.
+//    blockDim.x = maxU rounded up to a warp.  Thread u walks its own column t = n - u, with the log-probs of the
+//    next PF diagonals in flight in registers.  An utterance without frames (Tn = 0) has no diagonal: ll = -inf.
 // ---------------------------------------------------------------------------------------------
 template <typename T, int PF>
-__global__ void rnnt_lattice_kernel(const T* __restrict__ lpb, const T* __restrict__ lpl,
-                                    const int* __restrict__ xlen, const int* __restrict__ ylen,
-                                    T* __restrict__ alphas, T* __restrict__ betas,
-                                    T* __restrict__ ll_fwd, T* __restrict__ ll_bwd,
-                                    int maxT, int maxU, int do_beta) {
+__device__ __forceinline__ void lattice_body(const T* __restrict__ lpb, const T* __restrict__ lpl,
+                                             const int* __restrict__ xlen, const int* __restrict__ ylen,
+                                             T* __restrict__ alphas, T* __restrict__ betas,
+                                             T* __restrict__ ll_fwd, T* __restrict__ ll_bwd,
+                                             int maxT, int maxU, int do_beta) {
     extern __shared__ unsigned char sm_raw[];
     T* sh = reinterpret_cast<T*>(sm_raw);               // [2][blockDim.x]
     const int b = blockIdx.x, u = threadIdx.x;
-    const int Tn = xlen[b], Un = ylen[b] + 1;
+    const int Tn = clamp_T(xlen[b], maxT), Un = clamp_U(ylen[b], maxU);
     const long base = (long)b * maxT * maxU;
     const T* pb = lpb + base;
     const T* pl = lpl + base;
-    const int ND = Tn + Un - 1;                          // number of anti-diagonals
+    const int ND = Tn > 0 ? Tn + Un - 1 : 0;             // number of anti-diagonals
     const bool act = u < Un;
     const int W = blockDim.x;
     if (blockIdx.y == 0) {
@@ -198,7 +206,7 @@ __global__ void rnnt_lattice_kernel(const T* __restrict__ lpb, const T* __restri
 #pragma unroll
             for (int i = 0; i < PF; ++i) { cb[i] = nb[i]; cl[i] = nl[i]; }
         }
-        if (u == Un - 1) ll_fwd[b] = self + pb[(long)(Tn - 1) * maxU + Un - 1];
+        if (u == Un - 1) ll_fwd[b] = Tn > 0 ? self + pb[(long)(Tn - 1) * maxU + Un - 1] : M<T>::ninf();
     } else {
         if (!do_beta) return;
         T* be = betas + base;
@@ -243,8 +251,32 @@ __global__ void rnnt_lattice_kernel(const T* __restrict__ lpb, const T* __restri
 #pragma unroll
             for (int i = 0; i < PF; ++i) { cb[i] = nb[i]; cl[i] = nl[i]; }
         }
-        if (u == 0) ll_bwd[b] = self;
+        if (u == 0) ll_bwd[b] = self;                    // -inf when Tn = 0: no cell was written
     }
+}
+
+// The kernel for blocks of up to the thread count its registers allow (896 fp32 / 544 fp64 threads with ptxas of
+// CUDA 12.9), and the one for wider blocks: a shallower ring in the registers a 1024-thread block leaves.  The ring's
+// depth only moves loads earlier, so both give the same bits.
+template <typename T>
+__global__ void rnnt_lattice_kernel(const T* __restrict__ lpb, const T* __restrict__ lpl,
+                                    const int* __restrict__ xlen, const int* __restrict__ ylen,
+                                    T* __restrict__ alphas, T* __restrict__ betas,
+                                    T* __restrict__ ll_fwd, T* __restrict__ ll_bwd,
+                                    int maxT, int maxU, int do_beta) {
+    lattice_body<T, 8>(lpb, lpl, xlen, ylen, alphas, betas, ll_fwd, ll_bwd, maxT, maxU, do_beta);
+}
+
+template <typename T> constexpr int LATTICE_WIDE_PF = sizeof(T) == 8 ? 2 : 4;
+
+template <typename T>
+__global__ void __launch_bounds__(1024)
+rnnt_lattice_wide_kernel(const T* __restrict__ lpb, const T* __restrict__ lpl,
+                         const int* __restrict__ xlen, const int* __restrict__ ylen,
+                         T* __restrict__ alphas, T* __restrict__ betas,
+                         T* __restrict__ ll_fwd, T* __restrict__ ll_bwd,
+                         int maxT, int maxU, int do_beta) {
+    lattice_body<T, LATTICE_WIDE_PF<T>>(lpb, lpl, xlen, ylen, alphas, betas, ll_fwd, ll_bwd, maxT, maxU, do_beta);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -267,7 +299,7 @@ __global__ void __launch_bounds__(1024) rnnt_viterbi_kernel(const T* __restrict_
     int* pos = fr + W;                                   // [2] the backtrace's (t, u) between bands
     unsigned char* stage = reinterpret_cast<unsigned char*>(pos + 2);   // [rows][maxU] decision bytes
     const int b = blockIdx.x, u = threadIdx.x;
-    const int Tn = min(max(xlen[b], 0), maxT), Un = min(max(ylen[b], 0) + 1, maxU);
+    const int Tn = clamp_T(xlen[b], maxT), Un = clamp_U(ylen[b], maxU);
     const long base = (long)b * maxT * maxU;
     unsigned char* dec = dec_global ? dec_global + base : stage;
     const T* pb = lpb + base;
@@ -401,7 +433,7 @@ rnnt_grad_kernel(const TI* logits, TO* grads, const int* __restrict__ labels,
         const long bt = cell / maxU;
         const int t = (int)(bt % maxT);
         const int b = (int)(bt / maxT);
-        const int Tn = xlen[b], Un = ylen[b] + 1;
+        const int Tn = clamp_T(xlen[b], maxT), Un = clamp_U(ylen[b], maxU);
         const TI* row = logits + cell * (long)V;
         TO* orow = grads + cell * (long)V;
         if (t >= Tn || u >= Un) {                         // padded: zero, logits never read
@@ -462,7 +494,7 @@ rnnt_grad_bf16x8_kernel(const __nv_bfloat16* logits, __nv_bfloat16* grads, const
         const long bt = cell / maxU;
         const int t = (int)(bt % maxT);
         const int b = (int)(bt / maxT);
-        const int Tn = xlen[b], Un = ylen[b] + 1;
+        const int Tn = clamp_T(xlen[b], maxT), Un = clamp_U(ylen[b], maxU);
         const __nv_bfloat16* row = logits + cell * (long)V;
         __nv_bfloat16* orow = grads + cell * (long)V;
         if (t >= Tn || u >= Un) {
@@ -534,6 +566,34 @@ struct Workspace {
     }
 };
 
+// alpha / beta launch: the PF = 8 kernel when its register count lets a block of maxU threads (rounded up to a warp)
+// launch, else the wide one.  The limit comes from the compiled kernel, queried once per device.
+template <typename T>
+int launch_lattice(const Workspace<T>& w, const int* xlen, const int* ylen, int B, int maxT, int maxU, int need_beta,
+                   cudaStream_t st) {
+    // per device, each slot written once with the value any racing writer also computes
+    static std::atomic<int> cache[64];
+    int dev;
+    EB_CUDA(cudaGetDevice(&dev));
+    int narrow_max = dev < 64 ? cache[dev].load(std::memory_order_relaxed) : 0;
+    if (!narrow_max) {
+        cudaFuncAttributes a;
+        EB_CUDA(cudaFuncGetAttributes(&a, rnnt_lattice_kernel<T>));
+        narrow_max = a.maxThreadsPerBlock;
+        if (dev < 64) cache[dev].store(narrow_max, std::memory_order_relaxed);
+    }
+    const int threads = ((maxU + 31) / 32) * 32;
+    const size_t smem = 2 * threads * sizeof(T);
+    if (threads <= narrow_max)
+        rnnt_lattice_kernel<T><<<dim3(B, 2), threads, smem, st>>>(w.lpb, w.lpl, xlen, ylen, w.alphas, w.betas,
+                                                                  w.ll_fwd, w.ll_bwd, maxT, maxU, need_beta);
+    else
+        rnnt_lattice_wide_kernel<T><<<dim3(B, 2), threads, smem, st>>>(w.lpb, w.lpl, xlen, ylen, w.alphas, w.betas,
+                                                                       w.ll_fwd, w.ll_bwd, maxT, maxU, need_beta);
+    EB_CHECK_LAUNCH();
+    return EB_OK;
+}
+
 inline int row_grid(long ncells, int warps) {
     long blocks = (ncells + warps - 1) / warps;
     long cap = (long)eb_num_sms() * 16;                  // grid-stride above 16 CTAs/SM
@@ -563,11 +623,7 @@ int loss_fwd(const T* logits, const int* labels, const int* xlen, const int* yle
         rnnt_denom_kernel<T, false, WARPS><<<row_grid(ncells, WARPS), WARPS * 32, 0, st>>>(
             logits, labels, xlen, ylen, w.denom, w.lpb, w.lpl, B, maxT, maxU, V, blank);
     EB_CHECK_LAUNCH();
-    const int threads = ((maxU + 31) / 32) * 32;
-    rnnt_lattice_kernel<T, 8><<<dim3(B, 2), threads, 2 * threads * sizeof(T), st>>>(
-        w.lpb, w.lpl, xlen, ylen, w.alphas, w.betas, w.ll_fwd, w.ll_bwd, maxT, maxU, need_beta);
-    EB_CHECK_LAUNCH();
-    return EB_OK;
+    return launch_lattice<T>(w, xlen, ylen, B, maxT, maxU, need_beta, st);
 }
 
 template <typename T, typename TO>
@@ -736,10 +792,8 @@ EB_API int eb_rnnt_loss_lattice(const int* xlen, const int* ylen, int B, int max
     if (!xlen || !ylen || !workspace || B <= 0 || maxT <= 0 || maxU <= 0 || maxU > 1024) return EB_ERR_INVALID;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     Workspace<float> w(workspace, B, maxT, maxU);
-    const int threads = ((maxU + 31) / 32) * 32;
-    rnnt_lattice_kernel<float, 8><<<dim3(B, 2), threads, 2 * threads * sizeof(float), st>>>(
-        w.lpb, w.lpl, xlen, ylen, w.alphas, w.betas, w.ll_fwd, w.ll_bwd, maxT, maxU, need_beta);
-    EB_CHECK_LAUNCH();
+    const int rc = launch_lattice<float>(w, xlen, ylen, B, maxT, maxU, need_beta, st);
+    if (rc) return rc;
     if (costs_dev) neg_copy_kernel<float><<<(B + 127) / 128, 128, 0, st>>>(w.ll_fwd, costs_dev, B);
     EB_CHECK_LAUNCH();
     return EB_OK;

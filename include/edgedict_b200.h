@@ -19,7 +19,12 @@ extern "C" {
 /* ---- RNN-T loss, device-resident costs, no host sync ------------------------------------
  * replaces warp-transducer/include/detail/gpu_rnnt.h:82-215 (GpuRNNT::compute_cost_and_score)
  * and warprnnt_pytorch/__init__.py:10-50 (_RNNT.forward/backward).
- *   logits [B,maxT,maxU,V] (dtype_size 4|8), labels [B,maxU-1] int32, xlen/ylen [B] int32. */
+ *   logits [B,maxT,maxU,V] (dtype_size 4|8), labels [B,maxU-1] int32, xlen/ylen [B] int32, 1 <= maxU <= 1024.
+ * Lengths (eb_rnnt_loss_fwd / _bwd / _lattice / _bwd_bf16 and eb_joint_logits_lse alike): utterance b has the cells
+ *   t < T = min(max(xlen[b], 0), maxT), u < U = min(max(ylen[b], 0), maxU-1) + 1, the same clamp as eb_rnnt_viterbi;
+ *   no kernel reads or writes a cell, a label or a gradient row of b outside them, other than zero-filling the
+ *   gradient of its padded cells.
+ * T = 0 has no alignment: ll_fwd = ll_bwd = -inf (cost +inf) and a zero gradient. */
 size_t eb_rnnt_workspace_bytes(int B, int maxT, int maxU, int dtype_size);
 int eb_rnnt_loss_fwd(const void* logits, const int* labels, const int* xlen, const int* ylen,
                      int B, int maxT, int maxU, int V, int blank, int dtype_size,
@@ -50,7 +55,7 @@ int eb_rnnt_workspace_views(void* workspace, int B, int maxT, int maxU, int dtyp
  * The best path is backtraced from (T-1, U-1): frames [B, maxU-1] int32 holds the frame t at which label u is emitted
  * (the step (t,u) -> (t,u+1)) and label_logp [B, maxU-1] (workspace dtype) lpl(t,u); past ylen[b] they are -1 and 0
  * (both may be NULL when maxU = 1).
- * T = 0 has no alignment: score -inf, frames -1 and label_logp -inf for every label.
+ * T = 0 has no alignment: score -inf, frames -1 and label_logp -inf for every label (the loss: cost +inf).
  * decisions: eb_rnnt_align_bytes(B, maxT, maxU) bytes of scratch, NULL allowed when that is 0 (the decisions then stay
  * in shared memory).  No host synchronisation. */
 size_t eb_rnnt_align_bytes(int B, int maxT, int maxU);
@@ -145,7 +150,8 @@ int eb_gemm_bf16_dtanh(const void* A, int a_mn_major, const void* B, int b_mn_ma
 
 /* joint output layer + softmax statistics in one GEMM (bf16 mode): replaces the second Linear of Joint
  * (rnnt/models.py:165) together with reduce_max/reduce_exp (warp-transducer reduce.h:45-104) and the
- * blank/label gathers of the lattice kernels.  denom/lpb/lpl: the first three arrays of the loss workspace. */
+ * blank/label gathers of the lattice kernels.  denom/lpb/lpl: the first three arrays of the loss workspace, written
+ * for the valid cells of the loss's length rule above. */
 int eb_joint_logits_lse(const void* hidden16, const void* w2_16, const float* b2, void* logits16, const int* labels,
                         const int* xlen, const int* ylen, float* denom, float* lpb, float* lpl, int B, int maxT,
                         int maxU, int V, int J, int blank, void* stream);

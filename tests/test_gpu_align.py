@@ -70,27 +70,6 @@ def _check_rnnt(frames, logp, score, lpb, lpl, xlen, ylen, costs=None):
             assert score[b] <= -costs[b] + 1e-5 * abs(costs[b]) + 1e-5, (b, score[b], costs[b])
 
 
-# eb_rnnt_loss_fwd's alpha / beta kernel needs more registers than a 1024-thread CTA leaves: it launches up to
-# U + 1 = 896 in fp32 and 544 in fp64.  Wider lattices get their workspace from torch here; the Viterbi kernel itself
-# runs a full CTA.
-LOSS_MAX_U = 544
-
-
-def _workspace_from_torch(acts, labels, blank):
-    B, T, U1, V = acts.shape
-    from edgedict_b200 import _lib
-    n = B * T * U1
-    ws = torch.zeros(_lib.lib().eb_rnnt_workspace_bytes(B, T, U1, acts.element_size()), dtype=torch.uint8,
-                     device=acts.device)
-    lp = acts.log_softmax(-1)
-    lab = torch.zeros(B, U1, dtype=torch.long, device=acts.device)
-    lab[:, :U1 - 1] = labels.long()
-    w = ws.view(acts.dtype)
-    w[n:2 * n] = lp[..., blank].reshape(-1)
-    w[2 * n:3 * n] = lp.gather(-1, lab[:, None, :, None].expand(B, T, U1, 1)).reshape(-1)
-    return ws
-
-
 RNNT_CASES = [
     (1, 1, 1, 5, f32, 0, "random"),
     (3, 17, 5, 11, f32, 0, "random"),
@@ -98,7 +77,7 @@ RNNT_CASES = [
     (5, 40, 7, 13, f32, 12, "random"),                      # blank = V - 1
     (4, 30, 6, 9, f64, 0, "random"),
     (3, 1000, 20, 8, f32, 0, "random"),
-    (2, 100, 1024, 4, f32, 0, "random"),                    # a full CTA, decisions in shared memory
+    (2, 100, 1024, 4, f32, 0, "random"),                    # a full CTA, decisions in shared memory; the wide lattice
     (2, 300, 1024, 4, f32, 3, "random"),                    # a full CTA, decisions in the caller's buffer
     (1, 1000, 1024, 2, f32, 0, "random"),
     (2, 50, 1024, 3, f64, 0, "random"),
@@ -116,18 +95,14 @@ def test_rnnt_viterbi_teacher_forced_bitwise(B, T, U1, V, dtype, blank, kind):
     from edgedict_b200.align import rnnt_forced_align
     acts, labels, xlen, ylen = _rnnt_problem(B, T, U1, V, dtype, blank, kind, B * 1000 + T + U1)
     xl, yl = xlen.cuda(), ylen.cuda()
-    if U1 <= LOSS_MAX_U:
-        costs, ws = ops.rnnt_loss_fwd(acts, labels, xl, yl, blank, need_beta=False)
-        costs = _np(costs)
-    else:                                                    # the workspace filled by its documented layout
-        ws, costs = _workspace_from_torch(acts, labels, blank), None
+    costs, ws = ops.rnnt_loss_fwd(acts, labels, xl, yl, blank, need_beta=False)
+    costs = _np(costs)
     out = ops.rnnt_viterbi(xl, yl, B, T, U1, ws, dtype)
     lpb, lpl = _ws_logprobs(ws, B, T, U1, dtype)
     _check_rnnt(*out, lpb, lpl, xlen, ylen, costs)
-    if U1 <= LOSS_MAX_U:
-        again = rnnt_forced_align(acts, labels, xlen, ylen, blank=blank)
-        for a, b in zip(out, again):
-            assert torch.equal(a, b)
+    again = rnnt_forced_align(acts, labels, xlen, ylen, blank=blank)
+    for a, b in zip(out, again):
+        assert torch.equal(a, b)
     if kind == "constant":                                   # every path ties: all labels at the first frame
         assert np.all(_np(out[0])[0] == 0)
 

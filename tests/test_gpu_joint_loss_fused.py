@@ -22,6 +22,7 @@ import pytest
 import torch
 
 from oracle import loss as ol
+from tests import loss_restate as lr
 
 pytestmark = pytest.mark.gpu
 
@@ -65,21 +66,6 @@ CASES = {
 }
 
 
-def _labels(rng, B, U, V, blank):
-    """Random labels != blank, with columns 127, 128, V - 1 and the two neighbours of the blank planted in every row
-    (label capture at tile edges)."""
-    if U == 1:
-        return np.zeros((B, 0), np.int32)
-    r = rng.randint(0, V - 1, size=(B, U - 1))
-    lab = r + (r >= blank)
-    special = [c for c in (127, 128, V - 1, blank - 1, blank + 1) if 0 <= c < V and c != blank]
-    for b in range(B):
-        for i, c in enumerate(special[b % len(special):] + special[:b % len(special)]):
-            if i < U - 1:
-                lab[b, (i + b) % (U - 1)] = c
-    return lab.astype(np.int32)
-
-
 def _make_case(name):
     B, T, U, V, J, blank, xl, yl, bias = CASES[name]
     seed = sum(map(ord, name))
@@ -97,7 +83,7 @@ def _make_case(name):
     X = hid.double() @ w2.double().t()
     if bias:
         X += b2.double()
-    lab = _labels(rng, B, U, V, blank)
+    lab = lr.planted_labels(rng, B, U, V, blank)
     xlen, ylen = np.asarray(xl, np.int32), np.asarray(yl, np.int32)
     t = np.arange(T)[None, :, None]
     u = np.arange(U)[None, None, :]
@@ -342,29 +328,9 @@ def _restated_grad(c, L16):
 
 
 def _grad_formula(c, a, b, d, ll, x):
-    """g [B,T,U,V] fp64 from alpha, beta, denom [B,T,U], ll [B] and the logits x, zero on padded cells."""
-    B, T, U, blank = c["B"], c["T"], c["U"], c["blank"]
-    valid = torch.as_tensor(c["valid"], device="cuda")
-    ll = ll[:, None, None]
-    ninf = torch.full_like(a, -math.inf)
-    c_all = torch.where(valid, a + b - ll + d, ninf)
-    g = torch.exp(c_all[..., None] + x)
-    t_idx = torch.arange(T, device="cuda")[None, :, None]
-    u_idx = torch.arange(U, device="cuda")[None, None, :]
-    Tn = c["xlen_d"].long()[:, None, None]
-    Un = c["ylen_d"].long()[:, None, None] + 1
-    b_next_t = torch.cat([b[:, 1:], ninf[:, :1]], dim=1)
-    c_blank = torch.where(t_idx < Tn - 1, a - ll + d + b_next_t, torch.where(u_idx == Un - 1, a - ll + d, ninf))
-    c_blank = torch.where(valid, c_blank, ninf)
-    g[..., blank] -= torch.exp(c_blank + x[..., blank])
-    if U > 1:
-        b_next_u = torch.cat([b[:, :, 1:], ninf[:, :, :1]], dim=2)
-        c_lab = torch.where(valid & (u_idx < Un - 1), a - ll + d + b_next_u, ninf)[:, :, :U - 1]
-        lab = c["lab_d"].long()[:, None, :, None].expand(B, T, U - 1, 1)
-        xl = torch.gather(x[:, :, :U - 1], 3, lab)
-        g[:, :, :U - 1].scatter_add_(3, lab, -torch.exp(c_lab[..., None] + xl))
-    g[~valid] = 0
-    return g
+    """g [B,T,U,V] fp64 from alpha, beta, denom [B,T,U], ll [B] and the logits x, zero on padded cells
+    (loss_restate.grad_formula)."""
+    return lr.grad_formula(a, b, d, ll, x, c["lab"], c["xlen_d"], c["ylen_d"], c["blank"])
 
 
 def test_chained_path_as_joint_loss_runs_it(case):
