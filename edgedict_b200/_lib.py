@@ -10,6 +10,14 @@ _lib = None
 
 P, I, L, F, D, Z = C.c_void_p, C.c_int, C.c_long, C.c_float, C.c_double, C.c_size_t
 
+OPT_MAX_GROUPS = 16
+
+
+class OptHyper(C.Structure):
+    """eb_opt_hyper: the per-group optimizer hyperparameters, passed by value."""
+    _fields_ = [(k, D * OPT_MAX_GROUPS) for k in ("lr", "wd", "b1", "b2", "eps")]
+
+
 # name -> (restype, argtypes); mirrors include/edgedict_b200.h one to one
 SIGNATURES = {
     "eb_rnnt_workspace_bytes": (Z, [I, I, I, I]),
@@ -90,6 +98,12 @@ SIGNATURES = {
     "eb_adam_step": (I, [P, P, P, P, L, F, F, F, F, F, I, F, P]),
     "eb_adam_step_ex": (I, [P, P, P, P, L, F, F, F, F, F, I, F, P, F, I, P]),
     "eb_sumsq": (I, [P, L, P, P]),
+    "eb_opt_seg_sumsq": (I, [P, P, I, P, I, P, P, P, P]),
+    "eb_opt_prologue": (I, [P, F, F, I, P, P, P]),
+    "eb_opt_sgd_step": (I, [P, P, P, P, P, I, OptHyper, I, P, P, P]),
+    "eb_opt_sm3_step": (I, [P, P, P, P, L, P, P, I, OptHyper, I, P, P]),
+    "eb_opt_adamw_step": (I, [P, P, P, P, P, P, I, OptHyper, I, P, P, P]),
+    "eb_opt_novograd_step": (I, [P, P, P, P, P, P, I, P, I, OptHyper, I, P, P]),
     "eb_fe_preemph_pad": (I, [P, P, I, I, L, I, F, I, P]),
     "eb_fe_power": (I, [P, P, L, I, P]),
     "eb_fe_log_stack": (I, [P, P, I, I, I, I, I, I, I, I, P]),

@@ -824,6 +824,38 @@ def sumsq(x, out):
     check(lib().eb_sumsq(_p(x), x.numel(), _p(out), _s()), "eb_sumsq")
 
 
+# ---- the flat optimizers (optim.FlatOptimizer): seg / tiles are the int64 eb_opt_seg / eb_opt_tile tables, h an
+# _lib.OptHyper, ctl float [2], steps int32 [groups] ------------------------------------------------------------------
+def opt_seg_sumsq(g, seg, tiles, partial, segsum, total=None):
+    check(lib().eb_opt_seg_sumsq(_p(g), _p(seg), seg.shape[0], _p(tiles), tiles.shape[0], _p(partial), _p(segsum),
+                                 _p(total), _s()), "eb_opt_seg_sumsq")
+
+
+def opt_prologue(total, grad_scale, max_norm, steps, ctl):
+    check(lib().eb_opt_prologue(_p(total), float(grad_scale), float(max_norm or 0.0), steps.numel(), _p(steps),
+                                _p(ctl), _s()), "eb_opt_prologue")
+
+
+def opt_sgd_step(p, g, buf, seg, tiles, h, steps, ctl):
+    check(lib().eb_opt_sgd_step(_p(p), _p(g), _p(buf), _p(seg), _p(tiles), tiles.shape[0], h, steps.numel(), _p(ctl),
+                                _p(steps), _s()), "eb_opt_sgd_step")
+
+
+def opt_sm3_step(p, g, acc, acc_new, seg, tiles, h, steps, ctl):
+    check(lib().eb_opt_sm3_step(_p(p), _p(g), _p(acc), _p(acc_new), acc.numel(), _p(seg), _p(tiles), tiles.shape[0], h,
+                                steps.numel(), _p(ctl), _s()), "eb_opt_sm3_step")
+
+
+def opt_adamw_step(p, g, m, v, seg, tiles, h, steps, ctl):
+    check(lib().eb_opt_adamw_step(_p(p), _p(g), _p(m), _p(v), _p(seg), _p(tiles), tiles.shape[0], h, steps.numel(),
+                                  _p(ctl), _p(steps), _s()), "eb_opt_adamw_step")
+
+
+def opt_novograd_step(p, g, m, segv, segsum, seg, tiles, h, steps, ctl):
+    check(lib().eb_opt_novograd_step(_p(p), _p(g), _p(m), _p(segv), _p(segsum), _p(seg), seg.shape[0], _p(tiles),
+                                     tiles.shape[0], h, steps.numel(), _p(ctl), _s()), "eb_opt_novograd_step")
+
+
 # ---- log-mel front end (SURVEY 8(f) N2) ------------------------------------------------------------
 def logmel_frontend(x, basis, fbT, n_fft, hop, n_mels, n_stack, preemph, take_log=True, pad_to_divisible=True):
     """x [B, L] fp32 waveform -> [B, T, n_mels*n_stack] log-mel features (see csrc/frontend.cu).

@@ -407,6 +407,42 @@ int eb_adam_step_ex(float* p, const float* g, float* m, float* v, long n, float 
                     int adamw, void* stream);
 int eb_sumsq(const float* x, long n, float* out_accum, void* stream);
 
+/* ---- the reference trainers' optimizers over the flat buckets (optim.FlatOptimizer), csrc/optim.cu -------------------
+ * seg [nseg]: one entry per tensor: bucket offset, numel, rank (<= 4), parameter group, its tiles [tile_begin, tile_end),
+ *             shape, and for SM3 the offsets of its accumulators in the accumulator bucket (rank 0 and 1: one).
+ * tiles      : contiguous ranges [start, start + len) of one tensor (seg) cut from its own shape: whole rows of its last
+ *              dimension (ncols = the last dimension) or one piece of a row; r0 / c0 = the tile's first row / column.
+ * h          : the per-group hyperparameters, by value: lr, weight decay, b1 (SGD: momentum), b2, eps.
+ * ctl [2]    : written by eb_opt_prologue: ctl[0] = grad_scale x the clip coefficient, ctl[1] != 0: the step is skipped.
+ * steps [ngroups]: the device step counters; eb_opt_prologue advances them only when the step is taken.
+ * eb_opt_seg_sumsq : partial [ntiles] = per-tile sum g^2, segsum [nseg] = the tiles of each tensor summed in order,
+ *                    total (optional) = the tensors summed in order: no float atomics, bitwise repeatable.
+ * eb_opt_prologue  : total (optional, the unscaled sum g^2): with it, a non-finite norm skips the step and max_norm > 0
+ *                    clips like torch.nn.utils.clip_grad_norm_.
+ * eb_opt_sgd_step  : torch.optim.SGD; buf [n] may be NULL when every group's momentum is 0.
+ * eb_opt_sm3_step  : SM3 with beta = 0: reads acc [nacc], writes the new accumulators into acc_new [nacc] (zeroed here;
+ *                    a skipped step copies acc).  The caller swaps the two.
+ * eb_opt_adamw_step: the reference's AdamW; bias corrections from the device step counters.
+ * eb_opt_novograd_step: Novograd; segv [nseg] = the per-tensor second moment, segsum from eb_opt_seg_sumsq. */
+#define EB_OPT_MAX_GROUPS 16
+typedef struct { long long off, numel, rank, group, tile_begin, tile_end, shape[4], acc[4]; } eb_opt_seg;
+typedef struct { long long seg, start, len, r0, c0, ncols; } eb_opt_tile;
+typedef struct { double lr[EB_OPT_MAX_GROUPS], wd[EB_OPT_MAX_GROUPS], b1[EB_OPT_MAX_GROUPS], b2[EB_OPT_MAX_GROUPS],
+                 eps[EB_OPT_MAX_GROUPS]; } eb_opt_hyper;
+int eb_opt_seg_sumsq(const float* g, const eb_opt_seg* seg, int nseg, const eb_opt_tile* tiles, int ntiles,
+                     float* partial, float* segsum, float* total, void* stream);
+int eb_opt_prologue(const float* total, float grad_scale, float max_norm, int ngroups, int* steps, float* ctl,
+                    void* stream);
+int eb_opt_sgd_step(float* p, const float* g, float* buf, const eb_opt_seg* seg, const eb_opt_tile* tiles, int ntiles,
+                    eb_opt_hyper h, int ngroups, const float* ctl, const int* steps, void* stream);
+int eb_opt_sm3_step(float* p, const float* g, const float* acc, float* acc_new, long nacc, const eb_opt_seg* seg,
+                    const eb_opt_tile* tiles, int ntiles, eb_opt_hyper h, int ngroups, const float* ctl, void* stream);
+int eb_opt_adamw_step(float* p, const float* g, float* m, float* v, const eb_opt_seg* seg, const eb_opt_tile* tiles,
+                      int ntiles, eb_opt_hyper h, int ngroups, const float* ctl, const int* steps, void* stream);
+int eb_opt_novograd_step(float* p, const float* g, float* m, float* segv, const float* segsum, const eb_opt_seg* seg,
+                         int nseg, const eb_opt_tile* tiles, int ntiles, eb_opt_hyper h, int ngroups,
+                         const float* ctl, void* stream);
+
 /* ---- log-mel front end (the step before the path; SURVEY 8(f) N2) ------------------------------
  * replaces FilterbankFeatures.forward (rnnt/features.py:126-164) + Downsample (rnnt/transforms.py:37-51).
  * eb_fe_preemph_pad : x[B,L] -> xp[B,Lp]: pre-emphasis (features.py:137-141) and the reflect padding of
