@@ -111,6 +111,34 @@ def _tiles(seg_index, shape, numel):
     return out
 
 
+def bucket_tables(group_shapes):
+    """The bucket of tensors given as one list of shapes per parameter group, in order: (seg, tiles, offs, n, nacc).
+    seg holds one eb_opt_seg row per tensor (off, numel, rank, group, tile_begin, tile_end, shape[4], acc[4]), tiles
+    the eb_opt_tile rows of every tensor in order (``_tiles``), offs each tensor's offset (a multiple of 4), n the
+    bucket's length and nacc the length of SM3's accumulator buffer (rank <= 1: one per element, at least one; rank >= 2:
+    one per index of every dimension)."""
+    seg, tiles, offs, n, nacc = [], [], [], 0, 0
+    for gi, shapes in enumerate(group_shapes):
+        for shape in shapes:
+            i, shape = len(offs), tuple(shape)
+            k = math.prod(shape)
+            acc = [0, 0, 0, 0]
+            if len(shape) <= 1:
+                acc[0] = nacc
+                nacc += max(k, 1)
+            else:
+                for d, nd in enumerate(shape):
+                    acc[d] = nacc
+                    nacc += nd
+            t = _tiles(i, shape, k)
+            seg.append([n, k, len(shape), gi, len(tiles), len(tiles) + len(t)] + list(shape) +
+                       [0] * (4 - len(shape)) + acc)
+            tiles.extend(t)
+            offs.append(n)
+            n += (k + 3) // 4 * 4
+    return seg, tiles, offs, n, nacc
+
+
 class FlatOptimizer(torch.optim.Optimizer):
     """Base of the flat-bucket optimizers: a ``torch.optim.Optimizer`` whose parameters live in one fp32 bucket.
 
@@ -149,24 +177,7 @@ class FlatOptimizer(torch.optim.Optimizer):
         dev = ps[0].device
         if any(p.device != dev for p in ps):
             raise RuntimeError("%s needs every parameter on one device" % type(self).__name__)
-        seg, tiles, offs, n, nacc = [], [], [], 0, 0
-        for gi, g in enumerate(self.param_groups):
-            for p in g["params"]:
-                i, shape, k = len(offs), tuple(p.shape), p.numel()
-                acc = [0, 0, 0, 0]
-                if len(shape) <= 1:
-                    acc[0] = nacc
-                    nacc += max(k, 1)
-                else:
-                    for d, nd in enumerate(shape):
-                        acc[d] = nacc
-                        nacc += nd
-                t = _tiles(i, shape, k)
-                seg.append([n, k, len(shape), gi, len(tiles), len(tiles) + len(t)] + list(shape) +
-                           [0] * (4 - len(shape)) + acc)
-                tiles.extend(t)
-                offs.append(n)
-                n += (k + 3) // 4 * 4
+        seg, tiles, offs, n, nacc = bucket_tables([[p.shape for p in g["params"]] for g in self.param_groups])
         self.n = n
         self.flat_params = torch.zeros(n, dtype=torch.float32, device=dev)
         self.flat_grads = torch.zeros(n, dtype=torch.float32, device=dev)
@@ -186,9 +197,11 @@ class FlatOptimizer(torch.optim.Optimizer):
         self._grad_ptrs = [gv.data_ptr() for gv in self._grad_views]
         self._seg_host = seg
         self._seg = torch.tensor(seg, dtype=torch.int64).to(dev)
-        self._tiles = torch.tensor(tiles if tiles else [[0] * 6], dtype=torch.int64).to(dev)
+        # a bucket of empty tensors has no tile: step() then runs only the prologue (the sum of squares is 0)
+        self._ntiles = len(tiles)
+        self._tiles = torch.tensor(tiles, dtype=torch.int64).reshape(-1, 6).to(dev)
         self._nacc = nacc
-        self._partial = torch.zeros(len(tiles) or 1, dtype=torch.float32, device=dev)
+        self._partial = torch.zeros(len(tiles), dtype=torch.float32, device=dev)
         self._segsum = torch.zeros(len(ps), dtype=torch.float32, device=dev)
         self._total = torch.zeros(1, dtype=torch.float32, device=dev)
         self._ctl = torch.zeros(2, dtype=torch.float32, device=dev)
@@ -244,12 +257,13 @@ class FlatOptimizer(torch.optim.Optimizer):
                 raise RuntimeError("parameter gradient left the flat bucket")
         h = self._hyper_struct()
         clip = bool(max_norm) or bool(check_overflow)
-        if clip or self._needs_segsum:
+        if (clip or self._needs_segsum) and self._ntiles:
             ops.opt_seg_sumsq(self.flat_grads, self._seg, self._tiles, self._partial, self._segsum,
                               self._total if clip else None)
         ops.opt_prologue(self._total if clip else None, grad_scale, max_norm if max_norm else 0.0, self._steps,
                          self._ctl)
-        self._update(h)
+        if self._ntiles:
+            self._update(h)
         return loss
 
     def _update(self, h):
@@ -265,7 +279,8 @@ class FlatOptimizer(torch.optim.Optimizer):
 
     def grad_norm(self):
         """The gradient norm, summed in the same fixed order as the clip."""
-        ops.opt_seg_sumsq(self.flat_grads, self._seg, self._tiles, self._partial, self._segsum, self._total)
+        if self._ntiles:
+            ops.opt_seg_sumsq(self.flat_grads, self._seg, self._tiles, self._partial, self._segsum, self._total)
         return self._total.sqrt()
 
     # -- checkpoints ----------------------------------------------------------------------------------------------

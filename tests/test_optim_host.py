@@ -1,6 +1,7 @@
 """CPU-side checks of the flat-bucket optimizers (edgedict_b200.optim.SGD / SM3 / AdamW / Novograd): the fp64 oracle
 against the reference's recorded steps (tests/golden/optim_tiny.npz), constructor validation with the reference's
-messages, the refused options, and the C entries' argument checks.  No GPU needed."""
+messages, the refused options, the C entries' argument checks, the bucket's segment and tile tables, and the one-step
+fp64 restatement of tests/optim_restate.py pinned against the oracle.  No GPU needed."""
 import os
 
 import numpy as np
@@ -121,3 +122,138 @@ def test_entry_points_reject_bad_arguments_before_touching_the_device(built):
     assert L.eb_opt_adamw_step(p, p, p, p, p, None, 1, h, 1, p, p, None) == 2
     assert L.eb_opt_novograd_step(p, p, p, p, None, p, 1, p, 1, h, 1, p, None) == 2
     assert L.eb_opt_novograd_step(p, p, p, p, p, p, -1, p, 1, h, 1, p, None) == 2
+
+
+# ---- the bucket tables (optim.bucket_tables) and the fp64 one-step restatement (tests/optim_restate.py) ---------------
+from tests import optim_restate as rs          # noqa: E402
+
+TABLE_SHAPES = ([(2, c) for c in (1, 3, 4, 5, 767, 768, 769, 1024, 4095, 4096, 4097, 8192, 8193)] +
+                [(r, 1) for r in (1023, 1024, 1025, 2049)] + [(1025, 16), (964, 17), (1024, 16), (963, 17)] +
+                [(), (1,), (5,), (6,), (7,), (8193,), (140000,), (33 * 1024 + 100, 1), (3, 1, 5), (1, 4, 6),
+                 (2, 3, 1, 5), (3, 2, 4, 7), (1, 1, 1, 1), (0,), (0, 5), (3, 0, 2), (2, 1, 0, 3), (3, 3), (5, 7, 9)])
+
+
+def test_tile_table_covers_every_element_once_within_the_sm3_caps():
+    from edgedict_b200.optim import TILE_COLS, TILE_ELEMS, TILE_ROWS, bucket_tables
+    seg, tiles, offs, n, nacc = bucket_tables([TABLE_SHAPES[0::2], TABLE_SHAPES[1::2]])
+    shapes = TABLE_SHAPES[0::2] + TABLE_SHAPES[1::2]
+    assert n == sum((int(np.prod(s)) + 3) // 4 * 4 for s in shapes)
+    for i, (row, s) in enumerate(zip(seg, shapes)):
+        k = int(np.prod(s))
+        C = s[-1] if s else 1
+        assert row[0] == offs[i] and offs[i] % 4 == 0
+        mine = tiles[row[4]:row[5]]
+        assert all(t[0] == i for t in mine)
+        covered = 0
+        for t in mine:
+            _, start, ln, r0, c0, ncols = t
+            assert ncols > 0 and ln > 0 and ln % ncols == 0            # sm3_kernel: nrows = len / ncols
+            assert ncols <= TILE_COLS and ln // ncols <= TILE_ROWS and ln <= TILE_ELEMS
+            assert start == covered                                    # in order, no gap, no overlap
+            assert start == r0 * C + c0 and 0 <= c0 and c0 + ncols <= C
+            assert c0 == 0 and ncols == C if C <= TILE_COLS else ln == ncols
+            covered += ln
+        assert covered == k, (s, covered)
+    assert tiles == [t for row in seg for t in tiles[row[4]:row[5]]] and seg[-1][5] == len(tiles)
+    assert bucket_tables([[(0,), (0, 3)], [(2, 0, 1)]])[1] == []              # an all-empty bucket has no tile
+
+
+def _header_fields(name):
+    src = open(os.path.join(HERE, "..", "include", "edgedict_b200.h")).read()
+    import re
+    body = re.search(r"typedef struct \{ long long ([^;]*); \} %s;" % name, src).group(1)
+    out = []
+    for f in body.split(","):
+        f = f.strip()
+        m = re.fullmatch(r"(\w+)\[(\d+)\]", f)
+        out += ["%s%d" % (m.group(1), d) for d in range(int(m.group(2)))] if m else [f]
+    return out
+
+
+def test_table_rows_follow_the_c_structs_field_order():
+    from edgedict_b200.optim import bucket_tables
+    assert _header_fields("eb_opt_seg") == ["off", "numel", "rank", "group", "tile_begin", "tile_end", "shape0",
+                                            "shape1", "shape2", "shape3", "acc0", "acc1", "acc2", "acc3"]
+    assert _header_fields("eb_opt_tile") == ["seg", "start", "len", "r0", "c0", "ncols"]
+    seg, tiles, _, _, nacc = bucket_tables([[(5,), (3, 4, 2)], [(), (2, 5000)]])
+    f = _header_fields("eb_opt_seg")
+    rows = [dict(zip(f, r)) for r in seg]
+    assert rows[1] == dict(off=8, numel=24, rank=3, group=0, tile_begin=1, tile_end=2, shape0=3, shape1=4, shape2=2,
+                           shape3=0, acc0=5, acc1=8, acc2=12, acc3=0)
+    assert rows[2]["acc0"] == 14 and rows[2]["numel"] == 1 and rows[2]["group"] == 1
+    assert rows[3]["acc0"] == 15 and rows[3]["acc1"] == 17 and nacc == 5017
+    assert [dict(zip(_header_fields("eb_opt_tile"), t)) for t in tiles[3:]] == [
+        dict(seg=3, start=s, len=k, r0=r, c0=c, ncols=k) for r in (0, 1) for c, k in ((0, 4096), (4096, 904))
+        for s in [r * 5000 + c]]
+
+
+def test_sumsq_terms_reads_the_loop_bounds():
+    assert rs.sumsq_terms(1) == (1, False)
+    assert rs.sumsq_terms(768) == (3, False)
+    assert rs.sumsq_terms(769) == (3, True)                    # thread 0 takes one body trip, thread 1 three tail
+    assert rs.sumsq_terms(1024) == (1, True)
+    assert rs.sumsq_terms(1025) == (2, True)                   # thread 0: one trip, then element 1024
+    assert rs.sumsq_terms(16384) == (16, True)
+    assert rs.sumsq_terms(4096 + 768) == (7, True)             # 4 trips, then 3 tail elements of thread 0 (j < 4864)
+
+
+@pytest.mark.parametrize("case", sorted(oo.HYPER))
+def test_restatement_chained_matches_the_oracle_and_the_fixture(z, case):
+    """Six one-step restatements chained on their own fp64 outputs reproduce tests/optim_oracle.run (to fp64 rounding)
+    and the reference's recorded steps."""
+    from edgedict_b200.optim import bucket_tables
+    init, grads, groups, hyp, two = oo.fixture(z, case)
+    kind = oo.KIND[case]
+    ng = 2 if two else 1
+    order = [[i for i in range(len(init)) if groups[i] == gi] for gi in range(ng)]
+    flat = [i for o in order for i in o]
+    seg, tiles, offs, n, nacc = bucket_tables([[np.shape(init[i]) for i in o] for o in order])
+    L = rs.Layout(seg, tiles, n, "cpu")
+
+    def bucket(arrs):
+        b = torch.full((n,), float("nan"), dtype=torch.float64)
+        for k, i in enumerate(flat):
+            b[offs[k]:offs[k] + np.size(init[i])] = torch.as_tensor(np.asarray(arrs[i], dtype=np.float64)).reshape(-1)
+        return b
+
+    def scatter(vals):
+        b = torch.full((n,), float("nan"), dtype=torch.float64)
+        b[L.pos] = vals
+        return b
+
+    want = oo.run(kind, init, list(zip(grads, hyp)), groups)
+    p = bucket(init)
+    st = {k: torch.zeros(n, dtype=torch.float64) for k in ("buf", "m", "v")}
+    segv = torch.zeros(len(seg), dtype=torch.float64)
+    acc = torch.zeros(nacc, dtype=torch.float64)
+    for step in range(1, oo.NSTEPS + 1):
+        h = {k: [hg[kk] for hg in hyp[step - 1]] for k, kk in (("lr", "lr"), ("wd", "wd"), ("b1", "b1"), ("b2", "b2"),
+                                                             ("eps", "eps"))}
+        g = bucket(grads[step - 1])
+        steps = [step] * ng
+        if kind == "sgd":
+            out, _ = rs.sgd(L, p, g, st["buf"], h, steps, 1.0)
+            st["buf"] = scatter(out["buf"][0])
+        elif kind == "adamw":
+            out = rs.adamw(L, p, g, st["m"], st["v"], h, steps, 1.0)
+            st["m"], st["v"] = scatter(out["m"][0]), scatter(out["v"][0])
+        elif kind == "novograd":
+            _, _, ssum, _ = rs.seg_sumsq(L, g)
+            segv, _ = rs.novograd_v(seg, ssum, segv, h, 1.0)
+            out = rs.novograd(L, p, g, st["m"], segv, h, 1.0)
+            st["m"] = scatter(out["m"][0])
+        else:
+            out, _ = rs.sm3(L, p, g, acc, nacc, h, 1.0)
+            acc = out["acc"][0]
+        p = scatter(out["p"][0])
+        wp, ws = want[step - 1]
+        for k, i in enumerate(flat):
+            mine = p[offs[k]:offs[k] + np.size(init[i])].numpy().reshape(np.shape(init[i]))
+            np.testing.assert_allclose(mine, wp[i], rtol=1e-12, atol=1e-15)
+            assert rel_err(mine, z["%s.p.%d.%d" % (case, step, i)]) < 1e-5, (case, step, i)
+            if kind == "novograd":
+                assert abs(float(segv[k]) - float(ws[i]["exp_avg_sq"])) <= 1e-12 * abs(float(ws[i]["exp_avg_sq"]))
+            if kind == "sm3" and np.ndim(init[i]) >= 2:
+                for d, nd in enumerate(np.shape(init[i])):
+                    a0 = seg[k][10 + d]
+                    np.testing.assert_array_equal(acc[a0:a0 + nd].numpy(), ws[i]["accumulator_%d" % d].reshape(-1))
