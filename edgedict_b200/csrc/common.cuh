@@ -113,6 +113,13 @@ __device__ __forceinline__ void spin_wait_ge(const unsigned* ctr, unsigned targe
     }
 }
 
+// eb_colsum's order for bf16 rows (elementwise.cu): row lane k of COLSUM_LANES adds rows k, k + COLSUM_LANES, ... in
+// order from 0.f, then a fixed tree (at stride st = COLSUM_LANES / 2, ..., 1, lane k < st adds lane k + st) adds the lane
+// sums, and out[c] += the total.  colsum_lanes_finish runs that tree over lane sums part[k * N + c] that a producer
+// summed in that order itself (the loss gradient, loss.cu): the same bits as eb_colsum over the same rows.
+constexpr int COLSUM_LANES = 512;
+int colsum_lanes_finish(const float* part, float* out, int N, cudaStream_t st);
+
 // exp through ex2.approx.ftz: FMUL + MUFU.  (__expf without -ftz=true is ex2.approx WITHOUT flush-to-zero, which
 // the compiler guards with a range test and two conditional multiplies per call: 3 extra instructions per element
 // in the streaming softmax loops.)  Results below 1.2e-38 flush to zero, irrelevant for softmax sums.

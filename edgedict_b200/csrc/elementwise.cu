@@ -489,7 +489,7 @@ __global__ void __launch_bounds__(1024) colsum_kernel(const TI* __restrict__ x, 
 // needs only 8.7 KB of shared memory: it fits beside a CTA of the joint's d-hidden GEMM (198 KB), under which this sum
 // runs.  The first tree levels add lane sums across the cluster through distributed shared memory, the rest run in the
 // CTA of rank 0.  Same additions in the same order as one CTA of 512 lanes: the same bits.
-constexpr int COLSUM_LANES = 512, COLSUM_CL = 4, COLSUM_CTA_LANES = COLSUM_LANES / COLSUM_CL;   // (the tree below assumes 4)
+constexpr int COLSUM_CL = 4, COLSUM_CTA_LANES = COLSUM_LANES / COLSUM_CL;   // (the tree below assumes 4)
 __global__ void __cluster_dims__(1, COLSUM_CL, 1) __launch_bounds__(2 * COLSUM_CTA_LANES)
 colsum_bf16_vec_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ out, long rows, int N) {
     __shared__ float sh[COLSUM_CTA_LANES][17];
@@ -551,6 +551,22 @@ colsum_bf16_vec_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ 
         __syncthreads();
     }
     if (threadIdx.x < 16 && blockIdx.x * 16 + (int)threadIdx.x < N) out[blockIdx.x * 16 + threadIdx.x] += sh[0][threadIdx.x];
+}
+
+// colsum_tree<COLSUM_LANES, 16> over lane sums in global memory (common.cuh): one CTA per 16 columns
+__global__ void __launch_bounds__(COLSUM_LANES) colsum_lanes_finish_kernel(const float* __restrict__ part,
+                                                                           float* __restrict__ out, int N) {
+    __shared__ float sh[COLSUM_LANES][17];
+    const int c0 = blockIdx.x * 16;
+    for (int e = threadIdx.x; e < COLSUM_LANES * 16; e += blockDim.x)
+        sh[e >> 4][e & 15] = c0 + (e & 15) < N ? part[(long)(e >> 4) * N + c0 + (e & 15)] : 0.f;
+    __syncthreads();
+#pragma unroll 1
+    for (int st = COLSUM_LANES / 2; st > 0; st >>= 1) {
+        for (int e = threadIdx.x; e < st * 16; e += blockDim.x) sh[e >> 4][e & 15] += sh[(e >> 4) + st][e & 15];
+        __syncthreads();
+    }
+    if (threadIdx.x < 16 && c0 + (int)threadIdx.x < N) out[c0 + threadIdx.x] += sh[0][threadIdx.x];
 }
 
 __global__ void cast_bf16_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, long n) {
@@ -830,6 +846,12 @@ EB_API int eb_colsum(const void* x, int x_bf16, float* out, long rows, int N, vo
         colsum_kernel<__nv_bfloat16><<<(N + 31) / 32, 1024, 0, ST(stream)>>>((const __nv_bfloat16*)x, out, rows, N);
     else
         colsum_kernel<float><<<(N + 31) / 32, 1024, 0, ST(stream)>>>((const float*)x, out, rows, N);
+    EB_CHECK_LAUNCH();
+    return EB_OK;
+}
+
+int colsum_lanes_finish(const float* part, float* out, int N, cudaStream_t st) {
+    colsum_lanes_finish_kernel<<<(N + 15) / 16, COLSUM_LANES, 0, st>>>(part, out, N);
     EB_CHECK_LAUNCH();
     return EB_OK;
 }

@@ -747,8 +747,9 @@ def _joint_bwd(ctx_p, dlog2, hid, he2, hd2, w1, w2, dims, db2=None):
 
     side = None
     if JOINT_WGRAD_SIDE and p == "bf16" and dlog2.is_cuda:
-        # the output layer's weight / bias gradients (a 4.2 GB column sum + the split-K dW2 GEMM, 2.5 ms at E6D2) are off
-        # the critical path to the encoder: they run on a side stream under the d-hidden GEMM and the two d-pre reductions
+        # the output layer's weight gradient (the split-K dW2 GEMM, and the 4.2 GB column sum for db2 unless the loss
+        # gradient already produced it) is off the critical path to the encoder: it runs on a side stream under the
+        # d-hidden GEMM and the d-pre reductions
         main = torch.cuda.current_stream(dlog2.device)
         side = _side_streams(dlog2.device)[1]
         side.wait_stream(main)
@@ -953,15 +954,18 @@ class JointLoss(torch.autograd.Function):
         B, T, U, E, Dd, J, V = ctx.dims
         p = ctx.precision
         g = _c(go.to(f32)).view(-1)
-        # (a variant of the gradient kernel that also accumulated the bias gradient in registers was
-        #  measured 2.5x slower -- occupancy -- than this kernel plus a separate column-sum pass)
-        if logits.dtype == bf16:
+        db2 = None
+        if logits.dtype == bf16 and V % 8 == 0:
+            # the bias gradient comes out of the gradient kernel, which holds every d logit it writes: the output layer's
+            # side stream is left with dW2 alone
+            dl, db2 = ops.rnnt_loss_bwd_bf16_db(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B)
+        elif logits.dtype == bf16:
             dl = ops.rnnt_loss_bwd_bf16(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B)
         elif p == "bf16":
             dl = ops.rnnt_loss_bwd(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B, out_bf16=True)
         else:
             dl = ops.rnnt_loss_bwd(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B, out=logits)
-        dhe, dhd, dw1, db1, dw2, db2 = _joint_bwd(p, dl.view(B * T * U, V), hid, he2, hd2, w1, w2, ctx.dims)
+        dhe, dhd, dw1, db1, dw2, db2 = _joint_bwd(p, dl.view(B * T * U, V), hid, he2, hd2, w1, w2, ctx.dims, db2)
         return dhe, dhd, dw1, db1, dw2, db2, None, None, None, None, None
 
 

@@ -29,6 +29,7 @@ def _need(t, dtype=None, name="tensor"):
 
 
 f32, bf16 = torch.float32, torch.bfloat16
+COLSUM_LANES = 512           # row lanes of eb_colsum's order for bf16 rows (csrc/common.cuh)
 
 
 # ---- optional per-kernel instrumentation (bench.py) ----------------------------------------------
@@ -674,6 +675,20 @@ def rnnt_loss_bwd_bf16(logits16, labels, xlen, ylen, blank, ws, gscale, host_sca
         check(lib().eb_rnnt_loss_bwd_bf16(_p(logits16), _p(logits16), _p(labels), _p(xlen), _p(ylen), B, T, U, V, blank,
                                           _p(ws), _p(gscale), per_batch, float(host_scale), _s()), "eb_rnnt_loss_bwd_bf16")
     return logits16
+
+
+def rnnt_loss_bwd_bf16_db(logits16, labels, xlen, ylen, blank, ws, gscale, host_scale):
+    """In place: logits16 becomes d loss / d logits (bf16), as rnnt_loss_bwd_bf16 writes them; also returns their column
+    sum db [V] fp32, the same bits as colsum(logits16.view(-1, V)) afterwards.  V % 8 == 0."""
+    B, T, U, V = logits16.shape
+    per_batch = int(gscale is not None and gscale.numel() > 1)
+    part = torch.empty(COLSUM_LANES * V, dtype=f32, device=logits16.device)
+    db = torch.zeros(V, dtype=f32, device=logits16.device)
+    with _timed("rnnt_loss_bwd", 2, 4.0 * B * T * U * V, 0.0):
+        check(lib().eb_rnnt_loss_bwd_bf16_db(_p(logits16), _p(logits16), _p(labels), _p(xlen), _p(ylen), B, T, U, V,
+                                             blank, _p(ws), _p(gscale), per_batch, float(host_scale), _p(part), _p(db),
+                                             _s()), "eb_rnnt_loss_bwd_bf16_db")
+    return logits16, db
 
 
 # ---- language-model cross-entropy (csrc/lm.cu, csrc/gemm_tc.cu) ---------------------------------------

@@ -43,6 +43,12 @@ int eb_rnnt_loss_lattice(const int* xlen, const int* ylen, int B, int maxT, int 
 int eb_rnnt_loss_bwd_bf16(const void* logits16, void* grads16, const int* labels, const int* xlen, const int* ylen,
                           int B, int maxT, int maxU, int V, int blank, void* workspace, const float* gscale_dev,
                           int gscale_per_batch, double host_scale, void* stream);
+/* The same d logits as eb_rnnt_loss_bwd_bf16 (V % 8 == 0; logits16, grads16, db_part 16-byte aligned, else
+ * EB_ERR_INVALID), and db_accum[c] += the column sum of the bf16 d logits over all B*maxT*maxU rows, the same bits as
+ * eb_colsum on them.  db_part: fp32 scratch of 512 * V. */
+int eb_rnnt_loss_bwd_bf16_db(const void* logits16, void* grads16, const int* labels, const int* xlen, const int* ylen,
+                             int B, int maxT, int maxU, int V, int blank, void* workspace, const float* gscale_dev,
+                             int gscale_per_batch, double host_scale, float* db_part, float* db_accum, void* stream);
 int eb_rnnt_workspace_views(void* workspace, int B, int maxT, int maxU, int dtype_size,
                             void** denom, void** alphas, void** betas, void** ll_fwd, void** ll_bwd);
 /* Forced (Viterbi) alignment over a workspace that eb_rnnt_loss_fwd (any need_beta) or eb_joint_logits_lse filled;
