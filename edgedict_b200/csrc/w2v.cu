@@ -17,8 +17,10 @@
 //   eb_w2v_quant_stats   : one CTA: the perplexities from sum_r p and the counts of k0, and the coefficients
 //                          d prob_ppl / d avg_probs.
 //   eb_w2v_quant_bwd     : d logits = (1/tau) J_s d_soft + (g_ppl / N) J_p coef, J the softmax Jacobians.
-//   eb_w2v_logits_fwd    : cosine logits [K+1, B, M] / logit_temp, -inf where a negative equals the positive.
-//   eb_w2v_logits_bwd    : the dense per-utterance weights A, AC [B, M, M], then dxp and dyp.
+//   eb_w2v_logits_fwd    : cosine logits [K+1, B, M] / logit_temp, -inf where a negative equals the positive (there
+//                          the saved cosine is -inf too: it carries the mask to the backward).
+//   eb_w2v_logits_bwd    : the dense per-utterance weights A, AC [B, M, M], then dxp and dyp; a masked candidate (-inf
+//                          cosine) contributes nothing, as the reference's index_put of -inf passes no gradient.
 //   eb_w2v_ce            : one CTA: InfoNCE cross-entropy (target 0) over the rows (m, b), its unscaled gradient,
 //                          the summed loss and the count of correct rows.
 #include "common.cuh"
@@ -248,13 +250,14 @@ __global__ void logits_fwd_kernel(const float* __restrict__ xh, const float* __r
         }
         acc = warp_sum(acc);
         same = __all_sync(0xffffffffu, same);
-        cosv[c * BM + w] = acc;
-        logits[c * BM + w] = (c > 0 && same) ? -INFINITY : acc / temp;
+        const bool masked = c > 0 && same;
+        cosv[c * BM + w] = masked ? -INFINITY : acc;
+        logits[c * BM + w] = masked ? -INFINITY : acc / temp;
     }
 }
 
-// one thread per (b, r): A[b, r, j] = sum of dlogit over the candidates of row r that are row j (k order, the
-// positive first); AC the same sum of dlogit * cos
+// one thread per (b, r): A[b, r, j] = sum of dlogit over the unmasked candidates of row r that are row j (k order,
+// the positive first); AC the same sum of dlogit * cos
 __global__ void logits_bwd_a_kernel(const float* __restrict__ dlog, const float* __restrict__ cosv,
                                     const int* __restrict__ neg, int B, int M, int K, float* __restrict__ A,
                                     float* __restrict__ AC) {
@@ -266,6 +269,7 @@ __global__ void logits_bwd_a_kernel(const float* __restrict__ dlog, const float*
     for (int j = 0; j < M; ++j) a[j] = ac[j] = 0.f;
     const int m = (int)(w % M);
     for (int c = 0; c <= K; ++c) {
+        if (c > 0 && cosv[c * BM + w] == -INFINITY) continue;       // masked: no gradient
         const int j = c == 0 ? m : neg[w * K + c - 1];
         const float g = dlog[c * BM + w];
         a[j] += g;

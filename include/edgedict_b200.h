@@ -525,8 +525,10 @@ int eb_gemm_f32_splitk(const float* A, long sam, long sak, const float* B, long 
  *                      dsoft or g_ppl may be NULL (that term is dropped).
  * eb_w2v_logits_fwd  : xp, yp [B, M, D], neg int32 [B, M, K] (frames of the same utterance) -> xh, yh (rows over
  *                      max(|row|, eps)), xn, yn [B*M] (|row|), cosv and logits [K+1, B, M]: candidate 0 is row m of yp,
- *                      candidate 1 + k row neg[b, m, k]; logits = cos / temp, -inf where a negative equals yp[b, m].
- * eb_w2v_logits_bwd  : dlogits [K+1, B, M] -> dxp, dyp; A, AC [B, M, M] scratch.
+ *                      candidate 1 + k row neg[b, m, k]; logits = cos / temp, -inf where a negative equals yp[b, m]
+ *                      (cosv is -inf there too: it marks the masked candidates for the backward).
+ * eb_w2v_logits_bwd  : dlogits, cosv (the forward's) [K+1, B, M] -> dxp, dyp; A, AC [B, M, M] scratch.  A masked
+ *                      candidate (c > 0 with a -inf cosv) passes no gradient, whatever its dlogit.
  * eb_w2v_ce          : logits [C, B, M], rows (m, b) -> grad (softmax - onehot(0)), out[0] = sum of lse - logit 0,
  *                      out[1] = rows whose argmax is 0 and argmin is not (first index on ties). */
 int eb_w2v_mask_fwd(const float* x, const float* mask_emb, const int* inv, float* out, long rows, int D, void* stream);

@@ -234,3 +234,89 @@ def test_c_entries_check_their_arguments():
     assert L.eb_w2v_logits_fwd(p, p, p, 2, 3, 4, 3, 0.0, 1e-8, p, p, p, p, p, p, None) == 2   # temp 0
     assert L.eb_w2v_logits_bwd(p, p, p, p, p, p, p, p, p, 2, 3, 4, 0, 0.1, 1e-8, p, p, p, p, None) == 2
     assert L.eb_w2v_ce(p, 2, 3, 1, p, p, None) == 2
+
+
+# ---- tests/w2v_restate.py, the per-kernel restatement of test_gpu_w2v_fp64.py, pinned to the oracle ---------------
+def test_restate_lane_argmax_is_the_first_index_argmax():
+    """Without NaN the kernels' lane map is torch's first-index argmax / argmin, ties across and within lanes included;
+    a NaN a lane meets first sticks in that lane, a later one is skipped."""
+    from tests import w2v_restate as rs
+    g = torch.Generator().manual_seed(1)
+    for n in (1, 2, 31, 32, 33, 70, 1100):
+        v = torch.randint(-3, 4, (200, n), generator=g).float()        # many ties
+        assert torch.equal(rs.lane_arg(v.numpy()), v.argmax(-1)), n
+        assert torch.equal(rs.lane_arg(v.numpy(), largest=False), v.argmin(-1)), n
+    v = torch.arange(70.0).repeat(3, 1)
+    v[0, 0] = v[1, 37] = v[2, 69] = float("nan")
+    assert rs.lane_arg(v.numpy()).tolist() == [0, 69, 68]
+
+
+def test_restate_quantizer_is_the_oracle():
+    """k, the perplexities (from psum = sum_r p) and d logits = quant_bwd(dsoft = dq vars^T, g_ppl) of the restatement
+    equal wav2vec_oracle.quantize and its fp64 autograd."""
+    from tests import w2v_restate as rs
+    g = torch.Generator().manual_seed(2)
+    N, G, V, vd, tau = 37, 3, 20, 5, 1.7
+    tau = float(np.float32(tau))
+    logits = (3 * torch.randn(N, G * V, generator=g)).double().requires_grad_()
+    noise = -torch.empty(N, G * V).exponential_(generator=g).log().double()
+    vars = torch.rand(G * V, vd, generator=g).double()
+    q, pp, cp, k, _ = wo.quantize(logits, vars, noise, G, tau)
+    R = torch.randn(N, G * vd, generator=g).double()
+    ((q * R).sum() + 3.0 * pp).backward()
+    pp, cp = pp.detach(), cp.detach()
+    z = ((logits.detach() + noise) / tau).view(N * G, V)
+    s, _ = rs.softmax(z, V)
+    p, _ = rs.softmax(logits.detach().view(N * G, V), V)
+    assert torch.equal(s.argmax(-1).view(N, G), k)
+    k0 = logits.detach().view(N, G, V).argmax(-1)
+    st = rs.quant_stats(p.view(N, G * V).sum(0), k0, N, G, V)
+    assert abs(float(st["pp"]) - float(pp)) < 1e-12 * float(pp) and abs(float(st["cp"]) - float(cp)) < 1e-12 * float(cp)
+    ds = torch.einsum("ngd,gvd->ngv", R.view(N, G, vd), vars.view(G, V, vd)).reshape(N, G * V)
+    dl, _ = rs.quant_bwd(ds, s.view(N, -1), p.view(N, -1), st["coef"], torch.tensor([3.0], dtype=torch.float64), N, G,
+                         V, tau)
+    assert float((dl - logits.grad).abs().max()) < 1e-12 * float(logits.grad.abs().max())
+
+
+def test_restate_cosine_logits_and_gradients_are_the_oracle():
+    """normalize + logits_fwd equal contrastive_logits (the -inf included), and logits_a + logits_bwd under a dense
+    upstream gradient, nonzero at the masked candidates, equal its fp64 autograd: a masked candidate passes nothing."""
+    from tests import w2v_restate as rs
+    g = torch.Generator().manual_seed(3)
+    B, M, D, K, temp, eps = 2, 12, 9, 6, float(np.float32(0.1)), float(np.float32(1e-8))
+    xp, yp = torch.randn(B, M, D, generator=g), torch.randn(B, M, D, generator=g)
+    yp[0, 5] = yp[0, 3]
+    xp[1, 2] *= 1e-12
+    yp[1, 4] = 0.0
+    neg = torch.randint(0, M, (B, M, K), generator=g)
+    neg[0, 3, 0], neg[0, 5, 1], neg[1, 6, 2] = 5, 3, 6
+    X, Y = xp.double().requires_grad_(), yp.double().requires_grad_()
+    want = wo.contrastive_logits(X, Y, neg, temp, eps)          # the kernel's float eps
+    xh, _, xn, _ = rs.normalize(xp, eps)
+    yh, _, yn, _ = rs.normalize(yp, eps)
+    cos, _, lo, _ = rs.logits_fwd(xh, yh, yp, neg, temp)
+    assert torch.equal(lo.isinf(), want.isinf()) and int(lo.isinf().sum()) >= 3
+    fin = torch.isfinite(want)
+    assert float((lo[fin] - want.detach()[fin]).abs().max()) < 1e-12 / temp
+    R = torch.randn(want.shape, generator=g).double() + 3.0
+    (torch.where(fin, want, torch.zeros_like(want)) * R).sum().backward()
+    A, _, AC, _ = rs.logits_a(R, cos, neg, lo.isinf())
+    dx, _, dy, _ = rs.logits_bwd(A, AC, xh, yh, xp, yp, xn, yn, temp, eps)
+    for got, ref in ((dx, X.grad), (dy, Y.grad)):
+        assert float((got - ref).abs().max()) < 1e-10 * float(ref.abs().max())
+
+
+def test_restate_cross_entropy_is_the_oracle():
+    from tests import w2v_restate as rs
+    g = torch.Generator().manual_seed(4)
+    C, B, M = 33, 3, 7
+    lo = 5 * torch.randn(C, B, M, generator=g)
+    lo[1:4, 1, 2] = -float("inf")
+    lo[:, 2, 5] = 0.25
+    lo[0, 0, 3] = lo[7, 0, 3] = 40.0
+    X = lo.double().requires_grad_()
+    loss, correct = wo.cross_entropy(X)
+    loss.backward()
+    r = rs.ce(lo)
+    assert abs(r["loss"] - float(loss)) < 1e-12 * float(loss) and r["correct"] == correct
+    assert float((r["grad"] - X.grad).abs().max()) < 1e-12
