@@ -109,6 +109,10 @@ SIGNATURES = {
     "eb_fe_power": (I, [P, P, L, I, P]),
     "eb_fe_log_stack": (I, [P, P, I, I, I, I, I, I, I, I, P]),
     "eb_fe_mask": (I, [P, P, I, I, I, I, I, F, P]),
+    "eb_fe_preemph_pad_lens": (I, [P, P, P, P, I, I, L, I, F, I, P]),
+    "eb_fe_log": (I, [P, L, F, P]),
+    "eb_fe_finish": (I, [P, P, P, P, I, I, I, I, I, I, I, I, I, I, P]),
+    "eb_fe_deltas": (I, [P, P, I, I, I, P]),
     "eb_conv_rows_per_split": (I, [I]),
     "eb_conv1d_first_fwd": (I, [P, P, P, P, I, I, I, I, I, I, P]),
     "eb_conv1d_first_dw": (I, [P, P, P, I, L, I, I, I, I, I, I, P]),

@@ -14,21 +14,30 @@
 //   G2 eb_gemm_f32      : mel[g,m] = P[g,:] @ fb[m,:]^T;
 //   K3 fe_log_stack     : out[b,t,s*n_mels+m] = log(mel[g(b, t*n_frame+s), m] + 1e-20), zero for masked / padded
 //                         frames -- directly in the [B, T, n_mels*n_frame] layout Encoder.forward consumes.
+//
+// Per-utterance lengths (a padded batch, as rnnt/dataset.py:202-240 collates the reference's per-utterance features):
+// K1 and K3 take a device int32 lens[B] (nullptr: every utterance is L long).  Utterance b then reflects at its own
+// L_b, has F_b = 1 + L_b/hop frames and T_b = ceil(F_b/n) (or floor) output rows, and rows t >= T_b are zero.  K3 also
+// computes CatDeltas (rnnt/transforms.py:10-16: torchaudio compute_deltas twice, window 5, replicate edge at F_b - 1)
+// and writes [static | d1 | d2] per stacked frame, the channel order Downsample's reshape gives.  The MFCC path adds
+// fe_log (log(mel + 1e-6)) and one more eb_gemm_f32 against the orthonormal DCT-II matrix before K3.
 #include "common.cuh"
 #include "../../include/edgedict_b200.h"
 
 namespace {
 
-__global__ void fe_preemph_pad_kernel(const float* __restrict__ x, float* __restrict__ xp, int L, long Lp, int pad,
-                                      float preemph, int use_preemph) {
+// row b of x is L samples apart; its first lens[b] (or L) are the utterance
+__global__ void fe_preemph_pad_kernel(const float* __restrict__ x, const int* __restrict__ lens, float* __restrict__ xp,
+                                      int L, long Lp, int pad, float preemph, int use_preemph) {
     const int b = blockIdx.y;
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= Lp) return;
+    const int Lb = lens ? lens[b] : L;
     float v = 0.f;
-    if (i < (long)L + 2 * pad) {
+    if (i < (long)Lb + 2 * pad) {
         long r = i - pad;                               // reflect (no edge repeat): -1 -> 1, L -> L-2
         if (r < 0) r = -r;
-        if (r >= L) r = 2L * (L - 1) - r;
+        if (r >= Lb) r = 2L * (Lb - 1) - r;
         const float* row = x + (long)b * L;
         v = row[r];
         if (use_preemph && r > 0) v -= preemph * row[r - 1];
@@ -45,21 +54,68 @@ __global__ void fe_power_kernel(const float* __restrict__ spec, float* __restric
     pw[i] = re * re + im * im;
 }
 
-__global__ void fe_log_stack_kernel(const float* __restrict__ mel, float* __restrict__ out, int R, int F, int seq_len,
-                                    int n_mels, int n_frame, int Tout, int take_log) {
+// Static feature of frame f (< F), channel c: the optional log(x + 1e-20) of features.py:155-156, zero from frame `seq`
+// on (features.py:160-164; seq = F when there is no mask).
+__device__ __forceinline__ float fe_static(const float* __restrict__ rows, int f, int c, int C, int seq, int take_log) {
+    if (f >= seq) return 0.f;
+    const float v = rows[(long)f * C + c];
+    return take_log ? logf(v + 1e-20f) : v;
+}
+
+__device__ __forceinline__ int fe_clamp(int f, int F) { return f < 0 ? 0 : (f >= F ? F - 1 : f); }
+
+// torchaudio compute_deltas (window 5, replicate padding): d[f] = sum_{k=-2..2} k x[clamp(f+k, 0, F-1)] / 10
+__device__ float fe_delta1(const float* __restrict__ rows, int f, int c, int C, int seq, int F, int take_log) {
+    const float m2 = fe_static(rows, fe_clamp(f - 2, F), c, C, seq, take_log);
+    const float m1 = fe_static(rows, fe_clamp(f - 1, F), c, C, seq, take_log);
+    const float p1 = fe_static(rows, fe_clamp(f + 1, F), c, C, seq, take_log);
+    const float p2 = fe_static(rows, fe_clamp(f + 2, F), c, C, seq, take_log);
+    return (2.f * (p2 - m2) + (p1 - m1)) / 10.f;
+}
+
+__device__ float fe_delta2(const float* __restrict__ rows, int f, int c, int C, int seq, int F, int take_log) {
+    const float m2 = fe_delta1(rows, fe_clamp(f - 2, F), c, C, seq, F, take_log);
+    const float m1 = fe_delta1(rows, fe_clamp(f - 1, F), c, C, seq, F, take_log);
+    const float p1 = fe_delta1(rows, fe_clamp(f + 1, F), c, C, seq, F, take_log);
+    const float p2 = fe_delta1(rows, fe_clamp(f + 2, F), c, C, seq, F, take_log);
+    return (2.f * (p2 - m2) + (p1 - m1)) / 10.f;
+}
+
+// feat [B*R, C] per-frame rows -> out[b, t, s*Cd + j*C + c] (Cd = C * (delta ? 3 : 1); j = 0 static, 1 d1, 2 d2) for
+// frame f = t*n_frame + s < F_stack, zero elsewhere.  lens == nullptr: every utterance has F_stack = F = n_frames
+// frames and its mask at seq_len; else utterance b has F = 1 + lens[b]/hop, its mask at ceil(lens[b]/hop) (use_mask)
+// or none, and F_stack = F (pad_div) or F - F % n_frame.
+__global__ void fe_finish_kernel(const float* __restrict__ feat, float* __restrict__ out, const int* __restrict__ lens,
+                                 int R, int n_frames, int seq_len, int hop, int use_mask, int pad_div, int C,
+                                 int n_frame, int Tout, int take_log, int delta) {
     const int b = blockIdx.y;
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-    const int W = n_mels * n_frame;
+    const int Cd = delta ? 3 * C : C;
+    const int W = Cd * n_frame;
     if (i >= (long)Tout * W) return;
-    const int t = (int)(i / W), c = (int)(i % W);
-    const int s = c / n_mels, m = c % n_mels;
+    int F = n_frames, Fs = n_frames, seq = seq_len;
+    if (lens) {
+        const int Lb = lens[b];
+        F = 1 + Lb / hop;
+        seq = use_mask ? (Lb + hop - 1) / hop : F;
+        Fs = pad_div ? F : F - F % n_frame;
+    }
+    const int t = (int)(i / W), w = (int)(i % W);
+    const int s = w / Cd, j = (w % Cd) / C, c = w % C;
     const int f = t * n_frame + s;
+    const float* rows = feat + (long)b * R * C;
     float v = 0.f;
-    if (f < F && f < seq_len) {
-        v = mel[((long)b * R + f) * n_mels + m];
-        if (take_log) v = logf(v + 1e-20f);
+    if (f < Fs) {
+        if (j == 0) v = fe_static(rows, f, c, C, seq, take_log);
+        else if (j == 1) v = fe_delta1(rows, f, c, C, seq, F, take_log);
+        else v = fe_delta2(rows, f, c, C, seq, F, take_log);
     }
     out[(long)b * Tout * W + i] = v;
+}
+
+__global__ void fe_log_kernel(float* __restrict__ x, long n, float offset) {
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) x[i] = logf(x[i] + offset);
 }
 
 // SpecAugment masking (rnnt/transforms.py:53-147): x [B, D1, D2]; spans [B, nmask, 2] = [start, end) along dim `axis`
@@ -90,7 +146,8 @@ EB_API int eb_fe_preemph_pad(const float* x, float* xp, int B, int L, long Lp, i
                              int use_preemph, void* stream) {
     if (!x || !xp || B <= 0 || L <= 1 || pad < 0 || pad >= L || Lp < (long)L + 2 * pad) return EB_ERR_INVALID;
     dim3 grid((unsigned)((Lp + 255) / 256), B);
-    fe_preemph_pad_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x, xp, L, Lp, pad, preemph, use_preemph);
+    fe_preemph_pad_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x, nullptr, xp, L, Lp, pad, preemph,
+                                                                                    use_preemph);
     EB_CHECK_LAUNCH();
     return EB_OK;
 }
@@ -110,8 +167,64 @@ EB_API int eb_fe_log_stack(const float* mel, float* out, int B, int rows_per_utt
         return EB_ERR_INVALID;
     const long per = (long)t_out * n_mels * n_stack;
     dim3 grid((unsigned)((per + 255) / 256), B);
-    fe_log_stack_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(mel, out, rows_per_utt, n_frames, seq_len,
-                                                                                  n_mels, n_stack, t_out, take_log);
+    fe_finish_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(mel, out, nullptr, rows_per_utt, n_frames,
+                                                                               seq_len, 1, 0, 1, n_mels, n_stack, t_out,
+                                                                               take_log, 0);
+    EB_CHECK_LAUNCH();
+    return EB_OK;
+}
+
+// Host-side checks of the per-utterance lengths (lens, on the host; lens_dev holds the same values on the device).
+static bool fe_lens_ok(const int* lens, int B, int lo, int hi) {
+    for (int b = 0; b < B; ++b)
+        if (lens[b] <= lo || lens[b] > hi) return false;
+    return true;
+}
+
+EB_API int eb_fe_preemph_pad_lens(const float* x, const int* lens, const int* lens_dev, float* xp, int B, int L, long Lp,
+                                  int pad, float preemph, int use_preemph, void* stream) {
+    if (!x || !lens || !lens_dev || !xp || B <= 0 || L <= 1 || pad < 0 || Lp < (long)L + 2 * pad) return EB_ERR_INVALID;
+    if (!fe_lens_ok(lens, B, pad, L)) return EB_ERR_INVALID;       // torch's reflect pad needs pad < L_b
+    dim3 grid((unsigned)((Lp + 255) / 256), B);
+    fe_preemph_pad_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x, lens_dev, xp, L, Lp, pad, preemph,
+                                                                                    use_preemph);
+    EB_CHECK_LAUNCH();
+    return EB_OK;
+}
+
+EB_API int eb_fe_log(float* x, long n, float offset, void* stream) {
+    if (!x || n <= 0 || !(offset > 0.f)) return EB_ERR_INVALID;
+    fe_log_kernel<<<(unsigned)((n + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x, n, offset);
+    EB_CHECK_LAUNCH();
+    return EB_OK;
+}
+
+EB_API int eb_fe_finish(const float* feat, float* out, const int* lens, const int* lens_dev, int B, int rows_per_utt,
+                        int hop, int n_ch, int n_stack, int t_out, int take_log, int use_mask, int delta,
+                        int pad_to_divisible, void* stream) {
+    if (!feat || !out || !lens || !lens_dev || B <= 0 || rows_per_utt <= 0 || hop <= 0 || n_ch <= 0 || n_stack <= 0 ||
+        t_out <= 0)
+        return EB_ERR_INVALID;
+    for (int b = 0; b < B; ++b) {
+        if (lens[b] <= 0) return EB_ERR_INVALID;
+        const int F = 1 + lens[b] / hop;
+        const int T = pad_to_divisible ? (F + n_stack - 1) / n_stack : F / n_stack;
+        if (F > rows_per_utt || T > t_out) return EB_ERR_INVALID;
+    }
+    const int W = n_ch * (delta ? 3 : 1) * n_stack;
+    dim3 grid((unsigned)(((long)t_out * W + 255) / 256), B);
+    fe_finish_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(feat, out, lens_dev, rows_per_utt, 0, 0, hop,
+                                                                               use_mask, pad_to_divisible, n_ch, n_stack,
+                                                                               t_out, take_log, delta);
+    EB_CHECK_LAUNCH();
+    return EB_OK;
+}
+
+EB_API int eb_fe_deltas(const float* feat, float* out, int B, int n_frames, int n_ch, void* stream) {
+    if (!feat || !out || B <= 0 || n_frames <= 0 || n_ch <= 0) return EB_ERR_INVALID;
+    dim3 grid((unsigned)(((long)n_frames * 3 * n_ch + 255) / 256), B);
+    fe_finish_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(feat, out, nullptr, n_frames, n_frames,
+                                                                               n_frames, 1, 0, 1, n_ch, 1, n_frames, 0, 1);
     EB_CHECK_LAUNCH();
     return EB_OK;
 }

@@ -900,6 +900,68 @@ def logmel_frontend(x, basis, fbT, n_fft, hop, n_mels, n_stack, preemph, take_lo
     return out
 
 
+def fe_lengths(lens, hop, n_stack, pad_to_divisible=True):
+    """Host geometry of utterances of lens samples: (frames F_b = 1 + L_b // hop, output rows T_b after stacking)."""
+    F = [1 + int(n) // hop for n in lens]
+    T = [-(-f // n_stack) if pad_to_divisible else f // n_stack for f in F]
+    return F, T
+
+
+def fe_batch(x, lens, basis, fbT, n_fft, hop, n_stack, preemph=None, dct=None, take_log=False, use_mask=False,
+             delta=False, pad_to_divisible=True):
+    """Per-utterance features of a padded batch (see csrc/frontend.cu).  x [B, L] fp32 waveforms whose row b holds
+    lens[b] samples (lens: host int [B], n_fft//2 < lens[b] <= L); basis [n_fft, 2*nbins] = window * (cos | -sin);
+    fbT [nbins, n_mels]; dct [n_mels, n_mfcc] for MFCC (log(mel + 1e-6), then the DCT).  Returns (out [B, T_max,
+    C*(3 if delta)*n_stack], T int32 CPU [B]); rows t >= T[b] of utterance b are zero."""
+    _need(x, f32, "x")
+    for t, name in ((basis, "basis"), (fbT, "fbT"), (dct, "dct")):
+        if t is not None:
+            _need(t, f32, name)
+    B, L = x.shape
+    lens = torch.as_tensor(lens).to("cpu", torch.int32).contiguous()
+    if tuple(lens.shape) != (B,):
+        raise ValueError("lengths must have shape [%d], got %s" % (B, tuple(lens.shape)))
+    pad = n_fft // 2
+    if int(lens.min()) <= pad or int(lens.max()) > L:
+        raise ValueError("every length must be in (n_fft // 2, L] = (%d, %d], got %s" % (pad, L, lens.tolist()))
+    nb = n_fft // 2 + 1
+    R = -(-(L + 2 * pad) // hop)                       # frame slots per utterance (>= the 1 + L_b//hop real frames)
+    Lp = R * hop
+    dev = x.device
+    lens_dev = lens.to(dev)
+    hl = lens.numpy()
+    xp = torch.zeros(B * Lp + n_fft, dtype=f32, device=dev)      # tail: the last slots' windows stay in bounds
+    check(lib().eb_fe_preemph_pad_lens(_p(x), hl.ctypes.data, _p(lens_dev), _p(xp), B, L, Lp, pad,
+                                       float(preemph or 0.0), int(preemph is not None), _s()), "eb_fe_preemph_pad_lens")
+    rows = B * R
+    spec = gemm_f32(xp, hop, 1, basis, 2 * nb, 1, rows, 2 * nb, n_fft)
+    power = torch.empty(rows, nb, dtype=f32, device=dev)
+    check(lib().eb_fe_power(_p(spec), _p(power), rows, nb, _s()), "eb_fe_power")
+    n_mels = fbT.shape[1]
+    feat = gemm_f32(power, nb, 1, fbT, n_mels, 1, rows, n_mels, nb)
+    if dct is not None:
+        check(lib().eb_fe_log(_p(feat), feat.numel(), 1e-6, _s()), "eb_fe_log")
+        feat = gemm_f32(feat, n_mels, 1, dct, dct.shape[1], 1, rows, dct.shape[1], n_mels)
+    C = feat.shape[1]
+    _, T = fe_lengths(hl, hop, n_stack, pad_to_divisible)
+    T_max = max(T)
+    out = torch.empty(B, T_max, C * (3 if delta else 1) * n_stack, dtype=f32, device=dev)
+    if T_max > 0:
+        check(lib().eb_fe_finish(_p(feat), _p(out), hl.ctypes.data, _p(lens_dev), B, R, hop, C, n_stack, T_max,
+                                 int(take_log), int(use_mask), int(delta), int(pad_to_divisible), _s()), "eb_fe_finish")
+    return out, torch.tensor(T, dtype=torch.int32)
+
+
+def fe_deltas(feat):
+    """CatDeltas on frame-major features: feat [B, F, C] fp32 -> [B, F, 3C] = [x, d1, d2] per frame."""
+    _need(feat, f32, "feat")
+    B, F, C = feat.shape
+    out = torch.empty(B, F, 3 * C, dtype=f32, device=feat.device)
+    if out.numel():
+        check(lib().eb_fe_deltas(_p(feat), _p(out), B, F, C, _s()), "eb_fe_deltas")
+    return out
+
+
 def fe_mask(x, spans, axis, fill=0.0):
     """SpecAugment masking in place: x [B, D1, D2] fp32, spans int32 [B, nmask, 2] along axis 1 or 2."""
     _need(x, f32, "x")

@@ -464,6 +464,27 @@ int eb_fe_preemph_pad(const float* x, float* xp, int B, int L, long Lp, int pad,
 int eb_fe_power(const float* spec, float* power, long rows, int nbins, void* stream);
 int eb_fe_log_stack(const float* mel, float* out, int B, int rows_per_utt, int n_frames, int seq_len,
                     int n_mels, int n_stack, int t_out, int take_log, void* stream);
+/* Per-utterance features of a padded batch (rnnt/transforms.py:165-203 applied to each x[b, :L_b] alone, then
+ * rnnt/dataset.py:202-240's zero padding).  Lengths come twice: `lens` on the host, checked before any launch, and
+ * `lens_dev`, the same int32 [B] values on the device, read by the kernels.
+ * eb_fe_preemph_pad_lens : eb_fe_preemph_pad with row b reflected at its own L_b (x rows stay L apart) and zero from
+ *                          L_b + 2*pad on; every L_b must satisfy pad < L_b <= L (torch's reflect pad refuses L_b <= pad).
+ * eb_fe_log              : x := log(x + offset) in place (the MFCC's log(mel + 1e-6), torchaudio MFCC log_mels=True).
+ * eb_fe_finish           : feat[B*rows_per_utt, n_ch] per-frame rows -> out[B, t_out, n_ch*(delta ? 3 : 1)*n_stack]:
+ *                          per utterance the optional log(x + 1e-20), the mask from frame ceil(L_b/hop) on (use_mask),
+ *                          CatDeltas' [x, d1, d2] (compute_deltas twice, window 5, replicate edge at F_b - 1 with
+ *                          F_b = 1 + L_b/hop), Downsample's stacking of n_stack frames, and zeros from
+ *                          T_b = ceil(F_b/n_stack) (floor unless pad_to_divisible) on.  Needs F_b <= rows_per_utt and
+ *                          T_b <= t_out.
+ * eb_fe_deltas           : CatDeltas on feat [B, n_frames, n_ch] -> out [B, n_frames, 3*n_ch] (eb_fe_finish's arithmetic
+ *                          with every utterance n_frames long, no log, no mask, no stacking). */
+int eb_fe_preemph_pad_lens(const float* x, const int* lens, const int* lens_dev, float* xp, int B, int L, long Lp,
+                           int pad, float preemph, int use_preemph, void* stream);
+int eb_fe_log(float* x, long n, float offset, void* stream);
+int eb_fe_finish(const float* feat, float* out, const int* lens, const int* lens_dev, int B, int rows_per_utt, int hop,
+                 int n_ch, int n_stack, int t_out, int take_log, int use_mask, int delta, int pad_to_divisible,
+                 void* stream);
+int eb_fe_deltas(const float* feat, float* out, int B, int n_frames, int n_ch, void* stream);
 /* SpecAugment masks (rnnt/transforms.py:53-147) in place on x [B, D1, D2]: spans int32 [B, nmask, 2] = [start, end)
  * along axis 1 (frequency) or 2 (time); masked elements := fill. */
 int eb_fe_mask(float* x, const int* spans, int B, int D1, int D2, int nmask, int axis, float fill, void* stream);
