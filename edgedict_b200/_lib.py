@@ -26,6 +26,9 @@ SIGNATURES = {
     "eb_rnnt_loss_lattice": (I, [P, P, I, I, I, P, P, I, P]),
     "eb_rnnt_loss_bwd_bf16": (I, [P, P, P, P, P, I, I, I, I, I, P, P, I, D, P]),
     "eb_rnnt_loss_bwd_bf16_db": (I, [P, P, P, P, P, I, I, I, I, I, P, P, I, D, P, P, P]),
+    "eb_rnnt_loss_bwd_fe": (I, [P, P, I, P, P, P, I, I, I, I, I, I, P, P, I, D, D, P]),
+    "eb_rnnt_loss_bwd_bf16_fe": (I, [P, P, P, P, P, I, I, I, I, I, P, P, I, D, D, P]),
+    "eb_rnnt_loss_bwd_bf16_db_fe": (I, [P, P, P, P, P, I, I, I, I, I, P, P, I, D, P, P, D, P]),
     "eb_joint_logits_lse": (I, [P, P, P, P, P, P, P, P, P, P, I, I, I, I, I, I, P]),
     "eb_lm_logits_ce": (I, [P, P, P, P, P, I, P, P, L, I, I, P]),
     "eb_lm_ce_rows": (I, [P, P, I, P, P, L, I, P]),

@@ -20,6 +20,8 @@
 //
 // Arithmetic follows include/detail/gpu_rnnt_kernel.h:5-179 and rnnt_helper.h:17-24.
 #include <atomic>
+#include <cmath>
+#include <type_traits>
 
 #include "common.cuh"
 #include "../../include/rnnt.h"
@@ -417,14 +419,26 @@ template <> struct Store4<__nv_bfloat16> {
     }
 };
 
-template <typename T, typename TO, bool VEC, int WARPS, typename TI = T>
+// FastEmit (Yu et al., ICASSP 2021): the gradient of the surrogate -log P - lambda sum sg(gamma) log p(label | t,u),
+// gamma the occupancy of the emit edge, which scales the gradient along every label edge by (1 + lambda) and leaves
+// the cost alone.  Per cell with a label (u < U-1) it changes two row scalars (include/edgedict_b200.h):
+//   c_all = d + logaddexp(a + beta - ll, log lambda + a + beta(t,u+1) + lpl - ll),   c_lab += log1p(lambda)
+// so the per-element work is unchanged.  The kernels take it as a template flag: FE = false is the plain loss's
+// arithmetic, and never reads lpl.
+template <typename T>
+struct FastEmit {
+    const T* lpl;                                         // log p(label[u] | t,u) of the loss workspace
+    T log_lam, log1p_lam;
+};
+
+template <typename T, typename TO, bool VEC, int WARPS, typename TI = T, bool FE = false>
 __global__ void __launch_bounds__(WARPS * 32)
 rnnt_grad_kernel(const TI* logits, TO* grads, const int* __restrict__ labels,
                  const int* __restrict__ xlen, const int* __restrict__ ylen,
                  const T* __restrict__ denom, const T* __restrict__ alphas,
                  const T* __restrict__ betas, const T* __restrict__ ll_fwd,
                  const T* __restrict__ gscale, int gscale_per_batch, T hscale,
-                 int B, int maxT, int maxU, int V, int blank) {
+                 int B, int maxT, int maxU, int V, int blank, FastEmit<T> fe) {
     const int lane = threadIdx.x & 31;
     const long ncells = (long)B * maxT * maxU;
     const long wstride = (long)gridDim.x * WARPS;
@@ -451,11 +465,15 @@ rnnt_grad_kernel(const TI* logits, TO* grads, const int* __restrict__ labels,
         const T a = alphas[cell], bt_ = betas[cell], ll = ll_fwd[b], d = denom[cell];
         const int lab = (u < Un - 1) ? labels[b * (maxU - 1) + u] : -1;
         // scalar pieces shared by the row
-        const T c_all = a + bt_ - ll + d;                 // exp(c_all + x_v) = exp(a+b+logp-ll)
+        T c_all = a + bt_ - ll + d;                       // exp(c_all + x_v) = exp(a+b+logp-ll)
         T c_blank = M<T>::ninf();                         // log-factor subtracted at v == blank
         if (t < Tn - 1) c_blank = a - ll + d + betas[cell + maxU];
         else if (u == Un - 1) c_blank = a - ll + d;
-        const T c_lab = (lab >= 0) ? a - ll + d + betas[cell + 1] : M<T>::ninf();
+        T c_lab = (lab >= 0) ? a - ll + d + betas[cell + 1] : M<T>::ninf();
+        if (FE && lab >= 0) {
+            c_all = d + lse2(a + bt_ - ll, fe.log_lam + a + betas[cell + 1] + fe.lpl[cell] - ll);
+            c_lab += fe.log1p_lam;
+        }
         for (int v = lane * 4; v < V; v += 128) {
             T x[4];
             Row4<TI, VEC>::load(row, v, V, x);
@@ -497,34 +515,42 @@ __device__ __forceinline__ void cell_btu(long cell, int maxT, int maxU, int& b, 
 // What the row of cell (b, t, u) reads from the workspace, given its clamped lengths Tn, Un.  The loads are kept
 // apart from the arithmetic (grad_row) so that a thread can issue those of several cells before it waits for any.
 struct GradLoads {
-    float a, bt_, ll, d, gs, b_next, b_lab;
+    float a, bt_, ll, d, gs, b_next, b_lab, lpl;
     int lab;
 };
 
+template <bool FE>
 __device__ __forceinline__ GradLoads grad_loads(long cell, int b, int t, int u, int Tn, int Un,
                                                 const int* __restrict__ labels, const float* __restrict__ denom,
                                                 const float* __restrict__ alphas, const float* __restrict__ betas,
                                                 const float* __restrict__ ll_fwd, const float* __restrict__ gscale,
-                                                int gscale_per_batch, int maxU) {
+                                                int gscale_per_batch, int maxU, const FastEmit<float>& fe) {
     GradLoads l;
     l.gs = gscale ? gscale[gscale_per_batch ? b : 0] : 1.f;
     l.a = alphas[cell]; l.bt_ = betas[cell]; l.ll = ll_fwd[b]; l.d = denom[cell];
     l.lab = (u < Un - 1) ? labels[b * (maxU - 1) + u] : -1;
     l.b_next = (t < Tn - 1) ? betas[cell + maxU] : 0.f;
     l.b_lab = (u < Un - 1) ? betas[cell + 1] : 0.f;
+    l.lpl = (FE && u < Un - 1) ? fe.lpl[cell] : 0.f;
     return l;
 }
 
-__device__ __forceinline__ GradRow grad_row(const GradLoads& l, int t, int u, int Tn, int Un, float hscale) {
+template <bool FE>
+__device__ __forceinline__ GradRow grad_row(const GradLoads& l, int t, int u, int Tn, int Un, float hscale,
+                                            const FastEmit<float>& fe) {
     GradRow r;
     r.pad = t >= Tn || u >= Un;
     r.sc = hscale * l.gs;
     r.lab = l.lab;
-    const float c_all = l.a + l.bt_ - l.ll + l.d;
+    float c_all = l.a + l.bt_ - l.ll + l.d;
     r.c_blank = -INFINITY;
     if (t < Tn - 1) r.c_blank = l.a - l.ll + l.d + l.b_next;
     else if (u == Un - 1) r.c_blank = l.a - l.ll + l.d;
     r.c_lab = (r.lab >= 0) ? l.a - l.ll + l.d + l.b_lab : -INFINITY;
+    if (FE && r.lab >= 0) {                               // the same arithmetic as rnnt_grad_kernel's FastEmit branch
+        c_all = l.d + lse2(l.a + l.bt_ - l.ll, fe.log_lam + l.a + l.b_lab + l.lpl - l.ll);
+        r.c_lab += fe.log1p_lam;
+    }
     constexpr float LOG2E = 1.4426950408889634f;
     r.c2 = c_all * LOG2E;
     return r;
@@ -559,13 +585,13 @@ __device__ __forceinline__ uint4 grad_bf16x8(uint4 q, int v, const GradRow& r, i
     return make_uint4(ow[0], ow[1], ow[2], ow[3]);
 }
 
-template <int WARPS>
+template <int WARPS, bool FE>
 __global__ void __launch_bounds__(WARPS * 32)
 rnnt_grad_bf16x8_kernel(const __nv_bfloat16* logits, __nv_bfloat16* grads, const int* __restrict__ labels,
                         const int* __restrict__ xlen, const int* __restrict__ ylen, const float* __restrict__ denom,
                         const float* __restrict__ alphas, const float* __restrict__ betas,
                         const float* __restrict__ ll_fwd, const float* __restrict__ gscale, int gscale_per_batch,
-                        float hscale, int B, int maxT, int maxU, int V, int blank) {
+                        float hscale, int B, int maxT, int maxU, int V, int blank, FastEmit<float> fe) {
     const int lane = threadIdx.x & 31;
     const long ncells = (long)B * maxT * maxU;
     const long wstride = (long)gridDim.x * WARPS;
@@ -574,9 +600,10 @@ rnnt_grad_bf16x8_kernel(const __nv_bfloat16* logits, __nv_bfloat16* grads, const
         cell_btu(cell, maxT, maxU, b, t, u);
         const int Tn = clamp_T(xlen[b], maxT), Un = clamp_U(ylen[b], maxU);
         const bool pad = t >= Tn || u >= Un;
-        const GradRow r = grad_row(pad ? GradLoads{} : grad_loads(cell, b, t, u, Tn, Un, labels, denom, alphas, betas,
-                                                                  ll_fwd, gscale, gscale_per_batch, maxU),
-                                   t, u, Tn, Un, hscale);
+        const GradRow r = grad_row<FE>(pad ? GradLoads{} : grad_loads<FE>(cell, b, t, u, Tn, Un, labels, denom, alphas,
+                                                                          betas, ll_fwd, gscale, gscale_per_batch, maxU,
+                                                                          fe),
+                                       t, u, Tn, Un, hscale, fe);
         const __nv_bfloat16* row = logits + cell * (long)V;
         __nv_bfloat16* orow = grads + cell * (long)V;
         if (r.pad) {
@@ -609,12 +636,14 @@ rnnt_grad_bf16x8_kernel(const __nv_bfloat16* logits, __nv_bfloat16* grads, const
 // That leaves COLSUM_LANES * V / 8 threads (16 warps per SM at V = 1024 on 132 SMs), so each thread keeps the loads
 // of DB_ROWS cells in flight; as in rnnt_grad_bf16x8_kernel, all of them are issued before the first store.
 constexpr int DB_THREADS = 128, DB_ROWS = 4;
+template <bool FE>
 __global__ void __launch_bounds__(DB_THREADS, 4)
 rnnt_grad_db_bf16x8_kernel(const __nv_bfloat16* logits, __nv_bfloat16* grads, const int* __restrict__ labels,
                            const int* __restrict__ xlen, const int* __restrict__ ylen, const float* __restrict__ denom,
                            const float* __restrict__ alphas, const float* __restrict__ betas,
                            const float* __restrict__ ll_fwd, const float* __restrict__ gscale, int gscale_per_batch,
-                           float hscale, int B, int maxT, int maxU, int V, int blank, float* __restrict__ part) {
+                           float hscale, int B, int maxT, int maxU, int V, int blank, float* __restrict__ part,
+                           FastEmit<float> fe) {
     const int V8 = V / 8;
     const int tid = blockIdx.x * DB_THREADS + threadIdx.x;
     if (tid >= COLSUM_LANES * V8) return;
@@ -637,15 +666,15 @@ rnnt_grad_db_bf16x8_kernel(const __nv_bfloat16* logits, __nv_bfloat16* grads, co
         for (int i = 0; i < DB_ROWS; ++i) {
             const long cell = c0 + (long)i * COLSUM_LANES;
             const long cl = cell < ncells ? cell : ncells - 1;
-            l[i] = grad_loads(cl, bi[i], ti[i], ui[i], Tn[i], Un[i], labels, denom, alphas, betas, ll_fwd, gscale,
-                              gscale_per_batch, maxU);
+            l[i] = grad_loads<FE>(cl, bi[i], ti[i], ui[i], Tn[i], Un[i], labels, denom, alphas, betas, ll_fwd, gscale,
+                                  gscale_per_batch, maxU, fe);
             if (ti[i] < Tn[i] && ui[i] < Un[i]) q[i] = *reinterpret_cast<const uint4*>(logits + cell * (long)V + v);
         }
 #pragma unroll
         for (int i = 0; i < DB_ROWS; ++i) {
             const long cell = c0 + (long)i * COLSUM_LANES;
             if (cell >= ncells) break;
-            const GradRow r = grad_row(l[i], ti[i], ui[i], Tn[i], Un[i], hscale);
+            const GradRow r = grad_row<FE>(l[i], ti[i], ui[i], Tn[i], Un[i], hscale, fe);
             const uint4 g = r.pad ? make_uint4(0u, 0u, 0u, 0u) : grad_bf16x8(q[i], v, r, blank);
             *reinterpret_cast<uint4*>(grads + cell * (long)V + v) = g;
             const uint32_t w[4] = {g.x, g.y, g.z, g.w};
@@ -718,6 +747,17 @@ inline bool bad_problem(const int* labels, const int* xlen, const int* ylen, int
            blank >= V || maxU > 1024;
 }
 
+// fastemit_lambda must be a finite lambda >= 0 (NaN fails the comparison)
+inline bool bad_lambda(double lam) { return !(lam >= 0.0) || !std::isfinite(lam); }
+
+// f(std::true_type) for lambda > 0, the FastEmit instantiation of a gradient kernel; f(std::false_type) at lambda = 0,
+// the plain loss's kernel, which runs the same instructions as before FastEmit existed.
+template <typename T, typename F>
+void with_fastemit(const T* lpl, double lam, F&& f) {
+    if (lam > 0.0) f(std::true_type{}, FastEmit<T>{lpl, (T)std::log(lam), (T)std::log1p(lam)});
+    else f(std::false_type{}, FastEmit<T>{nullptr, T(0), T(0)});
+}
+
 template <typename T>
 int loss_fwd(const T* logits, const int* labels, const int* xlen, const int* ylen, int B, int maxT,
              int maxU, int V, int blank, void* ws, int need_beta, cudaStream_t st) {
@@ -739,21 +779,25 @@ int loss_fwd(const T* logits, const int* labels, const int* xlen, const int* yle
 template <typename T, typename TO>
 int loss_bwd(const T* logits, TO* grads, const int* labels, const int* xlen, const int* ylen, int B,
              int maxT, int maxU, int V, int blank, void* ws, const T* gscale, int per_batch,
-             T hscale, cudaStream_t st) {
-    if (!logits || !grads || !ws || bad_problem(labels, xlen, ylen, B, maxT, maxU, V, blank)) return EB_ERR_INVALID;
+             T hscale, double lam, cudaStream_t st) {
+    if (!logits || !grads || !ws || bad_problem(labels, xlen, ylen, B, maxT, maxU, V, blank) || bad_lambda(lam))
+        return EB_ERR_INVALID;
     Workspace<T> w(ws, B, maxT, maxU);
     const long ncells = (long)B * maxT * maxU;
     constexpr int WARPS = 8;
     const bool vec = (V % 4 == 0) && ((reinterpret_cast<uintptr_t>(logits) & 15) == 0) &&
                      ((reinterpret_cast<uintptr_t>(grads) & 15) == 0);
-    if (vec)
-        rnnt_grad_kernel<T, TO, true, WARPS><<<row_grid(ncells, WARPS), WARPS * 32, 0, st>>>(
-            logits, grads, labels, xlen, ylen, w.denom, w.alphas, w.betas, w.ll_fwd, gscale,
-            per_batch, hscale, B, maxT, maxU, V, blank);
-    else
-        rnnt_grad_kernel<T, TO, false, WARPS><<<row_grid(ncells, WARPS), WARPS * 32, 0, st>>>(
-            logits, grads, labels, xlen, ylen, w.denom, w.alphas, w.betas, w.ll_fwd, gscale,
-            per_batch, hscale, B, maxT, maxU, V, blank);
+    with_fastemit(w.lpl, lam, [&](auto fe_on, const FastEmit<T>& fe) {
+        constexpr bool FE = decltype(fe_on)::value;
+        if (vec)
+            rnnt_grad_kernel<T, TO, true, WARPS, T, FE><<<row_grid(ncells, WARPS), WARPS * 32, 0, st>>>(
+                logits, grads, labels, xlen, ylen, w.denom, w.alphas, w.betas, w.ll_fwd, gscale,
+                per_batch, hscale, B, maxT, maxU, V, blank, fe);
+        else
+            rnnt_grad_kernel<T, TO, false, WARPS, T, FE><<<row_grid(ncells, WARPS), WARPS * 32, 0, st>>>(
+                logits, grads, labels, xlen, ylen, w.denom, w.alphas, w.betas, w.ll_fwd, gscale,
+                per_batch, hscale, B, maxT, maxU, V, blank, fe);
+    });
     EB_CHECK_LAUNCH();
     return EB_OK;
 }
@@ -785,7 +829,7 @@ rnntStatus_t compat_entry(const T* acts, T* grads, const int* labels, const int*
     if (rc != EB_OK) return RNNT_STATUS_EXECUTION_FAILED;
     if (grads) {
         rc = loss_bwd<T, T>(acts, grads, labels, input_lengths, label_lengths, B, o.maxT, o.maxU, V,
-                            o.blank_label, workspace, nullptr, 0, T(1), st);
+                            o.blank_label, workspace, nullptr, 0, T(1), 0.0, st);
         if (rc != EB_OK) return RNNT_STATUS_EXECUTION_FAILED;
     }
     Workspace<T> w(workspace, B, o.maxT, o.maxU);
@@ -874,26 +918,34 @@ EB_API int eb_rnnt_loss_fwd(const void* logits, const int* labels, const int* xl
     return EB_OK;
 }
 
-EB_API int eb_rnnt_loss_bwd(const void* logits, void* grads, int grads_bf16, const int* labels,
-                            const int* xlen, const int* ylen, int B, int maxT, int maxU, int V,
-                            int blank, int dtype_size, void* workspace, const void* gscale_dev,
-                            int gscale_per_batch, double host_scale, void* stream) {
+EB_API int eb_rnnt_loss_bwd_fe(const void* logits, void* grads, int grads_bf16, const int* labels,
+                               const int* xlen, const int* ylen, int B, int maxT, int maxU, int V,
+                               int blank, int dtype_size, void* workspace, const void* gscale_dev,
+                               int gscale_per_batch, double host_scale, double fastemit_lambda, void* stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (dtype_size == 4) {
         if (grads_bf16)
             return loss_bwd<float, __nv_bfloat16>((const float*)logits, (__nv_bfloat16*)grads, labels,
                                                   xlen, ylen, B, maxT, maxU, V, blank, workspace,
                                                   (const float*)gscale_dev, gscale_per_batch,
-                                                  (float)host_scale, st);
+                                                  (float)host_scale, fastemit_lambda, st);
         return loss_bwd<float, float>((const float*)logits, (float*)grads, labels, xlen, ylen, B, maxT,
                                       maxU, V, blank, workspace, (const float*)gscale_dev,
-                                      gscale_per_batch, (float)host_scale, st);
+                                      gscale_per_batch, (float)host_scale, fastemit_lambda, st);
     }
     if (dtype_size == 8 && !grads_bf16)
         return loss_bwd<double, double>((const double*)logits, (double*)grads, labels, xlen, ylen, B,
                                         maxT, maxU, V, blank, workspace, (const double*)gscale_dev,
-                                        gscale_per_batch, host_scale, st);
+                                        gscale_per_batch, host_scale, fastemit_lambda, st);
     return EB_ERR_INVALID;
+}
+
+EB_API int eb_rnnt_loss_bwd(const void* logits, void* grads, int grads_bf16, const int* labels,
+                            const int* xlen, const int* ylen, int B, int maxT, int maxU, int V,
+                            int blank, int dtype_size, void* workspace, const void* gscale_dev,
+                            int gscale_per_batch, double host_scale, void* stream) {
+    return eb_rnnt_loss_bwd_fe(logits, grads, grads_bf16, labels, xlen, ylen, B, maxT, maxU, V, blank, dtype_size,
+                               workspace, gscale_dev, gscale_per_batch, host_scale, 0.0, stream);
 }
 
 // Lattice only: denom / lpb / lpl of the workspace were already produced by eb_joint_logits_lse.
@@ -967,10 +1019,12 @@ EB_API int eb_rnnt_viterbi(const int* xlen, const int* ylen, int B, int maxT, in
 }
 
 // Gradient wrt bf16 logits, written as bf16 (grads16 may alias logits16: in place).
-EB_API int eb_rnnt_loss_bwd_bf16(const void* logits16, void* grads16, const int* labels, const int* xlen,
-                                 const int* ylen, int B, int maxT, int maxU, int V, int blank, void* workspace,
-                                 const float* gscale_dev, int gscale_per_batch, double host_scale, void* stream) {
-    if (!logits16 || !grads16 || !workspace || bad_problem(labels, xlen, ylen, B, maxT, maxU, V, blank))
+EB_API int eb_rnnt_loss_bwd_bf16_fe(const void* logits16, void* grads16, const int* labels, const int* xlen,
+                                    const int* ylen, int B, int maxT, int maxU, int V, int blank, void* workspace,
+                                    const float* gscale_dev, int gscale_per_batch, double host_scale,
+                                    double fastemit_lambda, void* stream) {
+    if (!logits16 || !grads16 || !workspace || bad_problem(labels, xlen, ylen, B, maxT, maxU, V, blank) ||
+        bad_lambda(fastemit_lambda))
         return EB_ERR_INVALID;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     Workspace<float> w(workspace, B, maxT, maxU);
@@ -982,42 +1036,64 @@ EB_API int eb_rnnt_loss_bwd_bf16(const void* logits16, void* grads16, const int*
     __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(grads16);
     const bool vec8 = (V % 8 == 0) && ((reinterpret_cast<uintptr_t>(logits16) & 15) == 0) &&
                       ((reinterpret_cast<uintptr_t>(grads16) & 15) == 0);
-    if (vec8)
-        rnnt_grad_bf16x8_kernel<WARPS><<<row_grid(ncells, WARPS), WARPS * 32, 0, st>>>(
-            in, out, labels, xlen, ylen, w.denom, w.alphas, w.betas, w.ll_fwd, gscale_dev, gscale_per_batch,
-            (float)host_scale, B, maxT, maxU, V, blank);
-    else if (vec)
-        rnnt_grad_kernel<float, __nv_bfloat16, true, WARPS, __nv_bfloat16><<<row_grid(ncells, WARPS), WARPS * 32, 0, st>>>(
-            in, out, labels, xlen, ylen, w.denom, w.alphas, w.betas, w.ll_fwd, gscale_dev, gscale_per_batch,
-            (float)host_scale, B, maxT, maxU, V, blank);
-    else
-        rnnt_grad_kernel<float, __nv_bfloat16, false, WARPS, __nv_bfloat16><<<row_grid(ncells, WARPS), WARPS * 32, 0, st>>>(
-            in, out, labels, xlen, ylen, w.denom, w.alphas, w.betas, w.ll_fwd, gscale_dev, gscale_per_batch,
-            (float)host_scale, B, maxT, maxU, V, blank);
+    with_fastemit(w.lpl, fastemit_lambda, [&](auto fe_on, const FastEmit<float>& fe) {
+        constexpr bool FE = decltype(fe_on)::value;
+        if (vec8)
+            rnnt_grad_bf16x8_kernel<WARPS, FE><<<row_grid(ncells, WARPS), WARPS * 32, 0, st>>>(
+                in, out, labels, xlen, ylen, w.denom, w.alphas, w.betas, w.ll_fwd, gscale_dev, gscale_per_batch,
+                (float)host_scale, B, maxT, maxU, V, blank, fe);
+        else if (vec)
+            rnnt_grad_kernel<float, __nv_bfloat16, true, WARPS, __nv_bfloat16, FE>
+                <<<row_grid(ncells, WARPS), WARPS * 32, 0, st>>>(
+                    in, out, labels, xlen, ylen, w.denom, w.alphas, w.betas, w.ll_fwd, gscale_dev, gscale_per_batch,
+                    (float)host_scale, B, maxT, maxU, V, blank, fe);
+        else
+            rnnt_grad_kernel<float, __nv_bfloat16, false, WARPS, __nv_bfloat16, FE>
+                <<<row_grid(ncells, WARPS), WARPS * 32, 0, st>>>(
+                    in, out, labels, xlen, ylen, w.denom, w.alphas, w.betas, w.ll_fwd, gscale_dev, gscale_per_batch,
+                    (float)host_scale, B, maxT, maxU, V, blank, fe);
+    });
     EB_CHECK_LAUNCH();
     return EB_OK;
 }
 
+EB_API int eb_rnnt_loss_bwd_bf16(const void* logits16, void* grads16, const int* labels, const int* xlen,
+                                 const int* ylen, int B, int maxT, int maxU, int V, int blank, void* workspace,
+                                 const float* gscale_dev, int gscale_per_batch, double host_scale, void* stream) {
+    return eb_rnnt_loss_bwd_bf16_fe(logits16, grads16, labels, xlen, ylen, B, maxT, maxU, V, blank, workspace,
+                                    gscale_dev, gscale_per_batch, host_scale, 0.0, stream);
+}
+
 // The same d logits as eb_rnnt_loss_bwd_bf16's 16-byte kernel, and db_accum[c] += sum over the B*maxT*maxU rows of
 // them in eb_colsum's order.  db_part: fp32 scratch of COLSUM_LANES * V.
-EB_API int eb_rnnt_loss_bwd_bf16_db(const void* logits16, void* grads16, const int* labels, const int* xlen,
-                                    const int* ylen, int B, int maxT, int maxU, int V, int blank, void* workspace,
-                                    const float* gscale_dev, int gscale_per_batch, double host_scale, float* db_part,
-                                    float* db_accum, void* stream) {
+EB_API int eb_rnnt_loss_bwd_bf16_db_fe(const void* logits16, void* grads16, const int* labels, const int* xlen,
+                                       const int* ylen, int B, int maxT, int maxU, int V, int blank, void* workspace,
+                                       const float* gscale_dev, int gscale_per_batch, double host_scale,
+                                       float* db_part, float* db_accum, double fastemit_lambda, void* stream) {
     if (!logits16 || !grads16 || !workspace || !db_part || !db_accum ||
-        bad_problem(labels, xlen, ylen, B, maxT, maxU, V, blank) || V % 8 ||
+        bad_problem(labels, xlen, ylen, B, maxT, maxU, V, blank) || bad_lambda(fastemit_lambda) || V % 8 ||
         ((reinterpret_cast<uintptr_t>(logits16) | reinterpret_cast<uintptr_t>(grads16) |
           reinterpret_cast<uintptr_t>(db_part)) & 15))
         return EB_ERR_INVALID;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     Workspace<float> w(workspace, B, maxT, maxU);
     const int threads = COLSUM_LANES * (V / 8);
-    rnnt_grad_db_bf16x8_kernel<<<(threads + DB_THREADS - 1) / DB_THREADS, DB_THREADS, 0, st>>>(
-        reinterpret_cast<const __nv_bfloat16*>(logits16), reinterpret_cast<__nv_bfloat16*>(grads16), labels, xlen, ylen,
-        w.denom, w.alphas, w.betas, w.ll_fwd, gscale_dev, gscale_per_batch, (float)host_scale, B, maxT, maxU, V, blank,
-        db_part);
+    with_fastemit(w.lpl, fastemit_lambda, [&](auto fe_on, const FastEmit<float>& fe) {
+        rnnt_grad_db_bf16x8_kernel<decltype(fe_on)::value><<<(threads + DB_THREADS - 1) / DB_THREADS, DB_THREADS, 0, st>>>(
+            reinterpret_cast<const __nv_bfloat16*>(logits16), reinterpret_cast<__nv_bfloat16*>(grads16), labels, xlen,
+            ylen, w.denom, w.alphas, w.betas, w.ll_fwd, gscale_dev, gscale_per_batch, (float)host_scale, B, maxT, maxU,
+            V, blank, db_part, fe);
+    });
     EB_CHECK_LAUNCH();
     return colsum_lanes_finish(db_part, db_accum, V, st);
+}
+
+EB_API int eb_rnnt_loss_bwd_bf16_db(const void* logits16, void* grads16, const int* labels, const int* xlen,
+                                    const int* ylen, int B, int maxT, int maxU, int V, int blank, void* workspace,
+                                    const float* gscale_dev, int gscale_per_batch, double host_scale, float* db_part,
+                                    float* db_accum, void* stream) {
+    return eb_rnnt_loss_bwd_bf16_db_fe(logits16, grads16, labels, xlen, ylen, B, maxT, maxU, V, blank, workspace,
+                                       gscale_dev, gscale_per_batch, host_scale, db_part, db_accum, 0.0, stream);
 }
 
 // debugging / test access to the lattice (device pointers into the workspace)

@@ -4,6 +4,9 @@ through a torch op on the hot path.
 
 Reference semantics per Function are cited next to each class (paths relative to the reference project).
 """
+import math
+import numbers
+
 import torch
 
 from . import ops
@@ -806,13 +809,26 @@ class JointLogits(torch.autograd.Function):
         return dhe, dhd, dw1, db1, dw2, db2, None
 
 
+def check_fastemit_lambda(value):
+    """FastEmit's lambda as a float: a real number (TypeError otherwise) that is finite and >= 0 (ValueError)."""
+    if isinstance(value, bool) or not isinstance(value, numbers.Real):
+        raise TypeError("fastemit_lambda must be a real number, got %s" % type(value).__name__)
+    lam = float(value)
+    if not math.isfinite(lam) or lam < 0:
+        raise ValueError("fastemit_lambda must be finite and >= 0, got %r" % lam)
+    return lam
+
+
 class RNNTLossFn(torch.autograd.Function):
     """warprnnt_pytorch._RNNT (pytorch_binding/warprnnt_pytorch/__init__.py:10-50) on CUDA logits:
     costs stay on the device, the gradient kernel runs in backward with the upstream gradient
-    folded in (the reference computes it eagerly and rescales it in a second pass)."""
+    folded in (the reference computes it eagerly and rescales it in a second pass).
+    fastemit_lambda > 0 gives backward the FastEmit gradient (include/edgedict_b200.h, eb_rnnt_loss_bwd_fe); the
+    costs are the plain negative log-likelihoods whatever it is."""
 
     @staticmethod
-    def forward(ctx, acts, labels, act_lens, label_lens, blank, reduction):
+    def forward(ctx, acts, labels, act_lens, label_lens, blank, reduction, fastemit_lambda=0.0):
+        ctx.fastemit_lambda = check_fastemit_lambda(fastemit_lambda)
         acts = _c(acts)
         costs, ws = ops.rnnt_loss_fwd(acts, labels, act_lens, label_lens, blank, need_beta=True)
         B = acts.shape[0]
@@ -829,8 +845,9 @@ class RNNTLossFn(torch.autograd.Function):
         acts, labels, act_lens, label_lens, ws = ctx.saved_tensors
         scale = 1.0 / ctx.B if ctx.reduction == "mean" else 1.0
         g = _c(go.to(acts.dtype)).view(-1)
-        grads = ops.rnnt_loss_bwd(acts, labels, act_lens, label_lens, ctx.blank, ws, g, scale)
-        return grads, None, None, None, None, None
+        grads = ops.rnnt_loss_bwd(acts, labels, act_lens, label_lens, ctx.blank, ws, g, scale,
+                                  fastemit_lambda=ctx.fastemit_lambda)
+        return grads, None, None, None, None, None, None
 
 
 class LogSoftmax(torch.autograd.Function):
@@ -916,10 +933,12 @@ class CTCLossFn(torch.autograd.Function):
 class JointLoss(torch.autograd.Function):
     """Transducer.forward's joint + loss (rnnt/models.py:234-239) as one autograd node: logits are
     produced, consumed by the loss, and their gradient is written IN PLACE over them (fp32 mode)
-    or straight to bf16 (bf16 mode) -- no autograd copy of the 8 GB tensor is ever made."""
+    or straight to bf16 (bf16 mode) -- no autograd copy of the 8 GB tensor is ever made.
+    fastemit_lambda > 0: every backward branch writes the FastEmit gradient; the loss and costs do not change."""
 
     @staticmethod
-    def forward(ctx, h_enc, h_dec, w1, b1, w2, b2, labels, act_lens, label_lens, blank, precision):
+    def forward(ctx, h_enc, h_dec, w1, b1, w2, b2, labels, act_lens, label_lens, blank, precision, fastemit_lambda=0.0):
+        ctx.fastemit_lambda = check_fastemit_lambda(fastemit_lambda)
         B, T, E = h_enc.shape
         U, Dd = h_dec.shape[1], h_dec.shape[2]
         J, V = w1.shape[0], w2.shape[0]
@@ -954,19 +973,24 @@ class JointLoss(torch.autograd.Function):
         B, T, U, E, Dd, J, V = ctx.dims
         p = ctx.precision
         g = _c(go.to(f32)).view(-1)
+        lam = ctx.fastemit_lambda
         db2 = None
         if logits.dtype == bf16 and V % 8 == 0:
             # the bias gradient comes out of the gradient kernel, which holds every d logit it writes: the output layer's
             # side stream is left with dW2 alone
-            dl, db2 = ops.rnnt_loss_bwd_bf16_db(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B)
+            dl, db2 = ops.rnnt_loss_bwd_bf16_db(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B,
+                                                fastemit_lambda=lam)
         elif logits.dtype == bf16:
-            dl = ops.rnnt_loss_bwd_bf16(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B)
+            dl = ops.rnnt_loss_bwd_bf16(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B,
+                                        fastemit_lambda=lam)
         elif p == "bf16":
-            dl = ops.rnnt_loss_bwd(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B, out_bf16=True)
+            dl = ops.rnnt_loss_bwd(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B, out_bf16=True,
+                                   fastemit_lambda=lam)
         else:
-            dl = ops.rnnt_loss_bwd(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B, out=logits)
+            dl = ops.rnnt_loss_bwd(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B, out=logits,
+                                   fastemit_lambda=lam)
         dhe, dhd, dw1, db1, dw2, db2 = _joint_bwd(p, dl.view(B * T * U, V), hid, he2, hd2, w1, w2, ctx.dims, db2)
-        return dhe, dhd, dw1, db1, dw2, db2, None, None, None, None, None
+        return dhe, dhd, dw1, db1, dw2, db2, None, None, None, None, None, None
 
 
 def conv_out_len(T, k, s):

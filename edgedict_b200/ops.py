@@ -616,16 +616,19 @@ def rnnt_loss_fwd(logits, labels, xlen, ylen, blank, need_beta=True):
     return costs, ws
 
 
-def rnnt_loss_bwd(logits, labels, xlen, ylen, blank, ws, gscale, host_scale, out=None, out_bf16=False):
+def rnnt_loss_bwd(logits, labels, xlen, ylen, blank, ws, gscale, host_scale, out=None, out_bf16=False,
+                  fastemit_lambda=0.0):
+    """d loss / d logits (fp32 / fp64, or bf16 with out_bf16), with the FastEmit gradient for fastemit_lambda > 0
+    (include/edgedict_b200.h, eb_rnnt_loss_bwd_fe); at 0 the plain loss's gradient."""
     B, T, U, V = logits.shape
     ds = 8 if logits.dtype == torch.float64 else 4
     if out is None:
         out = torch.empty(logits.shape, dtype=bf16 if out_bf16 else logits.dtype, device=logits.device)
     per_batch = int(gscale is not None and gscale.numel() > 1)
     with _timed("rnnt_loss_bwd", 1, float(ds + out.element_size()) * B * T * U * V, 0.0):
-        check(lib().eb_rnnt_loss_bwd(_p(logits), _p(out), int(out.dtype == bf16), _p(labels), _p(xlen), _p(ylen), B, T,
-                                     U, V, blank, ds, _p(ws), _p(gscale), per_batch, float(host_scale), _s()),
-              "eb_rnnt_loss_bwd")
+        check(lib().eb_rnnt_loss_bwd_fe(_p(logits), _p(out), int(out.dtype == bf16), _p(labels), _p(xlen), _p(ylen), B,
+                                        T, U, V, blank, ds, _p(ws), _p(gscale), per_batch, float(host_scale),
+                                        float(fastemit_lambda), _s()), "eb_rnnt_loss_bwd_fe")
     return out
 
 
@@ -667,27 +670,29 @@ def rnnt_viterbi(xlen, ylen, B, T, U, ws, dtype):
     return frames, label_logp, score
 
 
-def rnnt_loss_bwd_bf16(logits16, labels, xlen, ylen, blank, ws, gscale, host_scale):
-    """In place: logits16 becomes d loss / d logits (bf16)."""
+def rnnt_loss_bwd_bf16(logits16, labels, xlen, ylen, blank, ws, gscale, host_scale, fastemit_lambda=0.0):
+    """In place: logits16 becomes d loss / d logits (bf16), FastEmit's for fastemit_lambda > 0."""
     B, T, U, V = logits16.shape
     per_batch = int(gscale is not None and gscale.numel() > 1)
     with _timed("rnnt_loss_bwd", 1, 4.0 * B * T * U * V, 0.0):
-        check(lib().eb_rnnt_loss_bwd_bf16(_p(logits16), _p(logits16), _p(labels), _p(xlen), _p(ylen), B, T, U, V, blank,
-                                          _p(ws), _p(gscale), per_batch, float(host_scale), _s()), "eb_rnnt_loss_bwd_bf16")
+        check(lib().eb_rnnt_loss_bwd_bf16_fe(_p(logits16), _p(logits16), _p(labels), _p(xlen), _p(ylen), B, T, U, V,
+                                             blank, _p(ws), _p(gscale), per_batch, float(host_scale),
+                                             float(fastemit_lambda), _s()), "eb_rnnt_loss_bwd_bf16_fe")
     return logits16
 
 
-def rnnt_loss_bwd_bf16_db(logits16, labels, xlen, ylen, blank, ws, gscale, host_scale):
-    """In place: logits16 becomes d loss / d logits (bf16), as rnnt_loss_bwd_bf16 writes them; also returns their column
-    sum db [V] fp32, the same bits as colsum(logits16.view(-1, V)) afterwards.  V % 8 == 0."""
+def rnnt_loss_bwd_bf16_db(logits16, labels, xlen, ylen, blank, ws, gscale, host_scale, fastemit_lambda=0.0):
+    """In place: logits16 becomes d loss / d logits (bf16), as rnnt_loss_bwd_bf16 writes them for the same
+    fastemit_lambda; also returns their column sum db [V] fp32, the same bits as colsum(logits16.view(-1, V))
+    afterwards.  V % 8 == 0."""
     B, T, U, V = logits16.shape
     per_batch = int(gscale is not None and gscale.numel() > 1)
     part = torch.empty(COLSUM_LANES * V, dtype=f32, device=logits16.device)
     db = torch.zeros(V, dtype=f32, device=logits16.device)
     with _timed("rnnt_loss_bwd", 2, 4.0 * B * T * U * V, 0.0):
-        check(lib().eb_rnnt_loss_bwd_bf16_db(_p(logits16), _p(logits16), _p(labels), _p(xlen), _p(ylen), B, T, U, V,
-                                             blank, _p(ws), _p(gscale), per_batch, float(host_scale), _p(part), _p(db),
-                                             _s()), "eb_rnnt_loss_bwd_bf16_db")
+        check(lib().eb_rnnt_loss_bwd_bf16_db_fe(_p(logits16), _p(logits16), _p(labels), _p(xlen), _p(ylen), B, T, U, V,
+                                                blank, _p(ws), _p(gscale), per_batch, float(host_scale), _p(part),
+                                                _p(db), float(fastemit_lambda), _s()), "eb_rnnt_loss_bwd_bf16_db_fe")
     return logits16, db
 
 

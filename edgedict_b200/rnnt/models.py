@@ -243,7 +243,8 @@ class Transducer(nn.Module):
 
     def __init__(self, vocab_embed_size, vocab_size, input_size, enc_hidden_size, enc_layers,
                  enc_dropout, enc_proj_size, dec_hidden_size, dec_layers, dec_dropout, dec_proj_size,
-                 joint_size, enc_time_reductions=[1], blank=NUL, module_type='LSTM', output_loss=True):
+                 joint_size, enc_time_reductions=[1], blank=NUL, module_type='LSTM', output_loss=True,
+                 fastemit_lambda=0.0):
         super().__init__()
         self.blank = blank
         if module_type not in ['GRU', 'LSTM']:
@@ -263,6 +264,10 @@ class Transducer(nn.Module):
             from ..warprnnt_pytorch import RNNTLoss
             self.loss_fn = RNNTLoss(blank=blank)
         self.last_costs = None
+        # FastEmit's lambda for the loss's backward (warprnnt_pytorch.rnnt_loss): a plain attribute, read at every
+        # forward, so a trainer can ramp it between steps; not part of the state_dict.  The loss value and last_costs
+        # do not depend on it.
+        self.fastemit_lambda = Fn.check_fastemit_lambda(fastemit_lambda)
 
     def set_precision(self, precision):
         return _set_precision(self, precision)
@@ -271,6 +276,7 @@ class Transducer(nn.Module):
         return scale_length(logits.shape[1], xlen)
 
     def forward(self, xs, ys, xlen, ylen):
+        lam = Fn.check_fastemit_lambda(self.fastemit_lambda) if self.output_loss else 0.0
         h_enc, h_dec = self._encode(xs, ys, xlen, ylen)
         if not self.output_loss:
             return self.joint(h_enc, h_dec)
@@ -278,7 +284,7 @@ class Transducer(nn.Module):
         yl = _lens_to_device(_i32(ylen), h_enc.device)
         l0, l2 = self.joint.joint[0], self.joint.joint[2]
         loss, costs = Fn.JointLoss.apply(h_enc, h_dec, l0.weight, l0.bias, l2.weight, l2.bias,
-                                         _i32(ys[:, :int(ylen.max())]), xl, yl, self.blank, _precision(self))
+                                         _i32(ys[:, :int(ylen.max())]), xl, yl, self.blank, _precision(self), lam)
         self.last_costs = costs
         return loss
 

@@ -6,7 +6,7 @@ the native status code is checked (the reference's binding drops it, binding.cpp
 import torch
 from torch.nn import Module
 
-from ..functional import RNNTLossFn
+from ..functional import RNNTLossFn, check_fastemit_lambda
 
 __all__ = ['rnnt_loss', 'RNNTLoss']
 
@@ -52,24 +52,33 @@ def certify_inputs(log_probs, labels, lengths, label_lengths):
         raise ValueError("Output length mismatch")
 
 
-def rnnt_loss(acts, labels, act_lens, label_lens, blank=0, reduction='mean'):
-    """acts [B,T,U+1,V] raw logits on CUDA (fp32 or fp64); labels [B,U] int32; lengths int32."""
+def rnnt_loss(acts, labels, act_lens, label_lens, blank=0, reduction='mean', fastemit_lambda=0.0):
+    """acts [B,T,U+1,V] raw logits on CUDA (fp32 or fp64); labels [B,U] int32; lengths int32.
+
+    fastemit_lambda: FastEmit's regularisation weight (Yu et al., ICASSP 2021), a finite real >= 0.  Above 0 the
+    gradient along every label-emitting edge of the lattice is scaled by (1 + fastemit_lambda), which teaches a
+    streaming transducer to emit its tokens earlier (include/edgedict_b200.h, eb_rnnt_loss_bwd_fe).  It acts in the
+    backward pass only: the returned costs are the plain negative log-likelihoods, bit for bit those of 0."""
+    fastemit_lambda = check_fastemit_lambda(fastemit_lambda)
     certify_inputs(acts, labels, act_lens, label_lens)
     if not acts.is_cuda:
         raise RuntimeError("edgedict_b200.warprnnt_pytorch is CUDA-only (sm_90a); got CPU activations")
     if acts.dtype not in (torch.float32, torch.float64):
         raise TypeError("unsupported data type {} (float32/float64 only, as in binding.cpp:46-80)".format(acts.dtype))
     dev = acts.device
-    return RNNTLossFn.apply(acts, labels.to(dev), act_lens.to(dev), label_lens.to(dev), blank, reduction)
+    return RNNTLossFn.apply(acts, labels.to(dev), act_lens.to(dev), label_lens.to(dev), blank, reduction,
+                            fastemit_lambda)
 
 
 class RNNTLoss(Module):
-    """RNNTLoss(blank=0, reduction='mean'): 'none' | 'sum' | 'mean' (= sum / batch size)."""
+    """RNNTLoss(blank=0, reduction='mean', fastemit_lambda=0.0): 'none' | 'sum' | 'mean' (= sum / batch size);
+    fastemit_lambda as in rnnt_loss (backward only, the costs do not change)."""
 
-    def __init__(self, blank=0, reduction='mean'):
+    def __init__(self, blank=0, reduction='mean', fastemit_lambda=0.0):
         super(RNNTLoss, self).__init__()
         self.blank = blank
         self.reduction = reduction
+        self.fastemit_lambda = check_fastemit_lambda(fastemit_lambda)
 
     def forward(self, acts, labels, act_lens, label_lens):
-        return rnnt_loss(acts, labels, act_lens, label_lens, self.blank, self.reduction)
+        return rnnt_loss(acts, labels, act_lens, label_lens, self.blank, self.reduction, self.fastemit_lambda)

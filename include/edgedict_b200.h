@@ -49,6 +49,30 @@ int eb_rnnt_loss_bwd_bf16(const void* logits16, void* grads16, const int* labels
 int eb_rnnt_loss_bwd_bf16_db(const void* logits16, void* grads16, const int* labels, const int* xlen, const int* ylen,
                              int B, int maxT, int maxU, int V, int blank, void* workspace, const float* gscale_dev,
                              int gscale_per_batch, double host_scale, float* db_part, float* db_accum, void* stream);
+/* FastEmit (Yu et al., ICASSP 2021): the three backward entries above with fastemit_lambda = lambda >= 0 (finite, else
+ * EB_ERR_INVALID before any launch); each of those is the _fe entry with lambda = 0, whose gradient is the same bits.
+ * The gradient is that of the surrogate
+ *   S_b = -log P_b - lambda sum_{t < T, u < U-1} sg(gamma(t,u)) y(t,u),  y(t,u) = log p(label[u] | t,u),
+ *   gamma(t,u) = exp(alpha(t,u) + y(t,u) + beta(t,u+1) - log P_b)   (the occupancy of the emit edge; sg: no gradient),
+ * which scales the gradient along every label-emitting edge by (1 + lambda).  With a = alpha(t,u), beta = beta(t,u),
+ * d = denom(t,u), ll = ll_fwd[b] and lpl = lpl(t,u) of the workspace, the cells u < U-1 of the gradient become
+ *   g_v = exp(c_all + x_v) - [v = blank] exp(c_blank + x_v) - [v = label[u]] exp(c_lab + x_v),
+ *   c_all = d + logaddexp(a + beta - ll, log lambda + a + beta(t,u+1) + lpl - ll),
+ *   c_lab = a - ll + d + beta(t,u+1) + log1p(lambda),
+ * and everything else is the plain loss's gradient: c_blank, the cells u = U-1, zero on padded cells and for T = 0, and
+ * the scaling by host_scale * gscale.  Every valid row still sums to zero.  lambda changes no cost: costs and the
+ * workspace are those of eb_rnnt_loss_fwd / eb_joint_logits_lse + eb_rnnt_loss_lattice, which take no lambda. */
+int eb_rnnt_loss_bwd_fe(const void* logits, void* grads, int grads_bf16, const int* labels, const int* xlen,
+                        const int* ylen, int B, int maxT, int maxU, int V, int blank, int dtype_size, void* workspace,
+                        const void* gscale_dev, int gscale_per_batch, double host_scale, double fastemit_lambda,
+                        void* stream);
+int eb_rnnt_loss_bwd_bf16_fe(const void* logits16, void* grads16, const int* labels, const int* xlen, const int* ylen,
+                             int B, int maxT, int maxU, int V, int blank, void* workspace, const float* gscale_dev,
+                             int gscale_per_batch, double host_scale, double fastemit_lambda, void* stream);
+int eb_rnnt_loss_bwd_bf16_db_fe(const void* logits16, void* grads16, const int* labels, const int* xlen,
+                                const int* ylen, int B, int maxT, int maxU, int V, int blank, void* workspace,
+                                const float* gscale_dev, int gscale_per_batch, double host_scale, float* db_part,
+                                float* db_accum, double fastemit_lambda, void* stream);
 int eb_rnnt_workspace_views(void* workspace, int B, int maxT, int maxU, int dtype_size,
                             void** denom, void** alphas, void** betas, void** ll_fwd, void** ll_bwd);
 /* Forced (Viterbi) alignment over a workspace that eb_rnnt_loss_fwd (any need_beta) or eb_joint_logits_lse filled;
