@@ -52,6 +52,17 @@ SIGNATURES = {
     "eb_gemm_bf16_dtanh": (I, [P, I, P, I, P, P, L, I, L, P]),
     "eb_gemm_tc_set_trace": (I, [P, I]),
     "eb_joint_dpre_reduce": (I, [P, P, P, I, I, I, I, P]),
+    "eb_rnnt_simple_scratch_bytes": (Z, [I, I, I, I]),
+    "eb_rnnt_simple_stats": (I, [P, P, P, P, P, I, I, I, I, I, P, P, P]),
+    "eb_rnnt_simple_bwd": (I, [P, P, P, P, P, I, I, I, I, I, P, P, P, I, D, P, P, P]),
+    "eb_rnnt_band_choice": (I, [P, P, I, I, I, I, P, P, P, P]),
+    "eb_joint_band_hidden_fwd": (I, [P, P, P, P, P, P, I, I, I, I, I, I, P]),
+    "eb_rnnt_band_loss_fwd": (I, [P, P, P, P, P, P, I, I, I, I, I, I, P, P, I, P]),
+    "eb_rnnt_band_loss_bwd": (I, [P, P, I, P, P, P, P, P, I, I, I, I, I, I, P, P, I, D, P]),
+    "eb_joint_band_dpre_reduce": (I, [P, P, I, P, P, P, P, P, I, I, I, I, I, P]),
+    "eb_rnnt_band_lattice": (I, [P, P, P, P, I, I, I, I, P, P, I, P]),
+    "eb_joint_band_logits_lse": (I, [P, P, P, P, P, P, P, P, P, P, P, I, I, I, I, I, I, I, P]),
+    "eb_rnnt_band_loss_bwd_bf16_db": (I, [P, P, P, P, P, P, P, I, I, I, I, I, I, P, P, I, D, P, P, P]),
     "eb_lstm_scratch_bytes": (Z, [I, I]),
     "eb_lstm_seq_fwd": (I, [P, P, P, P, P, P, P, P, P, P, I, I, I, P]),
     "eb_lstm_seq_bwd": (I, [P, P, P, P, P, P, P, P, P, P, P, I, I, I, P]),

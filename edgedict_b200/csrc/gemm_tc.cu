@@ -87,7 +87,10 @@ struct Sched {
 // LSE_ROWS is the same epilogue for the language model's output layer (eb_lm_logits_ce): row r has its own target
 // targets[r], denom[r] receives the row's log-sum-exp and lpl[r] the target's logit (0 for a target outside [0, N),
 // which is never used to index anything).
-constexpr int LSE_NONE = 0, LSE_RNNT = 1, LSE_ROWS = 2;
+// LSE_BAND is LSE_RNNT over the pruned loss's band rows m = (b*maxT + t)*R + r (eb_joint_band_logits_lse): row m holds
+// cell (t, u = s_begin[b*maxT + t] + r), targets = s_begin and targets64 = R; rows with t >= T_b, r >= min(R, U_b) or u
+// outside [0, U_b) write nothing.
+constexpr int LSE_NONE = 0, LSE_RNNT = 1, LSE_ROWS = 2, LSE_BAND = 3;
 struct LseArgs {
     const int* labels; const int* xlen; const int* ylen;     // [B,maxU-1], [B], [B]
     float* denom; float* lpb; float* lpl;                     // [B*maxT*maxU] each (loss workspace)
@@ -311,6 +314,18 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                             lab[h] = (t >= 0 && t < N) ? (int)t : -1;
                             cell_ok[h] = true;
                         }
+                    } else if constexpr (LSE == LSE_BAND) {
+                        if (cell < M) {
+                            const int R = lse.targets64;
+                            const long bt = cell / R;
+                            const int r = (int)(cell % R);
+                            const int t = (int)(bt % lse.maxT), b = (int)(bt / lse.maxT);
+                            const int Tn = min(max(lse.xlen[b], 0), lse.maxT);
+                            const int Un = min(max(lse.ylen[b], 0) + 1, lse.maxU);
+                            const int u = static_cast<const int*>(lse.targets)[bt] + r;
+                            cell_ok[h] = t < Tn && r < min(R, Un) && u >= r && u < Un;
+                            if (cell_ok[h] && u < Un - 1) lab[h] = lse.labels[b * (lse.maxU - 1) + u];
+                        }
                     } else if (cell < M) {
                         const int u = (int)(cell % lse.maxU);
                         const long bt = cell / lse.maxU;
@@ -392,7 +407,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                             lse.lpl[row] = xl[h];
                         }
                     } else if ((lane & 3) == 0 && cell_ok[h]) {
-                        const long cell = m0 + r_in + 8 * h;
+                        long cell = m0 + r_in + 8 * h;
+                        if constexpr (LSE == LSE_BAND) {
+                            const long bt = cell / lse.targets64;
+                            cell = bt * lse.maxU + static_cast<const int*>(lse.targets)[bt] + (int)(cell % lse.targets64);
+                        }
                         const float d = -(rm[h] + logf(rs[h]));
                         lse.denom[cell] = d;
                         lse.lpb[cell] = d + xb[h];
@@ -672,6 +691,36 @@ EB_API int eb_joint_logits_lse(const void* hidden16, const void* w2_16, const fl
     lse.targets = nullptr; lse.targets64 = 0;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     return launch_lse<LSE_RNNT>(ta, tb, sc ? &tc : nullptr, logits16, b2, M, V, J, lse, st);
+}
+
+// The same epilogue over the pruned loss's band rows (LSE_BAND): logits16 [B*maxT*R, V], and the statistics of band
+// row m = (b*maxT + t)*R + r at cell (t, s_begin[b*maxT + t] + r) of the [B, maxT, maxU] workspace arrays (valid band
+// rows only; include/edgedict_b200.h).
+EB_API int eb_joint_band_logits_lse(const void* hidden16, const void* w2_16, const float* b2, void* logits16,
+                                    const int* labels, const int* xlen, const int* ylen, const int* s_begin,
+                                    float* denom, float* lpb, float* lpl, int B, int maxT, int maxU, int R, int V, int J,
+                                    int blank, void* stream) {
+    if (!hidden16 || !w2_16 || !logits16 || !xlen || !ylen || !s_begin || !denom || !lpb || !lpl ||
+        (!labels && maxU > 1) || B <= 0 || maxT <= 0 || maxU <= 0 || maxU > 1024 || R < 2 || R > 64 || V <= 0 ||
+        J <= 0 || J % 8 || blank < 0 || blank >= V)
+        return EB_ERR_INVALID;
+    if ((reinterpret_cast<uintptr_t>(hidden16) & 15) || (reinterpret_cast<uintptr_t>(w2_16) & 15) ||
+        (b2 && (reinterpret_cast<uintptr_t>(b2) & 15)) || (reinterpret_cast<uintptr_t>(logits16) & 3))
+        return EB_ERR_INVALID;
+    const long M = (long)B * maxT * R;
+    CUtensorMap ta, tb, tc;
+    const bool sc = staged_c(logits16, 1, 0, V, 1, nullptr);
+    if (!make_map(&ta, hidden16, (uint64_t)J, (uint64_t)M, 128) || !make_map(&tb, w2_16, (uint64_t)J, (uint64_t)V, 128) ||
+        (sc && !make_c_maps(&tc, nullptr, logits16, nullptr, M, V))) {
+        fprintf(stderr, "[edgedict_b200] cuTensorMapEncodeTiled failed\n");
+        return EB_ERR_CUDA;
+    }
+    LseArgs lse;
+    lse.labels = labels; lse.xlen = xlen; lse.ylen = ylen; lse.denom = denom; lse.lpb = lpb; lse.lpl = lpl;
+    lse.maxT = maxT; lse.maxU = maxU; lse.blank = blank; lse.aux = nullptr;
+    lse.targets = s_begin; lse.targets64 = R;
+    return launch_lse<LSE_BAND>(ta, tb, sc ? &tc : nullptr, logits16, b2, M, V, J, lse,
+                                reinterpret_cast<cudaStream_t>(stream));
 }
 
 // The language model's output layer with the statistics of its cross-entropy (LMModel.loss, bf16 mode): the joint's

@@ -19,6 +19,7 @@
 // compute_rnnt_loss(), whose contract returns costs in HOST memory (include/rnnt.h).
 //
 // Arithmetic follows include/detail/gpu_rnnt_kernel.h:5-179 and rnnt_helper.h:17-24.
+#include <algorithm>
 #include <atomic>
 #include <cmath>
 #include <type_traits>
@@ -96,6 +97,37 @@ template <bool VEC> struct Row4<__nv_bfloat16, VEC> {
 // ---------------------------------------------------------------------------------------------
 // 1. denominators + (blank, label) gather
 // ---------------------------------------------------------------------------------------------
+// One warp's statistics of one row of V logits: d = -logsumexp and the blank / label logits xb, xl (0 where absent).
+// rnnt_denom_kernel and rnnt_band_denom_kernel share it, so a band row and the same dense cell get the same bits.
+template <typename T, bool VEC>
+__device__ __forceinline__ void denom_row(const T* row, int lane, int V, int blank, int lab, T& d, T& xb_out,
+                                          T& xl_out) {
+    // online max / sum-exp over this lane's 4-wide chunks
+    T m = M<T>::ninf(), s = 0, xb = 0, xl = 0;
+    for (int v = lane * 4; v < V; v += 128) {
+        T x[4];
+        Row4<T, VEC>::load(row, v, V, x);
+        T cm = fmax(fmax(x[0], x[1]), fmax(x[2], x[3]));
+        T nm = fmax(m, cm);
+        T acc = 0;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            acc += M<T>::exp_fast(x[i] - nm);       // exp(-inf) = 0 for the masked tail
+            if (v + i == blank) xb = x[i];
+            if (v + i == lab) xl = x[i];
+        }
+        s = s * M<T>::exp_fast(m - nm) + acc;       // m = -inf on first chunk => s*0
+        m = nm;
+    }
+    T gm = warp_max(m);
+    s *= M<T>::exp_fast(m - gm);
+    s = warp_sum(s);
+    d = -gm - M<T>::log_acc(s);
+    // the lane that saw the blank / label column owns the value: reduce by sum of one-hot
+    xb_out = warp_sum(xb);
+    xl_out = warp_sum(xl);
+}
+
 template <typename T, bool VEC, int WARPS>
 __global__ void __launch_bounds__(WARPS * 32)
 rnnt_denom_kernel(const T* __restrict__ logits, const int* __restrict__ labels,
@@ -114,30 +146,8 @@ rnnt_denom_kernel(const T* __restrict__ logits, const int* __restrict__ labels,
         if (t >= Tn || u >= Un) continue;                // padded cell: never read
         const T* row = logits + cell * (long)V;
         const int lab = (u < Un - 1) ? labels[b * (maxU - 1) + u] : -1;
-        // online max / sum-exp over this lane's 4-wide chunks
-        T m = M<T>::ninf(), s = 0, xb = 0, xl = 0;
-        for (int v = lane * 4; v < V; v += 128) {
-            T x[4];
-            Row4<T, VEC>::load(row, v, V, x);
-            T cm = fmax(fmax(x[0], x[1]), fmax(x[2], x[3]));
-            T nm = fmax(m, cm);
-            T acc = 0;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                acc += M<T>::exp_fast(x[i] - nm);       // exp(-inf) = 0 for the masked tail
-                if (v + i == blank) xb = x[i];
-                if (v + i == lab) xl = x[i];
-            }
-            s = s * M<T>::exp_fast(m - nm) + acc;       // m = -inf on first chunk => s*0
-            m = nm;
-        }
-        T gm = warp_max(m);
-        s *= M<T>::exp_fast(m - gm);
-        s = warp_sum(s);
-        const T d = -gm - M<T>::log_acc(s);
-        // the lane that saw the blank / label column owns the value: reduce by sum of one-hot
-        xb = warp_sum(xb);
-        xl = warp_sum(xl);
+        T d, xb, xl;
+        denom_row<T, VEC>(row, lane, V, blank, lab, d, xb, xl);
         if (lane == 0) {
             denom[cell] = d;
             lpb[cell] = d + xb;
@@ -840,6 +850,177 @@ rnntStatus_t compat_entry(const T* acts, T* grads, const int* labels, const int*
     return RNNT_STATUS_SUCCESS;
 }
 
+// ---------------------------------------------------------------------------------------------
+// 4. Pruned RNN-T (include/edgedict_b200.h, eb_rnnt_band_loss_fwd): band rows m = (b*maxT + t)*R + r hold the
+//    logits of cell (b, t, u = s_begin[b,t] + r) for r < Rb = min(R, U_b).  The statistics of a band row go to that
+//    cell of a full [B, maxT, maxU] workspace (the same bits rnnt_denom_kernel writes for the same logits), every other
+//    valid cell gets -inf, and the unchanged lattice runs on it.  The gradient of a band row is rnnt_grad_kernel's.
+// ---------------------------------------------------------------------------------------------
+struct Band {
+    const int* s_begin;                                   // [B, maxT]
+    const int* nopath;                                    // [B]: 1 when the bands hold no path (cost +inf)
+    int R;
+};
+
+// the cell of band row m, or false for a padding row (t >= T_b, r >= Rb, or an utterance without a band path)
+__device__ __forceinline__ bool band_cell(long m, const Band& bd, const int* xlen, const int* ylen, int maxT, int maxU,
+                                          int& b, int& t, int& u, int& Tn, int& Un) {
+    const int r = (int)(m % bd.R);
+    const long bt = m / bd.R;
+    t = (int)(bt % maxT);
+    b = (int)(bt / maxT);
+    Tn = clamp_T(xlen[b], maxT);
+    Un = clamp_U(ylen[b], maxU);
+    if (t >= Tn || r >= min(bd.R, Un) || bd.nopath[b]) return false;
+    u = bd.s_begin[bt] + r;
+    return u >= r && u < Un;                              // a start outside [0, U_b - r): a padding row
+}
+
+template <bool VEC, int WARPS>
+__global__ void __launch_bounds__(WARPS * 32)
+rnnt_band_denom_kernel(const float* __restrict__ logits, const int* __restrict__ labels,
+                       const int* __restrict__ xlen, const int* __restrict__ ylen, Band bd,
+                       float* __restrict__ denom, float* __restrict__ lpb, float* __restrict__ lpl,
+                       int B, int maxT, int maxU, int V, int blank) {
+    const int lane = threadIdx.x & 31;
+    const long nrows = (long)B * maxT * bd.R;
+    const long wstride = (long)gridDim.x * WARPS;
+    for (long m = (long)blockIdx.x * WARPS + (threadIdx.x >> 5); m < nrows; m += wstride) {
+        int b, t, u, Tn, Un;
+        if (!band_cell(m, bd, xlen, ylen, maxT, maxU, b, t, u, Tn, Un)) continue;
+        const long cell = ((long)b * maxT + t) * maxU + u;
+        const int lab = (u < Un - 1) ? labels[b * (maxU - 1) + u] : -1;
+        float d, xb, xl;
+        denom_row<float, VEC>(logits + m * (long)V, lane, V, blank, lab, d, xb, xl);
+        if (lane == 0) {
+            denom[cell] = d;
+            lpb[cell] = d + xb;
+            lpl[cell] = d + xl;
+        }
+    }
+}
+
+// -inf statistics for the valid cells outside the band of their frame (all of them when the bands hold no path)
+__global__ void rnnt_band_fill_kernel(const int* __restrict__ xlen, const int* __restrict__ ylen, Band bd,
+                                      float* __restrict__ denom, float* __restrict__ lpb, float* __restrict__ lpl,
+                                      int B, int maxT, int maxU) {
+    const long ncells = (long)B * maxT * maxU;
+    for (long cell = (long)blockIdx.x * blockDim.x + threadIdx.x; cell < ncells; cell += (long)gridDim.x * blockDim.x) {
+        int b, t, u;
+        cell_btu(cell, maxT, maxU, b, t, u);
+        const int Tn = clamp_T(xlen[b], maxT), Un = clamp_U(ylen[b], maxU);
+        if (t >= Tn || u >= Un) continue;
+        const int s = bd.s_begin[(long)b * maxT + t];
+        if (bd.nopath[b] || u < s || u >= s + min(bd.R, Un)) {
+            denom[cell] = -INFINITY;
+            lpb[cell] = -INFINITY;
+            lpl[cell] = -INFINITY;
+        }
+    }
+}
+
+// rnnt_grad_kernel (FE = false) on band rows: the row scalars of cell (t, s_begin + r), zero on padding rows
+template <typename TO, bool VEC, int WARPS>
+__global__ void __launch_bounds__(WARPS * 32)
+rnnt_band_grad_kernel(const float* logits, TO* grads, const int* __restrict__ labels,
+                      const int* __restrict__ xlen, const int* __restrict__ ylen, Band bd,
+                      const float* __restrict__ denom, const float* __restrict__ alphas,
+                      const float* __restrict__ betas, const float* __restrict__ ll_fwd,
+                      const float* __restrict__ gscale, int gscale_per_batch, float hscale,
+                      int B, int maxT, int maxU, int V, int blank) {
+    const int lane = threadIdx.x & 31;
+    const long nrows = (long)B * maxT * bd.R;
+    const long wstride = (long)gridDim.x * WARPS;
+    for (long m = (long)blockIdx.x * WARPS + (threadIdx.x >> 5); m < nrows; m += wstride) {
+        int b, t, u, Tn, Un;
+        const float* row = logits + m * (long)V;
+        TO* orow = grads + m * (long)V;
+        if (!band_cell(m, bd, xlen, ylen, maxT, maxU, b, t, u, Tn, Un)) {
+            for (int v = lane * 4; v < V; v += 128) {
+                if (VEC) {
+                    const float z[4] = {0, 0, 0, 0};
+                    Store4<TO>::st(orow + v, z);
+                } else {
+                    for (int i = 0; i < 4 && v + i < V; ++i) orow[v + i] = TO(0.f);
+                }
+            }
+            continue;
+        }
+        const long cell = ((long)b * maxT + t) * maxU + u;
+        const float sc = hscale * (gscale ? gscale[gscale_per_batch ? b : 0] : 1.f);
+        const float a = alphas[cell], bt_ = betas[cell], ll = ll_fwd[b], d = denom[cell];
+        const int lab = (u < Un - 1) ? labels[b * (maxU - 1) + u] : -1;
+        const float c_all = a + bt_ - ll + d;
+        float c_blank = -INFINITY;
+        if (t < Tn - 1) c_blank = a - ll + d + betas[cell + maxU];
+        else if (u == Un - 1) c_blank = a - ll + d;
+        const float c_lab = (lab >= 0) ? a - ll + d + betas[cell + 1] : -INFINITY;
+        for (int v = lane * 4; v < V; v += 128) {
+            float x[4];
+            Row4<float, VEC>::load(row, v, V, x);
+            float g[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                float gr = fast_exp(c_all + x[i]);
+                if (v + i == blank) gr -= expf(c_blank + x[i]);
+                if (v + i == lab) gr -= expf(c_lab + x[i]);
+                g[i] = gr * sc;
+            }
+            if (VEC) {
+                Store4<TO>::st(orow + v, g);
+            } else {
+                for (int i = 0; i < 4 && v + i < V; ++i) orow[v + i] = TO(g[i]);
+            }
+        }
+    }
+}
+
+// rnnt_grad_db_bf16x8_kernel over band rows: the same row scalars (grad_loads / grad_row) and d logits (grad_bf16x8)
+// at the band row's cell, zero on padding rows, and the bias gradient's lane sums over the band rows in eb_colsum's
+// order.  Thread (k, q) walks the rows k, k + COLSUM_LANES, ... for the 8 columns 8q .. 8q+7.
+__global__ void __launch_bounds__(DB_THREADS)
+rnnt_band_grad_db_bf16x8_kernel(const __nv_bfloat16* logits, __nv_bfloat16* grads, const int* __restrict__ labels,
+                                const int* __restrict__ xlen, const int* __restrict__ ylen, Band bd,
+                                const float* __restrict__ denom, const float* __restrict__ alphas,
+                                const float* __restrict__ betas, const float* __restrict__ ll_fwd,
+                                const float* __restrict__ gscale, int gscale_per_batch, float hscale, int B, int maxT,
+                                int maxU, int V, int blank, float* __restrict__ part) {
+    const int V8 = V / 8;
+    const int tid = blockIdx.x * DB_THREADS + threadIdx.x;
+    if (tid >= COLSUM_LANES * V8) return;
+    const int k = tid / V8, v = (tid - k * V8) * 8;
+    const long nrows = (long)B * maxT * bd.R;
+    const FastEmit<float> fe{nullptr, 0.f, 0.f};
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (long m = k; m < nrows; m += COLSUM_LANES) {
+        int b, t, u, Tn, Un;
+        uint4 g = make_uint4(0u, 0u, 0u, 0u);
+        if (band_cell(m, bd, xlen, ylen, maxT, maxU, b, t, u, Tn, Un)) {
+            const long cell = ((long)b * maxT + t) * maxU + u;
+            const GradRow r = grad_row<false>(grad_loads<false>(cell, b, t, u, Tn, Un, labels, denom, alphas, betas,
+                                                                ll_fwd, gscale, gscale_per_batch, maxU, fe),
+                                              t, u, Tn, Un, hscale, fe);
+            g = grad_bf16x8(*reinterpret_cast<const uint4*>(logits + m * (long)V + v), v, r, blank);
+        }
+        *reinterpret_cast<uint4*>(grads + m * (long)V + v) = g;
+        const uint32_t w[4] = {g.x, g.y, g.z, g.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w[j]));
+            acc[2 * j] += f.x;
+            acc[2 * j + 1] += f.y;
+        }
+    }
+    float* o = part + (long)k * V + v;
+    *reinterpret_cast<float4*>(o) = make_float4(acc[0], acc[1], acc[2], acc[3]);
+    *reinterpret_cast<float4*>(o + 4) = make_float4(acc[4], acc[5], acc[6], acc[7]);
+}
+
+// what every band entry checks before it launches anything
+inline bool bad_band(const int* s_begin, const int* nopath, int R) {
+    return !s_begin || !nopath || R < 2 || R > 64;
+}
+
 }  // namespace
 
 // ------------------------------ warp-transducer compatible C ABI ------------------------------
@@ -1107,5 +1288,98 @@ EB_API int eb_rnnt_workspace_views(void* workspace, int B, int maxT, int maxU, i
         Workspace<double> w(workspace, B, maxT, maxU);
         *denom = w.denom; *alphas = w.alphas; *betas = w.betas; *ll_fwd = w.ll_fwd; *ll_bwd = w.ll_bwd;
     }
+    return EB_OK;
+}
+
+EB_API int eb_rnnt_band_loss_fwd(const float* logits, const int* labels, const int* xlen, const int* ylen,
+                                 const int* s_begin, const int* nopath, int B, int maxT, int maxU, int R, int V,
+                                 int blank, void* workspace, float* costs_dev, int need_beta, void* stream) {
+    if (!logits || !workspace || bad_problem(labels, xlen, ylen, B, maxT, maxU, V, blank) ||
+        bad_band(s_begin, nopath, R))
+        return EB_ERR_INVALID;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    Workspace<float> w(workspace, B, maxT, maxU);
+    const Band bd{s_begin, nopath, R};
+    const long nrows = (long)B * maxT * R;
+    constexpr int WARPS = 8;
+    if (V % 4 == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0)
+        rnnt_band_denom_kernel<true, WARPS><<<row_grid(nrows, WARPS), WARPS * 32, 0, st>>>(
+            logits, labels, xlen, ylen, bd, w.denom, w.lpb, w.lpl, B, maxT, maxU, V, blank);
+    else
+        rnnt_band_denom_kernel<false, WARPS><<<row_grid(nrows, WARPS), WARPS * 32, 0, st>>>(
+            logits, labels, xlen, ylen, bd, w.denom, w.lpb, w.lpl, B, maxT, maxU, V, blank);
+    EB_CHECK_LAUNCH();
+    return eb_rnnt_band_lattice(xlen, ylen, s_begin, nopath, B, maxT, maxU, R, workspace, costs_dev, need_beta, stream);
+}
+
+EB_API int eb_rnnt_band_lattice(const int* xlen, const int* ylen, const int* s_begin, const int* nopath, int B,
+                                int maxT, int maxU, int R, void* workspace, float* costs_dev, int need_beta,
+                                void* stream) {
+    if (!xlen || !ylen || !workspace || B <= 0 || maxT <= 0 || maxU <= 0 || maxU > 1024 || bad_band(s_begin, nopath, R))
+        return EB_ERR_INVALID;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    Workspace<float> w(workspace, B, maxT, maxU);
+    const Band bd{s_begin, nopath, R};
+    const long ncells = (long)B * maxT * maxU;
+    rnnt_band_fill_kernel<<<(int)std::min<long>((ncells + 255) / 256, (long)eb_num_sms() * 16), 256, 0, st>>>(
+        xlen, ylen, bd, w.denom, w.lpb, w.lpl, B, maxT, maxU);
+    EB_CHECK_LAUNCH();
+    const int rc = launch_lattice<float>(w, xlen, ylen, B, maxT, maxU, need_beta, st);
+    if (rc) return rc;
+    if (costs_dev) neg_copy_kernel<float><<<(B + 127) / 128, 128, 0, st>>>(w.ll_fwd, costs_dev, B);
+    EB_CHECK_LAUNCH();
+    return EB_OK;
+}
+
+EB_API int eb_rnnt_band_loss_bwd_bf16_db(const void* logits16, void* grads16, const int* labels, const int* xlen,
+                                         const int* ylen, const int* s_begin, const int* nopath, int B, int maxT,
+                                         int maxU, int R, int V, int blank, void* workspace, const float* gscale_dev,
+                                         int gscale_per_batch, double host_scale, float* db_part, float* db_accum,
+                                         void* stream) {
+    if (!logits16 || !grads16 || !workspace || !db_part || !db_accum ||
+        bad_problem(labels, xlen, ylen, B, maxT, maxU, V, blank) || bad_band(s_begin, nopath, R) || V % 8 ||
+        ((reinterpret_cast<uintptr_t>(logits16) | reinterpret_cast<uintptr_t>(grads16) |
+          reinterpret_cast<uintptr_t>(db_part)) & 15))
+        return EB_ERR_INVALID;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    Workspace<float> w(workspace, B, maxT, maxU);
+    const int threads = COLSUM_LANES * (V / 8);
+    rnnt_band_grad_db_bf16x8_kernel<<<(threads + DB_THREADS - 1) / DB_THREADS, DB_THREADS, 0, st>>>(
+        reinterpret_cast<const __nv_bfloat16*>(logits16), reinterpret_cast<__nv_bfloat16*>(grads16), labels, xlen,
+        ylen, Band{s_begin, nopath, R}, w.denom, w.alphas, w.betas, w.ll_fwd, gscale_dev, gscale_per_batch,
+        (float)host_scale, B, maxT, maxU, V, blank, db_part);
+    EB_CHECK_LAUNCH();
+    return colsum_lanes_finish(db_part, db_accum, V, st);
+}
+
+EB_API int eb_rnnt_band_loss_bwd(const float* logits, void* grads, int grads_bf16, const int* labels,
+                                 const int* xlen, const int* ylen, const int* s_begin, const int* nopath, int B,
+                                 int maxT, int maxU, int R, int V, int blank, void* workspace,
+                                 const float* gscale_dev, int gscale_per_batch, double host_scale, void* stream) {
+    if (!logits || !grads || !workspace || bad_problem(labels, xlen, ylen, B, maxT, maxU, V, blank) ||
+        bad_band(s_begin, nopath, R) || (grads_bf16 && (reinterpret_cast<uintptr_t>(grads) & 1)))
+        return EB_ERR_INVALID;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    Workspace<float> w(workspace, B, maxT, maxU);
+    const Band bd{s_begin, nopath, R};
+    const long nrows = (long)B * maxT * R;
+    constexpr int WARPS = 8;
+    const int grid = row_grid(nrows, WARPS);
+    const bool vec = V % 4 == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0 &&
+                     (reinterpret_cast<uintptr_t>(grads) & (grads_bf16 ? 7 : 15)) == 0;
+    auto launch = [&](auto* g, auto vec_on) {
+        using TO = std::remove_pointer_t<decltype(g)>;
+        rnnt_band_grad_kernel<TO, decltype(vec_on)::value, WARPS><<<grid, WARPS * 32, 0, st>>>(
+            logits, g, labels, xlen, ylen, bd, w.denom, w.alphas, w.betas, w.ll_fwd, gscale_dev, gscale_per_batch,
+            (float)host_scale, B, maxT, maxU, V, blank);
+    };
+    if (grads_bf16) {
+        if (vec) launch((__nv_bfloat16*)grads, std::true_type{});
+        else launch((__nv_bfloat16*)grads, std::false_type{});
+    } else {
+        if (vec) launch((float*)grads, std::true_type{});
+        else launch((float*)grads, std::false_type{});
+    }
+    EB_CHECK_LAUNCH();
     return EB_OK;
 }

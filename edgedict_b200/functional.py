@@ -730,13 +730,14 @@ def _joint_pre(h_enc, h_dec, w1, b1, precision):
 JOINT_WGRAD_SIDE = __import__("os").environ.get("EDGEDICT_JOINT_WGRAD_SIDE", "1") != "0"
 
 
-def _joint_bwd(ctx_p, dlog2, hid, he2, hd2, w1, w2, dims, db2=None):
-    """Shared backward of the joint given d logits [N_cells, V] (fp32 or bf16); db2 may already have
-    been accumulated by the fused loss-gradient kernel."""
+def _joint_bwd(ctx_p, dlog2, hid, he2, hd2, w1, w2, dims, db2=None, band=None):
+    """Shared backward of the joint given d logits [N_rows, V] (fp32 or bf16); db2 may already have
+    been accumulated by the fused loss-gradient kernel.  band = (xlen, ylen, s_begin): the rows are the pruned loss's
+    band rows (hid [B, T, R, J]), reduced onto ep / dp by the banded reduction."""
     B, T, U, E, Dd, J, V = dims
     p = ctx_p
     dl16 = dlog2 if dlog2.dtype == bf16 else (ops.cast_bf16(dlog2) if p == "bf16" else None)
-    hid2 = hid.view(B * T * U, J)
+    hid2 = hid.view(-1, J)
 
     def out_layer_grads(db2):
         if db2 is None:
@@ -765,11 +766,17 @@ def _joint_bwd(ctx_p, dlog2, hid, he2, hd2, w1, w2, dims, db2=None):
         dw2, db2 = out_layer_grads(db2)
     if p == "bf16" and J % 8 == 0 and hid.dtype == bf16:
         # tanh' applied in the d-hidden GEMM's epilogue: d(pre-activation) leaves the GEMM, then two pure reductions
-        dpre = ops.gemm_bf16_dtanh(dl16, ops.cast_bf16(w2.contiguous()), True, hid2, B * T * U, J, V)
-        dep, ddp = ops.joint_dpre_reduce(dpre.view(B, T, U, J))
+        dpre = ops.gemm_bf16_dtanh(dl16, ops.cast_bf16(w2.contiguous()), True, hid2, hid2.shape[0], J, V)
+        if band is None:
+            dep, ddp = ops.joint_dpre_reduce(dpre.view(B, T, U, J))
+        else:
+            dep, ddp = ops.joint_band_dpre_reduce(dpre.view(hid.shape), None, *band, U)
     else:
         dhid = ops.mm_nn(dlog2, w2, p, dy16=dl16, out_bf16=(p == "bf16"))
-        dep, ddp = ops.joint_hidden_bwd(dhid.view(B, T, U, J), hid)
+        if band is None:
+            dep, ddp = ops.joint_hidden_bwd(dhid.view(B, T, U, J), hid)
+        else:
+            dep, ddp = ops.joint_band_dpre_reduce(dhid.view(hid.shape), hid, *band, U)
     dep2, ddp2 = dep.view(B * T, J), ddp.view(B * U, J)
     w1e, w1d = w1[:, :E], w1[:, E:]
     dhe = ops.mm_nn(dep2, w1e, p).view(B, T, E)
@@ -991,6 +998,103 @@ class JointLoss(torch.autograd.Function):
                                    fastemit_lambda=lam)
         dhe, dhd, dw1, db1, dw2, db2 = _joint_bwd(p, dl.view(B * T * U, V), hid, he2, hd2, w1, w2, ctx.dims, db2)
         return dhe, dhd, dw1, db1, dw2, db2, None, None, None, None, None, None
+
+
+class SimpleLoss(torch.autograd.Function):
+    """The pruned RNN-T loss's trivial joiner (Kuang et al., Interspeech 2022): am [B, T, V], lm [B, U, V] fp32 ->
+    costs [B] of the RNN-T lattice on log softmax(am[t] + lm[u]), and the loss workspace (alpha, beta, statistics)
+    that the band choice reads (ops.rnnt_band_choice).  The workspace takes no gradient."""
+
+    @staticmethod
+    def forward(ctx, am, lm, labels, act_lens, label_lens, blank):
+        am, lm = _c(am), _c(lm)
+        costs, ws, scratch = ops.rnnt_simple_fwd(am, lm, labels, act_lens, label_lens, blank)
+        ctx.save_for_backward(am, lm, labels, act_lens, label_lens, ws, scratch)
+        ctx.blank = blank
+        ctx.mark_non_differentiable(ws)
+        return costs, ws
+
+    @staticmethod
+    def backward(ctx, gcosts, _gws):
+        am, lm, labels, act_lens, label_lens, ws, scratch = ctx.saved_tensors
+        dam, dlm = ops.rnnt_simple_bwd(am, lm, labels, act_lens, label_lens, ctx.blank, ws, scratch,
+                                       _c(gcosts.to(f32)), 1.0)
+        return dam, dlm, None, None, None, None
+
+
+class RNNTBandLossFn(torch.autograd.Function):
+    """The RNN-T loss restricted to bands: logits [B, T, R, V] fp32 of the band rows given by s_begin / nopath
+    (ops.rnnt_band_choice) -> costs [B]; the cells outside the bands are dead ends of the lattice."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, act_lens, label_lens, s_begin, nopath, U, blank):
+        logits = _c(logits)
+        costs, ws = ops.rnnt_band_loss_fwd(logits, labels, act_lens, label_lens, s_begin, nopath, U, blank)
+        ctx.save_for_backward(logits, labels, act_lens, label_lens, s_begin, nopath, ws)
+        ctx.U, ctx.blank = U, blank
+        return costs
+
+    @staticmethod
+    def backward(ctx, gcosts):
+        logits, labels, act_lens, label_lens, s_begin, nopath, ws = ctx.saved_tensors
+        dl = ops.rnnt_band_loss_bwd(logits, labels, act_lens, label_lens, s_begin, nopath, ctx.U, ctx.blank, ws,
+                                    _c(gcosts.to(f32)), 1.0)
+        return dl, None, None, None, None, None, None, None
+
+
+class PrunedJointLoss(torch.autograd.Function):
+    """JointLoss on the pruned loss's band rows: the joint hidden, logits, statistics and gradient of the B*T*R rows
+    (b, t, r) at cell (t, s_begin[b,t] + r) only.  bf16 mode takes the statistics from the logits GEMM's epilogue and
+    writes the bf16 d logits and the bias gradient in place (JointLoss's fused branch); fp32 mode writes the gradient
+    in place over the fp32 logits.  The backward is _joint_bwd's over the band rows, with the banded reduction."""
+
+    @staticmethod
+    def forward(ctx, h_enc, h_dec, w1, b1, w2, b2, s_begin, nopath, R, labels, act_lens, label_lens, blank, precision):
+        B, T, E = h_enc.shape
+        U, Dd = h_dec.shape[1], h_dec.shape[2]
+        J, V = w1.shape[0], w2.shape[0]
+        if precision == "bf16" and J % 8:
+            raise ValueError("the pruned joint in bf16 mode needs joint_size % 8 == 0, got %d" % J)
+        he2, hd2, ep, dp = _joint_pre(h_enc, h_dec, w1, b1, precision)
+        hid = ops.joint_band_hidden_fwd(ep, dp, act_lens, label_lens, s_begin, R, precision == "bf16")
+        del ep, dp
+        hid2 = hid.view(-1, J)
+        if _fused_lse(precision, J, U) and V % 8 == 0:
+            # bf16 mode: the statistics come out of the logits GEMM's epilogue, as in JointLoss
+            b2a = b2 if (b2.is_contiguous() and b2.data_ptr() % 16 == 0) else b2.clone()
+            logits, costs, ws = ops.joint_band_logits_lse(hid, ops.cast_bf16(w2.contiguous()), b2a, labels, act_lens,
+                                                          label_lens, s_begin, nopath, U, blank)
+        else:
+            logits = ops.mm_nt(hid2, w2, b2, precision, x16=hid2 if precision == "bf16" else None).view(B, T, R, V)
+            costs, ws = ops.rnnt_band_loss_fwd(logits, labels, act_lens, label_lens, s_begin, nopath, U, blank)
+        ctx.save_for_backward(hid, he2, hd2, w1, w2, logits, labels, act_lens, label_lens, s_begin, nopath, ws)
+        ctx.precision, ctx.dims, ctx.blank = precision, (B, T, U, E, Dd, J, V), blank
+        ctx.mark_non_differentiable(costs)
+        return costs.sum().unsqueeze(-1) / B, costs
+
+    @staticmethod
+    def backward(ctx, go, _gc):
+        hid, he2, hd2, w1, w2, logits, labels, act_lens, label_lens, s_begin, nopath, ws = ctx.saved_tensors
+        if getattr(ctx, "consumed", False):
+            raise RuntimeError("PrunedJointLoss.backward ran twice on the same graph: the gradient is written in place "
+                               "over the saved logits (retain_graph is not supported by this node)")
+        ctx.consumed = True
+        B, T, U, E, Dd, J, V = ctx.dims
+        p = ctx.precision
+        g = _c(go.to(f32)).view(-1)
+        db2 = None
+        if logits.dtype == bf16:
+            dl, db2 = ops.rnnt_band_loss_bwd_bf16_db(logits, labels, act_lens, label_lens, s_begin, nopath, U, ctx.blank,
+                                                     ws, g, 1.0 / B)
+        elif p == "bf16":
+            dl = ops.rnnt_band_loss_bwd(logits, labels, act_lens, label_lens, s_begin, nopath, U, ctx.blank, ws, g,
+                                        1.0 / B, out_bf16=True)
+        else:
+            dl = ops.rnnt_band_loss_bwd(logits, labels, act_lens, label_lens, s_begin, nopath, U, ctx.blank, ws, g,
+                                        1.0 / B, out=logits)
+        dhe, dhd, dw1, db1, dw2, db2 = _joint_bwd(p, dl.view(-1, V), hid, he2, hd2, w1, w2, ctx.dims, db2,
+                                                  band=(act_lens, label_lens, s_begin))
+        return dhe, dhd, dw1, db1, dw2, db2, None, None, None, None, None, None, None, None
 
 
 def conv_out_len(T, k, s):

@@ -696,6 +696,126 @@ def rnnt_loss_bwd_bf16_db(logits16, labels, xlen, ylen, blank, ws, gscale, host_
     return logits16, db
 
 
+# ---- pruned RNN-T loss (csrc/pruned.cu, csrc/loss.cu; include/edgedict_b200.h) ----------------------------------
+def rnnt_simple_fwd(am, lm, labels, xlen, ylen, blank):
+    """The trivial joiner's loss: (costs [B], workspace with alpha, beta and the statistics of N(t,u), scratch that
+    rnnt_simple_bwd reads)."""
+    B, T, V = am.shape
+    U = lm.shape[1]
+    ws = rnnt_workspace(B, T, U, f32, am.device)
+    scratch = torch.empty(lib().eb_rnnt_simple_scratch_bytes(B, T, U, V), dtype=torch.uint8, device=am.device)
+    with _timed("rnnt_simple_fwd", 3 + B, 4.0 * (B * T + B * U) * V, 2.0 * B * T * U * V):
+        check(lib().eb_rnnt_simple_stats(_p(am), _p(lm), _p(labels), _p(xlen), _p(ylen), B, T, U, V, blank,
+                                         _p(scratch), _p(ws), _s()), "eb_rnnt_simple_stats")
+    return rnnt_lattice(xlen, ylen, B, T, U, ws), ws, scratch
+
+
+def rnnt_simple_bwd(am, lm, labels, xlen, ylen, blank, ws, scratch, gscale, host_scale):
+    """(d am, d lm) of sum_b gscale[b] * cost_b * host_scale."""
+    B, T, V = am.shape
+    U = lm.shape[1]
+    dam, dlm = torch.empty_like(am), torch.empty_like(lm)
+    per_batch = int(gscale is not None and gscale.numel() > 1)
+    with _timed("rnnt_simple_bwd", 3 + 2 * B, 8.0 * (B * T + B * U) * V, 4.0 * B * T * U * V):
+        check(lib().eb_rnnt_simple_bwd(_p(am), _p(lm), _p(labels), _p(xlen), _p(ylen), B, T, U, V, blank,
+                                       _p(scratch), _p(ws), _p(gscale), per_batch, float(host_scale), _p(dam), _p(dlm),
+                                       _s()), "eb_rnnt_simple_bwd")
+    return dam, dlm
+
+
+def rnnt_band_choice(xlen, ylen, B, T, U, R, ws):
+    """(s_begin [B, T] int32, nopath [B] int32) from a simple-loss workspace."""
+    s_begin = torch.empty(B, T, dtype=torch.int32, device=ws.device)
+    nopath = torch.empty(B, dtype=torch.int32, device=ws.device)
+    with _timed("rnnt_band_choice", 1, 0.0, 0.0):
+        check(lib().eb_rnnt_band_choice(_p(xlen), _p(ylen), B, T, U, R, _p(ws), _p(s_begin), _p(nopath), _s()),
+              "eb_rnnt_band_choice")
+    return s_begin, nopath
+
+
+def joint_band_hidden_fwd(ep, dp, xlen, ylen, s_begin, R, want_bf16):
+    """hidden [B, T, R, J] of the band rows (fp32, or bf16 with want_bf16)."""
+    B, T, J = ep.shape
+    U = dp.shape[1]
+    hid = torch.empty(B, T, R, J, dtype=bf16 if want_bf16 else f32, device=ep.device)
+    check(lib().eb_joint_band_hidden_fwd(_p(ep), _p(dp), _p(xlen), _p(ylen), _p(s_begin), _p(hid), int(want_bf16), B,
+                                         T, U, R, J, _s()), "eb_joint_band_hidden_fwd")
+    return hid
+
+
+def rnnt_band_loss_fwd(logits, labels, xlen, ylen, s_begin, nopath, U, blank, need_beta=True):
+    """logits [B, T, R, V] fp32 of the band rows -> (costs [B], full [B, T, U] loss workspace)."""
+    B, T, R, V = logits.shape
+    ws = rnnt_workspace(B, T, U, f32, logits.device)
+    costs = torch.empty(B, dtype=f32, device=logits.device)
+    with _timed("rnnt_band_loss_fwd", 4, 4.0 * B * T * R * V, 0.0):
+        check(lib().eb_rnnt_band_loss_fwd(_p(logits), _p(labels), _p(xlen), _p(ylen), _p(s_begin), _p(nopath), B, T, U,
+                                          R, V, blank, _p(ws), _p(costs), int(need_beta), _s()), "eb_rnnt_band_loss_fwd")
+    return costs, ws
+
+
+def joint_band_logits_lse(hid16, w2_16, b2, labels, xlen, ylen, s_begin, nopath, U, blank):
+    """bf16 mode: bf16 logits [B, T, R, V] of the band rows hid16 [B, T, R, J] and their statistics from the GEMM's
+    epilogue, then the fill and the lattice: (logits16, costs [B], full [B, T, U] loss workspace)."""
+    B, T, R, J = hid16.shape
+    V = w2_16.shape[0]
+    logits16 = torch.empty(B, T, R, V, dtype=bf16, device=hid16.device)
+    ws = rnnt_workspace(B, T, U, f32, hid16.device)
+    n = B * T * U
+    wsf = ws.view(f32)
+    N = float(B * T * R) * V
+    with _timed("joint_band_logits_lse", 1, 2.0 * B * T * R * J + 2.0 * N, 2.0 * N * J):
+        check(lib().eb_joint_band_logits_lse(_p(hid16), _p(w2_16), _p(b2), _p(logits16), _p(labels), _p(xlen),
+                                             _p(ylen), _p(s_begin), _p(wsf[0:n]), _p(wsf[n:2 * n]),
+                                             _p(wsf[2 * n:3 * n]), B, T, U, R, V, J, blank, _s()),
+              "eb_joint_band_logits_lse")
+    costs = torch.empty(B, dtype=f32, device=hid16.device)
+    with _timed("rnnt_band_lattice", 3, 0.0, 0.0):
+        check(lib().eb_rnnt_band_lattice(_p(xlen), _p(ylen), _p(s_begin), _p(nopath), B, T, U, R, _p(ws), _p(costs), 1,
+                                         _s()), "eb_rnnt_band_lattice")
+    return logits16, costs, ws
+
+
+def rnnt_band_loss_bwd_bf16_db(logits16, labels, xlen, ylen, s_begin, nopath, U, blank, ws, gscale, host_scale):
+    """In place: logits16 [B, T, R, V] becomes the band rows' bf16 d logits; also returns their column sum db [V]."""
+    B, T, R, V = logits16.shape
+    per_batch = int(gscale is not None and gscale.numel() > 1)
+    part = torch.empty(COLSUM_LANES * V, dtype=f32, device=logits16.device)
+    db = torch.zeros(V, dtype=f32, device=logits16.device)
+    with _timed("rnnt_band_loss_bwd", 2, 4.0 * B * T * R * V, 0.0):
+        check(lib().eb_rnnt_band_loss_bwd_bf16_db(_p(logits16), _p(logits16), _p(labels), _p(xlen), _p(ylen),
+                                                  _p(s_begin), _p(nopath), B, T, U, R, V, blank, _p(ws), _p(gscale),
+                                                  per_batch, float(host_scale), _p(part), _p(db), _s()),
+              "eb_rnnt_band_loss_bwd_bf16_db")
+    return logits16, db
+
+
+def rnnt_band_loss_bwd(logits, labels, xlen, ylen, s_begin, nopath, U, blank, ws, gscale, host_scale, out=None,
+                       out_bf16=False):
+    """d loss / d logits of the band rows: fp32 (out may be logits: in place) or bf16 with out_bf16."""
+    B, T, R, V = logits.shape
+    if out is None:
+        out = torch.empty(logits.shape, dtype=bf16 if out_bf16 else f32, device=logits.device)
+    per_batch = int(gscale is not None and gscale.numel() > 1)
+    with _timed("rnnt_band_loss_bwd", 1, float(4 + out.element_size()) * B * T * R * V, 0.0):
+        check(lib().eb_rnnt_band_loss_bwd(_p(logits), _p(out), int(out.dtype == bf16), _p(labels), _p(xlen), _p(ylen),
+                                          _p(s_begin), _p(nopath), B, T, U, R, V, blank, _p(ws), _p(gscale), per_batch,
+                                          float(host_scale), _s()), "eb_rnnt_band_loss_bwd")
+    return out
+
+
+def joint_band_dpre_reduce(dx, hid, xlen, ylen, s_begin, U):
+    """(dep [B, T, J], ddp [B, U, J]) fp32 from the band rows' d hidden dx [B, T, R, J] fp32 with hid fp32, or from
+    the bf16 d(pre-activation) dx with hid None."""
+    B, T, R, J = dx.shape
+    dep = torch.empty(B, T, J, dtype=f32, device=dx.device)
+    ddp = torch.empty(B, U, J, dtype=f32, device=dx.device)
+    with _timed("joint_band_dpre_reduce", 2, 2.0 * dx.numel() * dx.element_size(), 0.0):
+        check(lib().eb_joint_band_dpre_reduce(_p(dx), _p(hid), int(dx.dtype == bf16), _p(xlen), _p(ylen), _p(s_begin),
+                                              _p(dep), _p(ddp), B, T, U, R, J, _s()), "eb_joint_band_dpre_reduce")
+    return dep, ddp
+
+
 # ---- language-model cross-entropy (csrc/lm.cu, csrc/gemm_tc.cu) ---------------------------------------
 def _targets(t):
     _need(t, None, "targets")

@@ -244,7 +244,7 @@ class Transducer(nn.Module):
     def __init__(self, vocab_embed_size, vocab_size, input_size, enc_hidden_size, enc_layers,
                  enc_dropout, enc_proj_size, dec_hidden_size, dec_layers, dec_dropout, dec_proj_size,
                  joint_size, enc_time_reductions=[1], blank=NUL, module_type='LSTM', output_loss=True,
-                 fastemit_lambda=0.0):
+                 fastemit_lambda=0.0, prune_range=None, simple_loss_scale=0.5, pruned_loss_scale=1.0):
         super().__init__()
         self.blank = blank
         if module_type not in ['GRU', 'LSTM']:
@@ -268,6 +268,21 @@ class Transducer(nn.Module):
         # forward, so a trainer can ramp it between steps; not part of the state_dict.  The loss value and last_costs
         # do not depend on it.
         self.fastemit_lambda = Fn.check_fastemit_lambda(fastemit_lambda)
+        # Pruned RNN-T loss (edgedict_b200/pruned.py): with an int prune_range R the model also owns the trivial
+        # joiner's projections, and forward returns simple_loss_scale * mean(simple costs) + pruned_loss_scale *
+        # mean(pruned costs).  The scales are plain attributes read at every forward (a trainer may ramp them);
+        # prune_range=None keeps the modules, state_dict keys and code path of the full loss.
+        self.prune_range = None
+        if prune_range is not None:
+            from ..pruned import check_prune_range
+            self.prune_range = check_prune_range(prune_range)
+            if self.fastemit_lambda > 0:
+                raise ValueError("fastemit_lambda > 0 is not supported together with prune_range")
+            self.simple_am_proj = nn.Linear(enc_proj_size, vocab_size)
+            self.simple_lm_proj = nn.Linear(dec_proj_size, vocab_size)
+            self.simple_loss_scale = simple_loss_scale
+            self.pruned_loss_scale = pruned_loss_scale
+            self.last_simple_costs = None
 
     def set_precision(self, precision):
         return _set_precision(self, precision)
@@ -283,10 +298,36 @@ class Transducer(nn.Module):
         xl = _lens_to_device(_i32(scale_length(h_enc.shape[1], xlen)), h_enc.device)
         yl = _lens_to_device(_i32(ylen), h_enc.device)
         l0, l2 = self.joint.joint[0], self.joint.joint[2]
+        if self.prune_range is not None:
+            return self._pruned_loss(h_enc, h_dec, _i32(ys[:, :int(ylen.max())]), xl, yl, lam)
         loss, costs = Fn.JointLoss.apply(h_enc, h_dec, l0.weight, l0.bias, l2.weight, l2.bias,
                                          _i32(ys[:, :int(ylen.max())]), xl, yl, self.blank, _precision(self), lam)
         self.last_costs = costs
         return loss
+
+    def _pruned_loss(self, h_enc, h_dec, labels, xl, yl, lam):
+        """The simple loss on the trivial joiner, the bands it picks, and the joint + loss on the bands only."""
+        if lam > 0:
+            raise ValueError("fastemit_lambda > 0 is not supported together with prune_range")
+        p = _precision(self)
+        B, T = h_enc.shape[:2]
+        U = h_dec.shape[1]
+        if T > 12288 or U > 1024:
+            raise ValueError("the pruned loss needs T' <= 12288 encoder frames and U + 1 <= 1024, got %d and %d" % (T, U))
+        am = Fn.Linear.apply(h_enc, self.simple_am_proj.weight, self.simple_am_proj.bias, p)
+        lm = Fn.Linear.apply(h_dec, self.simple_lm_proj.weight, self.simple_lm_proj.bias, p)
+        simple_costs, ws = Fn.SimpleLoss.apply(am, lm, labels, xl, yl, self.blank)
+        self.last_simple_costs = simple_costs.detach()
+        loss = float(self.simple_loss_scale) * simple_costs.mean()
+        self.last_costs = None
+        if float(self.pruned_loss_scale) != 0.0:
+            s_begin, nopath = ops.rnnt_band_choice(xl, yl, B, T, U, self.prune_range, ws)
+            l0, l2 = self.joint.joint[0], self.joint.joint[2]
+            pl, costs = Fn.PrunedJointLoss.apply(h_enc, h_dec, l0.weight, l0.bias, l2.weight, l2.bias, s_begin, nopath,
+                                                 self.prune_range, labels, xl, yl, self.blank, p)
+            self.last_costs = costs
+            loss = loss + float(self.pruned_loss_scale) * pl[0]
+        return loss.reshape(1)
 
     def _encode(self, xs, ys, xlen, ylen):
         """The encoder and the prediction network of forward / align on xs[:, :max xlen] and ys[:, :max ylen]."""

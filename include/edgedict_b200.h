@@ -335,6 +335,94 @@ int eb_joint_hidden_bwd(void* dhidden_inout, const void* hidden, int is_bf16, fl
  * J % 8 == 0 and dpre16, dep, ddp 16-byte aligned, else EB_ERR_INVALID */
 int eb_joint_dpre_reduce(const void* dpre16, float* dep, float* ddp, int B, int T, int U, int J, void* stream);
 
+/* ---- pruned RNN-T loss (Kuang et al., Interspeech 2022) ----------------------------------------
+ * Lengths as the RNN-T loss above: utterance b has T_b = min(max(xlen[b], 0), maxT) frames and U_b = min(max(ylen[b],
+ * 0), maxU-1) + 1 symbol positions; 1 <= maxU <= 1024.  R is the prune range, 2 <= R <= 64, and Rb = min(R, U_b).
+ * Every entry below returns EB_ERR_INVALID before any launch for R outside [2, 64], maxU > 1024, a missing pointer or a
+ * misaligned bf16 pointer, and none synchronises with the host.
+ *
+ * Trivial-joiner ("simple") loss on am [B, maxT, V] and lm [B, maxU, V] fp32:
+ *   N(t,u) = log sum_v exp(am[t,v] + lm[u,v]),  lpb = am[t,blank] + lm[u,blank] - N,  lpl = am[t,y_u] + lm[u,y_u] - N.
+ * eb_rnnt_simple_stats writes denom = -N, lpb and lpl of a dtype_size-4 loss workspace (eb_rnnt_workspace_bytes) for
+ * the valid cells; eb_rnnt_loss_lattice on that workspace then gives alpha, beta and the costs.  N is taken in product
+ * form, amax[t] + lmax[u] + log(exp(am - amax) . exp(lm - lmax)^T) with one fp32 GEMM per utterance, and a cell whose
+ * product is below 1e-25 (where terms lost to underflow could matter) is recomputed by a direct log-sum-exp over v in
+ * ascending order, so a finite N never comes out +-inf.  scratch: eb_rnnt_simple_scratch_bytes, filled by
+ * eb_rnnt_simple_stats and read by eb_rnnt_simple_bwd.  eb_rnnt_simple_bwd, from that workspace (need_beta = 1), writes
+ * with occ = exp(alpha + beta - ll), gamma_blank(t,u) = exp(alpha + lpb + beta(t+1,u) - ll) (alpha + lpb - ll at the
+ * final cell) and gamma_emit(t,u) = exp(alpha + lpl + beta(t,u+1) - ll):
+ *   dam[t,v] = sum_u occ * softmax_v(am[t] + lm[u]) - sum_u [v = y_u] gamma_emit - [v = blank] sum_u gamma_blank,
+ *   dlm[u,v] = the same summed over t,
+ * times host_scale * gscale ([1] or [B] with gscale_per_batch, or NULL for 1); zero for t >= T_b, u >= U_b and T_b = 0.
+ * The occupancy terms are exp(am - amax) * (G . exp(lm - lmax)) and exp(lm - lmax) * (G^T . exp(am - amax)) with
+ * G(t,u) = occ exp(amax + lmax - N), two fp32 GEMMs per utterance; the fallback cells' terms are added directly.  Fixed
+ * order, no atomics: the same bits on every run. */
+size_t eb_rnnt_simple_scratch_bytes(int B, int maxT, int maxU, int V);
+int eb_rnnt_simple_stats(const float* am, const float* lm, const int* labels, const int* xlen, const int* ylen, int B,
+                         int maxT, int maxU, int V, int blank, void* scratch, void* workspace, void* stream);
+int eb_rnnt_simple_bwd(const float* am, const float* lm, const int* labels, const int* xlen, const int* ylen, int B,
+                       int maxT, int maxU, int V, int blank, void* scratch, const void* workspace,
+                       const float* gscale_dev, int gscale_per_batch, double host_scale, float* dam, float* dlm,
+                       void* stream);
+/* Band choice from the simple loss's workspace (alpha, beta, ll_fwd), per utterance:
+ *   1. score(t,s) = sum_{u=s}^{s+Rb-1} occ(t,u) in ascending u in fp32, s in [0, U_b - Rb]; s*(t) = its argmax, ties to
+ *      the lowest s;
+ *   2. s[0] = 0, s[t] = min(max(s*(t), s[t-1]), s[t-1] + Rb - 1);
+ *   3. s[T_b-1] = U_b - Rb, then s[t] = max(s[t], s[t+1] - (Rb - 1)) for t = T_b-2 down to 0;
+ *   4. nopath[b] = s[0] > 0 (the bands hold no path: U_b - Rb > (T_b - 1)(Rb - 1));
+ *   5. s_begin[b, t] = s[t] for t < T_b, 0 for t >= T_b.
+ * s_begin [B, maxT] int32, nopath [B] int32; maxT <= 12288. */
+int eb_rnnt_band_choice(const int* xlen, const int* ylen, int B, int maxT, int maxU, int R, const void* workspace,
+                        int* s_begin, int* nopath, void* stream);
+/* Band rows m = (b*maxT + t)*R + r, r < R: row m is cell (t, u = s_begin[b,t] + r) when t < T_b, r < Rb (and, for the
+ * loss entries, nopath[b] = 0), else a padding row.
+ * eb_joint_band_hidden_fwd: hidden[m, :] = tanh(ep[b,t,:] + dp[b,u,:]) ([B*maxT*R, J]; ep [B, maxT, J], dp [B, maxU,
+ *   J] fp32), fp32 with tanhf, or bf16 with tanh.approx (hidden_bf16 = 1, hidden 16-byte aligned); padding rows zero.
+ * eb_rnnt_band_loss_fwd: the statistics of each valid band row of logits [B*maxT*R, V] fp32 (the same per-row
+ *   arithmetic as eb_rnnt_loss_fwd, so a row gets the bits its cell would get there) go to cell (t, u) of a full
+ *   [B, maxT, maxU] fp32 loss workspace; every other valid cell gets denom = lpb = lpl = -inf (all of them when
+ *   nopath[b]), then the lattice of eb_rnnt_loss_lattice runs: costs_dev[b] = -ll (+inf when nopath[b] or T_b = 0).
+ * eb_rnnt_band_loss_bwd: d loss / d logits of the band rows, each row eb_rnnt_loss_bwd's gradient of its cell (lambda
+ *   = 0), fp32 (grads may alias logits) or bf16 (grads_bf16); zero on padding rows. */
+int eb_joint_band_hidden_fwd(const float* ep, const float* dp, const int* xlen, const int* ylen, const int* s_begin,
+                             void* hidden, int hidden_bf16, int B, int maxT, int maxU, int R, int J, void* stream);
+int eb_rnnt_band_loss_fwd(const float* logits, const int* labels, const int* xlen, const int* ylen,
+                          const int* s_begin, const int* nopath, int B, int maxT, int maxU, int R, int V, int blank,
+                          void* workspace, float* costs_dev, int need_beta, void* stream);
+/* eb_rnnt_band_lattice: the -inf fill and the lattice of eb_rnnt_band_loss_fwd alone, for band statistics that
+ *   eb_joint_band_logits_lse wrote.  Run it after them: it also clears the band cells of an utterance with nopath[b].
+ * eb_joint_band_logits_lse: eb_joint_logits_lse's GEMM and statistics epilogue over the band rows of hidden16
+ *   [B*maxT*R, J] (bf16 mode): bf16 logits16 [B*maxT*R, V] and the statistics of each valid band row at its cell, the
+ *   bits eb_joint_logits_lse gives the same row (J % 8 == 0, 16-byte aligned hidden16 / w2_16 / b2).
+ * eb_rnnt_band_loss_bwd_bf16_db: eb_rnnt_loss_bwd_bf16_db (lambda = 0) over the band rows, in place allowed: bf16 d
+ *   logits with the row scalars of the band row's cell, zero on padding rows, and db_accum[c] += their column sum in
+ *   eb_colsum's order (V % 8 == 0, 16-byte aligned pointers; db_part: fp32 scratch of 512 * V).
+ * A band row whose s_begin + r lies outside [0, U_b) is a padding row in every band entry. */
+int eb_rnnt_band_lattice(const int* xlen, const int* ylen, const int* s_begin, const int* nopath, int B, int maxT,
+                         int maxU, int R, void* workspace, float* costs_dev, int need_beta, void* stream);
+int eb_joint_band_logits_lse(const void* hidden16, const void* w2_16, const float* b2, void* logits16,
+                             const int* labels, const int* xlen, const int* ylen, const int* s_begin, float* denom,
+                             float* lpb, float* lpl, int B, int maxT, int maxU, int R, int V, int J, int blank,
+                             void* stream);
+int eb_rnnt_band_loss_bwd_bf16_db(const void* logits16, void* grads16, const int* labels, const int* xlen,
+                                  const int* ylen, const int* s_begin, const int* nopath, int B, int maxT, int maxU,
+                                  int R, int V, int blank, void* workspace, const float* gscale_dev,
+                                  int gscale_per_batch, double host_scale, float* db_part, float* db_accum,
+                                  void* stream);
+int eb_rnnt_band_loss_bwd(const float* logits, void* grads, int grads_bf16, const int* labels, const int* xlen,
+                          const int* ylen, const int* s_begin, const int* nopath, int B, int maxT, int maxU, int R,
+                          int V, int blank, void* workspace, const float* gscale_dev, int gscale_per_batch,
+                          double host_scale, void* stream);
+/* Banded d-pre reduction: dpre = dx * (1 - hidden^2) for fp32 d hidden dx (is_bf16 = 0), or dx itself, the bf16
+ * d(pre-activation) of eb_gemm_bf16_dtanh (is_bf16 = 1, hidden NULL, dx 16-byte aligned), over band rows as above:
+ *   dep[b,t,:] = sum_{r < Rb} dpre[m(b,t,r), :] in ascending r (zero for t >= T_b),
+ *   ddp[b,u,:] = sum over the t < T_b with s_begin[t] <= u < s_begin[t] + Rb, in ascending t, of dpre[m(b,t,u -
+ *                s_begin[t]), :] (zero for u >= U_b).
+ * The bands are monotone, so those t are a contiguous range: one thread sums each output, no atomics. */
+int eb_joint_band_dpre_reduce(const void* dx, const float* hidden, int is_bf16, const int* xlen, const int* ylen,
+                              const int* s_begin, float* dep, float* ddp, int B, int maxT, int maxU, int R, int J,
+                              void* stream);
+
 /* ---- streaming greedy decode: one persistent kernel per audio chunk -----------------------------
  * replaces PytorchStreamDecoder.decode's Python loop (rnnt/stream.py:93-120).  The host builds a
  * phase program once (edgedict_b200/stream_engine.py) and launches it per chunk; see decode.cu. */
