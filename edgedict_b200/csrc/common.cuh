@@ -120,6 +120,13 @@ __device__ __forceinline__ void spin_wait_ge(const unsigned* ctr, unsigned targe
 constexpr int COLSUM_LANES = 512;
 int colsum_lanes_finish(const float* part, float* out, int N, cudaStream_t st);
 
+// The pruned RNN-T loss's padding rule (include/edgedict_b200.h): band row r of frame t, whose band starts at symbol
+// position s, holds cell (t, s + r) when t < T_b, r < min(R, U_b), s >= 0 and s + r < U_b; every other row is padding.
+// A frame with a negative start has no live row.  The loss entries also treat every row of a nopath utterance as padding.
+__device__ __forceinline__ bool band_row_live(int t, int Tn, int Un, int R, int s, int r) {
+    return t < Tn && r < min(R, Un) && s + r < Un && s >= 0;
+}
+
 // exp through ex2.approx.ftz: FMUL + MUFU.  (__expf without -ftz=true is ex2.approx WITHOUT flush-to-zero, which
 // the compiler guards with a range test and two conditional multiplies per call: 3 extra instructions per element
 // in the streaming softmax loops.)  Results below 1.2e-38 flush to zero, irrelevant for softmax sums.

@@ -88,8 +88,8 @@ struct Sched {
 // targets[r], denom[r] receives the row's log-sum-exp and lpl[r] the target's logit (0 for a target outside [0, N),
 // which is never used to index anything).
 // LSE_BAND is LSE_RNNT over the pruned loss's band rows m = (b*maxT + t)*R + r (eb_joint_band_logits_lse): row m holds
-// cell (t, u = s_begin[b*maxT + t] + r), targets = s_begin and targets64 = R; rows with t >= T_b, r >= min(R, U_b) or u
-// outside [0, U_b) write nothing.
+// cell (t, u = s_begin[b*maxT + t] + r), targets = s_begin and targets64 = R; padding rows (band_row_live) write
+// nothing.
 constexpr int LSE_NONE = 0, LSE_RNNT = 1, LSE_ROWS = 2, LSE_BAND = 3;
 struct LseArgs {
     const int* labels; const int* xlen; const int* ylen;     // [B,maxU-1], [B], [B]
@@ -322,8 +322,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
                             const int t = (int)(bt % lse.maxT), b = (int)(bt / lse.maxT);
                             const int Tn = min(max(lse.xlen[b], 0), lse.maxT);
                             const int Un = min(max(lse.ylen[b], 0) + 1, lse.maxU);
-                            const int u = static_cast<const int*>(lse.targets)[bt] + r;
-                            cell_ok[h] = t < Tn && r < min(R, Un) && u >= r && u < Un;
+                            const int s = static_cast<const int*>(lse.targets)[bt], u = s + r;
+                            cell_ok[h] = band_row_live(t, Tn, Un, R, s, r);
                             if (cell_ok[h] && u < Un - 1) lab[h] = lse.labels[b * (lse.maxU - 1) + u];
                         }
                     } else if (cell < M) {

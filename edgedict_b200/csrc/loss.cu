@@ -862,7 +862,7 @@ struct Band {
     int R;
 };
 
-// the cell of band row m, or false for a padding row (t >= T_b, r >= Rb, or an utterance without a band path)
+// the cell of band row m, or false for a padding row (band_row_live, or an utterance without a band path)
 __device__ __forceinline__ bool band_cell(long m, const Band& bd, const int* xlen, const int* ylen, int maxT, int maxU,
                                           int& b, int& t, int& u, int& Tn, int& Un) {
     const int r = (int)(m % bd.R);
@@ -872,8 +872,9 @@ __device__ __forceinline__ bool band_cell(long m, const Band& bd, const int* xle
     Tn = clamp_T(xlen[b], maxT);
     Un = clamp_U(ylen[b], maxU);
     if (t >= Tn || r >= min(bd.R, Un) || bd.nopath[b]) return false;
-    u = bd.s_begin[bt] + r;
-    return u >= r && u < Un;                              // a start outside [0, U_b - r): a padding row
+    const int s = bd.s_begin[bt];
+    u = s + r;
+    return band_row_live(t, Tn, Un, bd.R, s, r);
 }
 
 template <bool VEC, int WARPS>
@@ -900,7 +901,8 @@ rnnt_band_denom_kernel(const float* __restrict__ logits, const int* __restrict__
     }
 }
 
-// -inf statistics for the valid cells outside the band of their frame (all of them when the bands hold no path)
+// -inf statistics for the valid cells that no live band row holds (all of them when the bands hold no path, and every
+// cell of a frame whose start is negative)
 __global__ void rnnt_band_fill_kernel(const int* __restrict__ xlen, const int* __restrict__ ylen, Band bd,
                                       float* __restrict__ denom, float* __restrict__ lpb, float* __restrict__ lpl,
                                       int B, int maxT, int maxU) {
@@ -911,7 +913,7 @@ __global__ void rnnt_band_fill_kernel(const int* __restrict__ xlen, const int* _
         const int Tn = clamp_T(xlen[b], maxT), Un = clamp_U(ylen[b], maxU);
         if (t >= Tn || u >= Un) continue;
         const int s = bd.s_begin[(long)b * maxT + t];
-        if (bd.nopath[b] || u < s || u >= s + min(bd.R, Un)) {
+        if (bd.nopath[b] || u < s || !band_row_live(t, Tn, Un, bd.R, s, u - s)) {
             denom[cell] = -INFINITY;
             lpb[cell] = -INFINITY;
             lpl[cell] = -INFINITY;

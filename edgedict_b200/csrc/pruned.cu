@@ -290,7 +290,7 @@ __global__ void band_choice_kernel(const int* __restrict__ xlen, const int* __re
 }
 
 // ---------------------------------------------------------------------------------------------
-// 4. band hidden rows: one CTA per (b, t), zero rows for t >= T_b and r >= Rb
+// 4. band hidden rows: one CTA per (b, t), zero padding rows (band_row_live)
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ float tanh_fast(float x) {     // MUFU.TANH, as eb_joint_hidden_fwd's bf16 kernel
     float y;
@@ -306,17 +306,17 @@ __global__ void band_hidden_kernel(const float* __restrict__ ep, const float* __
     const long bt = blockIdx.x;
     const int t = (int)(bt % maxT), b = (int)(bt / maxT);
     const int Tn = clamp_T(xlen[b], maxT), Un = clamp_U(ylen[b], maxU);
-    const int Rb = t < Tn ? min(R, Un) : 0;
     const int s = s_begin[bt];
     const float* e = ep + bt * J;
-    const float* d = dp + ((long)b * maxU + s) * J;
+    const float* d = dp + (long)b * maxU * J;
     for (int i = threadIdx.x; i < R * J; i += blockDim.x) {
         const int r = i / J, j = i - r * J;
+        const bool live = band_row_live(t, Tn, Un, R, s, r);
         if (BF16) {
             reinterpret_cast<__nv_bfloat16*>(hid)[bt * R * J + i] =
-                __float2bfloat16_rn(r < Rb ? tanh_fast(e[j] + d[(long)r * J + j]) : 0.f);
+                __float2bfloat16_rn(live ? tanh_fast(e[j] + d[(long)(s + r) * J + j]) : 0.f);
         } else {
-            reinterpret_cast<float*>(hid)[bt * R * J + i] = r < Rb ? tanhf(e[j] + d[(long)r * J + j]) : 0.f;
+            reinterpret_cast<float*>(hid)[bt * R * J + i] = live ? tanhf(e[j] + d[(long)(s + r) * J + j]) : 0.f;
         }
     }
 }
@@ -332,24 +332,27 @@ __device__ __forceinline__ float dpre_at(const void* dx, const float* h, long i)
     return reinterpret_cast<const float*>(dx)[i] * (1.f - hv * hv);
 }
 
-// dep[b,t,:] = sum_{r < Rb} dpre[b,t,r,:] in ascending r; one CTA per (b, t)
+// dep[b,t,:] = sum over the live rows r of dpre[b,t,r,:] in ascending r; one CTA per (b, t)
 template <bool BF16>
 __global__ void band_dep_kernel(const void* __restrict__ dx, const float* __restrict__ h,
                                 const int* __restrict__ xlen, const int* __restrict__ ylen,
-                                float* __restrict__ dep, int maxT, int maxU, int R, int J) {
+                                const int* __restrict__ s_begin, float* __restrict__ dep, int maxT, int maxU, int R,
+                                int J) {
     const long bt = blockIdx.x;
     const int t = (int)(bt % maxT), b = (int)(bt / maxT);
     const int Tn = clamp_T(xlen[b], maxT), Un = clamp_U(ylen[b], maxU);
-    const int Rb = t < Tn ? min(R, Un) : 0;
+    const int s = s_begin[bt];
     for (int j = threadIdx.x; j < J; j += blockDim.x) {
         float acc = 0.f;
-        for (int r = 0; r < Rb; ++r) acc += dpre_at<BF16>(dx, h, (bt * R + r) * J + j);
+        for (int r = 0; r < R; ++r)
+            if (band_row_live(t, Tn, Un, R, s, r)) acc += dpre_at<BF16>(dx, h, (bt * R + r) * J + j);
         dep[bt * J + j] = acc;
     }
 }
 
 // ddp[b,u,:] = sum over the frames t whose band covers u, in ascending t, of dpre[b,t,u - s_begin[t],:]; one CTA per
-// (b, u).  {t : s[t] <= u < s[t] + Rb} = [first t with s[t] > u - Rb, first t with s[t] > u): two binary searches.
+// (b, u).  With s[t] non-decreasing over t < T_b, {t : s[t] <= u < s[t] + Rb} = [first t with s[t] > u - Rb, first t
+// with s[t] > u): two binary searches.  A frame with a negative start has no live row and adds nothing.
 template <bool BF16>
 __global__ void band_ddp_kernel(const void* __restrict__ dx, const float* __restrict__ h,
                                 const int* __restrict__ xlen, const int* __restrict__ ylen,
@@ -371,7 +374,9 @@ __global__ void band_ddp_kernel(const void* __restrict__ dx, const float* __rest
     const int t0 = u < Un ? first_above(u - Rb) : 0, t1 = u < Un ? first_above(u) : 0;
     for (int j = threadIdx.x; j < J; j += blockDim.x) {
         float acc = 0.f;
-        for (int t = t0; t < t1; ++t) acc += dpre_at<BF16>(dx, h, ((((long)b * maxT + t) * R) + u - s[t]) * J + j);
+        for (int t = t0; t < t1; ++t)
+            if (band_row_live(t, Tn, Un, R, s[t], u - s[t]))
+                acc += dpre_at<BF16>(dx, h, ((((long)b * maxT + t) * R) + u - s[t]) * J + j);
         ddp[bu * J + j] = acc;
     }
 }
@@ -477,11 +482,13 @@ EB_API int eb_joint_band_dpre_reduce(const void* dx, const float* hidden, int is
         bad_R(R) || J <= 0 || (is_bf16 && (reinterpret_cast<uintptr_t>(dx) & 15)))
         return EB_ERR_INVALID;
     if (is_bf16) {
-        band_dep_kernel<true><<<B * maxT, 256, 0, ST(stream)>>>(dx, nullptr, xlen, ylen, dep, maxT, maxU, R, J);
+        band_dep_kernel<true><<<B * maxT, 256, 0, ST(stream)>>>(dx, nullptr, xlen, ylen, s_begin, dep, maxT, maxU, R,
+                                                              J);
         band_ddp_kernel<true><<<B * maxU, 256, 0, ST(stream)>>>(dx, nullptr, xlen, ylen, s_begin, ddp, maxT, maxU, R,
                                                                 J);
     } else {
-        band_dep_kernel<false><<<B * maxT, 256, 0, ST(stream)>>>(dx, hidden, xlen, ylen, dep, maxT, maxU, R, J);
+        band_dep_kernel<false><<<B * maxT, 256, 0, ST(stream)>>>(dx, hidden, xlen, ylen, s_begin, dep, maxT, maxU, R,
+                                                               J);
         band_ddp_kernel<false><<<B * maxU, 256, 0, ST(stream)>>>(dx, hidden, xlen, ylen, s_begin, ddp, maxT, maxU, R,
                                                                  J);
     }

@@ -374,8 +374,9 @@ int eb_rnnt_simple_bwd(const float* am, const float* lm, const int* labels, cons
  * s_begin [B, maxT] int32, nopath [B] int32; maxT <= 12288. */
 int eb_rnnt_band_choice(const int* xlen, const int* ylen, int B, int maxT, int maxU, int R, const void* workspace,
                         int* s_begin, int* nopath, void* stream);
-/* Band rows m = (b*maxT + t)*R + r, r < R: row m is cell (t, u = s_begin[b,t] + r) when t < T_b, r < Rb (and, for the
- * loss entries, nopath[b] = 0), else a padding row.
+/* Band rows m = (b*maxT + t)*R + r, r < R: row m is cell (t, u = s_begin[b,t] + r) when t < T_b, r < Rb, s_begin[b,t]
+ * >= 0 and u < U_b (and, for the loss entries, nopath[b] = 0), else a padding row.  So every row of a frame with a
+ * negative start is padding, and so is each row past U_b; eb_rnnt_band_choice only writes starts in [0, U_b - Rb].
  * eb_joint_band_hidden_fwd: hidden[m, :] = tanh(ep[b,t,:] + dp[b,u,:]) ([B*maxT*R, J]; ep [B, maxT, J], dp [B, maxU,
  *   J] fp32), fp32 with tanhf, or bf16 with tanh.approx (hidden_bf16 = 1, hidden 16-byte aligned); padding rows zero.
  * eb_rnnt_band_loss_fwd: the statistics of each valid band row of logits [B*maxT*R, V] fp32 (the same per-row
@@ -397,7 +398,7 @@ int eb_rnnt_band_loss_fwd(const float* logits, const int* labels, const int* xle
  * eb_rnnt_band_loss_bwd_bf16_db: eb_rnnt_loss_bwd_bf16_db (lambda = 0) over the band rows, in place allowed: bf16 d
  *   logits with the row scalars of the band row's cell, zero on padding rows, and db_accum[c] += their column sum in
  *   eb_colsum's order (V % 8 == 0, 16-byte aligned pointers; db_part: fp32 scratch of 512 * V).
- * A band row whose s_begin + r lies outside [0, U_b) is a padding row in every band entry. */
+ * Every band entry follows the padding rule above; a valid cell that no live row holds gets -inf statistics. */
 int eb_rnnt_band_lattice(const int* xlen, const int* ylen, const int* s_begin, const int* nopath, int B, int maxT,
                          int maxU, int R, void* workspace, float* costs_dev, int need_beta, void* stream);
 int eb_joint_band_logits_lse(const void* hidden16, const void* w2_16, const float* b2, void* logits16,
@@ -417,8 +418,10 @@ int eb_rnnt_band_loss_bwd(const float* logits, void* grads, int grads_bf16, cons
  * d(pre-activation) of eb_gemm_bf16_dtanh (is_bf16 = 1, hidden NULL, dx 16-byte aligned), over band rows as above:
  *   dep[b,t,:] = sum_{r < Rb} dpre[m(b,t,r), :] in ascending r (zero for t >= T_b),
  *   ddp[b,u,:] = sum over the t < T_b with s_begin[t] <= u < s_begin[t] + Rb, in ascending t, of dpre[m(b,t,u -
- *                s_begin[t]), :] (zero for u >= U_b).
- * The bands are monotone, so those t are a contiguous range: one thread sums each output, no atomics. */
+ *                s_begin[t]), :] (zero for u >= U_b),
+ * each over the live rows only (padding rows are skipped, whatever dx holds there).  Precondition: s_begin[b, t] is
+ * non-decreasing over t < T_b (as eb_rnnt_band_choice writes it), so those t are a contiguous range found by binary
+ * search: one thread sums each output, no atomics.  It is not checked (that would need a device sync). */
 int eb_joint_band_dpre_reduce(const void* dx, const float* hidden, int is_bf16, const int* xlen, const int* ylen,
                               const int* s_begin, float* dep, float* ddp, int B, int maxT, int maxU, int R, int J,
                               void* stream);

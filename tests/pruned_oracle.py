@@ -92,9 +92,15 @@ def band_rule(occ, Tn, Un, R):
     return s, s[0] > 0
 
 
+def live(s, r, Un):
+    """The padding rule for row r < min(R, U_b) of a frame t < T_b that starts at s: it holds cell s + r when s >= 0 and
+    s + r < U_b (a frame with a negative start has no live row)."""
+    return s >= 0 and s + r < Un
+
+
 def pruned_costs(band_logits, labels, xlen, ylen, s_begin, U, blank):
-    """Costs [B] of the RNN-T loss on band rows [B, T, R, V]: cell (t, s_begin[b][t] + r) for r < Rb, every other cell
-    -inf; +inf when the bands hold no path."""
+    """Costs [B] of the RNN-T loss on band rows [B, T, R, V]: cell (t, s_begin[b][t] + r) for the live rows r < Rb,
+    every other cell -inf; +inf when the bands hold no path."""
     B, T, R, V = band_logits.shape
     out = []
     for b in range(B):
@@ -109,6 +115,8 @@ def pruned_costs(band_logits, labels, xlen, ylen, s_begin, U, blank):
         for t in range(Tn):
             for r in range(Rb):
                 u = int(s_begin[b][t]) + r
+                if not live(int(s_begin[b][t]), r, Un):
+                    continue
                 lpb[t][u] = logp[t, r, blank]
                 if u < Un - 1:
                     lpl[t][u] = logp[t, r, labels[b][u]]
@@ -144,6 +152,8 @@ def band_reduce(dpre, s_begin, xlen, ylen, U):
         Rb = min(R, Un)
         for t in range(Tn):
             for r in range(Rb):
+                if not live(int(s_begin[b][t]), r, Un):
+                    continue
                 dep[b, t] += dpre[b, t, r]
                 ddp[b, int(s_begin[b][t]) + r] += dpre[b, t, r]
     return dep, ddp
