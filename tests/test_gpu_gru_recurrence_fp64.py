@@ -119,10 +119,11 @@ def hprev_of(y, h0):
     return torch.cat([first, y[:, :-1]], 1)
 
 
-def fwd_ref(xg, w, bhn, hin, hst=None, kernel="seq", u_acc=U24, eps=EPS_LIBM):
+def fwd_ref(xg, w, bhn, hin, hst=None, kernel="seq", u_acc=U24, eps=EPS_LIBM, dxg=0.0):
     """Teacher-forced forward, every step at once: xg [B,T,3H], w [3H,H] (the values the kernel multiplies), bhn [H],
-    hin [B,T,H] the h_{t-1} the kernel multiplied, hst the h_{t-1} of its update (default: hin).  Returns
-    {name: (value, bar)} for r, z, n, gh_n and y [B,T,H]."""
+    hin [B,T,H] the h_{t-1} the kernel multiplied, hst the h_{t-1} of its update (default: hin).  dxg [B,T,3H] is a
+    bar the xg input already carries (0 when xg is the kernel's own input).  Returns {name: (value, bar)} for r, z, n,
+    gh_n and y [B,T,H]."""
     hst = hin if hst is None else hst
     xg, w, bhn, hin, hst = (a.to(f64) for a in (xg, w, bhn, hin, hst))
     B, T, H3 = xg.shape
@@ -132,11 +133,12 @@ def fwd_ref(xg, w, bhn, hin, hst=None, kernel="seq", u_acc=U24, eps=EPS_LIBM):
     xr, xz, xn = xg.view(B, T, 3, H).unbind(2)
     sr, sz, sn = s.view(B, T, 3, H).unbind(2)
     dsr, dsz, dsn = ds.view(B, T, 3, H).unbind(2)
+    dxr, dxz, dxn = dxg.to(f64).view(B, T, 3, H).unbind(2) if torch.is_tensor(dxg) else (dxg,) * 3
     out = {}
     gates = {}
-    for name, x, sv, dv in (("r", xr, sr, dsr), ("z", xz, sz, dsz)):
+    for name, x, sv, dv, dx in (("r", xr, sr, dsr, dxr), ("z", xz, sz, dsz, dxz)):
         pre = x + sv
-        dpre = dv + U24 * (sv.abs() + x.abs())
+        dpre = dv + dx + U24 * (sv.abs() + x.abs())
         g = torch.sigmoid(pre)
         gates[name] = g
         out[name] = (g, g * (1 - g) * dpre + eps + U24 * g)
@@ -146,7 +148,7 @@ def fwd_ref(xg, w, bhn, hin, hst=None, kernel="seq", u_acc=U24, eps=EPS_LIBM):
     dghn = dsn + U24 * ghn.abs()
     out["ghn"] = (ghn, dghn)
     a = xn + r * ghn
-    da = dr * ghn.abs() + r * dghn + 2 * U24 * ((r * ghn).abs() + a.abs())
+    da = dxn + dr * ghn.abs() + r * dghn + 2 * U24 * ((r * ghn).abs() + a.abs())
     n = torch.tanh(a)
     dn = (1 - n * n) * da + eps + U24 * n.abs()
     out["n"] = (n, dn)
