@@ -27,13 +27,16 @@
 //           beam to its best slot when a stored suffix would outgrow its capacity (or on a flush)
 //   GRU     one nn.GRU cell step for S streams (ResLayerNormGRU, models.py:77-116): CTCEncoder's streaming encoder
 //   CTC_EMIT per stream: log-softmax, argmax, repeats (carried across chunks) and blanks dropped (CTCEncoder.greedy_decode)
+//   FE_*    the feature transform of a chunk of raw audio (framing, direct-DFT product, power, mel / DCT products, MFCC
+//           log, log / mask / deltas / stacking into the encoder input), a front-end program run by a GATHER with flags
+//           1024 at the head of the chunk program, bit for bit build_batch_transform's features of each stream's window
 //
 // LINEAR's x1 row divisor (x1_div) lets the W rows of one utterance's beam share its encoder frame without copies.
 // fp32-accurate arithmetic throughout: the north star asks for token-for-token identical greedy output, which
 // bf16 (or plain tf32) near-ties would break.  The matrix products run on the tensor cores as 3xTF32 split
 // products with fp32 accumulation (see tile_mma); everything else is fp32 CUDA-core code.
 #include <cooperative_groups.h>
-#include "common.cuh"
+#include "frontend.cuh"
 #include "../../include/edgedict_b200.h"
 
 namespace {
@@ -475,6 +478,150 @@ __device__ __noinline__ void phase_ctc_emit(const EbPhase& p) {
     }
 }
 
+// ---- front end: the feature transform of a streaming chunk of raw audio, at the head of the chunk program.  Each value
+// is computed by frontend.cuh's expression for it, and the products keep eb_gemm_f32's order, so the model input equals
+// bit for bit what build_batch_transform's module (ops.fe_batch) gives each stream's window.  Field use:
+//   FE_FRAME  S streams of N samples (x1 [S, N]; x2, optional, the dither noise [S, N]; fuse = {dither, preemph}):
+//             y [S, ldy] = the dithered fl(x + fl(dither * noise)), pre-emphasised (flags 1) and reflect-padded by K1
+//             samples, zero past N + 2 K1;
+//   FE_GEMM   y [S, N] (ldy) = A [S, K1] B [K1, N], A(m, k) = x1[(m / aux) ldx1 + (m % aux) ldx2 + k] (aux rows per
+//             group: the strided frames of a padded signal, or plain rows), B(k, n) = w1[k ldw1 + n]; per output the
+//             k-ascending fmaf chain from 0.f over K1 rounded up to a multiple of 16 with zero operands (sgemm_kernel's);
+//   FE_POWER  y [S, N] = |X|^2 of the rows x1 [S, 2N] = [re | im];
+//   FE_LOG    y [S*N] = log(x1 + 1e-6) (MFCC's log of the mel power, in place allowed);
+//   FE_FINISH S streams of K1 per-frame rows x1 [S*K1, N] -> y [S, aux2, W] (ldy = aux2 * W, W = N (3 with flags 2)
+//             aux): stacks of aux frames, with the log (flags 1) and deltas (flags 2); hist_ld = F frames, hist_col =
+//             Fs frames kept, x1_div = the frame the seq_len mask starts at.
+// They are not phases of the kernel's loop but of a front-end program that the GATHER opening a chunk program runs
+// (flags 1024, fe_program).
+constexpr int FE_BM = 64, FE_BN = 64, FE_BK = 16, FE_LD = FE_BM + 4;
+static_assert(2 * FE_BK * FE_LD <= RED_FLOATS + TR * OUT_LD, "front-end product tiles");
+
+__device__ __forceinline__ void fe_gemm(const EbPhase& p, float* sm) {
+    float* As = sm;                                          // [FE_BK][FE_LD]: As[k][m]
+    float* Bs = sm + FE_BK * FE_LD;                          // [FE_BK][FE_LD]: Bs[k][n]
+    const int M = p.S, N = p.N, K = p.K1, tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
+    const int ntn = (N + FE_BN - 1) / FE_BN, ntiles = ((M + FE_BM - 1) / FE_BM) * ntn;
+    const int ak = tid & 15, bk = tid >> 6, bn = tid & 63;   // A: 4 rows (tid / 16 + 16 r) at k ak; B: 4 k at col bn
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const int m0 = (tile / ntn) * FE_BM, n0 = (tile % ntn) * FE_BN;
+        const float* arow[4];
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            const int m = m0 + ty + 16 * r;
+            arow[r] = m < M ? p.x1 + (long)(m / p.aux) * p.ldx1 + (long)(m % p.aux) * p.ldx2 : nullptr;
+        }
+        const bool bcol = n0 + bn < N;
+        float ra[4], rb[4];
+        auto fetch = [&](int k0) {
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                ra[r] = arow[r] && k0 + ak < K ? __ldcg(arow[r] + k0 + ak) : 0.f;
+                const int k = k0 + bk + 4 * r;
+                rb[r] = bcol && k < K ? __ldg(p.w1 + (long)k * p.ldw1 + n0 + bn) : 0.f;
+            }
+        };
+        float acc[4][4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+        fetch(0);
+        for (int k0 = 0; k0 < K; k0 += FE_BK) {
+            __syncthreads();                                 // the previous step's readers are done with the tiles
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                As[ak * FE_LD + ty + 16 * r] = ra[r];
+                Bs[(bk + 4 * r) * FE_LD + bn] = rb[r];
+            }
+            __syncthreads();
+            if (k0 + FE_BK < K) fetch(k0 + FE_BK);
+#pragma unroll
+            for (int k = 0; k < FE_BK; ++k) {
+                const float4 a4 = *reinterpret_cast<const float4*>(As + k * FE_LD + ty * 4);
+                const float4 b4 = *reinterpret_cast<const float4*>(Bs + k * FE_LD + tx * 4);
+                const float a[4] = {a4.x, a4.y, a4.z, a4.w}, b[4] = {b4.x, b4.y, b4.z, b4.w};
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int m = m0 + ty * 4 + i;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int n = n0 + tx * 4 + j;
+                if (m < M && n < N) p.y[(long)m * p.ldy + n] = acc[i][j];
+            }
+        }
+    }
+}
+
+__device__ __forceinline__ void phase_fe(const EbPhase& p, float* sm) {
+    const long gtid = (long)blockIdx.x * blockDim.x + threadIdx.x, gn = (long)gridDim.x * blockDim.x;
+    switch (p.type) {
+        case EB_PH_FE_FRAME: {
+            const int L = p.N, pad = p.K1;
+            const long Lp = p.ldy;
+            const float dither = __ldg(p.fuse), preemph = __ldg(p.fuse + 1);
+            for (long k = gtid; k < (long)p.S * Lp; k += gn) {
+                const long s = k / Lp, i = k % Lp;
+                const float* x = p.x1 + s * L;
+                const float* nz = p.x2 ? p.x2 + s * L : nullptr;
+                // FilterbankFeatures._batch: x + dither * randn_like(x), two roundings (torch's mul, then its add)
+                auto sample = [&](long r) {
+                    return nz ? __fadd_rn(__ldg(x + r), __fmul_rn(dither, __ldg(nz + r))) : __ldg(x + r);
+                };
+                p.y[k] = fe_framed_sample(sample, i, L, pad, preemph, p.flags & 1);
+            }
+        } break;
+        case EB_PH_FE_GEMM: fe_gemm(p, sm); break;
+        case EB_PH_FE_POWER:
+            for (long k = gtid; k < (long)p.S * p.N; k += gn) {
+                const long g = k / p.N;
+                const int b = (int)(k % p.N);
+                p.y[k] = fe_power_value(__ldcg(p.x1 + g * 2 * p.N + b), __ldcg(p.x1 + g * 2 * p.N + p.N + b));
+            }
+            break;
+        case EB_PH_FE_LOG:
+            for (long k = gtid; k < (long)p.S * p.N; k += gn) p.y[k] = fe_log_value(__ldcg(p.x1 + k), 1e-6f);
+            break;
+        case EB_PH_FE_FINISH: {
+            const int C = p.N, n_frame = p.aux, Tout = p.aux2, take_log = p.flags & 1, delta = (p.flags >> 1) & 1;
+            const int W = (delta ? 3 * C : C) * n_frame;
+            for (long k = gtid; k < (long)p.S * Tout * W; k += gn) {
+                const long s = k / ((long)Tout * W), i = k % ((long)Tout * W);
+                const float* rows = p.x1 + s * p.K1 * C;
+                p.y[k] = fe_finish_value([&](long e) { return __ldcg(rows + e); }, (int)(i / W), (int)(i % W),
+                                         p.hist_ld, p.hist_col, p.x1_div, C, n_frame, take_log, delta);
+            }
+        } break;
+        default: break;
+    }
+}
+
+// The front-end program of a chunk (K1 phases at x1), run by the GATHER with flags 1024 that opens the chunk program:
+// each phase is closed by a grid barrier on the counter tok_out (the entry zeroes it at every launch), the last one
+// included.  Run from inside the __noinline__ GATHER, the front end leaves the phase loop's code as it was: any new call
+// site or phase case in the loop, whose matrix phases are compiled at the register cap, costs 4 - 40 more bytes of
+// spills in some of the kernel's instantiations.
+__device__ __forceinline__ void fe_program(const EbPhase& head) {
+    extern __shared__ __align__(16) float dsm[];
+    __shared__ EbPhase ph;
+    const EbPhase* prog = reinterpret_cast<const EbPhase*>(head.x1);
+    unsigned* bar = reinterpret_cast<unsigned*>(head.tok_out);
+    for (int i = 0; i < head.K1; ++i) {
+        __syncthreads();
+        if (threadIdx.x < sizeof(EbPhase) / 4)
+            reinterpret_cast<int*>(&ph)[threadIdx.x] = reinterpret_cast<const int*>(prog + i)[threadIdx.x];
+        __syncthreads();
+        phase_fe(ph, dsm);
+        grid_sync(bar, (unsigned)(i + 1) * gridDim.x);
+    }
+}
+
 // ---- beam search: B utterances x W slots, row r = b*W + slot, T' = hist_ld frames.  Field use:
 //   BEAM_SELECT (S = B, aux = W, N = V, aux2 = blank, hist_col = t, flags 16 = merge): x1 logits [B*W, V] (ldx1);
 //     y slot log p [B*W] (in/out, dead slots -inf); tok_in frames [B]; tok_out token per row (blank for dead and
@@ -886,6 +1033,10 @@ __device__ __noinline__ void phase_beam_select(const EbPhase& p, float* sm) {
 }
 
 __device__ __noinline__ void phase_gather(const EbPhase& p) {
+    if (p.flags & 1024) {                                    // a chunk's front end: no gather
+        fe_program(p);
+        return;
+    }
     const long gtid = (long)blockIdx.x * blockDim.x + threadIdx.x, gn = (long)gridDim.x * blockDim.x;
     const int S = p.S, N = p.N;
     for (long e = gtid; e < (long)p.aux * S * N; e += gn) {
@@ -1424,7 +1575,7 @@ template <bool CTC, bool CTC_STREAM, bool GRU_RNNT, bool CTC_STREAM_BEAM = false
 int decode_run(const void* phases_dev, int nphase, void* barrier_dev, int max_ctas, void* stream) {
     if (!phases_dev || nphase <= 0 || !barrier_dev) return EB_ERR_INVALID;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    EB_CUDA(cudaMemsetAsync(barrier_dev, 0, 4, st));
+    EB_CUDA(cudaMemsetAsync(barrier_dev, 0, 8, st));        // the phase loop's barrier counter and fe_program's
     int grid = eb_num_sms();
     if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
     const EbPhase* prog = reinterpret_cast<const EbPhase*>(phases_dev);

@@ -21,7 +21,7 @@
 // computes CatDeltas (rnnt/transforms.py:10-16: torchaudio compute_deltas twice, window 5, replicate edge at F_b - 1)
 // and writes [static | d1 | d2] per stacked frame, the channel order Downsample's reshape gives.  The MFCC path adds
 // fe_log (log(mel + 1e-6)) and one more eb_gemm_f32 against the orthonormal DCT-II matrix before K3.
-#include "common.cuh"
+#include "frontend.cuh"
 #include "../../include/edgedict_b200.h"
 
 namespace {
@@ -33,16 +33,8 @@ __global__ void fe_preemph_pad_kernel(const float* __restrict__ x, const int* __
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= Lp) return;
     const int Lb = lens ? lens[b] : L;
-    float v = 0.f;
-    if (i < (long)Lb + 2 * pad) {
-        long r = i - pad;                               // reflect (no edge repeat): -1 -> 1, L -> L-2
-        if (r < 0) r = -r;
-        if (r >= Lb) r = 2L * (Lb - 1) - r;
-        const float* row = x + (long)b * L;
-        v = row[r];
-        if (use_preemph && r > 0) v -= preemph * row[r - 1];
-    }
-    xp[(long)b * Lp + i] = v;
+    const float* row = x + (long)b * L;
+    xp[(long)b * Lp + i] = fe_framed_sample([&](long r) { return row[r]; }, i, Lb, pad, preemph, use_preemph);
 }
 
 __global__ void fe_power_kernel(const float* __restrict__ spec, float* __restrict__ pw, long rows, int NB) {
@@ -50,35 +42,7 @@ __global__ void fe_power_kernel(const float* __restrict__ spec, float* __restric
     if (i >= rows * NB) return;
     const long g = i / NB;
     const int k = (int)(i % NB);
-    const float re = spec[g * 2 * NB + k], im = spec[g * 2 * NB + NB + k];
-    pw[i] = re * re + im * im;
-}
-
-// Static feature of frame f (< F), channel c: the optional log(x + 1e-20) of features.py:155-156, zero from frame `seq`
-// on (features.py:160-164; seq = F when there is no mask).
-__device__ __forceinline__ float fe_static(const float* __restrict__ rows, int f, int c, int C, int seq, int take_log) {
-    if (f >= seq) return 0.f;
-    const float v = rows[(long)f * C + c];
-    return take_log ? logf(v + 1e-20f) : v;
-}
-
-__device__ __forceinline__ int fe_clamp(int f, int F) { return f < 0 ? 0 : (f >= F ? F - 1 : f); }
-
-// torchaudio compute_deltas (window 5, replicate padding): d[f] = sum_{k=-2..2} k x[clamp(f+k, 0, F-1)] / 10
-__device__ float fe_delta1(const float* __restrict__ rows, int f, int c, int C, int seq, int F, int take_log) {
-    const float m2 = fe_static(rows, fe_clamp(f - 2, F), c, C, seq, take_log);
-    const float m1 = fe_static(rows, fe_clamp(f - 1, F), c, C, seq, take_log);
-    const float p1 = fe_static(rows, fe_clamp(f + 1, F), c, C, seq, take_log);
-    const float p2 = fe_static(rows, fe_clamp(f + 2, F), c, C, seq, take_log);
-    return (2.f * (p2 - m2) + (p1 - m1)) / 10.f;
-}
-
-__device__ float fe_delta2(const float* __restrict__ rows, int f, int c, int C, int seq, int F, int take_log) {
-    const float m2 = fe_delta1(rows, fe_clamp(f - 2, F), c, C, seq, F, take_log);
-    const float m1 = fe_delta1(rows, fe_clamp(f - 1, F), c, C, seq, F, take_log);
-    const float p1 = fe_delta1(rows, fe_clamp(f + 1, F), c, C, seq, F, take_log);
-    const float p2 = fe_delta1(rows, fe_clamp(f + 2, F), c, C, seq, F, take_log);
-    return (2.f * (p2 - m2) + (p1 - m1)) / 10.f;
+    pw[i] = fe_power_value(spec[g * 2 * NB + k], spec[g * 2 * NB + NB + k]);
 }
 
 // feat [B*R, C] per-frame rows -> out[b, t, s*Cd + j*C + c] (Cd = C * (delta ? 3 : 1); j = 0 static, 1 d1, 2 d2) for
@@ -90,8 +54,7 @@ __global__ void fe_finish_kernel(const float* __restrict__ feat, float* __restri
                                  int n_frame, int Tout, int take_log, int delta) {
     const int b = blockIdx.y;
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-    const int Cd = delta ? 3 * C : C;
-    const int W = Cd * n_frame;
+    const int W = (delta ? 3 * C : C) * n_frame;
     if (i >= (long)Tout * W) return;
     int F = n_frames, Fs = n_frames, seq = seq_len;
     if (lens) {
@@ -100,22 +63,14 @@ __global__ void fe_finish_kernel(const float* __restrict__ feat, float* __restri
         seq = use_mask ? (Lb + hop - 1) / hop : F;
         Fs = pad_div ? F : F - F % n_frame;
     }
-    const int t = (int)(i / W), w = (int)(i % W);
-    const int s = w / Cd, j = (w % Cd) / C, c = w % C;
-    const int f = t * n_frame + s;
     const float* rows = feat + (long)b * R * C;
-    float v = 0.f;
-    if (f < Fs) {
-        if (j == 0) v = fe_static(rows, f, c, C, seq, take_log);
-        else if (j == 1) v = fe_delta1(rows, f, c, C, seq, F, take_log);
-        else v = fe_delta2(rows, f, c, C, seq, F, take_log);
-    }
-    out[(long)b * Tout * W + i] = v;
+    out[(long)b * Tout * W + i] = fe_finish_value([&](long k) { return __ldg(rows + k); }, (int)(i / W), (int)(i % W), F,
+                                                  Fs, seq, C, n_frame, take_log, delta);
 }
 
 __global__ void fe_log_kernel(float* __restrict__ x, long n, float offset) {
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) x[i] = logf(x[i] + offset);
+    if (i < n) x[i] = fe_log_value(x[i], offset);
 }
 
 // SpecAugment masking (rnnt/transforms.py:53-147): x [B, D1, D2]; spans [B, nmask, 2] = [start, end) along dim `axis`

@@ -260,7 +260,10 @@ class CTCStreamDecoder:
     ``lm_token_map`` fuse the reference's LSTM LM as ``CTCEncoder.beam_search`` does; ``max_pending`` bounds the
     uncommitted tokens a prefix may hold before the beam collapses to its best prefix.
 
-    ``transform`` maps a chunk of audio to log-mel features [1, F, n] (the reference's feature transform);
+    ``transform`` maps a chunk of audio to log-mel features [1, F, n] (the reference's feature transform), on the host
+    before each chunk; when it is build_batch_transform's test module (a BatchTransform), ``decode`` uploads the
+    window's audio instead and the engine computes those features in its launch, bit for bit what the module gives the
+    window (``frames_per_chunk`` is then ignored: the first window builds the program);
     ``tokenizer`` is the reference's HuggingFaceTokenizer (``tokenizer.tokenizer.id_to_token``).  A chunk whose frame
     count differs from the previous one's (a short last chunk), or weights that moved (``.to()``, an optimizer's flat
     bucket), rebuild the program and carry the state (the beam included) over; only ``reset()`` starts a new utterance.
@@ -300,8 +303,10 @@ class CTCStreamDecoder:
         self.model = model
         self._engine = None
         self._frames = frames_per_chunk
+        from .rnnt.features import BatchTransform
+        self._device_fe = isinstance(transform, BatchTransform)    # the features run inside the decode launch
         self.reset_profile()
-        if frames_per_chunk is not None:
+        if frames_per_chunk is not None and not self._device_fe:
             self._build(operator.index(frames_per_chunk))
 
     def reset_profile(self):
@@ -312,11 +317,14 @@ class CTCStreamDecoder:
     def _build(self, n):
         from .stream_engine import CTCStreamBeamEngine, CTCStreamEngine
         st = self._engine.state() if self._engine is not None else None
+        fe = dict(frontend=self.transform, samples_per_chunk=n) if self._device_fe else {}
+        frames = None if self._device_fe else n                # n: the window's samples with a device front end
         if self._beam is None:
-            self._engine = CTCStreamEngine(self.model, 1, n, blank=self.model.blank, state=st)
+            self._engine = CTCStreamEngine(self.model, 1, frames, blank=self.model.blank, state=st, **fe)
         else:
             b = dict(self._beam)
-            self._engine = CTCStreamBeamEngine(self.model, 1, n, b.pop("W"), blank=self.model.blank, state=st, **b)
+            self._engine = CTCStreamBeamEngine(self.model, 1, frames, b.pop("W"), blank=self.model.blank, state=st,
+                                               **b, **fe)
         self._frames = n
 
     def _text(self, ids, counts):
@@ -333,11 +341,14 @@ class CTCStreamDecoder:
         import time
         from .stream_engine import param_fingerprint
         start = time.time()
-        xs = self.transform(frame).transpose(1, 2)                 # [1, n, F] log-mel
+        if self._device_fe:                                        # the window's audio, transformed in the launch
+            xs = torch.as_tensor(frame).to(self.device, torch.float32).reshape(1, -1)
+        else:
+            xs = self.transform(frame).transpose(1, 2).to(self.device, non_blocking=True)   # [1, n, F] log-mel
         if self._engine is None or xs.shape[1] != self._frames or \
                 self._engine.fingerprint != param_fingerprint(self.model):
             self._build(xs.shape[1])
-        ids, counts = self._engine.step(xs.to(self.device, non_blocking=True))   # one D2H per chunk
+        ids, counts = self._engine.step(xs)                        # one D2H per chunk
         self.encoder_elapsed.append(time.time() - start)
         return self._text(ids, counts)
 

@@ -7,9 +7,12 @@ joint_elapsed``, ``tokenizer`` -- so ``stream.py`` / ``youtube_live.py`` /
 launch per chunk (edgedict_b200/stream_engine.py) instead of a Python loop with a host sync per
 encoder frame.  With ``beam_width`` it decodes by streaming beam search instead (optionally with a fused LSTM
 language model): ``decode`` returns the text that became final in that chunk and ``flush()`` the rest.
-The feature transform and the BPE tokenizer are host-side components outside the
-hot path: they are taken from the caller (``transform=``, ``tokenizer=``) or, like the reference,
-built from FLAGS when the reference's ``rnnt.transforms`` / ``rnnt.tokenizer`` are importable.
+The BPE tokenizer is a host-side component, taken from the caller (``tokenizer=``) or, like the reference, built
+from FLAGS when the reference's ``rnnt.tokenizer`` is importable.  The feature transform runs on the device, in the
+same launch as the decode, when ``transform`` is build_batch_transform's test module (a BatchTransform): ``decode``
+then uploads the window of raw audio and the engine's front end computes, bit for bit, what that module gives the
+window.  Any other ``transform`` (a callable mapping a window to [1, F, n] features, or, with ``transform=None``, the
+reference's ``rnnt.transforms.build_transform`` from FLAGS) runs on the host before each chunk, as in the reference.
 """
 import operator
 import os
@@ -17,6 +20,7 @@ import time
 
 import torch
 
+from .features import BatchTransform
 from .models import ResLayerNormGRU, Transducer, convert_lightning2normal
 from .tokenizer import NUL, BOS, UNK
 from ..stream_engine import BEAM_MAX_W, GRUStreamBeamEngine, GRUStreamEngine, StreamBeamEngine, StreamEngine, \
@@ -76,10 +80,13 @@ class PytorchStreamDecoder(StreamTransducerDecoder):
                 win_length=FLAGS.win_length, hop_length=FLAGS.hop_length, delta=FLAGS.delta, cmvn=FLAGS.cmvn,
                 downsample=FLAGS.downsample, pad_to_divisible=False, T_mask=FLAGS.T_mask,
                 T_num_mask=FLAGS.T_num_mask, F_mask=FLAGS.F_mask, F_num_mask=FLAGS.F_num_mask)
+        elif isinstance(transform, BatchTransform):
+            input_size = transform.input_size if input_size is None else input_size
         elif input_size is None and transducer is None:
             # a caller-supplied transform: the feature width follows the flagfile (rnnt/transforms.py:30-51)
             input_size = FLAGS.feature_size * FLAGS.downsample * (3 if getattr(FLAGS, "delta", False) else 1)
         self.transform = transform
+        self._device_fe = isinstance(transform, BatchTransform)    # the features run inside the decode launch
         if transducer is None:
             logdir = os.path.join('logs', FLAGS.name)
             model_path = os.path.join(logdir, 'models', FLAGS.model_name)
@@ -110,7 +117,7 @@ class PytorchStreamDecoder(StreamTransducerDecoder):
         self._engine = None
         self._frames = frames_per_chunk
         self.reset_profile()
-        if frames_per_chunk is not None:
+        if frames_per_chunk is not None and not self._device_fe:   # a device front end builds for its first window
             self._build(frames_per_chunk)
 
     def _token_id(self, token):
@@ -123,16 +130,19 @@ class PytorchStreamDecoder(StreamTransducerDecoder):
     def _build(self, n):
         # a different chunk length (a short last chunk, a changed block size) or re-homed weights need a new phase
         # program, NOT a new utterance: the recurrent state moves over (rnnt/stream.py:94-120 carries it across
-        # arbitrary chunk lengths); only reset() starts from the primed zero state
+        # arbitrary chunk lengths); only reset() starts from the primed zero state.  n counts frames, or with a device
+        # front end the window's samples.
         st = self._engine.state() if self._engine is not None else None
         gru = isinstance(self.encoder.lstm, ResLayerNormGRU)
+        fe = dict(frontend=self.transform, samples_per_chunk=n) if self._device_fe else {}
+        frames = None if self._device_fe else n
         if self._beam is None:
-            self._engine = (GRUStreamEngine if gru else StreamEngine)(self._transducer, 1, n, unk_id=self._unk,
+            self._engine = (GRUStreamEngine if gru else StreamEngine)(self._transducer, 1, frames, unk_id=self._unk,
                                                                       blank=NUL, state=st,
-                                                                      max_symbols=self._max_symbols)
+                                                                      max_symbols=self._max_symbols, **fe)
         else:
-            self._engine = (GRUStreamBeamEngine if gru else StreamBeamEngine)(self._transducer, 1, n, blank=NUL,
-                                                                              state=st, **self._beam)
+            self._engine = (GRUStreamBeamEngine if gru else StreamBeamEngine)(self._transducer, 1, frames, blank=NUL,
+                                                                              state=st, **self._beam, **fe)
         self._frames = n
 
     @torch.no_grad()
@@ -143,16 +153,19 @@ class PytorchStreamDecoder(StreamTransducerDecoder):
     @torch.no_grad()
     def decode(self, frame):
         start = time.time()
-        xs = self.transform(frame).transpose(1, 2)                  # [1, n, F] log-mel, as stream.py:96
+        if self._device_fe:                                         # the window's audio, transformed in the launch
+            xs = torch.as_tensor(frame).to(self.device, torch.float32).reshape(1, -1)
+        else:
+            xs = self.transform(frame).transpose(1, 2).to(self.device, non_blocking=True)   # [1, n, F], stream.py:96
         if self._engine is None or xs.shape[1] != self._frames or \
                 self._engine.fingerprint != param_fingerprint(self._transducer):
             self._build(xs.shape[1])
         if self._beam is not None:
-            ids, counts = self._engine.step(xs.to(self.device, non_blocking=True))  # one D2H per chunk
+            ids, counts = self._engine.step(xs)                     # one D2H per chunk
             self.encoder_elapsed.append(time.time() - start)
             self.joint_elapsed += [0.0] * self._engine.n_out      # fused into the chunk kernel
             return self._text(ids[0, :int(counts[0])].tolist())
-        ids = self._engine.step(xs.to(self.device, non_blocking=True))[0].tolist()   # one D2H per chunk
+        ids = self._engine.step(xs)[0].tolist()                     # one D2H per chunk
         self.encoder_elapsed.append(time.time() - start)
         tokens = []
         for pred in ids:

@@ -17,13 +17,14 @@ import operator
 
 import torch
 
+from . import ops
 from ._lib import lib, check
 from .rnnt.tokenizer import NUL, BOS, UNK
 
 PH_LN, PH_PAIR, PH_LSTM, PH_LINEAR, PH_ARGMAX, PH_COPY, PH_BEAM_SELECT, PH_GATHER, PH_BEAM_FINAL, PH_BEAM_COMMIT, \
-    PH_SKIP, PH_CTC_BEAM, PH_GRU, PH_CTC_EMIT = range(14)
-F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE, F_LM, F_STREAM, F_FLUSH, F_CONT, F_ROUNDS = 1, 2, 4, 8, 16, 32, 64, 128, \
-    256, 512
+    PH_SKIP, PH_CTC_BEAM, PH_GRU, PH_CTC_EMIT, PH_FE_FRAME, PH_FE_GEMM, PH_FE_POWER, PH_FE_LOG, PH_FE_FINISH = range(19)
+F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE, F_LM, F_STREAM, F_FLUSH, F_CONT, F_ROUNDS, F_FRONTEND = 1, 2, 4, 8, 16, 32, \
+    64, 128, 256, 512, 1024
 BEAM_MAX_W = 1024                                     # EB_BEAM_MAX_W
 CTC_SEQ_HEAD = 5                                      # CTC_BEAM's token rows: {len, hash lo / hi, parent hash lo / hi}
 MAX_SYMBOLS = 16                                      # bounds the program: about (5 + L_dec) * K phases per frame
@@ -350,6 +351,91 @@ def check_stream_shape(enc, n_streams, frames_per_chunk):
     return S, n, T
 
 
+def frontend_geometry(frontend, samples_per_chunk):
+    """What a stream engine's device front end computes per window of L = ``samples_per_chunk`` samples: the operands
+    and flags of the feature module of ``frontend`` (build_batch_transform's test module, a BatchTransform) and the
+    window's frame arithmetic, as ops.fe_batch lays it out for one utterance of L samples: F = 1 + L // hop frames,
+    Fs of them kept by Downsample (all with pad_to_divisible, else F - F % n_stack), T = ceil(Fs / n_stack) model input
+    frames, the seq_len mask from frame ``seq`` on (logfbank; F for melspec and MFCC), ``Fc`` frames computed (Fs, or F
+    when the deltas read up to frame F - 1), the reflect padding ``pad`` = n_fft // 2 and the padded row of ``Lp`` = R
+    hop samples.  Raises TypeError / ValueError for a module that is not a BatchTransform, a train module that carries
+    SpecAugment masks or L <= n_fft // 2; touches no device."""
+    from .rnnt.features import BatchTransform, FilterbankFeatures, MelSpectrogram, MFCC
+    if not isinstance(frontend, BatchTransform):
+        raise TypeError("frontend must be a BatchTransform (build_batch_transform's test module), got %s"
+                        % type(frontend).__name__)
+    if (frontend.T_mask > 0 and frontend.T_num_mask > 0) or (frontend.F_mask > 0 and frontend.F_num_mask > 0):
+        raise ValueError("frontend carries SpecAugment masks: stream with build_batch_transform's test module, as the "
+                         "reference streams its test transform")
+    f = frontend.features
+    g = dict(dct=None, preemph=None, take_log=False, use_mask=False, dither=0.0)
+    if isinstance(f, FilterbankFeatures):
+        g.update(basis=f.dft_basis, fbT=f.fb_t, n_fft=f.n_fft, hop=f.hop_length, preemph=f.preemph, take_log=f.log,
+                 use_mask=True, dither=float(f.dither))
+    else:
+        ms = f.MelSpectrogram if isinstance(f, MFCC) else f
+        if not isinstance(ms, MelSpectrogram):
+            raise TypeError("frontend.features must be FilterbankFeatures, MelSpectrogram or MFCC, got %s"
+                            % type(f).__name__)
+        g.update(basis=ms.spectrogram.dft_basis, fbT=ms.mel_scale.fb, n_fft=ms.n_fft, hop=ms.hop_length)
+        if isinstance(f, MFCC):
+            g["dct"] = f.dct_mat
+    L = operator.index(samples_per_chunk)
+    n_fft, hop, n_stack = g["n_fft"], g["hop"], frontend.downsample
+    pad = n_fft // 2
+    if L <= pad:
+        raise ValueError("samples_per_chunk must exceed n_fft // 2 = %d (reflect padding), got %d" % (pad, L))
+    F = 1 + L // hop
+    Fs = F if frontend.pad_to_divisible else F - F % n_stack
+    _, (T,) = ops.fe_lengths([L], hop, n_stack, frontend.pad_to_divisible)
+    R = -(-(L + 2 * pad) // hop)
+    g.update(L=L, pad=pad, R=R, Lp=R * hop, F=F, Fs=Fs, T=T, seq=-(-L // hop) if g["use_mask"] else F,
+             Fc=F if frontend.delta else Fs, n_stack=n_stack, delta=frontend.delta, input_size=frontend.input_size)
+    return g
+
+
+def frontend_phases(engine, g, S):
+    """The front-end program of engine ``engine`` (whose ``dev`` and ``xin`` [S, T, input_size] are set) for S streams
+    of windows with frontend_geometry ``g``: FE_FRAME (dither, pre-emphasis, reflect padding), the direct-DFT FE_GEMM
+    over the Fc computed frames of each stream (the strided frames of the padded row), FE_POWER, the mel FE_GEMM, for
+    MFCC FE_LOG and the DCT FE_GEMM, and FE_FINISH into xin.  Allocates its buffers on ``engine``: ``audio`` [S, L],
+    ``noise`` [S, L] (with dither, else None) and the intermediates; keeps the module's tables on the device in
+    engine._keep.  Returns the phase list."""
+    dev, L, Lp, Fc = engine.dev, g["L"], g["Lp"], g["Fc"]
+    z = lambda *shape: torch.zeros(*shape, dtype=torch.float32, device=dev)
+    on_dev = lambda t: None if t is None else t.detach().to(dev, torch.float32).contiguous()
+    basis, fbT, dct = on_dev(g["basis"]), on_dev(g["fbT"]), on_dev(g["dct"])
+    nb2, n_mels = basis.shape[1], fbT.shape[1]
+    M = S * Fc
+    engine.audio = z(S, L)
+    engine.noise = z(S, L) if g["dither"] > 0 else None
+    pre = g["preemph"]
+    engine._fe_consts = torch.tensor([g["dither"], float(pre or 0.0)], dtype=torch.float32, device=dev)
+    xp, spec, power, feat = z(S * Lp + g["n_fft"]), z(M, nb2), z(M, nb2 // 2), z(M, n_mels)
+    engine._fe_bufs = [xp, spec, power, feat]
+    engine._keep += [t for t in (basis, fbT, dct) if t is not None]
+    gemm = lambda x1, aux, ldx1, ldx2, K, w, y: EbPhase(type=PH_FE_GEMM, S=M, N=w.shape[1], K1=K, aux=aux, ldx1=ldx1,
+                                                        ldx2=ldx2, x1=_ptr(x1), w1=_ptr(w), ldw1=w.shape[1], y=_ptr(y),
+                                                        ldy=w.shape[1])
+    fe = [EbPhase(type=PH_FE_FRAME, S=S, N=L, K1=g["pad"], ldy=Lp, x1=_ptr(engine.audio), x2=_ptr(engine.noise),
+                  fuse=_ptr(engine._fe_consts), flags=int(pre is not None), y=_ptr(xp)),
+          gemm(xp, Fc, Lp, g["hop"], g["n_fft"], basis, spec),
+          EbPhase(type=PH_FE_POWER, S=M, N=nb2 // 2, x1=_ptr(spec), y=_ptr(power)),
+          gemm(power, M, 0, nb2 // 2, nb2 // 2, fbT, feat)]
+    if dct is not None:
+        cep = z(M, dct.shape[1])
+        engine._fe_bufs.append(cep)
+        fe += [EbPhase(type=PH_FE_LOG, S=M, N=n_mels, x1=_ptr(feat), y=_ptr(feat)),
+               gemm(feat, M, 0, n_mels, n_mels, dct, cep)]
+        feat = cep
+    C, T = feat.shape[1], g["T"]
+    fe.append(EbPhase(type=PH_FE_FINISH, S=S, K1=Fc, N=C, aux=g["n_stack"], aux2=T, hist_ld=g["F"], hist_col=g["Fs"],
+                      x1_div=g["seq"], flags=int(g["take_log"]) | (2 if g["delta"] else 0), x1=_ptr(feat),
+                      y=_ptr(engine.xin), ldy=engine.xin.shape[1] * engine.xin.shape[2]))
+    assert tuple(engine.xin.shape) == (S, T, C * (3 if g["delta"] else 1) * g["n_stack"])
+    return fe
+
+
 def encoder_phases(prog, engine, enc, S, n):
     """Append the stateful streaming encoder for S streams and chunks of n log-mel frames to the phase list ``prog``:
     LayerNorm of the input, then per layer n LSTM cell steps from the carried (h, c), the residual LayerNorm and the
@@ -423,7 +509,13 @@ class _ChunkEngine:
     """What the streaming engines (StreamEngine, StreamBeamEngine, CTCStreamEngine) share: the host-side checks in a
     fixed order (the encoder kind, check_stream_shape, then the CUDA device), the stateful encoder at the head of the
     chunk program and the COPY that closes it, the launches, and ``state()`` / ``load_state()`` over
-    ``_state_views()``."""
+    ``_state_views()``.
+
+    Every engine takes ``frontend`` (build_batch_transform's test module) with ``samples_per_chunk`` = L: ``step`` then
+    takes fp32 audio [S, L] on the device, one window per stream, and the chunk program opens with the feature
+    transform (frontend_phases, in the same launch), which writes into ``xin`` bit for bit what ``frontend(audio, [L] *
+    S)[0]`` gives.  frames_per_chunk then follows from L (None, or the same count).  No front-end state is carried
+    between chunks: each window is transformed on its own, as the reference streams overlapping windows."""
     GRU = False          # the encoder kind: ResLayerNormGRU cells, carrying enc_h alone, or ResLayerNormLSTM cells
     HOST_STATE = ()      # keys of state() that are host tensors, outside _state_views
 
@@ -432,15 +524,37 @@ class _ChunkEngine:
         """The decode kernel entry every program of the engine runs through (an instance may set another)."""
         return "eb_decode_run_gru_rnnt" if self.GRU else "eb_decode_run"
 
-    def _check_shape(self, enc, n_streams, frames_per_chunk):
+    def _check_shape(self, enc, n_streams, frames_per_chunk, frontend=None, samples_per_chunk=None):
         """check_stream_shape's (S, n, encoder output frames per chunk), after refusing an encoder of the other kind
-        with ValueError.  Touches no device."""
+        with ValueError.  With a ``frontend`` (see frontend_geometry) the chunk is L = ``samples_per_chunk`` samples of
+        audio per stream, n follows from L, and a ``frames_per_chunk`` given as well must agree with it; the window
+        must give at least one model input frame, and the module's input_size must be the encoder's input width.
+        Sets ``_fe`` (the geometry, or None).  Touches no device."""
         from .rnnt.models import ResLayerNormGRU, ResLayerNormLSTM
         if not isinstance(enc.lstm, ResLayerNormGRU if self.GRU else ResLayerNormLSTM):
             # the encoder phases are cells of one kind: LSTM (4H-row weights) or GRU (3H rows)
             who, kind, got = type(self).__name__, "a GRU" if self.GRU else "an LSTM", type(enc.lstm).__name__
             raise ValueError("%s streams %s encoder only, got %s" % (who, kind, got))
-        return check_stream_shape(enc, n_streams, frames_per_chunk)
+        self._fe = None
+        if frontend is None:
+            if samples_per_chunk is not None:
+                raise ValueError("samples_per_chunk needs a frontend")
+            return check_stream_shape(enc, n_streams, frames_per_chunk)
+        if samples_per_chunk is None:
+            raise ValueError("a frontend needs samples_per_chunk, the audio samples of a chunk per stream")
+        g = frontend_geometry(frontend, samples_per_chunk)
+        if g["T"] < 1:
+            raise ValueError("a window of %d samples gives %d frames, no model input frame after stacking by %d"
+                             % (g["L"], g["F"], g["n_stack"]))
+        if frames_per_chunk is not None and operator.index(frames_per_chunk) != g["T"]:
+            raise ValueError("frames_per_chunk (%d) disagrees with the %d model input frames a window of %d samples "
+                             "gives" % (operator.index(frames_per_chunk), g["T"], g["L"]))
+        F = enc.norm.weight.shape[0]
+        if g["input_size"] != F:
+            raise ValueError("frontend.input_size (%d) differs from the encoder's input width (%d)"
+                             % (g["input_size"], F))
+        self._fe = g
+        return check_stream_shape(enc, n_streams, g["T"])
 
     def _build_encoder(self, prog, model, enc, S, n, T):
         """After every other check, the CUDA device check; then encoder_phases into ``prog`` (T output frames per
@@ -451,8 +565,14 @@ class _ChunkEngine:
             raise RuntimeError("%s needs the model on a CUDA device" % type(self).__name__)
         self._keep = [p.detach() for p in model.parameters()]
         self.fingerprint = param_fingerprint(model)
+        self._bar = torch.zeros(64, dtype=torch.int32, device=self.dev)
         E = encoder_phases(prog, self, enc, S, n)
         assert self.n_out == T
+        if self._fe is not None:                             # the front end opens the chunk program
+            fe = frontend_phases(self, self._fe, S)
+            self._fe_prog = _upload(fe, self.dev)
+            prog.insert(0, EbPhase(type=PH_GATHER, flags=F_FRONTEND, x1=_ptr(self._fe_prog), K1=len(fe),
+                                   tok_out=_ptr(self._bar, 1)))
         return E
 
     def _finish(self, prog, state):
@@ -462,7 +582,6 @@ class _ChunkEngine:
         L, S, H = self.enc_h.shape
         prog.append(EbPhase(type=PH_COPY, S=L * S, N=H, x1=_ptr(self.enc_htmp), y=_ptr(self.enc_h)))
         self._chunk, self.n_chunk_phases = _upload(prog, self.dev), len(prog)
-        self._bar = torch.zeros(64, dtype=torch.int32, device=self.dev)
         if state is None:
             self.reset()
         else:
@@ -470,6 +589,23 @@ class _ChunkEngine:
 
     def _run(self, prog, nphase):
         _launch(self.RUN, prog, nphase, self._bar, self.max_ctas)
+
+    def _load(self, chunk):
+        """Put a chunk where the chunk program reads it: log-mel frames [S, n, F] (device or pinned host) into xin, or
+        with a front end fp32 audio [S, L] on the engine's device into ``audio`` and, with dither, N(0, 1) noise from
+        the current generator into ``noise`` (what the module's randn_like(x) draws).  ValueError for a chunk of the
+        wrong shape, dtype or device, before any device work."""
+        if self._fe is None:
+            self.xin.copy_(chunk, non_blocking=True)
+            return
+        if not isinstance(chunk, torch.Tensor) or chunk.dtype != torch.float32 or chunk.device != self.dev or \
+                tuple(chunk.shape) != tuple(self.audio.shape):
+            raise ValueError("with a front end a chunk is fp32 audio %s on %s, got %s" % (
+                list(self.audio.shape), self.dev, "%s %s on %s" % (chunk.dtype, list(chunk.shape), chunk.device)
+                if isinstance(chunk, torch.Tensor) else type(chunk).__name__))
+        self.audio.copy_(chunk)
+        if self.noise is not None:
+            torch.randn(self.noise.shape, device=self.dev, out=self.noise)
 
     def _fetch(self, width):
         """Copy ``_out`` (ids [S, width] | counts [S] | any further values) to the pinned ``_host``: the chunk's only
@@ -592,11 +728,12 @@ class _CommitEngine(_ChunkEngine):
 
     @torch.no_grad()
     def step(self, chunk):
-        """chunk [S, n, F] log-mel frames (device or pinned host) -> (committed ids int32 [S, K], counts int32 [S]) on
+        """chunk [S, n, F] log-mel frames (device or pinned host), or with a front end fp32 audio [S, L] on the device,
+        -> (committed ids int32 [S, K], counts int32 [S]) on
         the host: row s holds in its first counts[s] entries the tokens stream s committed in this chunk.  K is
         max_pending, or more on the first step after load_state had to commit carried tokens (they come first).
         ``n_collapses`` counts the forced collapses so far."""
-        self.xin.copy_(chunk, non_blocking=True)
+        self._load(chunk)
         self._run(self._chunk, self.n_chunk_phases)
         ids, counts, collapsed = self._fetch(self.max_pending)
         self.n_collapses += int(collapsed.sum())
@@ -617,13 +754,13 @@ class StreamEngine(_ChunkEngine):
     STATE = ("enc_h", "enc_c", "dec_h", "dec_c", "dec_x", "tok")   # the carried state (enc_c: None for a GRU encoder)
 
     def __init__(self, transducer, n_streams, frames_per_chunk, unk_id=UNK, blank=NUL, max_ctas=0, state=None,
-                 max_symbols=1):
+                 max_symbols=1, frontend=None, samples_per_chunk=None):
         """``max_symbols`` = K: per output frame up to K rounds of joint -> argmax (with the <unk> rule) -> masked
         predictor step; a stream's frame ends at its first blank or after K non-blank tokens.  ``step`` then returns
         [S, n_out * K]: K entries per frame, blank for the rounds a stream did not take."""
         K = check_max_symbols(max_symbols)
         enc, dec, joint = transducer.encoder, transducer.decoder, transducer.joint.joint
-        S, n, T = self._check_shape(enc, n_streams, frames_per_chunk)
+        S, n, T = self._check_shape(enc, n_streams, frames_per_chunk, frontend, samples_per_chunk)
         self.S, self.n, self.blank, self.unk, self.max_ctas, self.max_symbols = S, n, blank, unk_id, max_ctas, K
         prog = []
         E = self._build_encoder(prog, transducer, enc, S, n, T)
@@ -661,9 +798,10 @@ class StreamEngine(_ChunkEngine):
 
     @torch.no_grad()
     def step(self, chunk):
-        """chunk [S, n, F] log-mel frames (device or pinned host) -> int32 [S, n_out * max_symbols] token ids, the
+        """chunk [S, n, F] log-mel frames (device or pinned host), or with a front end fp32 audio [S, L] on the device,
+        -> int32 [S, n_out * max_symbols] token ids, the
         max_symbols rounds of each frame in order (blank = 0 means 'no symbol in this round')."""
-        self.xin.copy_(chunk, non_blocking=True)
+        self._load(chunk)
         if self.max_symbols > 1:
             self.hist.fill_(self.blank)             # the columns of rounds skipped for every stream are not written
         self._run(self._chunk, self.n_chunk_phases)
@@ -840,7 +978,7 @@ class StreamBeamEngine(_CommitEngine):
 
     def __init__(self, transducer, n_streams, frames_per_chunk, W, merge=True, lm=None, lm_weight=0.0,
                  length_bonus=0.0, lm_bos=1, lm_token_map=None, max_pending=64, state=None, blank=NUL, max_ctas=0,
-                 max_symbols=1):
+                 max_symbols=1, frontend=None, samples_per_chunk=None):
         K = check_max_symbols(max_symbols)
         W = operator.index(W)
         if not 1 <= W <= BEAM_MAX_W:
@@ -848,7 +986,7 @@ class StreamBeamEngine(_CommitEngine):
         V = transducer.joint.joint[2].weight.shape[0]
         fusion = check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map)
         enc, dec, joint = transducer.encoder, transducer.decoder, transducer.joint.joint
-        S, n, T = self._check_shape(enc, n_streams, frames_per_chunk)
+        S, n, T = self._check_shape(enc, n_streams, frames_per_chunk, frontend, samples_per_chunk)
         P = operator.index(max_pending)
         if P < T * K:
             raise ValueError("max_pending (%d) must be at least the encoder frames per chunk times max_symbols (%d x %d):"
@@ -1078,12 +1216,13 @@ class CTCStreamEngine(_ChunkEngine):
     GRU = True
     RUN = "eb_decode_run_ctc_stream"
 
-    def __init__(self, ctc_model, n_streams, frames_per_chunk, blank=0, max_ctas=0, state=None):
+    def __init__(self, ctc_model, n_streams, frames_per_chunk, blank=0, max_ctas=0, state=None, frontend=None,
+                 samples_per_chunk=None):
         from .rnnt.models import CTCEncoder
         if not isinstance(ctc_model, CTCEncoder):
             raise TypeError("CTCStreamEngine streams a CTCEncoder, got %s" % type(ctc_model).__name__)
         enc, lin = ctc_model.model, ctc_model.tovocab[0]
-        S, n, T = self._check_shape(enc, n_streams, frames_per_chunk)
+        S, n, T = self._check_shape(enc, n_streams, frames_per_chunk, frontend, samples_per_chunk)
         V, blank = lin.weight.shape[0], operator.index(blank)
         if not 0 <= blank < V:
             raise ValueError("blank must lie in [0, %d), got %d" % (V, blank))
@@ -1122,10 +1261,10 @@ class CTCStreamEngine(_ChunkEngine):
 
     @torch.no_grad()
     def step(self, chunk):
-        """chunk [S, n, F] log-mel frames (device or pinned host) -> (ids int32 [S, n_out], counts int32 [S]) on the
-        host: row s holds in its first counts[s] entries the ids stream s emitted in this chunk.  One device-to-host
+        """chunk [S, n, F] log-mel frames (device or pinned host), or with a front end fp32 audio [S, L] on the device,
+        -> (ids int32 [S, n_out], counts int32 [S]) on the host: row s holds in its first counts[s] entries the ids stream s emitted in this chunk.  One device-to-host
         copy per chunk."""
-        self.xin.copy_(chunk, non_blocking=True)
+        self._load(chunk)
         self._run(self._chunk, self.n_chunk_phases)
         ids, counts, _ = self._fetch(self.n_out)
         return ids, counts
@@ -1154,7 +1293,8 @@ class CTCStreamBeamEngine(_CommitEngine):
     RUN = "eb_decode_run_ctc_stream_beam"
 
     def __init__(self, ctc_model, n_streams, frames_per_chunk, W, *, lm=None, lm_weight=0.0, length_bonus=0.0,
-                 lm_bos=1, lm_token_map=None, max_pending=64, blank=0, max_ctas=0, state=None):
+                 lm_bos=1, lm_token_map=None, max_pending=64, blank=0, max_ctas=0, state=None, frontend=None,
+                 samples_per_chunk=None):
         from .rnnt.models import CTCEncoder
         if not isinstance(ctc_model, CTCEncoder):
             raise TypeError("CTCStreamBeamEngine streams a CTCEncoder, got %s" % type(ctc_model).__name__)
@@ -1167,7 +1307,7 @@ class CTCStreamBeamEngine(_CommitEngine):
         if not 0 <= blank < V:
             raise ValueError("blank must lie in [0, %d), got %d" % (V, blank))
         fusion = check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map)
-        S, n, T = self._check_shape(enc, n_streams, frames_per_chunk)
+        S, n, T = self._check_shape(enc, n_streams, frames_per_chunk, frontend, samples_per_chunk)
         P = operator.index(max_pending)
         if P < T:
             raise ValueError("max_pending (%d) must be at least the encoder frames per chunk (%d): a chunk can add that "

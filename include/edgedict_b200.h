@@ -431,7 +431,8 @@ int eb_joint_band_dpre_reduce(const void* dx, const float* hidden, int is_bf16, 
  * phase program once (edgedict_b200/stream_engine.py) and launches it per chunk; see decode.cu. */
 enum { EB_PH_LN = 0, EB_PH_PAIR = 1, EB_PH_LSTM = 2, EB_PH_LINEAR = 3, EB_PH_ARGMAX = 4, EB_PH_COPY = 5,
        EB_PH_BEAM_SELECT = 6, EB_PH_GATHER = 7, EB_PH_BEAM_FINAL = 8, EB_PH_BEAM_COMMIT = 9, EB_PH_SKIP = 10,
-       EB_PH_CTC_BEAM = 11, EB_PH_GRU = 12, EB_PH_CTC_EMIT = 13 };
+       EB_PH_CTC_BEAM = 11, EB_PH_GRU = 12, EB_PH_CTC_EMIT = 13, EB_PH_FE_FRAME = 14, EB_PH_FE_GEMM = 15,
+       EB_PH_FE_POWER = 16, EB_PH_FE_LOG = 17, EB_PH_FE_FINISH = 18 };
 typedef struct EbPhase {
     int32_t type, S, K1, K2, N, flags, ldx1, ldx2, ldw1, ldw2, ldy, aux, aux2, hist_ld, hist_col, x1_div;
     const float *x1, *x2, *w1, *w2, *b1, *b2;
@@ -477,6 +478,20 @@ typedef struct EbPhase {
  * to its best slot by y; src receives the gather sources that move the kept slots' state into place.  K2 is the rows'
  * head before their tokens (0 for BEAM_SELECT's 3, 5 for CTC_BEAM's); y2, when set, int32 [S], receives each stream's
  * last committed token whenever it commits any.
+ *     1024 = GATHER runs a front-end program instead of gathering: the K1 phases at x1 (an EbPhase array), each closed
+ *            by a grid barrier on the counter tok_out, which the decode entries zero at every launch (barrier_dev holds
+ *            two counters, 8 bytes).  Its phases are FE_* only; they compute a chunk's features from raw audio:
+ *   FE_FRAME  S streams of N samples x1 (x2: optional dither noise [S, N]; fuse = {dither, preemph} on the device) ->
+ *             y [S, ldy]: fl(x + fl(dither * noise)), pre-emphasised with flags 1, reflect-padded by K1 samples, zeros
+ *             after;
+ *   FE_GEMM   y [S, N] (ldy) = A [S, K1] B [K1, N] with A(m, k) = x1[(m / aux) ldx1 + (m % aux) ldx2 + k] and
+ *             B(k, n) = w1[k ldw1 + n], each output eb_gemm_f32's k-ascending fmaf chain from 0;
+ *   FE_POWER  y [S, N] = re^2 + im^2 of x1 rows [S, 2N] = [re | im];
+ *   FE_LOG    y [S*N] = log(x1 + 1e-6);
+ *   FE_FINISH x1 [S*K1, N] per-frame rows of S streams -> y [S, aux2, W] (W = N (3 with flags 2) aux): aux frames
+ *             stacked per row, log(x + 1e-20) with flags 1, deltas with flags 2; hist_ld = frames F, hist_col = frames
+ *             kept Fs, x1_div = the first masked frame.
+ *            Each value is frontend.cu's expression for it, so the features equal eb_fe_* / eb_gemm_f32's bit for bit.
  * x1_div (LINEAR): row r of x1 is x1[r / x1_div] (0 or 1: row r), the encoder frame a beam's W rows share.
  * Beam search (batched, W slots per utterance, row r = b*W + slot; see decode.cu for the field use of each phase):
  * at most EB_BEAM_MAX_W slots per utterance.
