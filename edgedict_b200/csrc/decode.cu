@@ -632,7 +632,10 @@ __device__ __forceinline__ void fe_program(const EbPhase& head) {
 //     flags 32 = LM fusion: x2 LM logits [B*W, K2] (ldx2), fuse {lm_weight, length_bonus}, tok_map [V] -> LM token or
 //     -1, tok_out2 LM token per row (-1 where the LM rests, its masked step's sentinel).
 //   BEAM_FINAL (S = B, aux = W, aux2 = blank): y slot log p; hist; tok_out ids [B][ldy], the non-blank tokens of the
-//     best live slot right-aligned in the row and -1 before them; y2 -log p of that slot [B].
+//     best live slot right-aligned in the row and -1 before them; y2 -log p of that slot [B].  N-best (all unused, so
+//     zero / NULL, by the best-only program): K1 = N ranks (0: 1), tok_out ids [B*N][ldy] and y2 [B*N] per rank;
+//     seq_out (optional) each token's frame [B*N][ldy] (column / ldw2, ldw2 = K columns per frame, 0: 1); tok_out2
+//     (optional) the count min(N, live) [B].
 //   BEAM_COMMIT (S = B streams, aux = W, N = max_pending, aux2 = max_pending - n_out, K1 = sequence row stride, K2 = the
 //     row's head before its tokens (0: 3, BEAM_SELECT's {len, hash lo, hash hi}; CTC_SEQ_HEAD = 5 for CTC_BEAM's rows),
 //     hist_ld = T', flags 128 = collapse unconditionally): y slot value (in/out: log p, or CTC_BEAM's ranking value);
@@ -1135,41 +1138,73 @@ __device__ __noinline__ void phase_beam_commit(const EbPhase& p, float* sm) {
     }
 }
 
+// The N best live slots of each utterance (N = K1, 0 read as 1), ranked by value descending, lowest slot on ties
+// (logp.argmax() at rank 0, -0 with +0): the 64-bit composites order_key(value) << 32 | tie_key(slot) of the live
+// slots, bitonic-sorted in shared memory as BEAM_SELECT sorts its survivors, by the CTA's first warp (up to 32 keys
+// per lane and step at W = 1024; with all 256 threads eb_decode_run_ctc spills 4 bytes more).  Lane n walks rank n's
+// back-pointers (then n + 32, ...) over the hist_ld columns and writes its non-blank tokens right-aligned in row
+// b*N + n of tok_out (-1 before them), with seq_out set each token's frame (column / ldw2, ldw2 = K rounds per frame, 0 read as 1) in the same positions, and
+// y2[b*N + n] = -value; tok_out2, when set, gets the count min(N, live) per utterance.  Ranks at or past the count hold
+// ids and frames -1 and y2 = +inf.  The walk is one dependent load per column, as for N = 1.
 __device__ __noinline__ void phase_beam_final(const EbPhase& p) {
+    extern __shared__ __align__(16) float dsm[];
+    unsigned long long* comp = reinterpret_cast<unsigned long long*>(dsm);     // [BEAM_MAX_W]
     const int W = p.aux, T = p.hist_ld, blank = p.aux2, lane = threadIdx.x & 31;
     const long BTW = (long)p.S * T * W;
     const int* hpar = p.hist;
     const int* htok = p.hist + BTW;
     const int* hlive = p.hist + 3 * BTW;
-    if (threadIdx.x >= 32) return;
+    if (threadIdx.x >= 32) return;                           // one warp: with the whole CTA the CTC entry spills more
     for (int b = blockIdx.x; b < p.S; b += gridDim.x) {
         const int nlive = T == 0 ? 1 : __ldcg(hlive + (long)b * T + T - 1);
-        float best = -INFINITY;
-        int bi = -1;
-        for (int j = lane; j < nlive; j += 32) {
-            const float v = __ldcg(p.y + (long)b * W + j);
-            if (bi < 0 || v > best) { best = v; bi = j; }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {                   // logp.argmax(): the lowest slot on ties
-            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (oi >= 0 && (bi < 0 || ob > best || (ob == best && oi < bi))) { best = ob; bi = oi; }
-        }
-        int* ids = p.tok_out + (long)b * p.ldy;
-        int pos = T;
-        if (lane == 0) {
-            int slot = bi;
-            for (int tt = T - 1; tt >= 0; --tt) {
-                const long h = ((long)b * T + tt) * W + slot;
-                const int k = __ldcg(htok + h);
-                if (k != blank) ids[--pos] = k;
-                slot = __ldcg(hpar + h);
+        int P = 1;
+        while (P < nlive) P <<= 1;
+        __syncwarp();                                        // the previous utterance is done with shared memory
+        for (int i = lane; i < P; i += 32)
+            comp[i] = i < nlive ? ((unsigned long long)order_key(__ldcg(p.y + (long)b * W + i)) << 32) | tie_key(i) : 0;
+        __syncwarp();
+        for (int kk = 2; kk <= P; kk <<= 1)                  // bitonic sort, descending
+            for (int jj = kk >> 1; jj > 0; jj >>= 1) {
+                for (int i = lane; i < P; i += 32) {
+                    const int l = i ^ jj;
+                    if (l > i) {
+                        const unsigned long long a = comp[i], c = comp[l];
+                        if ((i & kk) == 0 ? a < c : a > c) {
+                            comp[i] = c;
+                            comp[l] = a;
+                        }
+                    }
+                }
+                __syncwarp();
             }
-            p.y2[b] = -best;
+        const int NB = p.K1 > 0 ? p.K1 : 1, KR = p.ldw2 > 0 ? p.ldw2 : 1, cnt = min(NB, nlive);
+        for (int n = lane; n < NB; n += 32) {
+            const long row = (long)b * NB + n;
+            int* ids = p.tok_out + row * p.ldy;
+            int* fr = p.seq_out ? p.seq_out + row * p.ldy : nullptr;
+            int pos = T;
+            if (n < cnt) {
+                const int top = (int)tie_key((unsigned)comp[n]);
+                int slot = top;
+                for (int tt = T - 1; tt >= 0; --tt) {
+                    const long h = ((long)b * T + tt) * W + slot;
+                    const int k = __ldcg(htok + h);
+                    if (k != blank) {
+                        ids[--pos] = k;
+                        if (fr) fr[pos] = tt / KR;
+                    }
+                    slot = __ldcg(hpar + h);
+                }
+                p.y2[row] = -__ldcg(p.y + (long)b * W + top);  // the value itself: -0 stays -0, as argmax gave it
+            } else {
+                p.y2[row] = INFINITY;
+            }
+            for (int j = 0; j < pos; ++j) {
+                ids[j] = -1;
+                if (fr) fr[j] = -1;
+            }
         }
-        pos = __shfl_sync(0xffffffffu, pos, 0);
-        for (int j = lane; j < pos; j += 32) ids[j] = -1;
+        if (p.tok_out2 && lane == 0) p.tok_out2[b] = cnt;
     }
 }
 

@@ -186,7 +186,7 @@ def free_beam_search():
 
 
 def beam_search(log_probs, input_lengths, beam_width, blank=0, *, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1,
-                lm_token_map=None):
+                lm_token_map=None, nbest=None):
     """CTC prefix beam search (Hannun et al., 2014) on the device, optionally with shallow fusion of the reference's
     LSTM language model (LMModel, or its state_dict).  ``CTCEncoder.beam_search`` states the rule.
 
@@ -200,9 +200,18 @@ def beam_search(log_probs, input_lengths, beam_width, blank=0, *, lm=None, lm_we
     (pb (+) pnb) + f).  Every argument is checked on the host before any device work (TypeError / ValueError, and
     RuntimeError for CPU log_probs: there is no CPU path).  One persistent kernel launch (stream_engine.CTCBeamEngine)
     and one device-to-host copy of the ids.  The engine stays resident for the next call with the same shapes and LM
-    (about 4·B·T·(V + 4·W) bytes and the LM's weights); ``free_beam_search()`` releases it."""
+    (about 4·B·T·(V + 4·W) bytes and the LM's weights); ``free_beam_search()`` releases it.
+
+    N-best lists: ``nbest`` = N (an integer in [1, W]) returns instead a list of B lists of
+    ``stream_engine.Hypothesis(tokens, frames, nlogp)``, best first: the live prefixes at the end of the search, ranked
+    by (pb (+) pnb) + f descending (lowest slot on ties, the rule the best-only call picks by), min(N, live) of them.
+    nlogp is the negated (pb (+) pnb) + f, and entry 0 of each list is bitwise the best-only call's ids and score.
+    ``frames`` gives each token's log-prob frame: the frame of the extension that put it into the prefix, on the path
+    the history recorded (an extension merged into another prefix's stay adds no token to it), so frames are strictly
+    increasing.  An utterance of length 0 gives one empty hypothesis with nlogp 0.  Still one device-to-host copy;
+    ``nbest`` is part of the engine cache key."""
     import numbers
-    from .stream_engine import BEAM_MAX_W, CTCBeamEngine, check_lm_args, lm_cache_key
+    from .stream_engine import BEAM_MAX_W, CTCBeamEngine, check_lm_args, check_nbest, lm_cache_key, nbest_lists
     if not isinstance(log_probs, torch.Tensor):
         raise TypeError("log_probs must be a tensor")
     if log_probs.dtype != torch.float32:
@@ -220,6 +229,7 @@ def beam_search(log_probs, input_lengths, beam_width, blank=0, *, lm=None, lm_we
         raise ValueError("beam_width must be in [1, %d], got %d" % (BEAM_MAX_W, W))
     if W * V >= 2 ** 31:
         raise ValueError("beam_width x V must stay below 2^31, got %d x %d" % (W, V))
+    N = 0 if nbest is None else check_nbest(nbest, W)
     blank = operator.index(blank)
     if not 0 <= blank < V:
         raise ValueError("blank must lie in [0, %d), got %d" % (V, blank))
@@ -231,16 +241,18 @@ def beam_search(log_probs, input_lengths, beam_width, blank=0, *, lm=None, lm_we
         raise RuntimeError("edgedict_b200 ctc beam_search needs CUDA log_probs (got a %s tensor); there is no CPU path"
                            % log_probs.device)
     dev = log_probs.device
-    key = (B, T, V, W, blank, dev, lm_cache_key(fusion))
+    key = (B, T, V, W, N, blank, dev, lm_cache_key(fusion))
     eng = _beam_engines.get(key)
     if eng is None:
         _beam_engines.clear()                                  # one resident program is enough
         eng = _beam_engines[key] = CTCBeamEngine(B, T, V, W, blank, lm=lm, lm_weight=lm_weight,
                                                  length_bonus=length_bonus, lm_bos=lm_bos, lm_token_map=lm_token_map,
-                                                 device=dev)
+                                                 device=dev, nbest=N)
     lens = torch.empty(B, dtype=torch.int32, pin_memory=True)
     lens.copy_(il)
     with torch.no_grad():
+        if N:
+            return nbest_lists(eng.run(log_probs, lens.to(dev, non_blocking=True)), B, N, T)
         ids, nlogp = eng.run(log_probs, lens.to(dev, non_blocking=True))
         ids = ids.cpu().numpy()
     return [row[row >= 0].astype("int64") for row in ids], nlogp.clone()

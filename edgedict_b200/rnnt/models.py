@@ -407,7 +407,7 @@ class Transducer(nn.Module):
 
     @torch.no_grad()
     def beam_search(self, xs, xlen=None, W=4, merge=True, *, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1,
-                    lm_token_map=None, max_symbols=1):
+                    lm_token_map=None, max_symbols=1, nbest=None):
         """SURVEY 8(f) N4: beam decode.  The reference has no beam search in rnnt/ (north_star mentions one); its
         legacy v0 stack holds a batch-1 Graves-style search (models.py:121-202, with no-op `sorted(...)` calls and a
         removed `volatile=` API).  This is a time-synchronous beam under the SAME emission constraint as
@@ -444,13 +444,26 @@ class Transducer(nn.Module):
         merge only when both their sequences and their closedness are equal.  A survivor that took a non-blank token
         steps its predictor (and LM); the others keep their parent's state.  An utterance's frame ends after round K-1
         or as soon as none of its hypotheses is open.  K = 1 is the search above, bit for bit, and W = 1 gives the
-        non-blank tokens of `greedy_decode(max_symbols=K)`."""
-        from ..stream_engine import (BeamEngine, BEAM_MAX_W, check_lm_args, check_max_symbols, lm_cache_key,
-                                     param_fingerprint)
+        non-blank tokens of `greedy_decode(max_symbols=K)`.
+
+        N-best lists: ``nbest`` = N (an integer in [1, W]) returns, instead of the pair above, a list of B lists of
+        `stream_engine.Hypothesis(tokens, frames, nlogp)`, best first: the live hypotheses at the end of the search,
+        ranked by log p descending (lowest slot on ties, the rule the best-only call picks by), min(N, live) of them.
+        nlogp is the negated log p (the fused score with an LM), and entry 0 of each list is bitwise the best-only
+        call's ids and -log p, for every W, K, `merge` and LM setting.  ``frames`` gives each token's encoder output
+        frame (after the time reductions): the frame in which the search's own path took it.  The tokens of one frame
+        appear in round order, at most K per frame, so frames are non-decreasing (strictly increasing for K = 1).
+        With `merge` the frames are those of the back-pointer chain the history recorded for the surviving
+        candidate, and nlogp is the merged score.  An utterance of 0 frames gives one empty hypothesis with nlogp 0.
+        For the E6D2 front end, frame f starts at f * 2**len(reductions) * downsample * hop / sample_rate seconds of
+        audio, as in `align`.  Still one device-to-host copy; `nbest` is part of the engine cache key."""
+        from ..stream_engine import (BeamEngine, BEAM_MAX_W, check_lm_args, check_max_symbols, check_nbest,
+                                     lm_cache_key, nbest_lists, param_fingerprint)
         K = check_max_symbols(max_symbols)
         W = operator.index(W)
         if not 1 <= W <= BEAM_MAX_W:
             raise ValueError("beam width W must be in [1, %d], got %d" % (BEAM_MAX_W, W))
+        N = 0 if nbest is None else check_nbest(nbest, W)
         fusion = check_lm_args(lm, self.joint.joint[2].weight.shape[0], lm_weight, length_bonus, lm_bos, lm_token_map)
         lm_key = lm_cache_key(fusion)
         h_enc, _ = self.encoder(xs)
@@ -461,14 +474,16 @@ class Transducer(nn.Module):
             frames = scale_length(T, xlen).clamp(max=T).to(torch.int32)
         frames = _lens_to_device(frames.cpu(), h_enc.device)
         # the phase program bakes raw weight pointers: re-homed parameters (FlatAdam, .to(), .float()) rebuild it
-        key = (B, T, W, bool(merge), K, h_enc.device, param_fingerprint(self), lm_key)
+        key = (B, T, W, bool(merge), K, N, h_enc.device, param_fingerprint(self), lm_key)
         cache = self.__dict__.setdefault("_beam_engines", {})
         eng = cache.get(key)
         if eng is None:
             cache.clear()                                  # one resident program is enough
             eng = cache[key] = BeamEngine(self, B, T, W, merge=bool(merge), blank=self.blank, lm=lm,
                                           lm_weight=lm_weight, length_bonus=length_bonus, lm_bos=lm_bos,
-                                          lm_token_map=lm_token_map, max_symbols=K)
+                                          lm_token_map=lm_token_map, max_symbols=K, nbest=N)
+        if N:
+            return nbest_lists(eng.run(h_enc, frames), B, N, eng.ids.shape[-1])
         ids, nlogp = eng.run(h_enc, frames)
         ids = ids.cpu().numpy()
         return [[int(k) for k in row if k >= 0] for row in ids], nlogp.clone()
@@ -517,7 +532,8 @@ class CTCEncoder(nn.Module):
         return [ids[i, :int(counts[i])].astype("int64") for i in range(B)], out[B * T + B:].view(torch.float32).clone()
 
     @torch.no_grad()
-    def beam_search(self, xs, xlen=None, W=4, *, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1, lm_token_map=None):
+    def beam_search(self, xs, xlen=None, W=4, *, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1, lm_token_map=None,
+                    nbest=None):
         """CTC prefix beam search (Hannun et al., 2014) after ``forward`` (which follows ``set_precision``), optionally
         with shallow fusion of the reference's LSTM language model.  xs [B, T, F] -> (list of B int64 id arrays, -score
         [B] on the device).  Utterance b decodes min(T', scale_length(xlen)[b]) log-prob frames (all T' when xlen is
@@ -542,18 +558,21 @@ class CTCEncoder(nn.Module):
         runs in fp32-accurate arithmetic whatever the precision setting.  lm_weight = length_bonus = 0 gives the
         result of lm=None bit for bit.  NaN log-probs are outside the contract: the search still ends and stays in
         bounds, but which hypotheses a NaN keeps is unspecified.  See ``edgedict_b200.ctc.beam_search`` (this search on
-        log-probs you already have) for the arguments."""
+        log-probs you already have) for the arguments, and for ``nbest``, which returns N-best lists with the log-prob
+        frame of each token."""
         from .. import ctc
-        from ..stream_engine import BEAM_MAX_W, check_lm_args
+        from ..stream_engine import BEAM_MAX_W, check_lm_args, check_nbest
         W = operator.index(W)
         if not 1 <= W <= BEAM_MAX_W:
             raise ValueError("beam width W must be in [1, %d], got %d" % (BEAM_MAX_W, W))
+        if nbest is not None:
+            check_nbest(nbest, W)
         check_lm_args(lm, self.tovocab[0].weight.shape[0], lm_weight, length_bonus, lm_bos, lm_token_map)
         lp = self.forward(xs)
         B, T = lp.shape[0], lp.shape[1]
         frames = torch.full((B,), T, dtype=torch.int64) if xlen is None else _ctc_frames(T, xlen, B)
         return ctc.beam_search(lp, frames, W, self.blank, lm=lm, lm_weight=lm_weight, length_bonus=length_bonus,
-                               lm_bos=lm_bos, lm_token_map=lm_token_map)
+                               lm_bos=lm_bos, lm_token_map=lm_token_map, nbest=nbest)
 
     @torch.no_grad()
     def align(self, xs, ys, xlen, ylen):

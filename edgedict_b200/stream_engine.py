@@ -9,6 +9,7 @@ PytorchStreamDecoder.reset/decode (reference rnnt/stream.py:78-120): at most one
 encoder frame, argmax over raw logits, predictor advanced only on non-blank.  With ``max_symbols`` = K > 1 a frame
 repeats joint -> argmax -> predictor step until a blank or K symbols (GreedyEngine likewise).
 """
+import collections
 import ctypes as C
 import functools
 import math
@@ -81,6 +82,76 @@ def check_max_symbols(max_symbols):
     if not 1 <= K <= MAX_SYMBOLS:
         raise ValueError("max_symbols must be in [1, %d], got %d" % (MAX_SYMBOLS, K))
     return K
+
+
+Hypothesis = collections.namedtuple("Hypothesis", ["tokens", "frames", "nlogp"])
+Hypothesis.__doc__ = """One entry of an N-best list (``beam_search(nbest=N)``): the non-blank token ids (int64 ndarray),
+the encoder output frame each of them entered the hypothesis at (int32 ndarray, same length) and nlogp, the negated
+score the best-only call returns for its one hypothesis."""
+
+
+def check_nbest(nbest, W):
+    """The list length N of an N-best beam search of width W, an integer in [1, W].  Raises TypeError / ValueError;
+    touches no device."""
+    if isinstance(nbest, bool) or not isinstance(nbest, numbers.Integral):
+        raise TypeError("nbest must be an integer, got %r" % (nbest,))
+    N = int(nbest)
+    if not 1 <= N <= W:
+        raise ValueError("nbest must be in [1, W = %d], got %d" % (W, N))
+    return N
+
+
+def _engine_nbest(nbest, W):
+    """An engine's nbest: 0 (the best hypothesis alone, the program as without N-best) or check_nbest's N."""
+    if isinstance(nbest, numbers.Integral) and not isinstance(nbest, bool) and nbest == 0:
+        return 0
+    return check_nbest(nbest, W)
+
+
+def final_outputs(e, B, N, L):
+    """Allocate on engine ``e`` what BEAM_FINAL writes for B utterances, ids rows of length L.  N = 0 (the best
+    hypothesis alone): e.ids int32 [B, L] and e.nlogp [B].  N >= 1: one int32 buffer ``e.nbest_out`` (one copy to the
+    host), ids | frames [B, N, L] | -log p (fp32 bits) [B, N] | count [B], with the views e.ids, e.nbest_frames,
+    e.nlogp and e.nbest_count."""
+    e.nbest = N
+    if not N:
+        e.ids = torch.zeros(B, L, dtype=torch.int32, device=e.dev)
+        e.nlogp = torch.zeros(B, dtype=torch.float32, device=e.dev)
+        e.nbest_out = e.nbest_frames = e.nbest_count = None
+        return
+    n = B * N * L
+    e.nbest_out = torch.zeros(2 * n + B * N + B, dtype=torch.int32, device=e.dev)
+    e.ids, e.nbest_frames = e.nbest_out[:n].view(B, N, L), e.nbest_out[n:2 * n].view(B, N, L)
+    e.nlogp = e.nbest_out[2 * n:2 * n + B * N].view(torch.float32).view(B, N)
+    e.nbest_count = e.nbest_out[2 * n + B * N:]
+
+
+def final_phase(e, W, y, K):
+    """The BEAM_FINAL phase of engine ``e`` (final_outputs done, e.hist from beam_history) over the slot values y, K
+    history columns per frame.  With e.nbest = 0 the N-best fields stay zero / NULL: the best-only phase."""
+    B, L = e.ids.shape[0], e.ids.shape[-1]
+    return EbPhase(type=PH_BEAM_FINAL, S=B, aux=W, aux2=e.blank, y=_ptr(y), hist=_ptr(e.hist),
+                   hist_ld=e.hist_live.shape[1], tok_out=_ptr(e.ids), ldy=L, y2=_ptr(e.nlogp), K1=e.nbest,
+                   ldw2=K if e.nbest else 0, seq_out=_ptr(e.nbest_frames), tok_out2=_ptr(e.nbest_count))
+
+
+def nbest_lists(buf, B, N, L):
+    """An engine's N-best output ``buf`` (nbest_buffer's layout, on the device) -> B lists of Hypothesis, best first,
+    each of length min(N, live slots).  One device-to-host copy."""
+    host = buf.cpu().numpy()
+    n = B * N * L
+    ids, frames = host[:n].reshape(B, N, L), host[n:2 * n].reshape(B, N, L)
+    nlogp = host[2 * n:2 * n + B * N].view("float32").reshape(B, N)
+    count = host[2 * n + B * N:]
+    out = []
+    for b in range(B):
+        hyps = []
+        for r in range(int(count[b])):
+            keep = ids[b, r] >= 0
+            hyps.append(Hypothesis(ids[b, r][keep].astype("int64"), frames[b, r][keep].astype("int32"),
+                                   float(nlogp[b, r])))
+        out.append(hyps)
+    return out
 
 
 def greedy_frame(prog, K, S, tok, blank, round_phases):
@@ -883,14 +954,16 @@ class BeamEngine:
     rows (a row that did not step gets its parent's logits bit for bit, rows being independent)."""
 
     def __init__(self, transducer, batch, t_out, W, merge=True, blank=NUL, max_ctas=0, lm=None, lm_weight=0.0,
-                 length_bonus=0.0, lm_bos=1, lm_token_map=None, max_symbols=1):
+                 length_bonus=0.0, lm_bos=1, lm_token_map=None, max_symbols=1, nbest=0):
         """``max_symbols`` = K: up to K rounds per encoder frame (Transducer.beam_search states the rule).  The history
         then has one column per round, [B, T' * K, W] (column t*K + j; a round a row did not take holds parent = slot,
         token = blank and live count 0, except the last column, which holds the final live count), and ``ids`` is
-        [B, T' * K]."""
+        [B, T' * K].  ``nbest`` = N in [1, W]: BEAM_FINAL writes the N best hypotheses with their frames into
+        ``nbest_out`` (final_outputs' layout, L = max(T' * K, 1)); 0 builds the best-only program."""
         K = check_max_symbols(max_symbols)
         if not 1 <= W <= BEAM_MAX_W:
             raise ValueError("beam width must be in [1, %d], got %r" % (BEAM_MAX_W, W))
+        N = _engine_nbest(nbest, W)
         fusion = check_lm_args(lm, transducer.joint.joint[2].weight.shape[0], lm_weight, length_bonus, lm_bos,
                                lm_token_map)
         dec, joint = transducer.decoder, transducer.joint.joint
@@ -917,7 +990,7 @@ class BeamEngine:
         self.tok, self.src, self.logp = z(R, dtype=i32), z(R, dtype=i32), z(R)
         beam_history(self, B, TK, W)
         self._slots = torch.arange(W, dtype=i32, device=self.dev)
-        self.ids, self.nlogp = z(B, max(TK, 1), dtype=i32), z(B)
+        final_outputs(self, B, N, max(TK, 1))
         self._joint = (joint[0].weight, joint[0].bias, joint[2].weight, joint[2].bias)
         prog = []
         _dec_phases(prog, dec, R, self.dec_h[0], self.dec_c[0], self.dec_htmp, self.dec_x[0], self.tok, blank,
@@ -930,8 +1003,7 @@ class BeamEngine:
                    hist=_ptr(self.hist), hist_ld=TK, **lm_sel)
         for t in range(T):
             beam_frame(prog, self, dec, t, _ptr(self.h_enc, t * E), T * E, sel, lm_step)
-        prog.append(EbPhase(type=PH_BEAM_FINAL, S=B, aux=W, aux2=blank, y=_ptr(self.logp), hist=_ptr(self.hist),
-                            hist_ld=TK, tok_out=_ptr(self.ids), ldy=self.ids.shape[1], y2=_ptr(self.nlogp)))
+        prog.append(final_phase(self, W, self.logp, K))
         self.nphase = len(prog)
         self._prog = _upload(prog, self.dev)
         self._bar = torch.zeros(64, dtype=torch.int32, device=self.dev)
@@ -940,7 +1012,8 @@ class BeamEngine:
     def run(self, h_enc, frames):
         """h_enc [B, T', E], frames int32 [B] on the device (encoder frames each utterance decodes, <= T') ->
         (ids int32 [B, max(T', 1)]: the best hypothesis' non-blank tokens right-aligned, -1 before them;
-        -log p [B] of that hypothesis, the negated fused score with an LM)."""
+        -log p [B] of that hypothesis, the negated fused score with an LM).  With ``nbest`` it returns ``nbest_out``
+        (nbest_lists reads it), rank 0 of which holds those same values."""
         self.h_enc.copy_(h_enc)
         self.frames.copy_(frames)
         beam_reset(self)
@@ -950,7 +1023,7 @@ class BeamEngine:
             self.hist_live.zero_()
             self.hist_live[:, -1] = 1                           # the live count every round reads and writes
         _launch("eb_decode_run", self._prog, self.nphase, self._bar, self.max_ctas)
-        return self.ids, self.nlogp
+        return self.nbest_out if self.nbest else (self.ids, self.nlogp)
 
 
 class StreamBeamEngine(_CommitEngine):
@@ -1116,10 +1189,11 @@ class CTCBeamEngine:
     history, where a stay is recorded as blank."""
 
     def __init__(self, batch, t_out, V, W, blank=0, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1,
-                 lm_token_map=None, max_ctas=0, device=None, frames_per_phase=0):
+                 lm_token_map=None, max_ctas=0, device=None, frames_per_phase=0, nbest=0):
         B, T, V, W, blank = (operator.index(v) for v in (batch, t_out, V, W, blank))
         if not 1 <= W <= BEAM_MAX_W:
             raise ValueError("beam width must be in [1, %d], got %d" % (BEAM_MAX_W, W))
+        N = _engine_nbest(nbest, W)
         if B < 1 or T < 1 or V < 1:
             raise ValueError("batch, t_out and V must be positive, got %d, %d, %d" % (B, T, V))
         if not 0 <= blank < V:
@@ -1143,7 +1217,7 @@ class CTCBeamEngine:
         self.seqs = z(2, R, LS, dtype=i32)           # per parity: {len, hash lo / hi, parent hash lo / hi, tokens}
         self.score, self.src = z(R), z(R, dtype=i32)
         beam_history(self, B, T, W)
-        self.ids, self.nlogp = z(B, T, dtype=i32), z(B)
+        final_outputs(self, B, N, T)
         self.lm = fusion is not None
         self._keep = []
         lm_sel, lm_step = lm_fusion(self, fusion, R) if self.lm else ({}, None)
@@ -1162,8 +1236,7 @@ class CTCBeamEngine:
                 prog.append(EbPhase(type=PH_GATHER, S=R, N=Hl, aux=2 * Ll, x1=_ptr(self.lm_state[p]),
                                     y=_ptr(self.lm_state[q]), src=_ptr(self.src)))
                 lm_step(prog, self.lm_state[q, :Ll], self.lm_state[q, Ll:], masked=True)
-        prog.append(EbPhase(type=PH_BEAM_FINAL, S=B, aux=W, aux2=blank, y=_ptr(self.score), hist=_ptr(self.hist),
-                            hist_ld=T, tok_out=_ptr(self.ids), ldy=T, y2=_ptr(self.nlogp)))
+        prog.append(final_phase(self, W, self.score, 1))
         self.nphase = len(prog)
         self._prog = _upload(prog, self.dev)
         self._bar = torch.zeros(64, dtype=torch.int32, device=self.dev)
@@ -1172,7 +1245,8 @@ class CTCBeamEngine:
     def run(self, log_probs, lengths):
         """log_probs [B, T', V] fp32 on the device (any strides), lengths int32 [B] on the device (frames each utterance
         decodes, clamped to [0, T']) -> (ids int32 [B, T']: the best prefix right-aligned, -1 before it; -score [B],
-        the negated (pb (+) pnb) + f of that prefix).  Both stay on the device."""
+        the negated (pb (+) pnb) + f of that prefix).  Both stay on the device.  With ``nbest`` it returns
+        ``nbest_out`` (nbest_lists reads it, L = T'), rank 0 of which holds those same values."""
         self.lp.copy_(log_probs)
         self.frames.copy_(lengths.clamp(0, self.T))
         self.state.zero_()
@@ -1185,7 +1259,7 @@ class CTCBeamEngine:
             self.lm_state[0].zero_()
             self.lm_tok.fill_(self.lm_bos)
         _launch("eb_decode_run_ctc", self._prog, self.nphase, self._bar, self.max_ctas)
-        return self.ids, self.nlogp
+        return self.nbest_out if self.nbest else (self.ids, self.nlogp)
 
     def hypotheses(self, b):
         """The live slots of utterance b after ``run``, in slot order: [(prefix tuple, pb, pnb, f)] on the host."""

@@ -494,7 +494,10 @@ typedef struct EbPhase {
  *            Each value is frontend.cu's expression for it, so the features equal eb_fe_* / eb_gemm_f32's bit for bit.
  * x1_div (LINEAR): row r of x1 is x1[r / x1_div] (0 or 1: row r), the encoder frame a beam's W rows share.
  * Beam search (batched, W slots per utterance, row r = b*W + slot; see decode.cu for the field use of each phase):
- * at most EB_BEAM_MAX_W slots per utterance.
+ * at most EB_BEAM_MAX_W slots per utterance.  BEAM_FINAL writes the K1 = N best live slots of each utterance (0 reads
+ * as 1: the best one alone), ranked by value descending, lowest slot on ties: ids [B*N][ldy] in tok_out, -value [B*N] in
+ * y2, and, when set, each token's frame (history column / ldw2, 0 read as 1) in seq_out and min(N, live) [B] in
+ * tok_out2.  Ranks past the count hold ids and frames -1 and +inf.
  * CTC_BEAM (CTC prefix beam search over log-probs, one CTA per utterance; see decode.cu for the field use): frames
  * hist_col .. hist_col + ldw1 - 1 in one phase; each slot carries log P(prefix, ends in blank / non-blank) and a fusion
  * term in an engine-owned state buffer (c), an extension that reaches another live slot's prefix is log-added into that
