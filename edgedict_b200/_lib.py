@@ -147,6 +147,11 @@ SIGNATURES = {
     "eb_w2v_logits_fwd": (I, [P, P, P, I, I, I, I, F, F, P, P, P, P, P, P, P]),
     "eb_w2v_logits_bwd": (I, [P, P, P, P, P, P, P, P, P, I, I, I, I, F, F, P, P, P, P, P]),
     "eb_w2v_ce": (I, [P, I, I, I, P, P, P]),
+    "eb_edit_distance_smem_bytes": (Z, [I, I, I]),
+    "eb_edit_distance": (I, [P, L, P, L, P, P, I, I, P, P, I, I, P, P]),
+    "eb_nbest_pack": (I, [P, P, I, I, I, P, I, P, P, I, P, P, P]),
+    "eb_mwer_risk_fwd": (I, [P, P, P, I, I, P, P, P, P]),
+    "eb_mwer_risk_bwd": (I, [P, P, P, I, I, P, P, P]),
     # warp-transducer compatible ABI (include/rnnt.h)
     "get_warprnnt_version": (I, []),
     "rnntGetStatusString": (C.c_char_p, [I]),

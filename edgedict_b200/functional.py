@@ -937,6 +937,59 @@ class CTCLossFn(torch.autograd.Function):
         return grad, None, None, None, None, None
 
 
+def _joint_loss_fwd(ctx, h_enc, h_dec, w1, b1, w2, b2, labels, act_lens, label_lens, blank, precision):
+    """The joint and the RNN-T loss of JointLoss / JointCosts: costs [B] of the rows, with what backward needs saved
+    on ctx."""
+    B, T, E = h_enc.shape
+    U, Dd = h_dec.shape[1], h_dec.shape[2]
+    J, V = w1.shape[0], w2.shape[0]
+    he2, hd2, ep, dp = _joint_pre(h_enc, h_dec, w1, b1, precision)
+    hid = ops.joint_hidden_fwd(ep, dp, precision == "bf16")
+    hid2 = hid.view(B * T * U, J)
+    fused = _fused_lse(precision, J, U)
+    if fused:
+        # bf16 mode: the logits GEMM epilogue also produces the softmax statistics (fp32, from the
+        # register accumulators) and writes bf16 logits; the denominator pass over 8 GB disappears
+        b2a = b2 if (b2.is_contiguous() and b2.data_ptr() % 16 == 0) else b2.clone()
+        logits, ws = ops.joint_logits_lse(hid2, ops.cast_bf16(w2.contiguous()), b2a, labels, act_lens,
+                                          label_lens, B, T, U, blank)
+        costs = ops.rnnt_lattice(act_lens, label_lens, B, T, U, ws)
+    else:
+        logits = ops.mm_nt(hid2, w2, b2, precision, x16=hid2 if precision == "bf16" else None).view(B, T, U, V)
+        costs, ws = ops.rnnt_loss_fwd(logits, labels, act_lens, label_lens, blank, need_beta=True)
+    ctx.save_for_backward(hid, he2, hd2, w1, w2, logits, labels, act_lens, label_lens, ws)
+    ctx.precision, ctx.dims, ctx.blank = precision, (B, T, U, E, Dd, J, V), blank
+    return costs
+
+
+def _joint_loss_bwd(ctx, g, host_scale, lam, node):
+    """The gradients (h_enc, h_dec, w1, b1, w2, b2) of _joint_loss_fwd's costs, each row's scaled by g (one element:
+    every row) times host_scale, written over the saved logits."""
+    hid, he2, hd2, w1, w2, logits, labels, act_lens, label_lens, ws = ctx.saved_tensors
+    if getattr(ctx, "consumed", False):
+        raise RuntimeError("%s.backward ran twice on the same graph: the gradient is written in place over "
+                           "the saved logits (retain_graph is not supported by this node)" % node)
+    ctx.consumed = True
+    B, T, U, E, Dd, J, V = ctx.dims
+    p = ctx.precision
+    db2 = None
+    if logits.dtype == bf16 and V % 8 == 0:
+        # the bias gradient comes out of the gradient kernel, which holds every d logit it writes: the output layer's
+        # side stream is left with dW2 alone
+        dl, db2 = ops.rnnt_loss_bwd_bf16_db(logits, labels, act_lens, label_lens, ctx.blank, ws, g, host_scale,
+                                            fastemit_lambda=lam)
+    elif logits.dtype == bf16:
+        dl = ops.rnnt_loss_bwd_bf16(logits, labels, act_lens, label_lens, ctx.blank, ws, g, host_scale,
+                                    fastemit_lambda=lam)
+    elif p == "bf16":
+        dl = ops.rnnt_loss_bwd(logits, labels, act_lens, label_lens, ctx.blank, ws, g, host_scale, out_bf16=True,
+                               fastemit_lambda=lam)
+    else:
+        dl = ops.rnnt_loss_bwd(logits, labels, act_lens, label_lens, ctx.blank, ws, g, host_scale, out=logits,
+                               fastemit_lambda=lam)
+    return _joint_bwd(p, dl.view(B * T * U, V), hid, he2, hd2, w1, w2, ctx.dims, db2)
+
+
 class JointLoss(torch.autograd.Function):
     """Transducer.forward's joint + loss (rnnt/models.py:234-239) as one autograd node: logits are
     produced, consumed by the loss, and their gradient is written IN PLACE over them (fp32 mode)
@@ -946,58 +999,52 @@ class JointLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, h_enc, h_dec, w1, b1, w2, b2, labels, act_lens, label_lens, blank, precision, fastemit_lambda=0.0):
         ctx.fastemit_lambda = check_fastemit_lambda(fastemit_lambda)
-        B, T, E = h_enc.shape
-        U, Dd = h_dec.shape[1], h_dec.shape[2]
-        J, V = w1.shape[0], w2.shape[0]
-        he2, hd2, ep, dp = _joint_pre(h_enc, h_dec, w1, b1, precision)
-        hid = ops.joint_hidden_fwd(ep, dp, precision == "bf16")
-        hid2 = hid.view(B * T * U, J)
-        fused = _fused_lse(precision, J, U)
-        if fused:
-            # bf16 mode: the logits GEMM epilogue also produces the softmax statistics (fp32, from the
-            # register accumulators) and writes bf16 logits; the denominator pass over 8 GB disappears
-            b2a = b2 if (b2.is_contiguous() and b2.data_ptr() % 16 == 0) else b2.clone()
-            logits, ws = ops.joint_logits_lse(hid2, ops.cast_bf16(w2.contiguous()), b2a, labels, act_lens,
-                                              label_lens, B, T, U, blank)
-            costs = ops.rnnt_lattice(act_lens, label_lens, B, T, U, ws)
-        else:
-            logits = ops.mm_nt(hid2, w2, b2, precision, x16=hid2 if precision == "bf16" else None).view(B, T, U, V)
-            costs, ws = ops.rnnt_loss_fwd(logits, labels, act_lens, label_lens, blank, need_beta=True)
-        ctx.save_for_backward(hid, he2, hd2, w1, w2, logits, labels, act_lens, label_lens, ws)
-        ctx.precision, ctx.dims, ctx.blank = precision, (B, T, U, E, Dd, J, V), blank
+        costs = _joint_loss_fwd(ctx, h_enc, h_dec, w1, b1, w2, b2, labels, act_lens, label_lens, blank, precision)
         ctx.mark_non_differentiable(costs)
-        loss = costs.sum().unsqueeze(-1) / B
+        loss = costs.sum().unsqueeze(-1) / h_enc.shape[0]
         ctx.costs = costs
         return loss, costs
 
     @staticmethod
     def backward(ctx, go, _gc):
-        hid, he2, hd2, w1, w2, logits, labels, act_lens, label_lens, ws = ctx.saved_tensors
-        if getattr(ctx, "consumed", False):
-            raise RuntimeError("JointLoss.backward ran twice on the same graph: the gradient is written in place over "
-                               "the saved logits (retain_graph is not supported by this node)")
-        ctx.consumed = True
-        B, T, U, E, Dd, J, V = ctx.dims
-        p = ctx.precision
         g = _c(go.to(f32)).view(-1)
-        lam = ctx.fastemit_lambda
-        db2 = None
-        if logits.dtype == bf16 and V % 8 == 0:
-            # the bias gradient comes out of the gradient kernel, which holds every d logit it writes: the output layer's
-            # side stream is left with dW2 alone
-            dl, db2 = ops.rnnt_loss_bwd_bf16_db(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B,
-                                                fastemit_lambda=lam)
-        elif logits.dtype == bf16:
-            dl = ops.rnnt_loss_bwd_bf16(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B,
-                                        fastemit_lambda=lam)
-        elif p == "bf16":
-            dl = ops.rnnt_loss_bwd(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B, out_bf16=True,
-                                   fastemit_lambda=lam)
-        else:
-            dl = ops.rnnt_loss_bwd(logits, labels, act_lens, label_lens, ctx.blank, ws, g, 1.0 / B, out=logits,
-                                   fastemit_lambda=lam)
-        dhe, dhd, dw1, db1, dw2, db2 = _joint_bwd(p, dl.view(B * T * U, V), hid, he2, hd2, w1, w2, ctx.dims, db2)
-        return dhe, dhd, dw1, db1, dw2, db2, None, None, None, None, None, None
+        grads = _joint_loss_bwd(ctx, g, 1.0 / ctx.dims[0], ctx.fastemit_lambda, "JointLoss")
+        return (*grads, None, None, None, None, None, None)
+
+
+class JointCosts(torch.autograd.Function):
+    """JointLoss's joint + loss with the per-row costs [B] as the differentiable output: backward hands each row's
+    upstream gradient to the loss-gradient kernel as its per-utterance scale (what minimum word error rate training
+    needs, whose rows are weighted by their posteriors).  No FastEmit: on negatively weighted rows it regularises
+    nothing."""
+
+    @staticmethod
+    def forward(ctx, h_enc, h_dec, w1, b1, w2, b2, labels, act_lens, label_lens, blank, precision):
+        return _joint_loss_fwd(ctx, h_enc, h_dec, w1, b1, w2, b2, labels, act_lens, label_lens, blank, precision)
+
+    @staticmethod
+    def backward(ctx, gcosts):
+        grads = _joint_loss_bwd(ctx, _c(gcosts.to(f32)).view(-1), 1.0, 0.0, "JointCosts")
+        return (*grads, None, None, None, None, None)
+
+
+class ExpectedRisk(torch.autograd.Function):
+    """The expected risk of N-best lists (ops.mwer_risk_fwd): costs [B, N] fp32 (-log P of each hypothesis), errors
+    and valid int32 [B, N] -> (loss [1] = mean over utterances of sum_i P_i (E_i - mean E), P the posteriors
+    renormalised over the valid ranks [B, N], not differentiable).  The gradient reaches the costs alone."""
+
+    @staticmethod
+    def forward(ctx, costs, errors, valid):
+        costs = _c(costs)
+        loss, post, _ = ops.mwer_risk_fwd(costs, errors, valid)
+        ctx.save_for_backward(costs, errors, valid)
+        ctx.mark_non_differentiable(post)
+        return loss, post
+
+    @staticmethod
+    def backward(ctx, gloss, _gpost):
+        costs, errors, valid = ctx.saved_tensors
+        return ops.mwer_risk_bwd(costs, errors, valid, gloss), None, None
 
 
 class SimpleLoss(torch.autograd.Function):

@@ -1330,3 +1330,78 @@ def w2v_ce(logits):
     out = torch.empty(2, dtype=f32, device=logits.device)
     check(lib().eb_w2v_ce(_p(logits), B, M, C, _p(grad), _p(out), _s()), "eb_w2v_ce")
     return grad, out
+
+
+# ---- minimum word error rate training (csrc/mwer.cu; include/edgedict_b200.h) ------------------------------------
+def edit_distance(hyp, ref, meta, meta_host, n_hyp, n_ref, word_table=None, word_chars=None, vocab=0):
+    """Counts [n_hyp, 5] int32 {errors, S, D, I, reference length} of hypothesis rows hyp [n_hyp, ld_h] against
+    reference rows ref [n_ref, ld_r] (int32, contiguous).  meta int32 on the device = hyp_len | ref_len | ref_index and
+    meta_host the same values in host memory (eb_edit_distance checks them); word_table [n_table, 3] / word_chars
+    int32 on the device select word units."""
+    _need(hyp, torch.int32, "hyp")
+    _need(ref, torch.int32, "ref")
+    _need(meta, torch.int32, "meta")
+    if meta_host.device.type != "cpu" or meta_host.dtype != torch.int32 or not meta_host.is_contiguous():
+        raise ValueError("meta_host must be a contiguous int32 host tensor")
+    if meta.numel() != 2 * n_hyp + n_ref or meta_host.numel() != meta.numel():
+        raise ValueError("meta must hold 2 * n_hyp + n_ref entries")
+    out = torch.empty(n_hyp, 5, dtype=torch.int32, device=hyp.device)
+    n_table = 0
+    if word_table is not None:
+        _need(word_table, torch.int32, "word_table")
+        _need(word_chars, torch.int32, "word_chars")
+        n_table = word_table.shape[0]
+    ld_h = hyp.shape[1] if hyp.dim() == 2 else 0
+    ld_r = ref.shape[1] if ref.dim() == 2 else 0
+    if n_hyp == 0:
+        return out
+    # an empty row buffer (width 0) is never read: meta stands in for its null pointer
+    with _timed("edit_distance"):
+        check(lib().eb_edit_distance(hyp.data_ptr() or _p(meta), ld_h, ref.data_ptr() or _p(meta), ld_r, _p(meta),
+                                     meta_host.data_ptr(), n_hyp, n_ref, _p(word_table),
+                                     _p(word_chars) if word_table is not None else None, n_table, vocab, _p(out), _s()),
+              "eb_edit_distance")
+    return out
+
+
+def nbest_pack(ids, count, ref, ref_len, ld_out):
+    """ids int32 [B, N, L] (a beam engine's N-best ids), count [B], ref int32 [B, S], ref_len int32 [B] -> (labels
+    int32 [B*(N+1), ld_out], lens int32 [B*(N+1)], valid int32 [B, N]) (include/edgedict_b200.h, eb_nbest_pack)."""
+    B, N, L = ids.shape
+    _need(ids, torch.int32, "ids")
+    _need(count, torch.int32, "count")
+    _need(ref, torch.int32, "ref")
+    _need(ref_len, torch.int32, "ref_len")
+    dev = ids.device
+    labels = torch.empty(B * (N + 1), ld_out, dtype=torch.int32, device=dev)
+    lens = torch.empty(B * (N + 1), dtype=torch.int32, device=dev)
+    valid = torch.empty(B, N, dtype=torch.int32, device=dev)
+    with _timed("nbest_pack"):
+        check(lib().eb_nbest_pack(_p(ids), _p(count), B, N, L, ref.data_ptr() or _p(lens), ref.shape[1], _p(ref_len),
+                                  _p(labels), ld_out, _p(lens), _p(valid), _s()), "eb_nbest_pack")
+    return labels, lens, valid
+
+
+def mwer_risk_fwd(costs, errors, valid):
+    """costs fp32 [B, N], errors / valid int32 [B, N] -> (loss [1] fp32, posteriors [B, N] fp32, risk [B] fp64)."""
+    _need(costs, f32, "costs")
+    _need(errors, torch.int32, "errors")
+    _need(valid, torch.int32, "valid")
+    B, N = costs.shape
+    post = torch.empty(B, N, dtype=f32, device=costs.device)
+    risk = torch.empty(B, dtype=torch.float64, device=costs.device)
+    loss = torch.empty(1, dtype=f32, device=costs.device)
+    with _timed("mwer_risk_fwd", 2):
+        check(lib().eb_mwer_risk_fwd(_p(costs), _p(errors), _p(valid), B, N, _p(post), _p(risk), _p(loss), _s()),
+              "eb_mwer_risk_fwd")
+    return loss, post, risk
+
+
+def mwer_risk_bwd(costs, errors, valid, gout):
+    """d loss / d costs [B, N] fp32 for the upstream gradient gout (fp32, one element, on the device)."""
+    B, N = costs.shape
+    g = gout.to(f32).reshape(1).contiguous()
+    dc = torch.empty(B, N, dtype=f32, device=costs.device)
+    with _timed("mwer_risk_bwd"):
+        check(lib().eb_mwer_risk_bwd(_p(costs), _p(errors), _p(valid), B, N, _p(g), _p(dc), _s()), "eb_mwer_risk_bwd")
+    return dc

@@ -488,6 +488,57 @@ class Transducer(nn.Module):
         ids = ids.cpu().numpy()
         return [[int(k) for k in row if k >= 0] for row in ids], nlogp.clone()
 
+    def mwer_loss(self, xs, ys, xlen, ylen, W=4, nbest=None, ce_weight=0.01, max_symbols=1, word_table=None):
+        """Minimum word error rate loss (Prabhavalkar et al., ICASSP 2018; Weng et al., Interspeech 2019 for RNN-T):
+        the expected number of errors over the N-best list of each utterance, plus ``ce_weight`` times the RNN-T loss
+        of the reference.  Takes ``forward``'s arguments and returns [1] like it.
+
+        The encoder runs as in ``forward``; the beam search (``beam_search(W, merge=True, max_symbols,
+        nbest=N)``, N = ``nbest`` or W) runs on its detached output and gives N distinct hypotheses per utterance
+        (fewer when fewer are live).  Each hypothesis' errors E_i are its edit distance to ys, in tokens, or in words with
+        ``word_table`` (mwer.word_table); its cost c_i = -log P(y_i | x) is the RNN-T loss of the hypothesis as a
+        label sequence, through the predictor and the full joint on the same encoder output.  With P_i = softmax of
+        -c_i over the utterance's hypotheses, the loss is mean_b sum_i P_i (E_i - mean E) + ce_weight * mean_b c_ref,
+        and gradients reach the encoder, the predictor and the joint through every cost (the search takes none).
+        fastemit_lambda > 0 raises ValueError, and the pruned loss's trivial joiner (``prune_range``) is not used.
+
+        ``self.last_mwer`` keeps, on the device, costs [B, N+1] (the reference last), errors [B, N], posteriors [B, N]
+        (0 past the count) and count [B].  One device-to-host copy of the label row lengths per call."""
+        from .. import mwer
+        from ..stream_engine import BeamEngine, BEAM_MAX_W, check_max_symbols, check_nbest, param_fingerprint
+        K = check_max_symbols(max_symbols)
+        W = operator.index(W)
+        if not 1 <= W <= BEAM_MAX_W:
+            raise ValueError("beam width W must be in [1, %d], got %d" % (BEAM_MAX_W, W))
+        N = W if nbest is None else check_nbest(nbest, W)
+        ce = mwer.check_ce_weight(ce_weight)
+        table = mwer.check_word_table(word_table, self.joint.joint[2].weight.shape[0])
+        if Fn.check_fastemit_lambda(self.fastemit_lambda) > 0:
+            raise ValueError("mwer_loss does not take FastEmit (fastemit_lambda > 0): its rows are weighted by signed "
+                             "risks, which FastEmit does not regularise")
+        p = _precision(self)
+        h_enc, _ = self.encoder(xs[:, :int(xlen.max())].contiguous())
+        B, T, dev = h_enc.shape[0], h_enc.shape[1], h_enc.device
+        xl = _lens_to_device(_i32(scale_length(T, xlen)), dev)
+        key = (B, T, W, K, N, dev, param_fingerprint(self))
+        cache = self.__dict__.setdefault("_mwer_engines", {})
+        eng = cache.get(key)
+        if eng is None:
+            cache.clear()                                  # one resident program is enough
+            eng = cache[key] = BeamEngine(self, B, T, W, merge=True, blank=self.blank, max_symbols=K, nbest=N)
+        with torch.no_grad():
+            buf = eng.run(h_enc.detach(), xl)
+        ylen = torch.as_tensor(ylen).reshape(-1).cpu().to(torch.int64)
+        refs = _i32(ys[:, :int(ylen.max())])
+        labels, lens, _, valid, errors, count = mwer.nbest_rows(buf, B, N, eng.ids.shape[-1], refs, ylen, table,
+                                                                self.joint.joint[2].weight.shape[0])
+        rows = torch.arange(B, device=dev).repeat_interleave(N + 1)
+        h_dec, _ = self.decoder(labels)
+        l0, l2 = self.joint.joint[0], self.joint.joint[2]
+        costs = Fn.JointCosts.apply(h_enc.index_select(0, rows), h_dec, l0.weight, l0.bias, l2.weight, l2.bias, labels,
+                                    xl.index_select(0, rows), lens, self.blank, p).view(B, N + 1)
+        return _mwer_result(self, costs, errors, valid, count, ce)
+
 
 class CTCEncoder(nn.Module):
     """rnnt/models.py:272-310: the GRU encoder stack (``model.*``) and a ``Linear(proj_size, vocab_size)`` + LogSoftmax
@@ -583,6 +634,51 @@ class CTCEncoder(nn.Module):
         from .. import ctc
         lp = self.forward(xs)
         return ctc.forced_align(lp, ys, _ctc_frames(lp.shape[1], xlen, lp.shape[0]), ylen, self.blank)
+
+    def mwer_loss(self, xs, ys, xlen, ylen, W=4, nbest=None, ce_weight=0.01, max_symbols=1, word_table=None):
+        """``Transducer.mwer_loss`` for CTC: ``forward`` gives the log-probs, the prefix beam search
+        (``beam_search(W, nbest=N)``, N = ``nbest`` or W, over min(T', scale_length(xlen)) frames) runs on them
+        detached, and each hypothesis' cost is its CTC loss (``ctc.ctc_loss(reduction='none')``) on the same log-probs
+        and frames; the loss is mean_b sum_i P_i (E_i - mean E) + ce_weight * mean_b (CTC loss of ys).  CTC takes one
+        label per frame: ``max_symbols`` must be 1.  ``self.last_mwer`` as in ``Transducer.mwer_loss``; one
+        device-to-host copy of the label row lengths per call."""
+        from .. import ctc, mwer
+        from ..stream_engine import BEAM_MAX_W, CTCBeamEngine, check_max_symbols, check_nbest
+        if check_max_symbols(max_symbols) != 1:
+            raise ValueError("CTC emits at most one label per frame: max_symbols must be 1, got %d" % max_symbols)
+        W = operator.index(W)
+        if not 1 <= W <= BEAM_MAX_W:
+            raise ValueError("beam width W must be in [1, %d], got %d" % (BEAM_MAX_W, W))
+        N = W if nbest is None else check_nbest(nbest, W)
+        ce = mwer.check_ce_weight(ce_weight)
+        V = self.tovocab[0].weight.shape[0]
+        table = mwer.check_word_table(word_table, V)
+        lp = self.forward(xs)
+        B, T, dev = lp.shape[0], lp.shape[1], lp.device
+        frames = _ctc_frames(T, xlen, B)
+        key = (B, T, V, W, N, dev)
+        cache = self.__dict__.setdefault("_mwer_engines", {})
+        eng = cache.get(key)
+        if eng is None:
+            cache.clear()                                  # one resident program is enough
+            eng = cache[key] = CTCBeamEngine(B, T, V, W, self.blank, device=dev, nbest=N)
+        with torch.no_grad():
+            buf = eng.run(lp.detach(), _lens_to_device(frames.to(torch.int32), dev))
+        ylen = torch.as_tensor(ylen).reshape(-1).cpu().to(torch.int64)
+        refs = _i32(ys[:, :int(ylen.max())])
+        labels, _, lens_h, valid, errors, count = mwer.nbest_rows(buf, B, N, T, refs, ylen, table, V)
+        rows = torch.arange(B, device=dev).repeat_interleave(N + 1)
+        costs = ctc.ctc_loss(lp.index_select(0, rows).transpose(0, 1), labels, frames.repeat_interleave(N + 1), lens_h,
+                             blank=self.blank, reduction="none").view(B, N + 1)
+        return _mwer_result(self, costs, errors, valid, count, ce)
+
+
+def _mwer_result(model, costs, errors, valid, count, ce_weight):
+    """The MWER loss [1] of costs [B, N+1] (the reference's last) and model.last_mwer."""
+    B, N = errors.shape
+    risk, post = Fn.ExpectedRisk.apply(costs[:, :N], errors, valid)
+    model.last_mwer = dict(costs=costs.detach(), errors=errors, posteriors=post, count=count)
+    return (risk + ce_weight * costs[:, N].sum() / B).reshape(1)
 
 
 def _ctc_frames(T, xlen, B):

@@ -704,6 +704,45 @@ int eb_w2v_logits_bwd(const float* dlogits, const float* cosv, const int* neg, c
                       float temp, float eps, float* A, float* AC, float* dxp, float* dyp, void* stream);
 int eb_w2v_ce(const float* logits, int B, int M, int C, float* grad, float* out, void* stream);
 
+/* Minimum word error rate training (csrc/mwer.cu).
+ * eb_edit_distance: Levenshtein distance of n_hyp pairs, one CTA each.  Hypothesis row p is hyp[p*ld_h + k] and
+ * reference row r is ref[r*ld_r + k] (int32 ids, left-aligned); meta (device) = hyp_len [n_hyp] | ref_len [n_ref] |
+ * ref_index [n_hyp] (pair p compares hypothesis p with reference ref_index[p]) and meta_host the same values in host
+ * memory, which are checked and sized before the launch.  out [n_hyp][5] int32 = {errors, substitutions, deletions,
+ * insertions, reference length}, all in units.  Units are the ids, or, with word_table [n_table][3] = {char offset,
+ * char count, class} and word_chars (code points), words: ids of class EB_WORD_DROP (and ids outside [0, n_table)) are
+ * removed, a separator adds no characters, and a word is a maximal run of characters closed by a word end (whose
+ * characters it includes), a separator or the end of the row; two words are equal iff their characters are (a hash
+ * pre-filters, the comparison is exact).  D[i][j] over the first i reference and j hypothesis units takes the diagonal
+ * step on ties, else the deletion D[i-1][j] + 1 if it is not above the insertion D[i][j-1] + 1; S, D and I are carried
+ * along the chosen predecessor.  EB_ERR_INVALID before any launch for a missing pointer, a length below 0, above its
+ * row or above EB_EDIT_MAX_UNITS, a ref_index outside [0, n_ref), or a word table with n_table < vocab (the ids the
+ * rows may hold).
+ * eb_nbest_pack: a beam engine's N-best ids [B][N][L] (right-aligned, -1 before the tokens) and count [B], and the
+ * references ref [B][ld_ref] of ref_len [B] -> labels [B*(N+1)][ld_out] left-aligned and zero-padded, lens [B*(N+1)]:
+ * row b*(N+1)+i is rank i (length 0 at or past count[b]), row b*(N+1)+N the reference; valid [B][N] = i < count[b].
+ * ld_out >= max(L, ld_ref).
+ * eb_mwer_risk_fwd: costs c [B][N] (-log P(y_i | x)), errors E [B][N], valid [B][N] (nonzero: a hypothesis), N <=
+ * EB_BEAM_MAX_W; per utterance in fp64 and rank order P_i = softmax over the valid i of -c_i (0 elsewhere), Ebar = the
+ * mean valid E, risk[b] = sum_i P_i (E_i - Ebar); post [B][N] = P (fp32), loss [1] = sum_b risk[b] / B (fp64 sum in
+ * utterance order).  eb_mwer_risk_bwd: dcosts [B][N] = -P_i ((E_i - Ebar) - risk[b]) / B * gout[0] from the same fp64
+ * values, 0 for invalid ranks: an utterance of one valid rank, or of equal errors, gives exactly 0. */
+#define EB_EDIT_MAX_UNITS 4096
+#define EB_WORD_INSIDE 0
+#define EB_WORD_END 1
+#define EB_WORD_SEP 2
+#define EB_WORD_DROP 3
+size_t eb_edit_distance_smem_bytes(int cap_h, int cap_r, int word);
+int eb_edit_distance(const int* hyp, long ld_h, const int* ref, long ld_r, const int* meta, const int* meta_host,
+                     int n_hyp, int n_ref, const int* word_table, const int* word_chars, int n_table, int vocab,
+                     int* out, void* stream);
+int eb_nbest_pack(const int* ids, const int* count, int B, int N, int L, const int* ref, int ld_ref, const int* ref_len,
+                  int* labels, int ld_out, int* lens, int* valid, void* stream);
+int eb_mwer_risk_fwd(const float* costs, const int* errors, const int* valid, int B, int N, float* post, double* risk,
+                     float* loss, void* stream);
+int eb_mwer_risk_bwd(const float* costs, const int* errors, const int* valid, int B, int N, const float* gout,
+                     float* dcosts, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
