@@ -647,6 +647,10 @@ __device__ __forceinline__ void fe_program(const EbPhase& head) {
 //     hist_ld - 1], in every round (the host sets it before the launch), and each round a row takes also records it in
 //     its own column.  A round a row does not take (frozen, its frame ended, or SKIP jumped over it) writes no history:
 //     the host fills parent = slot, token = blank beforehand.  BEAM_FINAL and BEAM_COMMIT need no change.
+//   Contextual biasing (flags 2048, BEAM_SELECT / CTC_BEAM / BEAM_FINAL; DESIGN.md 4e): ctx -> EbContext {next, delta
+//     [n_states, V], pending [n_states], state[2] [B*W]}.  A non-blank candidate of slot q adds delta[state(q), k] to its
+//     fusion term; each survivor's state goes to the other parity; BEAM_FINAL ranks by y - pending[state], the states
+//     read from parity hist_col.
 // They run one CTA per utterance (grid-strided over B).  They are __noinline__ so that their registers do not
 // count against the tensor-core phases the streaming decode spends its time in.
 constexpr int BEAM_MAX_W = EB_BEAM_MAX_W;
@@ -752,6 +756,12 @@ __device__ __forceinline__ void beam_select(const EbPhase& p, float* sm) {
     unsigned* rhist = reinterpret_cast<unsigned*>(sopen + BEAM_MAX_W);          // [256]
     int* misc = reinterpret_cast<int*>(rhist + 256);
     const float lm_weight = lm ? __ldg(p.fuse) : 0.f, length_bonus = lm ? __ldg(p.fuse + 1) : 0.f;
+    // contextual biasing (flags 2048): the slots' automaton states alternate as the sequence rows do
+    const bool cx = p.flags & 2048;
+    const int* cnext = cx ? p.ctx->next : nullptr;
+    const float* cdelta = cx ? p.ctx->delta : nullptr;
+    const int* cst_in = cx ? p.ctx->state[MULTI ? 0 : t & 1] : nullptr;
+    int* cst_out = cx ? p.ctx->state[MULTI ? 1 : (t & 1) ^ 1] : nullptr;
     for (int b = blockIdx.x; b < p.S; b += gridDim.x) {
         const long r0 = (long)b * W, h0 = ((long)b * T + col) * W;
         const int nlive = MULTI ? __ldcg(hlive + (long)b * T + T - 1)
@@ -774,6 +784,7 @@ __device__ __forceinline__ void beam_select(const EbPhase& p, float* sm) {
                     p.tok_out[r0 + s] = blank;
                     p.src[r0 + s] = (int)(r0 + s);
                     if (lm) p.tok_out2[r0 + s] = -1;
+                    if (cx) cst_out[r0 + s] = __ldcg(cst_in + r0 + s);
                 }
                 for (int s = 0; s < nlive; ++s) {
                     const int* ps = p.seq_in + (r0 + s) * LS;
@@ -791,6 +802,7 @@ __device__ __forceinline__ void beam_select(const EbPhase& p, float* sm) {
                 p.tok_out[r0 + j] = blank;
                 p.src[r0 + j] = (int)(r0 + j);
                 if (lm) p.tok_out2[r0 + j] = -1;
+                if (cx) cst_out[r0 + j] = __ldcg(cst_in + r0 + j);   // the state BEAM_FINAL reads stays current
             }
             if (tid == 0) hlive[(long)b * T + t] = nlive;
             continue;
@@ -828,15 +840,19 @@ __device__ __forceinline__ void beam_select(const EbPhase& p, float* sm) {
             }
         }
         __syncthreads();
-        // the one expression every pass ranks by
-        auto composite = [&](int q, int k, const float* x) -> unsigned long long {
+        // the one expression every pass ranks by; d = the delta row of slot q's context state
+        auto composite = [&](int q, int k, const float* x, const float* d) -> unsigned long long {
             float v = (__ldcg(x + k) - rowm[q]) - rowls[q];
-            if (lm) {
+            if (lm || cx) {
                 float f = 0.f;
                 if (k != blank) {
-                    const int j = __ldg(p.tok_map + k);
-                    f = j >= 0 ? lm_weight * ((__ldcg(p.x2 + (r0 + q) * p.ldx2 + j) - lmm[q]) - lmls[q]) + length_bonus
-                               : length_bonus;
+                    if (lm) {
+                        const int j = __ldg(p.tok_map + k);
+                        f = j >= 0 ? lm_weight * ((__ldcg(p.x2 + (r0 + q) * p.ldx2 + j) - lmm[q]) - lmls[q]) +
+                                         length_bonus
+                                   : length_bonus;
+                    }
+                    if (cx) f = lm ? f + __ldg(d + k) : __ldg(d + k);
                 }
                 v = v + f;
             }
@@ -847,6 +863,7 @@ __device__ __forceinline__ void beam_select(const EbPhase& p, float* sm) {
         auto stay = [&](int q) -> unsigned long long {
             return ((unsigned long long)order_key(rowlp[q]) << 32) | tie_key((unsigned)(q * V + blank));
         };
+        auto drow = [&](int q) -> const float* { return cx ? cdelta + (long)__ldcg(cst_in + r0 + q) * V : nullptr; };
         const int nsel = (int)min((long)W, (long)nopen * V + (nlive - nopen));
         unsigned need = nsel;
         unsigned long long prefix = 0, mask = 0;
@@ -860,8 +877,9 @@ __device__ __forceinline__ void beam_select(const EbPhase& p, float* sm) {
                     if (tid == 0 && (c & mask) == prefix) atomicAdd(&rhist[(c >> shift) & 255], 1u);
                     continue;
                 }
+                const float* d = drow(q);
                 for (int k = tid; k < V; k += nt) {
-                    const unsigned long long c = composite(q, k, x);
+                    const unsigned long long c = composite(q, k, x, d);
                     if ((c & mask) == prefix) atomicAdd(&rhist[(c >> shift) & 255], 1u);
                 }
             }
@@ -906,8 +924,9 @@ __device__ __forceinline__ void beam_select(const EbPhase& p, float* sm) {
                 }
                 continue;
             }
+            const float* d = drow(q);
             for (int k = tid; k < V; k += nt) {
-                const unsigned long long c = composite(q, k, x);
+                const unsigned long long c = composite(q, k, x, d);
                 if ((c & mask) >= prefix) {
                     const int i = atomicAdd(&misc[3], 1);
                     if (i < nsel) comp[i] = c;               // exactly nsel pass; the guard keeps smem safe regardless
@@ -1006,10 +1025,15 @@ __device__ __forceinline__ void beam_select(const EbPhase& p, float* sm) {
                 d[0] = slen[i];
                 d[1] = (int)(unsigned)shash[i];
                 d[2] = (int)(unsigned)(shash[i] >> 32);
+                if (cx) {
+                    const int cs = __ldcg(cst_in + r0 + spar[i]);
+                    cst_out[r] = k != blank ? __ldg(cnext + (long)cs * V + k) : cs;
+                }
             } else {
                 p.y[r] = -INFINITY;
                 p.tok_out[r] = blank;
                 if (lm) p.tok_out2[r] = -1;
+                if (cx) cst_out[r] = 0;
                 p.src[r] = (int)r;
                 hpar[h] = s;
                 htok[h] = blank;
@@ -1155,13 +1179,21 @@ __device__ __noinline__ void phase_beam_final(const EbPhase& p) {
     const int* htok = p.hist + BTW;
     const int* hlive = p.hist + 3 * BTW;
     if (threadIdx.x >= 32) return;                           // one warp: with the whole CTA the CTC entry spills more
+    // the ranking value: y, or with contextual biasing (flags 2048) y - pending[state], the state from parity hist_col
+    const bool cx = p.flags & 2048;
+    const float* cpend = cx ? p.ctx->pending : nullptr;
+    const int* cst = cx ? p.ctx->state[p.hist_col & 1] : nullptr;
+    auto value = [&](long r) -> float {
+        const float v = __ldcg(p.y + r);
+        return cx ? v - __ldg(cpend + __ldcg(cst + r)) : v;
+    };
     for (int b = blockIdx.x; b < p.S; b += gridDim.x) {
         const int nlive = T == 0 ? 1 : __ldcg(hlive + (long)b * T + T - 1);
         int P = 1;
         while (P < nlive) P <<= 1;
         __syncwarp();                                        // the previous utterance is done with shared memory
         for (int i = lane; i < P; i += 32)
-            comp[i] = i < nlive ? ((unsigned long long)order_key(__ldcg(p.y + (long)b * W + i)) << 32) | tie_key(i) : 0;
+            comp[i] = i < nlive ? ((unsigned long long)order_key(value((long)b * W + i)) << 32) | tie_key(i) : 0;
         __syncwarp();
         for (int kk = 2; kk <= P; kk <<= 1)                  // bitonic sort, descending
             for (int jj = kk >> 1; jj > 0; jj >>= 1) {
@@ -1195,7 +1227,7 @@ __device__ __noinline__ void phase_beam_final(const EbPhase& p) {
                     }
                     slot = __ldcg(hpar + h);
                 }
-                p.y2[row] = -__ldcg(p.y + (long)b * W + top);  // the value itself: -0 stays -0, as argmax gave it
+                p.y2[row] = -value((long)b * W + top);         // the value itself: -0 stays -0, as argmax gave it
             } else {
                 p.y2[row] = INFINITY;
             }
@@ -1241,8 +1273,9 @@ __device__ __noinline__ void phase_beam_final(const EbPhase& p) {
 // stay's repeat term and the extension rule see the real last token across a commit.  Without the flag e is -1 there,
 // which is the same thing at the start of an utterance.
 constexpr int CTC_SEQ_HEAD = 5;
-// CTC_BEAM's shared memory (2 x u64 + 11 x 32-bit arrays of BEAM_MAX_W, histogram, scalars) in the dynamic shared memory
-static_assert(BEAM_MAX_W * (2 * 8 + 11 * 4) + 256 * 4 + 8 * 4 <= (RED_FLOATS + TR * OUT_LD) * 4, "ctc beam smem");
+// CTC_BEAM's shared memory (2 x u64 + 11 x 32-bit arrays of BEAM_MAX_W, histogram, scalars, the context states) in the
+// dynamic shared memory
+static_assert(BEAM_MAX_W * (2 * 8 + 12 * 4) + 256 * 4 + 8 * 4 <= (RED_FLOATS + TR * OUT_LD) * 4, "ctc beam smem");
 
 __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
     const int W = p.aux, V = p.N, T = p.hist_ld, blank = p.aux2, LS = p.K1;
@@ -1268,7 +1301,12 @@ __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
     int* cnext = chead + BEAM_MAX_W;
     unsigned* rhist = reinterpret_cast<unsigned*>(cnext + BEAM_MAX_W);          // [256]
     int* misc = reinterpret_cast<int*>(rhist + 256);
+    int* sst = misc + 8;                                                        // context state of each slot
     const float lm_weight = lm ? __ldg(p.fuse) : 0.f, length_bonus = lm ? __ldg(p.fuse + 1) : 0.f;
+    const bool cx = p.flags & 2048;                                             // contextual biasing
+    const int* ctx_next = cx ? p.ctx->next : nullptr;
+    const float* ctx_delta = cx ? p.ctx->delta : nullptr;
+    int* const* ctx_state = cx ? p.ctx->state : nullptr;                        // parity t & 1, as c and seq_out
     for (int b = blockIdx.x; b < p.S; b += gridDim.x) {
         const long r0 = (long)b * W;
         const int frames = __ldg(p.tok_in + b);
@@ -1284,6 +1322,7 @@ __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
                     hlp[h0 + j] = __ldcg(p.y + r0 + j);
                     p.src[r0 + j] = (int)(r0 + j);
                     if (lm) p.tok_out2[r0 + j] = -1;
+                    if (cx) ctx_state[(t + 1) & 1][r0 + j] = __ldcg(ctx_state[t & 1] + r0 + j);
                 }
                 if (tid == 0) hlive[(long)b * T + t] = nlive;
                 continue;
@@ -1305,6 +1344,7 @@ __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
                 shash[q] = (unsigned)__ldcg(ps + 1) | ((unsigned long long)(unsigned)__ldcg(ps + 2) << 32);
                 se[q] = len > 0 ? __ldcg(ps + CTC_SEQ_HEAD + len - 1) : e0;
                 chead[q] = -1;
+                if (cx) sst[q] = __ldcg(ctx_state[t & 1] + r0 + q);
             }
             __syncthreads();
             // merges: the slot whose prefix is slot q2's minus its last token
@@ -1367,6 +1407,7 @@ __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
                                             length_bonus
                                       : length_bonus);
                 }
+                if (cx) f2 = f2 + __ldg(ctx_delta + (long)sst[q] * V + k);
             };
             // candidate flat index e = q*V + k; false when it merged into a live slot's stay
             auto cand = [&](long e, unsigned long long& c) -> bool {
@@ -1468,6 +1509,7 @@ __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
                     st_out[r] = pb2;
                     st_out[R + r] = pnb2;
                     st_out[2 * R + r] = f2;
+                    if (cx) ctx_state[(t + 1) & 1][r] = k == blank ? sst[q] : __ldg(ctx_next + (long)sst[q] * V + k);
                     p.y[r] = v;
                     p.src[r] = (int)(r0 + q);
                     if (lm) p.tok_out2[r] = k != blank ? __ldg(p.tok_map + k) : -1;
@@ -1478,6 +1520,7 @@ __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
                     st_out[r] = -INFINITY;
                     st_out[R + r] = -INFINITY;
                     st_out[2 * R + r] = 0.f;
+                    if (cx) ctx_state[(t + 1) & 1][r] = 0;
                     p.y[r] = -INFINITY;
                     p.src[r] = (int)r;
                     if (lm) p.tok_out2[r] = -1;

@@ -186,7 +186,7 @@ def free_beam_search():
 
 
 def beam_search(log_probs, input_lengths, beam_width, blank=0, *, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1,
-                lm_token_map=None, nbest=None):
+                lm_token_map=None, nbest=None, context=None):
     """CTC prefix beam search (Hannun et al., 2014) on the device, optionally with shallow fusion of the reference's
     LSTM language model (LMModel, or its state_dict).  ``CTCEncoder.beam_search`` states the rule.
 
@@ -209,8 +209,16 @@ def beam_search(log_probs, input_lengths, beam_width, blank=0, *, lm=None, lm_we
     ``frames`` gives each token's log-prob frame: the frame of the extension that put it into the prefix, on the path
     the history recorded (an extension merged into another prefix's stay adds no token to it), so frames are strictly
     increasing.  An utterance of length 0 gives one empty hypothesis with nlogp 0.  Still one device-to-host copy;
-    ``nbest`` is part of the engine cache key."""
+    ``nbest`` is part of the engine cache key.
+
+    Contextual biasing: ``context`` is an ``edgedict_b200.context.ContextGraph`` over the V tokens with this blank (a
+    ValueError otherwise, before any device work).  An extension of a prefix in automaton state s by c adds the
+    graph's increment delta(s, c) to the fusion term: f' = (f + LM term) + delta (f' = f + delta without an LM); a stay
+    adds nothing and keeps the state.  The final ranking and every returned score use (pb (+) pnb) + f - P(s), P(s)
+    the pending bonus of the partial match, so a phrase earns its bonus only once it completes.  An empty graph (or
+    None) gives the search without context bit for bit; the graph's fingerprint is part of the engine cache key."""
     import numbers
+    from .context import check_context, context_cache_key
     from .stream_engine import BEAM_MAX_W, CTCBeamEngine, check_lm_args, check_nbest, lm_cache_key, nbest_lists
     if not isinstance(log_probs, torch.Tensor):
         raise TypeError("log_probs must be a tensor")
@@ -237,17 +245,18 @@ def beam_search(log_probs, input_lengths, beam_width, blank=0, *, lm=None, lm_we
     if bool((il < 0).any()) or bool((il > T).any()):
         raise ValueError("input_lengths must lie in [0, T = %d], got %s" % (T, il.tolist()))
     fusion = check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map)
+    graph = check_context(context, V, blank)
     if not log_probs.is_cuda:
         raise RuntimeError("edgedict_b200 ctc beam_search needs CUDA log_probs (got a %s tensor); there is no CPU path"
                            % log_probs.device)
     dev = log_probs.device
-    key = (B, T, V, W, N, blank, dev, lm_cache_key(fusion))
+    key = (B, T, V, W, N, blank, dev, lm_cache_key(fusion), context_cache_key(graph))
     eng = _beam_engines.get(key)
     if eng is None:
         _beam_engines.clear()                                  # one resident program is enough
         eng = _beam_engines[key] = CTCBeamEngine(B, T, V, W, blank, lm=lm, lm_weight=lm_weight,
                                                  length_bonus=length_bonus, lm_bos=lm_bos, lm_token_map=lm_token_map,
-                                                 device=dev, nbest=N)
+                                                 device=dev, nbest=N, context=graph)
     lens = torch.empty(B, dtype=torch.int32, pin_memory=True)
     lens.copy_(il)
     with torch.no_grad():

@@ -407,7 +407,7 @@ class Transducer(nn.Module):
 
     @torch.no_grad()
     def beam_search(self, xs, xlen=None, W=4, merge=True, *, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1,
-                    lm_token_map=None, max_symbols=1, nbest=None):
+                    lm_token_map=None, max_symbols=1, nbest=None, context=None):
         """SURVEY 8(f) N4: beam decode.  The reference has no beam search in rnnt/ (north_star mentions one); its
         legacy v0 stack holds a batch-1 Graves-style search (models.py:121-202, with no-op `sorted(...)` calls and a
         removed `volatile=` API).  This is a time-synchronous beam under the SAME emission constraint as
@@ -456,7 +456,18 @@ class Transducer(nn.Module):
         With `merge` the frames are those of the back-pointer chain the history recorded for the surviving
         candidate, and nlogp is the merged score.  An utterance of 0 frames gives one empty hypothesis with nlogp 0.
         For the E6D2 front end, frame f starts at f * 2**len(reductions) * downsample * hop / sample_rate seconds of
-        audio, as in `align`.  Still one device-to-host copy; `nbest` is part of the engine cache key."""
+        audio, as in `align`.  Still one device-to-host copy; `nbest` is part of the engine cache key.
+
+        Contextual biasing: ``context`` is an `edgedict_b200.context.ContextGraph` over this model's V tokens (a
+        ValueError otherwise, before any device work).  A candidate that appends a non-blank k to a hypothesis in
+        automaton state s adds the graph's increment delta(s, k) to its fusion term: f = f_LM + delta (f = delta
+        without an LM), value (a + f) + logp[q] as above; blank and a closed hypothesis' stay add nothing and keep the
+        state.  During the search a value therefore holds the banked phrase bonus plus the pending bonus P(s) of the
+        partial match; the final ranking, the returned -log p and every N-best nlogp use value - P(s), so a partly
+        matched phrase earns nothing.  The state is a function of the token sequence, so merging stays exact.  An empty
+        graph (or None) gives the search without context bit for bit; the graph's fingerprint is part of the engine
+        cache key."""
+        from ..context import check_context, context_cache_key
         from ..stream_engine import (BeamEngine, BEAM_MAX_W, check_lm_args, check_max_symbols, check_nbest,
                                      lm_cache_key, nbest_lists, param_fingerprint)
         K = check_max_symbols(max_symbols)
@@ -466,6 +477,7 @@ class Transducer(nn.Module):
         N = 0 if nbest is None else check_nbest(nbest, W)
         fusion = check_lm_args(lm, self.joint.joint[2].weight.shape[0], lm_weight, length_bonus, lm_bos, lm_token_map)
         lm_key = lm_cache_key(fusion)
+        graph = check_context(context, self.joint.joint[2].weight.shape[0], self.blank)
         h_enc, _ = self.encoder(xs)
         B, T = h_enc.shape[0], h_enc.shape[1]
         if xlen is None:
@@ -474,14 +486,14 @@ class Transducer(nn.Module):
             frames = scale_length(T, xlen).clamp(max=T).to(torch.int32)
         frames = _lens_to_device(frames.cpu(), h_enc.device)
         # the phase program bakes raw weight pointers: re-homed parameters (FlatAdam, .to(), .float()) rebuild it
-        key = (B, T, W, bool(merge), K, N, h_enc.device, param_fingerprint(self), lm_key)
+        key = (B, T, W, bool(merge), K, N, h_enc.device, param_fingerprint(self), lm_key, context_cache_key(graph))
         cache = self.__dict__.setdefault("_beam_engines", {})
         eng = cache.get(key)
         if eng is None:
             cache.clear()                                  # one resident program is enough
             eng = cache[key] = BeamEngine(self, B, T, W, merge=bool(merge), blank=self.blank, lm=lm,
                                           lm_weight=lm_weight, length_bonus=length_bonus, lm_bos=lm_bos,
-                                          lm_token_map=lm_token_map, max_symbols=K, nbest=N)
+                                          lm_token_map=lm_token_map, max_symbols=K, nbest=N, context=graph)
         if N:
             return nbest_lists(eng.run(h_enc, frames), B, N, eng.ids.shape[-1])
         ids, nlogp = eng.run(h_enc, frames)
@@ -584,7 +596,7 @@ class CTCEncoder(nn.Module):
 
     @torch.no_grad()
     def beam_search(self, xs, xlen=None, W=4, *, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1, lm_token_map=None,
-                    nbest=None):
+                    nbest=None, context=None):
         """CTC prefix beam search (Hannun et al., 2014) after ``forward`` (which follows ``set_precision``), optionally
         with shallow fusion of the reference's LSTM language model.  xs [B, T, F] -> (list of B int64 id arrays, -score
         [B] on the device).  Utterance b decodes min(T', scale_length(xlen)[b]) log-prob frames (all T' when xlen is
@@ -609,9 +621,10 @@ class CTCEncoder(nn.Module):
         runs in fp32-accurate arithmetic whatever the precision setting.  lm_weight = length_bonus = 0 gives the
         result of lm=None bit for bit.  NaN log-probs are outside the contract: the search still ends and stays in
         bounds, but which hypotheses a NaN keeps is unspecified.  See ``edgedict_b200.ctc.beam_search`` (this search on
-        log-probs you already have) for the arguments, and for ``nbest``, which returns N-best lists with the log-prob
-        frame of each token."""
+        log-probs you already have) for the arguments, for ``nbest``, which returns N-best lists with the log-prob
+        frame of each token, and for ``context``, contextual biasing toward a phrase list."""
         from .. import ctc
+        from ..context import check_context
         from ..stream_engine import BEAM_MAX_W, check_lm_args, check_nbest
         W = operator.index(W)
         if not 1 <= W <= BEAM_MAX_W:
@@ -619,11 +632,12 @@ class CTCEncoder(nn.Module):
         if nbest is not None:
             check_nbest(nbest, W)
         check_lm_args(lm, self.tovocab[0].weight.shape[0], lm_weight, length_bonus, lm_bos, lm_token_map)
+        check_context(context, self.tovocab[0].weight.shape[0], self.blank)
         lp = self.forward(xs)
         B, T = lp.shape[0], lp.shape[1]
         frames = torch.full((B,), T, dtype=torch.int64) if xlen is None else _ctc_frames(T, xlen, B)
         return ctc.beam_search(lp, frames, W, self.blank, lm=lm, lm_weight=lm_weight, length_bonus=length_bonus,
-                               lm_bos=lm_bos, lm_token_map=lm_token_map, nbest=nbest)
+                               lm_bos=lm_bos, lm_token_map=lm_token_map, nbest=nbest, context=context)
 
     @torch.no_grad()
     def align(self, xs, ys, xlen, ylen):

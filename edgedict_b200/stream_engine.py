@@ -20,12 +20,13 @@ import torch
 
 from . import ops
 from ._lib import lib, check
+from .context import check_context
 from .rnnt.tokenizer import NUL, BOS, UNK
 
 PH_LN, PH_PAIR, PH_LSTM, PH_LINEAR, PH_ARGMAX, PH_COPY, PH_BEAM_SELECT, PH_GATHER, PH_BEAM_FINAL, PH_BEAM_COMMIT, \
     PH_SKIP, PH_CTC_BEAM, PH_GRU, PH_CTC_EMIT, PH_FE_FRAME, PH_FE_GEMM, PH_FE_POWER, PH_FE_LOG, PH_FE_FINISH = range(19)
-F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE, F_LM, F_STREAM, F_FLUSH, F_CONT, F_ROUNDS, F_FRONTEND = 1, 2, 4, 8, 16, 32, \
-    64, 128, 256, 512, 1024
+F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE, F_LM, F_STREAM, F_FLUSH, F_CONT, F_ROUNDS, F_FRONTEND, F_CONTEXT = 1, 2, 4, \
+    8, 16, 32, 64, 128, 256, 512, 1024, 2048
 BEAM_MAX_W = 1024                                     # EB_BEAM_MAX_W
 CTC_SEQ_HEAD = 5                                      # CTC_BEAM's token rows: {len, hash lo / hi, parent hash lo / hi}
 MAX_SYMBOLS = 16                                      # bounds the program: about (5 + L_dec) * K phases per frame
@@ -35,7 +36,7 @@ class EbPhase(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("type", "S", "K1", "K2", "N", "flags", "ldx1", "ldx2", "ldw1", "ldw2",
                                          "ldy", "aux", "aux2", "hist_ld", "hist_col", "x1_div")] + \
                [(n, C.c_void_p) for n in ("x1", "x2", "w1", "w2", "b1", "b2", "y", "y2", "c", "tok_in", "tok_out",
-                                          "hist", "seq_in", "seq_out", "src", "fuse", "tok_map", "tok_out2")]
+                                          "hist", "seq_in", "seq_out", "src", "fuse", "tok_map", "tok_out2", "ctx")]
 
 
 def _ptr(t, off=0):
@@ -126,13 +127,32 @@ def final_outputs(e, B, N, L):
     e.nbest_count = e.nbest_out[2 * n + B * N:]
 
 
-def final_phase(e, W, y, K):
+def final_phase(e, W, y, K, ctx=None):
     """The BEAM_FINAL phase of engine ``e`` (final_outputs done, e.hist from beam_history) over the slot values y, K
-    history columns per frame.  With e.nbest = 0 the N-best fields stay zero / NULL: the best-only phase."""
+    history columns per frame.  With e.nbest = 0 the N-best fields stay zero / NULL: the best-only phase.  ``ctx``
+    (context_program's fields and the parity that holds the final context states) ranks by y - pending[state]."""
     B, L = e.ids.shape[0], e.ids.shape[-1]
-    return EbPhase(type=PH_BEAM_FINAL, S=B, aux=W, aux2=e.blank, y=_ptr(y), hist=_ptr(e.hist),
-                   hist_ld=e.hist_live.shape[1], tok_out=_ptr(e.ids), ldy=L, y2=_ptr(e.nlogp), K1=e.nbest,
-                   ldw2=K if e.nbest else 0, seq_out=_ptr(e.nbest_frames), tok_out2=_ptr(e.nbest_count))
+    ph = EbPhase(type=PH_BEAM_FINAL, S=B, aux=W, aux2=e.blank, y=_ptr(y), hist=_ptr(e.hist),
+                 hist_ld=e.hist_live.shape[1], tok_out=_ptr(e.ids), ldy=L, y2=_ptr(e.nlogp), K1=e.nbest,
+                 ldw2=K if e.nbest else 0, seq_out=_ptr(e.nbest_frames), tok_out2=_ptr(e.nbest_count))
+    if ctx is not None:
+        fields, parity = ctx
+        ph.flags, ph.ctx, ph.hist_col = fields["flags"], fields["ctx"], parity
+    return ph
+
+
+def context_program(e, graph, state):
+    """Contextual biasing on beam engine ``e`` (its ``dev`` set) with the ContextGraph ``graph`` (check_context done)
+    and the per-slot automaton states ``state`` (two int32 [R] parities on the device): uploads the tables and the
+    EbContext descriptor {next, delta, pending, state[0], state[1]} and returns the fields a BEAM_SELECT / CTC_BEAM /
+    BEAM_FINAL phase reads it through.  e._ctx keeps the buffers alive."""
+    tabs = graph.to(e.dev)
+    nV = graph.n_states * graph.vocab_size
+    base = tabs.data_ptr()
+    desc = torch.tensor([base, base + 4 * nV, base + 8 * nV, state[0].data_ptr(), state[1].data_ptr()],
+                        dtype=torch.int64).to(e.dev)
+    e._ctx = (tabs, desc, state)
+    return dict(flags=F_CONTEXT, ctx=desc.data_ptr())
 
 
 def nbest_lists(buf, B, N, L):
@@ -197,14 +217,15 @@ def greedy_round(prog, e, dec, h_enc, k, j, flags, unk, logp=None):
     _dec_phases(prog, dec, S, e.dec_h, e.dec_c, e.dec_htmp, e.dec_x, e.tok, e.blank, masked=True)
 
 
-def beam_state(e, R, Ld, Hd, D, LS):
+def beam_state(e, R, Ld, Hd, D, LS, context=False):
     """Allocate on engine ``e`` (its ``dev`` set) the per-slot state of a beam search over R rows, for each parity p
     in one flat buffer ``e._home[p]``: the predictor state e._st[p] [2 Ld, R, Hd] (h of every layer, then c; views
-    e.dec_h[p] / e.dec_c[p]), its output e.dec_x[p] [R, D], the token sequences e.seqs[p] int32 [R, LS] and, with an LM
-    (``e.lm``, lm_fusion done), its state e._lst[p] [2 Ll, R, Hl] (e.lm_h[p] / e.lm_c[p]).  One COPY of e._home[1]
-    into e._home[0] moves all of it, which a round of a multi-symbol frame needs (beam_frame)."""
+    e.dec_h[p] / e.dec_c[p]), its output e.dec_x[p] [R, D], the token sequences e.seqs[p] int32 [R, LS], with an LM
+    (``e.lm``, lm_fusion done) its state e._lst[p] [2 Ll, R, Hl] (e.lm_h[p] / e.lm_c[p]) and with ``context`` the
+    context automaton states e.ctx_state[p] int32 [R] (else None).  One COPY of e._home[1] into e._home[0] moves all
+    of it, which a round of a multi-symbol frame needs (beam_frame)."""
     Ll, _, Hl = e.lm_htmp.shape if e.lm else (0, 0, 0)
-    sizes = [2 * Ld * R * Hd, R * D, R * LS, 2 * Ll * R * Hl]
+    sizes = [2 * Ld * R * Hd, R * D, R * LS, 2 * Ll * R * Hl, R if context else 0]
     offs = [0]
     for n in sizes:
         offs.append(offs[-1] + -(-n // 64) * 64)           # 256-byte aligned segments
@@ -218,6 +239,7 @@ def beam_state(e, R, Ld, Hd, D, LS):
     e._lst = [seg(p, 3).view(2 * Ll, R, Hl) for p in (0, 1)] if Ll else None
     if Ll:
         e.lm_h, e.lm_c = [s[:Ll] for s in e._lst], [s[Ll:] for s in e._lst]
+    e.ctx_state = [seg(p, 4).view(torch.int32) for p in (0, 1)] if context else None
 
 
 def beam_history(e, B, T, W):
@@ -237,6 +259,8 @@ def beam_reset(e):
     LM state primed with lm_bos."""
     e._st[0].zero_()
     e.seqs[0].zero_()
+    if e.ctx_state is not None:
+        e.ctx_state[0].zero_()                                  # every slot at the automaton's root
     e.logp.fill_(float("-inf"))
     e.logp.view(-1, e.W)[:, 0] = 0.0
     e.tok.fill_(BOS)
@@ -951,10 +975,15 @@ class BeamEngine:
     values (shallow fusion, decode.cu flag 32): each slot carries an LM state ``lm_h`` / ``lm_c`` (two parities, like
     the predictor's), primed with ``lm_bos`` and stepped with ``lm_token_map[k]`` only when the slot emitted a
     non-blank token k the LM scores; after the predictor step, the LM's output Linear recomputes ``lm_logits`` for all
-    rows (a row that did not step gets its parent's logits bit for bit, rows being independent)."""
+    rows (a row that did not step gets its parent's logits bit for bit, rows being independent).
+
+    With ``context`` (a ContextGraph over the transducer's V tokens, edgedict_b200.context) each slot carries its
+    phrase-automaton state (``ctx_state``, two parities beside the token sequences) and BEAM_SELECT adds the
+    automaton's increment to every non-blank candidate's fusion term (decode.cu flag 2048); BEAM_FINAL ranks by the
+    value minus the pending bonus of the slot's state.  An empty graph builds the program without context."""
 
     def __init__(self, transducer, batch, t_out, W, merge=True, blank=NUL, max_ctas=0, lm=None, lm_weight=0.0,
-                 length_bonus=0.0, lm_bos=1, lm_token_map=None, max_symbols=1, nbest=0):
+                 length_bonus=0.0, lm_bos=1, lm_token_map=None, max_symbols=1, nbest=0, context=None):
         """``max_symbols`` = K: up to K rounds per encoder frame (Transducer.beam_search states the rule).  The history
         then has one column per round, [B, T' * K, W] (column t*K + j; a round a row did not take holds parent = slot,
         token = blank and live count 0, except the last column, which holds the final live count), and ``ids`` is
@@ -966,6 +995,7 @@ class BeamEngine:
         N = _engine_nbest(nbest, W)
         fusion = check_lm_args(lm, transducer.joint.joint[2].weight.shape[0], lm_weight, length_bonus, lm_bos,
                                lm_token_map)
+        graph = check_context(context, transducer.joint.joint[2].weight.shape[0], blank)
         dec, joint = transducer.decoder, transducer.joint.joint
         self.dev = dec.embed.weight.device
         if self.dev.type != "cuda":
@@ -985,7 +1015,7 @@ class BeamEngine:
         self.lm = fusion is not None
         lm_sel, lm_step = lm_fusion(self, fusion, R) if self.lm else ({}, None)
         # per parity: predictor state, its output, {len, hash lo, hash hi, tokens} per row and the LM state
-        beam_state(self, R, Ld, Hd, D, TK + 3)
+        beam_state(self, R, Ld, Hd, D, TK + 3, context=graph is not None)
         self.dec_htmp, self.hidden, self.logits = z(Ld, R, Hd), z(R, J), z(R, V)
         self.tok, self.src, self.logp = z(R, dtype=i32), z(R, dtype=i32), z(R)
         beam_history(self, B, TK, W)
@@ -1001,9 +1031,14 @@ class BeamEngine:
                    flags=(F_MERGE if merge else 0) | (F_LM if self.lm else 0), x1=_ptr(self.logits), ldx1=V,
                    y=_ptr(self.logp), tok_in=_ptr(self.frames), tok_out=_ptr(self.tok), src=_ptr(self.src),
                    hist=_ptr(self.hist), hist_ld=TK, **lm_sel)
+        ctx = None
+        if graph is not None:
+            cf = context_program(self, graph, self.ctx_state)
+            sel.update(flags=sel["flags"] | cf["flags"], ctx=cf["ctx"])
+            ctx = (cf, T & 1 if K == 1 else 0)                 # where the last frame left the states (beam_frame)
         for t in range(T):
             beam_frame(prog, self, dec, t, _ptr(self.h_enc, t * E), T * E, sel, lm_step)
-        prog.append(final_phase(self, W, self.logp, K))
+        prog.append(final_phase(self, W, self.logp, K, ctx))
         self.nphase = len(prog)
         self._prog = _upload(prog, self.dev)
         self._bar = torch.zeros(64, dtype=torch.int32, device=self.dev)
@@ -1186,10 +1221,14 @@ class CTCBeamEngine:
     is one CTC_BEAM phase, the GATHER of the LM state by parent and the masked LM step and output Linear
     (predictor_phases resting on -1, as BeamEngine's LM), after a priming step on ``lm_bos``; frames_per_phase must
     then be 0 or 1.  BEAM_FINAL picks the best live slot by (pb (+) pnb) + f, lowest slot on ties, and walks the
-    history, where a stay is recorded as blank."""
+    history, where a stay is recorded as blank.
+
+    With ``context`` (a ContextGraph over V tokens) each slot carries its phrase-automaton state (``ctx_state``
+    [2, R], parity t & 1 as ``state``), an extension by c adds the automaton's increment to f', and BEAM_FINAL ranks
+    by (pb (+) pnb) + f minus the pending bonus of the slot's state.  An empty graph builds the program without it."""
 
     def __init__(self, batch, t_out, V, W, blank=0, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1,
-                 lm_token_map=None, max_ctas=0, device=None, frames_per_phase=0, nbest=0):
+                 lm_token_map=None, max_ctas=0, device=None, frames_per_phase=0, nbest=0, context=None):
         B, T, V, W, blank = (operator.index(v) for v in (batch, t_out, V, W, blank))
         if not 1 <= W <= BEAM_MAX_W:
             raise ValueError("beam width must be in [1, %d], got %d" % (BEAM_MAX_W, W))
@@ -1201,6 +1240,7 @@ class CTCBeamEngine:
         if W * V >= 2 ** 31:
             raise ValueError("beam width x vocabulary must stay below 2^31 (flat candidate index), got %d x %d" % (W, V))
         fusion = check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map)
+        graph = check_context(context, V, blank)
         n = operator.index(frames_per_phase)
         if n < 0 or (fusion is not None and n > 1):
             raise ValueError("frames_per_phase must be >= 0 (0: all), and 0 or 1 with an lm; got %d" % n)
@@ -1225,6 +1265,12 @@ class CTCBeamEngine:
         sel = dict(type=PH_CTC_BEAM, S=B, N=V, aux=W, aux2=blank, K1=LS, flags=F_LM if self.lm else 0,
                    x1=_ptr(self.lp), tok_in=_ptr(self.frames), c=_ptr(self.state), seq_out=_ptr(self.seqs),
                    y=_ptr(self.score), src=_ptr(self.src), hist=_ptr(self.hist), hist_ld=T, **lm_sel)
+        ctx, self.ctx_state = None, None
+        if graph is not None:
+            self.ctx_state = z(2, R, dtype=i32)          # per parity: the automaton state of each slot
+            cf = context_program(self, graph, self.ctx_state)
+            sel.update(flags=sel["flags"] | cf["flags"], ctx=cf["ctx"])
+            ctx = (cf, T & 1)                            # frozen frames carry the states, so frame T-1 wrote them
         if self.lm:
             Ll, _, Hl = self.lm_htmp.shape
             self.lm_state = z(2, 2 * Ll, R, Hl)      # per parity: h of every layer, then c
@@ -1236,7 +1282,7 @@ class CTCBeamEngine:
                 prog.append(EbPhase(type=PH_GATHER, S=R, N=Hl, aux=2 * Ll, x1=_ptr(self.lm_state[p]),
                                     y=_ptr(self.lm_state[q]), src=_ptr(self.src)))
                 lm_step(prog, self.lm_state[q, :Ll], self.lm_state[q, Ll:], masked=True)
-        prog.append(final_phase(self, W, self.score, 1))
+        prog.append(final_phase(self, W, self.score, 1, ctx))
         self.nphase = len(prog)
         self._prog = _upload(prog, self.dev)
         self._bar = torch.zeros(64, dtype=torch.int32, device=self.dev)
@@ -1255,6 +1301,8 @@ class CTCBeamEngine:
         self.score.fill_(float("-inf"))
         self.score.view(self.B, self.W)[:, 0] = 0.0
         self.seqs[0].zero_()
+        if self.ctx_state is not None:
+            self.ctx_state[0].zero_()
         if self.lm:
             self.lm_state[0].zero_()
             self.lm_tok.fill_(self.lm_bos)

@@ -433,6 +433,15 @@ enum { EB_PH_LN = 0, EB_PH_PAIR = 1, EB_PH_LSTM = 2, EB_PH_LINEAR = 3, EB_PH_ARG
        EB_PH_BEAM_SELECT = 6, EB_PH_GATHER = 7, EB_PH_BEAM_FINAL = 8, EB_PH_BEAM_COMMIT = 9, EB_PH_SKIP = 10,
        EB_PH_CTC_BEAM = 11, EB_PH_GRU = 12, EB_PH_CTC_EMIT = 13, EB_PH_FE_FRAME = 14, EB_PH_FE_GEMM = 15,
        EB_PH_FE_POWER = 16, EB_PH_FE_LOG = 17, EB_PH_FE_FINISH = 18 };
+/* The phrase automaton of contextual biasing (flag 2048; edgedict_b200/context.py builds it): dense tables over
+ * n_states states and the N tokens of the phase, and the automaton state of every slot [B*W] in two parities, beside
+ * the token sequences. */
+typedef struct EbContext {
+    const int32_t* next;      /* [n_states, N]: the state after a non-blank token */
+    const float* delta;       /* [n_states, N]: the increment a non-blank token adds to a candidate's value */
+    const float* pending;     /* [n_states]: boost * the state's length, what BEAM_FINAL takes back */
+    int32_t* state[2];        /* per-slot state, parity 0 / 1 */
+} EbContext;
 typedef struct EbPhase {
     int32_t type, S, K1, K2, N, flags, ldx1, ldx2, ldw1, ldw2, ldy, aux, aux2, hist_ld, hist_col, x1_div;
     const float *x1, *x2, *w1, *w2, *b1, *b2;
@@ -445,6 +454,7 @@ typedef struct EbPhase {
     const float* fuse;
     const int32_t* tok_map;
     int32_t* tok_out2;
+    const EbContext* ctx;
 } EbPhase;
 /* flags: 1 = tanh epilogue (LINEAR); 2 = x1 rows are embedding rows indexed by tok_in, a negative token reading as a
  *            zero row (LSTM);
@@ -470,6 +480,12 @@ typedef struct EbPhase {
  *            candidate, its stay (value log p, flat index slot*N + blank); a non-blank token at j = K-1 closes; only
  *            hypotheses of equal closedness merge; the live count lives in the last history column; a row with no open
  *            slot (or frozen) keeps its beam and writes no history.
+ *     2048 = contextual biasing (BEAM_SELECT, CTC_BEAM, BEAM_FINAL): ctx points to an EbContext.  A candidate that
+ *            appends a non-blank token k to slot q adds delta[state(q), k] to its value (BEAM_SELECT: inside the fusion
+ *            term f, for k != blank; CTC_BEAM: to the extension's f'), and each survivor's state (next[state(q), k], or
+ *            state(q) for blank, a stay or a frozen frame) is written to the other parity: BEAM_SELECT reads parity
+ *            t & 1 (parity 0 under flag 512), CTC_BEAM parity t & 1, as their sequence rows.  BEAM_FINAL ranks and writes
+ *            y - pending[state] with the state from parity hist_col.
  * SKIP (no flags, writes nothing, no grid barrier): when no row of tok_in[0..S) differs from aux2 (blank), every CTA
  * jumps over the next aux phases.  It reads only data final at the preceding barrier, so all CTAs take the same branch.
  * BEAM_COMMIT (streaming beam, after a chunk's last frame, one CTA per stream): commits the common prefix of the live
