@@ -647,10 +647,11 @@ __device__ __forceinline__ void fe_program(const EbPhase& head) {
 //     hist_ld - 1], in every round (the host sets it before the launch), and each round a row takes also records it in
 //     its own column.  A round a row does not take (frozen, its frame ended, or SKIP jumped over it) writes no history:
 //     the host fills parent = slot, token = blank beforehand.  BEAM_FINAL and BEAM_COMMIT need no change.
-//   Contextual biasing (flags 2048, BEAM_SELECT / CTC_BEAM / BEAM_FINAL; DESIGN.md 4e): ctx -> EbContext {next, delta
-//     [n_states, V], pending [n_states], state[2] [B*W]}.  A non-blank candidate of slot q adds delta[state(q), k] to its
-//     fusion term; each survivor's state goes to the other parity; BEAM_FINAL ranks by y - pending[state], the states
-//     read from parity hist_col.
+//   Contextual biasing (flags 2048, BEAM_SELECT / CTC_BEAM / BEAM_FINAL / BEAM_COMMIT; DESIGN.md 4e): ctx -> EbContext
+//     {next, delta [n_states, V], pending [n_states], state[2] [B*W]}.  A non-blank candidate of slot q adds
+//     delta[state(q), k] to its fusion term; each survivor's state goes to the other parity; BEAM_FINAL ranks by
+//     y - pending[state], the states read from parity hist_col; BEAM_COMMIT reads the states from parity 1, collapses
+//     by y - pending[state] and writes them, moved by src, to parity 0.
 // They run one CTA per utterance (grid-strided over B).  They are __noinline__ so that their registers do not
 // count against the tensor-core phases the streaming decode spends its time in.
 constexpr int BEAM_MAX_W = EB_BEAM_MAX_W;
@@ -1087,12 +1088,16 @@ __device__ __noinline__ void phase_gather(const EbPhase& p) {
 // (identity without a collapse), tok_out2[b] the committed count and tok_out2[S + b] whether the beam collapsed.  The
 // row head (K2) is copied unchanged: the hashes describe the whole sequence, committed part included.  With y2, the last
 // token committed is kept per stream: a CTC slot whose stored suffix is empty takes it as its last token.
+// Contextual biasing (flags 2048): the slots' automaton states are read from ctx->state[1], a collapse ranks by
+// y - pending[state] (BEAM_FINAL's value and tie rule; the kept slot keeps its y and its state), and each slot's state
+// moves to ctx->state[0] by the same gather sources as the rest of its state.
 __device__ __noinline__ void phase_beam_commit(const EbPhase& p, float* sm) {
     const int W = p.aux, T = p.hist_ld, LS = p.K1, HEAD = p.K2 > 0 ? p.K2 : 3;
     int* last = reinterpret_cast<int*>(p.y2);
     const int tid = threadIdx.x, nt = blockDim.x;
     int* hlive = p.hist + 3 * (long)p.S * T * W;
     int* misc = reinterpret_cast<int*>(sm);
+    const bool cx = p.flags & 2048;
     for (int b = blockIdx.x; b < p.S; b += gridDim.x) {
         const long r0 = (long)b * W;
         const int nlive = __ldcg(hlive + (long)b * T + T - 1);
@@ -1122,7 +1127,8 @@ __device__ __noinline__ void phase_beam_commit(const EbPhase& p, float* sm) {
             float best = -INFINITY;
             int bi = -1;
             for (int j = tid; j < nlive; j += 32) {
-                const float v = __ldcg(p.y + r0 + j);
+                float v = __ldcg(p.y + r0 + j);
+                if (cx) v = v - __ldg(p.ctx->pending + __ldcg(p.ctx->state[1] + r0 + j));
                 if (bi < 0 || v > best) { best = v; bi = j; }
             }
 #pragma unroll
@@ -1133,7 +1139,7 @@ __device__ __noinline__ void phase_beam_commit(const EbPhase& p, float* sm) {
             }
             if (tid == 0) {
                 misc[2] = bi;
-                misc[3] = __float_as_int(best);
+                misc[3] = __float_as_int(cx && bi >= 0 ? __ldcg(p.y + r0 + bi) : best);   // the kept slot's y
             }
         }
         __syncthreads();
@@ -1152,6 +1158,7 @@ __device__ __noinline__ void phase_beam_commit(const EbPhase& p, float* sm) {
         for (int s = tid; s < W; s += nt) {
             p.src[r0 + s] = (int)(r0 + (s == 0 ? best : s));
             if (collapse) p.y[r0 + s] = s == 0 ? __int_as_float(misc[3]) : -INFINITY;
+            if (cx) p.ctx->state[0][r0 + s] = __ldcg(p.ctx->state[1] + r0 + (s == 0 ? best : s));
         }
         if (tid == 0) {
             p.tok_out2[b] = ncommit;

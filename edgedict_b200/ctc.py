@@ -279,7 +279,10 @@ class CTCStreamDecoder:
     the common prefix of all live prefixes that became final in it, never revised; ``flush()`` returns the rest of the
     best prefix, and decoding goes on from it.  ``lm``, ``lm_weight``, ``length_bonus``, ``lm_bos`` and
     ``lm_token_map`` fuse the reference's LSTM LM as ``CTCEncoder.beam_search`` does; ``max_pending`` bounds the
-    uncommitted tokens a prefix may hold before the beam collapses to its best prefix.
+    uncommitted tokens a prefix may hold before the beam collapses to its best prefix.  ``context`` (an
+    edgedict_b200.context.ContextGraph over the model's vocabulary and blank; beam search only) biases the search as
+    in ``CTCEncoder.beam_search``: each prefix carries its phrase-automaton state across chunks and commits, and the
+    text of ``decode`` plus ``flush`` is that of the offline biased best prefix.
 
     ``transform`` maps a chunk of audio to log-mel features [1, F, n] (the reference's feature transform), on the host
     before each chunk; when it is build_batch_transform's test module (a BatchTransform), ``decode`` uploads the
@@ -292,8 +295,9 @@ class CTCStreamDecoder:
     work."""
 
     def __init__(self, model, transform, tokenizer, device="cuda", frames_per_chunk=None, *, beam_width=None, lm=None,
-                 lm_weight=0.0, length_bonus=0.0, lm_bos=1, lm_token_map=None, max_pending=64):
+                 lm_weight=0.0, length_bonus=0.0, lm_bos=1, lm_token_map=None, max_pending=64, context=None):
         import numbers
+        from .context import check_context
         from .rnnt.models import CTCEncoder
         from .stream_engine import BEAM_MAX_W, check_lm_args, check_stream_shape
         if not isinstance(model, CTCEncoder):
@@ -308,15 +312,18 @@ class CTCStreamDecoder:
             if W * V >= 2 ** 31:
                 raise ValueError("beam_width x V must stay below 2^31, got %d x %d" % (W, V))
             check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map)
+            check_context(context, V, model.blank)
             P = operator.index(max_pending)
             if frames_per_chunk is not None:
                 _, _, T = check_stream_shape(model.model, 1, frames_per_chunk)
                 if P < T:
                     raise ValueError("max_pending (%d) must be at least the encoder frames per chunk (%d)" % (P, T))
             self._beam = dict(W=W, lm=lm, lm_weight=lm_weight, length_bonus=length_bonus, lm_bos=lm_bos,
-                              lm_token_map=lm_token_map, max_pending=P)
+                              lm_token_map=lm_token_map, max_pending=P, context=context)
         elif lm is not None or lm_weight != 0.0 or length_bonus != 0.0 or lm_token_map is not None:
             raise ValueError("lm, lm_weight, length_bonus and lm_token_map need beam_width")
+        elif context is not None:
+            raise ValueError("context needs beam_width: greedy decoding has no contextual biasing")
         self.device = torch.device(device)
         self.transform, self.tokenizer = transform, tokenizer
         model.eval()

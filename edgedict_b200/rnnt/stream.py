@@ -23,6 +23,7 @@ import torch
 from .features import BatchTransform
 from .models import ResLayerNormGRU, Transducer, convert_lightning2normal
 from .tokenizer import NUL, BOS, UNK
+from ..context import check_context
 from ..stream_engine import BEAM_MAX_W, GRUStreamBeamEngine, GRUStreamEngine, StreamBeamEngine, StreamEngine, \
     check_lm_args, check_max_symbols, param_fingerprint
 
@@ -51,6 +52,12 @@ class PytorchStreamDecoder(StreamTransducerDecoder):
     best hypothesis of Transducer.beam_search over the same encoder frames.  The beam does not apply the reference's
     ``<unk>`` rule, which belongs to greedy argmax decoding; Transducer.beam_search does not apply it either.
 
+    ``context`` (an edgedict_b200.context.ContextGraph over the transducer's vocabulary, blank NUL; beam search only)
+    biases the streaming beam towards its phrases, as Transducer.beam_search(context=...) biases the offline one: each
+    hypothesis carries its phrase-automaton state across chunks and commits, so a phrase may straddle them, and the text
+    of ``decode`` plus ``flush`` is that of the offline biased best hypothesis over the same encoder frames.  Every
+    rebuilt engine (another chunk length, moved weights) takes the same graph and the carried states.
+
     ``max_symbols`` = K (1 to 16, greedy decoding only) lets each encoder frame emit up to K symbols: the frame repeats
     joint -> argmax (with the ``<unk>`` rule) -> predictor step until a blank or K non-blank tokens.
 
@@ -62,10 +69,12 @@ class PytorchStreamDecoder(StreamTransducerDecoder):
 
     def __init__(self, FLAGS, transducer=None, transform=None, tokenizer=None, device="cuda",
                  frames_per_chunk=None, input_size=None, *, beam_width=None, merge=True, lm=None, lm_weight=0.0,
-                 length_bonus=0.0, lm_bos=1, lm_token_map=None, max_pending=64, max_symbols=1):
+                 length_bonus=0.0, lm_bos=1, lm_token_map=None, max_pending=64, max_symbols=1, context=None):
         self._max_symbols = check_max_symbols(max_symbols)
         if beam_width is not None and self._max_symbols != 1:
             raise ValueError("max_symbols > 1 is a greedy decoding option; the beam search emits one symbol per frame")
+        if beam_width is None and context is not None:
+            raise ValueError("context needs beam_width: greedy decoding has no contextual biasing")
         self.FLAGS = FLAGS
         self.device = torch.device(device)
         if tokenizer is None:
@@ -112,8 +121,10 @@ class PytorchStreamDecoder(StreamTransducerDecoder):
             if not 1 <= W <= BEAM_MAX_W:
                 raise ValueError("beam_width must be in [1, %d], got %d" % (BEAM_MAX_W, W))
             check_lm_args(lm, transducer.joint.joint[2].weight.shape[0], lm_weight, length_bonus, lm_bos, lm_token_map)
+            check_context(context, transducer.joint.joint[2].weight.shape[0], NUL)
             self._beam = dict(W=W, merge=bool(merge), lm=lm, lm_weight=lm_weight, length_bonus=length_bonus,
-                              lm_bos=lm_bos, lm_token_map=lm_token_map, max_pending=operator.index(max_pending))
+                              lm_bos=lm_bos, lm_token_map=lm_token_map, max_pending=operator.index(max_pending),
+                              context=context)
         self._engine = None
         self._frames = frames_per_chunk
         self.reset_profile()

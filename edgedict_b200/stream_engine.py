@@ -612,7 +612,7 @@ class _ChunkEngine:
     S)[0]`` gives.  frames_per_chunk then follows from L (None, or the same count).  No front-end state is carried
     between chunks: each window is transformed on its own, as the reference streams overlapping windows."""
     GRU = False          # the encoder kind: ResLayerNormGRU cells, carrying enc_h alone, or ResLayerNormLSTM cells
-    HOST_STATE = ()      # keys of state() that are host tensors, outside _state_views
+    HOST_STATE = ()      # keys of state() kept on the host, outside _state_views
 
     @functools.cached_property
     def RUN(self):
@@ -743,8 +743,25 @@ class _CommitEngine(_ChunkEngine):
     commits each stream's common prefix with BEAM_COMMIT (``_chunk_end``, which each engine appends for its own state),
     the flush and re-bound programs built from it, and the host bookkeeping of committed tokens: ``step`` / ``flush``
     return them, ``state()`` carries those not yet returned, and ``load_state`` re-bounds the carried beam.  The beam
-    rests in the parity-0 buffers between launches; ``logp`` [S*W] is the value BEAM_COMMIT collapses by."""
-    HOST_STATE = ("unreturned_ids", "unreturned_counts")
+    rests in the parity-0 buffers between launches; ``logp`` [S*W] is the value BEAM_COMMIT collapses by.
+
+    With contextual biasing (``_context``) each slot's phrase-automaton state ``ctx_state`` (two parities) rides along:
+    the chunk end copies it beside the rest of the beam, BEAM_COMMIT collapses by logp - pending[state] and moves it
+    with its slot, ``flush`` reports that value, and ``state()`` carries it with the graph's fingerprint."""
+    UNRETURNED = ("unreturned_ids", "unreturned_counts")
+    HOST_STATE = UNRETURNED
+    _graph = _cf = None          # the ContextGraph and context_program's fields, with contextual biasing
+
+    def _context(self, graph, sel):
+        """Contextual biasing with the checked ContextGraph ``graph`` (None: none), the slot states ``ctx_state`` already
+        allocated: uploads the tables and adds the flag and descriptor to the search phase's fields ``sel``.  The chunk
+        end's BEAM_COMMIT then reads them too (_commit_phase), and state() gains the key ``context``."""
+        if graph is None:
+            return
+        self._graph, self._cf = graph, context_program(self, graph, self.ctx_state)
+        self._pending = torch.from_numpy(graph.pending).to(self.dev)
+        sel.update(flags=sel["flags"] | F_CONTEXT, ctx=self._cf["ctx"])
+        self.HOST_STATE = self.UNRETURNED + ("context",)
 
     def _chunk_end(self, pr, in_parity0, flush):
         """Append the chunk end to ``pr``: commit (and collapse) from parity 1 into parity 0, the state found in parity 0
@@ -762,10 +779,13 @@ class _CommitEngine(_ChunkEngine):
         """BEAM_COMMIT of every stream from parity 1 into parity 0, for chunks that add up to ``n_add`` tokens to a
         hypothesis; ``kw`` adds the row head (K2) and the last-token buffer (y2) of CTC rows."""
         S, P = self.S, self.max_pending
+        if self._cf is not None:                 # the automaton states: parity 1 in, parity 0 out
+            kw.update(ctx=self._cf["ctx"])
         return EbPhase(type=PH_BEAM_COMMIT, S=S, N=P, aux=self.W, aux2=P - n_add, K1=self.seqs[0].shape[1],
-                       flags=F_FLUSH if flush else 0, y=_ptr(self.logp), hist=_ptr(self.hist),
-                       hist_ld=self.hist_live.shape[1], seq_in=_ptr(self.seqs[1]), seq_out=_ptr(self.seqs[0]),
-                       tok_out=_ptr(self._out), tok_out2=_ptr(self._out, S * P), src=_ptr(self.src), **kw)
+                       flags=(F_FLUSH if flush else 0) | (F_CONTEXT if self._cf is not None else 0), y=_ptr(self.logp),
+                       hist=_ptr(self.hist), hist_ld=self.hist_live.shape[1], seq_in=_ptr(self.seqs[1]),
+                       seq_out=_ptr(self.seqs[0]), tok_out=_ptr(self._out), tok_out2=_ptr(self._out, S * P),
+                       src=_ptr(self.src), **kw)
 
     def _commit_programs(self, prog, in_parity0):
         """Close the chunk program ``prog`` with the chunk end (the frames left the state in parity 0 when
@@ -787,16 +807,46 @@ class _CommitEngine(_ChunkEngine):
         ``step`` (host ids [S, K] and counts [S])."""
         st = super().state()
         st["unreturned_ids"], st["unreturned_counts"] = (t.clone() for t in self._unreturned)
+        if self._graph is not None:
+            st["context"] = self._graph.fingerprint
         return st
+
+    def _check_context_state(self, st):
+        """ValueError, before any device work, for a state carried with another context graph, with or without
+        contextual biasing where this engine differs, or with a live slot's automaton state outside [0, n_states)."""
+        mine, theirs = (self._graph.fingerprint if self._graph is not None else None), st.get("context")
+        if (mine is None) != (theirs is None):
+            raise ValueError("the state was carried %s contextual biasing and this engine decodes %s it; build the "
+                             "engine with the same context" % (("with", "without") if mine is None else
+                                                               ("without", "with")))
+        if mine is None:
+            return
+        if theirs != mine:
+            raise ValueError("the state was carried with another context graph (fingerprint %s, this engine's %s): "
+                             "build a new engine and reset() to change the phrases" % (theirs, mine))
+        cs, live = st.get("ctx_state"), st.get("live")
+        if not isinstance(cs, torch.Tensor) or not isinstance(live, torch.Tensor) or \
+                tuple(cs.shape) != (self.R,) or tuple(live.shape) != (self.S,):
+            return                                       # the key and shape checks of load_state refuse it
+        cs = cs.to("cpu", torch.int64).view(self.S, self.W)
+        used = torch.arange(self.W)[None, :] < live.to("cpu", torch.int64)[:, None]
+        bad = used & ((cs < 0) | (cs >= self._graph.n_states))
+        if bool(bad.any()):
+            s, j = (int(v) for v in bad.nonzero()[0])
+            raise ValueError("state ctx_state: live slot %d of stream %d holds automaton state %d, outside [0, %d)"
+                             % (j, s, int(cs[s, j]), self._graph.n_states))
 
     @torch.no_grad()
     def load_state(self, st):
         """Continue from ``state()`` of an engine of the same kind over the same model, LM, n_streams, W and max_pending,
         with any chunk length.  The previous engine bounded every stored suffix by max_pending minus ITS n_out; when
         this engine's chunks yield more encoder frames, that bound is too loose, so the chunk-end commit and collapse
-        rule runs once here with this engine's bound.  The tokens it commits are returned by the next ``step``."""
+        rule runs once here with this engine's bound.  The tokens it commits are returned by the next ``step``.  With
+        contextual biasing the state must come from an engine with the same graph (its fingerprint), and every live
+        slot's automaton state must lie in [0, n_states); ValueError otherwise, before any device work."""
+        self._check_context_state(st)
         super().load_state(st)
-        self._unreturned = tuple(st[k].to("cpu", torch.int32) for k in self.HOST_STATE)
+        self._unreturned = tuple(st[k].to("cpu", torch.int32) for k in self.UNRETURNED)
         self._run(self._rebound, self.n_rebound_phases)
         ids, counts, collapsed = self._fetch(self.max_pending)
         self.n_collapses += int(collapsed.sum())
@@ -838,11 +888,15 @@ class _CommitEngine(_ChunkEngine):
     def flush(self):
         """Collapse every stream's beam to its best hypothesis and commit all of that hypothesis' remaining tokens;
         decoding continues from it.  -> (ids int32 [S, K], counts int32 [S] as from ``step``, -log p [S] of the best
-        hypothesis, the negated fused score with an LM), on the host."""
+        hypothesis, the negated fused score with an LM), on the host.  With contextual biasing the score is
+        -(value - pending[state]) in fp32, what BEAM_FINAL reports: a phrase only partly matched earns nothing."""
         self._run(self._flush, self.n_flush_phases)
         ids, counts, _ = self._fetch(self.max_pending)
         ids, counts = self._take(ids, counts)
-        return ids, counts, -self.logp.view(self.S, self.W)[:, 0].cpu()
+        y = self.logp.view(self.S, self.W)[:, 0]
+        if self._graph is not None:
+            y = y - self._pending[self.ctx_state[0].view(self.S, self.W)[:, 0].long()]
+        return ids, counts, -y.cpu()
 
 
 class StreamEngine(_ChunkEngine):
@@ -1082,17 +1136,27 @@ class StreamBeamEngine(_CommitEngine):
     tokens that commits come first in the next ``step``'s output.
 
     The reference's ``<unk>`` rule (re-argmax when the argmax is ``<unk>``) is a device of the greedy loop; the beam,
-    like Transducer.beam_search, does not apply it."""
+    like Transducer.beam_search, does not apply it.
+
+    With ``context`` (a ContextGraph over the transducer's V tokens, edgedict_b200.context) every slot carries its
+    phrase-automaton state from chunk to chunk, as BeamEngine's slots do from frame to frame: BEAM_SELECT adds the
+    automaton's increment, a collapse picks the live slot of highest log p - pending[state] (BEAM_FINAL's ranking), and
+    ``flush`` returns -(log p - pending[state]).  A phrase may straddle chunks and commits, so the committed ids plus
+    ``flush`` are BeamEngine(context=...)'s best hypothesis on the concatenated encoder output, its -log p bit for bit,
+    when no forced collapse happens.  ``state()`` carries the states and the graph's fingerprint; ``load_state``
+    refuses a state of another graph, or of an engine that differs in using context.  An empty graph builds the program
+    without context."""
 
     def __init__(self, transducer, n_streams, frames_per_chunk, W, merge=True, lm=None, lm_weight=0.0,
                  length_bonus=0.0, lm_bos=1, lm_token_map=None, max_pending=64, state=None, blank=NUL, max_ctas=0,
-                 max_symbols=1, frontend=None, samples_per_chunk=None):
+                 max_symbols=1, frontend=None, samples_per_chunk=None, context=None):
         K = check_max_symbols(max_symbols)
         W = operator.index(W)
         if not 1 <= W <= BEAM_MAX_W:
             raise ValueError("beam width must be in [1, %d], got %r" % (BEAM_MAX_W, W))
         V = transducer.joint.joint[2].weight.shape[0]
         fusion = check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map)
+        graph = check_context(context, V, blank)
         enc, dec, joint = transducer.encoder, transducer.decoder, transducer.joint.joint
         S, n, T = self._check_shape(enc, n_streams, frames_per_chunk, frontend, samples_per_chunk)
         P = operator.index(max_pending)
@@ -1113,7 +1177,7 @@ class StreamBeamEngine(_CommitEngine):
         lm_sel, lm_step = lm_fusion(self, fusion, R) if self.lm else ({}, None)
         # per parity: predictor state, its output, {suffix length, hash lo, hash hi, tokens since the last commit} per
         # row and the LM state
-        beam_state(self, R, Ld, Hd, D, LS)
+        beam_state(self, R, Ld, Hd, D, LS, context=graph is not None)
         self.dec_htmp, self.hidden, self.logits = z(Ld, R, Hd), z(R, J), z(R, V)
         self.tok, self.src, self.logp = z(R, dtype=i32), z(R, dtype=i32), z(R)
         self.frames = torch.full((S,), T, dtype=i32, device=self.dev)      # a stream never freezes
@@ -1130,6 +1194,7 @@ class StreamBeamEngine(_CommitEngine):
                    flags=F_STREAM | (F_MERGE if merge else 0) | (F_LM if self.lm else 0), K1=LS, x1=_ptr(self.logits),
                    ldx1=V, y=_ptr(self.logp), tok_in=_ptr(self.frames), tok_out=_ptr(self.tok), src=_ptr(self.src),
                    hist=_ptr(self.hist), hist_ld=TK, **lm_sel)
+        self._context(graph, sel)
         for t in range(T):
             beam_frame(prog, self, dec, t, _ptr(self.enc_out, t * E), T * E, sel, lm_step)
         self._prime, self.n_prime_phases = _upload(prime, self.dev), len(prime)
@@ -1146,6 +1211,8 @@ class StreamBeamEngine(_CommitEngine):
             if self.lm:
                 pr.append(EbPhase(type=PH_COPY, S=self._lst[0].shape[0] * R, N=self._lst[0].shape[2],
                                   x1=_ptr(self._lst[0]), y=_ptr(self._lst[1])))
+            if self.ctx_state is not None:
+                pr.append(EbPhase(type=PH_COPY, S=1, N=R, x1=_ptr(self.ctx_state[0]), y=_ptr(self.ctx_state[1])))
         if self.lm:
             ntok = self.lm_logits.shape[1]
             pr.append(EbPhase(type=PH_COPY, S=R, N=ntok, x1=_ptr(self.lm_logits), y=_ptr(self._lm_logits_tmp)))
@@ -1162,12 +1229,15 @@ class StreamBeamEngine(_CommitEngine):
                  live=self.hist_live[:, -1])
         if self.lm:
             v.update(lm_state=self._lst[0], lm_logits=self.lm_logits)
+        if self.ctx_state is not None:
+            v.update(ctx_state=self.ctx_state[0])
         return v
 
     @torch.no_grad()
     def reset(self):
-        """Every stream starts a new utterance: zero encoder state, one live slot of log p 0 with the empty sequence,
-        predictor primed with <bos> and the LM with lm_bos from zeros."""
+        """Every stream starts a new utterance: zero encoder state, one live slot of log p 0 with the empty sequence
+        (at the phrase automaton's root with contextual biasing), predictor primed with <bos> and the LM with lm_bos
+        from zeros."""
         for t in (self.enc_h, self.enc_c):
             if t is not None:
                 t.zero_()
@@ -1193,10 +1263,10 @@ class GRUStreamEngine(StreamEngine):
 class GRUStreamBeamEngine(StreamBeamEngine):
     """StreamBeamEngine for a transducer with a GRU encoder: the same signature and contract (W, merge, the LM fusion
     arguments, max_pending and the forced collapse, max_symbols, ``step`` / ``flush`` / ``reset`` / ``state`` /
-    ``load_state`` with the re-bound).  The chunk program is encoder_phases' GRU encoder followed by StreamBeamEngine's
-    beam frames and chunk end; every program (chunk, prime, flush, re-bound) runs through eb_decode_run_gru_rnnt.  The
-    state carries ``enc_h`` and no ``enc_c``, so the state of an LSTM-encoder engine does not load here, nor this one's
-    there."""
+    ``load_state`` with the re-bound, ``context``).  The chunk program is encoder_phases' GRU encoder followed by
+    StreamBeamEngine's beam frames and chunk end; every program (chunk, prime, flush, re-bound) runs through
+    eb_decode_run_gru_rnnt.  The state carries ``enc_h`` and no ``enc_c``, so the state of an LSTM-encoder engine does
+    not load here, nor this one's there."""
     GRU = True
 
 
@@ -1410,13 +1480,16 @@ class CTCStreamBeamEngine(_CommitEngine):
     beam collapses to its best slot (highest (pb (+) pnb) + f, lowest slot on ties), whose pb | pnb | f and LM state
     move to slot 0.  Each stream keeps its last committed token ``last`` [S] (-1 after ``reset``): a slot whose stored
     suffix is empty takes it as its last token, so a token held across a commit is not emitted twice.  ``flush()``,
-    ``state()`` / ``load_state()`` (with the re-bound) and ``n_collapses`` are StreamBeamEngine's."""
+    ``state()`` / ``load_state()`` (with the re-bound) and ``n_collapses`` are StreamBeamEngine's, and so is
+    ``context``: each slot carries its phrase-automaton state (``ctx_state`` [2, R]) across chunks, an extension adds
+    the automaton's increment to f', and collapses and ``flush`` use (pb (+) pnb) + f - pending[state], so the ids of
+    the chunks plus ``flush`` are ctc.beam_search(context=...)'s on the concatenated log-probs."""
     GRU = True
     RUN = "eb_decode_run_ctc_stream_beam"
 
     def __init__(self, ctc_model, n_streams, frames_per_chunk, W, *, lm=None, lm_weight=0.0, length_bonus=0.0,
                  lm_bos=1, lm_token_map=None, max_pending=64, blank=0, max_ctas=0, state=None, frontend=None,
-                 samples_per_chunk=None):
+                 samples_per_chunk=None, context=None):
         from .rnnt.models import CTCEncoder
         if not isinstance(ctc_model, CTCEncoder):
             raise TypeError("CTCStreamBeamEngine streams a CTCEncoder, got %s" % type(ctc_model).__name__)
@@ -1429,6 +1502,7 @@ class CTCStreamBeamEngine(_CommitEngine):
         if not 0 <= blank < V:
             raise ValueError("blank must lie in [0, %d), got %d" % (V, blank))
         fusion = check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map)
+        graph = check_context(context, V, blank)
         S, n, T = self._check_shape(enc, n_streams, frames_per_chunk, frontend, samples_per_chunk)
         P = operator.index(max_pending)
         if P < T:
@@ -1462,6 +1536,8 @@ class CTCStreamBeamEngine(_CommitEngine):
         sel = dict(type=PH_CTC_BEAM, S=S, N=V, aux=W, aux2=blank, K1=LS, flags=F_STREAM | (F_LM if self.lm else 0),
                    x1=_ptr(self.logprobs), tok_in=_ptr(self.frames), c=_ptr(self.beam), seq_out=_ptr(self.seqs),
                    y=_ptr(self.logp), src=_ptr(self.src), hist=_ptr(self.hist), hist_ld=T, y2=_ptr(self.last), **lm_sel)
+        self.ctx_state = z(2, R, dtype=i32) if graph is not None else None   # per parity: each slot's automaton state
+        self._context(graph, sel)
         prime = []
         if self.lm:
             Ll, _, Hl = self.lm_htmp.shape
@@ -1488,6 +1564,8 @@ class CTCStreamBeamEngine(_CommitEngine):
             if self.lm:
                 pr.append(EbPhase(type=PH_COPY, S=self.lm_state.shape[1] * R, N=self.lm_state.shape[3],
                                   x1=_ptr(self.lm_state[0]), y=_ptr(self.lm_state[1])))
+            if self.ctx_state is not None:
+                pr.append(EbPhase(type=PH_COPY, S=1, N=R, x1=_ptr(self.ctx_state[0]), y=_ptr(self.ctx_state[1])))
         if self.lm:
             ntok = self.lm_logits.shape[1]
             pr.append(EbPhase(type=PH_COPY, S=R, N=ntok, x1=_ptr(self.lm_logits), y=_ptr(self._lm_logits_tmp)))
@@ -1504,14 +1582,19 @@ class CTCStreamBeamEngine(_CommitEngine):
                  live=self.hist_live[:, -1], last=self.last)
         if self.lm:
             v.update(lm_state=self.lm_state[0], lm_logits=self.lm_logits)
+        if self.ctx_state is not None:
+            v.update(ctx_state=self.ctx_state[0])
         return v
 
     @torch.no_grad()
     def reset(self):
         """Every stream starts a new utterance: zero encoder state, one live slot holding the empty prefix (pb = 0,
-        pnb = -inf, f = 0), no committed token (last = -1), and the LM primed with lm_bos from zeros."""
+        pnb = -inf, f = 0) at the phrase automaton's root with contextual biasing, no committed token (last = -1), and
+        the LM primed with lm_bos from zeros."""
         S, W = self.S, self.W
         self.enc_h.zero_()
+        if self.ctx_state is not None:
+            self.ctx_state[0].zero_()
         self.beam[0].zero_()
         self.beam[0, :2].fill_(float("-inf"))
         self.beam[0, 0].view(S, W)[:, 0] = 0.0

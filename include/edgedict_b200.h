@@ -480,12 +480,15 @@ typedef struct EbPhase {
  *            candidate, its stay (value log p, flat index slot*N + blank); a non-blank token at j = K-1 closes; only
  *            hypotheses of equal closedness merge; the live count lives in the last history column; a row with no open
  *            slot (or frozen) keeps its beam and writes no history.
- *     2048 = contextual biasing (BEAM_SELECT, CTC_BEAM, BEAM_FINAL): ctx points to an EbContext.  A candidate that
+ *     2048 = contextual biasing (BEAM_SELECT, CTC_BEAM, BEAM_FINAL, BEAM_COMMIT): ctx points to an EbContext.  A
+ *            candidate that
  *            appends a non-blank token k to slot q adds delta[state(q), k] to its value (BEAM_SELECT: inside the fusion
  *            term f, for k != blank; CTC_BEAM: to the extension's f'), and each survivor's state (next[state(q), k], or
  *            state(q) for blank, a stay or a frozen frame) is written to the other parity: BEAM_SELECT reads parity
  *            t & 1 (parity 0 under flag 512), CTC_BEAM parity t & 1, as their sequence rows.  BEAM_FINAL ranks and writes
- *            y - pending[state] with the state from parity hist_col.
+ *            y - pending[state] with the state from parity hist_col.  BEAM_COMMIT reads the states from parity 1,
+ *            collapses to the live slot of highest y - pending[state] (lowest slot on ties; it keeps its y and state)
+ *            and writes every slot's state, moved by src, to parity 0.
  * SKIP (no flags, writes nothing, no grid barrier): when no row of tok_in[0..S) differs from aux2 (blank), every CTA
  * jumps over the next aux phases.  It reads only data final at the preceding barrier, so all CTAs take the same branch.
  * BEAM_COMMIT (streaming beam, after a chunk's last frame, one CTA per stream): commits the common prefix of the live
