@@ -2,9 +2,11 @@
 configuration, against the fp64 oracle (tests/features_batch_oracle.py) and the reference's own per-utterance transform
 (tests/golden/features_tiny.npz), plus the bitwise invariants of the batched path and two integrations.
 
-Bars: logfbank / mfcc and their deltas absolute 2e-3 (tests/test_gpu_features.py's log-mel bar: fp32 direct DFT against
-an fp64 FFT); melspec and its deltas 1e-5 x the frame's total power sum_k P (for a delta, the largest over the +-4
-frames it reads)."""
+Bars: per element, the first-order bound tests/features_fp64.py propagates through the fp64 restatement of the chain
+on the module's own fp32 tables, in table mode (plus the effect of those tables' distance from the oracle's exact ones).
+Against the reference's own fp32 features (the golden fixture), which carry their own error, the bar grows by
+|oracle - golden|, measured per element: |device - golden| <= bar + |oracle - golden| by the triangle inequality.  The
+melspec rows also print their ratio to the former bar, 1e-5 x the frame's total power sum_k P."""
 import random
 
 import numpy as np
@@ -12,6 +14,7 @@ import pytest
 import torch
 
 from tests import features_batch_oracle as O
+from tests import features_fp64 as X
 from tests.test_features_batch_host import CONFIGS, golden, melspec_bar, tag
 
 pytestmark = pytest.mark.gpu
@@ -24,17 +27,21 @@ def _build(ft, size, n_fft=512, delta=False, ds=1, ptd=True, **kw):
     return train.cuda(), test.cuda(), n
 
 
-def _check(ft, got, want, x, lens, n_fft, delta, ds, C, ptd, what):
-    """Assert the bar; return the worst error as a fraction of it."""
-    err = np.abs(got.astype(np.float64) - want)
+def _bar(test, ft, x, lens, n_fft, C, delta, ds, ptd):
+    """Per-element bar and where it holds (features_fp64.chain in table mode) for the module `test` on fp32 x [B, L]."""
+    basis, fbT, dct, pre = X.module_tables(test)
+    te = X.tables_err(ft, basis, fbT, dct, n_fft, C, pre)
+    _, bar, ok = X.chain(x.cuda(), lens, ft, basis, fbT, n_fft, 200, ds, delta, ptd, preemph=pre, dct=dct, tables_err=te)
+    return bar, ok
+
+
+def _check(ft, got, want, bar, ok, x, lens, n_fft, delta, ds, C, ptd, what, extra=None):
+    """Assert the propagated bar; return the worst error as a fraction of it."""
     if ft == "melspec":
-        bar = 1e-5 * melspec_bar(x, lens, n_fft, 400, 200, delta, ds, C, ptd)
-        ratio = float(np.max(err / np.maximum(bar, 1e-30)))
-    else:
-        ratio = float(err.max() / 2e-3)
-    print("%s %s worst error / bar = %.3g" % (what, ft, ratio))
-    assert ratio <= 1.0, (what, ratio)
-    return ratio
+        err = np.abs(np.asarray(got, np.float64) - want)
+        old = 1e-5 * melspec_bar(x, lens, n_fft, 400, 200, delta, ds, C, ptd)
+        print("%s %s worst error / former bar 1e-5 sum_k P = %.3g" % (what, ft, float(np.max(err / np.maximum(old, 1e-30)))))
+    return X.report("%s %s d%d n%d ds%d p%d" % (what, ft, delta, n_fft, ds, ptd), got, want, bar, ok, extra)
 
 
 @pytest.mark.parametrize("ft,delta,n_fft,ds,ptd", CONFIGS)
@@ -50,10 +57,13 @@ def test_golden_and_oracle_parity(ft, delta, n_fft, ds, ptd):
     assert np.array_equal(xlen.numpy(), z[k + ".xlen"]) and xs.shape == z[k + ".xs"].shape and xs.shape[2] == n
     for b, T in enumerate(xlen.tolist()):
         assert (xs[b, T:] == 0).all()
-    _check(ft, xs, z[k + ".xs"].astype(np.float64), x.astype(np.float64), z["lens"], n_fft, delta, ds, C, ptd, "golden")
+    bar, ok = _bar(test, ft, torch.tensor(x), z["lens"], n_fft, C, delta, ds, ptd)
     want, _ = O.batch_transform(x.astype(np.float64), z["lens"], ft, C, n_fft=n_fft, win_length=400, hop_length=200,
                                 delta=delta, downsample=ds, pad_to_divisible=ptd)
-    _check(ft, xs, want, x.astype(np.float64), z["lens"], n_fft, delta, ds, C, ptd, "oracle")
+    gold = z[k + ".xs"].astype(np.float64)
+    _check(ft, xs, want, bar, ok, x.astype(np.float64), z["lens"], n_fft, delta, ds, C, ptd, "oracle")
+    _check(ft, xs, gold, bar, ok, x.astype(np.float64), z["lens"], n_fft, delta, ds, C, ptd, "golden",
+           extra=np.abs(want - gold))
 
 
 def _speech_like(lens, seed):
@@ -80,7 +90,9 @@ def test_long_utterances_against_the_oracle(ft, delta):
     want, wlen = O.batch_transform(x.numpy().astype(np.float64), LONG_LENS, ft, 80, n_fft=512, win_length=400,
                                    hop_length=200, delta=delta, downsample=3, pad_to_divisible=True)
     assert np.array_equal(xlen.numpy(), wlen)
-    _check(ft, xs.cpu().numpy(), want, x.numpy().astype(np.float64), LONG_LENS, 512, delta, 3, 80, True, "8 x 1-16 s")
+    bar, ok = _bar(test, ft, x, LONG_LENS, 512, 80, delta, 3, True)
+    _check(ft, xs.cpu().numpy(), want, bar, ok, x.numpy().astype(np.float64), LONG_LENS, 512, delta, 3, 80, True,
+           "8 x 1-16 s")
 
 
 def test_masks_reproduce_the_reference_draws():
@@ -98,8 +110,15 @@ def test_masks_reproduce_the_reference_draws():
         g, c = got.cpu().numpy(), clean.cpu().numpy()
         assert np.array_equal(g == 0, want == 0)
         assert ((g == c) | (g == 0)).all()                              # unmasked elements are the test transform's
-        tol = 2e-3 if ft != "melspec" else 1e-5 * np.abs(want).max()
-        assert np.abs(g - want).max() <= tol
+        # the oracle with the same spans; the golden masked rows carry their own distance from it
+        oc, olen = O.batch_transform(z["x"].astype(np.float64), z["lens"], ft, int(z["size"]), n_fft=int(n_fft),
+                                     win_length=400, hop_length=200, delta=bool(int(delta)), downsample=int(ds),
+                                     pad_to_divisible=bool(int(ptd)))
+        random.seed(int(z["mask_seed"]))
+        om = O.apply_spans(oc, *O.reference_spans(olen.tolist(), oc.shape[2], int(tm), int(tn), int(fm), int(fn)))
+        bar, ok = _bar(test, ft, torch.tensor(z["x"]), z["lens"], int(n_fft), int(z["size"]), bool(int(delta)), int(ds),
+                       bool(int(ptd)))
+        X.report("masked%d %s vs golden" % (i, ft), g, want, bar, ok, np.abs(om - want))
 
 
 @pytest.mark.parametrize("ft", ["logfbank", "mfcc", "melspec"])

@@ -85,11 +85,15 @@ def test_e6d2_features_against_the_fp64_oracle():
     x = _audio(64, E6D2_L, 5)
     eng = StreamEngine(_transducer(240), 64, None, frontend=tr, samples_per_chunk=E6D2_L)
     eng.step(x)
+    from tests import features_fp64 as X
     want, _ = O.batch_transform(x.cpu().numpy().astype(np.float64), [E6D2_L] * 64, "logfbank", 80, n_fft=512,
                                 win_length=320, hop_length=200, delta=False, downsample=3, pad_to_divisible=False)
-    err = float(np.abs(eng.xin.cpu().numpy().astype(np.float64) - want).max())
-    print("E6D2 window vs fp64 oracle: worst error / bar = %.3g" % (err / 2e-3))
-    assert err <= 2e-3                          # test_gpu_features_batch.py's logfbank bar
+    # test_gpu_features_batch.py's bar: the chain's propagated per-element bound, in table mode
+    basis, fbT, dct, pre = X.module_tables(tr)
+    te = X.tables_err("logfbank", basis, fbT, dct, 512, 80, pre)
+    _, bar, ok = X.chain(x, [E6D2_L] * 64, "logfbank", basis, fbT, 512, 200, 3, False, False, preemph=pre,
+                         tables_err=te)
+    X.report("E6D2 window vs fp64 oracle", eng.xin, want, bar, ok)
 
 
 def test_dither_bitwise():
