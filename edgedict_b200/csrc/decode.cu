@@ -693,6 +693,66 @@ __device__ bool seq_equal_ext(const int* s1, int e1, const int* s2, int e2) {
     return true;
 }
 
+// N-gram shallow fusion (flags 4096, BEAM_SELECT / CTC_BEAM / BEAM_FINAL; DESIGN.md 4f): ng -> EbNgram.  ngram_rows
+// builds, for the slots q < n with want(q), row r0 + q of the workspace: g(state(q), k) for every token k in the fp32
+// order of the backoff rule.  It starts from the unigram row and, for each state of the slot's suffix chain from depth
+// 1 up to state(q), does row = bo + row over all V tokens, then overwrites that state's children with their p: depth * V
+// adds per slot, one pass per chain level for all slots, two __syncthreads per level.  All threads of the CTA call it;
+// it ends at a __syncthreads, after which the rows are read like the logits.
+template <class State, class Want>
+__device__ void ngram_rows(const EbNgram* ng, long r0, int n, int V, State state, Want want, int* smax) {
+    const int tid = threadIdx.x, nt = blockDim.x;
+    const int *depth = ng->depth, *suffix = ng->suffix;
+    float* rows = ng->row;
+    if (tid == 0) *smax = 0;
+    __syncthreads();
+    int dmax = 0;
+    for (int q = tid; q < n; q += nt)
+        if (want(q)) dmax = max(dmax, __ldg(depth + state(q)));
+    if (dmax) atomicMax(smax, dmax);
+    for (int q = 0; q < n; ++q) {
+        if (!want(q)) continue;
+        float* row = rows + (r0 + q) * V;
+        for (int k = tid; k < V; k += nt) row[k] = __ldg(ng->unigram + k);
+    }
+    __syncthreads();
+    const int D = *smax;
+    for (int i = 1; i <= D; ++i)
+        for (int pass = 0; pass < 2; ++pass) {           // bo + row, then the children of the level-i state
+            for (int q = 0; q < n; ++q) {
+                if (!want(q)) continue;
+                int s = state(q), d = __ldg(depth + s);
+                if (d < i) continue;
+                for (; d > i; --d) s = __ldg(suffix + s);
+                float* row = rows + (r0 + q) * V;
+                if (pass == 0) {
+                    const float b = __ldg(ng->bo + s);
+                    for (int k = tid; k < V; k += nt) row[k] = __fadd_rn(b, row[k]);
+                } else {
+                    const int c0 = __ldg(ng->first + s), c1 = c0 + __ldg(ng->count + s);
+                    for (int c = c0 + tid; c < c1; c += nt) row[__ldg(ng->tok + c)] = __ldg(ng->prob + c);
+                }
+            }
+            __syncthreads();
+        }
+}
+// The n-gram state after a non-blank token k in state s: the next state of the first child k found walking down the
+// suffix chain from s (a binary search in each state's sorted children, at most depth(s) + 1 states), the root if none.
+__device__ int ngram_next(const EbNgram* ng, int s, int k) {
+    for (;;) {
+        int lo = __ldg(ng->first + s), hi = lo + __ldg(ng->count + s);
+        const int end = hi;
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (__ldg(ng->tok + mid) < k) lo = mid + 1;
+            else hi = mid;
+        }
+        if (lo < end && __ldg(ng->tok + lo) == k) return __ldg(ng->next + lo);
+        if (s == 0) return 0;
+        s = __ldg(ng->suffix + s);
+    }
+}
+
 // Selection: the candidates of one utterance are (slot q < live, token k) with value
 //   lp = ((x[q,k] - max_q) - log sum_k exp(x[q,k] - max_q)) + logp[q],
 // or with LM fusion (flags 32) lp = (a + f) + logp[q] where a is the first term above and, for k != blank,
@@ -756,7 +816,14 @@ __device__ __forceinline__ void beam_select(const EbPhase& p, float* sm) {
     int* sopen = reinterpret_cast<int*>(lmls + BEAM_MAX_W);                      // slot open (MULTI)
     unsigned* rhist = reinterpret_cast<unsigned*>(sopen + BEAM_MAX_W);          // [256]
     int* misc = reinterpret_cast<int*>(rhist + 256);
-    const float lm_weight = lm ? __ldg(p.fuse) : 0.f, length_bonus = lm ? __ldg(p.fuse + 1) : 0.f;
+    // n-gram fusion (flags 4096): its states alternate as the context states do, its rows are built per frame / round
+    const bool ng = p.flags & 4096;
+    const EbNgram* ngd = ng ? p.ctx->ng : nullptr;
+    const float lm_weight = lm ? __ldg(p.fuse) : 0.f, length_bonus = lm || ng ? __ldg(p.fuse + 1) : 0.f;
+    const float ng_w = ng ? ngd->weight : 0.f;
+    const float* ng_row = ng ? ngd->row : nullptr;
+    const int* nst_in = ng ? ngd->state[MULTI ? 0 : t & 1] : nullptr;
+    int* nst_out = ng ? ngd->state[MULTI ? 1 : (t & 1) ^ 1] : nullptr;
     // contextual biasing (flags 2048): the slots' automaton states alternate as the sequence rows do
     const bool cx = p.flags & 2048;
     const int* cnext = cx ? p.ctx->next : nullptr;
@@ -786,6 +853,7 @@ __device__ __forceinline__ void beam_select(const EbPhase& p, float* sm) {
                     p.src[r0 + s] = (int)(r0 + s);
                     if (lm) p.tok_out2[r0 + s] = -1;
                     if (cx) cst_out[r0 + s] = __ldcg(cst_in + r0 + s);
+                    if (ng) nst_out[r0 + s] = __ldcg(nst_in + r0 + s);
                 }
                 for (int s = 0; s < nlive; ++s) {
                     const int* ps = p.seq_in + (r0 + s) * LS;
@@ -804,6 +872,7 @@ __device__ __forceinline__ void beam_select(const EbPhase& p, float* sm) {
                 p.src[r0 + j] = (int)(r0 + j);
                 if (lm) p.tok_out2[r0 + j] = -1;
                 if (cx) cst_out[r0 + j] = __ldcg(cst_in + r0 + j);   // the state BEAM_FINAL reads stays current
+                if (ng) nst_out[r0 + j] = __ldcg(nst_in + r0 + j);
             }
             if (tid == 0) hlive[(long)b * T + t] = nlive;
             continue;
@@ -841,10 +910,13 @@ __device__ __forceinline__ void beam_select(const EbPhase& p, float* sm) {
             }
         }
         __syncthreads();
+        if (ng)                                              // g(state(q), .) of every slot with candidates
+            ngram_rows(ngd, r0, nlive, V, [&](int q) { return __ldcg(nst_in + r0 + q); },
+                       [&](int q) { return !MULTI || sopen[q]; }, misc + 6);
         // the one expression every pass ranks by; d = the delta row of slot q's context state
         auto composite = [&](int q, int k, const float* x, const float* d) -> unsigned long long {
             float v = (__ldcg(x + k) - rowm[q]) - rowls[q];
-            if (lm || cx) {
+            if (lm || cx || ng) {
                 float f = 0.f;
                 if (k != blank) {
                     if (lm) {
@@ -852,8 +924,11 @@ __device__ __forceinline__ void beam_select(const EbPhase& p, float* sm) {
                         f = j >= 0 ? lm_weight * ((__ldcg(p.x2 + (r0 + q) * p.ldx2 + j) - lmm[q]) - lmls[q]) +
                                          length_bonus
                                    : length_bonus;
+                    } else if (ng) {
+                        f = length_bonus;
                     }
-                    if (cx) f = lm ? f + __ldg(d + k) : __ldg(d + k);
+                    if (ng) f = __fadd_rn(f, __fmul_rn(ng_w, __ldcg(ng_row + (r0 + q) * V + k)));
+                    if (cx) f = lm || ng ? f + __ldg(d + k) : __ldg(d + k);
                 }
                 v = v + f;
             }
@@ -1030,11 +1105,16 @@ __device__ __forceinline__ void beam_select(const EbPhase& p, float* sm) {
                     const int cs = __ldcg(cst_in + r0 + spar[i]);
                     cst_out[r] = k != blank ? __ldg(cnext + (long)cs * V + k) : cs;
                 }
+                if (ng) {
+                    const int ns = __ldcg(nst_in + r0 + spar[i]);
+                    nst_out[r] = k != blank ? ngram_next(ngd, ns, k) : ns;
+                }
             } else {
                 p.y[r] = -INFINITY;
                 p.tok_out[r] = blank;
                 if (lm) p.tok_out2[r] = -1;
                 if (cx) cst_out[r] = 0;
+                if (ng) nst_out[r] = 0;
                 p.src[r] = (int)r;
                 hpar[h] = s;
                 htok[h] = blank;
@@ -1186,12 +1266,17 @@ __device__ __noinline__ void phase_beam_final(const EbPhase& p) {
     const int* htok = p.hist + BTW;
     const int* hlive = p.hist + 3 * BTW;
     if (threadIdx.x >= 32) return;                           // one warp: with the whole CTA the CTC entry spills more
-    // the ranking value: y, or with contextual biasing (flags 2048) y - pending[state], the state from parity hist_col
+    // the ranking value: y, with n-gram fusion (flags 4096) y + w*e(state), with contextual biasing (flags 2048) then
+    // - pending[state], the states from parity hist_col
     const bool cx = p.flags & 2048;
     const float* cpend = cx ? p.ctx->pending : nullptr;
     const int* cst = cx ? p.ctx->state[p.hist_col & 1] : nullptr;
+    const float* nend = p.flags & 4096 ? p.ctx->ng->end : nullptr;
+    const int* nst = nend ? p.ctx->ng->state[p.hist_col & 1] : nullptr;
+    const float ng_w = nend ? p.ctx->ng->weight : 0.f;
     auto value = [&](long r) -> float {
-        const float v = __ldcg(p.y + r);
+        float v = __ldcg(p.y + r);
+        if (nend) v = __fadd_rn(v, __fmul_rn(ng_w, __ldg(nend + __ldcg(nst + r))));
         return cx ? v - __ldg(cpend + __ldcg(cst + r)) : v;
     };
     for (int b = blockIdx.x; b < p.S; b += gridDim.x) {
@@ -1280,11 +1365,12 @@ __device__ __noinline__ void phase_beam_final(const EbPhase& p) {
 // stay's repeat term and the extension rule see the real last token across a commit.  Without the flag e is -1 there,
 // which is the same thing at the start of an utterance.
 constexpr int CTC_SEQ_HEAD = 5;
-// CTC_BEAM's shared memory (2 x u64 + 11 x 32-bit arrays of BEAM_MAX_W, histogram, scalars, the context states) in the
-// dynamic shared memory
-static_assert(BEAM_MAX_W * (2 * 8 + 12 * 4) + 256 * 4 + 8 * 4 <= (RED_FLOATS + TR * OUT_LD) * 4, "ctc beam smem");
+// CTC_BEAM's shared memory (2 x u64 + 11 x 32-bit arrays of BEAM_MAX_W, histogram, scalars, the context and n-gram
+// states) in the dynamic shared memory
+static_assert(BEAM_MAX_W * (2 * 8 + 13 * 4) + 256 * 4 + 8 * 4 <= (RED_FLOATS + TR * OUT_LD) * 4, "ctc beam smem");
 
-__device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
+template <bool NG>
+__device__ __noinline__ void ctc_beam(const EbPhase& p, float* sm) {
     const int W = p.aux, V = p.N, T = p.hist_ld, blank = p.aux2, LS = p.K1;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nt = blockDim.x;
     const bool lm = p.flags & 32, stream = p.flags & 64;
@@ -1309,7 +1395,13 @@ __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
     unsigned* rhist = reinterpret_cast<unsigned*>(cnext + BEAM_MAX_W);          // [256]
     int* misc = reinterpret_cast<int*>(rhist + 256);
     int* sst = misc + 8;                                                        // context state of each slot
-    const float lm_weight = lm ? __ldg(p.fuse) : 0.f, length_bonus = lm ? __ldg(p.fuse + 1) : 0.f;
+    int* sng = sst + BEAM_MAX_W;                                                // n-gram state of each slot
+    const bool ng = NG;                                                         // n-gram fusion (flags 4096)
+    const EbNgram* ngd = ng ? p.ctx->ng : nullptr;
+    const float ng_w = ng ? ngd->weight : 0.f;
+    const float* ng_row = ng ? ngd->row : nullptr;
+    int* const* ng_state = ng ? ngd->state : nullptr;                           // parity t & 1, as c and seq_out
+    const float lm_weight = lm ? __ldg(p.fuse) : 0.f, length_bonus = lm || ng ? __ldg(p.fuse + 1) : 0.f;
     const bool cx = p.flags & 2048;                                             // contextual biasing
     const int* ctx_next = cx ? p.ctx->next : nullptr;
     const float* ctx_delta = cx ? p.ctx->delta : nullptr;
@@ -1330,6 +1422,7 @@ __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
                     p.src[r0 + j] = (int)(r0 + j);
                     if (lm) p.tok_out2[r0 + j] = -1;
                     if (cx) ctx_state[(t + 1) & 1][r0 + j] = __ldcg(ctx_state[t & 1] + r0 + j);
+                    if (ng) ng_state[(t + 1) & 1][r0 + j] = __ldcg(ng_state[t & 1] + r0 + j);
                 }
                 if (tid == 0) hlive[(long)b * T + t] = nlive;
                 continue;
@@ -1352,8 +1445,11 @@ __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
                 se[q] = len > 0 ? __ldcg(ps + CTC_SEQ_HEAD + len - 1) : e0;
                 chead[q] = -1;
                 if (cx) sst[q] = __ldcg(ctx_state[t & 1] + r0 + q);
+                if (ng) sng[q] = __ldcg(ng_state[t & 1] + r0 + q);
             }
             __syncthreads();
+            if (ng)                                          // g(state(q), .) of every live slot
+                ngram_rows(ngd, r0, nlive, V, [&](int q) { return sng[q]; }, [](int) { return true; }, misc + 7);
             // merges: the slot whose prefix is slot q2's minus its last token
             for (int q2 = tid; q2 < nlive; q2 += nt) {
                 int par = -1;
@@ -1413,7 +1509,10 @@ __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
                     f2 = f2 + (j >= 0 ? lm_weight * ((__ldcg(p.x2 + (r0 + q) * p.ldx2 + j) - lmm[q]) - lmls[q]) +
                                             length_bonus
                                       : length_bonus);
+                } else if (ng) {
+                    f2 = f2 + length_bonus;
                 }
+                if (ng) f2 = __fadd_rn(f2, __fmul_rn(ng_w, __ldcg(ng_row + (r0 + q) * V + k)));
                 if (cx) f2 = f2 + __ldg(ctx_delta + (long)sst[q] * V + k);
             };
             // candidate flat index e = q*V + k; false when it merged into a live slot's stay
@@ -1517,6 +1616,7 @@ __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
                     st_out[R + r] = pnb2;
                     st_out[2 * R + r] = f2;
                     if (cx) ctx_state[(t + 1) & 1][r] = k == blank ? sst[q] : __ldg(ctx_next + (long)sst[q] * V + k);
+                    if (ng) ng_state[(t + 1) & 1][r] = k == blank ? sng[q] : ngram_next(ngd, sng[q], k);
                     p.y[r] = v;
                     p.src[r] = (int)(r0 + q);
                     if (lm) p.tok_out2[r] = k != blank ? __ldg(p.tok_map + k) : -1;
@@ -1528,6 +1628,7 @@ __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
                     st_out[R + r] = -INFINITY;
                     st_out[2 * R + r] = 0.f;
                     if (cx) ctx_state[(t + 1) & 1][r] = 0;
+                    if (ng) ng_state[(t + 1) & 1][r] = 0;
                     p.y[r] = -INFINITY;
                     p.src[r] = (int)r;
                     if (lm) p.tok_out2[r] = -1;
@@ -1556,6 +1657,14 @@ __device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
             }
         }
     }
+}
+
+// One call site in the kernel and two __noinline__ instantiations behind it: a program without n-gram fusion runs a
+// body compiled without the term.  With the term's flag tests in one body the offline CTC beam without an n-gram model
+// measured 12 % slower than before (W = 4 / 8 / 16, DESIGN.md 4f).
+__device__ __noinline__ void phase_ctc_beam(const EbPhase& p, float* sm) {
+    if (p.flags & 4096) ctc_beam<true>(p, sm);
+    else ctc_beam<false>(p, sm);
 }
 
 // SKIP: does any row of tok_in[0..S) differ from aux2 (blank)?  tok_in is final at the preceding grid barrier, so every

@@ -186,7 +186,7 @@ def free_beam_search():
 
 
 def beam_search(log_probs, input_lengths, beam_width, blank=0, *, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1,
-                lm_token_map=None, nbest=None, context=None):
+                lm_token_map=None, nbest=None, context=None, ngram=None, ngram_weight=0.0):
     """CTC prefix beam search (Hannun et al., 2014) on the device, optionally with shallow fusion of the reference's
     LSTM language model (LMModel, or its state_dict).  ``CTCEncoder.beam_search`` states the rule.
 
@@ -216,9 +216,18 @@ def beam_search(log_probs, input_lengths, beam_width, blank=0, *, lm=None, lm_we
     graph's increment delta(s, c) to the fusion term: f' = (f + LM term) + delta (f' = f + delta without an LM); a stay
     adds nothing and keeps the state.  The final ranking and every returned score use (pb (+) pnb) + f - P(s), P(s)
     the pending bonus of the partial match, so a phrase earns its bonus only once it completes.  An empty graph (or
-    None) gives the search without context bit for bit; the graph's fingerprint is part of the engine cache key."""
+    None) gives the search without context bit for bit; the graph's fingerprint is part of the engine cache key.
+
+    N-gram shallow fusion: ``ngram`` is an ``edgedict_b200.ngram.NgramLM`` over the V tokens with this blank (a
+    ValueError otherwise, before any device work), ``ngram_weight`` = w finite.  Each prefix carries the model's state h
+    (the start state first); an extension by c adds w g(h, c) after the LM term, f' = ((f + T_LM) + w g) + delta, T_LM
+    the LM term or, without an LM, ``length_bonus`` (legal with an ngram alone); a stay keeps the state and adds
+    nothing.  The final ranking and every returned score use ((pb (+) pnb) + f + w e(h)) - P(s), e(h) the model's
+    end-of-sentence term (absent without </s>).  The model's fingerprint, w and the length bonus are part of the
+    engine cache key."""
     import numbers
     from .context import check_context, context_cache_key
+    from .ngram import check_ngram, check_ngram_weight, ngram_cache_key
     from .stream_engine import BEAM_MAX_W, CTCBeamEngine, check_lm_args, check_nbest, lm_cache_key, nbest_lists
     if not isinstance(log_probs, torch.Tensor):
         raise TypeError("log_probs must be a tensor")
@@ -244,19 +253,23 @@ def beam_search(log_probs, input_lengths, beam_width, blank=0, *, lm=None, lm_we
     il = _lengths(input_lengths, B, "input_lengths")
     if bool((il < 0).any()) or bool((il > T).any()):
         raise ValueError("input_lengths must lie in [0, T = %d], got %s" % (T, il.tolist()))
-    fusion = check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map)
+    model = check_ngram(ngram, V, blank)
+    ng_w = check_ngram_weight(model, ngram_weight)
+    fusion = check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map, ngram=model is not None)
     graph = check_context(context, V, blank)
     if not log_probs.is_cuda:
         raise RuntimeError("edgedict_b200 ctc beam_search needs CUDA log_probs (got a %s tensor); there is no CPU path"
                            % log_probs.device)
     dev = log_probs.device
-    key = (B, T, V, W, N, blank, dev, lm_cache_key(fusion), context_cache_key(graph))
+    key = (B, T, V, W, N, blank, dev, lm_cache_key(fusion), context_cache_key(graph),
+           ngram_cache_key(model, ng_w, length_bonus))
     eng = _beam_engines.get(key)
     if eng is None:
         _beam_engines.clear()                                  # one resident program is enough
         eng = _beam_engines[key] = CTCBeamEngine(B, T, V, W, blank, lm=lm, lm_weight=lm_weight,
                                                  length_bonus=length_bonus, lm_bos=lm_bos, lm_token_map=lm_token_map,
-                                                 device=dev, nbest=N, context=graph)
+                                                 device=dev, nbest=N, context=graph, ngram=model,
+                                                 ngram_weight=ng_w)
     lens = torch.empty(B, dtype=torch.int32, pin_memory=True)
     lens.copy_(il)
     with torch.no_grad():

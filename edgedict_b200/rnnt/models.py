@@ -407,7 +407,7 @@ class Transducer(nn.Module):
 
     @torch.no_grad()
     def beam_search(self, xs, xlen=None, W=4, merge=True, *, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1,
-                    lm_token_map=None, max_symbols=1, nbest=None, context=None):
+                    lm_token_map=None, max_symbols=1, nbest=None, context=None, ngram=None, ngram_weight=0.0):
         """SURVEY 8(f) N4: beam decode.  The reference has no beam search in rnnt/ (north_star mentions one); its
         legacy v0 stack holds a batch-1 Graves-style search (models.py:121-202, with no-op `sorted(...)` calls and a
         removed `volatile=` API).  This is a time-synchronous beam under the SAME emission constraint as
@@ -466,8 +466,19 @@ class Transducer(nn.Module):
         partial match; the final ranking, the returned -log p and every N-best nlogp use value - P(s), so a partly
         matched phrase earns nothing.  The state is a function of the token sequence, so merging stays exact.  An empty
         graph (or None) gives the search without context bit for bit; the graph's fingerprint is part of the engine
-        cache key."""
+        cache key.
+
+        N-gram shallow fusion: ``ngram`` is an `edgedict_b200.ngram.NgramLM` over this model's V tokens and blank (a
+        ValueError otherwise, before the encoder runs) and ``ngram_weight`` = w a finite real.  Each hypothesis carries
+        the model's state h (the start state first).  A candidate that appends a non-blank k adds w g(h, k) right after
+        the LM term: f = f0 + w g, f0 the LM term or, without an LM, ``length_bonus`` (legal with an ngram alone), then
+        + delta with context; value (a + f) + logp[q].  Blank and a closed hypothesis' stay keep the state and add
+        nothing.  The final ranking, the returned -log p and every N-best nlogp use (value + w e(h)) - P(s), e(h) the
+        model's end-of-sentence term (absent without </s> in the model).  The state is a function of the token sequence,
+        so merging stays exact.  ngram=None builds the search without it; the model's fingerprint, w and the length
+        bonus are part of the engine cache key."""
         from ..context import check_context, context_cache_key
+        from ..ngram import check_ngram, check_ngram_weight, ngram_cache_key
         from ..stream_engine import (BeamEngine, BEAM_MAX_W, check_lm_args, check_max_symbols, check_nbest,
                                      lm_cache_key, nbest_lists, param_fingerprint)
         K = check_max_symbols(max_symbols)
@@ -475,7 +486,10 @@ class Transducer(nn.Module):
         if not 1 <= W <= BEAM_MAX_W:
             raise ValueError("beam width W must be in [1, %d], got %d" % (BEAM_MAX_W, W))
         N = 0 if nbest is None else check_nbest(nbest, W)
-        fusion = check_lm_args(lm, self.joint.joint[2].weight.shape[0], lm_weight, length_bonus, lm_bos, lm_token_map)
+        model = check_ngram(ngram, self.joint.joint[2].weight.shape[0], self.blank)
+        ng_w = check_ngram_weight(model, ngram_weight)
+        fusion = check_lm_args(lm, self.joint.joint[2].weight.shape[0], lm_weight, length_bonus, lm_bos, lm_token_map,
+                               ngram=model is not None)
         lm_key = lm_cache_key(fusion)
         graph = check_context(context, self.joint.joint[2].weight.shape[0], self.blank)
         h_enc, _ = self.encoder(xs)
@@ -486,14 +500,16 @@ class Transducer(nn.Module):
             frames = scale_length(T, xlen).clamp(max=T).to(torch.int32)
         frames = _lens_to_device(frames.cpu(), h_enc.device)
         # the phase program bakes raw weight pointers: re-homed parameters (FlatAdam, .to(), .float()) rebuild it
-        key = (B, T, W, bool(merge), K, N, h_enc.device, param_fingerprint(self), lm_key, context_cache_key(graph))
+        key = (B, T, W, bool(merge), K, N, h_enc.device, param_fingerprint(self), lm_key, context_cache_key(graph),
+               ngram_cache_key(model, ng_w, length_bonus))
         cache = self.__dict__.setdefault("_beam_engines", {})
         eng = cache.get(key)
         if eng is None:
             cache.clear()                                  # one resident program is enough
             eng = cache[key] = BeamEngine(self, B, T, W, merge=bool(merge), blank=self.blank, lm=lm,
                                           lm_weight=lm_weight, length_bonus=length_bonus, lm_bos=lm_bos,
-                                          lm_token_map=lm_token_map, max_symbols=K, nbest=N, context=graph)
+                                          lm_token_map=lm_token_map, max_symbols=K, nbest=N, context=graph,
+                                          ngram=model, ngram_weight=ng_w)
         if N:
             return nbest_lists(eng.run(h_enc, frames), B, N, eng.ids.shape[-1])
         ids, nlogp = eng.run(h_enc, frames)
@@ -596,7 +612,7 @@ class CTCEncoder(nn.Module):
 
     @torch.no_grad()
     def beam_search(self, xs, xlen=None, W=4, *, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1, lm_token_map=None,
-                    nbest=None, context=None):
+                    nbest=None, context=None, ngram=None, ngram_weight=0.0):
         """CTC prefix beam search (Hannun et al., 2014) after ``forward`` (which follows ``set_precision``), optionally
         with shallow fusion of the reference's LSTM language model.  xs [B, T, F] -> (list of B int64 id arrays, -score
         [B] on the device).  Utterance b decodes min(T', scale_length(xlen)[b]) log-prob frames (all T' when xlen is
@@ -622,22 +638,28 @@ class CTCEncoder(nn.Module):
         result of lm=None bit for bit.  NaN log-probs are outside the contract: the search still ends and stays in
         bounds, but which hypotheses a NaN keeps is unspecified.  See ``edgedict_b200.ctc.beam_search`` (this search on
         log-probs you already have) for the arguments, for ``nbest``, which returns N-best lists with the log-prob
-        frame of each token, and for ``context``, contextual biasing toward a phrase list."""
+        frame of each token, for ``context``, contextual biasing toward a phrase list, and for ``ngram`` /
+        ``ngram_weight``, shallow fusion of a token n-gram model."""
         from .. import ctc
         from ..context import check_context
+        from ..ngram import check_ngram, check_ngram_weight
         from ..stream_engine import BEAM_MAX_W, check_lm_args, check_nbest
         W = operator.index(W)
         if not 1 <= W <= BEAM_MAX_W:
             raise ValueError("beam width W must be in [1, %d], got %d" % (BEAM_MAX_W, W))
         if nbest is not None:
             check_nbest(nbest, W)
-        check_lm_args(lm, self.tovocab[0].weight.shape[0], lm_weight, length_bonus, lm_bos, lm_token_map)
+        model = check_ngram(ngram, self.tovocab[0].weight.shape[0], self.blank)
+        check_ngram_weight(model, ngram_weight)
         check_context(context, self.tovocab[0].weight.shape[0], self.blank)
+        check_lm_args(lm, self.tovocab[0].weight.shape[0], lm_weight, length_bonus, lm_bos, lm_token_map,
+                      ngram=model is not None)
         lp = self.forward(xs)
         B, T = lp.shape[0], lp.shape[1]
         frames = torch.full((B,), T, dtype=torch.int64) if xlen is None else _ctc_frames(T, xlen, B)
         return ctc.beam_search(lp, frames, W, self.blank, lm=lm, lm_weight=lm_weight, length_bonus=length_bonus,
-                               lm_bos=lm_bos, lm_token_map=lm_token_map, nbest=nbest, context=context)
+                               lm_bos=lm_bos, lm_token_map=lm_token_map, nbest=nbest, context=context, ngram=ngram,
+                               ngram_weight=ngram_weight)
 
     @torch.no_grad()
     def align(self, xs, ys, xlen, ylen):

@@ -21,12 +21,13 @@ import torch
 from . import ops
 from ._lib import lib, check
 from .context import check_context
+from .ngram import check_ngram, check_ngram_weight
 from .rnnt.tokenizer import NUL, BOS, UNK
 
 PH_LN, PH_PAIR, PH_LSTM, PH_LINEAR, PH_ARGMAX, PH_COPY, PH_BEAM_SELECT, PH_GATHER, PH_BEAM_FINAL, PH_BEAM_COMMIT, \
     PH_SKIP, PH_CTC_BEAM, PH_GRU, PH_CTC_EMIT, PH_FE_FRAME, PH_FE_GEMM, PH_FE_POWER, PH_FE_LOG, PH_FE_FINISH = range(19)
-F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE, F_LM, F_STREAM, F_FLUSH, F_CONT, F_ROUNDS, F_FRONTEND, F_CONTEXT = 1, 2, 4, \
-    8, 16, 32, 64, 128, 256, 512, 1024, 2048
+F_TANH, F_EMBED, F_MASKED, F_LOGP, F_MERGE, F_LM, F_STREAM, F_FLUSH, F_CONT, F_ROUNDS, F_FRONTEND, F_CONTEXT, \
+    F_NGRAM = 1, 2, 4, 8, 16, 32, 64, 128, 256, 512, 1024, 2048, 4096
 BEAM_MAX_W = 1024                                     # EB_BEAM_MAX_W
 CTC_SEQ_HEAD = 5                                      # CTC_BEAM's token rows: {len, hash lo / hi, parent hash lo / hi}
 MAX_SYMBOLS = 16                                      # bounds the program: about (5 + L_dec) * K phases per frame
@@ -37,6 +38,11 @@ class EbPhase(C.Structure):
                                          "ldy", "aux", "aux2", "hist_ld", "hist_col", "x1_div")] + \
                [(n, C.c_void_p) for n in ("x1", "x2", "w1", "w2", "b1", "b2", "y", "y2", "c", "tok_in", "tok_out",
                                           "hist", "seq_in", "seq_out", "src", "fuse", "tok_map", "tok_out2", "ctx")]
+
+
+class EbNgram(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("unigram", "bo", "suffix", "depth", "first", "count", "tok", "prob", "next",
+                                          "end", "state0", "state1", "row")] + [("weight", C.c_float), ("pad_", C.c_int32)]
 
 
 def _ptr(t, off=0):
@@ -141,18 +147,55 @@ def final_phase(e, W, y, K, ctx=None):
     return ph
 
 
-def context_program(e, graph, state):
+def context_program(e, graph, state, ng=None):
     """Contextual biasing on beam engine ``e`` (its ``dev`` set) with the ContextGraph ``graph`` (check_context done)
     and the per-slot automaton states ``state`` (two int32 [R] parities on the device): uploads the tables and the
-    EbContext descriptor {next, delta, pending, state[0], state[1]} and returns the fields a BEAM_SELECT / CTC_BEAM /
-    BEAM_FINAL phase reads it through.  e._ctx keeps the buffers alive."""
-    tabs = graph.to(e.dev)
-    nV = graph.n_states * graph.vocab_size
-    base = tabs.data_ptr()
-    desc = torch.tensor([base, base + 4 * nV, base + 8 * nV, state[0].data_ptr(), state[1].data_ptr()],
-                        dtype=torch.int64).to(e.dev)
+    EbContext descriptor {next, delta, pending, state[0], state[1], ng} and returns the fields a BEAM_SELECT / CTC_BEAM /
+    BEAM_FINAL phase reads it through.  e._ctx keeps the buffers alive.  ``ng`` (ngram_program's descriptor) rides in
+    the same descriptor and adds flag F_NGRAM; graph = None then leaves the context fields NULL and F_CONTEXT unset."""
+    ptrs, tabs, flags = [0] * 5, None, 0
+    if graph is not None:
+        tabs = graph.to(e.dev)
+        nV = graph.n_states * graph.vocab_size
+        base = tabs.data_ptr()
+        ptrs = [base, base + 4 * nV, base + 8 * nV, state[0].data_ptr(), state[1].data_ptr()]
+        flags |= F_CONTEXT
+    if ng is not None:
+        flags |= F_NGRAM
+    desc = torch.tensor(ptrs + [ng or 0], dtype=torch.int64).to(e.dev)
     e._ctx = (tabs, desc, state)
-    return dict(flags=F_CONTEXT, ctx=desc.data_ptr())
+    return dict(flags=flags, ctx=desc.data_ptr())
+
+
+def ngram_program(e, model, state, weight, length_bonus, R, V):
+    """N-gram fusion on beam engine ``e`` (its ``dev`` and ``lm`` set) with the NgramLM ``model`` (check_ngram done),
+    the per-slot n-gram states ``state`` (two int32 [R] parities on the device) and ``weight``: uploads the tables,
+    allocates the row workspace e.ng_row [R, V] and the EbNgram descriptor, and returns its device address (for
+    context_program) and the phase fields it needs besides: without an LM, ``fuse`` = {0, length_bonus}."""
+    buf, offs = model.to(e.dev)
+    base = buf.data_ptr()
+    tabs = [base + 4 * o for o in offs] + ([] if model.has_end else [None])
+    e.ng_row = torch.zeros(R, V, dtype=torch.float32, device=e.dev)
+    d = EbNgram(*tabs, state[0].data_ptr(), state[1].data_ptr(), e.ng_row.data_ptr(), weight, 0)
+    desc = torch.frombuffer(bytearray(bytes(d)), dtype=torch.uint8).to(e.dev)
+    e.ng_start = model.start
+    fields = {}
+    if not e.lm:
+        e.ng_fuse = torch.tensor([0.0, length_bonus], dtype=torch.float32, device=e.dev)
+        fields["fuse"] = _ptr(e.ng_fuse)
+    e._ng = (buf, desc, state)
+    return desc.data_ptr(), fields
+
+
+def fusion_fields(e, sel, graph, cstate, model, nstate, weight, length_bonus, R, V):
+    """Add contextual biasing (graph) and n-gram fusion (model) to the BEAM_SELECT / CTC_BEAM fields ``sel`` of engine
+    ``e``; returns what final_phase needs (None without either)."""
+    if graph is None and model is None:
+        return None
+    ng, extra = ngram_program(e, model, nstate, weight, length_bonus, R, V) if model is not None else (None, {})
+    cf = context_program(e, graph, cstate, ng)
+    sel.update(flags=sel["flags"] | cf["flags"], ctx=cf["ctx"], **extra)
+    return cf
 
 
 def nbest_lists(buf, B, N, L):
@@ -217,15 +260,16 @@ def greedy_round(prog, e, dec, h_enc, k, j, flags, unk, logp=None):
     _dec_phases(prog, dec, S, e.dec_h, e.dec_c, e.dec_htmp, e.dec_x, e.tok, e.blank, masked=True)
 
 
-def beam_state(e, R, Ld, Hd, D, LS, context=False):
+def beam_state(e, R, Ld, Hd, D, LS, context=False, ngram=False):
     """Allocate on engine ``e`` (its ``dev`` set) the per-slot state of a beam search over R rows, for each parity p
     in one flat buffer ``e._home[p]``: the predictor state e._st[p] [2 Ld, R, Hd] (h of every layer, then c; views
     e.dec_h[p] / e.dec_c[p]), its output e.dec_x[p] [R, D], the token sequences e.seqs[p] int32 [R, LS], with an LM
     (``e.lm``, lm_fusion done) its state e._lst[p] [2 Ll, R, Hl] (e.lm_h[p] / e.lm_c[p]) and with ``context`` the
-    context automaton states e.ctx_state[p] int32 [R] (else None).  One COPY of e._home[1] into e._home[0] moves all
-    of it, which a round of a multi-symbol frame needs (beam_frame)."""
+    context automaton states e.ctx_state[p] int32 [R] (else None), with ``ngram`` the n-gram states e.ng_state[p] int32
+    [R] (else None).  One COPY of e._home[1] into e._home[0] moves all of it, which a round of a multi-symbol frame
+    needs (beam_frame)."""
     Ll, _, Hl = e.lm_htmp.shape if e.lm else (0, 0, 0)
-    sizes = [2 * Ld * R * Hd, R * D, R * LS, 2 * Ll * R * Hl, R if context else 0]
+    sizes = [2 * Ld * R * Hd, R * D, R * LS, 2 * Ll * R * Hl, R if context else 0, R if ngram else 0]
     offs = [0]
     for n in sizes:
         offs.append(offs[-1] + -(-n // 64) * 64)           # 256-byte aligned segments
@@ -240,6 +284,7 @@ def beam_state(e, R, Ld, Hd, D, LS, context=False):
     if Ll:
         e.lm_h, e.lm_c = [s[:Ll] for s in e._lst], [s[Ll:] for s in e._lst]
     e.ctx_state = [seg(p, 4).view(torch.int32) for p in (0, 1)] if context else None
+    e.ng_state = [seg(p, 5).view(torch.int32) for p in (0, 1)] if ngram else None
 
 
 def beam_history(e, B, T, W):
@@ -261,6 +306,8 @@ def beam_reset(e):
     e.seqs[0].zero_()
     if e.ctx_state is not None:
         e.ctx_state[0].zero_()                                  # every slot at the automaton's root
+    if e.ng_state is not None:
+        e.ng_state[0].fill_(e.ng_start)                         # every slot at the n-gram start state
     e.logp.fill_(float("-inf"))
     e.logp.view(-1, e.W)[:, 0] = 0.0
     e.tok.fill_(BOS)
@@ -349,24 +396,29 @@ def lm_state_dict(lm):
     return sd
 
 
-def check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map):
+def _finite(name, v):
+    if isinstance(v, bool) or not isinstance(v, numbers.Real):
+        raise TypeError("%s must be a real number, got %r" % (name, v))
+    v = float(v)
+    if not math.isfinite(v):
+        raise ValueError("%s must be finite, got %r" % (name, v))
+    return v
+
+
+def check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map, ngram=False):
     """Validate the shallow-fusion arguments of a beam search over a vocabulary of V tokens.  Returns
     (lm state_dict, lm_weight, length_bonus, lm_bos, token map int64 [V] on the host) or None without ``lm``.
-    Raises TypeError / ValueError; touches no device."""
+    ``ngram``: an n-gram model is fused too, so length_bonus is legal without ``lm``.  Raises TypeError /
+    ValueError; touches no device."""
     if lm is None:
-        if lm_weight != 0.0 or length_bonus != 0.0 or lm_token_map is not None:
+        if lm_weight != 0.0 or (length_bonus != 0.0 and not ngram) or lm_token_map is not None:
             raise ValueError("lm_weight, length_bonus and lm_token_map need an lm")
+        if ngram:
+            _finite("length_bonus", length_bonus)
         return None
     sd = lm_state_dict(lm)
     ntok = sd["encoder.weight"].shape[0]
-    vals = []
-    for name, v in (("lm_weight", lm_weight), ("length_bonus", length_bonus)):
-        if isinstance(v, bool) or not isinstance(v, numbers.Real):
-            raise TypeError("%s must be a real number, got %r" % (name, v))
-        v = float(v)
-        if not math.isfinite(v):
-            raise ValueError("%s must be finite, got %r" % (name, v))
-        vals.append(v)
+    vals = [_finite(name, v) for name, v in (("lm_weight", lm_weight), ("length_bonus", length_bonus))]
     lm_bos = operator.index(lm_bos)
     if not 0 <= lm_bos < ntok:
         raise ValueError("lm_bos must be in [0, %d), got %d" % (ntok, lm_bos))
@@ -1034,10 +1086,16 @@ class BeamEngine:
     With ``context`` (a ContextGraph over the transducer's V tokens, edgedict_b200.context) each slot carries its
     phrase-automaton state (``ctx_state``, two parities beside the token sequences) and BEAM_SELECT adds the
     automaton's increment to every non-blank candidate's fusion term (decode.cu flag 2048); BEAM_FINAL ranks by the
-    value minus the pending bonus of the slot's state.  An empty graph builds the program without context."""
+    value minus the pending bonus of the slot's state.  An empty graph builds the program without context.
+
+    With ``ngram`` (an NgramLM over the transducer's V tokens, edgedict_b200.ngram) each slot carries its n-gram state
+    (``ng_state``, two parities beside the token sequences, every slot at the model's start state after ``run``'s
+    reset); BEAM_SELECT builds each slot's row of g(state, .) in ``ng_row`` and adds ngram_weight * g right after the LM
+    term (decode.cu flag 4096), and BEAM_FINAL adds ngram_weight * e(state).  Transducer.beam_search states the rule."""
 
     def __init__(self, transducer, batch, t_out, W, merge=True, blank=NUL, max_ctas=0, lm=None, lm_weight=0.0,
-                 length_bonus=0.0, lm_bos=1, lm_token_map=None, max_symbols=1, nbest=0, context=None):
+                 length_bonus=0.0, lm_bos=1, lm_token_map=None, max_symbols=1, nbest=0, context=None, ngram=None,
+                 ngram_weight=0.0):
         """``max_symbols`` = K: up to K rounds per encoder frame (Transducer.beam_search states the rule).  The history
         then has one column per round, [B, T' * K, W] (column t*K + j; a round a row did not take holds parent = slot,
         token = blank and live count 0, except the last column, which holds the final live count), and ``ids`` is
@@ -1047,8 +1105,10 @@ class BeamEngine:
         if not 1 <= W <= BEAM_MAX_W:
             raise ValueError("beam width must be in [1, %d], got %r" % (BEAM_MAX_W, W))
         N = _engine_nbest(nbest, W)
+        model = check_ngram(ngram, transducer.joint.joint[2].weight.shape[0], blank)
+        ng_w = check_ngram_weight(model, ngram_weight)
         fusion = check_lm_args(lm, transducer.joint.joint[2].weight.shape[0], lm_weight, length_bonus, lm_bos,
-                               lm_token_map)
+                               lm_token_map, ngram=model is not None)
         graph = check_context(context, transducer.joint.joint[2].weight.shape[0], blank)
         dec, joint = transducer.decoder, transducer.joint.joint
         self.dev = dec.embed.weight.device
@@ -1069,7 +1129,7 @@ class BeamEngine:
         self.lm = fusion is not None
         lm_sel, lm_step = lm_fusion(self, fusion, R) if self.lm else ({}, None)
         # per parity: predictor state, its output, {len, hash lo, hash hi, tokens} per row and the LM state
-        beam_state(self, R, Ld, Hd, D, TK + 3, context=graph is not None)
+        beam_state(self, R, Ld, Hd, D, TK + 3, context=graph is not None, ngram=model is not None)
         self.dec_htmp, self.hidden, self.logits = z(Ld, R, Hd), z(R, J), z(R, V)
         self.tok, self.src, self.logp = z(R, dtype=i32), z(R, dtype=i32), z(R)
         beam_history(self, B, TK, W)
@@ -1085,11 +1145,8 @@ class BeamEngine:
                    flags=(F_MERGE if merge else 0) | (F_LM if self.lm else 0), x1=_ptr(self.logits), ldx1=V,
                    y=_ptr(self.logp), tok_in=_ptr(self.frames), tok_out=_ptr(self.tok), src=_ptr(self.src),
                    hist=_ptr(self.hist), hist_ld=TK, **lm_sel)
-        ctx = None
-        if graph is not None:
-            cf = context_program(self, graph, self.ctx_state)
-            sel.update(flags=sel["flags"] | cf["flags"], ctx=cf["ctx"])
-            ctx = (cf, T & 1 if K == 1 else 0)                 # where the last frame left the states (beam_frame)
+        cf = fusion_fields(self, sel, graph, self.ctx_state, model, self.ng_state, ng_w, length_bonus, R, V)
+        ctx = None if cf is None else (cf, T & 1 if K == 1 else 0)   # where the last frame left the states (beam_frame)
         for t in range(T):
             beam_frame(prog, self, dec, t, _ptr(self.h_enc, t * E), T * E, sel, lm_step)
         prog.append(final_phase(self, W, self.logp, K, ctx))
@@ -1295,10 +1352,16 @@ class CTCBeamEngine:
 
     With ``context`` (a ContextGraph over V tokens) each slot carries its phrase-automaton state (``ctx_state``
     [2, R], parity t & 1 as ``state``), an extension by c adds the automaton's increment to f', and BEAM_FINAL ranks
-    by (pb (+) pnb) + f minus the pending bonus of the slot's state.  An empty graph builds the program without it."""
+    by (pb (+) pnb) + f minus the pending bonus of the slot's state.  An empty graph builds the program without it.
+
+    With ``ngram`` (an NgramLM over V tokens) each slot carries its n-gram state (``ng_state`` [2, R], parity t & 1,
+    the model's start state after ``run``'s reset), an extension by c adds the length bonus (without an LM) and
+    ngram_weight * g(state, c) after the LM term, f' = ((f + LM term) + w g) + delta, and BEAM_FINAL ranks by
+    ((pb (+) pnb) + f + w e(state)) - pending."""
 
     def __init__(self, batch, t_out, V, W, blank=0, lm=None, lm_weight=0.0, length_bonus=0.0, lm_bos=1,
-                 lm_token_map=None, max_ctas=0, device=None, frames_per_phase=0, nbest=0, context=None):
+                 lm_token_map=None, max_ctas=0, device=None, frames_per_phase=0, nbest=0, context=None, ngram=None,
+                 ngram_weight=0.0):
         B, T, V, W, blank = (operator.index(v) for v in (batch, t_out, V, W, blank))
         if not 1 <= W <= BEAM_MAX_W:
             raise ValueError("beam width must be in [1, %d], got %d" % (BEAM_MAX_W, W))
@@ -1309,7 +1372,9 @@ class CTCBeamEngine:
             raise ValueError("blank must lie in [0, %d), got %d" % (V, blank))
         if W * V >= 2 ** 31:
             raise ValueError("beam width x vocabulary must stay below 2^31 (flat candidate index), got %d x %d" % (W, V))
-        fusion = check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map)
+        model = check_ngram(ngram, V, blank)
+        ng_w = check_ngram_weight(model, ngram_weight)
+        fusion = check_lm_args(lm, V, lm_weight, length_bonus, lm_bos, lm_token_map, ngram=model is not None)
         graph = check_context(context, V, blank)
         n = operator.index(frames_per_phase)
         if n < 0 or (fusion is not None and n > 1):
@@ -1335,12 +1400,11 @@ class CTCBeamEngine:
         sel = dict(type=PH_CTC_BEAM, S=B, N=V, aux=W, aux2=blank, K1=LS, flags=F_LM if self.lm else 0,
                    x1=_ptr(self.lp), tok_in=_ptr(self.frames), c=_ptr(self.state), seq_out=_ptr(self.seqs),
                    y=_ptr(self.score), src=_ptr(self.src), hist=_ptr(self.hist), hist_ld=T, **lm_sel)
-        ctx, self.ctx_state = None, None
-        if graph is not None:
-            self.ctx_state = z(2, R, dtype=i32)          # per parity: the automaton state of each slot
-            cf = context_program(self, graph, self.ctx_state)
-            sel.update(flags=sel["flags"] | cf["flags"], ctx=cf["ctx"])
-            ctx = (cf, T & 1)                            # frozen frames carry the states, so frame T-1 wrote them
+        # per parity: the context automaton state and the n-gram state of each slot
+        self.ctx_state = z(2, R, dtype=i32) if graph is not None else None
+        self.ng_state = z(2, R, dtype=i32) if model is not None else None
+        cf = fusion_fields(self, sel, graph, self.ctx_state, model, self.ng_state, ng_w, length_bonus, R, V)
+        ctx = None if cf is None else (cf, T & 1)        # frozen frames carry the states, so frame T-1 wrote them
         if self.lm:
             Ll, _, Hl = self.lm_htmp.shape
             self.lm_state = z(2, 2 * Ll, R, Hl)      # per parity: h of every layer, then c
@@ -1373,6 +1437,8 @@ class CTCBeamEngine:
         self.seqs[0].zero_()
         if self.ctx_state is not None:
             self.ctx_state[0].zero_()
+        if self.ng_state is not None:
+            self.ng_state[0].fill_(self.ng_start)
         if self.lm:
             self.lm_state[0].zero_()
             self.lm_tok.fill_(self.lm_bos)

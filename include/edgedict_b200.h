@@ -433,6 +433,25 @@ enum { EB_PH_LN = 0, EB_PH_PAIR = 1, EB_PH_LSTM = 2, EB_PH_LINEAR = 3, EB_PH_ARG
        EB_PH_BEAM_SELECT = 6, EB_PH_GATHER = 7, EB_PH_BEAM_FINAL = 8, EB_PH_BEAM_COMMIT = 9, EB_PH_SKIP = 10,
        EB_PH_CTC_BEAM = 11, EB_PH_GRU = 12, EB_PH_CTC_EMIT = 13, EB_PH_FE_FRAME = 14, EB_PH_FE_GEMM = 15,
        EB_PH_FE_POWER = 16, EB_PH_FE_LOG = 17, EB_PH_FE_FINISH = 18 };
+/* The backoff tables of a token n-gram model (flag 4096; edgedict_b200/ngram.py builds them from an ARPA file), the
+ * n-gram state of every slot [B*W] in two parities beside the token sequences, and a row workspace: the CTA that owns
+ * an utterance builds there, per frame (or round), g(state(q), k) for all N tokens of each slot q it scores. */
+typedef struct EbNgram {
+    const float* unigram;     /* [N]: ln P(k), the <unk> fill applied */
+    const float* bo;          /* [n_states]: backoff weight */
+    const int32_t* suffix;    /* [n_states]: longest proper suffix that is a state (the root, 0, for itself) */
+    const int32_t* depth;     /* [n_states]: suffix links to the root (at most 7) */
+    const int32_t* first;     /* [n_states]: first child */
+    const int32_t* count;     /* [n_states]: number of children */
+    const int32_t* tok;       /* [n_children]: token, ascending within a state */
+    const float* prob;        /* [n_children]: g(state, tok) */
+    const int32_t* next;      /* [n_children]: the state after tok */
+    const float* end;         /* [n_states]: e(state) = g(state, </s>), or NULL without </s> */
+    int32_t* state[2];        /* per-slot state, parity 0 / 1 */
+    float* row;               /* [B*W, N] workspace */
+    float weight;             /* ngram_weight */
+    int32_t pad_;
+} EbNgram;
 /* The phrase automaton of contextual biasing (flag 2048; edgedict_b200/context.py builds it): dense tables over
  * n_states states and the N tokens of the phase, and the automaton state of every slot [B*W] in two parities, beside
  * the token sequences. */
@@ -441,6 +460,7 @@ typedef struct EbContext {
     const float* delta;       /* [n_states, N]: the increment a non-blank token adds to a candidate's value */
     const float* pending;     /* [n_states]: boost * the state's length, what BEAM_FINAL takes back */
     int32_t* state[2];        /* per-slot state, parity 0 / 1 */
+    const EbNgram* ng;        /* the n-gram model under flag 4096 (the fields above unused without flag 2048) */
 } EbContext;
 typedef struct EbPhase {
     int32_t type, S, K1, K2, N, flags, ldx1, ldx2, ldw1, ldw2, ldy, aux, aux2, hist_ld, hist_col, x1_div;
@@ -489,6 +509,12 @@ typedef struct EbPhase {
  *            y - pending[state] with the state from parity hist_col.  BEAM_COMMIT reads the states from parity 1,
  *            collapses to the live slot of highest y - pending[state] (lowest slot on ties; it keeps its y and state)
  *            and writes every slot's state, moved by src, to parity 0.
+ *     4096 = n-gram shallow fusion (BEAM_SELECT, CTC_BEAM, BEAM_FINAL): ctx->ng points to an EbNgram and fuse[1] holds the
+ *            length bonus even without flag 32.  A candidate that appends a non-blank token k to slot q adds w*g(state(q),
+ *            k), unfused by __fmul_rn / __fadd_rn, right after the LM term (BEAM_SELECT: f = f0 + w*g, f0 the LM term or
+ *            the length bonus, then + delta under 2048; CTC_BEAM: f' = ((f + f0) + w*g) + delta), and each survivor's
+ *            state is written to the other parity exactly where the context state is.  BEAM_FINAL ranks and writes
+ *            (y + w*e(state)) - pending, the state from parity hist_col (no w*e term when end is NULL).
  * SKIP (no flags, writes nothing, no grid barrier): when no row of tok_in[0..S) differs from aux2 (blank), every CTA
  * jumps over the next aux phases.  It reads only data final at the preceding barrier, so all CTAs take the same branch.
  * BEAM_COMMIT (streaming beam, after a chunk's last frame, one CTA per stream): commits the common prefix of the live
